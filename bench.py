@@ -1,18 +1,19 @@
 #!/usr/bin/env python
-"""bench.py -- 480x640 4-iteration pose refinements/sec (BASELINE.json metric) on N B200s.
+"""bench.py -- 480x640 4-iteration pose refinements/sec (BASELINE.json metric) on N H100s.
 
     python bench.py --gpus 1 --steps 20 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
            --master-port P bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference --steps 5 --warmup 1      # restated reference CPU path (oracle)
+    python bench.py --gpus 1 --steps 20 --warmup 3 --dump-outputs DIR   # + the last timed step's results as DIR/*.npy
 
 One "step" = STEP_BATCHES (32) passes of the fused hot path (dim_refine: 4 x render -> bbox+zoom -> FlowNetS ->
 se3 compose), each over one batch of 16 synthetic instances = 512 refinements; workload = BASELINE.json configs[1]
 (C2: ~5k-vert mesh, 4 iters, batch 16 per GPU, random-init FlowNetS).  32 batches per step make the default
-20-step timed region ~1.5-2 s long, so the clocks settle under the power cap, the clock sampler sees >= 15 samples and
-the SUSTAINED tensor peak of MEASURED_PEAKS.json is the right roofline denominator.  Instances are independent:
+20-step timed region long enough for the clocks to settle under the power cap and for the clock sampler to see >= 15
+samples.  Instances are independent:
 N GPUs = N replicas of the per-GPU work, no data-path collective ("scaling": "weak").
-The headline precision is DIM_PREC_FP16 (one fp16 tcgen05 pass; the mode whose -m gpu tests assert the north-star
+The headline precision is DIM_PREC_FP16 (one fp16 wgmma pass; the mode whose -m gpu tests assert the north-star
 1e-4 rot / 1e-3 trans tolerance at batch 16); the bf16 fast mode is reported as the labelled secondary `fast_mode`.
 Prints ONE JSON line on rank 0.
 """
@@ -35,6 +36,7 @@ METRIC = "480x640 4-iter pose refinements/sec"
 UNIT = "refinements/s"
 N_ITER = 4
 STEP_BATCHES = 32  # device batches per bench step
+N_INPUT_SETS = 3  # rotating input sets (see make_inputs)
 WORKLOAD = "C2: synthetic 5k-vert mesh (5151 verts / 10000 tris), 4 iters, batch=16 per GPU, FlowNetS random-init"
 
 
@@ -49,18 +51,20 @@ def conv_flops_per_instance_iter():
 
 
 def measured_peaks():
-    """MEASURED_PEAKS.json (driver-written): fp16 and bf16 share the tcgen05 kind::f16 rate, so the cuBLAS bf16 figures are the
-    denominators.  `burst` for a region shorter than ~1 s (boost clocks), `sustained` for a long one (power-capped clocks)."""
+    """Roofline denominators.  MEASURED_PEAKS.json (optional, next to this file; keys bf16_tflops[_sustained], hbm_gbs): peaks
+    measured on the card at hand -- fp16 and bf16 share the wgmma rate, so the bf16 figures serve both.  Without it: NVIDIA's
+    H100 SXM data sheet (dense bf16 989 TFLOP/s, HBM3 3350 GB/s, for a card allowed 700 W): an upper bound a power-limited
+    card does not reach.  `burst` for a region shorter than ~1 s (boost clocks), `sustained` for a long one."""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         d = json.load(open(path))
         burst = d.get("bf16_tflops")
         return {"burst": burst, "sustained": d.get("bf16_tflops_sustained", burst), "hbm": d.get("hbm_gbs"), "src": "measured"}
-    return {"burst": 1590.0, "sustained": 1400.0, "hbm": 6650.0, "src": "fallback"}
+    return {"burst": 989.0, "sustained": 989.0, "hbm": 3350.0, "src": "H100 SXM data sheet (700 W)"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -169,7 +173,7 @@ def run_b200(args):
     refiner = PoseRefiner(meshes, weights, K, device=local_rank, max_batch=B, n_iter=N_ITER, pixel_means_rgb=means,
                           precision=args.precision, n_slots=args.slots)
     ctx = refiner.ctx
-    sets = make_inputs(ctx, synth, mesh, B, 3, 1000 + rank, dev, torch, z_mean=0.6 if args.config == "c5" else 0.8,
+    sets = make_inputs(ctx, synth, mesh, B, N_INPUT_SETS, 1000 + rank, dev, torch, z_mean=0.6 if args.config == "c5" else 0.8,
                        n_classes=len(meshes))
     train_info = None
     if args.train_steps > 0:
@@ -255,6 +259,8 @@ def run_b200(args):
     ms_total, launches, clocks, out = device_pass(prec, K_steps, True)
     poses_last = out["poses"][-1].cpu().numpy()
     idx_last = (K_steps * SB - 1) % len(sets)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, outs, K_steps * SB, len(sets), len(streams))
 
     # ---------------- secondary: the bf16 fast mode (fails the 1e-4 rot tolerance -- NOT the headline), same pass shape
     fast = None
@@ -300,17 +306,13 @@ def run_b200(args):
     if rank == 0:
         peaks = measured_peaks()
         flops_ii = conv_flops_per_instance_iter()
-        # roofline of the conv tower IN THE SAME multi-stream pass that produced `value`: every tcgen05 FLOP of the timed
+        # roofline of the conv tower IN THE SAME multi-stream pass that produced `value`: every wgmma FLOP of the timed
         # region over the whole region (the other kernels of the step run inside it: this is a lower bound of the conv
         # kernels' own rate).  Denominator: sustained bf16/fp16 peak when the region is >= 1 s, else the burst peak.
         long_run = ms_total >= 1000.0
         peak = peaks["sustained"] if long_run else peaks["burst"]
         step_tflops = flops_ii * N_ITER * B * SB * K_steps / (ms_total / 1e3) / 1e12
         conv_single = flops_ii * B * n_rec / (stages["conv"] / 1e3) / 1e12 if stages["conv"] > 0 else 0.0
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "roofline_traffic.json")
-        if os.path.exists(tpath):
-            traffic = json.load(open(tpath)).get("conv_igemm_bytes_per_launch")
         # ADD(-S) sanity of the last batch against the observed pose (blob is asymmetric -> ADD)
         s_last = sets[idx_last]
         def add(p, q, b):
@@ -329,19 +331,19 @@ def run_b200(args):
                        "parity": "DIM_PREC_FP16: tests/test_gpu_headline_b16.py asserts 1e-4 rot / 1e-3 trans per iteration at batch 16"
                                  if args.precision == "fp16" else "see tests/test_gpu_parity.py for this mode's bounds",
                        "l2": "per-batch working set (~1.6 GB of activations + 90 MB weights + 59 MB inputs) exceeds the "
-                             "126 MB L2; 3 rotating input sets"},
+                             "50 MB L2; 3 rotating input sets"},
             "clocks": clocks,
             "e2e": {"value": round(e2e_value, 2), "unit": UNIT,
                     "h2d_bytes_per_step": int(SB * (B * 480 * 640 * 3 + B * 4 + B * 96)),
                     "d2h_bytes_per_step": int(SB * N_ITER * B * (96 + 28)), "ms_per_step": round(ms_e2e / K_steps, 4),
                     "api": "PoseRefiner.submit/result -> dim_refine_host_async (uint8 BGR HWC pinned host images in, float64 poses out; %d batches in flight)" % args.slots, "timer": "host wall clock around K steps, bracketed by barrier + cuda synchronize"},
             "gpu_launches": int(launches),
-            "roofline": {"bound": "tensor", "kernel": "conv1_stack_kernel + conv_igemm_pair_kernel (conv2) + conv_igemm_persistent_kernel x8 (10 launches per batch-iteration)",
+            "roofline": {"bound": "tensor", "kernel": "conv1_kernel + conv_igemm_persistent_kernel x9 (10 launches per batch-iteration)",
                          "achieved": round(step_tflops, 2), "peak": peak, "unit": "TFLOP/s",
-                         "frac": round(step_tflops / peak, 4), "traffic": traffic,
+                         "frac": round(step_tflops / peak, 4),
                          "how": "algorithmic conv FLOPs of the timed region (38.79 GFLOP x %d instances x %d iterations x %d batches x %d steps) / "
                                 "the CUDA-event duration of the same multi-stream region that produced `value`" % (B, N_ITER, SB, K_steps),
-                         "peak_source": "%s bf16 %s (MEASURED_PEAKS.json; timed region %.2f s)" % (peaks["src"], "sustained" if long_run else "burst", ms_total / 1e3),
+                         "peak_source": "%s bf16 %s (timed region %.2f s)" % (peaks["src"], "sustained" if long_run else "burst", ms_total / 1e3),
                          "frac_of_burst": round(step_tflops / peaks["burst"], 4), "frac_of_sustained": round(step_tflops / peaks["sustained"], 4),
                          "conv_tower_single_stream_tflops": round(conv_single, 2),
                          "launches_per_batch_iteration": n_launch_kernels},
@@ -368,6 +370,20 @@ def run_b200(args):
     refiner.close()
     if result is not None:
         print(json.dumps(result), flush=True)
+
+
+def dump_outputs(out_dir, outs, n_batches, n_sets, n_slots):
+    """What the timed pass returned for its last batches, as DIR/set<s>_<name>.npy (float32 / float64).  Batch k of the pass
+    ran input set k % n_sets on slot k % n_slots, and every slot's result tensors hold its last batch; the pass is
+    deterministic, so the last batch of each input set stands for every batch of the last step that ran that set."""
+    os.makedirs(out_dir, exist_ok=True)
+    for s in range(n_sets):
+        k = max(k for k in range(max(0, n_batches - n_sets * n_slots), n_batches) if k % n_sets == s)
+        assert k >= n_batches - n_slots, "input set %d has no batch among the last %d" % (s, n_slots)
+        for name, t in outs[k % n_slots].items():
+            a = t.cpu().numpy()
+            np.save(os.path.join(out_dir, "set%d_%s.npy" % (s, name)),
+                    a.astype(np.float64) if a.dtype.kind in "iu" else a.astype(np.float64 if a.dtype == np.float64 else np.float32))
 
 
 def train_on_sets(meshes, sets, B, K, means, device, steps, torch):
@@ -539,9 +555,12 @@ def main():
     ap.add_argument("--steps", type=int, default=None)
     ap.add_argument("--warmup", type=int, default=None)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the results of the last step (poses, se3, zoom_factor, bbox per input set) "
+                         "as DIR/*.npy")
     ap.add_argument("--batch", type=int, default=16, help="instances per GPU")
     ap.add_argument("--precision", default="fp16", choices=["fp16", "bf16x3", "bf16"],
-                    help="fp16 = headline (single tcgen05 pass, meets 1e-4 rot / 1e-3 trans); bf16x3 = 3-pass; bf16 = fast mode")
+                    help="fp16 = headline (single wgmma pass, meets 1e-4 rot / 1e-3 trans); bf16x3 = 3-pass; bf16 = fast mode")
     ap.add_argument("--step-batches", type=int, default=STEP_BATCHES, help="device batches per bench step")
     ap.add_argument("--no-fast-mode", action="store_true", help="skip the secondary bf16 fast-mode pass")
     ap.add_argument("--train-steps", type=int, default=900,
@@ -556,6 +575,13 @@ def main():
     ap.add_argument("--workload", default="refine", choices=["refine", "train"],
                     help="refine = the headline metric (default); train = config C4 training step (tools/train_bench.py)")
     args = ap.parse_args()
+    if args.dump_outputs is not None:
+        # the dump holds the last batch of every input set; each batch's results live in its slot's tensors until the slot's
+        # next batch, so the last step's batches of all sets are still there only when every set has a slot of its own
+        if args.workload != "refine" or args.impl != "b200":
+            ap.error("--dump-outputs writes the results of the timed refinement pass: it needs --workload refine --impl b200")
+        if args.slots < N_INPUT_SETS:
+            ap.error("--dump-outputs needs --slots >= %d (one slot per input set)" % N_INPUT_SETS)
     if args.workload == "train":  # secondary workload: BASELINE.json configs[3]; same launch contract (torchrun for N > 1)
         sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "tools"))
         import train_bench

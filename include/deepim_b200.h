@@ -1,5 +1,5 @@
 /*
- * deepim_b200.h -- C ABI of libdeepim_b200.so (hand-written sm_100a CUDA, no CPU fallback).
+ * deepim_b200.h -- C ABI of libdeepim_b200.so (hand-written sm_90a CUDA, no CPU fallback).
  *
  * Drop-in boundary for the mx-DeepIM render-and-compare hot path.  Each entry point names the
  * reference interface it replaces (paths relative to the mx-DeepIM repo).  The reference binds its
@@ -203,9 +203,9 @@ DIM_API int32_t dim_net_load(dim_ctx *ctx, const float *const *weights_host,
                              const float *const *biases_host);
 
 /* precision of the conv stack */
-#define DIM_PREC_BF16 0   /* one bf16 tcgen05 pass, fp32 accumulate (throughput mode)          */
-#define DIM_PREC_BF16X3 1 /* hi/lo split, 3 tcgen05 passes, ~fp32 accuracy (parity mode)       */
-#define DIM_PREC_FP16 2   /* one fp16 tcgen05 pass (11 significant bits), fp32 accumulate, saturating stores:
+#define DIM_PREC_BF16 0   /* one bf16 wgmma pass, fp32 accumulate (throughput mode)            */
+#define DIM_PREC_BF16X3 1 /* hi/lo split, 3 wgmma passes, ~fp32 accuracy (parity mode)         */
+#define DIM_PREC_FP16 2   /* one fp16 wgmma pass (11 significant bits), fp32 accumulate, saturating stores:
                              the single-pass mode that meets the 1e-4 rot / 1e-3 trans se3 tolerance (headline mode) */
 
 /* Encoder + fc + heads on already-zoomed blobs (get_convs, deepIM_flownet.py:53-116; heads
@@ -269,11 +269,9 @@ DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int3
 DIM_API int32_t dim_debug_activation(dim_ctx *ctx, int32_t idx, int32_t lo, void *host_dst,
                                      uint64_t bytes);
 DIM_API int32_t dim_debug_layer_geometry(dim_ctx *ctx, int32_t idx, int32_t *out8);
-/* tuning hooks (tools/conv_lab.py; not part of the drop-in surface).
- * dim_debug_set_option: run-time kernel-variant switch.  Keys: "pair_mask": bit i puts conv layer i (1..9) on the
- *   cta_group::2 kernel (default: conv2); "conv1_stack": 1 (default) = stacked-filter-rows conv1 kernel for the
- *   single-pass precisions, 0 = rolling-strip kernel; "graph": 1 (default) = replay the refinement chain as a CUDA graph.
- *   Synchronises the device and drops the cached launch descriptors / graphs.
+/* tuning hooks (not part of the drop-in surface).
+ * dim_debug_set_option: run-time switch.  Key "graph": 1 (default) = replay the refinement chain as a CUDA graph,
+ *   0 = enqueue it launch by launch.  Drops the captured graphs; any other key is an error.
  * dim_debug_layer_profile: enable = 1 records CUDA events around each conv layer of every dim_net_fwd / dim_refine
  *   iteration; ms10 (nullable) receives the 10 layer times of the LAST forward pass; enable = 0 stops. */
 DIM_API int32_t dim_debug_set_option(dim_ctx *ctx, const char *key, int32_t value);

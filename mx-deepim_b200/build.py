@@ -1,4 +1,4 @@
-"""Build libdeepim_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libdeepim_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python mx-deepim_b200/build.py [--force] [--verbose]
 
@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libdeepim_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
           "-Xcudafe", "--diag_suppress=177"]
 UNITS = {

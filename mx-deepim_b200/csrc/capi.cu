@@ -128,8 +128,8 @@ DIM_API int32_t dim_ctx_create(int32_t device, int32_t max_batch, int32_t H, int
   DIM_CHECK(cudaSetDevice(device));
   cudaDeviceProp prop;
   DIM_CHECK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("dim_ctx_create: device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("dim_ctx_create: device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major,
               prop.minor);
     return 11;
   }

@@ -88,7 +88,7 @@ struct NetState;  // conv.cu
 
 struct dim_ctx {
   int device = 0, max_batch = 0, H = 0, W = 0, max_classes = 0, max_verts = 0, max_faces = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   // meshes
   std::vector<dim::MeshDev> meshes_host;
   dim::MeshDev *meshes = nullptr;  // device table [max_classes]

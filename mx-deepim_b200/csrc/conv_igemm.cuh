@@ -1,5 +1,5 @@
-// conv_igemm.cuh -- implicit-GEMM convolution on 5th-gen tensor cores (tcgen05.mma, accumulators in
-// TMEM) fed by TMA (cp.async.bulk.tensor) through an mbarrier ring.  sm_100a only.
+// conv_igemm.cuh -- implicit-GEMM convolution on Hopper tensor cores (wgmma.mma_async, fp32 accumulators in
+// registers) fed by TMA (cp.async.bulk.tensor) through an mbarrier ring.  sm_90a.
 //
 // Replaces the cuDNN Convolution + LeakyReLU(0.1) pairs of the FlowNetS tower
 // (deepim/symbols/deepIM_flownet.py:63-107).
@@ -10,44 +10,40 @@
 // coordinates.  For a stride-2 layer the buffer is read through four parity views (row parity,
 // col parity): tap (kh,kw) = (2dh+ph, 2dw+pw) of output pixel (g,ow) is element (g+dh, ow+dw) of view
 // (ph,pw).  An M tile is a BW x BH rectangle of output pixels (BW*BH <= 128), i.e. exactly one TMA
-// box per tap, landing in shared memory as the K-major 128B/64B-swizzled operand tile UMMA expects.
+// box per tap, landing in shared memory as the K-major 128B-swizzled operand tile wgmma expects.
 // Weights are [Cout][kh][kw][Cin] bf16 (K-major), one 2-D tensor map.
 //
-// Warp roles (192 threads): warp 0 = TMA producer (one lane), warp 1 = TMEM allocator + MMA issuer
-// (one lane), warps 2..5 = epilogue (TMEM -> registers -> bias + LeakyReLU -> bf16 NHWC stores into
-// the next layer's bordered buffer, or fp32 split-K partials).
+// Warp roles (384 threads = 3 warpgroups): warp 0 = TMA producer (elected lane), warpgroups 1 and 2 = consumers.  Each
+// consumer issues the wgmmas of 64 of the tile's 128 rows (M = 64 per instruction) into its own register accumulator and
+// runs the epilogue for them (bias + LeakyReLU -> bf16 NHWC stores into the next layer's bordered buffer).  The producer
+// keeps loading the next tile while the consumers drain the current one.
 //
 // SPLIT3 = bf16x3 precision mode: operands are hi/lo bf16 pairs (x = hi + lo); each K step issues
 // hi*hi + lo*hi + hi*lo into the same fp32 accumulator (error ~2^-16 relative, near-fp32).
-// ConvKParams::f16 = fp16 precision mode (DIM_PREC_FP16): the same one-pass kernels with IEEE half
-// operands (instruction-descriptor a/b format F16; 11 significant bits instead of bf16's 8) and
-// epilogues that store saturating fp16; the 16-bit activation / weight buffers are shared with the
-// bf16 modes (typed __nv_bfloat16* in the signatures, the bits are whatever the mode stores).
+// F16 = fp16 precision mode (DIM_PREC_FP16): the same one-pass kernels with IEEE half operands (11 significant bits
+// instead of bf16's 8) and epilogues that store saturating fp16; the 16-bit activation / weight buffers are shared with
+// the bf16 modes (typed __nv_bfloat16* in the signatures, the bits are whatever the mode stores).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace dim {
 
 struct ConvKParams {
   CUtensorMap a_map[4];     // activation views (hi); [0] only for stride 1
   CUtensorMap a_lo_map[4];  // activation views (lo), SPLIT3 only
-  CUtensorMap b_map;        // weights hi
+  CUtensorMap b_map;        // weights hi (fp16 pack in F16 mode)
   CUtensorMap b_lo_map;     // weights lo
-  CUtensorMap b2_map;       // weights hi, box = BLOCK_N/2 rows (CTA-pair kernel: each CTA loads half of N)
-  CUtensorMap b2_lo_map;
   int KH, KW, stride, cchunks;  // taps and channel chunks (Cin_eff / BLOCK_K)
   int BW, BH, n_col_tiles;
   int Hq, Ho, Wo, Bn;           // virtual rows per image, valid output extent, batch
   int out_Hp, out_Wp, out_py, out_px, Cout;
-  int kblocks, ksplit;
-  int f16;  // 1: outputs are stored as fp16 (operands are fp16 as well: see idesc)
-  uint32_t idesc;
+  int kblocks;
   float slope;
   const float *bias;
   __nv_bfloat16 *out_hi, *out_lo;
-  float *partial;  // [ksplit][Bn*Ho*Wo][Cout] when ksplit > 1
   // ---- generic epilogue (EPI = 1: decoder deconvolutions as parity sub-convolutions, data gradients)
   //   TMA coordinates get (in_off_c, in_off_r) added; virtual output pixel (oh, ow) of image n lands at
   //   interior pixel (oh*out_sy + out_oy, ow*out_sx + out_ox) of the output buffer when that is inside
@@ -64,11 +60,9 @@ namespace ptx {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// One lane of a CONVERGED warp.  The TMA-producer and MMA-issuer warps run their loops with all 32 lanes (warp-uniform
-// control flow and operands) and only the instruction that must be issued once sits under elect.sync: descriptors,
-// coordinates and barrier addresses then live in uniform registers.  Issuing from inside `if (lane == 0)` instead made the
-// compiler wrap EVERY tcgen05.mma / TMA instruction in an ELECT + R2UR.BROADCAST + BRA.U.ANY loop (~17 SASS instructions
-// per MMA on one thread): slower than the 32-cycle N = 64 MMA it issues, and the limiter of conv1 / conv2 in round 1.
+// One lane of a CONVERGED warp.  The TMA producer runs its loop with all 32 lanes (warp-uniform control flow and
+// operands) and only the instruction that must be issued once sits under elect.sync: descriptors, coordinates and barrier
+// addresses then live in uniform registers instead of being re-broadcast around every issue from `if (lane == 0)`.
 // Every function below that says "elected lane" must be called by all 32 lanes of the warp.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
@@ -138,116 +132,41 @@ __device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, u
         : "memory");
 }
 
-// --- TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t *slot_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// raw variants for callers that already sit inside `if (elect_one()) { ... }` (one election per K-block instead of one per
-// instruction).  A descriptor advanced by `bytes` inside its tile is desc + (bytes >> 4): the 14-bit start-address field
-// cannot carry for shared-memory addresses below 256 KB.
-__device__ __forceinline__ void umma_f16_raw(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_raw(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 (or fp16 x fp16: idesc) -> fp32, issued by the elected lane
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
+// elected lane
+__device__ __forceinline__ void tma_load_4d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2, int c3) {
   if (elect_one())
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u)
-      : "memory");
-}
-// arrive on an mbarrier when all previously issued tcgen05.mma of the elected lane have completed (elect.sync picks the same
-// lane for the same member mask, so this tracks the MMAs issued through umma_f16)
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-  if (elect_one())
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (lane i of the warp's quadrant)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t *r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
+            "r"(smem_u32(dst)),
+        "l"((uint64_t)map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+        : "memory");
 }
 
-// zero 32 lanes x 32 consecutive fp32 columns of TMEM (the accumulator block is handed back cleared)
-__device__ __forceinline__ void tmem_zero_32x32(uint32_t taddr) {
-  const uint32_t z = 0u;
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, "
-      "%1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1, %1};" ::"r"(taddr), "r"(z)
-      : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
-
-// K-major swizzled operand descriptor (cute::UMMA::SmemDescriptor, mma_sm100_desc.hpp): start>>4 in
-// [0,14), LBO [16,30) (unused for swizzled K-major, set 1), SBO>>4 in [32,46) = 8 rows * row bytes,
-// version 1 at [46,48), layout type at [61,64) (2 = SWIZZLE_128B, 4 = SWIZZLE_64B).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t sbo_bytes, uint32_t layout_type) {
+// wgmma shared-memory operand descriptor (PTX ISA "matrix descriptor"): start >> 4 in [0,14), leading byte offset >> 4 in
+// [16,30), stride byte offset >> 4 in [32,46), layout in [62,64) (0 = no swizzle, 1 = 128B, 2 = 64B swizzle).
+//   K-major, swizzled : SBO = 8 rows * row bytes, LBO unused (1)
+//   K-major, none     : core matrices of 8 rows x 16 B; LBO = bytes between K-adjacent core matrices, SBO = between 8-row groups
+//   MN-major, swizzled: LBO = bytes between 64- (128B) / 32-element (64B) groups along M/N, SBO = between groups of 8 K rows
+// A descriptor advanced by `bytes` is desc + (bytes >> 4): the 14-bit start field cannot carry below 256 KB.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout_type << 61;
+  d |= (uint64_t)layout << 62;
   return d;
 }
+constexpr uint32_t kSW128 = 1u, kSW64 = 2u, kNoSwizzle = 0u;
+
+// register split between the producer warpgroup and the two consumer warpgroups (128 * 40 + 256 * 232 <= 64 K)
+__device__ __forceinline__ void regs_producer() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void regs_consumer() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
 
 }  // namespace ptx
-
-// explicit shared-state-space accesses for the epilogues.  The staging tiles and the bias vector live in DYNAMIC shared memory
-// reached through an aligned generic pointer; the compiler cannot prove the address space and emitted generic LD / ST for them
-// (ncu: 8.6 M shared-load bank conflicts per conv1 launch, ~800 wasted shared-memory cycles per output tile on the pipe the
-// tensor core reads its operands through).  These go straight to LDS / STS.
-__device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
-  return v;
-}
-__device__ __forceinline__ float4 lds128f(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
 
 // two fp32 -> packed 16-bit pair (element 0 in the low half).  fp16 saturates to +-65504 instead of
 // overflowing to inf (the reference computes in fp32: a finite value must stay finite).
@@ -262,258 +181,107 @@ __device__ __forceinline__ uint32_t pack2_bf16(float a, float b) {
   return r;
 }
 
-// ---------------------------------------------------------------------------------------------
-// Epilogue helper: one warp owns 32 accumulator rows (its TMEM lane quadrant).  64 fp32 columns per
-// call are biased, LeakyReLU'd, converted to bf16 (hi[, lo]) and staged through a per-warp 4 KB
-// XOR-swizzled shared-memory tile so that the global stores are full 128-byte lines (lane l writes 16 B
-// of row i*4 + l/8): the "one thread = one output row" register layout would otherwise emit 16-byte
-// stores 128+ bytes apart (half-sector writes, 32 lines per instruction).
-template <bool SPLIT3>
-__device__ __forceinline__ void epilogue_store64(const uint32_t *r, const float *bias_s, float slope, uint8_t *stage,
-                                                 __nv_bfloat16 *out_hi, __nv_bfloat16 *out_lo, long long my_off,
-                                                 bool my_valid, int lane, bool f16 = false) {
-  __align__(16) uint32_t h[32];
-  __align__(16) uint32_t l[SPLIT3 ? 32 : 4];
-  const uint32_t ba = ptx::smem_u32(bias_s), sa = ptx::smem_u32(stage);
-#pragma unroll
-  for (int j = 0; j < 64; j += 4) {
-    const float4 b4 = lds128f(ba + j * 4);
-    float v0 = __uint_as_float(r[j]) + b4.x, v1 = __uint_as_float(r[j + 1]) + b4.y;
-    float v2 = __uint_as_float(r[j + 2]) + b4.z, v3 = __uint_as_float(r[j + 3]) + b4.w;
-    v0 = v0 > 0.f ? v0 : v0 * slope;
-    v1 = v1 > 0.f ? v1 : v1 * slope;
-    v2 = v2 > 0.f ? v2 : v2 * slope;
-    v3 = v3 > 0.f ? v3 : v3 * slope;
-    if (!SPLIT3 && f16) {
-      h[j >> 1] = pack2_f16(v0, v1);
-      h[(j >> 1) + 1] = pack2_f16(v2, v3);
-    } else {
-      const uint32_t h0 = pack2_bf16(v0, v1), h1 = pack2_bf16(v2, v3);
-      h[j >> 1] = h0;
-      h[(j >> 1) + 1] = h1;
-      if (SPLIT3) {
-        l[j >> 1] = pack2_bf16(v0 - __uint_as_float(h0 << 16), v1 - __uint_as_float(h0 & 0xFFFF0000u));
-        l[(j >> 1) + 1] = pack2_bf16(v2 - __uint_as_float(h1 << 16), v3 - __uint_as_float(h1 & 0xFFFF0000u));
-      }
-    }
-  }
-  const unsigned vmask = __ballot_sync(0xffffffffu, my_valid);
-  const int ch = lane & 7;
-#pragma unroll
-  for (int pass = 0; pass < (SPLIT3 ? 2 : 1); ++pass) {
-    const uint32_t *src = pass ? l : h;
-    __nv_bfloat16 *out = pass ? out_lo : out_hi;
-#pragma unroll
-    for (int c = 0; c < 8; ++c)
-      sts128(sa + lane * 128 + ((c ^ (lane & 7)) << 4), *reinterpret_cast<const uint4 *>(src + c * 4));
-    __syncwarp();
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int row = i * 4 + (lane >> 3);
-      const long long off = __shfl_sync(0xffffffffu, my_off, row);
-      const uint4 v = lds128(sa + row * 128 + ((ch ^ (row & 7)) << 4));
-      if ((vmask >> row) & 1u) *reinterpret_cast<uint4 *>(out + off + ch * 8) = v;
-    }
-    __syncwarp();
+// conv1: MMA rows >= BW of the last ring slot read up to (128 - BW) * 16 bytes past it
+constexpr int kConv1Slack = 2048;
+
+
+// Rows of the m64nN accumulator fragment owned by thread `t` of a warpgroup: row0 and row0 + 8; columns 8j + 2(t & 3) (+1).
+__device__ __forceinline__ int frag_row(int t) { return ((t >> 5) << 4) + ((t & 31) >> 2); }
+
+// One fragment row pair (j-th 8-column group) of the forward epilogue: + bias, LeakyReLU, 16-bit store (hi[, lo]).
+template <bool SPLIT3, bool F16>
+__device__ __forceinline__ void store_pair(float v0, float v1, float2 b, float slope, __nv_bfloat16 *out_hi, __nv_bfloat16 *out_lo,
+                                           long long off) {
+  v0 += b.x;
+  v1 += b.y;
+  v0 = v0 > 0.f ? v0 : v0 * slope;
+  v1 = v1 > 0.f ? v1 : v1 * slope;
+  if (F16) {
+    *reinterpret_cast<uint32_t *>(out_hi + off) = pack2_f16(v0, v1);
+  } else {
+    const uint32_t h = pack2_bf16(v0, v1);
+    *reinterpret_cast<uint32_t *>(out_hi + off) = h;
+    if (SPLIT3)
+      *reinterpret_cast<uint32_t *>(out_lo + off) = pack2_bf16(v0 - __uint_as_float(h << 16), v1 - __uint_as_float(h & 0xFFFF0000u));
   }
 }
 
-// LINEAR: the 32 rows of the warp are consecutive pixels of one output row (conv1): row r lives at my_off(row 0) + r * row_stride
-// elements and rows [0, n_valid) are valid -- no per-row offset shuffle, no ballot (my_off / my_valid are then warp-uniform:
-// offset of the warp's row 0 and unused).
-// BIAS_REG: bias_s points at 32 floats the caller keeps in registers (a fully unrolled local array) instead of shared memory.
-template <bool SPLIT3, bool LINEAR = false, bool BIAS_REG = false>
-__device__ __forceinline__ void epilogue_store32(const uint32_t *r, const float *bias_s, float slope, uint8_t *stage,
-                                                 __nv_bfloat16 *out_hi, __nv_bfloat16 *out_lo, long long my_off,
-                                                 bool my_valid, int lane, bool f16, int n_valid = 32, int row_stride = 0) {
-  __align__(16) uint32_t h[16];
-  __align__(16) uint32_t l[SPLIT3 ? 16 : 4];
-  const uint32_t ba = BIAS_REG ? 0u : ptx::smem_u32(bias_s), sa = ptx::smem_u32(stage);
-#pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const float4 b4 = BIAS_REG ? make_float4(bias_s[j], bias_s[j + 1], bias_s[j + 2], bias_s[j + 3]) : lds128f(ba + j * 4);
-    float v0 = __uint_as_float(r[j]) + b4.x, v1 = __uint_as_float(r[j + 1]) + b4.y;
-    float v2 = __uint_as_float(r[j + 2]) + b4.z, v3 = __uint_as_float(r[j + 3]) + b4.w;
-    v0 = v0 > 0.f ? v0 : v0 * slope;
-    v1 = v1 > 0.f ? v1 : v1 * slope;
-    v2 = v2 > 0.f ? v2 : v2 * slope;
-    v3 = v3 > 0.f ? v3 : v3 * slope;
-    if (!SPLIT3 && f16) {
-      h[j >> 1] = pack2_f16(v0, v1);
-      h[(j >> 1) + 1] = pack2_f16(v2, v3);
-    } else {
-      const uint32_t h0 = pack2_bf16(v0, v1), h1 = pack2_bf16(v2, v3);
-      h[j >> 1] = h0;
-      h[(j >> 1) + 1] = h1;
-      if (SPLIT3) {
-        l[j >> 1] = pack2_bf16(v0 - __uint_as_float(h0 << 16), v1 - __uint_as_float(h0 & 0xFFFF0000u));
-        l[(j >> 1) + 1] = pack2_bf16(v2 - __uint_as_float(h1 << 16), v3 - __uint_as_float(h1 & 0xFFFF0000u));
-      }
-    }
+// generic epilogue of the training-step kernels (see ConvKParams): two channels n, n + 1 of one output pixel
+__device__ __forceinline__ void store_pair_generic(float v0, float v1, const ConvKParams &p, int n, bool valid, long long off,
+                                                   long long add_off, long long mask_off) {
+  if (!valid || n >= p.Cout) return;
+  if (p.bias) {
+    v0 += __ldg(p.bias + n);
+    v1 += __ldg(p.bias + n + 1);
   }
-  const unsigned vmask = LINEAR ? 0u : __ballot_sync(0xffffffffu, my_valid);
-  const int ch = lane & 3;
-#pragma unroll
-  for (int pass = 0; pass < (SPLIT3 ? 2 : 1); ++pass) {
-    const uint32_t *src = pass ? l : h;
-    __nv_bfloat16 *out = pass ? out_lo : out_hi;
-#pragma unroll
-    for (int c = 0; c < 4; ++c)
-      sts128(sa + lane * 64 + ((c ^ ((lane >> 1) & 3)) << 4), *reinterpret_cast<const uint4 *>(src + c * 4));
-    __syncwarp();
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int row = i * 8 + (lane >> 2);
-      const uint4 v = lds128(sa + row * 64 + ((ch ^ ((row >> 1) & 3)) << 4));
-      if (LINEAR) {
-        if (row < n_valid) *reinterpret_cast<uint4 *>(out + my_off + (long long)row * row_stride + ch * 8) = v;
-      } else {
-        const long long off = __shfl_sync(0xffffffffu, my_off, row);
-        if ((vmask >> row) & 1u) *reinterpret_cast<uint4 *>(out + off + ch * 8) = v;
-      }
-    }
-    __syncwarp();
+  if (p.addend.p) {
+    const __nv_bfloat162 a = *reinterpret_cast<const __nv_bfloat162 *>(p.addend.p + add_off);
+    v0 += __low2float(a);
+    v1 += __high2float(a);
   }
-}
-
-// generic epilogue of the training-step kernels (see ConvKParams): 64 channels of one output pixel per thread
-__device__ __forceinline__ void epilogue_generic64(const uint32_t *r, const ConvKParams &p, const float *bias_s, uint8_t *stage,
-                                                   long long my_off, long long add_off, long long mask_off, bool my_valid,
-                                                   bool use_mask, bool chan_ok, int lane) {
-  __align__(16) __nv_bfloat16 h[64];
-  const bool has_bias = p.bias != nullptr;
-  const bool has_add = p.addend.p != nullptr && my_valid && chan_ok;
-  const bool has_mask = p.mask.p != nullptr && my_valid && use_mask && chan_ok;
-  const uint32_t ba = ptx::smem_u32(bias_s), sa = ptx::smem_u32(stage);
-#pragma unroll
-  for (int q = 0; q < 8; ++q) {
-    __align__(16) __nv_bfloat16 a8[8];
-    __align__(16) __nv_bfloat16 m8[8];
-    float b8[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (has_bias) {
-      const float4 b0 = lds128f(ba + q * 32), b1 = lds128f(ba + q * 32 + 16);
-      b8[0] = b0.x; b8[1] = b0.y; b8[2] = b0.z; b8[3] = b0.w; b8[4] = b1.x; b8[5] = b1.y; b8[6] = b1.z; b8[7] = b1.w;
+  if (p.mask.p) {
+    if (n < p.mask_climit) {
+      const __nv_bfloat162 m = *reinterpret_cast<const __nv_bfloat162 *>(p.mask.p + mask_off);
+      if (!(__low2float(m) > 0.f)) v0 *= p.slope;
+      if (!(__high2float(m) > 0.f)) v1 *= p.slope;
     }
-    if (has_add) *reinterpret_cast<uint4 *>(a8) = *reinterpret_cast<const uint4 *>(p.addend.p + add_off + q * 8);
-    if (has_mask) *reinterpret_cast<uint4 *>(m8) = *reinterpret_cast<const uint4 *>(p.mask.p + mask_off + q * 8);
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const int j = q * 8 + e;
-      float v = __uint_as_float(r[j]);
-      if (has_bias) v += b8[e];
-      if (has_add) v += __bfloat162float(a8[e]);
-      if (p.mask.p != nullptr) {
-        if (has_mask && !(__bfloat162float(m8[e]) > 0.f)) v *= p.slope;
-      } else {
-        v = v > 0.f ? v : v * p.slope;
-      }
-      h[j] = __float2bfloat16_rn(v);
-    }
+  } else {
+    v0 = v0 > 0.f ? v0 : v0 * p.slope;
+    v1 = v1 > 0.f ? v1 : v1 * p.slope;
   }
-  const unsigned vmask = __ballot_sync(0xffffffffu, my_valid && chan_ok);
-  const int ch = lane & 7;
-#pragma unroll
-  for (int c = 0; c < 8; ++c) sts128(sa + lane * 128 + ((c ^ (lane & 7)) << 4), *reinterpret_cast<const uint4 *>(h + c * 8));
-  __syncwarp();
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int row = i * 4 + (lane >> 3);
-    const long long off = __shfl_sync(0xffffffffu, my_off, row);
-    const uint4 v = lds128(sa + row * 128 + ((ch ^ (row & 7)) << 4));
-    if ((vmask >> row) & 1u) *reinterpret_cast<uint4 *>(p.out_hi + off + ch * 8) = v;
-  }
-  __syncwarp();
+  *reinterpret_cast<__nv_bfloat162 *>(p.out_hi + off) = __floats2bfloat162_rn(v0, v1);
 }
 
 // ---------------------------------------------------------------------------------------------
-// v2: persistent, warp-specialised, double-buffered TMEM accumulators.
-//   grid = min(#tiles, SMs x CTAs/SM); CTA c walks tiles c, c+G, c+2G ... (tile id = m*Nn + n,
-//   n fastest so CTAs that share an activation tile run side by side and hit it in L2 together).
-//   No split-K / tail splitting: measured slower than leaving the last partial wave to the batches in flight on the
-//   other streams (round-1 experiments: stream-K, tail K-slices + finalize kernel; DESIGN.md 5).
-//   The smem ring runs across tile boundaries (the producer is already loading tile t+1 while the
-//   epilogue of tile t drains its accumulator); two TMEM accumulator stages of BLOCK_N columns let the
-//   MMA warp start tile t+1 while warps 2..5 read tile t.
-//   RESIDENT_B (conv1: whole 64 x 512 weight matrix = 64 KB): weights are loaded once per CTA and stay
-//   in shared memory; the ring then carries activation tiles only.
-template <int BLOCK_N, int BLOCK_K, int STAGES, bool SPLIT3, bool RESIDENT_B, int KBLOCKS_RES>
+// Persistent, warp-specialised implicit GEMM.  grid = min(#tiles, SMs); CTA c walks tiles c, c+G, c+2G ... (tile id =
+// m*Nn + n, n fastest so CTAs that share an activation tile run side by side and hit it in L2 together).  The smem ring
+// runs across tile boundaries: the producer is already loading tile t+1 while the consumers store tile t.  A consumer
+// keeps one K block of wgmmas in flight (wait_group 1) and hands the stage of the previous block back to the producer.
+template <int BLOCK_N, int STAGES, bool SPLIT3>
 struct ConvSmem2 {
-  static constexpr int A_BYTES = 128 * BLOCK_K * 2;
-  static constexpr int B_BYTES = BLOCK_N * BLOCK_K * 2;
+  static constexpr int A_BYTES = 128 * 64 * 2;
+  static constexpr int B_BYTES = BLOCK_N * 64 * 2;
   static constexpr int NPREC = SPLIT3 ? 2 : 1;
-  static constexpr int STAGE_BYTES = (A_BYTES + (RESIDENT_B ? 0 : B_BYTES)) * NPREC;
-  static constexpr int RES_BYTES = RESIDENT_B ? KBLOCKS_RES * B_BYTES * NPREC : 0;
-  static constexpr int EPI_BYTES = 4 * 4096 + 4096 /*bias, up to 1024 channels*/;
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + RES_BYTES + EPI_BYTES + 1024 /*align slack*/ + 512 /*barriers*/;
+  static constexpr int STAGE_BYTES = (A_BYTES + B_BYTES) * NPREC;
+  static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(ptx::smem_u32(bar)) : "memory");
-}
-
-template <int BLOCK_N, int BLOCK_K, int STAGES, bool SPLIT3, bool RESIDENT_B, int KBLOCKS_RES, int EPI = 0>
-__global__ void __launch_bounds__(192) conv_igemm_persistent_kernel(const __grid_constant__ ConvKParams p,
-                                                                    const int total_tiles, const int n_tiles) {
-  using S = ConvSmem2<BLOCK_N, BLOCK_K, STAGES, SPLIT3, RESIDENT_B, KBLOCKS_RES>;
-  constexpr uint32_t LAYOUT = (BLOCK_K == 64) ? 2u : 4u;
-  constexpr uint32_t SBO = 8u * BLOCK_K * 2u;
-  constexpr uint32_t ACC_COLS = BLOCK_N < 32 ? 32 : BLOCK_N;
-  constexpr uint32_t TMEM_COLS = 2 * ACC_COLS;
+template <int BLOCK_N, int STAGES, bool SPLIT3, bool F16, int EPI = 0>
+__global__ void __launch_bounds__(384, 1) conv_igemm_persistent_kernel(const __grid_constant__ ConvKParams p,
+                                                                       const int total_tiles, const int n_tiles) {
+  using S = ConvSmem2<BLOCK_N, STAGES, SPLIT3>;
+  constexpr uint32_t SBO = 1024u;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t *res = smem + STAGES * S::STAGE_BYTES;
-  uint8_t *epi = res + S::RES_BYTES;
-  float *bias_s = reinterpret_cast<float *>(epi + 4 * 4096);
-  uint64_t *full_bar = reinterpret_cast<uint64_t *>(epi + S::EPI_BYTES);
+  uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + STAGES * S::STAGE_BYTES);
   uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *tmem_full_bar = empty_bar + STAGES;   // [2]
-  uint64_t *tmem_empty_bar = tmem_full_bar + 2;   // [2]
-  uint64_t *res_bar = tmem_empty_bar + 2;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(res_bar + 1);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int kb0 = 0, kb1 = p.kblocks;
+  const int wgi = threadIdx.x >> 7, warp = threadIdx.x >> 5;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
+      ptx::mbar_init(&empty_bar[s], 2);  // one arrive per consumer warpgroup
     }
-    for (int a = 0; a < 2; ++a) {
-      ptx::mbar_init(&tmem_full_bar[a], 1);
-      ptx::mbar_init(&tmem_empty_bar[a], 4);  // one arrive per epilogue warp
-    }
-    ptx::mbar_init(res_bar, 1);
     ptx::fence_barrier_init();
     ptx::prefetch_tmap(&p.b_map);
     ptx::prefetch_tmap(&p.a_map[0]);
   }
-  for (int c = threadIdx.x; c < p.Cout && c < 1024; c += blockDim.x) bias_s[c] = p.bias ? p.bias[c] : 0.f;
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, TMEM_COLS);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (whole warp, elected lane issues)
-    {
-      if (RESIDENT_B) {
-        ptx::mbar_expect_tx(res_bar, (uint32_t)S::RES_BYTES);
-        for (int kb = 0; kb < KBLOCKS_RES; ++kb) {
-          ptx::tma_load_2d(res + kb * S::B_BYTES, &p.b_map, res_bar, kb * BLOCK_K, 0);
-          if (SPLIT3) ptx::tma_load_2d(res + (KBLOCKS_RES + kb) * S::B_BYTES, &p.b_lo_map, res_bar, kb * BLOCK_K, 0);
-        }
-      }
-      const uint32_t tx = (uint32_t)(p.BW * p.BH * BLOCK_K * 2 + (RESIDENT_B ? 0 : BLOCK_N * BLOCK_K * 2)) * S::NPREC;
+  if (wgi == 0) {
+    ptx::regs_producer();
+    if (warp == 0) {
+      // ------------------------------------------------------------------ TMA producer (whole warp, elected lane issues)
+      const uint32_t tx = (uint32_t)(p.BW * p.BH * 64 * 2 + BLOCK_N * 64 * 2) * S::NPREC;
       int s = 0;
       uint32_t ph = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int nt = tile % n_tiles, mt = tile / n_tiles;
         const int col_tile = mt % p.n_col_tiles, row_tile = mt / p.n_col_tiles;
         const int g0 = row_tile * p.BH, ow0 = col_tile * p.BW, n0 = nt * BLOCK_N;
-        for (int kb = kb0; kb < kb1; ++kb) {
+        for (int kb = 0; kb < p.kblocks; ++kb) {
           ptx::mbar_wait(&empty_bar[s], ph ^ 1u);
           const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
           const int kh = tap / p.KW, kw = tap - kh * p.KW;
@@ -527,205 +295,136 @@ __global__ void __launch_bounds__(192) conv_igemm_persistent_kernel(const __grid
           if (EPI) { dr += p.in_off_r; dc += p.in_off_c; }
           if (ptx::elect_one()) {
             ptx::mbar_expect_tx_raw(&full_bar[s], tx);
-            ptx::tma_load_3d_raw(st, &p.a_map[view], &full_bar[s], cc * BLOCK_K, ow0 + dc, g0 + dr);
-            uint8_t *nxt = st + S::A_BYTES;
-            if (!RESIDENT_B) {
-              ptx::tma_load_2d_raw(nxt, &p.b_map, &full_bar[s], kb * BLOCK_K, n0);
-              nxt += S::B_BYTES;
-            }
+            ptx::tma_load_3d_raw(st, &p.a_map[view], &full_bar[s], cc * 64, ow0 + dc, g0 + dr);
+            ptx::tma_load_2d_raw(st + S::A_BYTES, &p.b_map, &full_bar[s], kb * 64, n0);
             if (SPLIT3) {
-              ptx::tma_load_3d_raw(nxt, &p.a_lo_map[view], &full_bar[s], cc * BLOCK_K, ow0 + dc, g0 + dr);
-              if (!RESIDENT_B) ptx::tma_load_2d_raw(nxt + S::A_BYTES, &p.b_lo_map, &full_bar[s], kb * BLOCK_K, n0);
+              ptx::tma_load_3d_raw(st + S::A_BYTES + S::B_BYTES, &p.a_lo_map[view], &full_bar[s], cc * 64, ow0 + dc, g0 + dr);
+              ptx::tma_load_2d_raw(st + 2 * S::A_BYTES + S::B_BYTES, &p.b_lo_map, &full_bar[s], kb * 64, n0);
             }
           }
           __syncwarp();
           if (++s == STAGES) { s = 0; ph ^= 1u; }
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (whole warp, elected lane issues)
-    {
-      if (RESIDENT_B) {
-        ptx::mbar_wait(res_bar, 0);
-        ptx::tc_fence_after();
-      }
-      int s = 0, as = 0;
-      uint32_t ph = 0, aph = 0;
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        ptx::mbar_wait(&tmem_empty_bar[as], aph ^ 1u);  // epilogue has drained this accumulator stage
-        ptx::tc_fence_after();
-        const uint32_t tmem_acc = tmem_base + (uint32_t)as * ACC_COLS;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(&full_bar[s], ph);
-          ptx::tc_fence_after();
-          const uint32_t a_hi = ptx::smem_u32(smem + s * S::STAGE_BYTES);
-          uint32_t b_hi, a_lo, b_lo;
-          if (RESIDENT_B) {
-            b_hi = ptx::smem_u32(res + kb * S::B_BYTES);
-            b_lo = ptx::smem_u32(res + (KBLOCKS_RES + kb) * S::B_BYTES);
-            a_lo = a_hi + S::A_BYTES;
-          } else {
-            b_hi = a_hi + S::A_BYTES;
-            a_lo = b_hi + S::B_BYTES;
-            b_lo = a_lo + S::A_BYTES;
-          }
-          if (ptx::elect_one()) {
-            const uint64_t da0 = ptx::umma_desc(a_hi, SBO, LAYOUT), db0 = ptx::umma_desc(b_hi, SBO, LAYOUT);
-            const uint64_t dal0 = ptx::umma_desc(a_lo, SBO, LAYOUT), dbl0 = ptx::umma_desc(b_lo, SBO, LAYOUT);
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / 16; ++k) {
-              const uint32_t acc = (kb > kb0 || k > 0) ? 1u : 0u;
-              const uint64_t da = da0 + (uint64_t)(2 * k), db = db0 + (uint64_t)(2 * k);  // + k * 32 bytes
-              ptx::umma_f16_raw(tmem_acc, da, db, p.idesc, acc);
-              if (SPLIT3) {
-                ptx::umma_f16_raw(tmem_acc, dal0 + (uint64_t)(2 * k), db, p.idesc, 1u);
-                ptx::umma_f16_raw(tmem_acc, da, dbl0 + (uint64_t)(2 * k), p.idesc, 1u);
-              }
-            }
-            ptx::umma_commit_raw(&empty_bar[s]);
-          }
-          __syncwarp();
-          if (++s == STAGES) { s = 0; ph ^= 1u; }
-        }
-        ptx::umma_commit(&tmem_full_bar[as]);
-        if (++as == 2) { as = 0; aph ^= 1u; }
       }
     }
   } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..5)
-    const int quad = warp & 3;
-    const int m = quad * 32 + lane;
-    const int bh = m / p.BW, bw = m - bh * p.BW;
-    uint8_t *stg = epi + (warp - 2) * 4096;
-    int as = 0;
-    uint32_t aph = 0;
+    ptx::regs_consumer();
+    // ------------------------------------------------------------------ consumers: rows 64*(wgi-1) .. +63 of the M tile
+    const int t = threadIdx.x & 127;
+    const int half = wgi - 1;
+    const int r0 = half * 64 + frag_row(t), q2 = (t & 3) * 2;
+    const bool arriver = t == 0;
+    const uint32_t base = ptx::smem_u32(smem);
+    float acc[BLOCK_N / 2];
+    int s = 0;
+    uint32_t ph = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      ptx::mbar_wait(&tmem_full_bar[as], aph);
-      ptx::tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)as * ACC_COLS;
-      if (EPI == 1) {
-        const int nt = tile % n_tiles, mt = tile / n_tiles;
-        const int col_tile = mt % p.n_col_tiles, row_tile = mt / p.n_col_tiles;
-        const int g = row_tile * p.BH + bh, ow = col_tile * p.BW + bw, n0 = nt * BLOCK_N;
-        const int n_img = g / p.Hq, oh = g - n_img * p.Hq;
-        const int y = oh * p.out_sy + p.out_oy, x = ow * p.out_sx + p.out_ox;
-        const bool valid = (m < p.BW * p.BH) && (n_img < p.Bn) && (oh < p.Ho) && (ow < p.Wo) && y >= 0 && y < p.out_H &&
-                           x >= 0 && x < p.out_W;
-        const long long my_off =
-            (((long long)n_img * p.out_Hp + y + p.out_py) * p.out_Wp + x + p.out_px) * p.out_cs + p.out_coff + n0;
-        const long long add_off =
-            (((long long)n_img * p.addend.Hp + y + p.addend.py) * p.addend.Wp + x + p.addend.px) * p.addend.cs + p.addend.coff + n0;
-        const long long mask_off =
-            (((long long)n_img * p.mask.Hp + y + p.mask.py) * p.mask.Wp + x + p.mask.px) * p.mask.cs + p.mask.coff + n0;
-#pragma unroll 1
-        for (int c = 0; c < BLOCK_N; c += 64) {
-          uint32_t r[64];
-          ptx::tmem_ld_32x32(trow + c, r);
-          ptx::tmem_ld_32x32(trow + c + 32, r + 32);
-          if (c + 64 >= BLOCK_N) {
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty_bar[as]);
+      int prev = -1;
+      for (int kb = 0; kb < p.kblocks; ++kb) {
+        ptx::mbar_wait(&full_bar[s], ph);
+        const uint32_t a_hi = base + s * S::STAGE_BYTES + half * 8192;
+        const uint32_t b_hi = base + s * S::STAGE_BYTES + S::A_BYTES;
+        const uint64_t da0 = ptx::gmma_desc(a_hi, 16, SBO, ptx::kSW128), db0 = ptx::gmma_desc(b_hi, 16, SBO, ptx::kSW128);
+        const uint64_t dal0 = da0 + ((S::A_BYTES + S::B_BYTES) >> 4), dbl0 = db0 + ((S::A_BYTES + S::B_BYTES) >> 4);
+        wg::fence_acc(acc);
+        wg::fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const uint64_t da = da0 + (uint64_t)(2 * k), db = db0 + (uint64_t)(2 * k);  // + k * 32 bytes
+          wg::mma<BLOCK_N, F16, 0, 0>(acc, da, db, (kb > 0 || k > 0) ? 1u : 0u);
+          if (SPLIT3) {
+            wg::mma<BLOCK_N, false, 0, 0>(acc, dal0 + (uint64_t)(2 * k), db, 1u);
+            wg::mma<BLOCK_N, false, 0, 0>(acc, da, dbl0 + (uint64_t)(2 * k), 1u);
           }
-          epilogue_generic64(r, p, bias_s + ((n0 + c) & 1023), stg, my_off + c, add_off + c, mask_off + c, valid,
-                             n0 + c < p.mask_climit, n0 + c < p.Cout, lane);
         }
-      } else {
-        const int nt = tile % n_tiles, mt = tile / n_tiles;
-        const int col_tile = mt % p.n_col_tiles, row_tile = mt / p.n_col_tiles;
-        const int g = row_tile * p.BH + bh, ow = col_tile * p.BW + bw, n0 = nt * BLOCK_N;
+        wg::commit();
+        wg::wait<1>();
+        wg::fence_acc(acc);
+        if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1u; }
+      }
+      wg::wait<0>();
+      wg::fence_acc(acc);
+      if (prev >= 0 && arriver) ptx::mbar_arrive(&empty_bar[prev]);
+
+      const int nt = tile % n_tiles, mt = tile / n_tiles;
+      const int col_tile = mt % p.n_col_tiles, row_tile = mt / p.n_col_tiles;
+      const int n0 = nt * BLOCK_N;
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int m = r0 + rr * 8;
+        const int bh = m / p.BW, bw = m - bh * p.BW;
+        const int g = row_tile * p.BH + bh, ow = col_tile * p.BW + bw;
         const int n_img = g / p.Hq, oh = g - n_img * p.Hq;
-        const bool valid = (m < p.BW * p.BH) && (n_img < p.Bn) && (oh < p.Ho) && (ow < p.Wo);
-        const long long my_off =
-            (((long long)n_img * p.out_Hp + oh + p.out_py) * p.out_Wp + ow + p.out_px) * p.Cout + n0;
-#pragma unroll 1
-        for (int c = 0; c < BLOCK_N; c += 64) {
-          uint32_t r[64];
-          ptx::tmem_ld_32x32(trow + c, r);
-          ptx::tmem_ld_32x32(trow + c + 32, r + 32);
-          if (c + 64 >= BLOCK_N) {  // last TMEM read of this tile: hand the accumulator stage back early
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty_bar[as]);
+        if (EPI == 1) {
+          const int y = oh * p.out_sy + p.out_oy, x = ow * p.out_sx + p.out_ox;
+          const bool valid = (m < p.BW * p.BH) && (n_img < p.Bn) && (oh < p.Ho) && (ow < p.Wo) && y >= 0 && y < p.out_H &&
+                             x >= 0 && x < p.out_W;
+          const long long off =
+              (((long long)n_img * p.out_Hp + y + p.out_py) * p.out_Wp + x + p.out_px) * p.out_cs + p.out_coff + n0 + q2;
+          const long long add_off =
+              (((long long)n_img * p.addend.Hp + y + p.addend.py) * p.addend.Wp + x + p.addend.px) * p.addend.cs + p.addend.coff +
+              n0 + q2;
+          const long long mask_off =
+              (((long long)n_img * p.mask.Hp + y + p.mask.py) * p.mask.Wp + x + p.mask.px) * p.mask.cs + p.mask.coff + n0 + q2;
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j)
+            store_pair_generic(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1], p, n0 + 8 * j + q2, valid, off + 8 * j,
+                               add_off + 8 * j, mask_off + 8 * j);
+        } else {
+          const bool valid = (m < p.BW * p.BH) && (n_img < p.Bn) && (oh < p.Ho) && (ow < p.Wo);
+          if (valid) {
+            const long long off = (((long long)n_img * p.out_Hp + oh + p.out_py) * p.out_Wp + ow + p.out_px) * p.Cout + n0 + q2;
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j)
+              store_pair<SPLIT3, F16>(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1],
+                                      make_float2(__ldg(p.bias + n0 + 8 * j + q2), __ldg(p.bias + n0 + 8 * j + q2 + 1)), p.slope, p.out_hi,
+                                      p.out_lo, off + 8 * j);
           }
-          epilogue_store64<SPLIT3>(r, bias_s + n0 + c, p.slope, stg, p.out_hi, p.out_lo, my_off + c, valid, lane, p.f16 != 0);
         }
       }
-      if (++as == 2) { as = 0; aph ^= 1u; }
     }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
 // ---------------------------------------------------------------------------------------------
 // conv1 (flow_conv1: 8 -> 64, 7x7 s2, i.e. 16 taps x 32 space-to-depth channels).  The generic path
-// fetches every tap's operand tile from L2 separately (16x re-read of the input: the layer is then
-// bound by L2 -> SMEM traffic, not by the tensor pipe).  Here one TMA box per filter row dh brings the
-// (BW+3)-pixel input strip into shared memory ONCE, in the un-swizzled K-major "interleave" layout
+// fetches every tap's operand tile from L2 separately (16x re-read of the input).  Here one TMA box per filter row dh
+// brings the (BW+3)-pixel input strip into shared memory ONCE, in the un-swizzled K-major layout
 //     addr(pixel r, channel-chunk c) = base + c*LBO + 16*r          (8-channel chunks of 16 B)
 // in which the row index is linear in memory, so the four horizontal taps dw = 0..3 are the same
-// strip read through descriptors whose start address is shifted by dw*16 bytes: 4 TMA loads per
-// tile instead of 16, the input is read from L2 ~4x instead of 16x.
+// strip read through descriptors whose start address is shifted by dw*16 bytes.
 // Input buffer layout (written by the zoom kernel): [B*Hs rows][4 chunks][Ws cols][8 ch] bf16.
-// Tile = one output row x BW output columns (BW <= 128; MMA rows >= BW are don't-care).
-// Weights: the whole 64 x 512 matrix stays resident in shared memory (64B-swizzled, 16 tap tiles).
-// elected lane
-__device__ __forceinline__ void tma_load_4d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2,
-                                            int c3) {
-  if (ptx::elect_one())
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
-          "r"(ptx::smem_u32(dst)),
-      "l"((uint64_t)map), "r"(ptx::smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ uint64_t umma_desc_interleave(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;  // version 1, layout type 0 = SWIZZLE_NONE
-  return d;
-}
-
-// conv1, rolling strips (used by the hi/lo precision; the single-pass precisions run conv1_stack_kernel below).  A CTA owns
-// one column tile and a CONTIGUOUS run of output rows [g_lo, g_hi) and walks down it: output row g uses the input strips
-// g .. g+3 (one per filter row dh), so moving to row g+1 needs ONE new strip; the other three are still in the ring --
-// every strip travels L2 -> shared memory once (plus a 3-row halo per chunk) instead of once per filter row.
-// Strip s of the chunk (input row g_lo + s) lives in ring slot s % STAGES from its TMA fill until the MMAs of output
-// row s (its last user) have completed (tcgen05.commit -> empty barrier).  Per output row: 4 dh x 4 dw x 2 K-halves of
-// 128 x 64 x 16 MMAs into one of two 64-column accumulator stages.  One CTA per SM (64 KB resident weights per precision
-// + the ring), grid = column tiles x chunks.  The per-row epilogue is a latency chain longer than the row's MMAs, so
-// EIGHT epilogue warps in two alternating sets of four (one warp per TMEM lane quadrant) drain the rows (320 threads).
-template <int STAGES, bool SPLIT3>
-__global__ void __launch_bounds__(320) conv1_roll_kernel(const __grid_constant__ ConvKParams p, const int rows_total,
-                                                         const int rows_per_chunk, const int chunks_per_col,
-                                                         const int strip_bytes /*per precision, multiple of 128*/) {
-  constexpr uint32_t ACC_COLS = 64, TMEM_COLS = 128;
+// Tile = one output row x BW output columns (BW <= 128; MMA rows >= BW are don't-care and read past the strip into the
+// slack behind the ring).  Weights: the whole 64 x 512 matrix stays resident in shared memory (64B-swizzled, 16 tap tiles).
+//
+// Rolling strips: a CTA owns one column tile and a CONTIGUOUS run of output rows [g_lo, g_hi) and walks down it: output
+// row t uses the input strips t .. t+3 (one per filter row dh), so moving to the next row needs ONE new strip; every strip
+// travels L2 -> shared memory once (plus a 3-row halo per chunk).  The two consumer warpgroups take alternate rows (each
+// the full M = 128 as two m64 halves) so that one runs its epilogue while the other's wgmmas run.  Strip s is used by rows
+// s-3 .. s; the warpgroup of parity p is done with strips <= t+1 after its row t (its next row t+2 starts at strip t+2),
+// so after row t it releases strips t and t+1: every strip gets one arrival from each warpgroup (the parity-1 warpgroup
+// never uses strip 0 and releases it up front).
+// Structurally-zero K steps are not issued: filter row 7 (dh = 3, odd input row) and filter column 7 (dw = 3, odd input
+// column) lie outside the 7 x 7 filter, so dh = 3 has no second K step and dw = 3 has ONE step over the input chunks
+// (0, 2) (weights packed in that order: conv1_kslot).
+template <int STAGES, bool SPLIT3, bool F16>
+__global__ void __launch_bounds__(384, 1) conv1_kernel(const __grid_constant__ ConvKParams p, const int rows_total,
+                                                       const int rows_per_chunk, const int chunks_per_col,
+                                                       const int strip_bytes /*per precision, multiple of 128*/) {
   constexpr int NPREC = SPLIT3 ? 2 : 1;
-  constexpr int STG = 2048;  // staging tile per epilogue warp
-  constexpr int B_BYTES = 64 * 32 * 2, RES_BYTES = 16 * B_BYTES * NPREC, EPI_BYTES = 8 * STG + 256;
+  constexpr int B_BYTES = 64 * 32 * 2, RES_BYTES = 16 * B_BYTES * NPREC;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 511) & ~(uintptr_t)511);
+  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t *res = smem;
   uint8_t *ring = smem + RES_BYTES;
   const int stage_bytes = strip_bytes * NPREC;
-  uint8_t *epi = ring + STAGES * stage_bytes;
-  float *bias_s = reinterpret_cast<float *>(epi + 8 * STG);
-  uint64_t *full_bar = reinterpret_cast<uint64_t *>(epi + EPI_BYTES);
+  uint64_t *full_bar = reinterpret_cast<uint64_t *>(ring + STAGES * stage_bytes + kConv1Slack);
   uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *tmem_full_bar = empty_bar + STAGES;
-  uint64_t *tmem_empty_bar = tmem_full_bar + 2;
-  uint64_t *res_bar = tmem_empty_bar + 2;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(res_bar + 1);
+  uint64_t *res_bar = empty_bar + STAGES;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wgi = threadIdx.x >> 7, warp = threadIdx.x >> 5;
   const int R = p.BW + 3;
   const uint32_t LBO = (uint32_t)R * 16u;
   const int ct = blockIdx.x / chunks_per_col, ck = blockIdx.x - ct * chunks_per_col;
@@ -735,639 +434,117 @@ __global__ void __launch_bounds__(320) conv1_roll_kernel(const __grid_constant__
   const int n_strips = n_rows > 0 ? n_rows + 3 : 0;
   const int ow0 = ct * p.BW;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      ptx::mbar_init(&tmem_full_bar[a], 1);
-      ptx::mbar_init(&tmem_empty_bar[a], 4);  // the four warps of the set that owns this stage
+      ptx::mbar_init(&empty_bar[s], 2);
     }
     ptx::mbar_init(res_bar, 1);
     ptx::fence_barrier_init();
     ptx::prefetch_tmap(&p.b_map);
     ptx::prefetch_tmap(&p.a_map[0]);
   }
-  if (threadIdx.x < 64) bias_s[threadIdx.x] = p.bias[threadIdx.x];
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, TMEM_COLS);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (n_rows > 0) {
-      ptx::mbar_expect_tx(res_bar, (uint32_t)RES_BYTES);
-      for (int kb = 0; kb < 16; ++kb) {
-        ptx::tma_load_2d(res + kb * B_BYTES, &p.b_map, res_bar, kb * 32, 0);
-        if (SPLIT3) ptx::tma_load_2d(res + (16 + kb) * B_BYTES, &p.b_lo_map, res_bar, kb * 32, 0);
+  if (wgi == 0) {
+    ptx::regs_producer();
+    if (warp == 0 && n_rows > 0) {
+      if (ptx::elect_one()) {
+        ptx::mbar_expect_tx_raw(res_bar, (uint32_t)RES_BYTES);
+        for (int kb = 0; kb < 16; ++kb) {
+          ptx::tma_load_2d_raw(res + kb * B_BYTES, &p.b_map, res_bar, kb * 32, 0);
+          if (SPLIT3) ptx::tma_load_2d_raw(res + (16 + kb) * B_BYTES, &p.b_lo_map, res_bar, kb * 32, 0);
+        }
       }
+      __syncwarp();
       const uint32_t tx = (uint32_t)(R * 64) * NPREC;
       for (int s = 0; s < n_strips; ++s) {
         const int slot = s % STAGES;
         ptx::mbar_wait(&empty_bar[slot], (((uint32_t)(s / STAGES)) & 1u) ^ 1u);
         uint8_t *st = ring + slot * stage_bytes;
         ptx::mbar_expect_tx(&full_bar[slot], tx);
-        tma_load_4d(st, &p.a_map[0], &full_bar[slot], 0, ow0, 0, g_lo + s);
-        if (SPLIT3) tma_load_4d(st + strip_bytes, &p.a_lo_map[0], &full_bar[slot], 0, ow0, 0, g_lo + s);
+        ptx::tma_load_4d(st, &p.a_map[0], &full_bar[slot], 0, ow0, 0, g_lo + s);
+        if (SPLIT3) ptx::tma_load_4d(st + strip_bytes, &p.a_lo_map[0], &full_bar[slot], 0, ow0, 0, g_lo + s);
       }
     }
-  } else if (warp == 1) {
-    if (n_rows > 0) {
-      ptx::mbar_wait(res_bar, 0);
-      ptx::tc_fence_after();
-      // everything that does not depend on the tile is formed once: ring-slot descriptor = dring + slot * slot_step, the four
-      // filter-row weight descriptors, the k step.  The MMA warp is one instruction stream; every scalar instruction
-      // between two MMA groups is exposed latency (measured: 2.5k cycles per tile for 0.9k cycles of MMAs).
-      const uint64_t dring = umma_desc_interleave(ptx::smem_u32(ring), LBO, 128);
-      const uint64_t dring_lo = umma_desc_interleave(ptx::smem_u32(ring) + (uint32_t)strip_bytes, LBO, 128);
-      // dw = 3 (kw = 6, 7): the odd input column (pw = 1) is outside the 7x7 filter, so its K step pairs the two pw = 0
-      // chunks (0 and 2: chunk stride 2 LBO) against weights packed in that order (conv1_kslot) and the other step is dropped
-      const uint64_t dring3 = umma_desc_interleave(ptx::smem_u32(ring), 2u * LBO, 128);
-      const uint64_t dring3_lo = umma_desc_interleave(ptx::smem_u32(ring) + (uint32_t)strip_bytes, 2u * LBO, 128);
-      const uint64_t slot_step = (uint64_t)((uint32_t)stage_bytes >> 4);
-      const uint64_t kstep = (uint64_t)(2u * LBO >> 4);
-      uint64_t dbh[4], dbl[4];
+  } else if (n_rows > 0) {
+    ptx::regs_consumer();
+    const int set = wgi - 1, t = threadIdx.x & 127;
+    const bool arriver = t == 0;
+    const int r0 = frag_row(t), q2 = (t & 3) * 2;
+    float2 bias[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) bias[j] = make_float2(__ldg(p.bias + 8 * j + q2), __ldg(p.bias + 8 * j + q2 + 1));
+    const uint32_t ring_a = ptx::smem_u32(ring);
+    // everything that does not depend on the row is formed once: ring-slot descriptor = dring + slot * slot_step
+    const uint64_t dring = ptx::gmma_desc(ring_a, LBO, 128, ptx::kNoSwizzle);
+    const uint64_t dring3 = ptx::gmma_desc(ring_a, 2u * LBO, 128, ptx::kNoSwizzle) + 3u;  // dw = 3: chunks 0 and 2, 3 pixels in
+    const uint64_t lo_step = (uint64_t)((uint32_t)strip_bytes >> 4);
+    const uint64_t slot_step = (uint64_t)((uint32_t)stage_bytes >> 4);
+    const uint64_t kstep = (uint64_t)(2u * LBO >> 4);
+    const uint64_t dres = ptx::gmma_desc(ptx::smem_u32(res), 16, 512, ptx::kSW64);
+    const uint64_t dres_lo = dres + (uint64_t)((16 * B_BYTES) >> 4);
+    const int n_cols_valid = min(p.BW, p.Wo - ow0);
+    ptx::mbar_wait(res_bar, 0);
+    if (set == 1 && arriver) ptx::mbar_arrive(&empty_bar[0]);
+    for (int row = set; row < n_rows; row += 2) {
+      float acc[2][32];
 #pragma unroll
       for (int dh = 0; dh < 4; ++dh) {
-        dbh[dh] = ptx::umma_desc(ptx::smem_u32(res) + dh * 4 * B_BYTES, 512, 4u);
-        dbl[dh] = ptx::umma_desc(ptx::smem_u32(res) + (16 + dh * 4) * B_BYTES, 512, 4u);
+        const int s = row + dh;
+        ptx::mbar_wait(&full_bar[s % STAGES], ((uint32_t)(s / STAGES)) & 1u);
       }
-      int as = 0, waited = 0;
-      uint32_t aph = 0;
-      for (int t = 0; t < n_rows; ++t) {
-        ptx::mbar_wait(&tmem_empty_bar[as], aph ^ 1u);
-        ptx::tc_fence_after();
-        const uint32_t tmem_acc = tmem_base + (uint32_t)as * ACC_COLS;
+      wg::fence_acc(acc[0]);
+      wg::fence_acc(acc[1]);
+      wg::fence();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
 #pragma unroll
         for (int dh = 0; dh < 4; ++dh) {
-          const int s = t + dh, slot = s % STAGES;
-          if (s >= waited) {  // first use of this strip
-            ptx::mbar_wait(&full_bar[slot], ((uint32_t)(s / STAGES)) & 1u);
-            ptx::tc_fence_after();
-            waited = s + 1;
-          }
-          if (ptx::elect_one()) {
-            const uint64_t da0 = dring + (uint64_t)slot * slot_step, dal0 = dring_lo + (uint64_t)slot * slot_step;
-            const uint64_t da3 = dring3 + (uint64_t)slot * slot_step + 3u, dal3 = dring3_lo + (uint64_t)slot * slot_step + 3u;
+          const uint64_t so = (uint64_t)((row + dh) % STAGES) * slot_step + (uint64_t)(h * 64);  // + 64 pixels of 16 B
 #pragma unroll
-            for (int k = 0; k < 2; ++k) {  // k-major like conv1_stack_kernel: same accumulation order, bitwise-equal results
+          for (int k = 0; k < 2; ++k) {
 #pragma unroll
-              for (int dw = 0; dw < 4; ++dw) {
-                if ((dh == 3 || dw == 3) && k == 1) continue;  // kh = 7 / kw = 7: outside the 7x7 filter, all-zero weights
-                const uint32_t acc = (dh | dw | k) ? 1u : 0u;
-                const uint64_t da = dw == 3 ? da3 : da0 + (uint64_t)dw + (uint64_t)k * kstep;
-                const uint64_t db = dbh[dh] + (uint64_t)(dw * (B_BYTES >> 4) + 2 * k);
-                ptx::umma_f16_raw(tmem_acc, da, db, p.idesc, acc);
-                if (SPLIT3) {
-                  ptx::umma_f16_raw(tmem_acc, dw == 3 ? dal3 : dal0 + (uint64_t)dw + (uint64_t)k * kstep, db, p.idesc, 1u);
-                  ptx::umma_f16_raw(tmem_acc, da, dbl[dh] + (uint64_t)(dw * (B_BYTES >> 4) + 2 * k), p.idesc, 1u);
-                }
-              }
-            }
-            if (dh == 3) {
-              ptx::umma_commit_raw(&empty_bar[t % STAGES]);  // strip t served output rows t-3 .. t: its slot may be refilled
-              ptx::umma_commit_raw(&tmem_full_bar[as]);
-            }
-          }
-          __syncwarp();
-        }
-        if (++as == 2) { as = 0; aph ^= 1u; }
-      }
-    }
-  } else {
-    // Two warp SETS of four (one warp per TMEM lane quadrant, all 64 columns): set k owns the tiles t = k (mod 2), i.e.
-    // accumulator stage k.  The epilogue of one tile is a LATENCY chain (barrier wake-up, tcgen05.ld, convert, stage, store:
-    // ~2k cycles measured) rather than a throughput limit; with alternating sets each chain has two tile periods to finish.
-    const int quad = warp & 3, set = (warp - 2) >> 2;
-    uint8_t *stg = epi + (warp - 2) * STG;
-    const int as = set;
-    uint32_t aph = 0;
-    // the tile is ONE output row: the warp's 32 rows are the consecutive pixels ow0 + quad*32 .. +31, 64 channels (128 B) apart
-    const int n_cols_valid = min(p.BW, p.Wo - ow0) - quad * 32;  // valid rows of this warp's quadrant (may be <= 0)
-    for (int t = set; t < n_rows; t += 2) {
-      const int g = g_lo + t;
-      const int n_img = g / p.Hq, oh = g - n_img * p.Hq;
-      const bool row_ok = (n_img < p.Bn) && (oh < p.Ho);
-      ptx::mbar_wait(&tmem_full_bar[as], aph);
-      ptx::tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)as * ACC_COLS;
-      const long long warp_off =
-          (((long long)n_img * p.out_Hp + oh + p.out_py) * p.out_Wp + (ow0 + quad * 32) + p.out_px) * 64;
-      uint32_t r[64];
-      ptx::tmem_ld_32x32(trow, r);
-      ptx::tmem_ld_32x32(trow + 32, r + 32);
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty_bar[as]);
-#pragma unroll
-      for (int half = 0; half < 2; ++half)
-        epilogue_store32<SPLIT3, true>(r + half * 32, bias_s + half * 32, p.slope, stg, p.out_hi, p.out_lo, warp_off + half * 32,
-                                             true, lane, p.f16 != 0, row_ok ? n_cols_valid : 0, 64);
-      aph ^= 1u;
-    }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// conv1, stacked-filter-rows variant (single-pass precisions).  With Cout = 64 an MMA is 128 x 64 x 16: its A operand
-// (4 KB) is re-read from shared memory for 32 cycles of tensor work and the kernel is bound by shared-memory bandwidth
-// (measured 2.1k cycles per output row for 0.9k cycles of MMAs, on one CTA or two per SM alike).  Here the FOUR filter
-// rows are stacked along N: B = [W_dh3; W_dh2; W_dh1; W_dh0] (256 x 16 per (dw, k) step), so one 128 x 256 x 16 MMA of
-// input strip s adds its contribution to the four output rows s-3 .. s at once and A is read once instead of four
-// times.  The accumulators live in eight 64-column TMEM blocks (all 512 columns): virtual row v (= output row g_lo + v - 3)
-// sits in block v mod 8; strip s touches the blocks of rows s .. s+3 -- ascending rows are descending dh, which is why B's
-// order is fixed -- starts row s+3 and completes row s.  Every MMA accumulates (no per-block overwrite exists): a block is
-// handed back ZEROED by the epilogue warps (tcgen05.st) after they drain it, four strips before it is needed again.  When
-// the 4-block window wraps past column 512 the MMA is split in two (N = 64 n1 + 64 (4 - n1)).  Every strip is loaded and
-// consumed exactly once; the 3-row halo of a chunk costs three extra strips whose partial rows are discarded.
-// Structurally-zero K steps are not issued: filter row 7 (dh = 3, odd input row) and filter column 7 (dw = 3, odd input
-// column) lie outside the 7 x 7 filter, so the k = 1 steps run on [W_dh2; W_dh1; W_dh0] only (N = 192, window shifted by
-// one block) and dw = 3 has ONE step over the input chunks (0, 2) (weights packed in that order: conv1_kslot) -- 1600
-// instead of 2048 MMA columns per strip.  MMAs of one shape / accumulator window are issued back to back (k-major).
-template <int STAGES>
-__global__ void __launch_bounds__(320) conv1_stack_kernel(const __grid_constant__ ConvKParams p, const int rows_total,
-                                                          const int rows_per_chunk, const int chunks_per_col,
-                                                          const int strip_bytes /*multiple of 128*/) {
-  constexpr uint32_t TMEM_COLS = 512;
-  constexpr int B_BYTES = 64 * 32 * 2 /*one (dh, dw) tile: 64 couts x 32 K*/, DW_BYTES = 4 * B_BYTES, RES_BYTES = 4 * DW_BYTES;
-  constexpr int EPI_BYTES = 8 * 2048 + 256;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 511) & ~(uintptr_t)511);
-  uint8_t *res = smem;                       // [dw][dh = 3,2,1,0][64 couts][32 K] SW64
-  uint8_t *ring = smem + RES_BYTES;
-  uint8_t *epi = ring + STAGES * strip_bytes;
-  float *bias_s = reinterpret_cast<float *>(epi + 8 * 2048);
-  uint64_t *full_bar = reinterpret_cast<uint64_t *>(epi + EPI_BYTES);
-  uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *acc_full_bar = empty_bar + STAGES;   // [8] row block complete (MMA warp -> epilogue)
-  uint64_t *acc_empty_bar = acc_full_bar + 8;    // [8] block drained and zeroed (8 epilogue warps -> MMA warp)
-  uint64_t *res_bar = acc_empty_bar + 8;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(res_bar + 1);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int R = p.BW + 3;
-  const uint32_t LBO = (uint32_t)R * 16u;
-  const int ct = blockIdx.x / chunks_per_col, ck = blockIdx.x - ct * chunks_per_col;
-  const int g_lo = ck * rows_per_chunk;
-  const int g_hi = min(rows_total, g_lo + rows_per_chunk);
-  const int n_rows = max(0, g_hi - g_lo);
-  const int n_strips = n_rows > 0 ? n_rows + 3 : 0;   // strip s = input row g_lo + s; it completes virtual row v = s
-  const int ow0 = ct * p.BW;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 8; ++a) {
-      ptx::mbar_init(&acc_full_bar[a], 1);
-      ptx::mbar_init(&acc_empty_bar[a], 4);  // the four warps of the set that drains this block (v and v + 8 have the same parity)
-    }
-    ptx::mbar_init(res_bar, 1);
-    ptx::fence_barrier_init();
-    ptx::prefetch_tmap(&p.b_map);
-    ptx::prefetch_tmap(&p.a_map[0]);
-  }
-  if (threadIdx.x < 64) bias_s[threadIdx.x] = p.bias[threadIdx.x];
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, TMEM_COLS);
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (warp >= 2) {  // all eight accumulator blocks start cleared: each epilogue warp zeroes its lane quadrant x column half
-    const int quad = warp & 3, half = (warp - 2) >> 2;
-    for (int b = 0; b < 8; ++b) ptx::tmem_zero_32x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(b * 64 + half * 32));
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx::tc_fence_after();
-
-  if (warp == 0) {
-    if (n_rows > 0) {
-      if (ptx::elect_one()) {
-        ptx::mbar_expect_tx_raw(res_bar, (uint32_t)RES_BYTES);
-        for (int dh = 0; dh < 4; ++dh)
-          for (int dw = 0; dw < 4; ++dw)  // global K order is (dh, dw, 32); resident order is [dw][3 - dh]
-            ptx::tma_load_2d_raw(res + dw * DW_BYTES + (3 - dh) * B_BYTES, &p.b_map, res_bar, (dh * 4 + dw) * 32, 0);
-      }
-      __syncwarp();
-      const uint32_t tx = (uint32_t)(R * 64);
-      for (int s = 0; s < n_strips; ++s) {
-        const int slot = s % STAGES;
-        ptx::mbar_wait(&empty_bar[slot], (((uint32_t)(s / STAGES)) & 1u) ^ 1u);
-        ptx::mbar_expect_tx(&full_bar[slot], tx);
-        tma_load_4d(ring + slot * strip_bytes, &p.a_map[0], &full_bar[slot], 0, ow0, 0, g_lo + s);
-      }
-    }
-  } else if (warp == 1) {
-    if (n_rows > 0) {
-      ptx::mbar_wait(res_bar, 0);
-      ptx::tc_fence_after();
-      const uint64_t dring = umma_desc_interleave(ptx::smem_u32(ring), LBO, 128);
-      const uint64_t dring3 = umma_desc_interleave(ptx::smem_u32(ring), 2u * LBO, 128);  // dw = 3: chunks 0 and 2 (see conv1_roll_kernel)
-      const uint64_t slot_step = (uint64_t)((uint32_t)strip_bytes >> 4);
-      const uint64_t kstep = (uint64_t)(2u * LBO >> 4);
-      const uint64_t dres = ptx::umma_desc(ptx::smem_u32(res), 512, 4u);
-      const uint32_t idesc0 = p.idesc & ~(0x3Fu << 17);  // N field cleared; N >> 3 goes to bits [17, 23)
-      for (int s = 0; s < n_strips; ++s) {
-        const int slot = s % STAGES;
-        const int vnew = s + 3;  // the row this strip starts: its block must have been drained and zeroed
-        ptx::mbar_wait(&acc_empty_bar[vnew & 7], (((uint32_t)(vnew >> 3)) & 1u) ^ 1u);
-        ptx::mbar_wait(&full_bar[slot], ((uint32_t)(s / STAGES)) & 1u);
-        ptx::tc_fence_after();
-        if (ptx::elect_one()) {
-          const uint64_t da0 = dring + (uint64_t)slot * slot_step;
-          const int b0 = s & 7;                         // first block of the window (row v = s, filter row dh = 3)
-          const int n1 = b0 <= 4 ? 4 : 8 - b0;          // blocks before the window wraps past column 512
-          const uint32_t d1 = tmem_base + (uint32_t)b0 * 64u, id1 = idesc0 | ((uint32_t)(n1 * 64 >> 3) << 17);
-          const uint32_t id2 = idesc0 | ((uint32_t)((4 - n1) * 64 >> 3) << 17);
-          // K half k = 1 holds the odd input rows (ph = 1): filter row 2 * 3 + 1 = 7 does not exist, W_dh3 is zero there, so
-          // those steps skip the window's first block: rows s+1 .. s+3 <- [W_dh2; W_dh1; W_dh0] (N = 192)
-          const int c0 = (b0 + 1) & 7;
-          const int m1 = c0 <= 5 ? 3 : 8 - c0;
-          const uint32_t e1 = tmem_base + (uint32_t)c0 * 64u, ie1 = idesc0 | ((uint32_t)(m1 * 64 >> 3) << 17);
-          const uint32_t ie2 = idesc0 | ((uint32_t)((3 - m1) * 64 >> 3) << 17);
-          // MMAs that share an instruction descriptor and an accumulator window are issued back to back (k-major order):
-          // alternating N = 256 / 192 / split shapes from one MMA to the next cost the tensor pipe a drain each time
-          uint64_t da[4], db[4];
-#pragma unroll
-          for (int dw = 0; dw < 4; ++dw) {
-            da[dw] = dw == 3 ? dring3 + (uint64_t)slot * slot_step + 3u : da0 + (uint64_t)dw;
-            db[dw] = dres + (uint64_t)(dw * (DW_BYTES >> 4));
-          }
-#pragma unroll
-          for (int dw = 0; dw < 4; ++dw) ptx::umma_f16_raw(d1, da[dw], db[dw], id1, 1u);
-          if (n1 < 4) {
-#pragma unroll
-            for (int dw = 0; dw < 4; ++dw) ptx::umma_f16_raw(tmem_base, da[dw], db[dw] + (uint64_t)(n1 * (B_BYTES >> 4)), id2, 1u);
-          }
-          // K half 1; dw = 3 has none (kw = 7 does not exist: its (chunk 1, chunk 3) step has all-zero weights)
-#pragma unroll
-          for (int dw = 0; dw < 3; ++dw) ptx::umma_f16_raw(e1, da[dw] + kstep, db[dw] + (uint64_t)(2 + (B_BYTES >> 4)), ie1, 1u);
-          if (m1 < 3) {
-#pragma unroll
-            for (int dw = 0; dw < 3; ++dw)
-              ptx::umma_f16_raw(tmem_base, da[dw] + kstep, db[dw] + (uint64_t)(2 + (1 + m1) * (B_BYTES >> 4)), ie2, 1u);
-          }
-          ptx::umma_commit_raw(&empty_bar[slot]);        // the strip is consumed
-          ptx::umma_commit_raw(&acc_full_bar[s & 7]);    // row v = s has all four contributions
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    const int quad = warp & 3, set = (warp - 2) >> 2;  // two warp sets alternate rows (see conv1_roll_kernel)
-    uint8_t *stg = epi + (warp - 2) * 2048;
-    const int n_cols_valid = min(p.BW, p.Wo - ow0) - quad * 32;
-    float breg[64];  // the 64 biases live in registers: the shared-memory pipe belongs to the tensor core's operand reads
-#pragma unroll
-    for (int j = 0; j < 64; ++j) breg[j] = bias_s[j];
-    for (int v = set; v < n_strips; v += 2) {  // one completed row per strip; rows v < 3 belong to the previous chunk: discarded
-      const int g = g_lo + v - 3;
-      const bool mine = v >= 3;  // v - 3 < n_rows holds by construction
-      int n_img = 0, oh = 0;
-      if (mine) { n_img = g / p.Hq; oh = g - n_img * p.Hq; }
-      const bool row_ok = mine && (n_img < p.Bn) && (oh < p.Ho);
-      ptx::mbar_wait(&acc_full_bar[v & 7], ((uint32_t)(v >> 3)) & 1u);
-      ptx::tc_fence_after();
-      const uint32_t tcol = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)((v & 7) * 64);
-      uint32_t r[64];
-      if (row_ok) {
-        ptx::tmem_ld_32x32(tcol, r);
-        ptx::tmem_ld_32x32(tcol + 32, r + 32);
-      }
-      ptx::tmem_zero_32x32(tcol);
-      ptx::tmem_zero_32x32(tcol + 32);
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty_bar[v & 7]);
-      if (row_ok) {
-        const long long warp_off =
-            (((long long)n_img * p.out_Hp + oh + p.out_py) * p.out_Wp + (ow0 + quad * 32) + p.out_px) * 64;
-#pragma unroll
-        for (int half = 0; half < 2; ++half)
-          epilogue_store32<false, true, true>(r + half * 32, breg + half * 32, p.slope, stg, p.out_hi, p.out_lo, warp_off + half * 32,
-                                              true, lane, p.f16 != 0, n_cols_valid, 64);
-      }
-    }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// v3: CTA-pair kernel (tcgen05.mma.cta_group::2).  Two CTAs of a cluster (same TPC) compute a
-// 256 x BLOCK_N tile: each CTA stages its own 128 activation rows and HALF of the weight tile; the
-// leader CTA issues the MMAs for both, the hardware reads the operand halves from both shared
-// memories and writes each CTA's 128 accumulator rows into its own TMEM.  Per CTA and K-block this
-// moves 16 KB (A) + BLOCK_N/2*128 B (B half) through shared memory for 128 x BLOCK_N x 64 MACs, i.e.
-// half the weight traffic of the 1-CTA kernel: the 1-CTA kernel is bound by shared-memory bandwidth
-// (operand reads + TMA fills), not by the tensor pipe.
-//   full[s]   : leader's barrier, completed by the TMA bytes of BOTH CTAs (peer-bit-masked address)
-//   empty[s]  : per CTA, released by the leader's tcgen05.commit multicast to both CTAs
-//   tmem_full : per CTA, multicast commit;  tmem_empty: leader's, 8 arrivals (4 epilogue warps x 2 CTAs)
-namespace ptx2 {
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // cute::Sm100MmaPeerBitMask: address of CTA 0's copy
-__device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2) {
-  if (ptx::elect_one())
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::
-          "r"(ptx::smem_u32(dst)),
-      "l"((uint64_t)map), "r"(ptx::smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1) {
-  if (ptx::elect_one())
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::
-          "r"(ptx::smem_u32(dst)),
-      "l"((uint64_t)map), "r"(ptx::smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t *slot_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(ptx::smem_u32(slot_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_raw(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %6, %7, %8, %9, %10, %11, %12}, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u), "r"(0u), "r"(0u), "r"(0u), "r"(0u), "r"(0u),
-      "r"(0u), "r"(0u)
-      : "memory");
-}
-// arrive on the barrier at this smem offset in BOTH CTAs when the issued MMAs have completed
-__device__ __forceinline__ void umma_commit_mc_raw(uint64_t *bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          ptx::smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_mc(uint64_t *bar) {  // elected lane
-  if (ptx::elect_one()) umma_commit_mc_raw(bar);
-}
-// arrive on the leader CTA's copy of a barrier
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t *bar) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, 0;\n\tmbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(
-          ptx::smem_u32(bar))
-      : "memory");
-}
-}  // namespace ptx2
-
-template <int BLOCK_N, int STAGES, bool SPLIT3>
-struct ConvSmemPair {
-  static constexpr int A_BYTES = 128 * 64 * 2;
-  static constexpr int B_BYTES = (BLOCK_N / 2) * 64 * 2;  // this CTA's half of the weight tile
-  static constexpr int NPREC = SPLIT3 ? 2 : 1;
-  static constexpr int STAGE_BYTES = (A_BYTES + B_BYTES) * NPREC;
-  static constexpr int EPI_BYTES = 4 * 4096 + 4096;
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + EPI_BYTES + 1024 + 512;
-};
-
-template <int BLOCK_N, int STAGES, bool SPLIT3>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(192)
-    conv_igemm_pair_kernel(const __grid_constant__ ConvKParams p, const int total_pair_tiles, const int n_tiles) {
-  using S = ConvSmemPair<BLOCK_N, STAGES, SPLIT3>;
-  constexpr uint32_t LAYOUT = 2u, SBO = 1024u;
-  constexpr uint32_t TMEM_COLS = 2 * BLOCK_N;
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t *epi = smem + STAGES * S::STAGE_BYTES;
-  float *bias_s = reinterpret_cast<float *>(epi + 4 * 4096);
-  uint64_t *full_bar = reinterpret_cast<uint64_t *>(epi + S::EPI_BYTES);
-  uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *tmem_full_bar = empty_bar + STAGES;
-  uint64_t *tmem_empty_bar = tmem_full_bar + 2;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tmem_empty_bar + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = ptx2::cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const int kb_per = (p.kblocks + p.ksplit - 1) / p.ksplit;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      ptx::mbar_init(&tmem_full_bar[a], 1);
-      ptx::mbar_init(&tmem_empty_bar[a], 8);  // 4 epilogue warps x 2 CTAs (leader's copy is the one used)
-    }
-    ptx::fence_barrier_init();
-    ptx::prefetch_tmap(&p.b2_map);
-    ptx::prefetch_tmap(&p.a_map[0]);
-  }
-  for (int c = threadIdx.x; c < p.Cout; c += blockDim.x) bias_s[c] = p.bias[c];
-  if (warp == 1) ptx2::tmem_alloc(tmem_slot, TMEM_COLS);
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx2::cluster_sync();  // both CTAs' barriers are initialised before any remote arrive / multicast commit
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {
-    // ------------------------------------------------------------------ TMA producer (both CTAs; whole warp, elected lane issues)
-    {
-      const uint32_t tx_cta = (uint32_t)(p.BW * p.BH * 64 * 2 + (BLOCK_N / 2) * 64 * 2) * S::NPREC;
-      int s = 0;
-      uint32_t ph = 0;
-      for (int tile = pair; tile < total_pair_tiles; tile += npairs) {
-        const int z = tile % p.ksplit, mn = tile / p.ksplit;
-        const int nt = mn % n_tiles, mt = 2 * (mn / n_tiles) + (int)rank;
-        const int col_tile = mt % p.n_col_tiles, row_tile = mt / p.n_col_tiles;
-        const int g0 = row_tile * p.BH, ow0 = col_tile * p.BW;
-        const int n0 = nt * BLOCK_N + (int)rank * (BLOCK_N / 2);
-        const int kb0 = z * kb_per, kb1 = min(p.kblocks, kb0 + kb_per);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(&empty_bar[s], ph ^ 1u);
-          const int tap = kb / p.cchunks, cc = kb - tap * p.cchunks;
-          const int kh = tap / p.KW, kw = tap - kh * p.KW;
-          int view = 0, dr = kh, dc = kw;
-          if (p.stride == 2) {
-            view = ((kh & 1) << 1) | (kw & 1);
-            dr = kh >> 1;
-            dc = kw >> 1;
-          }
-          uint8_t *st = smem + s * S::STAGE_BYTES;
-          if (leader) ptx::mbar_expect_tx(&full_bar[s], 2u * tx_cta);  // bytes landing in both CTAs (leader: CTA-uniform)
-          ptx2::tma_load_3d(st, &p.a_map[view], &full_bar[s], cc * 64, ow0 + dc, g0 + dr);
-          ptx2::tma_load_2d(st + S::A_BYTES, &p.b2_map, &full_bar[s], kb * 64, n0);
-          if (SPLIT3) {
-            ptx2::tma_load_3d(st + S::A_BYTES + S::B_BYTES, &p.a_lo_map[view], &full_bar[s], cc * 64, ow0 + dc, g0 + dr);
-            ptx2::tma_load_2d(st + 2 * S::A_BYTES + S::B_BYTES, &p.b2_lo_map, &full_bar[s], kb * 64, n0);
-          }
-          if (++s == STAGES) { s = 0; ph ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (leader CTA only; whole warp)
-    if (leader) {
-      int s = 0, as = 0;
-      uint32_t ph = 0, aph = 0;
-      for (int tile = pair; tile < total_pair_tiles; tile += npairs) {
-        const int z = tile % p.ksplit;
-        const int kb0 = z * kb_per, kb1 = min(p.kblocks, kb0 + kb_per);
-        ptx::mbar_wait(&tmem_empty_bar[as], aph ^ 1u);
-        ptx::tc_fence_after();
-        const uint32_t tmem_acc = tmem_base + (uint32_t)as * BLOCK_N;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          ptx::mbar_wait(&full_bar[s], ph);
-          ptx::tc_fence_after();
-          const uint32_t a_hi = ptx::smem_u32(smem + s * S::STAGE_BYTES);
-          const uint32_t b_hi = a_hi + S::A_BYTES;
-          const uint32_t a_lo = b_hi + S::B_BYTES;
-          const uint32_t b_lo = a_lo + S::A_BYTES;
-          if (ptx::elect_one()) {
-            const uint64_t da0 = ptx::umma_desc(a_hi, SBO, LAYOUT), db0 = ptx::umma_desc(b_hi, SBO, LAYOUT);
-            const uint64_t dal0 = ptx::umma_desc(a_lo, SBO, LAYOUT), dbl0 = ptx::umma_desc(b_lo, SBO, LAYOUT);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint32_t acc = (kb > kb0 || k > 0) ? 1u : 0u;
-              const uint64_t da = da0 + (uint64_t)(2 * k), db = db0 + (uint64_t)(2 * k);
-              ptx2::umma_f16_raw(tmem_acc, da, db, p.idesc, acc);
+            for (int dw = 0; dw < 4; ++dw) {
+              if ((dh == 3 || dw == 3) && k == 1) continue;  // kh = 7 / kw = 7: outside the 7x7 filter, all-zero weights
+              const uint64_t da = (dw == 3 ? dring3 : dring + (uint64_t)dw + (uint64_t)k * kstep) + so;
+              const uint64_t wo = (uint64_t)((dh * 4 + dw) * (B_BYTES >> 4) + 2 * k);
+              wg::mma<64, F16, 0, 0>(acc[h], da, dres + wo, (dh | dw | k) ? 1u : 0u);
               if (SPLIT3) {
-                ptx2::umma_f16_raw(tmem_acc, dal0 + (uint64_t)(2 * k), db, p.idesc, 1u);
-                ptx2::umma_f16_raw(tmem_acc, da, dbl0 + (uint64_t)(2 * k), p.idesc, 1u);
+                wg::mma<64, false, 0, 0>(acc[h], da + lo_step, dres + wo, 1u);
+                wg::mma<64, false, 0, 0>(acc[h], da, dres_lo + wo, 1u);
               }
             }
-            ptx2::umma_commit_mc_raw(&empty_bar[s]);
           }
-          __syncwarp();
-          if (++s == STAGES) { s = 0; ph ^= 1u; }
         }
-        ptx2::umma_commit_mc(&tmem_full_bar[as]);
-        if (++as == 2) { as = 0; aph ^= 1u; }
       }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..5, both CTAs)
-    const int quad = warp & 3;
-    const int m = quad * 32 + lane;
-    const int bh = m / p.BW, bw = m - bh * p.BW;
-    uint8_t *stg = epi + (warp - 2) * 4096;
-    int as = 0;
-    uint32_t aph = 0;
-    for (int tile = pair; tile < total_pair_tiles; tile += npairs) {
-      const int z = tile % p.ksplit, mn = tile / p.ksplit;
-      const int nt = mn % n_tiles, mt = 2 * (mn / n_tiles) + (int)rank;
-      const int col_tile = mt % p.n_col_tiles, row_tile = mt / p.n_col_tiles;
-      const int g = row_tile * p.BH + bh, ow = col_tile * p.BW + bw, n0 = nt * BLOCK_N;
+      wg::commit();
+      wg::wait<0>();
+      wg::fence_acc(acc[0]);
+      wg::fence_acc(acc[1]);
+      if (arriver) {
+        ptx::mbar_arrive(&empty_bar[row % STAGES]);
+        ptx::mbar_arrive(&empty_bar[(row + 1) % STAGES]);
+      }
+      const int g = g_lo + row;
       const int n_img = g / p.Hq, oh = g - n_img * p.Hq;
-      const bool valid = (m < p.BW * p.BH) && (n_img < p.Bn) && (oh < p.Ho) && (ow < p.Wo);
-      ptx::mbar_wait(&tmem_full_bar[as], aph);
-      ptx::tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)as * BLOCK_N;
-      if (p.ksplit > 1) {
-        const size_t opix = ((size_t)n_img * p.Ho + oh) * p.Wo + ow;
-        float *dst = p.partial + ((size_t)z * ((size_t)p.Bn * p.Ho * p.Wo) + opix) * p.Cout + n0;
-#pragma unroll 1
-        for (int c = 0; c < BLOCK_N; c += 32) {
-          uint32_t r[32];
-          ptx::tmem_ld_32x32(trow + c, r);
-          if (valid) {
+      if (n_img < p.Bn && oh < p.Ho) {
+        const long long row_off = (((long long)n_img * p.out_Hp + oh + p.out_py) * p.out_Wp + ow0 + p.out_px) * 64 + q2;
 #pragma unroll
-            for (int j = 0; j < 32; j += 4)
-              *reinterpret_cast<uint4 *>(dst + c + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const int m = h * 64 + r0 + rr * 8;
+            if (m < n_cols_valid) {
+#pragma unroll
+              for (int j = 0; j < 8; ++j)
+                store_pair<SPLIT3, F16>(acc[h][4 * j + 2 * rr], acc[h][4 * j + 2 * rr + 1], bias[j], p.slope, p.out_hi, p.out_lo,
+                                        row_off + (long long)m * 64 + 8 * j);
+            }
           }
-        }
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx2::mbar_arrive_leader(&tmem_empty_bar[as]);
-      } else {
-        const long long my_off =
-            (((long long)n_img * p.out_Hp + oh + p.out_py) * p.out_Wp + ow + p.out_px) * p.Cout + n0;
-#pragma unroll 1
-        for (int c = 0; c < BLOCK_N; c += 64) {
-          uint32_t r[64];
-          ptx::tmem_ld_32x32(trow + c, r);
-          ptx::tmem_ld_32x32(trow + c + 32, r + 32);
-          if (c + 64 >= BLOCK_N) {
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx2::mbar_arrive_leader(&tmem_empty_bar[as]);
-          }
-          epilogue_store64<SPLIT3>(r, bias_s + n0 + c, p.slope, stg, p.out_hi, p.out_lo, my_off + c, valid, lane, p.f16 != 0);
-        }
       }
-      if (++as == 2) { as = 0; aph ^= 1u; }
     }
   }
-  ptx::tc_fence_before();
-  __syncthreads();
-  ptx2::cluster_sync();  // the peer may still be signalling our barriers / reading our shared memory
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx2::tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// split-K finalize: sum partials + bias + LeakyReLU -> bf16 (hi[, lo]) into the bordered NHWC buffer
-static __global__ void __launch_bounds__(256) conv_splitk_finalize_kernel(const float *partial, int ksplit, int npix,
-                                                                   int Cout, int Ho, int Wo, int out_Hp, int out_Wp,
-                                                                   int out_py, int out_px, const float *bias,
-                                                                   float slope, __nv_bfloat16 *out_hi,
-                                                                   __nv_bfloat16 *out_lo, int f16) {
-  const size_t idx4 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
-  if (idx4 >= (size_t)npix * Cout) return;
-  const size_t opix = idx4 / Cout;
-  const int c = (int)(idx4 - opix * Cout);
-  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int z = 0; z < ksplit; ++z) {
-    const float4 v = *reinterpret_cast<const float4 *>(partial + (size_t)z * npix * Cout + idx4);
-    acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
-  }
-  float v[4] = {acc.x + bias[c], acc.y + bias[c + 1], acc.z + bias[c + 2], acc.w + bias[c + 3]};
-  const int n_img = (int)(opix / ((size_t)Ho * Wo));
-  const int rem = (int)(opix - (size_t)n_img * Ho * Wo);
-  const int oh = rem / Wo, ow = rem - oh * Wo;
-  const size_t pix = ((size_t)n_img * out_Hp + oh + out_py) * out_Wp + ow + out_px;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) v[j] = v[j] > 0.f ? v[j] : v[j] * slope;
-  if (f16) {
-    *reinterpret_cast<uint2 *>(out_hi + pix * Cout + c) = make_uint2(pack2_f16(v[0], v[1]), pack2_f16(v[2], v[3]));
-    return;
-  }
-  const uint32_t h0 = pack2_bf16(v[0], v[1]), h1 = pack2_bf16(v[2], v[3]);
-  *reinterpret_cast<uint2 *>(out_hi + pix * Cout + c) = make_uint2(h0, h1);
-  if (out_lo)
-    *reinterpret_cast<uint2 *>(out_lo + pix * Cout + c) =
-        make_uint2(pack2_bf16(v[0] - __uint_as_float(h0 << 16), v[1] - __uint_as_float(h0 & 0xFFFF0000u)),
-                   pack2_bf16(v[2] - __uint_as_float(h1 << 16), v[3] - __uint_as_float(h1 & 0xFFFF0000u)));
 }
 
 }  // namespace dim

@@ -1,20 +1,20 @@
-// conv_wgrad.cuh -- weight gradients of the convolutions / deconvolutions on tcgen05 (training step,
+// conv_wgrad.cuh -- weight gradients of the convolutions / deconvolutions on wgmma (training step,
 // SURVEY 8 row a10; replaces cuDNN's backward-filter behind mx.symbol.Convolution/Deconvolution).
 //
 //   dW[m][tap][n] = sum over pixels (b, y, x) of  Z[b, y, x, m] * A[b, y*s + kh, x*s + kw, n]
 //
 // i.e. per filter tap one GEMM with M = channels of Z (the output gradient dZ for a convolution, the input
 // activation for a deconvolution), N = channels of A and the pixel index as the contraction dimension.
-// Both operands are NHWC, so the contraction index is the STRIDED one: the tiles are MN-major UMMA
-// operands (instruction-descriptor bits 15/16), which is exactly what a TMA box {64 channels, BW, BH}
-// with the 128-byte swizzle produces (row = pixel, 128 B = 64 channels):
-//     canonical layout ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units  (cute mma_traits_sm100 make_umma_desc<MN>)
-//     -> LBO = bytes between 64-channel groups (one TMA box = 8 KB), SBO = 1024 (8 pixel rows of 128 B).
+// Both operands are NHWC, so the contraction index is the STRIDED one: the tiles are MN-major (transposed)
+// wgmma operands, which is exactly what a TMA box {64 channels, BW, BH} with the 128-byte swizzle produces
+// (row = pixel, 128 B = 64 channels): LBO = bytes between 64-channel groups (one TMA box = 8 KB), SBO = 1024
+// (8 pixel rows of 128 B).
 // A K block is a BW x BH = 64 pixel rectangle of ONE image (4-D tensor maps carry the batch index, so a
 // block never straddles images); rows/cols beyond the buffer are zero-filled by TMA, the zero border of the
 // Z buffer makes overhanging pixels contribute nothing.
 // Work item = (K slice, tap, M tile, N tile); fp32 partial tiles are reduced (fixed order -> deterministic)
 // and re-laid out to the MXNet parameter layout by wgrad_reduce_kernel.
+// Warp roles as in conv_igemm.cuh: warp 0 loads, warpgroups 1 and 2 each own 64 of the 128 M rows.
 #pragma once
 #include "conv_igemm.cuh"
 
@@ -27,23 +27,48 @@ struct WgradParams {
   int BW, BH, rects_x, rects_y, Bn;
   int z_off_r, z_off_c, a_off_r, a_off_c;
   int m_tiles, n_tiles, kslices, kb_per_slice, kb_total;
-  uint32_t idesc;
   float *partial;  // [kslices][taps][m_tiles*128][n_tiles*BN]
 };
 
-namespace ptx {
-// MN-major swizzled operand descriptor: LBO = stride between 64-element (SW128) / 32-element (SW64) groups along
-// M/N, SBO = stride between groups of 8 K rows.
-__device__ __forceinline__ uint64_t umma_desc_mn(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)layout_type << 61;
-  return d;
+// consumer side shared by both wgrad kernels: K blocks [kb0, kb1) of the ring, then the fp32 tile rows of this warpgroup
+// (M rows 64*half .. +63) to dst (row stride ld floats).  a_off: byte offset of this warpgroup's M half in a stage.
+template <int BN, int STAGES, int STAGE_BYTES, int A_BYTES>
+__device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full_bar, uint64_t *empty_bar, int kb0, int kb1, int half,
+                                              uint64_t da_proto, uint32_t a_kstep, uint64_t db_proto, uint32_t b_kstep,
+                                              float *dst, size_t ld) {
+  const int t = threadIdx.x & 127;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  const uint32_t base = ptx::smem_u32(smem);
+  int s = 0, prev = -1;
+  uint32_t ph = 0;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    ptx::mbar_wait(&full_bar[s], ph);
+    const uint32_t st = base + s * STAGE_BYTES;
+    const uint64_t da0 = da_proto + (uint64_t)(st >> 4), db0 = db_proto + (uint64_t)((st + A_BYTES) >> 4);
+    wg::fence_acc(acc);
+    wg::fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)  // 64 pixels = 4 x K 16
+      wg::mma<BN, false, 1, 1>(acc, da0 + (uint64_t)(k * a_kstep), db0 + (uint64_t)(k * b_kstep), 1u);
+    wg::commit();
+    wg::wait<1>();
+    wg::fence_acc(acc);
+    if (prev >= 0 && t == 0) ptx::mbar_arrive(&empty_bar[prev]);
+    prev = s;
+    if (++s == STAGES) { s = 0; ph ^= 1u; }
+  }
+  wg::wait<0>();
+  wg::fence_acc(acc);
+  if (prev >= 0 && t == 0) ptx::mbar_arrive(&empty_bar[prev]);
+  const int r = half * 64 + frag_row(t), q2 = (t & 3) * 2;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    *reinterpret_cast<float2 *>(dst + (size_t)r * ld + 8 * j + q2) = make_float2(acc[4 * j], acc[4 * j + 1]);
+    *reinterpret_cast<float2 *>(dst + (size_t)(r + 8) * ld + 8 * j + q2) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+  }
 }
-}  // namespace ptx
 
 template <int BN, int STAGES>
 struct WgradSmem {
@@ -54,17 +79,14 @@ struct WgradSmem {
 };
 
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(192) conv_wgrad_kernel(const __grid_constant__ WgradParams p) {
+__global__ void __launch_bounds__(384, 1) conv_wgrad_kernel(const __grid_constant__ WgradParams p) {
   using S = WgradSmem<BN, STAGES>;
-  constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + STAGES * S::STAGE_BYTES);
   uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *done_bar = empty_bar + STAGES;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(done_bar + 1);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wgi = threadIdx.x >> 7, warp = threadIdx.x >> 5;
   const int taps = p.KH * p.KW;
   int w = blockIdx.x;
   const int nt = w % p.n_tiles; w /= p.n_tiles;
@@ -74,24 +96,20 @@ __global__ void __launch_bounds__(192) conv_wgrad_kernel(const __grid_constant__
   const int kb0 = slice * p.kb_per_slice;
   const int kb1 = min(p.kb_total, kb0 + p.kb_per_slice);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
+      ptx::mbar_init(&empty_bar[s], 2);
     }
-    ptx::mbar_init(done_bar, 1);
     ptx::fence_barrier_init();
     ptx::prefetch_tmap(&p.z_map);
     ptx::prefetch_tmap(&p.a_map[0]);
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, TMEM_COLS);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    {  // whole warp; the elected lane issues (conv_igemm.cuh ptx::elect_one)
+  if (wgi == 0) {
+    ptx::regs_producer();
+    if (warp == 0) {  // whole warp; the elected lane issues (conv_igemm.cuh ptx::elect_one)
       const int kh = tap / p.KW, kw = tap - kh * p.KW;
       int view = 0, dr = kh, dc = kw;
       if (p.stride == 2) {
@@ -109,71 +127,30 @@ __global__ void __launch_bounds__(192) conv_wgrad_kernel(const __grid_constant__
         const int oy0 = ry * p.BH, ox0 = rx * p.BW;
         uint8_t *st = smem + s * S::STAGE_BYTES;
         ptx::mbar_expect_tx(&full_bar[s], (uint32_t)S::STAGE_BYTES);
-        tma_load_4d(st, &p.z_map, &full_bar[s], mt * 128, ox0 + p.z_off_c, oy0 + p.z_off_r, b);
-        tma_load_4d(st + 8192, &p.z_map, &full_bar[s], mt * 128 + 64, ox0 + p.z_off_c, oy0 + p.z_off_r, b);
+        ptx::tma_load_4d(st, &p.z_map, &full_bar[s], mt * 128, ox0 + p.z_off_c, oy0 + p.z_off_r, b);
+        ptx::tma_load_4d(st + 8192, &p.z_map, &full_bar[s], mt * 128 + 64, ox0 + p.z_off_c, oy0 + p.z_off_r, b);
         uint8_t *bs = st + S::A_BYTES;
         if (BN >= 64) {
 #pragma unroll
           for (int j = 0; j < BN / 64; ++j)
-            tma_load_4d(bs + j * 8192, &p.a_map[view], &full_bar[s], nt * BN + j * 64, ox0 + dc + p.a_off_c,
-                        oy0 + dr + p.a_off_r, b);
+            ptx::tma_load_4d(bs + j * 8192, &p.a_map[view], &full_bar[s], nt * BN + j * 64, ox0 + dc + p.a_off_c,
+                             oy0 + dr + p.a_off_r, b);
         } else {
-          tma_load_4d(bs, &p.a_map[view], &full_bar[s], nt * BN, ox0 + dc + p.a_off_c, oy0 + dr + p.a_off_r, b);
+          ptx::tma_load_4d(bs, &p.a_map[view], &full_bar[s], nt * BN, ox0 + dc + p.a_off_c, oy0 + dr + p.a_off_r, b);
         }
         if (++s == STAGES) { s = 0; ph ^= 1u; }
       }
-    }
-  } else if (warp == 1) {
-    {  // whole warp; the elected lane issues
-      int s = 0;
-      uint32_t ph = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        ptx::mbar_wait(&full_bar[s], ph);
-        ptx::tc_fence_after();
-        const uint32_t a0 = ptx::smem_u32(smem + s * S::STAGE_BYTES);
-        const uint32_t b0 = a0 + S::A_BYTES;
-        if (ptx::elect_one()) {  // one election per K-block; descriptors advance by (bytes >> 4)
-          const uint64_t da0 = ptx::umma_desc_mn(a0, 8192, 1024, 2u);
-          const uint64_t db0 = BN >= 64 ? ptx::umma_desc_mn(b0, 8192, 1024, 2u) : ptx::umma_desc_mn(b0, 4096, 512, 4u);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)  // 64 pixels = 4 x UMMA_K 16
-            ptx::umma_f16_raw(tmem_base, da0 + (uint64_t)(k * 128), db0 + (uint64_t)(k * (BN >= 64 ? 128 : 64)), p.idesc,
-                              (kb > kb0 || k > 0) ? 1u : 0u);
-          ptx::umma_commit_raw(&empty_bar[s]);
-        }
-        __syncwarp();
-        if (++s == STAGES) { s = 0; ph ^= 1u; }
-      }
-      ptx::umma_commit(done_bar);
     }
   } else {
-    const int quad = warp & 3;
-    const int m = quad * 32 + lane;
-    if (kb1 > kb0) {
-      ptx::mbar_wait(done_bar, 0);
-      ptx::tc_fence_after();
-    }
+    ptx::regs_consumer();
+    const int half = wgi - 1;
     const size_t Mp = (size_t)p.m_tiles * 128, Np = (size_t)p.n_tiles * BN;
-    float *dst = p.partial + (((size_t)slice * taps + tap) * Mp + (size_t)mt * 128 + m) * Np + (size_t)nt * BN;
-    const uint32_t trow = tmem_base + ((uint32_t)(quad * 32) << 16);
-#pragma unroll 1
-    for (int c = 0; c < BN; c += 32) {
-      uint32_t r[32];
-      if (kb1 > kb0) {
-        ptx::tmem_ld_32x32(trow + c, r);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = 0u;
-      }
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) *reinterpret_cast<uint4 *>(dst + c + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
-    }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, TMEM_COLS);
+    float *dst = p.partial + (((size_t)slice * taps + tap) * Mp + (size_t)mt * 128) * Np + (size_t)nt * BN;
+    // A: this warpgroup's 64 channels are one 8 KB box; per K step of 16 pixels both operands advance 16 rows
+    const uint64_t da = ptx::gmma_desc(half * 8192, 8192, 1024, ptx::kSW128);
+    const uint64_t db = BN >= 64 ? ptx::gmma_desc(0, 8192, 1024, ptx::kSW128) : ptx::gmma_desc(0, 4096, 512, ptx::kSW64);
+    wgrad_consume<BN, STAGES, S::STAGE_BYTES, S::A_BYTES>(smem, full_bar, empty_bar, kb0, kb1, half, da, 128, db,
+                                                          BN >= 64 ? 128 : 64, dst, Np);
   }
 }
 
@@ -222,35 +199,29 @@ struct Conv1WgradSmem {
 };
 
 template <int STAGES>
-__global__ void __launch_bounds__(192) conv1_wgrad_kernel(const __grid_constant__ WgradParams p) {
+__global__ void __launch_bounds__(384, 1) conv1_wgrad_kernel(const __grid_constant__ WgradParams p) {
   using S = Conv1WgradSmem<STAGES>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + STAGES * S::STAGE_BYTES);
   uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *done_bar = empty_bar + STAGES;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(done_bar + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wgi = threadIdx.x >> 7, warp = threadIdx.x >> 5;
   const int dh = blockIdx.x % 4, slice = blockIdx.x / 4;
   const int kb0 = slice * p.kb_per_slice;
   const int kb1 = min(p.kb_total, kb0 + p.kb_per_slice);
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], 1);
+      ptx::mbar_init(&empty_bar[s], 2);
     }
-    ptx::mbar_init(done_bar, 1);
     ptx::fence_barrier_init();
     ptx::prefetch_tmap(&p.z_map);
     ptx::prefetch_tmap(&p.a_map[0]);
   }
-  if (warp == 1) ptx::tmem_alloc(tmem_slot, 64);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (warp == 0) {
-    {  // whole warp; the elected lane issues (conv_igemm.cuh ptx::elect_one)
+  if (wgi == 0) {
+    ptx::regs_producer();
+    if (warp == 0) {  // whole warp; the elected lane issues (conv_igemm.cuh ptx::elect_one)
       int s = 0;
       uint32_t ph = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
@@ -262,59 +233,19 @@ __global__ void __launch_bounds__(192) conv1_wgrad_kernel(const __grid_constant_
         uint8_t *st = smem + s * S::STAGE_BYTES;
         ptx::mbar_expect_tx(&full_bar[s], (uint32_t)S::STAGE_BYTES);
 #pragma unroll
-        for (int dw = 0; dw < 4; ++dw) tma_load_4d(st + dw * 4096, &p.a_map[0], &full_bar[s], 0, ox0 + dw, oy0 + dh, b);
-        tma_load_4d(st + S::A_BYTES, &p.z_map, &full_bar[s], 0, ox0 + p.z_off_c, oy0 + p.z_off_r, b);
+        for (int dw = 0; dw < 4; ++dw) ptx::tma_load_4d(st + dw * 4096, &p.a_map[0], &full_bar[s], 0, ox0 + dw, oy0 + dh, b);
+        ptx::tma_load_4d(st + S::A_BYTES, &p.z_map, &full_bar[s], 0, ox0 + p.z_off_c, oy0 + p.z_off_r, b);
         if (++s == STAGES) { s = 0; ph ^= 1u; }
       }
-    }
-  } else if (warp == 1) {
-    {  // whole warp; the elected lane issues
-      int s = 0;
-      uint32_t ph = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        ptx::mbar_wait(&full_bar[s], ph);
-        ptx::tc_fence_after();
-        const uint32_t a0 = ptx::smem_u32(smem + s * S::STAGE_BYTES);
-        const uint32_t b0 = a0 + S::A_BYTES;
-        if (ptx::elect_one()) {
-          const uint64_t da0 = ptx::umma_desc_mn(a0, 4096, 512, 4u), db0 = ptx::umma_desc_mn(b0, 8192, 1024, 2u);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            ptx::umma_f16_raw(tmem_base, da0 + (uint64_t)(k * 64), db0 + (uint64_t)(k * 128), p.idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          ptx::umma_commit_raw(&empty_bar[s]);
-        }
-        __syncwarp();
-        if (++s == STAGES) { s = 0; ph ^= 1u; }
-      }
-      ptx::umma_commit(done_bar);
     }
   } else {
-    const int quad = warp & 3;
-    const int m = quad * 32 + lane;
-    if (kb1 > kb0) {
-      ptx::mbar_wait(done_bar, 0);
-      ptx::tc_fence_after();
-    }
-    float *dst = p.partial + (((size_t)slice * 4 + dh) * 128 + m) * 64;
-    const uint32_t trow = tmem_base + ((uint32_t)(quad * 32) << 16);
-#pragma unroll 1
-    for (int c = 0; c < 64; c += 32) {
-      uint32_t r[32];
-      if (kb1 > kb0) {
-        ptx::tmem_ld_32x32(trow + c, r);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = 0u;
-      }
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) *reinterpret_cast<uint4 *>(dst + c + j) = make_uint4(r[j], r[j + 1], r[j + 2], r[j + 3]);
-    }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 64);
+    ptx::regs_consumer();
+    const int half = wgi - 1;
+    float *dst = p.partial + ((size_t)slice * 4 + dh) * 128 * 64;
+    // A: this warpgroup's 64 rows are two 32-channel boxes (dw = 2 half, 2 half + 1), 4 KB apart
+    const uint64_t da = ptx::gmma_desc(half * 8192, 4096, 512, ptx::kSW64);
+    const uint64_t db = ptx::gmma_desc(0, 8192, 1024, ptx::kSW128);
+    wgrad_consume<64, STAGES, S::STAGE_BYTES, S::A_BYTES>(smem, full_bar, empty_bar, kb0, kb1, half, da, 64, db, 128, dst, 64);
   }
 }
 

@@ -1,8 +1,7 @@
 // net.cu -- FlowNetS encoder + fc + heads on the device (deepim/symbols/deepIM_flownet.py:53-116 and
 // 716-726), weight repacking, tensor-map construction and layer scheduling.
 //
-//   conv tower : conv1_stack_kernel / conv1_roll_kernel + 9 x conv_igemm_persistent_kernel / conv_igemm_pair_kernel (tcgen05 + TMA,
-//                conv_igemm.cuh), split-K + finalize for the layers whose tile count cannot fill 148 SMs
+//   conv tower : conv1_kernel + 9 x conv_igemm_persistent_kernel (wgmma + TMA, conv_igemm.cuh)
 //   fc6        : 81920 -> 256, a pure weight stream (HBM-bound): split-K mma.sync kernel (batch = M = 16),
 //                deterministic two-pass reduction (partials reduced in fixed order by the head kernel)
 //   head       : fc6 reduce + bias + LeakyReLU -> fc7 -> LeakyReLU -> rot(4), trans(3) ->
@@ -60,40 +59,8 @@ static void build_geometry(NetState *ns, int H, int W) {
       g.BW = cdiv(g.Wo, nt); g.BH = 1; g.n_col_tiles = nt;
     }
     g.kblocks = g.KH * g.KW * (g.Ceff / g.BLOCK_K);
-    g.occ = (i == 0) ? 2 : 1;
-    g.pair = 0;  // per-layer kernel choice is applied per batch size in effective_geom() (NetState::pair_mask)
     h = g.Ho; w = g.Wo;
   }
-}
-
-// Kernel variant per layer.  bit i of NetState::pair_mask puts conv layer i (1..9) on the CTA-pair kernel
-// (cta_group::2, 256 x BLOCK_N tiles: each CTA stages its 128 activation rows and HALF of the weight tile, so the
-// shared-memory traffic per MMA drops from A + B to A + B/2 -- what bounds the N = 128 layer conv2).
-static LayerGeom effective_geom(const NetState *ns, int i, int B) {
-  LayerGeom g = ns->g[i];
-  (void)B;
-  if (i >= 1 && ((ns->pair_mask >> i) & 1)) g.pair = (g.BLOCK_N == 128) ? 2 : 1;  // 2: 3-stage ring, two pairs per SM pair
-  if (i >= 1 && g.BLOCK_N == 128 && !g.pair) g.occ = 2;  // conv2 on the 1-CTA kernel: two CTAs per SM
-  return g;
-}
-
-// split-K factor of the CTA-pair kernel (the 1-CTA persistent kernel never splits: see conv_igemm.cuh)
-static int choose_ksplit(const NetState *ns, const LayerGeom &g, int B) {
-  if (!g.pair) return 1;
-  const int tiles = cdiv(cdiv(B * g.Hq, g.BH) * g.n_col_tiles, 2) * (g.Cout / g.BLOCK_N);
-  const int cap = ns->num_sms / 2;
-  if (tiles >= 2 * cap || g.kblocks < 16) return 1;
-  int best = 1;
-  double best_score = -1.0;
-  for (int ks = 1; ks <= 8; ++ks) {
-    if (ks > 1 && g.kblocks / ks < 8) break;
-    if (ks > 1 && (ks - 1) * cdiv(g.kblocks, ks) >= g.kblocks) continue;  // no empty K slice
-    const int t = tiles * ks;
-    const double util = (double)t / (double)(cdiv(t, cap) * cap);
-    const double score = util - 0.06 * (ks - 1);
-    if (score > best_score + 1e-9) { best_score = score; best = ks; }
-  }
-  return best;
 }
 
 // --------------------------------------------------------------------------------- tensor maps
@@ -133,17 +100,9 @@ int encode_map(CUtensorMap *m, void *base, int rank, const uint64_t *dims, const
   return 0;
 }
 
-uint32_t make_idesc(int M, int N, bool f16) {
-  // cute::UMMA::InstrDescriptor: c_format F32 (1) @4, a/b_format @7/@10 (0 = F16, 1 = BF16), K-major both,
-  // n_dim = N>>3 @17, m_dim = M>>4 @24
-  const uint32_t fmt = f16 ? 0u : 1u;
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
 static int build_maps(NetState *ns, int B, bool f16, TensorMaps &tm) {
   for (int i = 0; i < 10; ++i) {
-    tm.g[i] = effective_geom(ns, i, B);
-    const LayerGeom &g = tm.g[i];
+    const LayerGeom &g = ns->g[i];
     ConvKParams &kp = tm.kp[i];
     memset(&kp, 0, sizeof(kp));
     for (int lo = 0; lo < 2; ++lo) {
@@ -180,9 +139,6 @@ static int build_maps(NetState *ns, int B, bool f16, TensorMaps &tm) {
       __nv_bfloat16 *wop = f16 ? ns->w_f16[i] : ns->w_hi[i];
       if (int rc = encode_map(&kp.b_map, wop, 2, dims, str, box, g.BLOCK_K)) return rc;
       if (int rc = encode_map(&kp.b_lo_map, ns->w_lo[i], 2, dims, str, box, g.BLOCK_K)) return rc;
-      const uint32_t box2[2] = {(uint32_t)g.BLOCK_K, (uint32_t)(g.BLOCK_N / 2)};
-      if (int rc = encode_map(&kp.b2_map, wop, 2, dims, str, box2, g.BLOCK_K)) return rc;
-      if (int rc = encode_map(&kp.b2_lo_map, ns->w_lo[i], 2, dims, str, box2, g.BLOCK_K)) return rc;
     }
     kp.KH = g.KH; kp.KW = g.KW; kp.stride = g.stride_eff; kp.cchunks = g.Ceff / g.BLOCK_K;
     kp.BW = g.BW; kp.BH = g.BH; kp.n_col_tiles = g.n_col_tiles;
@@ -195,14 +151,10 @@ static int build_maps(NetState *ns, int B, bool f16, TensorMaps &tm) {
     }
     kp.Cout = g.Cout;
     kp.kblocks = g.kblocks;
-    kp.ksplit = tm.ksplit[i] = choose_ksplit(ns, g, B);
-    kp.idesc = make_idesc(g.pair ? 256 : 128, g.BLOCK_N, f16);
-    kp.f16 = f16 ? 1 : 0;
     kp.slope = 0.1f;
     kp.bias = ns->bias[i];
     kp.out_hi = ns->act_hi[i + 1];
     kp.out_lo = ns->act_lo[i + 1];
-    kp.partial = ns->conv_partial;
   }
   return 0;
 }
@@ -378,21 +330,6 @@ int net_create(dim_ctx *ctx) {
     if (int rc = dev_alloc(ctx, &ns->act_lo[i], per * ctx->max_batch, true)) return rc;
   }
   ns->net_ok = ns->act_elems_per_image[10] == (size_t)FC6_K;  // fc6 is 81920 -> 256: needs 480x640
-  size_t pmax = 0;  // split-K partials of the CTA-pair kernel: sized for every layer on it (the choice may change at run time)
-  const int mask_now = ns->pair_mask;
-  ns->pair_mask = 0x3FE;
-  for (int B = 1; B <= ctx->max_batch; ++B)
-    for (int i = 0; i < 10; ++i) {
-      int ks = choose_ksplit(ns, effective_geom(ns, i, B), B);
-      if (ks > 1) {
-        size_t e = (size_t)ks * B * ns->g[i].Ho * ns->g[i].Wo * ns->g[i].Cout;
-        pmax = e > pmax ? e : pmax;
-      }
-    }
-  ns->pair_mask = mask_now;
-  ns->conv_partial_elems = pmax;
-  if (pmax)
-    if (int rc = dev_alloc(ctx, &ns->conv_partial, pmax, false)) return rc;
   if (int rc = dev_alloc(ctx, &ns->fc6_partial, (size_t)FC6_SPLITS * ctx->max_batch * 256, true)) return rc;
   return 0;
 }
@@ -521,32 +458,31 @@ int net_load(dim_ctx *ctx, const float *const *W, const float *const *Bv) {
   return 0;
 }
 
-template <int BN, int BK, int ST, bool S3, bool RES, int KRES>
-static int launch_conv2(NetState *ns, const ConvKParams &kp, int total_tiles, int n_tiles, int cap, cudaStream_t st) {
-  using S = ConvSmem2<BN, BK, ST, S3, RES, KRES>;
+template <int BN, int ST, bool S3, bool F16>
+static int launch_conv(const ConvKParams &kp, int total_tiles, int n_tiles, int cap, cudaStream_t st) {
+  using S = ConvSmem2<BN, ST, S3>;
   static bool attr_set = false;
   if (!attr_set) {
-    DIM_CHECK(cudaFuncSetAttribute(conv_igemm_persistent_kernel<BN, BK, ST, S3, RES, KRES>,
-                                   cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+    DIM_CHECK(cudaFuncSetAttribute(conv_igemm_persistent_kernel<BN, ST, S3, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   S::TOTAL));
     attr_set = true;
   }
   const int grid = total_tiles < cap ? total_tiles : cap;
-  conv_igemm_persistent_kernel<BN, BK, ST, S3, RES, KRES><<<grid, 192, S::TOTAL, st>>>(kp, total_tiles, n_tiles);
+  conv_igemm_persistent_kernel<BN, ST, S3, F16><<<grid, 384, S::TOTAL, st>>>(kp, total_tiles, n_tiles);
   DIM_LAUNCH_CHECK();
   return 0;
 }
 
-template <int BN, int ST, bool S3>
-static int launch_pair(const ConvKParams &kp, int pair_tiles, int n_tiles, int sms, cudaStream_t st) {
-  using S = ConvSmemPair<BN, ST, S3>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    DIM_CHECK(cudaFuncSetAttribute(conv_igemm_pair_kernel<BN, ST, S3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   S::TOTAL));
-    attr_set = true;
+template <int ST, bool S3, bool F16>
+static int launch_conv1(const ConvKParams &kp, int grid, int rows_total, int rpc, int chunks, int strip_bytes, cudaStream_t st) {
+  const int smem_bytes = (S3 ? 2 : 1) * 16 * 4096 + ST * (S3 ? 2 : 1) * strip_bytes + kConv1Slack + 1024 + 256;
+  DIM_REQUIRE(smem_bytes <= 227 * 1024, "conv1: image too wide for the rolling-strip ring");
+  static int set = 0;
+  if (set < smem_bytes) {
+    DIM_CHECK(cudaFuncSetAttribute(conv1_kernel<ST, S3, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
+    set = smem_bytes;
   }
-  const int pairs = pair_tiles < sms / 2 ? pair_tiles : sms / 2;
-  conv_igemm_pair_kernel<BN, ST, S3><<<2 * pairs, 192, S::TOTAL, st>>>(kp, pair_tiles, n_tiles);  // __cluster_dims__(2,1,1)
+  conv1_kernel<ST, S3, F16><<<grid, 384, smem_bytes, st>>>(kp, rows_total, rpc, chunks, strip_bytes);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -582,10 +518,10 @@ int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, fl
     if (int rc = net_refresh_f16(ctx, st)) return rc;
   if (ns->layer_events) DIM_CHECK(cudaEventRecord(ns->layer_events[0], st));
   for (int i = 0; i < 10; ++i) {
-    const LayerGeom &g = tm.g[i];
+    const LayerGeom &g = ns->g[i];
     const ConvKParams &kp = tm.kp[i];
     const int n_tiles = g.Cout / g.BLOCK_N;
-    const int total_tiles = cdiv(B * g.Hq, g.BH) * g.n_col_tiles * n_tiles * kp.ksplit;
+    const int total_tiles = cdiv(B * g.Hq, g.BH) * g.n_col_tiles * n_tiles;
     const int sms = ns->num_sms;
     int rc;
     if (i == 0) {
@@ -598,57 +534,20 @@ int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, fl
       chunks = cdiv(rows_total, rpc);
       const int strip_bytes = cdiv((g.BW + 3) * 64, 128) * 128;
       const int grid = g.n_col_tiles * chunks;
-      if (s3) {  // hi/lo operands: rolling strips, three MMA passes per step
-        constexpr int ST = 5;
-        const int smem_bytes = 2 * 16 * 4096 + ST * 2 * strip_bytes + (8 * 2048 + 256) + 1024 + 512;
-        DIM_REQUIRE(smem_bytes <= 227 * 1024, "conv1 (bf16x3): image too wide for the rolling-strip ring");
-        static int set1 = 0;
-        if (set1 < smem_bytes) { DIM_CHECK(cudaFuncSetAttribute(conv1_roll_kernel<ST, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes)); set1 = smem_bytes; }
-        conv1_roll_kernel<ST, true><<<grid, 320, smem_bytes, st>>>(kp, rows_total, rpc, chunks, strip_bytes);
-      } else if (ns->conv1_stack) {
-        // stacked filter rows: one 128 x 256 MMA per (dw, k) step feeds four output rows (A read once instead of four times)
-        constexpr int ST = 6;
-        const int smem_bytes = 16 * 4096 + ST * strip_bytes + (8 * 2048 + 256) + 512 + 512;
-        static int set3 = 0;
-        if (set3 < smem_bytes) { DIM_CHECK(cudaFuncSetAttribute(conv1_stack_kernel<ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes)); set3 = smem_bytes; }
-        conv1_stack_kernel<ST><<<grid, 320, smem_bytes, st>>>(kp, rows_total, rpc, chunks, strip_bytes);
-      } else {
-        constexpr int ST = 8;
-        const int smem_bytes = 16 * 4096 + ST * strip_bytes + (8 * 2048 + 256) + 1024 + 512;
-        static int set0 = 0;
-        if (set0 < smem_bytes) { DIM_CHECK(cudaFuncSetAttribute(conv1_roll_kernel<ST, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes)); set0 = smem_bytes; }
-        conv1_roll_kernel<ST, false><<<grid, 320, smem_bytes, st>>>(kp, rows_total, rpc, chunks, strip_bytes);
-      }
-      DIM_LAUNCH_CHECK();
-      rc = 0;
+      rc = s3 ? launch_conv1<5, true, false>(kp, grid, rows_total, rpc, chunks, strip_bytes, st)
+              : (f16 ? launch_conv1<8, false, true>(kp, grid, rows_total, rpc, chunks, strip_bytes, st)
+                     : launch_conv1<8, false, false>(kp, grid, rows_total, rpc, chunks, strip_bytes, st));
+    } else if (g.BLOCK_N == 128) {
+      rc = s3 ? launch_conv<128, 3, true, false>(kp, total_tiles, n_tiles, sms, st)
+              : (f16 ? launch_conv<128, 6, false, true>(kp, total_tiles, n_tiles, sms, st)
+                     : launch_conv<128, 6, false, false>(kp, total_tiles, n_tiles, sms, st));
+    } else {
+      rc = s3 ? launch_conv<256, 2, true, false>(kp, total_tiles, n_tiles, sms, st)
+              : (f16 ? launch_conv<256, 4, false, true>(kp, total_tiles, n_tiles, sms, st)
+                     : launch_conv<256, 4, false, false>(kp, total_tiles, n_tiles, sms, st));
     }
-    else if (g.pair) {
-      const int m_tiles = cdiv(B * g.Hq, g.BH) * g.n_col_tiles;
-      const int pair_tiles = cdiv(m_tiles, 2) * n_tiles * kp.ksplit;
-      if (g.BLOCK_N == 128 && g.pair == 2 && !s3)
-        rc = launch_pair<128, 3, false>(kp, pair_tiles, n_tiles, 2 * sms, st);
-      else if (g.BLOCK_N == 128)
-        rc = s3 ? launch_pair<128, 4, true>(kp, pair_tiles, n_tiles, sms, st) : launch_pair<128, 8, false>(kp, pair_tiles, n_tiles, sms, st);
-      else
-        rc = s3 ? launch_pair<256, 3, true>(kp, pair_tiles, n_tiles, sms, st) : launch_pair<256, 6, false>(kp, pair_tiles, n_tiles, sms, st);
-    } else if (g.BLOCK_N <= 128) {
-      rc = s3 ? launch_conv2<128, 64, 3, true, false, 0>(ns, kp, total_tiles, n_tiles, sms, st)
-              : (g.occ == 2 ? launch_conv2<128, 64, 2, false, false, 0>(ns, kp, total_tiles, n_tiles, 2 * sms, st)
-                            : launch_conv2<128, 64, 5, false, false, 0>(ns, kp, total_tiles, n_tiles, sms, st));
-    }
-    else
-      rc = s3 ? launch_conv2<256, 64, 2, true, false, 0>(ns, kp, total_tiles, n_tiles, sms, st)
-              : launch_conv2<256, 64, 4, false, false, 0>(ns, kp, total_tiles, n_tiles, sms, st);
     if (rc) return rc;
     if (ns->layer_events && i < 9) DIM_CHECK(cudaEventRecord(ns->layer_events[i + 1], st));
-    if (kp.ksplit > 1) {
-      const int npix = B * g.Ho * g.Wo;
-      const size_t n4 = (size_t)npix * g.Cout / 4;
-      conv_splitk_finalize_kernel<<<(unsigned)cdiv((int)n4, 256), 256, 0, st>>>(
-          ns->conv_partial, kp.ksplit, npix, g.Cout, g.Ho, g.Wo, kp.out_Hp, kp.out_Wp, kp.out_py, kp.out_px,
-          ns->bias[i], 0.1f, ns->act_hi[i + 1], s3 ? ns->act_lo[i + 1] : nullptr, f16 ? 1 : 0);
-      DIM_LAUNCH_CHECK();
-    }
   }
   if (ns->layer_events) DIM_CHECK(cudaEventRecord(ns->layer_events[10], st));
   if (after_conv) DIM_CHECK(cudaEventRecord(after_conv, st));
@@ -675,16 +574,12 @@ bool net_graph_safe(dim_ctx *ctx) {
   return ns && ns->loaded && !ns->layer_events && !ns->train_aliased;
 }
 
-// tuning hook (tools/conv_lab.py): kernel-variant switches at run time; cached launch descriptors are rebuilt
+// run-time switches of the conv tower: there are none (every layer has one kernel); unknown keys are an error
 int net_set_option(dim_ctx *ctx, const char *key, int value) {
-  NetState *ns = ctx->net;
-  DIM_REQUIRE(ns != nullptr, "net not created");
-  if (!strcmp(key, "pair_mask")) ns->pair_mask = value & 0x3FE;
-  else if (!strcmp(key, "conv1_stack")) ns->conv1_stack = value != 0;
-  else { set_error("dim_debug_set_option: unknown key '%s'", key); return 2; }
-  DIM_CHECK(cudaDeviceSynchronize());
-  ns->maps.clear();
-  return 0;
+  (void)value;
+  DIM_REQUIRE(ctx->net != nullptr, "net not created");
+  set_error("dim_debug_set_option: unknown key '%s'", key);
+  return 2;
 }
 
 // tuning hook: per-layer device times of the LAST net_forward (11 events: before conv1, after each of the 10 layers)

@@ -25,14 +25,10 @@ struct LayerGeom {
   // implicit GEMM view
   int KH, KW, stride_eff, Ceff, Hq;
   int BLOCK_N, BLOCK_K, BW, BH, n_col_tiles, kblocks;
-  int pair;  // 1: CTA-pair kernel (cta_group::2, 256 x BLOCK_N tiles)
-  int occ;  // resident CTAs per SM of the persistent kernel variant used for this layer (bf16 mode)
 };
 
 struct TensorMaps {
   ConvKParams kp[10];
-  int ksplit[10];
-  LayerGeom g[10];  // per-batch-size effective geometry (tile width may depend on the batch)
 };
 
 // conv1 operand K order inside one (dh, dw) tap of the space-to-depth form: the four 8-channel chunks (ph, pw) sit at
@@ -55,12 +51,6 @@ struct NetState {
   float *fc6_b = nullptr, *fc7_wT = nullptr, *fc7_b = nullptr, *rot_w = nullptr, *rot_b = nullptr,
         *trans_w = nullptr, *trans_b = nullptr;
   float *fc6_partial = nullptr;  // [FC6_SPLITS][max_batch][256]
-  float *conv_partial = nullptr;
-  size_t conv_partial_elems = 0;
-  // kernel variants; defaults = the measured-best set (tools/conv_lab.py, profiles/r02_conv_lab.json), switchable at run
-  // time through dim_debug_set_option for A/B measurements
-  bool conv1_stack = true;   // conv1 (single-pass precisions) on conv1_stack_kernel; false: conv1_roll_kernel (always used by bf16x3)
-  int pair_mask = 1 << 1;    // bit i: conv layer i runs on the CTA-pair (cta_group::2) kernel; default: conv2 (N = 128)
   cudaEvent_t *layer_events = nullptr;  // tuning hook: 11 events around the conv layers of the last forward
   bool loaded = false, net_ok = false;
   float *save_h6 = nullptr, *save_h7 = nullptr;
@@ -68,7 +58,7 @@ struct NetState {
                                       // every consumer (net_forward) orders itself behind this event
   bool lo_stale = false;  // training updated the weights without refreshing the bf16 'lo' halves (bf16x3 mode refreshes lazily)  // training: fc6 / fc7 activations kept for the backward pass ([B][256])
   std::map<int, TensorMaps> maps;  // per batch size (+ kF16MapKey for the fp16 operand maps)
-  int max_batch = 0, num_sms = 148;
+  int max_batch = 0, num_sms = 132;
 };
 
 static constexpr int FC6_K = 1024 * 8 * 10;
@@ -79,7 +69,6 @@ static constexpr int FC6_SPLITS = FC6_K / FC6_KC;  // 320
 // helpers implemented in net.cu
 int encode_map(CUtensorMap *m, void *base, int rank, const uint64_t *dims, const uint64_t *strides_bytes,
                const uint32_t *box, int block_k /*64: SW128, 32: SW64, 0: no swizzle*/);
-uint32_t make_idesc(int M, int N, bool f16 = false);
 static constexpr int kF16MapKey = 1 << 20;
 int train_refresh_lo(dim_ctx *ctx, cudaStream_t st);  // train.cu
 int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, float *rot_out, float *trans_out,

@@ -3,7 +3,7 @@
 // the whole graph, and the MXNet-SGD update (deepim/train.py:296-304; one update per inner iteration,
 // deepim/core/module.py:1131-1137).
 //
-//   tensor-core work (tcgen05 + TMA):
+//   tensor-core work (wgmma + TMA):
 //     forward   encoder convs (net.cu), deconv5 / deconv4 as 4 parity sub-convolutions (2x2 taps, stride-2 store)
 //     dgrad     stride-1 layers: flipped-kernel convolution of dZ; stride-2 layers: 4 parity sub-convolutions;
 //               deconvolutions: a stride-2 4x4 convolution of the (cropped) output gradient
@@ -924,30 +924,27 @@ static void pick_tile(int W, int rows_total, int cap, int &BW, int &BH, int max_
 
 template <int BN, int ST>
 static int launch_generic(const ConvKParams &kp, int total_tiles, int n_tiles, int cap, cudaStream_t st) {
-  using S = ConvSmem2<BN, 64, ST, false, false, 0>;
+  using S = ConvSmem2<BN, ST, false>;
   static bool attr_set = false;
   if (!attr_set) {
-    DIM_CHECK(cudaFuncSetAttribute(conv_igemm_persistent_kernel<BN, 64, ST, false, false, 0, 1>,
+    DIM_CHECK(cudaFuncSetAttribute(conv_igemm_persistent_kernel<BN, ST, false, false, 1>,
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
     attr_set = true;
   }
   const int grid = total_tiles < cap ? total_tiles : cap;
-  conv_igemm_persistent_kernel<BN, 64, ST, false, false, 0, 1><<<grid, 192, S::TOTAL, st>>>(kp, total_tiles, n_tiles);
+  conv_igemm_persistent_kernel<BN, ST, false, false, 1><<<grid, 384, S::TOTAL, st>>>(kp, total_tiles, n_tiles);
   DIM_LAUNCH_CHECK();
   return 0;
 }
 
-// N <= 128 tiles are bound by shared-memory operand traffic, not by the tensor pipe.  Two resident CTAs per SM with a shallow
-// ring (what conv2 of the forward tower used before its CTA-pair kernel) measured the same as one CTA with a deep ring for
-// the data-gradient classes (265.7 vs 266.0 instances/s at B = 4): one CTA per SM, deep ring.
+// one CTA per SM with the deepest ring that fits (STAGES x stage bytes <= 192 KB)
 static int run_generic(dim_ctx *ctx, const ConvKParams &kp, const LayerGeom &g, int B, cudaStream_t st) {
   const int n_tiles = cdiv(g.Cout, g.BLOCK_N);
   const int total = cdiv(B * g.Hq, g.BH) * g.n_col_tiles * n_tiles;
   const int sms = ctx->num_sms;
   if (g.BLOCK_N == 256) return launch_generic<256, 4>(kp, total, n_tiles, sms, st);
-  if (g.BLOCK_N == 128)
-    return launch_generic<128, 5>(kp, total, n_tiles, sms, st);
-  return launch_generic<64, 6>(kp, total, n_tiles, sms, st);
+  if (g.BLOCK_N == 128) return launch_generic<128, 6>(kp, total, n_tiles, sms, st);
+  return launch_generic<64, 8>(kp, total, n_tiles, sms, st);
 }
 
 // Describe one launch of the generic kernel.
@@ -993,8 +990,7 @@ static int make_generic(ConvKParams &kp, LayerGeom &g, int B, const Buf &in, int
   kp.BW = g.BW; kp.BH = g.BH; kp.n_col_tiles = g.n_col_tiles;
   kp.Hq = g.Hq; kp.Ho = Ho; kp.Wo = Wo; kp.Bn = B;
   kp.out_Hp = out.Hp; kp.out_Wp = out.Wp; kp.out_py = out.py; kp.out_px = out.px; kp.Cout = N;
-  kp.kblocks = g.kblocks; kp.ksplit = 1;
-  kp.idesc = make_idesc(128, g.BLOCK_N);
+  kp.kblocks = g.kblocks;
   kp.slope = slope; kp.bias = bias; kp.out_hi = out.p; kp.out_lo = nullptr;
   kp.in_off_r = off_r; kp.in_off_c = off_c;
   kp.out_sy = sy; kp.out_sx = sx; kp.out_oy = oy; kp.out_ox = ox; kp.out_H = out.H; kp.out_W = out.W;
@@ -1015,12 +1011,10 @@ static int launch_wgrad(const WgradParams &p, cudaStream_t st) {
     attr_set = true;
   }
   const int grid = p.KH * p.KW * p.m_tiles * p.n_tiles * p.kslices;
-  conv_wgrad_kernel<BN, ST><<<grid, 192, S::TOTAL, st>>>(p);
+  conv_wgrad_kernel<BN, ST><<<grid, 384, S::TOTAL, st>>>(p);
   DIM_LAUNCH_CHECK();
   return 0;
 }
-
-static uint32_t make_idesc_mn(int M, int N) { return make_idesc(M, N) | (1u << 15) | (1u << 16); }
 
 static int encode_map4(CUtensorMap *m, __nv_bfloat16 *base, uint64_t C, uint64_t cols, uint64_t rows, uint64_t B, uint64_t pix_stride,
                        uint64_t row_stride, uint64_t img_stride, uint32_t boxc, uint32_t bw, uint32_t bh) {
@@ -1043,7 +1037,7 @@ static int make_wgrad(TrainState *ts, WgradParams &p, int &BN, int B, const Buf 
   p.m_tiles = cdiv(M, 128); p.n_tiles = cdiv(N, BN);
   p.kb_total = B * p.rects_x * p.rects_y;
   const int tiles = KH * KW * p.m_tiles * p.n_tiles;
-  // K slices: one CTA per SM is resident (190 KB ring), so pick the slice count whose CTA total fills whole waves of `sms`
+  // K slices: one CTA per SM is resident (~192 KB ring), so pick the slice count whose CTA total fills whole waves of `sms`
   // best (e.g. 25 tiles: 11 slices = 275 CTAs = 2 waves at 93 %, where 12 slices = 300 CTAs would need a third wave)
   const size_t per_slice = (size_t)KH * KW * p.m_tiles * 128 * p.n_tiles * BN;
   int ks = 1;
@@ -1057,7 +1051,6 @@ static int make_wgrad(TrainState *ts, WgradParams &p, int &BN, int B, const Buf 
   DIM_REQUIRE(per_slice * ks <= ts->wg_partial_elems, "wgrad workspace too small");
   p.kb_per_slice = cdiv(p.kb_total, ks);
   p.kslices = cdiv(p.kb_total, p.kb_per_slice);
-  p.idesc = make_idesc_mn(128, BN);
   p.partial = ts->wg_partial;
   if (int rc = encode_map4(&p.z_map, Z.p + z_coff, M, Z.Wp, Z.Hp, B, Z.C, (uint64_t)Z.Wp * Z.C, (uint64_t)Z.Hp * Z.Wp * Z.C, 64, p.BW, p.BH))
     return rc;
@@ -1079,12 +1072,11 @@ static int make_wgrad(TrainState *ts, WgradParams &p, int &BN, int B, const Buf 
 
 static int run_wgrad(const WgradParams &p, int BN, int kind, int D0, int D1, int k, float *grad, cudaStream_t st) {
   int rc;
-  // Two resident CTAs per SM with half-depth rings (the same bytes in flight per SM as one CTA with a deep ring): the
-  // barrier-init / TMEM-alloc prologue and the fp32 epilogue of one CTA overlap the K loop of the other (measured +4 %).
-  if (BN == 256) rc = launch_wgrad<256, 2>(p, st);
-  else if (BN == 128) rc = launch_wgrad<128, 3>(p, st);
-  else if (BN == 64) rc = launch_wgrad<64, 4>(p, st);
-  else rc = launch_wgrad<32, 4>(p, st);
+  // one CTA per SM, ring depth = what fits in ~192 KB of shared memory
+  if (BN == 256) rc = launch_wgrad<256, 4>(p, st);
+  else if (BN == 128) rc = launch_wgrad<128, 6>(p, st);
+  else if (BN == 64) rc = launch_wgrad<64, 8>(p, st);
+  else rc = launch_wgrad<32, 8>(p, st);
   if (rc) return rc;
   const size_t total = (size_t)p.KH * p.KW * p.m_tiles * 128 * p.n_tiles * BN;
   wgrad_reduce_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(p.partial, p.kslices, p.KH * p.KW, p.m_tiles * 128,
@@ -1107,9 +1099,8 @@ static int run_wgrad_conv1(TrainState *ts, const WgradParams &p16, int sms, floa
   if (ks < 1) ks = 1;
   p.kb_per_slice = cdiv(p.kb_total, ks);
   p.kslices = cdiv(p.kb_total, p.kb_per_slice);
-  p.idesc = make_idesc_mn(128, 64);
   DIM_REQUIRE((size_t)p.kslices * 4 * 128 * 64 <= ts->wg_partial_elems, "wgrad workspace too small");
-  conv1_wgrad_kernel<8><<<4 * p.kslices, 192, S::TOTAL, st>>>(p);
+  conv1_wgrad_kernel<8><<<4 * p.kslices, 384, S::TOTAL, st>>>(p);
   DIM_LAUNCH_CHECK();
   const size_t total = (size_t)4 * 128 * 64;
   wgrad_reduce_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(p.partial, p.kslices, 4, 128, 64, WG_CONV1_ROW, 64, 8, 7, grad);

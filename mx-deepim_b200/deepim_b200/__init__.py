@@ -1,4 +1,4 @@
-"""deepim_b200 -- B200-native (sm_100a) render-and-compare pose refinement hot path of mx-DeepIM.
+"""deepim_b200 -- H100-native (sm_90a) render-and-compare pose refinement hot path of mx-DeepIM.
 
 Python host over the C ABI in include/deepim_b200.h.  The names mirror the reference:
   deepim_b200.operator_py.*      <- deepim/operator_py/*.py   (ZoomMask, ZoomImageWithFactor, ...)

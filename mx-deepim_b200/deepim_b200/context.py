@@ -39,7 +39,7 @@ class Context:
     def __init__(self, device=0, max_batch=16, height=480, width=640, max_classes=16, max_verts=60000,
                  max_faces=120000):
         if not torch.cuda.is_available():
-            raise capi.DeepIMError("deepim_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise capi.DeepIMError("deepim_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
         torch.cuda.set_device(self.device)
         self.H, self.W, self.max_batch = height, width, max_batch

@@ -134,7 +134,7 @@ def save_checkpoint(prefix, epoch, arg_params, aux_params=None):
 #             "inputs": [[node_id, output_index, version], ...]}, ...],
 #  "arg_nodes": [ids of the "null" nodes = variables], "node_row_ptr": [...], "heads": [[node_id, index, version], ...],
 #  "attrs": {"mxnet_version": ["int", 10200]}}.
-# The B200 path does not execute the graph (it IS the FlowNetS tower of deepim/symbols/deepIM_flownet.py:53-116); reading the
+# The CUDA path does not execute the graph (it IS the FlowNetS tower of deepim/symbols/deepIM_flownet.py:53-116); reading the
 # file serves to CHECK that a checkpoint belongs to this architecture before its tensors are repacked.
 def load_symbol_json(path_or_text):
     import json

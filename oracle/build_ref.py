@@ -26,7 +26,7 @@ def build_ref(force=False):
         return OUT
     os.makedirs(os.path.dirname(OUT), exist_ok=True)
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    subprocess.check_call([nvcc, "-shared", "--compiler-options", "-fPIC", "-gencode", "arch=compute_100a,code=sm_100a",
+    subprocess.check_call([nvcc, "-shared", "--compiler-options", "-fPIC", "-gencode", "arch=compute_90a,code=sm_90a",
                            "-I", os.path.dirname(REF_SRC), REF_SRC, "-o", OUT])
     return OUT
 

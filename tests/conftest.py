@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "mx-deepim_b200")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu on a GPU machine)")
 
 
 @pytest.fixture(scope="session")

@@ -1,4 +1,4 @@
-"""GPU parity at BASELINE.json's ACTUAL configurations (run with -m gpu on a B200):
+"""GPU parity at BASELINE.json's ACTUAL configurations (run with -m gpu on an H100):
 
 * C2 -- 5k-vert mesh, 4 iterations, batch 16 (the headline batch: tile schedules depend on B): teacher-forced
   per-iteration bounds on all 16 instances for the mode bench.py reports (DIM_PREC_FP16) and the 3-pass mode;

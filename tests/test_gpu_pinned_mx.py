@@ -2,7 +2,7 @@
 (tests/golden/ref_mx_*.npz, made by tests/golden/make_golden_mx.py under the numpy-backed mxnet stand-in): the same inputs,
 compared with the reference's outputs directly -- not through the oracle.  Bit-exact for the 8 integer zoom bbox indices,
 zoom_factor, every rounded mask / weight plane and ZoomTrans; <= 1 ulp for the sampled float planes; float32 rounding for
-Transform3D.  Run with -m gpu on a B200; reads nothing outside the repo."""
+Transform3D.  Run with -m gpu on an H100; reads nothing outside the repo."""
 import hashlib
 import os
 import sys

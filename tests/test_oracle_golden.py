@@ -70,7 +70,7 @@ def test_flow_matches_reference_calc_flow(golden_dir):
 
 def test_flow_matches_the_reference_cuda_kernel(golden_dir):
     """a13, second pin: the reference's UNMODIFIED lib/flow_c/gpu_flow_kernel.cu (compiled by oracle/build_ref.py into
-    oracle/_ref, executed on a B200 by tests/golden/make_golden_flow_cuda.py -> ref_flow_cuda.npz) against the C restatement:
+    oracle/_ref, executed on a GPU by tests/golden/make_golden_flow_cuda.py -> ref_flow_cuda.npz) against the C restatement:
     the validity masks are identical; the flow differs by at most 2 ulp of the pixel coordinate (the reference build lets nvcc
     contract multiply-adds, the restatement is compiled without contraction so that the CUDA path can be bit-exact to IT)."""
     g = np.load(os.path.join(golden_dir, "ref_flow_cuda.npz"))

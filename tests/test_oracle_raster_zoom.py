@@ -191,8 +191,7 @@ def test_net_forward_shapes_and_refine_runs():
 def test_bf16_storage_emulation_calibrates_the_throughput_mode_tolerance():
     """DIM_PREC_BF16 (what bench.py reports) stores conv activations and operand weights in bf16 with fp32 accumulation.
     The oracle network with exactly that storage emulated differs from the fp32 oracle by ~1e-4 on the regressed se3 delta
-    -- the size of the deviation the GPU tests allow that mode (2e-3) and that profiles/r01_parity_report.json records
-    for the device (1.5e-4 on the first-iteration pose over 64 instances).  The parity mode (bf16x3) does not have it."""
+    -- well inside the deviation the GPU tests allow that mode (2e-3).  The parity mode (bf16x3) does not have it."""
     from deepim_b200 import synth
     w = synth.make_weights(0)
     mesh = synth.make_blob(nlat=24, nlon=48, tex_size=128)

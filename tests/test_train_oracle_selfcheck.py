@@ -64,7 +64,8 @@ def test_training_oracle_gradients_match_finite_differences():
 def test_bf16_storage_explains_the_device_gradient_deviation():
     """Calibration of the GPU tolerances (tests/test_gpu_train.py: cosine >= 0.995, error <= 0.15 max|g| on 99 % of the entries): running the ORACLE
     with the device's storage format emulated (bf16 operand weights, activations and activation gradients; fp32 accumulation)
-    on the same batch deviates from the fp32 oracle like the device did in profiles/r01_train_check_first_light.json --
+    on the same batch deviates from the fp32 oracle like the device did (tests/golden/train_check_device.json: the gradient
+    cosines of tools/gpu_train_check.py on an H100) --
     i.e. the device's deviation is the cost of the storage format, not of the kernels."""
     import json
     import os
@@ -78,7 +79,7 @@ def test_bf16_storage_explains_the_device_gradient_deviation():
     zin, lab = T.zoom_inputs(batch, K, MEANS)
     _, g32 = T.graph(w, zin, lab, requires_grad=True)
     _, g16 = T.graph(w, zin, lab, requires_grad=True, emulate_bf16=True)
-    dev = json.load(open(os.path.join(root, "profiles", "r01_train_check_first_light.json")))["grads"]
+    dev = json.load(open(os.path.join(root, "tests", "golden", "train_check_device.json")))["grads"]
     worst_gap = 0.0
     for k, d in dev.items():
         if k in T.FROZEN:
