@@ -241,7 +241,7 @@ DIM_API int32_t dim_refine_host(dim_ctx *ctx, const uint8_t *image_observed_u8_h
                                 float zfar, const double *pixel_means_rgb_host, int32_t precision,
                                 double *poses_out_host, float *se3_out_host, void *stream);
 
-/* Per-iteration status of the LAST dim_refine / dim_refine_host(_async) call on this context, copied device -> host
+/* Per-iteration status of the LAST dim_refine(_lit) / dim_refine_host(_lit)(_async) call on this context, copied device -> host
  * asynchronously on `stream` (the stream that call ran on): [min(n_iter,8), B] int32.  0 = ok; bit 0 = the rendered mask
  * of that iteration was empty (the reference crashes there: np.min of an empty array, zoom_mask.py:55-58; here the
  * fallback zoom factor was used and the instance's pose is meaningless); bit 1 = class index out of range or no mesh
@@ -257,6 +257,56 @@ DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *image_observe
                                       float zfar, const double *pixel_means_rgb_host,
                                       int32_t precision, double *poses_out_host, float *se3_out_host,
                                       void *stream);
+
+/* ModelNet / unseen-object configuration (config.dataset.dataset "ModelNet*": deepim/core/tester.py:114-133,146-185;
+ * lib/pair_matching/batch_updater_py_multi.py:35-52,187-229): every render of the loop is the Lambert-lit renderer of
+ * dim_render_lit instead of the unlit one.  The light follows the pose being rendered: in the GL camera frame
+ *   light_position = float32(offset[0] + t_x, offset[1] - t_y, offset[2] - t_z)
+ * computed from the float64 pose (the reference's hard-coded light index 2 gives offset = (0, 0.5, 0.5)).  The reference
+ * draws light_intensity from U(0.9, 1.1)^3 afresh for every render; here the caller supplies the draws.
+ *   intensity: device f32 [n_iter,B,3] for dim_refine_lit (iteration it renders with intensity[it]), [B,3] for
+ *              dim_train_update_lit, HOST f32 [n_iter,B,3] for dim_refine_host_lit(_async) (n_iter <= 8; copied to the
+ *              context on `stream` before the call returns, so a pageable buffer may be reused at once).
+ *   brightness_ratio: colour = texel * ((1 - ratio) + ratio * brightness) * intensity (the reference: 0.7).
+ * Depth, masks, bboxes, zoom, labels and flow are those of the unlit calls; only the colours change.  Every uploaded mesh
+ * must have normals (dim_mesh_upload_normals).  The lit calls take every argument of their unlit counterparts plus
+ * `lighting`, share dim_refine_status, and are captured / replayed as CUDA graphs like dim_refine. */
+typedef struct dim_lighting {
+  const float *intensity; /* see above: device [n_iter,B,3] (refine) / [B,3] (train update); host for dim_refine_host_lit */
+  double offset[3];       /* light at zero translation, GL frame; the reference: (0, 0.5, 0.5) */
+  float brightness_ratio; /* the reference: 0.7 */
+} dim_lighting;
+DIM_API int32_t dim_refine_lit(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx,
+                               const double *pose_init, int32_t B, int32_t n_iter, const float *K9_host,
+                               float znear, float zfar, const double *pixel_means_rgb_host,
+                               int32_t precision, const double *pose_override, double *poses,
+                               float *se3, float *zoom_factor, int32_t *bbox, const dim_lighting *lighting,
+                               void *stream);
+DIM_API int32_t dim_refine_host_lit(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
+                                    const int32_t *cls_idx_host, const double *pose_init_host,
+                                    int32_t B, int32_t n_iter, const float *K9_host, float znear,
+                                    float zfar, const double *pixel_means_rgb_host, int32_t precision,
+                                    double *poses_out_host, float *se3_out_host,
+                                    const dim_lighting *lighting, void *stream);
+DIM_API int32_t dim_refine_host_lit_async(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
+                                          const int32_t *cls_idx_host, const double *pose_init_host,
+                                          int32_t B, int32_t n_iter, const float *K9_host, float znear,
+                                          float zfar, const double *pixel_means_rgb_host,
+                                          int32_t precision, double *poses_out_host, float *se3_out_host,
+                                          const dim_lighting *lighting, void *stream);
+
+/* dim_train_update for the ModelNet configuration (batch_updater_py_multi.py:187-235): the re-render is lit, the light
+ * follows the float64 refined pose (dim_lighting above; intensity device f32 [B,3]); image_rendered = float32 quantised
+ * lit colours - float32 means.  Every other output equals dim_train_update's. */
+DIM_API int32_t dim_train_update_lit(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose,
+                                     const float *rot_est, const float *trans_est, const float *tgt_pose,
+                                     const float *depth_gt_observed, int32_t B, const double *K9_host,
+                                     float znear, float zfar, const double *pixel_means_rgb_host,
+                                     const double *T_means_host, const double *T_stds_host,
+                                     int32_t rot_coord, float *image_rendered, float *depth_rendered,
+                                     float *mask_rendered, float *src_pose_new, float *rot_label,
+                                     float *trans_label, float *flow, float *flow_weights,
+                                     const dim_lighting *lighting, void *stream);
 
 /* BGR u8 HWC -> RGB-mean f32 CHW on device (lib/utils/image.py:583-594 transform). */
 DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int32_t B,

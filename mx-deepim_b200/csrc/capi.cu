@@ -40,10 +40,12 @@ int pack_nhwc8_launch(dim_ctx *, const float *, const float *, const float *, co
 int flow_launch(dim_ctx *, const float *, const float *, const float *, const float *, int B, float *, float *,
                 float *, cudaStream_t);
 int train_pose_launch(const float *, const float *, const float *, const float *, int B, const double *,
-                      const double *, int, const double *, float *, float *, float *, float *, cudaStream_t);
+                      const double *, int, const double *, float *, float *, float *, float *, cudaStream_t,
+                      float *light_pos = nullptr, const double *light_offset = nullptr);
 int se3_compose_launch(const double *, const float *, int B, const double *, const double *, int, double *, float *,
                        cudaStream_t);
 int f64_to_f32_launch(const double *, float *, int n, cudaStream_t);
+int pose_light_launch(const double *pose, float *pose_f32, float *light_pos, int B, const double *offset, cudaStream_t);
 int zoom_trans_launch(const float *, const float *, int B, int mul, int scale_xy, float *, cudaStream_t);
 int transform3d_fwd_launch(const float *, const float *, const float *, const float *, int, int, const float *,
                            const float *, int, float *, cudaStream_t);
@@ -161,6 +163,8 @@ DIM_API int32_t dim_ctx_create(int32_t device, int32_t max_batch, int32_t H, int
   rc |= ctx_alloc(ctx, &ctx->cls_dev, Bm);
   rc |= ctx_alloc(ctx, &ctx->poses_dev, 8 * Bm * 12);
   rc |= ctx_alloc(ctx, &ctx->se3_hist_dev, 8 * Bm * 7);
+  rc |= ctx_alloc(ctx, &ctx->light_pos, Bm * 3);
+  rc |= ctx_alloc(ctx, &ctx->lit_intensity, 8 * Bm * 3);
   if (rc) { dim_ctx_destroy(ctx); return 12; }
   ctx->meshes_host.assign(max_classes, MeshDev{nullptr, nullptr, nullptr, nullptr, 0, 0, 0, 0, nullptr});
   DIM_CHECK(cudaMemset(ctx->meshes, 0, sizeof(MeshDev) * max_classes));
@@ -227,6 +231,23 @@ DIM_API int32_t dim_mesh_upload_normals(dim_ctx *ctx, int32_t cls, const float *
   DIM_CHECK(cudaMemcpy(ctx->meshes + cls, &m, sizeof(MeshDev), cudaMemcpyHostToDevice));
   return 0;
 }
+// the lit loop / update entry points: lighting and its intensities are given and every uploaded mesh has normals
+static int lit_check(dim_ctx *ctx, const dim_lighting *lit, const char *fn) {
+  if (!ctx || !lit || !lit->intensity) {
+    set_error("%s: NULL context, lighting or lighting->intensity", fn);
+    return 2;
+  }
+  for (auto &m : ctx->meshes_host)
+    if (m.V > 0 && m.normals == nullptr) {
+      set_error("%s: a mesh has no normals (dim_mesh_upload_normals)", fn);
+      return 2;
+    }
+  return 0;
+}
+static LitParams lit_params(const float *light_pos, const float *intensity, float ratio) {
+  return LitParams{light_pos, intensity, (float)(1.0 - (double)ratio), ratio};
+}
+
 DIM_API int32_t dim_render_lit(dim_ctx *ctx, const int32_t *cls_idx, const float *pose, int32_t B, const float *K9, float zn,
                                float zf, const double *means, const float *light_pos, const float *light_int,
                                float brightness_ratio, float *out_image, float *out_depth, float *out_mask, float *out_bgr,
@@ -377,7 +398,7 @@ DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr, int32_t
 static int refine_core(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_idx, const double *pose_init, int32_t B,
                        int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
                        const double *pose_override, double *poses, float *se3, float *zoom_factor, int32_t *bbox,
-                       cudaStream_t st) {
+                       cudaStream_t st, const dim_lighting *lit) {
   const double Tm[3] = {ctx->cfg.trans_means[0], ctx->cfg.trans_means[1], ctx->cfg.trans_means[2]};
   const double Ts[3] = {ctx->cfg.trans_stds[0], ctx->cfg.trans_stds[1], ctx->cfg.trans_stds[2]};
   const float means_f[3] = {(float)means[0], (float)means[1], (float)means[2]};
@@ -398,14 +419,21 @@ static int refine_core(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_idx,
       DIM_CHECK(cudaEventRecord(ev[0], st));
     }
     if (pose_override) pose_src = pose_override + (size_t)it * B * 12;
-    // src_pose blob is float32 (nd.array), the host pose stays float64 (tester.py:391)
-    if (int rc = f64_to_f32_launch(pose_src, ctx->pose_cur_f32, B * 12, st)) return rc;
+    // src_pose blob is float32 (nd.array), the host pose stays float64 (tester.py:391); the lit chain also derives the
+    // light of this iteration's render from the float64 pose
+    if (lit) {
+      if (int rc = pose_light_launch(pose_src, ctx->pose_cur_f32, ctx->light_pos, B, lit->offset, st)) return rc;
+    } else if (int rc = f64_to_f32_launch(pose_src, ctx->pose_cur_f32, B * 12, st)) {
+      return rc;
+    }
     // render at the current pose (tester.py:427-442) straight into the pixel-interleaved
     // (R,G,B,mask) image the zoom kernel samples; mask_observed := box(mask_rendered) is analytic
     {
       DimNvtxRange r("render");
+      const LitParams lp = lit ? lit_params(ctx->light_pos, lit->intensity + (size_t)it * B * 3, lit->brightness_ratio)
+                               : LitParams{nullptr, nullptr, 0.f, 0.f};
       if (int rc = render_launch(ctx, cls_idx, ctx->pose_cur_f32, B, K9, zn, zf, means, 1, nullptr, nullptr, nullptr,
-                                 nullptr, nullptr, ctx->ren4, st))
+                                 nullptr, nullptr, ctx->ren4, st, lit ? &lp : nullptr))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[1], st));
@@ -445,18 +473,22 @@ static int refine_core(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_idx,
 static int refine_graphed(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_idx, const double *pose_init, int32_t B,
                           int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
                           const double *pose_override, double *poses, float *se3, float *zoom_factor, int32_t *bbox,
-                          cudaStream_t st) {
+                          cudaStream_t st, const dim_lighting *lit = nullptr) {
   // the legacy default stream (and the per-thread default stream handle) cannot be captured
   const bool capturable = st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread;
   if (!ctx->use_graph || ctx->prof || !capturable || !net_graph_safe(ctx))
     return refine_core(ctx, obs4, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override, poses, se3,
-                       zoom_factor, bbox, st);
+                       zoom_factor, bbox, st, lit);
   std::vector<unsigned char> key;
   auto put = [&key](const void *p, size_t n) { key.insert(key.end(), (const unsigned char *)p, (const unsigned char *)p + n); };
   const void *ptrs[8] = {obs4, cls_idx, pose_init, pose_override, poses, se3, zoom_factor, bbox};
   const int32_t ints[3] = {B, n_iter, precision};
   put(ptrs, sizeof(ptrs)); put(ints, sizeof(ints)); put(K9, 9 * sizeof(float)); put(&zn, sizeof(zn)); put(&zf, sizeof(zf));
   put(means, 3 * sizeof(double));
+  // a lit chain never shares a graph with an unlit one: the light's intensity buffer, offset and ratio are part of the key
+  const unsigned char is_lit = lit != nullptr;
+  put(&is_lit, 1);
+  if (lit) { put(&lit->intensity, sizeof(lit->intensity)); put(lit->offset, sizeof(lit->offset)); put(&lit->brightness_ratio, sizeof(float)); }
   dim_ctx::RefineGraph *g = nullptr;
   for (auto &e : ctx->graphs)
     if (e.key == key) { g = &e; break; }
@@ -469,12 +501,12 @@ static int refine_graphed(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_i
     if (ctx->graphs.size() >= 32) ctx->graphs.erase(ctx->graphs.begin());
     ctx->graphs.push_back(dim_ctx::RefineGraph{key, nullptr, 0});
     return refine_core(ctx, obs4, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override, poses, se3,
-                       zoom_factor, bbox, st);
+                       zoom_factor, bbox, st, lit);
   }
   const long long before = g_launches;
   DIM_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
   const int rc = refine_core(ctx, obs4, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override, poses,
-                             se3, zoom_factor, bbox, st);
+                             se3, zoom_factor, bbox, st, lit);
   cudaGraph_t graph = nullptr;
   const cudaError_t ce = cudaStreamEndCapture(st, &graph);
   if (rc != 0 || ce != cudaSuccess || graph == nullptr) {
@@ -509,10 +541,24 @@ DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int3
                         se3, zoom_factor, bbox, st);
 }
 
-DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host,
-                                      const double *pose_host, int32_t B, int32_t n_iter, const float *K9, float zn,
-                                      float zf, const double *means, int32_t precision, double *poses_out,
-                                      float *se3_out, void *stream) {
+DIM_API int32_t dim_refine_lit(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
+                               int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
+                               int32_t precision, const double *pose_override, double *poses, float *se3,
+                               float *zoom_factor, int32_t *bbox, const dim_lighting *lighting, void *stream) {
+  if (int rc = lit_check(ctx, lighting, "dim_refine_lit")) return rc;
+  DIM_REQUIRE(image_observed && cls_idx && pose_init && K9 && means && poses, "dim_refine_lit: NULL argument");
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_lit: batch exceeds max_batch");
+  DIM_REQUIRE(n_iter >= 1, "dim_refine_lit: n_iter must be >= 1");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (int rc = pack_obs4_launch(ctx, image_observed, B, ctx->obs4, means, st)) return rc;
+  return refine_graphed(ctx, ctx->obs4, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override, poses,
+                        se3, zoom_factor, bbox, st, lighting);
+}
+
+// dim_refine_host(_lit)_async; lit_host: the caller's lighting with HOST intensities [n_iter,B,3] (nullptr: unlit)
+static int refine_host_impl(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host, int32_t B,
+                            int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
+                            double *poses_out, float *se3_out, const dim_lighting *lit_host, cudaStream_t st) {
   DIM_REQUIRE(ctx && img_u8 && cls_host && pose_host && K9 && means && poses_out, "dim_refine_host: NULL argument");
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_host: batch exceeds max_batch");
   DIM_REQUIRE(n_iter >= 1 && n_iter <= 8, "dim_refine_host: n_iter must be in [1,8]");
@@ -524,18 +570,52 @@ DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *img_u8, const
       return 2;
     }
   }
-  cudaStream_t st = (cudaStream_t)stream;
   const size_t P = (size_t)ctx->H * ctx->W;
   DIM_CHECK(cudaMemcpyAsync(ctx->image_observed_u8, img_u8, (size_t)B * 3 * P, cudaMemcpyHostToDevice, st));
   DIM_CHECK(cudaMemcpyAsync(ctx->cls_dev, cls_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
   DIM_CHECK(cudaMemcpyAsync(ctx->pose_cur, pose_host, sizeof(double) * B * 12, cudaMemcpyHostToDevice, st));
+  dim_lighting lit_dev;  // the caller's lighting with the intensities moved to the context's buffer (fixed address: graphs)
+  if (lit_host) {
+    lit_dev = *lit_host;
+    lit_dev.intensity = ctx->lit_intensity;
+    DIM_CHECK(cudaMemcpyAsync(ctx->lit_intensity, lit_host->intensity, sizeof(float) * (size_t)n_iter * B * 3,
+                              cudaMemcpyHostToDevice, st));
+  }
   if (int rc = transform_u8_obs4_launch(ctx, ctx->image_observed_u8, B, means, ctx->obs4, st)) return rc;
   if (int rc = refine_graphed(ctx, ctx->obs4, ctx->cls_dev, ctx->pose_cur, B, n_iter, K9, zn, zf, means, precision,
-                              nullptr, ctx->poses_dev, ctx->se3_hist_dev, nullptr, nullptr, st))
+                              nullptr, ctx->poses_dev, ctx->se3_hist_dev, nullptr, nullptr, st, lit_host ? &lit_dev : nullptr))
     return rc;
   DIM_CHECK(cudaMemcpyAsync(poses_out, ctx->poses_dev, sizeof(double) * (size_t)n_iter * B * 12, cudaMemcpyDeviceToHost, st));
   if (se3_out)
     DIM_CHECK(cudaMemcpyAsync(se3_out, ctx->se3_hist_dev, sizeof(float) * (size_t)n_iter * B * 7, cudaMemcpyDeviceToHost, st));
+  return 0;
+}
+
+DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host,
+                                      const double *pose_host, int32_t B, int32_t n_iter, const float *K9, float zn,
+                                      float zf, const double *means, int32_t precision, double *poses_out,
+                                      float *se3_out, void *stream) {
+  return refine_host_impl(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out, se3_out,
+                          nullptr, (cudaStream_t)stream);
+}
+
+DIM_API int32_t dim_refine_host_lit_async(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host,
+                                          const double *pose_host, int32_t B, int32_t n_iter, const float *K9, float zn,
+                                          float zf, const double *means, int32_t precision, double *poses_out,
+                                          float *se3_out, const dim_lighting *lighting, void *stream) {
+  if (int rc = lit_check(ctx, lighting, "dim_refine_host_lit")) return rc;
+  return refine_host_impl(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out, se3_out,
+                          lighting, (cudaStream_t)stream);
+}
+
+DIM_API int32_t dim_refine_host_lit(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host,
+                                    int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
+                                    int32_t precision, double *poses_out, float *se3_out, const dim_lighting *lighting,
+                                    void *stream) {
+  if (int rc = dim_refine_host_lit_async(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision,
+                                         poses_out, se3_out, lighting, stream))
+    return rc;
+  DIM_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
   return 0;
 }
 
@@ -561,28 +641,29 @@ DIM_API int32_t dim_refine_host(dim_ctx *ctx, const uint8_t *img_u8, const int32
   return 0;
 }
 
-DIM_API int32_t dim_train_update(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose, const float *rot_est,
-                                 const float *trans_est, const float *tgt_pose, const float *depth_gt_observed,
-                                 int32_t B, const double *K9, float zn, float zf, const double *means,
-                                 const double *Tm, const double *Ts, int32_t rot_coord, float *image_rendered,
-                                 float *depth_rendered, float *mask_rendered, float *src_pose_new, float *rot_label,
-                                 float *trans_label, float *flow, float *flow_weights, void *stream) {
+// dim_train_update(_lit); lit: nullptr = the unlit re-render
+static int train_update_impl(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose, const float *rot_est,
+                             const float *trans_est, const float *tgt_pose, const float *depth_gt_observed, int32_t B,
+                             const double *K9, float zn, float zf, const double *means, const double *Tm, const double *Ts,
+                             int32_t rot_coord, float *image_rendered, float *depth_rendered, float *mask_rendered,
+                             float *src_pose_new, float *rot_label, float *trans_label, float *flow, float *flow_weights,
+                             const dim_lighting *lit, cudaStream_t st) {
   DIM_REQUIRE(ctx && cls_idx && src_pose && rot_est && trans_est && tgt_pose && K9 && means && Tm && Ts,
               "dim_train_update: NULL argument");
   DIM_REQUIRE(image_rendered && depth_rendered && mask_rendered && src_pose_new && rot_label && trans_label,
               "dim_train_update: NULL output");
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_train_update: batch exceeds max_batch");
   DIM_REQUIRE(rot_coord >= 0 && rot_coord <= 2, "dim_train_update: unknown rot_coord");
-  cudaStream_t st = (cudaStream_t)stream;
   float *KT = ctx->pose_cur_f32;  // [B,12] scratch
   if (int rc = train_pose_launch(src_pose, rot_est, trans_est, tgt_pose, B, Tm, Ts, rot_coord, K9, src_pose_new,
-                                 rot_label, trans_label, KT, st))
+                                 rot_label, trans_label, KT, st, lit ? ctx->light_pos : nullptr, lit ? lit->offset : nullptr))
     return rc;
   const float K9f[9] = {(float)K9[0], (float)K9[1], (float)K9[2], (float)K9[3], (float)K9[4],
                         (float)K9[5], (float)K9[6], (float)K9[7], (float)K9[8]};
-  // no uint8 truncation on the train path (batch_updater_py_multi.py:184,234)
+  // no uint8 truncation on the train path (batch_updater_py_multi.py:184,234); the lit colours are already 8-bit quantised
+  const LitParams lp = lit ? lit_params(ctx->light_pos, lit->intensity, lit->brightness_ratio) : LitParams{nullptr, nullptr, 0.f, 0.f};
   if (int rc = render_launch(ctx, cls_idx, src_pose_new, B, K9f, zn, zf, means, 0, image_rendered, depth_rendered,
-                             mask_rendered, nullptr, nullptr, nullptr, st))
+                             mask_rendered, nullptr, nullptr, nullptr, st, lit ? &lp : nullptr))
     return rc;
   if (flow && flow_weights) {
     DIM_REQUIRE(depth_gt_observed != nullptr, "dim_train_update: flow labels need depth_gt_observed");
@@ -603,6 +684,30 @@ DIM_API int32_t dim_train_update(dim_ctx *ctx, const int32_t *cls_idx, const flo
                                   P * sizeof(float), B, cudaMemcpyDeviceToDevice, st));
   }
   return 0;
+}
+
+DIM_API int32_t dim_train_update(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose, const float *rot_est,
+                                 const float *trans_est, const float *tgt_pose, const float *depth_gt_observed,
+                                 int32_t B, const double *K9, float zn, float zf, const double *means,
+                                 const double *Tm, const double *Ts, int32_t rot_coord, float *image_rendered,
+                                 float *depth_rendered, float *mask_rendered, float *src_pose_new, float *rot_label,
+                                 float *trans_label, float *flow, float *flow_weights, void *stream) {
+  return train_update_impl(ctx, cls_idx, src_pose, rot_est, trans_est, tgt_pose, depth_gt_observed, B, K9, zn, zf, means, Tm,
+                           Ts, rot_coord, image_rendered, depth_rendered, mask_rendered, src_pose_new, rot_label, trans_label,
+                           flow, flow_weights, nullptr, (cudaStream_t)stream);
+}
+
+DIM_API int32_t dim_train_update_lit(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose, const float *rot_est,
+                                     const float *trans_est, const float *tgt_pose, const float *depth_gt_observed,
+                                     int32_t B, const double *K9, float zn, float zf, const double *means,
+                                     const double *Tm, const double *Ts, int32_t rot_coord, float *image_rendered,
+                                     float *depth_rendered, float *mask_rendered, float *src_pose_new, float *rot_label,
+                                     float *trans_label, float *flow, float *flow_weights, const dim_lighting *lighting,
+                                     void *stream) {
+  if (int rc = lit_check(ctx, lighting, "dim_train_update_lit")) return rc;
+  return train_update_impl(ctx, cls_idx, src_pose, rot_est, trans_est, tgt_pose, depth_gt_observed, B, K9, zn, zf, means, Tm,
+                           Ts, rot_coord, image_rendered, depth_rendered, mask_rendered, src_pose_new, rot_label, trans_label,
+                           flow, flow_weights, lighting, (cudaStream_t)stream);
 }
 
 DIM_API int32_t dim_profile_enable(dim_ctx *ctx, int32_t enable) {

@@ -116,6 +116,8 @@ struct dim_ctx {
   int *cls_dev = nullptr;
   double *poses_dev = nullptr;  // [8, max_batch, 12]
   float *se3_hist_dev = nullptr;
+  float *light_pos = nullptr;      // [max_batch,3] lit chain / lit train update: light of the pose being rendered
+  float *lit_intensity = nullptr;  // [8, max_batch, 3] dim_refine_host_lit: the caller's light intensities on the device
   dim::NetState *net = nullptr;
   // CUDA graphs of the fused refinement chain (capi.cu refine_graphed): one executable graph per distinct argument set
   struct RefineGraph {

@@ -202,7 +202,7 @@ __global__ void train_pose_kernel(const float *src_pose, const float *rot_est, c
                                   const float *tgt_pose, int B, double m0, double m1, double m2, double s0, double s1,
                                   double s2, int rot_coord, double k0, double k1, double k2, double k3, double k4,
                                   double k5, double k6, double k7, double k8, float *pose_new_f32, float *rot_label,
-                                  float *trans_label, float *KT) {
+                                  float *trans_label, float *KT, float *light_pos, double l0, double l1, double l2) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   double ps[12], pt[12], po[12];
@@ -213,6 +213,12 @@ __global__ void train_pose_kernel(const float *src_pose, const float *rot_est, c
   const double Tm[3] = {m0, m1, m2}, Ts[3] = {s0, s1, s2};
   rt_transform_f64(ps, quat, td, Tm, Ts, rot_coord, po);
   for (int k = 0; k < 12; ++k) pose_new_f32[12 * b + k] = (float)po[k];
+  // ModelNet branch (batch_updater_py_multi.py:203-207): the light follows the float64 refined pose
+  if (light_pos) {
+    light_pos[3 * b + 0] = (float)(l0 + po[3]);
+    light_pos[3 * b + 1] = (float)(l1 - po[7]);
+    light_pos[3 * b + 2] = (float)(l2 - po[11]);
+  }
   // calc_RT_delta(refined, tgt, QUAT)  (RT_transform.py:16-44)
   double Rd[9];
   for (int i = 0; i < 3; ++i)
@@ -256,12 +262,17 @@ __global__ void train_pose_kernel(const float *src_pose, const float *rot_est, c
                                         Kd[i * 3 + 2] * (double)se3[2 * 4 + j]);
 }
 
+// light_pos (nullable) [B,3]: also write the light of the ModelNet branch, light_offset + (t_x, -t_y, -t_z) of the refined pose
 int train_pose_launch(const float *src_pose, const float *rot_est, const float *trans_est, const float *tgt_pose, int B,
                       const double *Tm, const double *Ts, int rot_coord, const double *K9, float *pose_new_f32,
-                      float *rot_label, float *trans_label, float *KT, cudaStream_t st) {
+                      float *rot_label, float *trans_label, float *KT, cudaStream_t st, float *light_pos,
+                      const double *light_offset) {
+  const double l0 = light_pos ? light_offset[0] : 0.0, l1 = light_pos ? light_offset[1] : 0.0,
+               l2 = light_pos ? light_offset[2] : 0.0;
   train_pose_kernel<<<cdiv(B, 32), 32, 0, st>>>(src_pose, rot_est, trans_est, tgt_pose, B, Tm[0], Tm[1], Tm[2], Ts[0],
                                                  Ts[1], Ts[2], rot_coord, K9[0], K9[1], K9[2], K9[3], K9[4], K9[5], K9[6],
-                                                 K9[7], K9[8], pose_new_f32, rot_label, trans_label, KT);
+                                                 K9[7], K9[8], pose_new_f32, rot_label, trans_label, KT, light_pos, l0, l1,
+                                                 l2);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -272,6 +283,26 @@ __global__ void f64_to_f32_kernel(const double *a, float *b, int n) {
 }
 int f64_to_f32_launch(const double *a, float *b, int n, cudaStream_t st) {
   f64_to_f32_kernel<<<cdiv(n, 256), 256, 0, st>>>(a, b, n);
+  DIM_LAUNCH_CHECK();
+  return 0;
+}
+
+// Per-iteration head of the lit refinement chain (ModelNet branch, deepim/core/tester.py:146-160): the float32 src_pose blob
+// (as f64_to_f32) and the light that follows the pose, light = float32(offset[0] + t_x, offset[1] - t_y, offset[2] - t_z)
+// evaluated on the FLOAT64 pose before the cast (numpy float64 arithmetic; glumpy casts the uniform to float32).
+__global__ void pose_light_kernel(const double *pose, float *pose_f32, float *light_pos, int B, double o0, double o1,
+                                  double o2) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < 12 * B) pose_f32[i] = (float)pose[i];
+  if (i < B) {
+    const double *p = pose + 12 * i;
+    light_pos[3 * i + 0] = (float)(o0 + p[3]);
+    light_pos[3 * i + 1] = (float)(o1 - p[7]);
+    light_pos[3 * i + 2] = (float)(o2 - p[11]);
+  }
+}
+int pose_light_launch(const double *pose, float *pose_f32, float *light_pos, int B, const double *offset, cudaStream_t st) {
+  pose_light_kernel<<<cdiv(12 * B, 256), 256, 0, st>>>(pose, pose_f32, light_pos, B, offset[0], offset[1], offset[2]);
   DIM_LAUNCH_CHECK();
   return 0;
 }

@@ -25,6 +25,12 @@ class TrainConfig(C.Structure):
                 ("normalize_flow", f32), ("trans_means", f32 * 3), ("trans_stds", f32 * 3), ("rot_coord", i32)]
 
 
+class Lighting(C.Structure):
+    """dim_lighting (include/deepim_b200.h): the ModelNet branch's light -- intensity pointer, offset at zero translation
+    (GL frame), brightness ratio"""
+    _fields_ = [("intensity", vp), ("offset", C.c_double * 3), ("brightness_ratio", f32)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/deepim_b200.h
 SIGNATURES = {
     "dim_abi_version": (i32, []),
@@ -56,6 +62,11 @@ SIGNATURES = {
     "dim_refine": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, vp]),
     "dim_refine_host": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp]),
     "dim_refine_host_async": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp]),
+    "dim_refine_lit": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, C.POINTER(Lighting), vp]),
+    "dim_refine_host_lit": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, C.POINTER(Lighting), vp]),
+    "dim_refine_host_lit_async": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, C.POINTER(Lighting), vp]),
+    "dim_train_update_lit": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, pf64, f32, f32, pf64, pf64, pf64, i32, vp, vp, vp, vp, vp,
+                                   vp, vp, vp, C.POINTER(Lighting), vp]),
     "dim_transform_image_u8": (i32, [vp, vp, i32, pf64, vp, vp]),
     "dim_debug_activation": (i32, [vp, i32, i32, vp, u64]),
     "dim_debug_layer_geometry": (i32, [vp, i32, C.POINTER(i32)]),

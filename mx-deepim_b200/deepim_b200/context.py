@@ -11,6 +11,7 @@ import numpy as np
 import torch
 
 from . import _capi as capi
+from . import lighting as _lighting
 from ._capi import check, farr, lib
 
 WEIGHT_ORDER = ["flow_conv1", "conv2", "conv3", "conv3_1", "conv4", "conv4_1", "conv5", "conv5_1", "conv6",
@@ -33,6 +34,31 @@ def _chk(t, dtype, shape=None, name="tensor"):
     if shape is not None and tuple(t.shape) != tuple(shape):
         raise ValueError("%s: expected shape %s, got %s" % (name, tuple(shape), tuple(t.shape)))
     return t
+
+
+def _lighting_arg(lighting, shape, on_device):
+    """dim_lighting for a lighting dict (see deepim_b200.lighting): intensity float32 `shape`, a contiguous CUDA tensor when
+    on_device, else a host array (numpy or CPU torch tensor).  Returns (struct, host array to keep alive)."""
+    if "intensity" not in lighting:
+        raise ValueError("lighting needs 'intensity' (float32 %s)" % (tuple(shape),))
+    offset, ratio = _lighting.params(lighting)
+    inten, keep = lighting["intensity"], None
+    if on_device:
+        _chk(inten, torch.float32, shape, "lighting['intensity']")
+        ptr = _p(inten)
+    else:
+        if isinstance(inten, torch.Tensor):
+            if inten.is_cuda:
+                raise ValueError("lighting['intensity'] must be a host array for the host entry point")
+            keep = inten.contiguous()
+            _chk(keep, torch.float32, shape, "lighting['intensity']")
+            ptr = C.c_void_p(keep.data_ptr())
+        else:
+            keep = np.ascontiguousarray(inten, np.float32)
+            if keep.shape != tuple(shape):
+                raise ValueError("lighting['intensity']: expected shape %s, got %s" % (tuple(shape), keep.shape))
+            ptr = C.c_void_p(keep.ctypes.data)
+    return capi.Lighting(ptr, (C.c_double * 3)(*offset), float(np.float32(ratio))), keep
 
 
 class Context:
@@ -281,8 +307,10 @@ class Context:
 
     def train_update(self, cls_idx, src_pose, rot_est, trans_est, tgt_pose, depth_gt_observed, K,
                      pixel_means_rgb=(103.939, 116.779, 123.68), T_means=(0, 0, 0), T_stds=(1, 1, 1),
-                     rot_coord="camera", znear=0.25, zfar=6.0, want_flow=True):
-        """batchUpdaterPyMulti.forward on the device (lib/pair_matching/batch_updater_py_multi.py:91-328)."""
+                     rot_coord="camera", znear=0.25, zfar=6.0, want_flow=True, lighting=None):
+        """batchUpdaterPyMulti.forward on the device (lib/pair_matching/batch_updater_py_multi.py:91-328).
+        lighting: None = the unlit re-render (LINEMOD); a dict {intensity float32 [B,3] CUDA, offset, brightness_ratio}
+        = the ModelNet branch's lit re-render (l.187-229; see deepim_b200.lighting), every other output unchanged."""
         B = src_pose.shape[0]
         for n, t, shp in (("src_pose", src_pose, (B, 3, 4)), ("tgt_pose", tgt_pose, (B, 3, 4)), ("rot_est", rot_est, (B, 4)),
                           ("trans_est", trans_est, (B, 3))):
@@ -297,14 +325,18 @@ class Context:
         }
         if want_flow:
             _chk(depth_gt_observed, torch.float32, (B, 1, self.H, self.W), "depth_gt_observed")
-        check(lib.dim_train_update(self._h, _p(cls_idx), _p(src_pose), _p(rot_est), _p(trans_est), _p(tgt_pose),
-                                   _p(depth_gt_observed) if want_flow else None, B,
-                                   farr(np.asarray(K, np.float64).reshape(9), 9, C.c_double), znear, zfar,
-                                   farr(pixel_means_rgb, 3, C.c_double), farr(T_means, 3, C.c_double),
-                                   farr(T_stds, 3, C.c_double), capi.ROT_COORD[rot_coord.lower()],
-                                   _p(out["image_rendered"]), _p(out["depth_rendered"]), _p(out["mask_rendered"]),
-                                   _p(out["src_pose"]), _p(out["rot"]), _p(out["trans"]), _p(out["flow"]),
-                                   _p(out["flow_weights"]), self._stream()))
+        args = (self._h, _p(cls_idx), _p(src_pose), _p(rot_est), _p(trans_est), _p(tgt_pose),
+                _p(depth_gt_observed) if want_flow else None, B,
+                farr(np.asarray(K, np.float64).reshape(9), 9, C.c_double), znear, zfar,
+                farr(pixel_means_rgb, 3, C.c_double), farr(T_means, 3, C.c_double),
+                farr(T_stds, 3, C.c_double), capi.ROT_COORD[rot_coord.lower()],
+                _p(out["image_rendered"]), _p(out["depth_rendered"]), _p(out["mask_rendered"]),
+                _p(out["src_pose"]), _p(out["rot"]), _p(out["trans"]), _p(out["flow"]), _p(out["flow_weights"]))
+        if lighting is None:
+            check(lib.dim_train_update(*args, self._stream()))
+        else:
+            lit, _ = _lighting_arg(lighting, (B, 3), True)
+            check(lib.dim_train_update_lit(*args, C.byref(lit), self._stream()))
         return out
 
     def transform_image_u8(self, bgr_u8, pixel_means_rgb):
@@ -363,10 +395,14 @@ class Context:
         check(lib.dim_train_set_config(self._h, C.byref(cfg)))
 
     def refine(self, image_observed, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
-               pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, pose_override=None, out=None):
+               pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, pose_override=None, out=None,
+               lighting=None):
         """Device-resident fused loop.  image_observed f32[B,3,H,W], cls_idx i32[B], pose_init f64[B,3,4].
         out = the dict returned by an earlier call with the same shapes: results are written into those tensors again
-        (same device addresses -> the library replays its CUDA graph of the chain instead of re-enqueuing ~90 launches)."""
+        (same device addresses -> the library replays its CUDA graph of the chain instead of re-enqueuing ~90 launches).
+        lighting: None = the unlit loop (LINEMOD); a dict {intensity float32 [n_iter,B,3] CUDA, offset, brightness_ratio}
+        = the ModelNet branch's lit loop (see deepim_b200.lighting).  Reusing the same intensity tensor lets the lit chain
+        replay its graph as well."""
         B = image_observed.shape[0]
         _chk(image_observed, torch.float32, (B, 3, self.H, self.W), "image_observed")
         _chk(cls_idx, torch.int32, (B,), "cls_idx")
@@ -384,18 +420,24 @@ class Context:
             bbox = self._new((n_iter, B, 8), torch.int32)
         if pose_override is not None:
             _chk(pose_override, torch.float64, (n_iter, B, 3, 4), "pose_override")
-        check(lib.dim_refine(self._h, _p(image_observed), _p(cls_idx), _p(pose_init), B, n_iter,
-                             farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
-                             farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses), _p(se3),
-                             _p(zf), _p(bbox), self._stream()))
+        args = (self._h, _p(image_observed), _p(cls_idx), _p(pose_init), B, n_iter,
+                farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
+                farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses), _p(se3), _p(zf), _p(bbox))
+        if lighting is None:
+            check(lib.dim_refine(*args, self._stream()))
+        else:
+            lit, _ = _lighting_arg(lighting, (n_iter, B, 3), True)
+            check(lib.dim_refine_lit(*args, C.byref(lit), self._stream()))
         return {"poses": poses, "se3": se3, "zoom_factor": zf, "bbox": bbox}
 
     def refine_host(self, image_observed_u8, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
                     pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, poses_out=None,
-                    se3_out=None, sync=True):
+                    se3_out=None, sync=True, lighting=None):
         """Host-buffer entry (what a tester loop calls): uint8 BGR HWC images (pinned torch tensors or
         numpy), host poses in / out.  sync=False only enqueues on the current torch stream (outputs must
-        then be pinned and are valid after the stream is synchronised)."""
+        then be pinned and are valid after the stream is synchronised).
+        lighting: as refine() but with a HOST intensity array float32 [n_iter,B,3] (copied before the call returns,
+        unless it is pinned: then it must stay untouched until the stream is synchronised)."""
         def hptr(a):
             return C.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else C.c_void_p(a.ctypes.data)
         B = image_observed_u8.shape[0]
@@ -403,10 +445,16 @@ class Context:
             poses_out = np.empty((n_iter, B, 3, 4), np.float64)
         if se3_out is None:
             se3_out = np.empty((n_iter, B, 7), np.float32)
-        fn = lib.dim_refine_host if sync else lib.dim_refine_host_async
-        check(fn(self._h, hptr(image_observed_u8), hptr(cls_idx), hptr(pose_init), B, n_iter,
-                                  farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
-                 farr(pixel_means_rgb, 3, C.c_double), precision, hptr(poses_out), hptr(se3_out), self._stream()))
+        args = (self._h, hptr(image_observed_u8), hptr(cls_idx), hptr(pose_init), B, n_iter,
+                farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
+                farr(pixel_means_rgb, 3, C.c_double), precision, hptr(poses_out), hptr(se3_out))
+        if lighting is None:
+            fn = lib.dim_refine_host if sync else lib.dim_refine_host_async
+            check(fn(*args, self._stream()))
+        else:
+            lit, _keep = _lighting_arg(lighting, (n_iter, B, 3), False)
+            fn = lib.dim_refine_host_lit if sync else lib.dim_refine_host_lit_async
+            check(fn(*args, C.byref(lit), self._stream()))
         return poses_out, se3_out
 
 

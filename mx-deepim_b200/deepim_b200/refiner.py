@@ -4,13 +4,18 @@ update_data_batch -> predict ...).  Also lifts the reference's batch=1 / single-
 (tester.py:83, SURVEY 3.1): any number of instances, sharded over ranks.
 
 Two device contexts on two CUDA streams are used round-robin, so the H2D copy of batch k+1 overlaps
-the kernels of batch k (instances are independent; nothing else is shared but read-only weights)."""
+the kernels of batch k (instances are independent; nothing else is shared but read-only weights).
+
+lighting={"seed", "offset", "brightness_ratio"} runs the ModelNet branch's lit loop (deepim_b200.lighting): every mesh must
+carry `normals`, and each submit draws its light intensities [n_iter, n, 3] from one Generator seeded once
+(lighting.sample_intensity), the fresh draw per render of the reference."""
 from __future__ import annotations
 
 import numpy as np
 import torch
 
 from . import _capi as capi
+from . import lighting as _lighting
 from . import sharding, synth
 from .context import Context
 
@@ -18,7 +23,12 @@ from .context import Context
 class PoseRefiner:
     def __init__(self, meshes, weights, K=synth.K_LINEMOD, device=0, max_batch=16, n_iter=4,
                  pixel_means_rgb=synth.PIXEL_MEANS_RGB, znear=synth.ZNEAR, zfar=synth.ZFAR, precision="fp16",
-                 n_slots=2):
+                 n_slots=2, lighting=None):
+        self.light = _lighting.LightSource.of(lighting)
+        if self.light is not None:
+            for i, m in enumerate(meshes):
+                if getattr(m, "normals", None) is None:
+                    raise ValueError("PoseRefiner(lighting=...): mesh %d has no per-vertex normals" % i)
         self.K = np.asarray(K, np.float32)
         self.n_iter, self.means, self.zn, self.zf = n_iter, np.asarray(pixel_means_rgb, np.float64), znear, zfar
         self.precision = capi.precision_id(precision)
@@ -37,6 +47,7 @@ class PoseRefiner:
                 "se3": torch.empty((n_iter, max_batch, 7), dtype=torch.float32).pin_memory(),
                 "status": torch.zeros((min(n_iter, 8) * max_batch,), dtype=torch.int32).pin_memory(),
                 "img": None, "cls": None, "pose": None,
+                "intensity": torch.empty((n_iter, max_batch, 3), dtype=torch.float32).pin_memory() if self.light else None,
             })
         self.ctx = self.slots[0]["ctx"]
         self._next = 0
@@ -68,9 +79,14 @@ class PoseRefiner:
         img = self._pinned(slot, "img", images_bgr_u8, torch.uint8)
         cls = self._pinned(slot, "cls", cls_idx, torch.int32)
         pose = self._pinned(slot, "pose", poses_init, torch.float64)
+        lit = None
+        if self.light is not None:  # a fresh draw per render; the pinned buffer lives until result() of this slot
+            inten = slot["intensity"].view(-1)[: self.n_iter * n * 3].view(self.n_iter, n, 3)
+            inten.copy_(torch.from_numpy(self.light.draw((self.n_iter, n))))
+            lit = self.light.lighting(inten)
         with torch.cuda.stream(slot["stream"]):
             slot["ctx"].refine_host(img, cls, pose, self.K, self.n_iter, self.zn, self.zf, self.means, self.precision,
-                                    poses_out=slot["poses"], se3_out=slot["se3"], sync=False)
+                                    poses_out=slot["poses"], se3_out=slot["se3"], sync=False, lighting=lit)
             slot["ctx"].refine_status(n, self.n_iter, out=slot["status"], sync=False)
         slot["busy"], slot["n"] = True, n
         self._next = (i + 1) % len(self.slots)

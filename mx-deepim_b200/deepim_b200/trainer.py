@@ -13,6 +13,7 @@ import numpy as np
 import torch
 
 from . import _capi as capi
+from . import lighting as _lighting
 from ._capi import check, lib
 
 NORMALIZE_FLOW = 20.0
@@ -247,13 +248,16 @@ class Trainer:
 
 
 def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000, init_mask="box_gt", poses=None,
-                      image_observed=None, cls_np=None):
+                      image_observed=None, cls_np=None, lighting=None):
     """Synthetic training batch built with the device kernels only (config C4: rendered pairs, labels from
     dim_train_update, INIT_MASK box_gt without dilation, 3000 sampled model points as get_point_cloud_model,
     lib/utils/image.py:452-478).  init_mask = "box_gt" (the reference's training config: mask_observed = box of the GT mask)
     or "box_rendered" (the TEST-time convention, yaml:118: box of the rendered mask -- train / test inputs then match).
     poses = (pose_observed, pose_init) [B,3,4] instead of sampling them from `seed`; image_observed = the observed blob to
     train on (float32 [B,3,H,W] RGB - mean, e.g. a render composited over a background) instead of the clean render.
+    lighting = None (LINEMOD) or the ModelNet branch's light ({"seed", "offset", "brightness_ratio"} or a
+    lighting.LightSource; the meshes' normals must be uploaded to ctx): the observed and the rendered images are lit renders,
+    each with a fresh intensity draw.
     Returns (batch dict of CUDA tensors, cls int32[B], tgt_pose f32[B,3,4], depth_gt)."""
     from . import synth
     obs, ini = synth.sample_pose_pairs(B, seed) if poses is None else poses
@@ -262,9 +266,16 @@ def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000,
     cls = torch.from_numpy(cls_np).to(dev)
     tgt = torch.from_numpy(obs.astype(np.float32)).to(dev)
     src = torch.from_numpy(ini.astype(np.float32)).to(dev)
-    r = ctx.render(cls, tgt, K, pixel_means_rgb=pixel_means_rgb, trunc_u8=True)
+    light = _lighting.LightSource.of(lighting)
+    if light is None:
+        r = ctx.render(cls, tgt, K, pixel_means_rgb=pixel_means_rgb, trunc_u8=True)
+    else:
+        lp = torch.from_numpy(_lighting.modelnet_light_position(obs)).to(dev)
+        r = ctx.render_lit(cls, tgt, K, lp, torch.from_numpy(light.draw(B)).to(dev), light.brightness_ratio,
+                           pixel_means_rgb=pixel_means_rgb, want=("image", "depth", "mask"))
     ident = torch.tensor([[1.0, 0, 0, 0]] * B, dtype=torch.float32, device=dev)
-    upd = ctx.train_update(cls, src, ident, torch.zeros(B, 3, device=dev), tgt, r["depth"], K, pixel_means_rgb=pixel_means_rgb)
+    upd = ctx.train_update(cls, src, ident, torch.zeros(B, 3, device=dev), tgt, r["depth"], K, pixel_means_rgb=pixel_means_rgb,
+                           lighting=_device_lighting(light, B, dev))
     rng = np.random.default_rng(seed)
     pts, pw = np.zeros((B, 3, num_points), np.float32), np.zeros((B, 3, num_points), np.float32)
     for b in range(B):
@@ -282,11 +293,19 @@ def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000,
     return batch, cls, tgt, r["depth"]
 
 
-def fit_batch(trainer, batch, cls, tgt_pose, depth_gt, K, n_inner=4, dist=None, update_mask="fixed"):
+def _device_lighting(light, B, dev):
+    """Context.train_update's lighting for one lit re-render of B instances (a fresh intensity draw), or None"""
+    return None if light is None else light.lighting(torch.from_numpy(light.draw(B)).to(dev))
+
+
+def fit_batch(trainer, batch, cls, tgt_pose, depth_gt, K, n_inner=4, dist=None, update_mask="fixed", lighting=None):
     """One data batch of Module.fit (deepim/core/module.py:1131-1137): n_inner x (forward_backward, update), the
     batch re-rendered at the predicted pose in between (batchUpdaterPyMulti.forward -> Context.train_update).
+    lighting = None or the ModelNet branch's light ({"seed", "offset", "brightness_ratio"} or a lighting.LightSource, which
+    keeps drawing fresh intensities across calls): the re-renders are lit (batch_updater_py_multi.py:187-229).
     Returns the objective of every inner iteration (device tensor [n_inner])."""
     ctx = trainer.ctx
+    light = _lighting.LightSource.of(lighting)
     b = dict(batch)
     objs = []
     for it in range(n_inner):
@@ -295,7 +314,8 @@ def fit_batch(trainer, batch, cls, tgt_pose, depth_gt, K, n_inner=4, dist=None, 
         objs.append(res["losses"][3])
         if it != n_inner - 1:
             upd = ctx.train_update(cls, b["src_pose"], res["rot_est_norm"], res["trans_est"], tgt_pose, depth_gt, K,
-                                   pixel_means_rgb=batch["pixel_means_rgb"])
+                                   pixel_means_rgb=batch["pixel_means_rgb"],
+                                   lighting=_device_lighting(light, cls.shape[0], ctx.device))
             for k in ("image_rendered", "mask_rendered", "src_pose", "flow", "flow_weights"):
                 b[k] = upd[k]
             if update_mask == "box_rendered":  # what update_data_batch does at test time (data_pair.py:93-105); the reference's
