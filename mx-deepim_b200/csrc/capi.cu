@@ -2,7 +2,7 @@
 #include <stdarg.h>
 #include <string.h>
 
-#include "common.cuh"
+#include "launch.cuh"
 
 namespace dim {
 
@@ -14,84 +14,6 @@ void set_error(const char *fmt, ...) {
   va_start(ap, fmt);
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
-}
-
-// implemented in raster.cu / zoom.cu / geom.cu / net.cu
-struct LitParams { const float *light_pos, *light_int; float a0, a1; };  // device [B,3] each; a0 = 1 - ratio, a1 = ratio
-int render_launch(dim_ctx *, const int *, const float *, int, const float *, float, float, const double *, int, float *,
-                  float *, float *, float *, int *, float4 *, cudaStream_t, const LitParams *lit = nullptr);
-int zoom_gather_launch(dim_ctx *, int mode, const float *src, float *dst, const float *zf, int B, int C, int inv,
-                       const float *param, cudaStream_t);
-int zoom_factor_launch(dim_ctx *, const float *, const float *, int C, const float *, int B, const float *K9, float *,
-                       int *, int *, cudaStream_t, const float *img_means = nullptr);
-int pose_error_launch(const double *, const double *, int M, const double *, int N, int symmetric, double *, cudaStream_t);
-int epe_launch(const float *, const float *, const float *, const float *, int B, int P, double *, cudaStream_t);
-int pose_error2d_launch(const double *, const double *, int M, const double *, int N, const double *K9, double *, cudaStream_t);
-int group_pick_launch(const float *, const float *, int B, int Ctot, int groups, size_t n, float *, int backward, cudaStream_t);
-int zoom_factor_from_ren_launch(dim_ctx *, const int *, const float *, int B, const float *K9, float *, int *, int *,
-                                cudaStream_t);
-int box_mask_launch(dim_ctx *, const int *, int B, float *, cudaStream_t);
-int zoom_fused_launch(dim_ctx *, const float4 *, const float4 *, const float *, const float *, int B, int Hs, int Ws,
-                      int pad, __nv_bfloat16 *, __nv_bfloat16 *, cudaStream_t, int f16, const double *means_d);
-int pack_obs4_launch(dim_ctx *, const float *, int B, float4 *, const double *means, cudaStream_t);
-int transform_u8_obs4_launch(dim_ctx *, const uint8_t *, int B, const double *, float4 *, cudaStream_t);
-int pack_nhwc8_launch(dim_ctx *, const float *, const float *, const float *, const float *, int B, int Hs, int Ws,
-                      int pad, __nv_bfloat16 *, __nv_bfloat16 *, cudaStream_t, int f16);
-int flow_launch(dim_ctx *, const float *, const float *, const float *, const float *, int B, float *, float *,
-                float *, cudaStream_t);
-int train_pose_launch(const float *, const float *, const float *, const float *, int B, const double *,
-                      const double *, int, const double *, float *, float *, float *, float *, cudaStream_t,
-                      float *light_pos = nullptr, const double *light_offset = nullptr);
-int se3_compose_launch(const double *, const float *, int B, const double *, const double *, int, double *, float *,
-                       cudaStream_t);
-int f64_to_f32_launch(const double *, float *, int n, cudaStream_t);
-int pose_light_launch(const double *pose, float *pose_f32, float *light_pos, int B, const double *offset, cudaStream_t);
-int zoom_trans_launch(const float *, const float *, int B, int mul, int scale_xy, float *, cudaStream_t);
-int transform3d_fwd_launch(const float *, const float *, const float *, const float *, int, int, const float *,
-                           const float *, int, float *, cudaStream_t);
-int transform3d_bwd_launch(const float *, const float *, const float *, const float *, const float *, int, int,
-                           const float *, const float *, int, float *, float *, cudaStream_t);
-int transform_u8_launch(dim_ctx *, const uint8_t *, int B, const double *, float *, cudaStream_t);
-int net_create(dim_ctx *);
-void net_destroy(dim_ctx *);
-int net_load(dim_ctx *, const float *const *, const float *const *);
-void net_input_geometry(dim_ctx *, int *rows, int *cols, int *pad, __nv_bfloat16 **hi, __nv_bfloat16 **lo);
-int net_forward(dim_ctx *, int B, int precision, const float *zoom_factor, float *rot, float *trans, float *se3,
-                cudaStream_t, cudaEvent_t after_conv);
-int net_debug_activation(dim_ctx *, int idx, int lo, void *host_dst, size_t bytes);
-void net_layer_geometry(dim_ctx *, int idx, int *out);
-bool net_graph_safe(dim_ctx *);
-int net_set_option(dim_ctx *, const char *key, int value);
-int net_layer_profile(dim_ctx *, int enable, float *ms10);
-// train.cu
-struct TrainIO {
-  const float *zio, *zir, *zmo, *zmr, *zoom_factor, *zflow, *zfw, *zmask_gt, *src_pose, *pc_model, *pc_weights, *pc_observed;
-  int B, N;
-  float *rot_est_norm, *trans_est, *flow_est, *mask_prob, *losses, *grads;
-  float *rot_raw;
-  void *const *bucket_events;
-  const int *bucket_first_tensor;
-  int n_buckets;
-};
-int train_create(dim_ctx *, int max_points);
-void train_destroy(dim_ctx *);
-int train_load_params(dim_ctx *, const float *flat_host, size_t n, cudaStream_t);
-int train_get_params(dim_ctx *, float *flat_host, size_t n, int which, cudaStream_t);
-size_t train_param_count(dim_ctx *);
-int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel);
-int train_forward_backward(dim_ctx *, const TrainIO &, cudaStream_t);
-int train_sgd_update(dim_ctx *, const float *grads, float lr, float momentum, float wd, float rescale, cudaStream_t);
-int train_debug_tensor(dim_ctx *, int id, void *host, size_t bytes);
-void train_debug_geometry(dim_ctx *, int id, int *out);
-int train_debug_phases(dim_ctx *, float *ms7);
-
-template <typename T>
-static int ctx_alloc(dim_ctx *ctx, T **p, size_t n) {
-  void *q = nullptr;
-  DIM_CHECK(cudaMalloc(&q, n * sizeof(T)));
-  ctx->owned.push_back(q);
-  *p = reinterpret_cast<T *>(q);
-  return 0;
 }
 
 }  // namespace dim
@@ -141,30 +63,27 @@ DIM_API int32_t dim_ctx_create(int32_t device, int32_t max_batch, int32_t H, int
   ctx->num_sms = prop.multiProcessorCount;
   const size_t P = (size_t)H * W, Bm = (size_t)max_batch;
   int rc = 0;
-  rc |= ctx_alloc(ctx, &ctx->meshes, (size_t)max_classes);
-  rc |= ctx_alloc(ctx, &ctx->pverts, Bm * (size_t)max_verts);
-  rc |= ctx_alloc(ctx, &ctx->vis, Bm * P);
-  rc |= ctx_alloc(ctx, &ctx->vbox, Bm * 4);
-  rc |= ctx_alloc(ctx, &ctx->bbox8, Bm * 8);
-  rc |= ctx_alloc(ctx, &ctx->status, Bm);
-  rc |= ctx_alloc(ctx, &ctx->cls_flag, Bm);
-  rc |= ctx_alloc(ctx, &ctx->status_hist, 8 * Bm);
-  rc |= ctx_alloc(ctx, &ctx->zoom_factor, Bm * 4);
-  rc |= ctx_alloc(ctx, &ctx->image_rendered, Bm * 3 * P);
-  rc |= ctx_alloc(ctx, &ctx->depth_rendered, Bm * P);
-  rc |= ctx_alloc(ctx, &ctx->mask_rendered, Bm * P);
-  rc |= ctx_alloc(ctx, &ctx->bbox_ren, Bm * 4);
-  rc |= ctx_alloc(ctx, &ctx->pose_cur, Bm * 12);
-  rc |= ctx_alloc(ctx, &ctx->pose_cur_f32, Bm * 12);
-  rc |= ctx_alloc(ctx, &ctx->se3_cur, Bm * 7);
-  rc |= ctx_alloc(ctx, &ctx->ren4, Bm * P);
-  rc |= ctx_alloc(ctx, &ctx->obs4, Bm * P);
-  rc |= ctx_alloc(ctx, &ctx->image_observed_u8, Bm * 3 * P);
-  rc |= ctx_alloc(ctx, &ctx->cls_dev, Bm);
-  rc |= ctx_alloc(ctx, &ctx->poses_dev, 8 * Bm * 12);
-  rc |= ctx_alloc(ctx, &ctx->se3_hist_dev, 8 * Bm * 7);
-  rc |= ctx_alloc(ctx, &ctx->light_pos, Bm * 3);
-  rc |= ctx_alloc(ctx, &ctx->lit_intensity, 8 * Bm * 3);
+  rc |= dev_alloc(ctx, &ctx->meshes, (size_t)max_classes);
+  rc |= dev_alloc(ctx, &ctx->pverts, Bm * (size_t)max_verts);
+  rc |= dev_alloc(ctx, &ctx->vis, Bm * P);
+  rc |= dev_alloc(ctx, &ctx->vbox, Bm * 4);
+  rc |= dev_alloc(ctx, &ctx->bbox8, Bm * 8);
+  rc |= dev_alloc(ctx, &ctx->cls_flag, Bm);
+  rc |= dev_alloc(ctx, &ctx->status_hist, 8 * Bm);
+  rc |= dev_alloc(ctx, &ctx->zoom_factor, Bm * 4);
+  rc |= dev_alloc(ctx, &ctx->mask_rendered, Bm * P);
+  rc |= dev_alloc(ctx, &ctx->bbox_ren, Bm * 4);
+  rc |= dev_alloc(ctx, &ctx->pose_cur, Bm * 12);
+  rc |= dev_alloc(ctx, &ctx->pose_cur_f32, Bm * 12);
+  rc |= dev_alloc(ctx, &ctx->se3_cur, Bm * 7);
+  rc |= dev_alloc(ctx, &ctx->ren4, Bm * P);
+  rc |= dev_alloc(ctx, &ctx->obs4, Bm * P);
+  rc |= dev_alloc(ctx, &ctx->image_observed_u8, Bm * 3 * P);
+  rc |= dev_alloc(ctx, &ctx->cls_dev, Bm);
+  rc |= dev_alloc(ctx, &ctx->poses_dev, 8 * Bm * 12);
+  rc |= dev_alloc(ctx, &ctx->se3_hist_dev, 8 * Bm * 7);
+  rc |= dev_alloc(ctx, &ctx->light_pos, Bm * 3);
+  rc |= dev_alloc(ctx, &ctx->lit_intensity, 8 * Bm * 3);
   if (rc) { dim_ctx_destroy(ctx); return 12; }
   ctx->meshes_host.assign(max_classes, MeshDev{nullptr, nullptr, nullptr, nullptr, 0, 0, 0, 0, nullptr});
   DIM_CHECK(cudaMemset(ctx->meshes, 0, sizeof(MeshDev) * max_classes));
@@ -198,8 +117,8 @@ DIM_API int32_t dim_mesh_upload(dim_ctx *ctx, int32_t cls, const float *verts, c
   for (int32_t i = 0; i < 3 * F; ++i) DIM_REQUIRE(faces[i] >= 0 && faces[i] < V, "dim_mesh_upload: face index out of range");
   MeshDev m;
   float *dv, *du; int *df; uint8_t *dt;
-  if (ctx_alloc(ctx, &dv, (size_t)3 * V) || ctx_alloc(ctx, &du, (size_t)2 * V) || ctx_alloc(ctx, &df, (size_t)3 * F) ||
-      ctx_alloc(ctx, &dt, (size_t)3 * Th * Tw))
+  if (dev_alloc(ctx, &dv, (size_t)3 * V) || dev_alloc(ctx, &du, (size_t)2 * V) || dev_alloc(ctx, &df, (size_t)3 * F) ||
+      dev_alloc(ctx, &dt, (size_t)3 * Th * Tw))
     return 12;
   DIM_CHECK(cudaMemcpy(dv, verts, sizeof(float) * 3 * V, cudaMemcpyHostToDevice));
   DIM_CHECK(cudaMemcpy(du, uvs, sizeof(float) * 2 * V, cudaMemcpyHostToDevice));
@@ -225,10 +144,19 @@ DIM_API int32_t dim_mesh_upload_normals(dim_ctx *ctx, int32_t cls, const float *
   MeshDev &m = ctx->meshes_host[cls];
   DIM_REQUIRE(m.V > 0 && m.V == V, "dim_mesh_upload_normals: upload the mesh first; V must match");
   float *dn;
-  if (ctx_alloc(ctx, &dn, (size_t)3 * V)) return 12;
+  if (dev_alloc(ctx, &dn, (size_t)3 * V)) return 12;
   DIM_CHECK(cudaMemcpy(dn, normals, sizeof(float) * 3 * V, cudaMemcpyHostToDevice));
   m.normals = dn;
   DIM_CHECK(cudaMemcpy(ctx->meshes + cls, &m, sizeof(MeshDev), cudaMemcpyHostToDevice));
+  return 0;
+}
+// the lit renderer shades with per-vertex normals: every uploaded mesh must have them
+static int normals_check(dim_ctx *ctx, const char *fn) {
+  for (auto &m : ctx->meshes_host)
+    if (m.V > 0 && m.normals == nullptr) {
+      set_error("%s: a mesh has no normals (dim_mesh_upload_normals)", fn);
+      return 2;
+    }
   return 0;
 }
 // the lit loop / update entry points: lighting and its intensities are given and every uploaded mesh has normals
@@ -237,12 +165,7 @@ static int lit_check(dim_ctx *ctx, const dim_lighting *lit, const char *fn) {
     set_error("%s: NULL context, lighting or lighting->intensity", fn);
     return 2;
   }
-  for (auto &m : ctx->meshes_host)
-    if (m.V > 0 && m.normals == nullptr) {
-      set_error("%s: a mesh has no normals (dim_mesh_upload_normals)", fn);
-      return 2;
-    }
-  return 0;
+  return normals_check(ctx, fn);
 }
 static LitParams lit_params(const float *light_pos, const float *intensity, float ratio) {
   return LitParams{light_pos, intensity, (float)(1.0 - (double)ratio), ratio};
@@ -253,8 +176,8 @@ DIM_API int32_t dim_render_lit(dim_ctx *ctx, const int32_t *cls_idx, const float
                                float brightness_ratio, float *out_image, float *out_depth, float *out_mask, float *out_bgr,
                                int32_t *out_bbox, void *stream) {
   DIM_REQUIRE(ctx && cls_idx && pose && K9 && light_pos && light_int, "dim_render_lit: NULL argument");
-  for (auto &m : ctx->meshes_host) DIM_REQUIRE(m.V == 0 || m.normals != nullptr, "dim_render_lit: a mesh has no normals (dim_mesh_upload_normals)");
-  LitParams lit{light_pos, light_int, (float)(1.0 - (double)brightness_ratio), brightness_ratio};
+  if (int rc = normals_check(ctx, "dim_render_lit")) return rc;
+  const LitParams lit = lit_params(light_pos, light_int, brightness_ratio);
   return render_launch(ctx, cls_idx, pose, B, K9, zn, zf, means, 1, out_image, out_depth, out_mask, out_bgr, out_bbox, nullptr,
                        (cudaStream_t)stream, &lit);
 }
@@ -395,17 +318,14 @@ DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr, int32_t
   return transform_u8_launch(ctx, bgr, B, means, image, (cudaStream_t)stream);
 }
 
-static int refine_core(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_idx, const double *pose_init, int32_t B,
-                       int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
-                       const double *pose_override, double *poses, float *se3, float *zoom_factor, int32_t *bbox,
-                       cudaStream_t st, const dim_lighting *lit) {
+static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
   const double Tm[3] = {ctx->cfg.trans_means[0], ctx->cfg.trans_means[1], ctx->cfg.trans_means[2]};
   const double Ts[3] = {ctx->cfg.trans_stds[0], ctx->cfg.trans_stds[1], ctx->cfg.trans_stds[2]};
-  const float means_f[3] = {(float)means[0], (float)means[1], (float)means[2]};
+  const float means_f[3] = {(float)a.means[0], (float)a.means[1], (float)a.means[2]};
   int rows, cols, pad; __nv_bfloat16 *hi, *lo;
   net_input_geometry(ctx, &rows, &cols, &pad, &hi, &lo);
-  const double *pose_src = pose_init;
-  for (int it = 0; it < n_iter; ++it) {
+  const double *pose_src = a.pose_init;
+  for (int it = 0; it < a.n_iter; ++it) {
     DimNvtxRange r_it("dim_refine iteration");
     cudaEvent_t *ev = nullptr;
     if (ctx->prof) {
@@ -418,47 +338,47 @@ static int refine_core(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_idx,
       ctx->prof_used += 5;
       DIM_CHECK(cudaEventRecord(ev[0], st));
     }
-    if (pose_override) pose_src = pose_override + (size_t)it * B * 12;
+    if (a.pose_override) pose_src = a.pose_override + (size_t)it * a.B * 12;
     // src_pose blob is float32 (nd.array), the host pose stays float64 (tester.py:391); the lit chain also derives the
     // light of this iteration's render from the float64 pose
-    if (lit) {
-      if (int rc = pose_light_launch(pose_src, ctx->pose_cur_f32, ctx->light_pos, B, lit->offset, st)) return rc;
-    } else if (int rc = f64_to_f32_launch(pose_src, ctx->pose_cur_f32, B * 12, st)) {
+    if (a.lit) {
+      if (int rc = pose_light_launch(pose_src, ctx->pose_cur_f32, ctx->light_pos, a.B, a.offset, st)) return rc;
+    } else if (int rc = f64_to_f32_launch(pose_src, ctx->pose_cur_f32, a.B * 12, st)) {
       return rc;
     }
     // render at the current pose (tester.py:427-442) straight into the pixel-interleaved
     // (R,G,B,mask) image the zoom kernel samples; mask_observed := box(mask_rendered) is analytic
     {
       DimNvtxRange r("render");
-      const LitParams lp = lit ? lit_params(ctx->light_pos, lit->intensity + (size_t)it * B * 3, lit->brightness_ratio)
-                               : LitParams{nullptr, nullptr, 0.f, 0.f};
-      if (int rc = render_launch(ctx, cls_idx, ctx->pose_cur_f32, B, K9, zn, zf, means, 1, nullptr, nullptr, nullptr,
-                                 nullptr, nullptr, ctx->ren4, st, lit ? &lp : nullptr))
+      const LitParams lp = a.lit ? lit_params(ctx->light_pos, a.intensity + (size_t)it * a.B * 3, a.brightness_ratio)
+                                 : LitParams{nullptr, nullptr, 0.f, 0.f};
+      if (int rc = render_launch(ctx, a.cls_idx, ctx->pose_cur_f32, a.B, a.K9, a.zn, a.zf, a.means, 1, nullptr, nullptr,
+                                 nullptr, nullptr, nullptr, ctx->ren4, st, a.lit ? &lp : nullptr))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[1], st));
-    float *zf_it = zoom_factor ? zoom_factor + (size_t)it * B * 4 : ctx->zoom_factor;
-    int *bbox_it = bbox ? bbox + (size_t)it * B * 8 : nullptr;
+    float *zf_it = a.zoom_factor ? a.zoom_factor + (size_t)it * a.B * 4 : ctx->zoom_factor;
+    int *bbox_it = a.bbox ? a.bbox + (size_t)it * a.B * 8 : nullptr;
     // per-iteration status (bit 0: rendered / observed mask empty -> fallback zoom factor; bit 1: bad class index)
     {
       DimNvtxRange r("bbox + zoom");
-      if (int rc = zoom_factor_from_ren_launch(ctx, ctx->bbox_ren, ctx->pose_cur_f32, B, K9, zf_it, bbox_it,
-                                               ctx->status_hist + (size_t)(it < 8 ? it : 7) * B, st))
+      if (int rc = zoom_factor_from_ren_launch(ctx, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it, bbox_it,
+                                               ctx->status_hist + (size_t)(it < 8 ? it : 7) * a.B, st))
         return rc;
-      if (int rc = zoom_fused_launch(ctx, obs4, ctx->ren4, zf_it, means_f, B, rows, cols, pad, hi,
-                                     precision == DIM_PREC_BF16X3 ? lo : nullptr, st, precision == DIM_PREC_FP16, means))
+      if (int rc = zoom_fused_launch(ctx, a.obs4, ctx->ren4, zf_it, means_f, a.B, rows, cols, pad, hi,
+                                     a.precision == DIM_PREC_BF16X3 ? lo : nullptr, st, a.precision == DIM_PREC_FP16, a.means))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[2], st));
-    float *se3_it = se3 ? se3 + (size_t)it * B * 7 : ctx->se3_cur;
+    float *se3_it = a.se3 ? a.se3 + (size_t)it * a.B * 7 : ctx->se3_cur;
     {
       DimNvtxRange r("FlowNetS tower + heads");
-      if (int rc = net_forward(ctx, B, precision, zf_it, nullptr, nullptr, se3_it, st, ev ? ev[3] : nullptr)) return rc;
+      if (int rc = net_forward(ctx, a.B, a.precision, zf_it, nullptr, nullptr, se3_it, st, ev ? ev[3] : nullptr)) return rc;
     }
-    double *pose_out = poses + (size_t)it * B * 12;
+    double *pose_out = a.poses + (size_t)it * a.B * 12;
     {
       DimNvtxRange r("SE(3) compose");
-      if (int rc = se3_compose_launch(pose_src, se3_it, B, Tm, Ts, ctx->cfg.rot_coord, pose_out, nullptr, st)) return rc;
+      if (int rc = se3_compose_launch(pose_src, se3_it, a.B, Tm, Ts, ctx->cfg.rot_coord, pose_out, nullptr, st)) return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[4], st));
     pose_src = pose_out;
@@ -470,28 +390,13 @@ static int refine_core(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_idx,
 // its buffers (PoseRefiner does; so does bench.py).  After one eager run of an argument set the chain is captured into a
 // CUDA graph (stream capture, thread-local mode) and replayed with one cudaGraphLaunch: the data-dependent parts of the
 // loop are already branch-free on the device.  Disabled while stage / layer profiling is on or the context trains.
-static int refine_graphed(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_idx, const double *pose_init, int32_t B,
-                          int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
-                          const double *pose_override, double *poses, float *se3, float *zoom_factor, int32_t *bbox,
-                          cudaStream_t st, const dim_lighting *lit = nullptr) {
+static int refine_graphed(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
   // the legacy default stream (and the per-thread default stream handle) cannot be captured
   const bool capturable = st != nullptr && st != cudaStreamLegacy && st != cudaStreamPerThread;
-  if (!ctx->use_graph || ctx->prof || !capturable || !net_graph_safe(ctx))
-    return refine_core(ctx, obs4, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override, poses, se3,
-                       zoom_factor, bbox, st, lit);
-  std::vector<unsigned char> key;
-  auto put = [&key](const void *p, size_t n) { key.insert(key.end(), (const unsigned char *)p, (const unsigned char *)p + n); };
-  const void *ptrs[8] = {obs4, cls_idx, pose_init, pose_override, poses, se3, zoom_factor, bbox};
-  const int32_t ints[3] = {B, n_iter, precision};
-  put(ptrs, sizeof(ptrs)); put(ints, sizeof(ints)); put(K9, 9 * sizeof(float)); put(&zn, sizeof(zn)); put(&zf, sizeof(zf));
-  put(means, 3 * sizeof(double));
-  // a lit chain never shares a graph with an unlit one: the light's intensity buffer, offset and ratio are part of the key
-  const unsigned char is_lit = lit != nullptr;
-  put(&is_lit, 1);
-  if (lit) { put(&lit->intensity, sizeof(lit->intensity)); put(lit->offset, sizeof(lit->offset)); put(&lit->brightness_ratio, sizeof(float)); }
+  if (!ctx->use_graph || ctx->prof || !capturable || !net_graph_safe(ctx)) return refine_core(ctx, a, st);
   dim_ctx::RefineGraph *g = nullptr;
   for (auto &e : ctx->graphs)
-    if (e.key == key) { g = &e; break; }
+    if (memcmp(&e.key, &a, sizeof(RefineArgs)) == 0) { g = &e; break; }
   if (g && g->exec) {
     DIM_CHECK(cudaGraphLaunch(g->exec, st));
     g_launches += g->kernels;
@@ -499,14 +404,12 @@ static int refine_graphed(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_i
   }
   if (!g) {  // first sight of this argument set: eager run (also builds tensor maps, sets function attributes)
     if (ctx->graphs.size() >= 32) ctx->graphs.erase(ctx->graphs.begin());
-    ctx->graphs.push_back(dim_ctx::RefineGraph{key, nullptr, 0});
-    return refine_core(ctx, obs4, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override, poses, se3,
-                       zoom_factor, bbox, st, lit);
+    ctx->graphs.push_back(dim_ctx::RefineGraph{a, nullptr, 0});
+    return refine_core(ctx, a, st);
   }
   const long long before = g_launches;
   DIM_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-  const int rc = refine_core(ctx, obs4, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override, poses,
-                             se3, zoom_factor, bbox, st, lit);
+  const int rc = refine_core(ctx, a, st);
   cudaGraph_t graph = nullptr;
   const cudaError_t ce = cudaStreamEndCapture(st, &graph);
   if (rc != 0 || ce != cudaSuccess || graph == nullptr) {
@@ -528,6 +431,34 @@ static int refine_graphed(dim_ctx *ctx, const float4 *obs4, const int32_t *cls_i
   return 0;
 }
 
+// the loop's host values; the caller sets the pointers (lit: nullptr = unlit)
+static RefineArgs refine_args(int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
+                              int32_t precision, const dim_lighting *lit) {
+  RefineArgs a{};
+  a.B = B; a.n_iter = n_iter; a.precision = precision; a.zn = zn; a.zf = zf;
+  memcpy(a.K9, K9, sizeof(a.K9));
+  memcpy(a.means, means, sizeof(a.means));
+  if (lit) {
+    a.lit = 1;
+    a.intensity = lit->intensity;
+    memcpy(a.offset, lit->offset, sizeof(a.offset));
+    a.brightness_ratio = lit->brightness_ratio;
+  }
+  return a;
+}
+
+// dim_refine(_lit) after their argument checks
+static int refine_device(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
+                         int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
+                         int32_t precision, const double *pose_override, double *poses, float *se3, float *zoom_factor,
+                         int32_t *bbox, const dim_lighting *lit, cudaStream_t st) {
+  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lit);
+  a.obs4 = ctx->obs4; a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
+  a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
+  if (int rc = pack_obs4_launch(ctx, image_observed, B, ctx->obs4, means, st)) return rc;
+  return refine_graphed(ctx, a, st);
+}
+
 DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
                            int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
                            int32_t precision, const double *pose_override, double *poses, float *se3,
@@ -535,10 +466,8 @@ DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int3
   DIM_REQUIRE(ctx && image_observed && cls_idx && pose_init && K9 && means && poses, "dim_refine: NULL argument");
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine: batch exceeds max_batch");
   DIM_REQUIRE(n_iter >= 1, "dim_refine: n_iter must be >= 1");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (int rc = pack_obs4_launch(ctx, image_observed, B, ctx->obs4, means, st)) return rc;
-  return refine_graphed(ctx, ctx->obs4, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override, poses,
-                        se3, zoom_factor, bbox, st);
+  return refine_device(ctx, image_observed, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override,
+                       poses, se3, zoom_factor, bbox, nullptr, (cudaStream_t)stream);
 }
 
 DIM_API int32_t dim_refine_lit(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
@@ -549,10 +478,8 @@ DIM_API int32_t dim_refine_lit(dim_ctx *ctx, const float *image_observed, const 
   DIM_REQUIRE(image_observed && cls_idx && pose_init && K9 && means && poses, "dim_refine_lit: NULL argument");
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_lit: batch exceeds max_batch");
   DIM_REQUIRE(n_iter >= 1, "dim_refine_lit: n_iter must be >= 1");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (int rc = pack_obs4_launch(ctx, image_observed, B, ctx->obs4, means, st)) return rc;
-  return refine_graphed(ctx, ctx->obs4, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override, poses,
-                        se3, zoom_factor, bbox, st, lighting);
+  return refine_device(ctx, image_observed, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override,
+                       poses, se3, zoom_factor, bbox, lighting, (cudaStream_t)stream);
 }
 
 // dim_refine_host(_lit)_async; lit_host: the caller's lighting with HOST intensities [n_iter,B,3] (nullptr: unlit)
@@ -574,17 +501,16 @@ static int refine_host_impl(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *
   DIM_CHECK(cudaMemcpyAsync(ctx->image_observed_u8, img_u8, (size_t)B * 3 * P, cudaMemcpyHostToDevice, st));
   DIM_CHECK(cudaMemcpyAsync(ctx->cls_dev, cls_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
   DIM_CHECK(cudaMemcpyAsync(ctx->pose_cur, pose_host, sizeof(double) * B * 12, cudaMemcpyHostToDevice, st));
-  dim_lighting lit_dev;  // the caller's lighting with the intensities moved to the context's buffer (fixed address: graphs)
-  if (lit_host) {
-    lit_dev = *lit_host;
-    lit_dev.intensity = ctx->lit_intensity;
+  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lit_host);
+  a.obs4 = ctx->obs4; a.cls_idx = ctx->cls_dev; a.pose_init = ctx->pose_cur; a.poses = ctx->poses_dev;
+  a.se3 = ctx->se3_hist_dev;
+  if (lit_host) {  // the intensities move to the context's buffer (a fixed address: graphs)
+    a.intensity = ctx->lit_intensity;
     DIM_CHECK(cudaMemcpyAsync(ctx->lit_intensity, lit_host->intensity, sizeof(float) * (size_t)n_iter * B * 3,
                               cudaMemcpyHostToDevice, st));
   }
   if (int rc = transform_u8_obs4_launch(ctx, ctx->image_observed_u8, B, means, ctx->obs4, st)) return rc;
-  if (int rc = refine_graphed(ctx, ctx->obs4, ctx->cls_dev, ctx->pose_cur, B, n_iter, K9, zn, zf, means, precision,
-                              nullptr, ctx->poses_dev, ctx->se3_hist_dev, nullptr, nullptr, st, lit_host ? &lit_dev : nullptr))
-    return rc;
+  if (int rc = refine_graphed(ctx, a, st)) return rc;
   DIM_CHECK(cudaMemcpyAsync(poses_out, ctx->poses_dev, sizeof(double) * (size_t)n_iter * B * 12, cudaMemcpyDeviceToHost, st));
   if (se3_out)
     DIM_CHECK(cudaMemcpyAsync(se3_out, ctx->se3_hist_dev, sizeof(float) * (size_t)n_iter * B * 7, cudaMemcpyDeviceToHost, st));
@@ -748,7 +674,8 @@ DIM_API int32_t dim_debug_set_option(dim_ctx *ctx, const char *key, int32_t valu
   DIM_REQUIRE(ctx && key, "dim_debug_set_option: NULL argument");
   drop_graphs(ctx);  // captured graphs hold the old kernel choice
   if (!strcmp(key, "graph")) { ctx->use_graph = value != 0; return 0; }
-  return net_set_option(ctx, key, value);
+  set_error("dim_debug_set_option: unknown key '%s'", key);
+  return 2;
 }
 DIM_API int32_t dim_debug_layer_profile(dim_ctx *ctx, int32_t enable, float *ms10) {
   DIM_REQUIRE(ctx, "dim_debug_layer_profile: NULL ctx");

@@ -74,15 +74,25 @@ struct MeshDev {
   const float *normals; // [V,3] per-vertex normals (lit renderer only; nullptr otherwise)
 };
 
-// ------------------------------------------------------------------------------------ network
-struct ConvLayer {
-  int Cin, Cout, k, stride, pad;
-  int Hin, Win, Hout, Wout;
-  // padded NHWC input buffer geometry (see conv.cu)
-  int Hp, Wp, py, px;
-};
+struct NetState;  // net_state.cuh
 
-struct NetState;  // conv.cu
+// Everything the fused refinement loop reads from its caller, and the key of its CUDA graphs, compared byte for byte (so
+// no padding).  Not in the key, because drop_graphs discards every graph when they change: ctx->cfg (trans means / stds,
+// rot_coord), mesh uploads, network weights and the "graph" option.
+struct RefineArgs {
+  const float4 *obs4;
+  const int32_t *cls_idx;
+  const double *pose_init, *pose_override;  // pose_override: nullable [n_iter,B,3,4] source pose of every iteration
+  double *poses;
+  float *se3, *zoom_factor;  // nullable: the context's scratch
+  int32_t *bbox;             // nullable
+  const float *intensity;    // lit: device [n_iter,B,3]; unlit: nullptr
+  double means[3], offset[3];  // offset: the light's (lit only)
+  float K9[9], zn, zf, brightness_ratio;
+  int32_t B, n_iter, precision, lit;
+};
+static_assert(sizeof(RefineArgs) == 9 * sizeof(void *) + 6 * sizeof(double) + 12 * sizeof(float) + 4 * sizeof(int32_t),
+              "RefineArgs must have no padding: its bytes are the graph key");
 
 }  // namespace dim
 
@@ -97,16 +107,13 @@ struct dim_ctx {
   dim::PVert *pverts = nullptr;          // [max_batch, max_verts]
   unsigned long long *vis = nullptr;     // [max_batch, H*W]
   int *vbox = nullptr;                   // [max_batch,4] screen bbox of projected vertices
-  float *colour_lut = nullptr;           // [2][3][256]: trunc / no-trunc, RGB - mean
-  double lut_means[3] = {-1, -1, -1};
   // zoom scratch
   int *bbox8 = nullptr;      // [max_batch, 8]
-  int *status = nullptr;     // [max_batch]
   int *cls_flag = nullptr;   // [max_batch] rasteriser: 2 = class index out of range / mesh missing (raster.cu mesh_for)
   int *status_hist = nullptr;  // [8, max_batch] per-iteration status of the last fused refinement (dim_refine_status)
   float *zoom_factor = nullptr;  // [max_batch,4]
   // refine-loop state
-  float *image_rendered = nullptr, *depth_rendered = nullptr, *mask_rendered = nullptr;
+  float *mask_rendered = nullptr;  // [max_batch,H,W] scratch of dim_train_update (flow validity)
   int *bbox_ren = nullptr;   // [max_batch,4]
   double *pose_cur = nullptr;  // [max_batch,3,4]
   float *pose_cur_f32 = nullptr;
@@ -121,7 +128,7 @@ struct dim_ctx {
   dim::NetState *net = nullptr;
   // CUDA graphs of the fused refinement chain (capi.cu refine_graphed): one executable graph per distinct argument set
   struct RefineGraph {
-    std::vector<unsigned char> key;  // every launch argument of refine_core, byte for byte
+    dim::RefineArgs key;
     cudaGraphExec_t exec = nullptr;  // nullptr: seen once (eager warm-up run), captured on the next call
     long long kernels = 0;           // kernel nodes (dim_launch_count bookkeeping)
   };
@@ -134,3 +141,14 @@ struct dim_ctx {
   std::vector<cudaEvent_t> prof_events;  // 5 per recorded iteration
   size_t prof_used = 0;
 };
+
+// device allocation owned by the context (freed by dim_ctx_destroy)
+template <typename T>
+static int dev_alloc(dim_ctx *ctx, T **p, size_t n, bool zero = false) {
+  void *q = nullptr;
+  DIM_CHECK(cudaMalloc(&q, n * sizeof(T)));
+  if (zero) DIM_CHECK(cudaMemset(q, 0, n * sizeof(T)));
+  ctx->owned.push_back(q);
+  *p = reinterpret_cast<T *>(q);
+  return 0;
+}

@@ -6,7 +6,7 @@
 //   ZoomTrans fwd/bwd          deepim/operator_py/zoom_trans.py:22-74
 //   Transform3D fwd/bwd        deepim/operator_py/transform3d.py:34-281
 //   image transform            lib/utils/image.py:583-594
-#include "common.cuh"
+#include "launch.cuh"
 
 namespace dim {
 

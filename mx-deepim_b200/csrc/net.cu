@@ -11,6 +11,7 @@
 
 #include <mutex>
 
+#include "launch.cuh"
 #include "net_state.cuh"
 
 namespace dim {
@@ -572,14 +573,6 @@ int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, fl
 bool net_graph_safe(dim_ctx *ctx) {
   NetState *ns = ctx->net;
   return ns && ns->loaded && !ns->layer_events && !ns->train_aliased;
-}
-
-// run-time switches of the conv tower: there are none (every layer has one kernel); unknown keys are an error
-int net_set_option(dim_ctx *ctx, const char *key, int value) {
-  (void)value;
-  DIM_REQUIRE(ctx->net != nullptr, "net not created");
-  set_error("dim_debug_set_option: unknown key '%s'", key);
-  return 2;
 }
 
 // tuning hook: per-layer device times of the LAST net_forward (11 events: before conv1, after each of the 10 layers)

@@ -66,22 +66,9 @@ static constexpr int FC6_KC = 256;
 static constexpr int FC6_SPLITS = FC6_K / FC6_KC;  // 320
 
 
-// helpers implemented in net.cu
+// net.cu (only net.cu and train.cu build tensor maps)
 int encode_map(CUtensorMap *m, void *base, int rank, const uint64_t *dims, const uint64_t *strides_bytes,
                const uint32_t *box, int block_k /*64: SW128, 32: SW64, 0: no swizzle*/);
 static constexpr int kF16MapKey = 1 << 20;
-int train_refresh_lo(dim_ctx *ctx, cudaStream_t st);  // train.cu
-int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, float *rot_out, float *trans_out,
-                float *se3_out, cudaStream_t st, cudaEvent_t after_conv);
-
-template <typename T>
-static int dev_alloc(dim_ctx *ctx, T **p, size_t n, bool zero) {
-  void *q = nullptr;
-  DIM_CHECK(cudaMalloc(&q, n * sizeof(T)));
-  if (zero) DIM_CHECK(cudaMemset(q, 0, n * sizeof(T)));
-  ctx->owned.push_back(q);
-  *p = reinterpret_cast<T *>(q);
-  return 0;
-}
 
 }  // namespace dim

@@ -20,13 +20,11 @@
 // writes the mask plane (4 B/px) and touches the visibility buffer only inside the vertex box.  In the fused
 // refinement loop the only output is the pixel-interleaved (R,G,B,mask) image and it is written only inside the
 // projected-vertex box: the zoom kernel knows the box and substitutes the background constant outside it.
-#include "common.cuh"
+#include "launch.cuh"
 
 namespace dim {
 
 static constexpr unsigned long long VIS_EMPTY = ~0ull;
-
-struct LitParams { const float *light_pos, *light_int; float a0, a1; };
 
 struct RasterParams {
   const MeshDev *meshes;

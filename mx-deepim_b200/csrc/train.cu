@@ -21,17 +21,10 @@
 #include <algorithm>
 
 #include "conv_wgrad.cuh"
+#include "launch.cuh"
 #include "net_state.cuh"
 
 namespace dim {
-
-int pack_nhwc8_launch(dim_ctx *, const float *, const float *, const float *, const float *, int B, int Hs, int Ws,
-                      int pad, __nv_bfloat16 *, __nv_bfloat16 *, cudaStream_t, int f16);
-int transform3d_fwd_launch(const float *, const float *, const float *, const float *, int, int, const float *,
-                           const float *, int, float *, cudaStream_t);
-int transform3d_bwd_launch(const float *, const float *, const float *, const float *, const float *, int, int,
-                           const float *, const float *, int, float *, float *, cudaStream_t);
-int net_load(dim_ctx *, const float *const *, const float *const *);
 
 // ------------------------------------------------------------------------------------ parameters
 enum { PK_CONV = 0, PK_FC = 1, PK_DECONV = 2, PK_FROZEN = 3 };
@@ -726,8 +719,6 @@ static TrainState *&train_of(dim_ctx *ctx) {
   return table[ctx];
 }
 
-void train_destroy(dim_ctx *ctx);
-
 int train_create(dim_ctx *ctx, int max_points) {
   NetState *ns = ctx->net;
   DIM_REQUIRE(ns && ns->net_ok, "dim_train_create: needs a 480x640 context");
@@ -1264,18 +1255,6 @@ static int fork_side(TrainState *ts, cudaStream_t st) {
 }
 
 // ------------------------------------------------------------------------------------ the step
-struct TrainIO {
-  const float *zio, *zir, *zmo, *zmr, *zoom_factor, *zflow, *zfw, *zmask_gt, *src_pose, *pc_model, *pc_weights, *pc_observed;
-  int B, N;
-  float *rot_est_norm, *trans_est, *flow_est, *mask_prob, *losses, *grads;
-  float *rot_raw;  // nullable: the un-normalised quaternion of the test graph (se3 = [rot_raw, trans_est], symbol:716-725)
-  // gradient-bucket readiness (overlap of the NCCL all-reduce with the rest of the backward pass): event k is recorded as
-  // soon as every gradient of the tensors with table index >= bucket_first_tensor[k] has been produced
-  void *const *bucket_events;
-  const int *bucket_first_tensor;
-  int n_buckets;
-};
-
 static int record_buckets(const TrainIO &io, int lo_inclusive, int hi_exclusive, cudaStream_t s) {
   for (int k = 0; k < io.n_buckets; ++k)
     if (io.bucket_first_tensor[k] >= lo_inclusive && io.bucket_first_tensor[k] < hi_exclusive)

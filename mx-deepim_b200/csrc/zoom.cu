@@ -9,7 +9,7 @@
 // GridGenerator launch per sample; here everything stays on the device.
 #include <cuda_fp16.h>
 
-#include "common.cuh"
+#include "launch.cuh"
 
 namespace dim {
 

@@ -453,6 +453,8 @@ def test_refine_cuda_graph_replay_equals_eager(ctx, loop_case):
     img, cls, ini = dev(c["img"]), dev(c["cls"]), dev(c["ini"])
     check(lib.dim_debug_set_option(ctx._h, b"graph", 0))
     eager = ctx.refine(img, cls, ini, K, 4, pixel_means_rgb=MEANS)
+    eager_bf = ctx.refine(img, cls, ini, K, 4, pixel_means_rgb=MEANS, precision=capi.PREC_BF16X3)
+    assert not torch.equal(eager_bf["se3"], eager["se3"])
     ini2 = dev(c["ini"][[1, 0, 3, 2]])
     cls2 = dev(c["cls"][[1, 0, 3, 2]])
     img2 = dev(c["img"][[1, 0, 3, 2]])
@@ -461,12 +463,14 @@ def test_refine_cuda_graph_replay_equals_eager(ctx, loop_case):
     check(lib.dim_debug_set_option(ctx._h, b"graph", 1))
     side = torch.cuda.Stream(device=DEV)
     out = None
-    for it in range(4):            # eager warm-up, capture + launch, replay, replay
-        with torch.cuda.stream(side):
-            out = ctx.refine(img, cls, ini, K, 4, pixel_means_rgb=MEANS, out=out)
-        side.synchronize()
-        for k in ("poses", "se3", "zoom_factor", "bbox"):
-            assert torch.equal(out[k], eager[k]), (it, k)
+    for it in range(4):            # eager warm-up, capture + launch, replay, replay -- for each chain
+        # the same buffers with only a by-value argument (the precision) changed must get a graph of their own
+        for want, kw in ((eager, {}), (eager_bf, {"precision": capi.PREC_BF16X3})):
+            with torch.cuda.stream(side):
+                out = ctx.refine(img, cls, ini, K, 4, pixel_means_rgb=MEANS, out=out, **kw)
+            side.synchronize()
+            for k in ("poses", "se3", "zoom_factor", "bbox"):
+                assert torch.equal(out[k], want[k]), (it, k, kw)
     with torch.cuda.stream(side):  # same addresses, new contents: the replayed graph reads the buffers, not captured values
         img.copy_(img2); cls.copy_(cls2); ini.copy_(ini2)
         out = ctx.refine(img, cls, ini, K, 4, pixel_means_rgb=MEANS, out=out)
