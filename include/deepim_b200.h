@@ -308,6 +308,52 @@ DIM_API int32_t dim_train_update_lit(dim_ctx *ctx, const int32_t *cls_idx, const
                                      float *trans_label, float *flow, float *flow_weights,
                                      const dim_lighting *lighting, void *stream);
 
+/* RGB-D refinement (config.network.INPUT_DEPTH: deepIM_flownet.py:33-51, tester.py:437-438).  The network's input gains
+ * two channels, in the order image_observed/255, image_rendered/255, depth_observed/255, depth_rendered/255,
+ * mask_observed, mask_rendered: flow_conv1_weight is (64, 10, 7, 7), the depths (metres, divided by 255 as the reference
+ * does) are channels 6 and 7.  depth_rendered is each iteration's render depth (0 = background), zoomed with the
+ * iteration's zoom factor like every other input (ZoomDepth, zoom_depth.py:24-44).
+ *
+ * dim_ctx_set_input_depth: enable = 1 switches the context's network to the 10-channel input, 0 back to the 8-channel one.
+ *   Only before dim_net_load / dim_train_create (an error afterwards); a context that never calls it is unchanged.  On an
+ *   RGB-D context dim_net_load takes the (64,10,7,7) flow_conv1 weight and the training step is
+ *   dim_train_forward_backward_rgbd (below).
+ * The RGB network's entries (dim_refine(_lit), dim_refine_host(_lit)(_async), dim_net_fwd) refuse an RGB-D context and the
+ * _rgbd entries an RGB one, with a message naming the call to use.
+ * dim_refine_rgbd: dim_refine's arguments plus depth_observed, device f32 [B,1,H,W] in metres (constant over the
+ *   iterations), and lighting (NULL: unlit; else as dim_refine_lit).  Shares dim_refine_status; captured / replayed as a
+ *   CUDA graph like dim_refine, keyed on the depth pointer as well.
+ * dim_refine_host_rgbd(_async): dim_refine_host's arguments plus the host depth file values u16 [B,H,W], converted on the
+ *   device as lib/utils/image.py:203,218 does: float32(u16) / float32(depth_factor) (LINEMOD: 1000); lighting as above
+ *   with a HOST intensity.
+ * dim_net_fwd_rgbd: dim_net_fwd on already-zoomed blobs plus the zoomed depths f32 [B,1,H,W]. */
+DIM_API int32_t dim_ctx_set_input_depth(dim_ctx *ctx, int32_t enable);
+DIM_API int32_t dim_refine_rgbd(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx,
+                                const double *pose_init, int32_t B, int32_t n_iter, const float *K9_host,
+                                float znear, float zfar, const double *pixel_means_rgb_host,
+                                int32_t precision, const double *pose_override, double *poses,
+                                float *se3, float *zoom_factor, int32_t *bbox, const float *depth_observed,
+                                const dim_lighting *lighting, void *stream);
+DIM_API int32_t dim_refine_host_rgbd(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
+                                     const int32_t *cls_idx_host, const double *pose_init_host,
+                                     int32_t B, int32_t n_iter, const float *K9_host, float znear,
+                                     float zfar, const double *pixel_means_rgb_host, int32_t precision,
+                                     double *poses_out_host, float *se3_out_host,
+                                     const uint16_t *depth_observed_u16_host, float depth_factor,
+                                     const dim_lighting *lighting, void *stream);
+DIM_API int32_t dim_refine_host_rgbd_async(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
+                                           const int32_t *cls_idx_host, const double *pose_init_host,
+                                           int32_t B, int32_t n_iter, const float *K9_host, float znear,
+                                           float zfar, const double *pixel_means_rgb_host, int32_t precision,
+                                           double *poses_out_host, float *se3_out_host,
+                                           const uint16_t *depth_observed_u16_host, float depth_factor,
+                                           const dim_lighting *lighting, void *stream);
+DIM_API int32_t dim_net_fwd_rgbd(dim_ctx *ctx, const float *zoom_image_observed,
+                                 const float *zoom_image_rendered, const float *zoom_depth_observed,
+                                 const float *zoom_depth_rendered, const float *zoom_mask_observed,
+                                 const float *zoom_mask_rendered, int32_t B, int32_t precision,
+                                 float *rot, float *trans, void *stream);
+
 /* BGR u8 HWC -> RGB-mean f32 CHW on device (lib/utils/image.py:583-594 transform). */
 DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int32_t B,
                                        const double *pixel_means_rgb_host, float *image,
@@ -401,6 +447,23 @@ DIM_API int32_t dim_train_forward_backward(
     float *flow_est, float *mask_prob, float *losses4, float *grads, float *rot_raw,
     void *const *bucket_events,
     const int32_t *bucket_first_tensor, int32_t n_buckets, void *stream);
+/* The training step of the RGB-D network (a context switched by dim_ctx_set_input_depth before dim_train_create):
+ * dim_train_forward_backward's arguments plus the zoomed depth_observed and depth_rendered f32 (B,1,H,W), metres (the
+ * train-time update's depth_rendered, zoomed with the pair's zoom factor; deepIM_flownet.py:33-51, batch_updater l.269).
+ * conv1 has no data gradient, so only flow_conv1_weight's gradient widens.  The flat parameter vector of such a context is
+ * the RGB-D table: dim_train_param_info_rgbd (flow_conv1 (64,10,7,7): 6 272 floats more; every other entry as
+ * dim_train_param_info); dim_train_param_count reports its size.  Each network's entry refuses the other's context. */
+DIM_API int32_t dim_train_param_info_rgbd(int32_t idx, const char **name, int64_t *weight_numel,
+                                          int64_t *bias_numel);
+DIM_API int32_t dim_train_forward_backward_rgbd(
+    dim_ctx *ctx, const float *zoom_image_observed, const float *zoom_image_rendered,
+    const float *zoom_mask_observed, const float *zoom_mask_rendered, const float *zoom_factor,
+    const float *zoom_flow, const float *zoom_flow_weights, const float *zoom_mask_gt_observed,
+    const float *src_pose, const float *point_cloud_model, const float *point_cloud_weights,
+    const float *point_cloud_observed, int32_t B, int32_t N, float *rot_est_norm, float *trans_est,
+    float *flow_est, float *mask_prob, float *losses4, float *grads, float *rot_raw,
+    void *const *bucket_events, const int32_t *bucket_first_tensor, int32_t n_buckets,
+    const float *zoom_depth_observed, const float *zoom_depth_rendered, void *stream);
 /* Loss weights / normalisers of the training step and the pose parameterisation shared with the refinement loop: the
  * values the reference reads from its yaml (experiments/deepim/cfgs/...: train.LW_FLOW / LW_MASK / LW_PM, NUM_3D_SAMPLE,
  * NORMALIZE_3D_POINT, NORMALIZE_FLOW, network.TRANS_MEANS / TRANS_STDS, ROT_COORD).  Defaults = the shipped LM6d config

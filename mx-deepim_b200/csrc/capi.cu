@@ -171,6 +171,18 @@ static LitParams lit_params(const float *light_pos, const float *intensity, floa
   return LitParams{light_pos, intensity, (float)(1.0 - (double)ratio), ratio};
 }
 
+// the RGB network's entries refuse an RGB-D context and the _rgbd entries an RGB one: never run conv1 on the wrong channels
+static int input_mode_check(dim_ctx *ctx, bool rgbd_entry, const char *fn, const char *use) {
+  if (!ctx) { set_error("%s: NULL context", fn); return 2; }
+  if (net_input_depth(ctx) == rgbd_entry) return 0;
+  if (rgbd_entry)
+    set_error("%s: this context's network takes no depth input; call %s, or switch the context with "
+              "dim_ctx_set_input_depth before loading weights", fn, use);
+  else
+    set_error("%s: this context's network takes depth input (dim_ctx_set_input_depth); call %s", fn, use);
+  return 2;
+}
+
 DIM_API int32_t dim_render_lit(dim_ctx *ctx, const int32_t *cls_idx, const float *pose, int32_t B, const float *K9, float zn,
                                float zf, const double *means, const float *light_pos, const float *light_int,
                                float brightness_ratio, float *out_image, float *out_depth, float *out_mask, float *out_bgr,
@@ -293,6 +305,16 @@ DIM_API int32_t dim_transform3d_bwd(dim_ctx *ctx, const float *og, const float *
   return transform3d_bwd_launch(og, pc, rot, tr, ps, B, N, Tm, Ts, rot_coord, rg, tg, (cudaStream_t)stream);
 }
 
+DIM_API int32_t dim_ctx_set_input_depth(dim_ctx *ctx, int32_t enable) {
+  DIM_REQUIRE(ctx != nullptr, "dim_ctx_set_input_depth: NULL context");
+  if (net_input_depth(ctx) == (enable != 0)) return 0;
+  DIM_REQUIRE(train_param_count(ctx) == 0, "dim_ctx_set_input_depth: call it before dim_train_create (this context trains)");
+  drop_graphs(ctx);
+  if (enable && !ctx->depth_u16)
+    if (dev_alloc(ctx, &ctx->depth_u16, (size_t)ctx->max_batch * ctx->H * ctx->W)) return 12;
+  return net_set_input_depth(ctx, enable != 0);
+}
+
 DIM_API int32_t dim_net_load(dim_ctx *ctx, const float *const *W, const float *const *Bv) {
   DIM_REQUIRE(ctx && W && Bv, "dim_net_load: NULL argument");
   drop_graphs(ctx);
@@ -302,12 +324,28 @@ DIM_API int32_t dim_net_load(dim_ctx *ctx, const float *const *W, const float *c
 DIM_API int32_t dim_net_fwd(dim_ctx *ctx, const float *zio, const float *zir, const float *zmo, const float *zmr,
                             int32_t B, int32_t precision, float *rot, float *trans, void *stream) {
   DIM_REQUIRE(ctx && zio && zir && zmo && zmr && rot && trans, "dim_net_fwd: NULL argument");
+  if (int rc = input_mode_check(ctx, false, "dim_net_fwd", "dim_net_fwd_rgbd")) return rc;
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_net_fwd: batch exceeds max_batch");
   cudaStream_t st = (cudaStream_t)stream;
   int rows, cols, pad; __nv_bfloat16 *hi, *lo;
   net_input_geometry(ctx, &rows, &cols, &pad, &hi, &lo);
   if (int rc = pack_nhwc8_launch(ctx, zio, zir, zmo, zmr, B, rows, cols, pad, hi,
                                  precision == DIM_PREC_BF16X3 ? lo : nullptr, st, precision == DIM_PREC_FP16))
+    return rc;
+  return net_forward(ctx, B, precision, nullptr, rot, trans, nullptr, st, nullptr);
+}
+
+DIM_API int32_t dim_net_fwd_rgbd(dim_ctx *ctx, const float *zio, const float *zir, const float *zdo, const float *zdr,
+                                 const float *zmo, const float *zmr, int32_t B, int32_t precision, float *rot, float *trans,
+                                 void *stream) {
+  DIM_REQUIRE(ctx && zio && zir && zdo && zdr && zmo && zmr && rot && trans, "dim_net_fwd_rgbd: NULL argument");
+  if (int rc = input_mode_check(ctx, true, "dim_net_fwd_rgbd", "dim_net_fwd")) return rc;
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_net_fwd_rgbd: batch exceeds max_batch");
+  cudaStream_t st = (cudaStream_t)stream;
+  int rows, cols, pad; __nv_bfloat16 *hi, *lo;
+  net_input_geometry(ctx, &rows, &cols, &pad, &hi, &lo);
+  if (int rc = pack_nhwc10_launch(ctx, zio, zir, zdo, zdr, zmo, zmr, B, rows, cols, pad, hi,
+                                  precision == DIM_PREC_BF16X3 ? lo : nullptr, st, precision == DIM_PREC_FP16))
     return rc;
   return net_forward(ctx, B, precision, nullptr, rot, trans, nullptr, st, nullptr);
 }
@@ -324,6 +362,7 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
   const float means_f[3] = {(float)a.means[0], (float)a.means[1], (float)a.means[2]};
   int rows, cols, pad; __nv_bfloat16 *hi, *lo;
   net_input_geometry(ctx, &rows, &cols, &pad, &hi, &lo);
+  const bool depth = net_input_depth(ctx);  // RGB-D network: ren4.w = depth, obs4.w = depth_observed
   const double *pose_src = a.pose_init;
   for (int it = 0; it < a.n_iter; ++it) {
     DimNvtxRange r_it("dim_refine iteration");
@@ -353,7 +392,7 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
       const LitParams lp = a.lit ? lit_params(ctx->light_pos, a.intensity + (size_t)it * a.B * 3, a.brightness_ratio)
                                  : LitParams{nullptr, nullptr, 0.f, 0.f};
       if (int rc = render_launch(ctx, a.cls_idx, ctx->pose_cur_f32, a.B, a.K9, a.zn, a.zf, a.means, 1, nullptr, nullptr,
-                                 nullptr, nullptr, nullptr, ctx->ren4, st, a.lit ? &lp : nullptr))
+                                 nullptr, nullptr, nullptr, ctx->ren4, st, a.lit ? &lp : nullptr, depth))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[1], st));
@@ -366,7 +405,8 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
                                                ctx->status_hist + (size_t)(it < 8 ? it : 7) * a.B, st))
         return rc;
       if (int rc = zoom_fused_launch(ctx, a.obs4, ctx->ren4, zf_it, means_f, a.B, rows, cols, pad, hi,
-                                     a.precision == DIM_PREC_BF16X3 ? lo : nullptr, st, a.precision == DIM_PREC_FP16, a.means))
+                                     a.precision == DIM_PREC_BF16X3 ? lo : nullptr, st, a.precision == DIM_PREC_FP16, a.means,
+                                     depth))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[2], st));
@@ -451,11 +491,16 @@ static RefineArgs refine_args(int32_t B, int32_t n_iter, const float *K9, float 
 static int refine_device(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
                          int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
                          int32_t precision, const double *pose_override, double *poses, float *se3, float *zoom_factor,
-                         int32_t *bbox, const dim_lighting *lit, cudaStream_t st) {
+                         int32_t *bbox, const dim_lighting *lit, cudaStream_t st, const float *depth_observed = nullptr) {
   RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lit);
   a.obs4 = ctx->obs4; a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
   a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
+  // the graph never reads depth_observed: it is packed into obs4.w below, outside the graph, like the image, so a replay is
+  // correct whatever the key holds; keying on it only costs one capture per distinct depth buffer
+  a.depth_observed = depth_observed;
   if (int rc = pack_obs4_launch(ctx, image_observed, B, ctx->obs4, means, st)) return rc;
+  if (depth_observed)
+    if (int rc = obs4_depth_launch(ctx, ctx->obs4, B, depth_observed, nullptr, 0.f, st)) return rc;
   return refine_graphed(ctx, a, st);
 }
 
@@ -464,6 +509,7 @@ DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int3
                            int32_t precision, const double *pose_override, double *poses, float *se3,
                            float *zoom_factor, int32_t *bbox, void *stream) {
   DIM_REQUIRE(ctx && image_observed && cls_idx && pose_init && K9 && means && poses, "dim_refine: NULL argument");
+  if (int rc = input_mode_check(ctx, false, "dim_refine", "dim_refine_rgbd")) return rc;
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine: batch exceeds max_batch");
   DIM_REQUIRE(n_iter >= 1, "dim_refine: n_iter must be >= 1");
   return refine_device(ctx, image_observed, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override,
@@ -475,6 +521,7 @@ DIM_API int32_t dim_refine_lit(dim_ctx *ctx, const float *image_observed, const 
                                int32_t precision, const double *pose_override, double *poses, float *se3,
                                float *zoom_factor, int32_t *bbox, const dim_lighting *lighting, void *stream) {
   if (int rc = lit_check(ctx, lighting, "dim_refine_lit")) return rc;
+  if (int rc = input_mode_check(ctx, false, "dim_refine_lit", "dim_refine_rgbd")) return rc;
   DIM_REQUIRE(image_observed && cls_idx && pose_init && K9 && means && poses, "dim_refine_lit: NULL argument");
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_lit: batch exceeds max_batch");
   DIM_REQUIRE(n_iter >= 1, "dim_refine_lit: n_iter must be >= 1");
@@ -482,10 +529,27 @@ DIM_API int32_t dim_refine_lit(dim_ctx *ctx, const float *image_observed, const 
                        poses, se3, zoom_factor, bbox, lighting, (cudaStream_t)stream);
 }
 
-// dim_refine_host(_lit)_async; lit_host: the caller's lighting with HOST intensities [n_iter,B,3] (nullptr: unlit)
+DIM_API int32_t dim_refine_rgbd(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
+                                int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
+                                int32_t precision, const double *pose_override, double *poses, float *se3, float *zoom_factor,
+                                int32_t *bbox, const float *depth_observed, const dim_lighting *lighting, void *stream) {
+  if (int rc = input_mode_check(ctx, true, "dim_refine_rgbd", "dim_refine / dim_refine_lit")) return rc;
+  if (lighting)
+    if (int rc = lit_check(ctx, lighting, "dim_refine_rgbd")) return rc;
+  DIM_REQUIRE(image_observed && depth_observed && cls_idx && pose_init && K9 && means && poses,
+              "dim_refine_rgbd: NULL argument (image_observed, depth_observed, cls_idx, pose_init, K9, means, poses)");
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_rgbd: batch exceeds max_batch");
+  DIM_REQUIRE(n_iter >= 1, "dim_refine_rgbd: n_iter must be >= 1");
+  return refine_device(ctx, image_observed, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override,
+                       poses, se3, zoom_factor, bbox, lighting, (cudaStream_t)stream, depth_observed);
+}
+
+// dim_refine_host(_lit)(_rgbd)_async; lit_host: the caller's lighting with HOST intensities [n_iter,B,3] (nullptr: unlit);
+// depth_u16: RGB-D network, the caller's host depth file values [B,H,W] (nullptr: RGB network)
 static int refine_host_impl(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host, int32_t B,
                             int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
-                            double *poses_out, float *se3_out, const dim_lighting *lit_host, cudaStream_t st) {
+                            double *poses_out, float *se3_out, const dim_lighting *lit_host, cudaStream_t st,
+                            const uint16_t *depth_u16 = nullptr, float depth_factor = 0.f) {
   DIM_REQUIRE(ctx && img_u8 && cls_host && pose_host && K9 && means && poses_out, "dim_refine_host: NULL argument");
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_host: batch exceeds max_batch");
   DIM_REQUIRE(n_iter >= 1 && n_iter <= 8, "dim_refine_host: n_iter must be in [1,8]");
@@ -510,6 +574,10 @@ static int refine_host_impl(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *
                               cudaMemcpyHostToDevice, st));
   }
   if (int rc = transform_u8_obs4_launch(ctx, ctx->image_observed_u8, B, means, ctx->obs4, st)) return rc;
+  if (depth_u16) {  // the converted depth lands in obs4 outside the graph, like the image
+    DIM_CHECK(cudaMemcpyAsync(ctx->depth_u16, depth_u16, sizeof(uint16_t) * B * P, cudaMemcpyHostToDevice, st));
+    if (int rc = obs4_depth_launch(ctx, ctx->obs4, B, nullptr, ctx->depth_u16, depth_factor, st)) return rc;
+  }
   if (int rc = refine_graphed(ctx, a, st)) return rc;
   DIM_CHECK(cudaMemcpyAsync(poses_out, ctx->poses_dev, sizeof(double) * (size_t)n_iter * B * 12, cudaMemcpyDeviceToHost, st));
   if (se3_out)
@@ -521,6 +589,7 @@ DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *img_u8, const
                                       const double *pose_host, int32_t B, int32_t n_iter, const float *K9, float zn,
                                       float zf, const double *means, int32_t precision, double *poses_out,
                                       float *se3_out, void *stream) {
+  if (int rc = input_mode_check(ctx, false, "dim_refine_host", "dim_refine_host_rgbd")) return rc;
   return refine_host_impl(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out, se3_out,
                           nullptr, (cudaStream_t)stream);
 }
@@ -530,6 +599,7 @@ DIM_API int32_t dim_refine_host_lit_async(dim_ctx *ctx, const uint8_t *img_u8, c
                                           float zf, const double *means, int32_t precision, double *poses_out,
                                           float *se3_out, const dim_lighting *lighting, void *stream) {
   if (int rc = lit_check(ctx, lighting, "dim_refine_host_lit")) return rc;
+  if (int rc = input_mode_check(ctx, false, "dim_refine_host_lit", "dim_refine_host_rgbd")) return rc;
   return refine_host_impl(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out, se3_out,
                           lighting, (cudaStream_t)stream);
 }
@@ -540,6 +610,31 @@ DIM_API int32_t dim_refine_host_lit(dim_ctx *ctx, const uint8_t *img_u8, const i
                                     void *stream) {
   if (int rc = dim_refine_host_lit_async(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision,
                                          poses_out, se3_out, lighting, stream))
+    return rc;
+  DIM_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
+  return 0;
+}
+
+DIM_API int32_t dim_refine_host_rgbd_async(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host,
+                                           const double *pose_host, int32_t B, int32_t n_iter, const float *K9, float zn,
+                                           float zf, const double *means, int32_t precision, double *poses_out,
+                                           float *se3_out, const uint16_t *depth_u16, float depth_factor,
+                                           const dim_lighting *lighting, void *stream) {
+  if (int rc = input_mode_check(ctx, true, "dim_refine_host_rgbd", "dim_refine_host / dim_refine_host_lit")) return rc;
+  if (lighting)
+    if (int rc = lit_check(ctx, lighting, "dim_refine_host_rgbd")) return rc;
+  DIM_REQUIRE(depth_u16 != nullptr, "dim_refine_host_rgbd: NULL depth");
+  DIM_REQUIRE(depth_factor > 0.f && depth_factor < 3.0e38f, "dim_refine_host_rgbd: depth_factor must be positive and finite");
+  return refine_host_impl(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out, se3_out,
+                          lighting, (cudaStream_t)stream, depth_u16, depth_factor);
+}
+
+DIM_API int32_t dim_refine_host_rgbd(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host,
+                                     int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
+                                     int32_t precision, double *poses_out, float *se3_out, const uint16_t *depth_u16,
+                                     float depth_factor, const dim_lighting *lighting, void *stream) {
+  if (int rc = dim_refine_host_rgbd_async(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision,
+                                          poses_out, se3_out, depth_u16, depth_factor, lighting, stream))
     return rc;
   DIM_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
   return 0;
@@ -716,6 +811,13 @@ DIM_API int32_t dim_train_param_info(int32_t idx, const char **name, int64_t *w_
   *w_numel = w; *b_numel = b;
   return 0;
 }
+DIM_API int32_t dim_train_param_info_rgbd(int32_t idx, const char **name, int64_t *w_numel, int64_t *b_numel) {
+  long long w = 0, b = 0;
+  DIM_REQUIRE(name && w_numel && b_numel, "dim_train_param_info_rgbd: NULL argument");
+  if (train_param_info(idx, name, &w, &b, true)) return 2;
+  *w_numel = w; *b_numel = b;
+  return 0;
+}
 DIM_API int32_t dim_train_load_params(dim_ctx *ctx, const float *flat_host, int64_t n, void *stream) {
   DIM_REQUIRE(ctx && flat_host && n > 0, "dim_train_load_params: bad argument");
   return train_load_params(ctx, flat_host, (size_t)n, (cudaStream_t)stream);
@@ -732,9 +834,24 @@ DIM_API int32_t dim_train_forward_backward(dim_ctx *ctx, const float *zio, const
                                            void *const *bucket_events, const int32_t *bucket_first_tensor, int32_t n_buckets,
                                            void *stream) {
   DIM_REQUIRE(ctx && zio && zir && zmo && zmr && zoom_factor, "dim_train_forward_backward: NULL argument");
+  if (int rc = input_mode_check(ctx, false, "dim_train_forward_backward", "dim_train_forward_backward_rgbd")) return rc;
   TrainIO io{zio, zir, zmo, zmr, zoom_factor, zflow, zfw, zmask_gt, src_pose, pc_model, pc_weights, pc_observed, B, N,
              rot_est_norm, trans_est, flow_est, mask_prob, losses4, grads, rot_raw, bucket_events, bucket_first_tensor,
              (bucket_events && bucket_first_tensor) ? n_buckets : 0};
+  return train_forward_backward(ctx, io, (cudaStream_t)stream);
+}
+DIM_API int32_t dim_train_forward_backward_rgbd(
+    dim_ctx *ctx, const float *zio, const float *zir, const float *zmo, const float *zmr, const float *zoom_factor, const float *zflow,
+    const float *zfw, const float *zmask_gt, const float *src_pose, const float *pc_model, const float *pc_weights,
+    const float *pc_observed, int32_t B, int32_t N, float *rot_est_norm, float *trans_est, float *flow_est, float *mask_prob,
+    float *losses4, float *grads, float *rot_raw, void *const *bucket_events, const int32_t *bucket_first_tensor, int32_t n_buckets,
+    const float *zoom_depth_observed, const float *zoom_depth_rendered, void *stream) {
+  DIM_REQUIRE(ctx && zio && zir && zmo && zmr && zoom_factor && zoom_depth_observed && zoom_depth_rendered,
+              "dim_train_forward_backward_rgbd: NULL argument");
+  if (int rc = input_mode_check(ctx, true, "dim_train_forward_backward_rgbd", "dim_train_forward_backward")) return rc;
+  TrainIO io{zio, zir, zmo, zmr, zoom_factor, zflow, zfw, zmask_gt, src_pose, pc_model, pc_weights, pc_observed, B, N,
+             rot_est_norm, trans_est, flow_est, mask_prob, losses4, grads, rot_raw, bucket_events, bucket_first_tensor,
+             (bucket_events && bucket_first_tensor) ? n_buckets : 0, zoom_depth_observed, zoom_depth_rendered};
   return train_forward_backward(ctx, io, (cudaStream_t)stream);
 }
 DIM_API int32_t dim_train_set_config(dim_ctx *ctx, const dim_train_config *cfg) {

@@ -87,11 +87,12 @@ struct RefineArgs {
   float *se3, *zoom_factor;  // nullable: the context's scratch
   int32_t *bbox;             // nullable
   const float *intensity;    // lit: device [n_iter,B,3]; unlit: nullptr
+  const float *depth_observed;  // RGB-D network, dim_refine_rgbd: the caller's device depth; otherwise nullptr
   double means[3], offset[3];  // offset: the light's (lit only)
   float K9[9], zn, zf, brightness_ratio;
   int32_t B, n_iter, precision, lit;
 };
-static_assert(sizeof(RefineArgs) == 9 * sizeof(void *) + 6 * sizeof(double) + 12 * sizeof(float) + 4 * sizeof(int32_t),
+static_assert(sizeof(RefineArgs) == 10 * sizeof(void *) + 6 * sizeof(double) + 12 * sizeof(float) + 4 * sizeof(int32_t),
               "RefineArgs must have no padding: its bytes are the graph key");
 
 }  // namespace dim
@@ -125,6 +126,7 @@ struct dim_ctx {
   float *se3_hist_dev = nullptr;
   float *light_pos = nullptr;      // [max_batch,3] lit chain / lit train update: light of the pose being rendered
   float *lit_intensity = nullptr;  // [8, max_batch, 3] dim_refine_host_lit: the caller's light intensities on the device
+  uint16_t *depth_u16 = nullptr;   // [max_batch,H,W] dim_refine_host_rgbd: the caller's depth file values (RGB-D contexts)
   dim::NetState *net = nullptr;
   // CUDA graphs of the fused refinement chain (capi.cu refine_graphed): one executable graph per distinct argument set
   struct RefineGraph {

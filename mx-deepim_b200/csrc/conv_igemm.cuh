@@ -547,4 +547,157 @@ __global__ void __launch_bounds__(384, 1) conv1_kernel(const __grid_constant__ C
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// conv1 of the RGB-D network (flow_conv1: 10 -> 64, 7x7 s2; deepIM_flownet.py:33-51 with INPUT_DEPTH).  Same rolling-strip
+// schedule as conv1_kernel; the space-to-depth input has 16-channel chunks: each of the four 2x2 phases (ph, pw) is a pair
+// of 8-channel chunk planes, channels 0-7 then 8-9 (+ 6 zero channels), so a strip is 8 chunk planes
+//     addr(pixel r, plane c) = base + c*LBO + 16*r,  plane c = (ph*2 + pw)*2 + half
+// and K step k (16 channels) of tap (dh, dw) is exactly phase k = ph*2 + pw: planes 2k, 2k + 1.  Phases with kh = 7
+// (dh = 3, ph = 1) or kw = 7 (dw = 3, pw = 1) lie outside the 7 x 7 filter and are not issued (49 of the 64 K steps run).
+// Input buffer: [B*Hs rows][8 planes][Ws cols][8 ch] bf16 / fp16.  Weights: [64][16 taps][4 phases][16 ch] = K 1024,
+// resident in shared memory as 16 SW128 tap tiles of NB x 64, loaded in boxes of 16 output channels.
+// NB = output channels per CTA.  The 64 x 1024 16-bit weight matrix (128 KB) fits beside a 6-deep strip ring; bf16x3's hi +
+// lo pair (256 KB) does not, so that mode runs NB = 16 (64 KB of weights) with four CTAs per (column tile, row run), each
+// re-reading the strips from L2: the parity mode is correct rather than fast.
+template <int STAGES, bool SPLIT3, bool F16, int NB>
+__global__ void __launch_bounds__(384, 1) conv1_rgbd_kernel(const __grid_constant__ ConvKParams p, const int rows_total,
+                                                            const int rows_per_chunk, const int chunks_per_col,
+                                                            const int strip_bytes /*per precision, multiple of 128*/) {
+  constexpr int NPREC = SPLIT3 ? 2 : 1;
+  constexpr int TAP_BYTES = NB * 128, RES_BYTES = 16 * TAP_BYTES * NPREC;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t *res = smem;
+  uint8_t *ring = smem + RES_BYTES;
+  const int stage_bytes = strip_bytes * NPREC;
+  uint64_t *full_bar = reinterpret_cast<uint64_t *>(ring + STAGES * stage_bytes + kConv1Slack);
+  uint64_t *empty_bar = full_bar + STAGES;
+  uint64_t *res_bar = empty_bar + STAGES;
+
+  const int wgi = threadIdx.x >> 7, warp = threadIdx.x >> 5;
+  const int R = p.BW + 3;
+  const uint32_t LBO = (uint32_t)R * 16u;
+  const int per_split = p.n_col_tiles * chunks_per_col;
+  const int nsplit = blockIdx.x / per_split, cidx = blockIdx.x - nsplit * per_split;
+  const int ct = cidx / chunks_per_col, ck = cidx - ct * chunks_per_col;
+  const int n0 = nsplit * NB;
+  const int g_lo = ck * rows_per_chunk;
+  const int g_hi = min(rows_total, g_lo + rows_per_chunk);
+  const int n_rows = max(0, g_hi - g_lo);
+  const int n_strips = n_rows > 0 ? n_rows + 3 : 0;
+  const int ow0 = ct * p.BW;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      ptx::mbar_init(&full_bar[s], 1);
+      ptx::mbar_init(&empty_bar[s], 2);
+    }
+    ptx::mbar_init(res_bar, 1);
+    ptx::fence_barrier_init();
+    ptx::prefetch_tmap(&p.b_map);
+    ptx::prefetch_tmap(&p.a_map[0]);
+  }
+  __syncthreads();
+
+  if (wgi == 0) {
+    ptx::regs_producer();
+    if (warp == 0 && n_rows > 0) {
+      if (ptx::elect_one()) {
+        ptx::mbar_expect_tx_raw(res_bar, (uint32_t)RES_BYTES);
+        for (int kb = 0; kb < 16; ++kb)
+          for (int r = 0; r < NB / 16; ++r) {
+            ptx::tma_load_2d_raw(res + kb * TAP_BYTES + r * 2048, &p.b_map, res_bar, kb * 64, n0 + r * 16);
+            if (SPLIT3) ptx::tma_load_2d_raw(res + (16 + kb) * TAP_BYTES + r * 2048, &p.b_lo_map, res_bar, kb * 64, n0 + r * 16);
+          }
+      }
+      __syncwarp();
+      const uint32_t tx = (uint32_t)(R * 128) * NPREC;
+      for (int s = 0; s < n_strips; ++s) {
+        const int slot = s % STAGES;
+        ptx::mbar_wait(&empty_bar[slot], (((uint32_t)(s / STAGES)) & 1u) ^ 1u);
+        uint8_t *st = ring + slot * stage_bytes;
+        ptx::mbar_expect_tx(&full_bar[slot], tx);
+        ptx::tma_load_4d(st, &p.a_map[0], &full_bar[slot], 0, ow0, 0, g_lo + s);
+        if (SPLIT3) ptx::tma_load_4d(st + strip_bytes, &p.a_lo_map[0], &full_bar[slot], 0, ow0, 0, g_lo + s);
+      }
+    }
+  } else if (n_rows > 0) {
+    ptx::regs_consumer();
+    const int set = wgi - 1, t = threadIdx.x & 127;
+    const bool arriver = t == 0;
+    const int r0 = frag_row(t), q2 = (t & 3) * 2;
+    float2 bias[NB / 8];
+#pragma unroll
+    for (int j = 0; j < NB / 8; ++j)
+      bias[j] = make_float2(__ldg(p.bias + n0 + 8 * j + q2), __ldg(p.bias + n0 + 8 * j + q2 + 1));
+    const uint32_t ring_a = ptx::smem_u32(ring);
+    const uint64_t dring = ptx::gmma_desc(ring_a, LBO, 128, ptx::kNoSwizzle);
+    const uint64_t lo_step = (uint64_t)((uint32_t)strip_bytes >> 4);
+    const uint64_t slot_step = (uint64_t)((uint32_t)stage_bytes >> 4);
+    const uint64_t phase_step = (uint64_t)(2u * LBO >> 4);  // two chunk planes
+    const uint64_t dres = ptx::gmma_desc(ptx::smem_u32(res), 16, 1024, ptx::kSW128);
+    const uint64_t dres_lo = dres + (uint64_t)((16 * TAP_BYTES) >> 4);
+    const int n_cols_valid = min(p.BW, p.Wo - ow0);
+    ptx::mbar_wait(res_bar, 0);
+    if (set == 1 && arriver) ptx::mbar_arrive(&empty_bar[0]);
+    for (int row = set; row < n_rows; row += 2) {
+      float acc[2][NB / 2];
+#pragma unroll
+      for (int dh = 0; dh < 4; ++dh) {
+        const int s = row + dh;
+        ptx::mbar_wait(&full_bar[s % STAGES], ((uint32_t)(s / STAGES)) & 1u);
+      }
+      wg::fence_acc(acc[0]);
+      wg::fence_acc(acc[1]);
+      wg::fence();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int dh = 0; dh < 4; ++dh) {
+          const uint64_t so = (uint64_t)((row + dh) % STAGES) * slot_step + (uint64_t)(h * 64);  // + 64 pixels of 16 B
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+#pragma unroll
+            for (int dw = 0; dw < 4; ++dw) {
+              if ((dh == 3 && (k >> 1)) || (dw == 3 && (k & 1))) continue;  // kh = 7 / kw = 7: outside the 7x7 filter
+              const uint64_t da = dring + (uint64_t)k * phase_step + (uint64_t)dw + so;
+              const uint64_t wo = (uint64_t)((dh * 4 + dw) * (TAP_BYTES >> 4) + 2 * k);
+              wg::mma<NB, F16, 0, 0>(acc[h], da, dres + wo, (dh | dw | k) ? 1u : 0u);
+              if (SPLIT3) {
+                wg::mma<NB, false, 0, 0>(acc[h], da + lo_step, dres + wo, 1u);
+                wg::mma<NB, false, 0, 0>(acc[h], da, dres_lo + wo, 1u);
+              }
+            }
+          }
+        }
+      }
+      wg::commit();
+      wg::wait<0>();
+      wg::fence_acc(acc[0]);
+      wg::fence_acc(acc[1]);
+      if (arriver) {
+        ptx::mbar_arrive(&empty_bar[row % STAGES]);
+        ptx::mbar_arrive(&empty_bar[(row + 1) % STAGES]);
+      }
+      const int g = g_lo + row;
+      const int n_img = g / p.Hq, oh = g - n_img * p.Hq;
+      if (n_img < p.Bn && oh < p.Ho) {
+        const long long row_off = (((long long)n_img * p.out_Hp + oh + p.out_py) * p.out_Wp + ow0 + p.out_px) * 64 + n0 + q2;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const int m = h * 64 + r0 + rr * 8;
+            if (m < n_cols_valid) {
+#pragma unroll
+              for (int j = 0; j < NB / 8; ++j)
+                store_pair<SPLIT3, F16>(acc[h][4 * j + 2 * rr], acc[h][4 * j + 2 * rr + 1], bias[j], p.slope, p.out_hi, p.out_lo,
+                                        row_off + (long long)m * 64 + 8 * j);
+            }
+          }
+      }
+    }
+  }
+}
+
 }  // namespace dim

@@ -155,7 +155,7 @@ __global__ void __launch_bounds__(384, 1) conv_wgrad_kernel(const __grid_constan
 }
 
 // kinds of parameter tensors the reduction writes (MXNet layouts, SURVEY App. B-22)
-enum { WG_CONV = 0, WG_CONV1_S2D = 1, WG_DECONV = 2, WG_CONV1_ROW = 3 };
+enum { WG_CONV = 0, WG_CONV1_S2D = 1, WG_DECONV = 2, WG_CONV1_ROW = 3, WG_CONV1_RGBD = 4 };
 
 // grad[dst] = sum_slices partial[slice][tap][m][n]; one thread per SOURCE element (tap, m, n) with n fastest, so the
 // partial tiles are read coalesced; the (Cout,Cin,kh,kw) destination is written with a k*k-element stride.
@@ -163,6 +163,8 @@ enum { WG_CONV = 0, WG_CONV1_S2D = 1, WG_DECONV = 2, WG_CONV1_ROW = 3 };
 //   WG_CONV1_S2D : m = co, n = ph*16+pw*8+c  -> (64, 8, 7, 7), kh = 2dh+ph, kw = 2dw+pw      (taps = 16)
 //   WG_CONV1_ROW : m = dw*32+ph*16+pw*8+c, n = co, tap = dh -> (64, 8, 7, 7)                  (conv1_wgrad_kernel, taps = 4)
 //   WG_DECONV    : m = ci, n = co            -> (Cin, Cout, k, k)
+//   WG_CONV1_RGBD: m = co, n = ph*32+pw*16+c -> (64, 10, 7, 7), kh = 2dh+ph, kw = 2dw+pw  (RGB-D conv1, taps = 16; c >= 10 and
+//                  taps outside the 7 x 7 filter are the layout's zero padding and are dropped)
 __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float *__restrict__ partial, int kslices, int taps,
                                                            int Mp, int Np, int kind, int D0, int D1, int k,
                                                            float *__restrict__ grad) {
@@ -174,6 +176,9 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float *__restri
     d0 = m; d1 = n & 7;
     kh = 2 * (tap >> 2) + ((n >> 4) & 1); kw = 2 * (tap & 3) + ((n >> 3) & 1);
     if (n >= 32) return;
+  } else if (kind == WG_CONV1_RGBD) {
+    d0 = m; d1 = n & 15;
+    kh = 2 * (tap >> 2) + (n >> 5); kw = 2 * (tap & 3) + ((n >> 4) & 1);
   } else if (kind == WG_CONV1_ROW) {
     d0 = n; d1 = m & 7;
     kh = 2 * tap + ((m >> 4) & 1); kw = 2 * (m >> 5) + ((m >> 3) & 1);

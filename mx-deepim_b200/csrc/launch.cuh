@@ -17,12 +17,13 @@ struct TrainIO {
   void *const *bucket_events;
   const int *bucket_first_tensor;
   int n_buckets;
+  const float *zdo, *zdr;  // RGB-D network: zoomed depth_observed / depth_rendered f32 [B,1,H,W]; nullptr otherwise
 };
 
 // raster.cu
 int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
                   const double *means, int trunc_u8, float *out_image, float *out_depth, float *out_mask, float *out_bgr,
-                  int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit = nullptr);
+                  int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit = nullptr, bool ren4_depth = false);
 
 // zoom.cu
 int zoom_gather_launch(dim_ctx *ctx, int mode, const float *src, float *dst, const float *zoom_factor, int B, int C,
@@ -35,7 +36,12 @@ int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *
 int box_mask_launch(dim_ctx *ctx, const int *bbox, int B, float *mask, cudaStream_t st);
 int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, const float *zoom_factor,
                       const float *means_rgb, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
-                      cudaStream_t st, int f16, const double *means_d);
+                      cudaStream_t st, int f16, const double *means_d, bool depth = false);
+int obs4_depth_launch(dim_ctx *ctx, float4 *obs4, int B, const float *depth, const uint16_t *depth_u16, float factor,
+                      cudaStream_t st);
+int pack_nhwc10_launch(dim_ctx *ctx, const float *io, const float *ir, const float *dobs, const float *dren, const float *mo,
+                       const float *mr, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo, cudaStream_t st,
+                       int f16);
 int pack_obs4_launch(dim_ctx *ctx, const float *img, int B, float4 *out, const double *means, cudaStream_t st);
 int pack_nhwc8_launch(dim_ctx *ctx, const float *io, const float *ir, const float *mo, const float *mr, int B, int Hs,
                       int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo, cudaStream_t st, int f16);
@@ -76,6 +82,8 @@ void net_input_geometry(dim_ctx *ctx, int *rows, int *cols, int *pad, __nv_bfloa
 int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, float *rot_out, float *trans_out,
                 float *se3_out, cudaStream_t st, cudaEvent_t after_conv);
 bool net_graph_safe(dim_ctx *ctx);
+int net_set_input_depth(dim_ctx *ctx, bool enable);
+bool net_input_depth(dim_ctx *ctx);
 int net_layer_profile(dim_ctx *ctx, int enable, float *ms10);
 int net_debug_activation(dim_ctx *ctx, int idx, int lo, void *host_dst, size_t bytes);
 void net_layer_geometry(dim_ctx *ctx, int idx, int *out /*rows, cols, Cbuf, py, px, Ho, Wo, Cout*/);
@@ -87,7 +95,7 @@ int train_load_params(dim_ctx *ctx, const float *flat_host, size_t n, cudaStream
 int train_refresh_lo(dim_ctx *ctx, cudaStream_t st);
 int train_get_params(dim_ctx *ctx, float *flat_host, size_t n, int which, cudaStream_t st);
 size_t train_param_count(dim_ctx *ctx);
-int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel);
+int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel, bool input_depth = false);
 int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st);
 int train_sgd_update(dim_ctx *ctx, const float *grads, float lr, float momentum, float wd, float rescale, cudaStream_t st);
 int train_debug_tensor(dim_ctx *ctx, int id, void *host, size_t bytes);

@@ -31,7 +31,13 @@ static void build_geometry(NetState *ns, int H, int W) {
     int Hp = h + 2 * s.pad, Wp = w + 2 * s.pad;
     if (s.stride == 2) { Hp += Hp & 1; Wp += Wp & 1; }
     g.py = g.px = s.pad;
-    if (i == 0) {
+    if (i == 0 && ns->input_depth) {
+      // RGB-D conv1 (Cin = 10): space-to-depth with 16-channel phase chunks -> 4x4 taps over 64 channels (K = 1024)
+      g.Cin = 10;
+      g.rows = Hp / 2; g.cols = Wp / 2; g.Cbuf = 64;
+      g.KH = g.KW = 4; g.stride_eff = 1; g.Ceff = 64; g.Hq = g.rows;
+      g.BLOCK_K = 64; g.BLOCK_N = 64;
+    } else if (i == 0) {
       // conv1 (Cin = 8, 7x7 s2): space-to-depth -> 4x4 stride-1 taps over 32 channels
       g.rows = Hp / 2; g.cols = Wp / 2; g.Cbuf = 32;
       g.KH = g.KW = 4; g.stride_eff = 1; g.Ceff = 32; g.Hq = g.rows;
@@ -110,7 +116,14 @@ static int build_maps(NetState *ns, int B, bool f16, TensorMaps &tm) {
       __nv_bfloat16 *base = lo ? ns->act_lo[i] : ns->act_hi[i];
       CUtensorMap *maps = lo ? kp.a_lo_map : kp.a_map;
       const uint32_t box[3] = {(uint32_t)g.BLOCK_K, (uint32_t)g.BW, (uint32_t)g.BH};
-      if (i == 0) {
+      if (i == 0 && ns->input_depth) {
+        // RGB-D conv1 strip layout [B*rows][8 chunks][cols][8 ch]: box = 8 ch x (BW+3) cols x 8 chunks x 1 row
+        const uint64_t dims[4] = {8, (uint64_t)g.cols, 8, (uint64_t)B * g.rows};
+        const uint64_t str[3] = {16, (uint64_t)g.cols * 16, (uint64_t)g.cols * 128};
+        const uint32_t box4[4] = {8, (uint32_t)(g.BW + 3), 8, 1};
+        if (int rc = encode_map(&maps[0], base, 4, dims, str, box4, 0)) return rc;
+        maps[1] = maps[2] = maps[3] = maps[0];
+      } else if (i == 0) {
         // conv1 strip layout [B*rows][4 chunks][cols][8 ch]: box = 8 ch x (BW+3) cols x 4 chunks x 1 row
         const uint64_t dims[4] = {8, (uint64_t)g.cols, 4, (uint64_t)B * g.rows};
         const uint64_t str[3] = {16, (uint64_t)g.cols * 16, (uint64_t)g.cols * 64};
@@ -136,7 +149,8 @@ static int build_maps(NetState *ns, int B, bool f16, TensorMaps &tm) {
       const uint64_t Ktot = (uint64_t)g.KH * g.KW * g.Ceff;
       const uint64_t dims[2] = {Ktot, (uint64_t)g.Cout};
       const uint64_t str[1] = {Ktot * 2};
-      const uint32_t box[2] = {(uint32_t)g.BLOCK_K, (uint32_t)g.BLOCK_N};
+      // RGB-D conv1 loads its resident weights in boxes of 16 output channels (bf16x3 CTAs own 16 of them)
+      const uint32_t box[2] = {(uint32_t)g.BLOCK_K, (uint32_t)(i == 0 && ns->input_depth ? 16 : g.BLOCK_N)};
       __nv_bfloat16 *wop = f16 ? ns->w_f16[i] : ns->w_hi[i];
       if (int rc = encode_map(&kp.b_map, wop, 2, dims, str, box, g.BLOCK_K)) return rc;
       if (int rc = encode_map(&kp.b_lo_map, ns->w_lo[i], 2, dims, str, box, g.BLOCK_K)) return rc;
@@ -405,7 +419,20 @@ int net_load(dim_ctx *ctx, const float *const *W, const float *const *Bv) {
     const size_t Ktot = (size_t)g.KH * g.KW * g.Ceff;
     std::vector<float> packed((size_t)g.Cout * Ktot, 0.f);
     const float *w = W[i];  // [Cout][Cin][k][k]
-    if (i == 0) {
+    if (i == 0 && ns->input_depth) {
+      // W'[co][dh][dw][(ph*2 + pw)*16 + c] = W[co][c][2dh+ph][2dw+pw] for c < 10 (0 beyond 7x7 and for c >= 10)
+      for (int co = 0; co < g.Cout; ++co)
+        for (int dh = 0; dh < 4; ++dh)
+          for (int dw = 0; dw < 4; ++dw)
+            for (int ph = 0; ph < 2; ++ph)
+              for (int pw = 0; pw < 2; ++pw)
+                for (int c = 0; c < 10; ++c) {
+                  const int kh = 2 * dh + ph, kw = 2 * dw + pw;
+                  if (kh >= 7 || kw >= 7) continue;
+                  packed[(size_t)co * Ktot + (size_t)(dh * 4 + dw) * 64 + (ph * 2 + pw) * 16 + c] =
+                      w[(((size_t)co * 10 + c) * 7 + kh) * 7 + kw];
+                }
+    } else if (i == 0) {
       // space-to-depth repack: W'[co][dh][dw][conv1_kslot(dw,ph,pw)+c] = W[co][c][2dh+ph][2dw+pw] (0 beyond 7x7)
       for (int co = 0; co < g.Cout; ++co)
         for (int dh = 0; dh < 4; ++dh)
@@ -488,6 +515,47 @@ static int launch_conv1(const ConvKParams &kp, int grid, int rows_total, int rpc
   return 0;
 }
 
+template <int ST, bool S3, bool F16, int NB>
+static int launch_conv1_rgbd(const ConvKParams &kp, int grid, int rows_total, int rpc, int chunks, int strip_bytes,
+                             cudaStream_t st) {
+  const int smem_bytes = 16 * NB * 128 * (S3 ? 2 : 1) + ST * (S3 ? 2 : 1) * strip_bytes + kConv1Slack + 1024 + 256;
+  DIM_REQUIRE(smem_bytes <= 227 * 1024, "conv1 (RGB-D): image too wide for the rolling-strip ring");
+  static int set = 0;
+  if (set < smem_bytes) {
+    DIM_CHECK(cudaFuncSetAttribute(conv1_rgbd_kernel<ST, S3, F16, NB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   smem_bytes));
+    set = smem_bytes;
+  }
+  conv1_rgbd_kernel<ST, S3, F16, NB><<<grid, 384, smem_bytes, st>>>(kp, rows_total, rpc, chunks, strip_bytes);
+  DIM_LAUNCH_CHECK();
+  return 0;
+}
+
+// switches conv1 between the 8-channel and the 10-channel (RGB-D) input; only before any weights are loaded.  The wider
+// input buffer is allocated on the first switch and kept.
+int net_set_input_depth(dim_ctx *ctx, bool enable) {
+  NetState *ns = ctx->net;
+  DIM_REQUIRE(ns != nullptr, "net not created");
+  if (ns->input_depth == enable) return 0;
+  DIM_REQUIRE(!ns->loaded, "dim_ctx_set_input_depth: call it before dim_net_load (this context's weights are loaded)");
+  if (!ns->act0_rgb_hi) { ns->act0_rgb_hi = ns->act_hi[0]; ns->act0_rgb_lo = ns->act_lo[0]; }
+  ns->input_depth = enable;
+  build_geometry(ns, ctx->H, ctx->W);
+  ns->maps.clear();
+  const LayerGeom &g = ns->g[0];
+  const size_t per = (size_t)g.rows * g.cols * g.Cbuf;
+  ns->act_elems_per_image[0] = per;
+  if (enable && ns->net_ok && !ns->act0_rgbd_hi) {
+    if (int rc = dev_alloc(ctx, &ns->act0_rgbd_hi, per * ctx->max_batch, true)) return rc;
+    if (int rc = dev_alloc(ctx, &ns->act0_rgbd_lo, per * ctx->max_batch, true)) return rc;
+  }
+  ns->act_hi[0] = enable ? ns->act0_rgbd_hi : ns->act0_rgb_hi;
+  ns->act_lo[0] = enable ? ns->act0_rgbd_lo : ns->act0_rgb_lo;
+  return 0;
+}
+
+bool net_input_depth(dim_ctx *ctx) { return ctx->net && ctx->net->input_depth; }
+
 // where conv1's input buffer expects pixel (i,j) of the 8-channel blob (space-to-depth, pad 3)
 void net_input_geometry(dim_ctx *ctx, int *rows, int *cols, int *pad, __nv_bfloat16 **hi, __nv_bfloat16 **lo) {
   NetState *ns = ctx->net;
@@ -525,7 +593,21 @@ int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, fl
     const int total_tiles = cdiv(B * g.Hq, g.BH) * g.n_col_tiles * n_tiles;
     const int sms = ns->num_sms;
     int rc;
-    if (i == 0) {
+    if (i == 0 && ns->input_depth) {
+      // RGB-D conv1: the same rolling strips, 8 chunk planes per strip; bf16x3 splits the output channels four ways
+      const int nsplit = s3 ? 4 : 1;
+      const int rows_total = B * g.Hq;
+      int chunks = sms / (g.n_col_tiles * nsplit);
+      if (chunks > cdiv(rows_total, 16)) chunks = cdiv(rows_total, 16);
+      if (chunks < 1) chunks = 1;
+      const int rpc = cdiv(rows_total, chunks);
+      chunks = cdiv(rows_total, rpc);
+      const int strip_bytes = cdiv((g.BW + 3) * 128, 128) * 128;
+      const int grid = g.n_col_tiles * chunks * nsplit;
+      rc = s3 ? launch_conv1_rgbd<5, true, false, 16>(kp, grid, rows_total, rpc, chunks, strip_bytes, st)
+              : (f16 ? launch_conv1_rgbd<6, false, true, 64>(kp, grid, rows_total, rpc, chunks, strip_bytes, st)
+                     : launch_conv1_rgbd<6, false, false, 64>(kp, grid, rows_total, rpc, chunks, strip_bytes, st));
+    } else if (i == 0) {
       // conv1: a CTA walks down a run of output rows of one column tile, one new input strip per row
       const int rows_total = B * g.Hq;
       int chunks = sms / g.n_col_tiles;

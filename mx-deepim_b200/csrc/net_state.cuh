@@ -53,6 +53,10 @@ struct NetState {
   float *fc6_partial = nullptr;  // [FC6_SPLITS][max_batch][256]
   cudaEvent_t *layer_events = nullptr;  // tuning hook: 11 events around the conv layers of the last forward
   bool loaded = false, net_ok = false;
+  // RGB-D network (dim_ctx_set_input_depth): flow_conv1 takes 10 channels and its space-to-depth input has 64 channels
+  // (conv1_rgbd_kernel); the 8-channel network's conv1 input buffers are kept for switching back
+  bool input_depth = false;
+  __nv_bfloat16 *act0_rgb_hi = nullptr, *act0_rgb_lo = nullptr, *act0_rgbd_hi = nullptr, *act0_rgbd_lo = nullptr;
   float *save_h6 = nullptr, *save_h7 = nullptr;
   cudaEvent_t repack_done = nullptr;  // training: the operand packs are refreshed on an internal stream after an update;
                                       // every consumer (net_forward) orders itself behind this event

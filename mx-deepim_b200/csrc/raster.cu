@@ -260,8 +260,10 @@ __device__ __forceinline__ float colour_of(unsigned char c, int trunc_u8) {
   return f;
 }
 
-// LIT is a compile-time switch: the unlit instantiation (the refinement loop's renderer) carries none of the shading code
-template <bool LIT>
+// LIT is a compile-time switch: the unlit instantiation (the refinement loop's renderer) carries none of the shading code.
+// REN4_DEPTH (the RGB-D network's loop): the w lane of out_ren4 holds the depth instead of the 0/1 mask; the zoom kernel
+// samples it as depth_rendered and re-derives the mask as depth > 0.2, which is how the mask is made here.
+template <bool LIT, bool REN4_DEPTH = false>
 __global__ void __launch_bounds__(256) raster_resolve_kernel(RasterParams p) {
   const int b = blockIdx.y;
   const int W4 = p.W >> 2;
@@ -386,7 +388,7 @@ __global__ void __launch_bounds__(256) raster_resolve_kernel(RasterParams p) {
       float4 *o4 = p.out_ren4 + (size_t)b * P + o;
 #pragma unroll
       for (int k = 0; k < 4; ++k)
-        o4[k] = make_float4(r[k] + (float)p.mean[0], g[k] + (float)p.mean[1], bl[k] + (float)p.mean[2], mk[k]);
+        o4[k] = make_float4(r[k] + (float)p.mean[0], g[k] + (float)p.mean[1], bl[k] + (float)p.mean[2], REN4_DEPTH ? d[k] : mk[k]);
     }
     if (p.out_depth) *reinterpret_cast<float4 *>(p.out_depth + (size_t)b * P + o) = make_float4(d[0], d[1], d[2], d[3]);
     if (p.out_mask) *reinterpret_cast<float4 *>(p.out_mask + (size_t)b * P + o) = make_float4(mk[0], mk[1], mk[2], mk[3]);
@@ -424,7 +426,7 @@ __global__ void raster_finish_kernel(int *bbox_ren, int *out_bbox, int B) {
 
 int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
                   const double *means, int trunc_u8, float *out_image, float *out_depth, float *out_mask,
-                  float *out_bgr, int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit) {
+                  float *out_bgr, int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit, bool ren4_depth) {
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_render: batch exceeds max_batch");
   DIM_REQUIRE((ctx->W & 3) == 0, "dim_render: width must be a multiple of 4");
   RasterParams p;
@@ -453,8 +455,15 @@ int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const 
   DIM_LAUNCH_CHECK();
   raster_coverage_kernel<<<dim3(cdiv(maxF, 128), B), 128, 0, st>>>(p);
   DIM_LAUNCH_CHECK();
-  if (p.lit) raster_resolve_kernel<true><<<dim3(cdiv((ctx->W / 4) * ctx->H, 256), B), 256, 0, st>>>(p);
-  else raster_resolve_kernel<false><<<dim3(cdiv((ctx->W / 4) * ctx->H, 256), B), 256, 0, st>>>(p);
+  const dim3 rgrid(cdiv((ctx->W / 4) * ctx->H, 256), B);
+  if (ren4_depth) {
+    if (p.lit) raster_resolve_kernel<true, true><<<rgrid, 256, 0, st>>>(p);
+    else raster_resolve_kernel<false, true><<<rgrid, 256, 0, st>>>(p);
+  } else if (p.lit) {
+    raster_resolve_kernel<true><<<rgrid, 256, 0, st>>>(p);
+  } else {
+    raster_resolve_kernel<false><<<rgrid, 256, 0, st>>>(p);
+  }
   DIM_LAUNCH_CHECK();
   raster_finish_kernel<<<cdiv(B, 128), 128, 0, st>>>(ctx->bbox_ren, out_bbox, B);
   DIM_LAUNCH_CHECK();

@@ -70,6 +70,8 @@ struct TrainState {
   size_t n_params = 0;
   float *master = nullptr, *mom = nullptr;
   Buf act10b, cat2, cat3, dcat2, dcat3, dA10p, gz[10], s2d32;
+  Buf s2d64;         // RGB-D network: conv1's input as NHWC-64 (weight gradient operand)
+  bool input_depth = false;  // the table's flow_conv1 is (64, 10, 7, 7)
   float *flow6 = nullptr, *flow5 = nullptr, *flow4 = nullptr, *mask4 = nullptr;
   float *dflow6 = nullptr, *dflow5 = nullptr, *dflow4 = nullptr, *dmask4 = nullptr;
   float *dfull = nullptr;        // [B][3][H][W] gradient wrt the full-resolution flow (2) / mask logit (1)
@@ -107,6 +109,17 @@ __global__ void __launch_bounds__(256) strip_to_nhwc32_kernel(const __nv_bfloat1
   const int chunk = (int)((i / Ws) % 4);
   const size_t row = i / ((size_t)Ws * 4);
   *reinterpret_cast<uint4 *>(dst + ((row * Ws + col) * 32 + chunk * 8)) = *reinterpret_cast<const uint4 *>(src + i * 8);
+}
+
+// RGB-D conv1 input: src [(b*Hs + r)][8][Ws][8] -> dst [(b*Hs + r)][Ws][64] (channel = phase*16 + c); one 16-byte chunk per thread
+__global__ void __launch_bounds__(256) strip_to_nhwc64_kernel(const __nv_bfloat16 *src, __nv_bfloat16 *dst, size_t n_chunks,
+                                                              int Ws) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_chunks) return;
+  const int col = (int)(i % Ws);
+  const int chunk = (int)((i / Ws) % 8);
+  const size_t row = i / ((size_t)Ws * 8);
+  *reinterpret_cast<uint4 *>(dst + ((row * Ws + col) * 64 + chunk * 8)) = *reinterpret_cast<const uint4 *>(src + i * 8);
 }
 
 // copy channels [0,C) of an NHWC buffer's valid region into another buffer (different border / channel stride)
@@ -625,6 +638,14 @@ __global__ void __launch_bounds__(256) pack_conv_fwd_kernel(const float *w, int 
     store_split(hi, lo, ((size_t)co * kk + tap) * Cin + c0 + cl, tile[cl * kk + tap]);
   }
 }
+// RGB-D conv1 space-to-depth pack [64][4][4][64]: K = (ph*2 + pw)*16 + c within a tap (net.cu net_load)
+__global__ void __launch_bounds__(256) pack_conv1_rgbd_kernel(const float *w, __nv_bfloat16 *hi, __nv_bfloat16 *lo) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 64 * 1024) return;
+  const int co = i >> 10, tap = (i >> 6) & 15, phase = (i >> 4) & 3, c = i & 15;
+  const int kh = 2 * (tap >> 2) + (phase >> 1), kw = 2 * (tap & 3) + (phase & 1);
+  store_split(hi, lo, i, (c < 10 && kh < 7 && kw < 7) ? w[((co * 10 + c) * 7 + kh) * 7 + kw] : 0.f);
+}
 // conv1 space-to-depth pack [64][4][4][32]
 __global__ void __launch_bounds__(256) pack_conv1_kernel(const float *w, __nv_bfloat16 *hi, __nv_bfloat16 *lo) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -702,6 +723,12 @@ __global__ void transpose256_kernel(const float *w, float *wT) {
 
 // ------------------------------------------------------------------------------------ host side
 static size_t param_numel(const ParamSpec &s) { return (size_t)s.d0 * s.d1 * s.k * s.k; }
+// the table entry of the RGB or the RGB-D network: they differ only in flow_conv1's input channels (8 / 10)
+static ParamSpec param_spec(int i, bool input_depth) {
+  ParamSpec s = kParams[i];
+  if (i == 0 && input_depth) s.d1 = 10;
+  return s;
+}
 static size_t bias_numel(const ParamSpec &s) {
   if (s.kind == PK_FROZEN) return 0;
   return s.kind == PK_DECONV ? s.d1 : s.d0;
@@ -727,9 +754,10 @@ int train_create(dim_ctx *ctx, int max_points) {
   TrainState *ts = new TrainState();
   train_of(ctx) = ts;
   ts->max_points = max_points;
+  ts->input_depth = ns->input_depth;
   size_t off = 0;
   for (int i = 0; i < 24; ++i) {
-    ts->off[i].w = off; ts->off[i].wn = param_numel(kParams[i]); off += ts->off[i].wn;
+    ts->off[i].w = off; ts->off[i].wn = param_numel(param_spec(i, ts->input_depth)); off += ts->off[i].wn;
     ts->off[i].b = off; ts->off[i].bn = bias_numel(kParams[i]); off += ts->off[i].bn;
   }
   ts->n_params = off;
@@ -745,7 +773,8 @@ int train_create(dim_ctx *ctx, int max_points) {
   rc |= alloc_buf(ctx, ts->dcat3, B, g[5].Ho, g[5].Wo, 832, 1, true);
   rc |= alloc_buf(ctx, ts->dA10p, B, g[9].Ho, g[9].Wo, 1024, 0, false);
   for (int i = 0; i < 10; ++i) rc |= alloc_buf(ctx, ts->gz[i], B, g[i].Ho, g[i].Wo, g[i].Cout, 1, false);
-  rc |= alloc_buf(ctx, ts->s2d32, B, g[0].rows, g[0].cols, 32, 0, false);
+  if (ts->input_depth) rc |= alloc_buf(ctx, ts->s2d64, B, g[0].rows, g[0].cols, 64, 0, false);
+  else rc |= alloc_buf(ctx, ts->s2d32, B, g[0].rows, g[0].cols, 32, 0, false);
   const size_t n6 = (size_t)B * g[9].Ho * g[9].Wo, n5 = (size_t)B * g[7].Ho * g[7].Wo, n4 = (size_t)B * g[5].Ho * g[5].Wo;
   rc |= dev_alloc(ctx, &ts->flow6, n6 * 2, true); rc |= dev_alloc(ctx, &ts->dflow6, n6 * 2, true);
   rc |= dev_alloc(ctx, &ts->flow5, n5 * 2, true); rc |= dev_alloc(ctx, &ts->dflow5, n5 * 2, true);
@@ -822,7 +851,8 @@ static int repack_all(dim_ctx *ctx, cudaStream_t st, bool with_lo) {
   NetState *ns = ctx->net;
   TrainState *ts = train_of(ctx);
   const float *M = ts->master;
-  LAUNCH1D(pack_conv1_kernel, 64 * 512, st, M + ts->off[0].w, ns->w_hi[0], with_lo ? ns->w_lo[0] : nullptr);
+  if (ts->input_depth) LAUNCH1D(pack_conv1_rgbd_kernel, 64 * 1024, st, M + ts->off[0].w, ns->w_hi[0], with_lo ? ns->w_lo[0] : nullptr);
+  else LAUNCH1D(pack_conv1_kernel, 64 * 512, st, M + ts->off[0].w, ns->w_hi[0], with_lo ? ns->w_lo[0] : nullptr);
   for (int i = 1; i < 10; ++i) {
     const LayerSpec &s = kLayers[i];
     pack_conv_fwd_kernel<<<dim3(s.Cout, cdiv(s.Cin, 64)), 256, 0, st>>>(M + ts->off[i].w, s.Cout, s.Cin, s.k, ns->w_hi[i],
@@ -892,9 +922,10 @@ int train_get_params(dim_ctx *ctx, float *flat_host, size_t n, int which, cudaSt
 }
 
 size_t train_param_count(dim_ctx *ctx) { TrainState *ts = train_of(ctx); return ts ? ts->n_params : 0; }
-int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel) {
+int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel, bool input_depth) {
   if (idx < 0 || idx >= 24) return 1;
-  *name = kParams[idx].name; *w_numel = (long long)param_numel(kParams[idx]); *b_numel = (long long)bias_numel(kParams[idx]);
+  const ParamSpec s = param_spec(idx, input_depth);
+  *name = s.name; *w_numel = (long long)param_numel(s); *b_numel = (long long)bias_numel(s);
   return 0;
 }
 
@@ -1203,7 +1234,10 @@ static int build_train_maps(dim_ctx *ctx, int B, TrainMaps &tm) {
   // weight gradients
   for (int i = 0; i < 10; ++i) {
     const LayerSpec &s = kLayers[i];
-    if (i == 0) {
+    if (i == 0 && ts->input_depth) {  // generic kernel over the 16 taps of the NHWC-64 copy (SW128 boxes), WG_CONV1_RGBD reduce
+      if (int rc = make_wgrad(ts, tm.wg[0], tm.wg_bn[0], B, ts->gz[0], 0, 64, ns->g[0].Ho, ns->g[0].Wo, ts->s2d64, 0, 64, 1, 4, 4, 0, 0, sms))
+        return rc;
+    } else if (i == 0) {
       if (int rc = make_wgrad(ts, tm.wg[0], tm.wg_bn[0], B, ts->gz[0], 0, 64, ns->g[0].Ho, ns->g[0].Wo, ts->s2d32, 0, 32, 1, 4, 4, 0, 0, sms))
         return rc;
     } else {
@@ -1289,7 +1323,15 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
   // ---------------- forward
   DimNvtxRange r_fwd("dim_train forward + losses");
   DIM_CHECK(cudaEventRecord(ts->ev_phase[0], st));
-  if (int rc = pack_nhwc8_launch(ctx, io.zio, io.zir, io.zmo, io.zmr, B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0], nullptr, st, 0)) return rc;
+  DIM_REQUIRE((io.zdo && io.zdr) == ts->input_depth && (io.zdo == nullptr) == (io.zdr == nullptr),
+              "dim_train_forward_backward: the RGB-D network takes both zoomed depths, the RGB network none");
+  if (ts->input_depth) {
+    if (int rc = pack_nhwc10_launch(ctx, io.zio, io.zir, io.zdo, io.zdr, io.zmo, io.zmr, B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0],
+                                    nullptr, st, 0))
+      return rc;
+  } else if (int rc = pack_nhwc8_launch(ctx, io.zio, io.zir, io.zmo, io.zmr, B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0], nullptr, st, 0)) {
+    return rc;
+  }
   if (int rc = net_forward(ctx, B, DIM_PREC_BF16, nullptr, ts->rot_raw, ts->ztrans, nullptr, st, nullptr)) return rc;
   DIM_CHECK(cudaEventRecord(ts->ev_phase[1], st));
   const Buf a10 = act_buf(ns, 10), a8 = act_buf(ns, 8), a6 = act_buf(ns, 6);
@@ -1402,15 +1444,21 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
   if (int rc = run_generic(ctx, tm.deconv5_dgrad, tm.g_deconv5_dgrad, B, st)) return rc;
   DIM_CHECK(cudaEventRecord(ts->ev_phase[5], st));
   // encoder
-  LAUNCH1D(strip_to_nhwc32_kernel, (size_t)B * g[0].rows * 4 * g[0].cols, st, ns->act_hi[0], ts->s2d32.p, (size_t)B * g[0].rows * 4 * g[0].cols,
-           g[0].cols);
+  if (ts->input_depth)
+    LAUNCH1D(strip_to_nhwc64_kernel, (size_t)B * g[0].rows * 8 * g[0].cols, st, ns->act_hi[0], ts->s2d64.p,
+             (size_t)B * g[0].rows * 8 * g[0].cols, g[0].cols);
+  else
+    LAUNCH1D(strip_to_nhwc32_kernel, (size_t)B * g[0].rows * 4 * g[0].cols, st, ns->act_hi[0], ts->s2d32.p,
+             (size_t)B * g[0].rows * 4 * g[0].cols, g[0].cols);
   for (int i = 9; i >= 0; --i) {
     const LayerSpec &s = kLayers[i];
     if (int rc = fork_side(ts, st)) return rc;  // gz[i] is complete on st
     if (i == 9)  // heads, decoder (thin kernels on st, deconvolution wgrads on sw): tensors 10..23 are done
       if (int rc = record_buckets(io, 10, 1 << 30, sw)) return rc;
     if (int rc = bias_grad(ts, ts->gz[i], B, 0, s.Cout, G + ts->off[i].b, sw)) return rc;
-    if (i == 0) {
+    if (i == 0 && ts->input_depth) {
+      if (int rc = run_wgrad(tm.wg[0], tm.wg_bn[0], WG_CONV1_RGBD, 64, 10, 7, G + ts->off[0].w, sw)) return rc;
+    } else if (i == 0) {
       if (int rc = run_wgrad_conv1(ts, tm.wg[0], ctx->num_sms, G + ts->off[0].w, sw)) return rc;
     } else if (int rc = run_wgrad(tm.wg[i], tm.wg_bn[i], WG_CONV, s.Cout, s.Cin, s.k, G + ts->off[i].w, sw)) return rc;
     if (int rc = record_buckets(io, i, i + 1, sw)) return rc;

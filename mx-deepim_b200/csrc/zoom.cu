@@ -301,8 +301,8 @@ int box_mask_launch(dim_ctx *ctx, const int *bbox, int B, float *mask, cudaStrea
 // The two source images already hold (image + mean) -- the sampler's first step, done once by their producers with the
 // same float32 addition -- so a tap costs no arithmetic before its weight.
 struct FusedZoomParams {
-  const float4 *obs4;   // [B,H,W,4] observed (RGB - mean) + mean (w unused)
-  const float4 *ren4;   // [B,H,W,4] rendered (RGB - mean) + mean, w = mask_rendered (0/1)
+  const float4 *obs4;   // [B,H,W,4] observed (RGB - mean) + mean, w unused (RGB-D network: w = depth_observed)
+  const float4 *ren4;   // [B,H,W,4] rendered (RGB - mean) + mean, w = mask_rendered (0/1) (RGB-D network: w = depth)
   const int *bbox8;     // observed box = bb[0..3] (inclusive)
   const int *vbox;      // [B,4] x0,x1,y0,y1: ren4 is only valid inside this box (rasteriser), background outside; nullable
   float bg[3];          // background of the rendered image + mean: (float)(0.0 - mean) + (float)mean
@@ -348,48 +348,10 @@ __device__ __forceinline__ AxisTap axis_tap(int o, float w, float t, int N, floa
   return a;
 }
 
+// eight channel values -> one 16-byte chunk (bf16 / fp16), `l` the bf16 residuals (bf16x3)
 template <bool LO, bool F16>
-__device__ __forceinline__ void zoom_fused_pixel(const FusedZoomParams &p, const float4 *__restrict__ ob,
-                                                 const float4 *__restrict__ rn, const AxisTap &x, const AxisTap &y,
-                                                 uint4 &h, uint4 &l) {
-  const int W = p.W;
-  const int y0 = y.a0 * W, y1 = y.a1 * W;
-  const float4 O00 = __ldg(ob + (y0 + x.a0)), O01 = __ldg(ob + (y0 + x.a1));
-  const float4 O10 = __ldg(ob + (y1 + x.a0)), O11 = __ldg(ob + (y1 + x.a1));
-  // rendered taps: outside the rasteriser's vertex box the image is background by construction (and ren4 is not written there)
-  const float4 bg4 = make_float4(p.bg[0], p.bg[1], p.bg[2], 0.f);
-  const float4 R00 = (y.r0 && x.r0) ? __ldg(rn + (y0 + x.a0)) : bg4;
-  const float4 R01 = (y.r0 && x.r1) ? __ldg(rn + (y0 + x.a1)) : bg4;
-  const float4 R10 = (y.r1 && x.r0) ? __ldg(rn + (y1 + x.a0)) : bg4;
-  const float4 R11 = (y.r1 && x.r1) ? __ldg(rn + (y1 + x.a1)) : bg4;
-  const float wa = y.w0 * x.w0, wb = y.w0 * x.w1, wc = y.w1 * x.w0, wd = y.w1 * x.w1;
-  float v[8];
-  // (img + mean) sampled with zero padding, then - mean, then the graph's /255.  The IEEE division is spelled out as
-  // q = x * (1/255); q += (x - q * 255) * (1/255) with two fused multiply-adds: the correctly rounded quotient for every
-  // |x| < 2^10 (exhaustively compared with x / 255.0f on 2e7 samples + all integer texels), at 3 instructions instead of ~10
-  const float rcp255 = 1.0f / 255.0f;
-  auto img = [&](float tl, float tr, float bl, float br, float m) -> float {
-    const float s = fmaf(br, wd, fmaf(bl, wc, fmaf(tr, wb, tl * wa))) - m;
-    const float q = s * rcp255;
-    return fmaf(fmaf(-q, 255.0f, s), rcp255, q);
-  };
-  v[0] = img(O00.x, O01.x, O10.x, O11.x, p.mean[0]);
-  v[1] = img(O00.y, O01.y, O10.y, O11.y, p.mean[1]);
-  v[2] = img(O00.z, O01.z, O10.z, O11.z, p.mean[2]);
-  v[3] = img(R00.x, R01.x, R10.x, R11.x, p.mean[0]);
-  v[4] = img(R00.y, R01.y, R10.y, R11.y, p.mean[1]);
-  v[5] = img(R00.z, R01.z, R10.z, R11.z, p.mean[2]);
-  {  // observed mask = rectangle (an empty box has m0 > m1 on both axes)
-    const float tl = (y.m0 && x.m0) ? 1.f : 0.f, tr = (y.m0 && x.m1) ? 1.f : 0.f;
-    const float bl = (y.m1 && x.m0) ? 1.f : 0.f, br = (y.m1 && x.m1) ? 1.f : 0.f;
-    v[6] = roundf(fmaf(br, wd, fmaf(bl, wc, fmaf(tr, wb, tl * wa))));
-  }
-  {  // rendered mask, binarised at 0.2 (zoom_mask.py:39-41)
-    const float tl = R00.w > 0.2f ? 1.f : 0.f, tr = R01.w > 0.2f ? 1.f : 0.f;
-    const float bl = R10.w > 0.2f ? 1.f : 0.f, br = R11.w > 0.2f ? 1.f : 0.f;
-    v[7] = roundf(fmaf(br, wd, fmaf(bl, wc, fmaf(tr, wb, tl * wa))));
-  }
-  if (F16) {  // |v| <= 1: always in range
+__device__ __forceinline__ void pack_chunk(const float *v, uint4 &h, uint4 &l) {
+  if (F16) {  // |v| <= 1 (depth: metres / 255): always in range
     h = make_uint4(pack2_f16(v[0], v[1]), pack2_f16(v[2], v[3]), pack2_f16(v[4], v[5]), pack2_f16(v[6], v[7]));
   } else {
     uint32_t hh[4], ll[4];
@@ -408,11 +370,69 @@ __device__ __forceinline__ void zoom_fused_pixel(const FusedZoomParams &p, const
   }
 }
 
+// DEPTH (RGB-D network, deepIM_flownet.py:35-43): the channels are image_observed/255, image_rendered/255,
+// depth_observed/255, depth_rendered/255, mask_observed, mask_rendered in two chunks (channels 0-7, then 8-9 and zeros).
+// The depths ride in the w lanes: obs4.w = depth_observed, ren4.w = the render's depth (0 = background, so the rendered
+// mask depth > 0.2 of tester.py:440 is the same binarisation at 0.2 as for the 0/1 mask).  ZoomDepth (zoom_depth.py:24-44)
+// is the plain bilinear sample, zero outside the frame: the image taps with no mean.
+template <bool LO, bool F16, bool DEPTH = false>
+__device__ __forceinline__ void zoom_fused_pixel(const FusedZoomParams &p, const float4 *__restrict__ ob,
+                                                 const float4 *__restrict__ rn, const AxisTap &x, const AxisTap &y,
+                                                 uint4 (&h)[DEPTH ? 2 : 1], uint4 (&l)[DEPTH ? 2 : 1]) {
+  const int W = p.W;
+  const int y0 = y.a0 * W, y1 = y.a1 * W;
+  const float4 O00 = __ldg(ob + (y0 + x.a0)), O01 = __ldg(ob + (y0 + x.a1));
+  const float4 O10 = __ldg(ob + (y1 + x.a0)), O11 = __ldg(ob + (y1 + x.a1));
+  // rendered taps: outside the rasteriser's vertex box the image is background by construction (and ren4 is not written there)
+  const float4 bg4 = make_float4(p.bg[0], p.bg[1], p.bg[2], 0.f);
+  const float4 R00 = (y.r0 && x.r0) ? __ldg(rn + (y0 + x.a0)) : bg4;
+  const float4 R01 = (y.r0 && x.r1) ? __ldg(rn + (y0 + x.a1)) : bg4;
+  const float4 R10 = (y.r1 && x.r0) ? __ldg(rn + (y1 + x.a0)) : bg4;
+  const float4 R11 = (y.r1 && x.r1) ? __ldg(rn + (y1 + x.a1)) : bg4;
+  const float wa = y.w0 * x.w0, wb = y.w0 * x.w1, wc = y.w1 * x.w0, wd = y.w1 * x.w1;
+  constexpr int MO = DEPTH ? 8 : 6;  // channel of mask_observed; mask_rendered follows
+  float v[DEPTH ? 16 : 8];
+  // (img + mean) sampled with zero padding, then - mean, then the graph's /255.  The IEEE division is spelled out as
+  // q = x * (1/255); q += (x - q * 255) * (1/255) with two fused multiply-adds: the correctly rounded quotient for every
+  // |x| < 2^10 (exhaustively compared with x / 255.0f on 2e7 samples + all integer texels), at 3 instructions instead of ~10
+  const float rcp255 = 1.0f / 255.0f;
+  auto img = [&](float tl, float tr, float bl, float br, float m) -> float {
+    const float s = fmaf(br, wd, fmaf(bl, wc, fmaf(tr, wb, tl * wa))) - m;
+    const float q = s * rcp255;
+    return fmaf(fmaf(-q, 255.0f, s), rcp255, q);
+  };
+  v[0] = img(O00.x, O01.x, O10.x, O11.x, p.mean[0]);
+  v[1] = img(O00.y, O01.y, O10.y, O11.y, p.mean[1]);
+  v[2] = img(O00.z, O01.z, O10.z, O11.z, p.mean[2]);
+  v[3] = img(R00.x, R01.x, R10.x, R11.x, p.mean[0]);
+  v[4] = img(R00.y, R01.y, R10.y, R11.y, p.mean[1]);
+  v[5] = img(R00.z, R01.z, R10.z, R11.z, p.mean[2]);
+  if constexpr (DEPTH) {
+    v[6] = img(O00.w, O01.w, O10.w, O11.w, 0.f);
+    v[7] = img(R00.w, R01.w, R10.w, R11.w, 0.f);
+#pragma unroll
+    for (int c = 10; c < 16; ++c) v[c] = 0.f;
+  }
+  {  // observed mask = rectangle (an empty box has m0 > m1 on both axes)
+    const float tl = (y.m0 && x.m0) ? 1.f : 0.f, tr = (y.m0 && x.m1) ? 1.f : 0.f;
+    const float bl = (y.m1 && x.m0) ? 1.f : 0.f, br = (y.m1 && x.m1) ? 1.f : 0.f;
+    v[MO] = roundf(fmaf(br, wd, fmaf(bl, wc, fmaf(tr, wb, tl * wa))));
+  }
+  {  // rendered mask, binarised at 0.2 (zoom_mask.py:39-41)
+    const float tl = R00.w > 0.2f ? 1.f : 0.f, tr = R01.w > 0.2f ? 1.f : 0.f;
+    const float bl = R10.w > 0.2f ? 1.f : 0.f, br = R11.w > 0.2f ? 1.f : 0.f;
+    v[MO + 1] = roundf(fmaf(br, wd, fmaf(bl, wc, fmaf(tr, wb, tl * wa))));
+  }
+  pack_chunk<LO, F16>(v, h[0], l[0]);
+  if constexpr (DEPTH) pack_chunk<LO, F16>(v + 8, h[1], l[1]);
+}
+
 // one thread per space-to-depth pixel = a 2x2 quad of output pixels = the four 16-byte channel chunks
 // of conv1's strip layout (consecutive threads write consecutive 16 B of each chunk plane); border
 // slots are rewritten with zeros.  Sources are the pixel-interleaved float4 images, so each tap is one 16-byte load
 // per image; the column taps of the quad's two columns and the row taps of its two rows are computed once each.
-template <bool LO, bool F16>
+// DEPTH: the RGB-D network's input, two chunk planes per quad slot: [B*Hs rows][8 planes = (slot, half)][Ws cols][8 ch]
+template <bool LO, bool F16, bool DEPTH = false>
 __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParams p) {
   const int b = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -432,21 +452,27 @@ __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParam
   }
   const size_t base = (size_t)b * p.H * p.W;
   const float4 *ob = p.obs4 + base, *rn = p.ren4 + base;
-  // conv1 strip layout: [B*Hs rows][4 chunks (= quad slot)][Ws cols][8 ch]
+  // conv1 strip layout: [B*Hs rows][4 chunks (= quad slot)][Ws cols][8 ch] (DEPTH: 2 chunks per slot)
+  constexpr int NC = DEPTH ? 2 : 1;
 #pragma unroll
   for (int s = 0; s < 4; ++s) {
     const int i = i0 + (s >> 1), j = j0 + (s & 1);
-    uint4 h = make_uint4(0u, 0u, 0u, 0u), l = make_uint4(0u, 0u, 0u, 0u);  // zero bits are the same in both formats
-    if (i >= 0 && i < p.H && j >= 0 && j < p.W) zoom_fused_pixel<LO, F16>(p, ob, rn, xt[s & 1], yt[s >> 1], h, l);
-    const size_t o = ((((size_t)b * p.Hs + sr) * 4 + s) * p.Ws + sc) * 8;
-    *reinterpret_cast<uint4 *>(p.hi + o) = h;
-    if (LO) *reinterpret_cast<uint4 *>(p.lo + o) = l;
+    uint4 h[NC], l[NC];
+#pragma unroll
+    for (int c = 0; c < NC; ++c) h[c] = l[c] = make_uint4(0u, 0u, 0u, 0u);  // zero bits are the same in both formats
+    if (i >= 0 && i < p.H && j >= 0 && j < p.W) zoom_fused_pixel<LO, F16, DEPTH>(p, ob, rn, xt[s & 1], yt[s >> 1], h, l);
+#pragma unroll
+    for (int c = 0; c < NC; ++c) {
+      const size_t o = ((((size_t)b * p.Hs + sr) * 4 * NC + s * NC + c) * p.Ws + sc) * 8;
+      *reinterpret_cast<uint4 *>(p.hi + o) = h[c];
+      if (LO) *reinterpret_cast<uint4 *>(p.lo + o) = l[c];
+    }
   }
 }
 
 int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, const float *zoom_factor,
                       const float *means_rgb, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
-                      cudaStream_t st, int f16, const double *means_d) {
+                      cudaStream_t st, int f16, const double *means_d, bool depth) {
   FusedZoomParams p;
   p.obs4 = obs4; p.ren4 = ren4;
   p.bbox8 = ctx->bbox8; p.zoom_factor = zoom_factor;
@@ -458,9 +484,36 @@ int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, cons
   p.stepy = (float)(2.0 / (double)(ctx->H - 1));
   p.hi = hi; p.lo = lo;
   dim3 grid(cdiv(Hs * Ws, 128), B);
-  if (f16) zoom_fused_nhwc8_kernel<false, true><<<grid, 128, 0, st>>>(p);  // zero bits are the same in both formats
-  else if (lo) zoom_fused_nhwc8_kernel<true, false><<<grid, 128, 0, st>>>(p);
-  else zoom_fused_nhwc8_kernel<false, false><<<grid, 128, 0, st>>>(p);
+  if (depth) {
+    if (f16) zoom_fused_nhwc8_kernel<false, true, true><<<grid, 128, 0, st>>>(p);
+    else if (lo) zoom_fused_nhwc8_kernel<true, false, true><<<grid, 128, 0, st>>>(p);
+    else zoom_fused_nhwc8_kernel<false, false, true><<<grid, 128, 0, st>>>(p);
+  } else if (f16) {
+    zoom_fused_nhwc8_kernel<false, true><<<grid, 128, 0, st>>>(p);  // zero bits are the same in both formats
+  } else if (lo) {
+    zoom_fused_nhwc8_kernel<true, false><<<grid, 128, 0, st>>>(p);
+  } else {
+    zoom_fused_nhwc8_kernel<false, false><<<grid, 128, 0, st>>>(p);
+  }
+  DIM_LAUNCH_CHECK();
+  return 0;
+}
+
+// RGB-D network: the observed depth into the w lanes of obs4 (constant over the iterations, like the image).  Device f32
+// depth in metres, or the loader's uint16 file values converted as lib/utils/image.py:203,218 does: float32(u16) /
+// float32(DEPTH_FACTOR) (a numpy float32 array divided by a Python float stays float32; IEEE division).
+__global__ void __launch_bounds__(256) obs4_depth_kernel(float4 *obs4, int P, const float *depth, const uint16_t *depth_u16,
+                                                         float factor) {
+  const int b = blockIdx.y;
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= P) return;
+  const size_t o = (size_t)b * P + q;
+  reinterpret_cast<float *>(obs4 + o)[3] = depth ? depth[o] : __fdiv_rn((float)depth_u16[o], factor);
+}
+int obs4_depth_launch(dim_ctx *ctx, float4 *obs4, int B, const float *depth, const uint16_t *depth_u16, float factor,
+                      cudaStream_t st) {
+  const int P = ctx->H * ctx->W;
+  obs4_depth_kernel<<<dim3(cdiv(P, 256), B), 256, 0, st>>>(obs4, P, depth, depth_u16, factor);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -518,6 +571,59 @@ int pack_nhwc8_launch(dim_ctx *ctx, const float *io, const float *ir, const floa
                       int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo, cudaStream_t st, int f16) {
   pack_nhwc8_kernel<<<dim3(cdiv(ctx->H * ctx->W, 256), B), 256, 0, st>>>(io, ir, mo, mr, ctx->H, ctx->W, Hs, Ws, pad,
                                                                          hi, f16 ? nullptr : lo, f16);
+  DIM_LAUNCH_CHECK();
+  return 0;
+}
+
+// NCHW float32 zoomed blobs + zoomed depths -> the RGB-D network's conv1 input (dim_net_fwd_rgbd): channels
+// io/255, ir/255, do/255, dr/255, mo, mr in two 8-channel chunks per space-to-depth phase
+__global__ void __launch_bounds__(256) pack_nhwc10_kernel(const float *io, const float *ir, const float *dobs,
+                                                          const float *dren, const float *mo, const float *mr, int H, int W,
+                                                          int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
+                                                          int f16) {
+  const int b = blockIdx.y;
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= H * W) return;
+  const size_t P = (size_t)H * W;
+  float v[16];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    v[c] = io[((size_t)b * 3 + c) * P + q] / 255.0f;
+    v[3 + c] = ir[((size_t)b * 3 + c) * P + q] / 255.0f;
+  }
+  v[6] = dobs[(size_t)b * P + q] / 255.0f;
+  v[7] = dren[(size_t)b * P + q] / 255.0f;
+  v[8] = mo[(size_t)b * P + q];
+  v[9] = mr[(size_t)b * P + q];
+#pragma unroll
+  for (int c = 10; c < 16; ++c) v[c] = 0.f;
+  const int oi = q / W + pad, oj = q % W + pad;
+  const int slot = (oi & 1) * 2 + (oj & 1);
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    __align__(16) __nv_bfloat16 h[8];
+    __align__(16) __nv_bfloat16 l[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) {
+      const float x = v[8 * half + c];
+      if (f16) {
+        reinterpret_cast<__half *>(h)[c] = __float2half_rn(x);
+      } else {
+        h[c] = __float2bfloat16_rn(x);
+        l[c] = __float2bfloat16_rn(x - __bfloat162float(h[c]));
+      }
+    }
+    const size_t o = ((((size_t)b * Hs + (oi >> 1)) * 8 + slot * 2 + half) * Ws + (oj >> 1)) * 8;
+    *reinterpret_cast<uint4 *>(hi + o) = *reinterpret_cast<const uint4 *>(h);
+    if (lo) *reinterpret_cast<uint4 *>(lo + o) = *reinterpret_cast<const uint4 *>(l);
+  }
+}
+
+int pack_nhwc10_launch(dim_ctx *ctx, const float *io, const float *ir, const float *dobs, const float *dren, const float *mo,
+                       const float *mr, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo, cudaStream_t st,
+                       int f16) {
+  pack_nhwc10_kernel<<<dim3(cdiv(ctx->H * ctx->W, 256), B), 256, 0, st>>>(io, ir, dobs, dren, mo, mr, ctx->H, ctx->W, Hs, Ws,
+                                                                          pad, hi, f16 ? nullptr : lo, f16);
   DIM_LAUNCH_CHECK();
   return 0;
 }

@@ -67,6 +67,14 @@ SIGNATURES = {
     "dim_refine_host_lit_async": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, C.POINTER(Lighting), vp]),
     "dim_train_update_lit": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, pf64, f32, f32, pf64, pf64, pf64, i32, vp, vp, vp, vp, vp,
                                    vp, vp, vp, C.POINTER(Lighting), vp]),
+    "dim_ctx_set_input_depth": (i32, [vp, i32]),
+    "dim_refine_rgbd": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, vp,
+                              C.POINTER(Lighting), vp]),
+    "dim_refine_host_rgbd": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32,
+                                   C.POINTER(Lighting), vp]),
+    "dim_refine_host_rgbd_async": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32,
+                                         C.POINTER(Lighting), vp]),
+    "dim_net_fwd_rgbd": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp]),
     "dim_transform_image_u8": (i32, [vp, vp, i32, pf64, vp, vp]),
     "dim_debug_activation": (i32, [vp, i32, i32, vp, u64]),
     "dim_debug_layer_geometry": (i32, [vp, i32, C.POINTER(i32)]),
@@ -85,6 +93,8 @@ SIGNATURES = {
     "dim_train_load_params": (i32, [vp, vp, i64, vp]),
     "dim_train_get_params": (i32, [vp, vp, i64, i32, vp]),
     "dim_train_forward_backward": (i32, [vp] + [vp] * 12 + [i32, i32] + [vp] * 7 + [vp, vp, i32] + [vp]),
+    "dim_train_param_info_rgbd": (i32, [i32, C.POINTER(C.c_char_p), C.POINTER(i64), C.POINTER(i64)]),
+    "dim_train_forward_backward_rgbd": (i32, [vp] + [vp] * 12 + [i32, i32] + [vp] * 7 + [vp, vp, i32] + [vp, vp] + [vp]),
     "dim_train_set_config": (i32, [vp, C.POINTER(TrainConfig)]),
     "dim_train_get_config": (i32, [vp, C.POINTER(TrainConfig)]),
     "dim_train_sgd_update": (i32, [vp, vp, f32, f32, f32, f32, vp]),

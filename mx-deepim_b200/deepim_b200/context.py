@@ -63,7 +63,10 @@ def _lighting_arg(lighting, shape, on_device):
 
 class Context:
     def __init__(self, device=0, max_batch=16, height=480, width=640, max_classes=16, max_verts=60000,
-                 max_faces=120000):
+                 max_faces=120000, input_depth=False):
+        """input_depth=True: the RGB-D network (config.network.INPUT_DEPTH, deepIM_flownet.py:33-51).  Its input gains
+        depth_observed/255 and depth_rendered/255 as channels 6 and 7, so flow_conv1_weight is (64, 10, 7, 7); refine /
+        refine_host then need the observed depth and net_forward the zoomed depths.  Training it is not supported."""
         if not torch.cuda.is_available():
             raise capi.DeepIMError("deepim_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
@@ -73,6 +76,9 @@ class Context:
         check(lib.dim_ctx_create(device, max_batch, height, width, max_classes, max_verts, max_faces, C.byref(h)))
         self._h = h
         self.num_classes = 0
+        self.input_depth = bool(input_depth)
+        if self.input_depth:
+            check(lib.dim_ctx_set_input_depth(h, 1))
 
     def _stream(self):
         """torch's current stream OF THIS CONTEXT'S DEVICE (a process may hold contexts on several GPUs)"""
@@ -108,6 +114,12 @@ class Context:
     def load_weights(self, weights: dict):
         """weights: name_weight / name_bias float32 arrays with MXNet layouts
         (deepim/symbols/deepIM_flownet.py:63-116,716-717)."""
+        shape = tuple(np.shape(weights["flow_conv1_weight"]))
+        want = (64, 10 if self.input_depth else 8, 7, 7)
+        if shape != want:
+            raise ValueError("flow_conv1_weight has shape %s: this context's network takes %s (Context(input_depth=%s)); "
+                             "(64, 8, 7, 7) belongs to Context(input_depth=False), (64, 10, 7, 7) to Context(input_depth=True)"
+                             % (shape, want, self.input_depth))
         keep = []
         W = (C.c_void_p * 14)()
         Bv = (C.c_void_p * 14)()
@@ -348,11 +360,21 @@ class Context:
 
     # --------------------------------------------------------------------------------- net
     def net_forward(self, zoom_image_observed, zoom_image_rendered, zoom_mask_observed, zoom_mask_rendered,
-                    precision=capi.PREC_BF16X3):
+                    precision=capi.PREC_BF16X3, zoom_depth_observed=None, zoom_depth_rendered=None):
+        """The network on already-zoomed blobs; an RGB-D context (input_depth=True) also takes the zoomed depths
+        f32 [B,1,H,W] (metres)."""
         B = zoom_image_observed.shape[0]
         rot, trans = self._new((B, 4)), self._new((B, 3))
-        check(lib.dim_net_fwd(self._h, _p(zoom_image_observed), _p(zoom_image_rendered), _p(zoom_mask_observed),
-                              _p(zoom_mask_rendered), B, precision, _p(rot), _p(trans), self._stream()))
+        if zoom_depth_observed is None and zoom_depth_rendered is None:
+            check(lib.dim_net_fwd(self._h, _p(zoom_image_observed), _p(zoom_image_rendered), _p(zoom_mask_observed),
+                                  _p(zoom_mask_rendered), B, precision, _p(rot), _p(trans), self._stream()))
+            return rot, trans
+        shp = (B, 1, self.H, self.W)
+        _chk(zoom_depth_observed, torch.float32, shp, "zoom_depth_observed")
+        _chk(zoom_depth_rendered, torch.float32, shp, "zoom_depth_rendered")
+        check(lib.dim_net_fwd_rgbd(self._h, _p(zoom_image_observed), _p(zoom_image_rendered), _p(zoom_depth_observed),
+                                   _p(zoom_depth_rendered), _p(zoom_mask_observed), _p(zoom_mask_rendered), B, precision,
+                                   _p(rot), _p(trans), self._stream()))
         return rot, trans
 
     def debug_activation(self, idx, B, lo=False, fp16=False):
@@ -396,13 +418,14 @@ class Context:
 
     def refine(self, image_observed, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
                pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, pose_override=None, out=None,
-               lighting=None):
+               lighting=None, depth_observed=None):
         """Device-resident fused loop.  image_observed f32[B,3,H,W], cls_idx i32[B], pose_init f64[B,3,4].
         out = the dict returned by an earlier call with the same shapes: results are written into those tensors again
         (same device addresses -> the library replays its CUDA graph of the chain instead of re-enqueuing ~90 launches).
         lighting: None = the unlit loop (LINEMOD); a dict {intensity float32 [n_iter,B,3] CUDA, offset, brightness_ratio}
         = the ModelNet branch's lit loop (see deepim_b200.lighting).  Reusing the same intensity tensor lets the lit chain
-        replay its graph as well."""
+        replay its graph as well.
+        depth_observed: f32 [B,1,H,W] CUDA, metres -- required on an RGB-D context (input_depth=True), refused otherwise."""
         B = image_observed.shape[0]
         _chk(image_observed, torch.float32, (B, 3, self.H, self.W), "image_observed")
         _chk(cls_idx, torch.int32, (B,), "cls_idx")
@@ -423,21 +446,27 @@ class Context:
         args = (self._h, _p(image_observed), _p(cls_idx), _p(pose_init), B, n_iter,
                 farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
                 farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses), _p(se3), _p(zf), _p(bbox))
-        if lighting is None:
+        lit = None if lighting is None else _lighting_arg(lighting, (n_iter, B, 3), True)[0]
+        if depth_observed is not None:
+            _chk(depth_observed, torch.float32, (B, 1, self.H, self.W), "depth_observed")
+            check(lib.dim_refine_rgbd(*args, _p(depth_observed), None if lit is None else C.byref(lit), self._stream()))
+        elif lit is None:
             check(lib.dim_refine(*args, self._stream()))
         else:
-            lit, _ = _lighting_arg(lighting, (n_iter, B, 3), True)
             check(lib.dim_refine_lit(*args, C.byref(lit), self._stream()))
         return {"poses": poses, "se3": se3, "zoom_factor": zf, "bbox": bbox}
 
     def refine_host(self, image_observed_u8, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
                     pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, poses_out=None,
-                    se3_out=None, sync=True, lighting=None):
+                    se3_out=None, sync=True, lighting=None, depth_observed_u16=None, depth_factor=1000.0):
         """Host-buffer entry (what a tester loop calls): uint8 BGR HWC images (pinned torch tensors or
         numpy), host poses in / out.  sync=False only enqueues on the current torch stream (outputs must
         then be pinned and are valid after the stream is synchronised).
         lighting: as refine() but with a HOST intensity array float32 [n_iter,B,3] (copied before the call returns,
-        unless it is pinned: then it must stay untouched until the stream is synchronised)."""
+        unless it is pinned: then it must stay untouched until the stream is synchronised).
+        depth_observed_u16: RGB-D context only, host uint16 [B,H,W] depth file values (the *-depth.png of the observed
+        frame); the device converts them as the reference's loader does, float32(u16) / float32(depth_factor).  With
+        sync=False a pinned depth array is copied asynchronously too: keep it untouched until the stream is synchronised."""
         def hptr(a):
             return C.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else C.c_void_p(a.ctypes.data)
         B = image_observed_u8.shape[0]
@@ -448,7 +477,20 @@ class Context:
         args = (self._h, hptr(image_observed_u8), hptr(cls_idx), hptr(pose_init), B, n_iter,
                 farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
                 farr(pixel_means_rgb, 3, C.c_double), precision, hptr(poses_out), hptr(se3_out))
-        if lighting is None:
+        if depth_observed_u16 is not None:
+            if isinstance(depth_observed_u16, torch.Tensor):
+                if depth_observed_u16.is_cuda or depth_observed_u16.dtype != torch.uint16:
+                    raise ValueError("depth_observed_u16 must be a host uint16 array")
+                dkeep = depth_observed_u16.contiguous()
+            else:
+                dkeep = np.ascontiguousarray(depth_observed_u16, np.uint16)
+            if tuple(dkeep.shape) != (B, self.H, self.W):
+                raise ValueError("depth_observed_u16: expected shape %s, got %s" % ((B, self.H, self.W), tuple(dkeep.shape)))
+            lit, _keep = (None, None) if lighting is None else _lighting_arg(lighting, (n_iter, B, 3), False)
+            fn = lib.dim_refine_host_rgbd if sync else lib.dim_refine_host_rgbd_async
+            check(fn(*args, hptr(dkeep), float(np.float32(depth_factor)), None if lit is None else C.byref(lit),
+                     self._stream()))
+        elif lighting is None:
             fn = lib.dim_refine_host if sync else lib.dim_refine_host_async
             check(fn(*args, self._stream()))
         else:

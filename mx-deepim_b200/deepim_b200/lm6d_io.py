@@ -109,11 +109,16 @@ def write_pose(path, cls_idx, pose):
             f.write(" ".join("%.10g" % x for x in r) + "\n")
 
 
-def read_depth(path):
+def read_depth_u16(path):
+    """The depth file's uint16 values (metres * DEPTH_FACTOR)."""
     d = _cv2().imread(path, _cv2().IMREAD_UNCHANGED)
     if d is None:
         raise FileNotFoundError(path)
-    return d.astype(np.float32) / np.float32(DEPTH_FACTOR)
+    return d
+
+
+def read_depth(path):
+    return read_depth_u16(path).astype(np.float32) / np.float32(DEPTH_FACTOR)
 
 
 def write_depth(path, depth_m):
@@ -165,16 +170,19 @@ class LM6DRefine:
 
 
 def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl", "cup"), n_iter=4, max_batch=16, device=0,
-             precision="fp16"):
+             precision="fp16", input_depth=False):
     """Batched pred_eval (deepim/core/tester.py:50-527 without its batch = 1 limit): refine every pair of the image set
     and score it the way the reference's dataset class does: ADD / ADI accuracy + AUC (evaluate_pose_add), 5 cm 5 deg
     (evaluate_pose) and Proj. 2D (evaluate_pose_arp_2d); the last two under res["rot_trans"] / res["arp_2d"].
+    input_depth=True refines with the RGB-D network (weights with a (64, 10, 7, 7) flow_conv1) and reads each observed frame's
+    `-depth.png` as well (image.py:190-219; converted on the device with DEPTH_FACTOR).
     Returns (evaluate_pose_add result + the two extra tables, poses_est [n_iter,M,3,4], poses_gt)."""
     from . import pose_eval
     from .refiner import PoseRefiner
     meshes = [dataset.mesh(c) for c in dataset.classes]
-    ref = PoseRefiner(meshes, weights, K=K, device=device, max_batch=max_batch, n_iter=n_iter, precision=precision)
-    imgs, cls_idx, init, gt = [], [], [], []
+    ref = PoseRefiner(meshes, weights, K=K, device=device, max_batch=max_batch, n_iter=n_iter, precision=precision,
+                      input_depth=input_depth, depth_factor=DEPTH_FACTOR)
+    imgs, cls_idx, init, gt, depths = [], [], [], [], []
     for ci, c in enumerate(dataset.classes):
         for pair in dataset.pairs(c):
             rec = dataset.load_pair(c, pair)
@@ -182,9 +190,11 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
             cls_idx.append(ci)
             init.append(rec["pose_rendered"])
             gt.append(rec["pose_observed"])
+            if input_depth:
+                depths.append(read_depth_u16(os.path.join(dataset.root, "data", "observed", pair[0] + "-depth.png")))
     imgs, cls_idx = np.stack(imgs), np.asarray(cls_idx, np.int32)
     init, gt = np.stack(init).astype(np.float64), np.stack(gt).astype(np.float64)
-    poses = ref.refine(imgs, cls_idx, init)
+    poses = ref.refine(imgs, cls_idx, init, depths_u16=np.stack(depths).astype(np.uint16) if input_depth else None)
     res = pose_eval.evaluate_pose_add(ref.ctx, poses, gt, cls_idx, [dataset.points(c) for c in dataset.classes],
                                       [dataset.diameters[c] for c in dataset.classes], [c in symmetric for c in dataset.classes])
     pts_all = [dataset.points(c) for c in dataset.classes]

@@ -128,6 +128,17 @@ def save_checkpoint(prefix, epoch, arg_params, aux_params=None):
     save("%s-%04d.params" % (prefix, epoch), d)
 
 
+def input_depth_of(arg_params) -> bool:
+    """Which network a checkpoint belongs to, from its flow_conv1_weight: (64, 8, 7, 7) = RGB (INPUT_MASK), (64, 10, 7, 7) =
+    RGB-D (INPUT_DEPTH + INPUT_MASK, deepIM_flownet.py:33-51).  Anything else raises ValueError."""
+    shape = tuple(np.shape(arg_params["flow_conv1_weight"]))
+    if shape == (64, 8, 7, 7):
+        return False
+    if shape == (64, 10, 7, 7):
+        return True
+    raise ValueError("flow_conv1_weight has shape %s: expected (64, 8, 7, 7) (RGB) or (64, 10, 7, 7) (RGB-D)" % (shape,))
+
+
 # ----------------------------------------------------------------------------------------- <prefix>-symbol.json
 # MXNet writes the network graph next to the checkpoint (`Module.save_checkpoint` -> `<prefix>-symbol.json`): a JSON object
 # {"nodes": [{"op": "null" | "<Operator>", "name": ..., "attrs" (>= 1.0) | "attr" | "param" (older): {str: str},

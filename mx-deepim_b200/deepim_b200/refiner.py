@@ -8,7 +8,11 @@ the kernels of batch k (instances are independent; nothing else is shared but re
 
 lighting={"seed", "offset", "brightness_ratio"} runs the ModelNet branch's lit loop (deepim_b200.lighting): every mesh must
 carry `normals`, and each submit draws its light intensities [n_iter, n, 3] from one Generator seeded once
-(lighting.sample_intensity), the fresh draw per render of the reference."""
+(lighting.sample_intensity), the fresh draw per render of the reference.
+
+input_depth=True runs the RGB-D network (config.network.INPUT_DEPTH; weights with a (64, 10, 7, 7) flow_conv1): submit /
+refine then also take the observed depth as the loader's uint16 file values [N,H,W] (LINEMOD's *-depth.png), converted on the
+device as float32(u16) / float32(depth_factor)."""
 from __future__ import annotations
 
 import numpy as np
@@ -23,7 +27,7 @@ from .context import Context
 class PoseRefiner:
     def __init__(self, meshes, weights, K=synth.K_LINEMOD, device=0, max_batch=16, n_iter=4,
                  pixel_means_rgb=synth.PIXEL_MEANS_RGB, znear=synth.ZNEAR, zfar=synth.ZFAR, precision="fp16",
-                 n_slots=2, lighting=None):
+                 n_slots=2, lighting=None, input_depth=False, depth_factor=1000.0):
         self.light = _lighting.LightSource.of(lighting)
         if self.light is not None:
             for i, m in enumerate(meshes):
@@ -35,9 +39,11 @@ class PoseRefiner:
         mv = max(len(m.verts) for m in meshes)
         mf = max(len(m.faces) for m in meshes)
         self.max_batch = max_batch
+        self.input_depth, self.depth_factor = bool(input_depth), float(depth_factor)
         self.slots = []
         for _ in range(n_slots):
-            ctx = Context(device, max_batch=max_batch, max_classes=len(meshes), max_verts=mv, max_faces=mf)
+            ctx = Context(device, max_batch=max_batch, max_classes=len(meshes), max_verts=mv, max_faces=mf,
+                          input_depth=self.input_depth)
             for i, m in enumerate(meshes):
                 ctx.upload_mesh(i, m)
             ctx.load_weights(weights)
@@ -46,7 +52,7 @@ class PoseRefiner:
                 "poses": torch.empty((n_iter, max_batch, 3, 4), dtype=torch.float64).pin_memory(),
                 "se3": torch.empty((n_iter, max_batch, 7), dtype=torch.float32).pin_memory(),
                 "status": torch.zeros((min(n_iter, 8) * max_batch,), dtype=torch.int32).pin_memory(),
-                "img": None, "cls": None, "pose": None,
+                "img": None, "cls": None, "pose": None, "depth": None,
                 "intensity": torch.empty((n_iter, max_batch, 3), dtype=torch.float32).pin_memory() if self.light else None,
             })
         self.ctx = self.slots[0]["ctx"]
@@ -66,8 +72,9 @@ class PoseRefiner:
         buf[: t.shape[0]].copy_(t)
         return buf[: t.shape[0]]
 
-    def submit(self, images_bgr_u8, cls_idx, poses_init):
+    def submit(self, images_bgr_u8, cls_idx, poses_init, depths_u16=None):
         """Enqueue one batch (<= max_batch instances, host arrays; pinned torch tensors are used in place).
+        depths_u16: uint16 [n,H,W], required with input_depth=True.
         Returns a ticket for result().  At most len(slots) batches may be in flight."""
         i = self._next
         slot = self.slots[i]
@@ -79,6 +86,10 @@ class PoseRefiner:
         img = self._pinned(slot, "img", images_bgr_u8, torch.uint8)
         cls = self._pinned(slot, "cls", cls_idx, torch.int32)
         pose = self._pinned(slot, "pose", poses_init, torch.float64)
+        if (depths_u16 is not None) != self.input_depth:
+            raise ValueError("PoseRefiner(input_depth=%s): depths_u16 %s" % (self.input_depth,
+                             "is required" if self.input_depth else "belongs to PoseRefiner(input_depth=True)"))
+        depth = None if depths_u16 is None else self._pinned(slot, "depth", depths_u16, torch.uint16)
         lit = None
         if self.light is not None:  # a fresh draw per render; the pinned buffer lives until result() of this slot
             inten = slot["intensity"].view(-1)[: self.n_iter * n * 3].view(self.n_iter, n, 3)
@@ -86,7 +97,8 @@ class PoseRefiner:
             lit = self.light.lighting(inten)
         with torch.cuda.stream(slot["stream"]):
             slot["ctx"].refine_host(img, cls, pose, self.K, self.n_iter, self.zn, self.zf, self.means, self.precision,
-                                    poses_out=slot["poses"], se3_out=slot["se3"], sync=False, lighting=lit)
+                                    poses_out=slot["poses"], se3_out=slot["se3"], sync=False, lighting=lit,
+                                    depth_observed_u16=depth, depth_factor=self.depth_factor)
             slot["ctx"].refine_status(n, self.n_iter, out=slot["status"], sync=False)
         slot["busy"], slot["n"] = True, n
         self._next = (i + 1) % len(self.slots)
@@ -113,8 +125,9 @@ class PoseRefiner:
         return p.numpy().copy()
 
     # ------------------------------------------------------------------------------ convenience
-    def refine(self, images_bgr_u8, cls_idx, poses_init, dist=None):
-        """images_bgr_u8 [N,H,W,3] uint8 (cv2 layout), cls_idx [N] int, poses_init [N,3,4] float64 (host).
+    def refine(self, images_bgr_u8, cls_idx, poses_init, dist=None, depths_u16=None):
+        """images_bgr_u8 [N,H,W,3] uint8 (cv2 layout), cls_idx [N] int, poses_init [N,3,4] float64 (host); depths_u16 [N,H,W]
+        uint16 with input_depth=True.
         Returns poses [n_iter,N,3,4] float64 (host).  With torch.distributed initialised each rank
         processes its contiguous slice and the poses are all-gathered."""
         n = len(cls_idx)
@@ -126,7 +139,8 @@ class PoseRefiner:
             if len(pending) == len(self.slots):
                 t, (pa, pb) = pending.pop(0)
                 out[:, pa - lo:pb - lo] = self.result(t)
-            pending.append((self.submit(images_bgr_u8[a:b], cls_idx[a:b], poses_init[a:b]), (a, b)))
+            d = None if depths_u16 is None else depths_u16[a:b]
+            pending.append((self.submit(images_bgr_u8[a:b], cls_idx[a:b], poses_init[a:b], d), (a, b)))
         for t, (pa, pb) in pending:
             out[:, pa - lo:pb - lo] = self.result(t)
         return sharding.gather_results(out, n, axis=1, dist=dist, device=self.ctx.device if world > 1 else None)

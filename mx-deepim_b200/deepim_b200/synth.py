@@ -206,7 +206,18 @@ def conv_out_hw(h, w, k, s, p):
     return (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
 
 
-def make_weights(seed: int = 0):
+def with_depth_channels(weights: dict, depth_weight=None):
+    """An 8-channel weight set as the RGB-D network's (config.network.INPUT_DEPTH): flow_conv1_weight (64, 8, 7, 7) ->
+    (64, 10, 7, 7) with the depth columns (channels 6, 7: depth_observed, depth_rendered) inserted before the two mask
+    channels; depth_weight (64, 2, 7, 7), zeros when None (the network then computes what the RGB one does)."""
+    w = dict(weights)
+    c1 = np.asarray(weights["flow_conv1_weight"], np.float32)
+    d = np.zeros((c1.shape[0], 2) + c1.shape[2:], np.float32) if depth_weight is None else np.asarray(depth_weight, np.float32)
+    w["flow_conv1_weight"] = np.ascontiguousarray(np.concatenate([c1[:, :6], d, c1[:, 6:]], axis=1))
+    return w
+
+
+def make_weights(seed: int = 0, input_depth: bool = False):
     """Random-init weights (dict name -> float32 array) with MXNet shapes
     (Convolution (Cout,Cin,kh,kw); FullyConnected (out,in), SURVEY App.B-22).
     He-normal convs (LeakyReLU 0.1 gain), small random biases, Xavier fc6/fc7; rot head biased to
@@ -232,6 +243,10 @@ def make_weights(seed: int = 0):
     w["fc7_bias"] = (rng.standard_normal((256,), dtype=np.float32) * np.float32(0.02))
     w["rot_bias"] = np.array([1.0, 0.02, -0.03, 0.015], dtype=np.float32)
     w["trans_bias"] = np.array([0.01, -0.015, 0.02], dtype=np.float32)
+    if input_depth:  # the 8-channel set plus He-normal depth columns (fan-in of the 10-channel conv1) from a separate stream
+        drng = np.random.default_rng(seed + 7919)
+        std = gain / np.sqrt(10 * 7 * 7)
+        w = with_depth_channels(w, drng.standard_normal((64, 2, 7, 7), dtype=np.float32) * np.float32(std))
     return w
 
 
@@ -251,11 +266,11 @@ def bilinear_upsampling_kernel(k: int = 32) -> np.ndarray:
     return np.outer(v, v).astype(np.float32)
 
 
-def make_train_weights(seed: int = 0):
+def make_train_weights(seed: int = 0, input_depth: bool = False):
     """make_weights + the train-only decoder / flow / mask heads (deepIM_flownet.py:121-167,176-193,317-338):
     He-normal decoder convs/deconvs (a k4 s2 deconv sums Cin*4 taps per output), N(0, 0.01) mask_conv3
     (init_weights l.811-813), frozen bilinear `upsampling` (2 groups) / `mask_upsampling` kernels."""
-    w = make_weights(seed)
+    w = make_weights(seed, input_depth)
     rng = np.random.default_rng(seed + 1000003)
     gain = np.sqrt(2.0 / (1.0 + 0.1 ** 2))
     for name, kind, shp, nb in DECODER_SPECS:

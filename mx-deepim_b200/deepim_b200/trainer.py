@@ -19,12 +19,21 @@ from ._capi import check, lib
 NORMALIZE_FLOW = 20.0
 
 
-def param_table():
-    """[(tensor name, numel)] in flat order, as the library reports it (dim_train_param_info)."""
+def _param_info(input_depth):
+    return lib.dim_train_param_info_rgbd if input_depth else lib.dim_train_param_info
+
+
+def _is_rgbd(weights) -> bool:
+    return np.shape(weights["flow_conv1_weight"])[1:2] == (10,)
+
+
+def param_table(input_depth=False):
+    """[(tensor name, numel)] in flat order, as the library reports it (dim_train_param_info; input_depth: the RGB-D
+    network's table, dim_train_param_info_rgbd, whose flow_conv1 is (64, 10, 7, 7))."""
     out = []
     for i in range(64):
         name, wn, bn = C.c_char_p(), C.c_int64(), C.c_int64()
-        if lib.dim_train_param_info(i, C.byref(name), C.byref(wn), C.byref(bn)) != 0:
+        if _param_info(input_depth)(i, C.byref(name), C.byref(wn), C.byref(bn)) != 0:
             break
         out.append((name.value.decode() + "_weight", wn.value))
         if bn.value:
@@ -33,8 +42,9 @@ def param_table():
 
 
 def flatten_params(weights: dict) -> np.ndarray:
+    """The flat vector of the table the weights belong to (RGB-D when flow_conv1_weight has 10 input channels)."""
     parts = []
-    for name, n in param_table():
+    for name, n in param_table(_is_rgbd(weights)):
         a = np.asarray(weights[name], dtype=np.float32)
         if name == "fc6_weight":  # the flat vector keeps fc6 as (out, h*10+w, c): NHWC order of the conv6_1 activation
             a = a.reshape(256, 1024, 80).transpose(0, 2, 1)
@@ -47,7 +57,7 @@ def flatten_params(weights: dict) -> np.ndarray:
 
 def unflatten_params(flat: np.ndarray, like: dict) -> dict:
     out, off = {}, 0
-    for name, n in param_table():
+    for name, n in param_table(_is_rgbd(like)):
         a = np.asarray(flat[off:off + n], np.float32)
         if name == "fc6_weight":  # back to MXNet's (out, c*80 + h*10 + w) (deepIM_flownet.py:110-112)
             a = a.reshape(256, 80, 1024).transpose(0, 2, 1)
@@ -56,12 +66,12 @@ def unflatten_params(flat: np.ndarray, like: dict) -> dict:
     return out
 
 
-def tensor_sizes():
+def tensor_sizes(input_depth=False):
     """[(table index, weight + bias numel)] of the tensors of the flat vector (dim_train_param_info order)."""
     out = []
     for i in range(64):
         nm, wn, bn = C.c_char_p(), C.c_int64(), C.c_int64()
-        if lib.dim_train_param_info(i, C.byref(nm), C.byref(wn), C.byref(bn)) != 0:
+        if _param_info(input_depth)(i, C.byref(nm), C.byref(wn), C.byref(bn)) != 0:
             break
         out.append((i, wn.value + bn.value))
     return out
@@ -98,18 +108,22 @@ class Trainer:
         normalize_3d_point, normalize_flow, trans_means, trans_stds, rot_coord = 'MODEL' | 'CAMERA'): the yaml's train.LW_* /
         NUM_3D_SAMPLE / NORMALIZE_* / network.TRANS_MEANS / TRANS_STDS / ROT_COORD.  Default: the shipped LM6d values."""
         self.ctx, self.lr, self.momentum, self.wd = ctx, lr, momentum, wd
+        self.input_depth = bool(getattr(ctx, "input_depth", False))  # Context(input_depth=True): the RGB-D network
+        if _is_rgbd(weights) != self.input_depth:
+            raise ValueError("flow_conv1_weight has %d input channels; this context's network takes %d"
+                             % (np.shape(weights["flow_conv1_weight"])[1], 10 if self.input_depth else 8))
         check(lib.dim_train_create(ctx._h, max_points))
         if config:
             ctx.set_config(**config)
         self.n = int(lib.dim_train_param_count(ctx._h))
-        self.table = param_table()
+        self.table = param_table(self.input_depth)
         flat = flatten_params(weights)
         assert flat.size == self.n
         self._shapes = {k: np.asarray(v).shape for k, v in weights.items()}
         check(lib.dim_train_load_params(ctx._h, flat.ctypes.data_as(C.c_void_p), self.n, self._stream()))
         torch.cuda.current_stream(ctx.device).synchronize()
         self.grads = torch.zeros(self.n, dtype=torch.float32, device=ctx.device)
-        self.buckets, self.bucket_first = make_buckets(bucket_mb)
+        self.buckets, self.bucket_first = make_buckets(bucket_mb, tensor_sizes(self.input_depth))
         self._events = None
         self._comm_stream = None
 
@@ -137,7 +151,7 @@ class Trainer:
         """z: dict of device float32 tensors (the outputs of the zoom front of the train symbol + labels):
         zoom_image_observed/rendered (B,3,H,W), zoom_mask_observed/rendered (B,1,H,W), zoom_factor (B,4),
         zoom_flow, zoom_flow_weights (B,2,H,W), zoom_mask_gt_observed (B,1,H,W), src_pose (B,3,4),
-        point_cloud_model/weights/observed (B,3,N)."""
+        point_cloud_model/weights/observed (B,3,N); RGB-D network: also zoom_depth_observed / zoom_depth_rendered (B,1,H,W)."""
         ctx = self.ctx
         B, N = z["zoom_image_observed"].shape[0], z["point_cloud_model"].shape[2]
         for k, t in z.items():
@@ -146,13 +160,17 @@ class Trainer:
         out = {"rot_est_norm": ctx._new((B, 4)), "trans_est": ctx._new((B, 3)), "losses": ctx._new((4,)),
                "flow_est": ctx._new((B, 2, ctx.H, ctx.W)) if want_maps else None,
                "mask_prob": ctx._new((B, 1, ctx.H, ctx.W)) if want_maps else None}
-        check(lib.dim_train_forward_backward(
-            ctx._h, _p(z["zoom_image_observed"]), _p(z["zoom_image_rendered"]), _p(z["zoom_mask_observed"]),
-            _p(z["zoom_mask_rendered"]), _p(z["zoom_factor"]), _p(z["zoom_flow"]), _p(z["zoom_flow_weights"]),
-            _p(z["zoom_mask_gt_observed"]), _p(z["src_pose"]), _p(z["point_cloud_model"]), _p(z["point_cloud_weights"]),
-            _p(z["point_cloud_observed"]), B, N, _p(out["rot_est_norm"]), _p(out["trans_est"]), _p(out["flow_est"]),
-            _p(out["mask_prob"]), _p(out["losses"]), _p(self.grads) if backward else None, None,
-            *((self._bucket_events() + (len(self.buckets),)) if (backward and overlap) else (None, None, 0)), self._stream()))
+        args = (ctx._h, _p(z["zoom_image_observed"]), _p(z["zoom_image_rendered"]), _p(z["zoom_mask_observed"]),
+                _p(z["zoom_mask_rendered"]), _p(z["zoom_factor"]), _p(z["zoom_flow"]), _p(z["zoom_flow_weights"]),
+                _p(z["zoom_mask_gt_observed"]), _p(z["src_pose"]), _p(z["point_cloud_model"]), _p(z["point_cloud_weights"]),
+                _p(z["point_cloud_observed"]), B, N, _p(out["rot_est_norm"]), _p(out["trans_est"]), _p(out["flow_est"]),
+                _p(out["mask_prob"]), _p(out["losses"]), _p(self.grads) if backward else None, None,
+                *((self._bucket_events() + (len(self.buckets),)) if (backward and overlap) else (None, None, 0)))
+        if self.input_depth:
+            check(lib.dim_train_forward_backward_rgbd(*args, _p(z["zoom_depth_observed"]), _p(z["zoom_depth_rendered"]),
+                                                      self._stream()))
+        else:
+            check(lib.dim_train_forward_backward(*args, self._stream()))
         return out
 
     def test_forward_full(self, batch, K):
@@ -215,7 +233,11 @@ class Trainer:
                                           batch["src_pose"], K)
         zio, zir = ctx.zoom_image_with_factor(zf, batch["image_observed"], batch["image_rendered"], batch["pixel_means_rgb"])
         zfl, zfw = ctx.zoom_flow(zf, batch["flow"], batch["flow_weights"], False)
-        return {"zoom_image_observed": zio, "zoom_image_rendered": zir, "zoom_mask_observed": zo, "zoom_mask_rendered": zr,
+        zd = {}
+        if self.input_depth:  # ZoomDepth with the pair's zoom factor (deepIM_flownet.py:461-475)
+            zdo, zdr = ctx.zoom_depth(zf, batch["depth_observed"], batch["depth_rendered"])
+            zd = {"zoom_depth_observed": zdo, "zoom_depth_rendered": zdr}
+        return {**zd, "zoom_image_observed": zio, "zoom_image_rendered": zir, "zoom_mask_observed": zo, "zoom_mask_rendered": zr,
                 "zoom_factor": zf, "zoom_flow": zfl, "zoom_flow_weights": zfw, "zoom_mask_gt_observed": zg,
                 "src_pose": batch["src_pose"], "point_cloud_model": batch["point_cloud_model"],
                 "point_cloud_weights": batch["point_cloud_weights"], "point_cloud_observed": batch["point_cloud_observed"]}
@@ -248,7 +270,7 @@ class Trainer:
 
 
 def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000, init_mask="box_gt", poses=None,
-                      image_observed=None, cls_np=None, lighting=None):
+                      image_observed=None, cls_np=None, lighting=None, input_depth=False):
     """Synthetic training batch built with the device kernels only (config C4: rendered pairs, labels from
     dim_train_update, INIT_MASK box_gt without dilation, 3000 sampled model points as get_point_cloud_model,
     lib/utils/image.py:452-478).  init_mask = "box_gt" (the reference's training config: mask_observed = box of the GT mask)
@@ -258,6 +280,8 @@ def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000,
     lighting = None (LINEMOD) or the ModelNet branch's light ({"seed", "offset", "brightness_ratio"} or a
     lighting.LightSource; the meshes' normals must be uploaded to ctx): the observed and the rendered images are lit renders,
     each with a fresh intensity draw.
+    input_depth = True adds the RGB-D network's blobs: depth_observed = the observed render's depth, depth_rendered = the
+    update's render depth (refined_depth_array, batch_updater_py_multi.py:269).
     Returns (batch dict of CUDA tensors, cls int32[B], tgt_pose f32[B,3,4], depth_gt)."""
     from . import synth
     obs, ini = synth.sample_pose_pairs(B, seed) if poses is None else poses
@@ -290,6 +314,8 @@ def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000,
              "flow_weights": upd["flow_weights"], "point_cloud_model": torch.from_numpy(pts).to(dev),
              "point_cloud_weights": torch.from_numpy(pw).to(dev), "point_cloud_observed": torch.from_numpy(pobs).to(dev),
              "pixel_means_rgb": np.asarray(pixel_means_rgb, np.float32)}
+    if input_depth:
+        batch["depth_observed"], batch["depth_rendered"] = r["depth"], upd["depth_rendered"]
     return batch, cls, tgt, r["depth"]
 
 
@@ -318,6 +344,8 @@ def fit_batch(trainer, batch, cls, tgt_pose, depth_gt, K, n_inner=4, dist=None, 
                                    lighting=_device_lighting(light, cls.shape[0], ctx.device))
             for k in ("image_rendered", "mask_rendered", "src_pose", "flow", "flow_weights"):
                 b[k] = upd[k]
+            if trainer.input_depth:  # the RGB-D network also sees the re-render's depth
+                b["depth_rendered"] = upd["depth_rendered"]
             if update_mask == "box_rendered":  # what update_data_batch does at test time (data_pair.py:93-105); the reference's
                 # training loop keeps mask_observed fixed (batch_updater_py_multi.py:267-301)
                 rb = ctx.render(cls, upd["src_pose"], K, pixel_means_rgb=batch["pixel_means_rgb"], want=("mask",))["bbox"]
