@@ -36,6 +36,11 @@ struct ConvKParams {
   CUtensorMap a_lo_map[4];  // activation views (lo), SPLIT3 only
   CUtensorMap b_map;        // weights hi (fp16 pack in F16 mode)
   CUtensorMap b_lo_map;     // weights lo
+  // conv1_kernel only: output store maps (hi, lo) over the INTERIOR of the next layer's bordered buffer, box = 64 ch x
+  // kConv1StoreN px, SW128; and the space-to-depth input it reads with plain bulk copies ([rows][4 chunks][in_cols][8 ch])
+  CUtensorMap out_map[2];
+  const __nv_bfloat16 *in_hi, *in_lo;
+  int in_cols;
   int KH, KW, stride, cchunks;  // taps and channel chunks (Cin_eff / BLOCK_K)
   int BW, BH, n_col_tiles;
   int Hq, Ho, Wo, Bn;           // virtual rows per image, valid output extent, batch
@@ -136,6 +141,33 @@ __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
+// contiguous global -> shared copy (bytes and both addresses multiples of 16), completing on `bar`
+__device__ __forceinline__ void bulk_load_raw(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+// shared -> global tensor store (bulk-group completion: commit, then wait on the issuing thread)
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap *map, const void *src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];" ::"l"((uint64_t)map),
+               "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the committed stores have finished reading their shared-memory source
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// ... and their global writes are done
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// four 8x8 16-bit matrices, each stored transposed: fragment column c becomes the 16-byte row at lane (8 * matrix + c)'s address
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+
 // elected lane
 __device__ __forceinline__ void tma_load_4d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2, int c3) {
   if (elect_one())
@@ -181,29 +213,36 @@ __device__ __forceinline__ uint32_t pack2_bf16(float a, float b) {
   return r;
 }
 
-// conv1: MMA rows >= BW of the last ring slot read up to (128 - BW) * 16 bytes past it
+// conv1_rgbd_kernel: MMA rows >= BW of the last ring slot read up to (128 - BW) * 16 bytes past it
 constexpr int kConv1Slack = 2048;
 
 
 // Rows of the m64nN accumulator fragment owned by thread `t` of a warpgroup: row0 and row0 + 8; columns 8j + 2(t & 3) (+1).
 __device__ __forceinline__ int frag_row(int t) { return ((t >> 5) << 4) + ((t & 31) >> 2); }
 
+// The forward epilogue of two accumulator values: + bias, LeakyReLU, packed 16-bit pair (hi[, lo]; element 0 low).
+template <bool SPLIT3, bool F16>
+__device__ __forceinline__ void epi_pack(float v0, float v1, float b0, float b1, float slope, uint32_t &hi, uint32_t &lo) {
+  v0 += b0;
+  v1 += b1;
+  v0 = v0 > 0.f ? v0 : v0 * slope;
+  v1 = v1 > 0.f ? v1 : v1 * slope;
+  if (F16) {
+    hi = pack2_f16(v0, v1);
+  } else {
+    hi = pack2_bf16(v0, v1);
+    if (SPLIT3) lo = pack2_bf16(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xFFFF0000u));
+  }
+}
+
 // One fragment row pair (j-th 8-column group) of the forward epilogue: + bias, LeakyReLU, 16-bit store (hi[, lo]).
 template <bool SPLIT3, bool F16>
 __device__ __forceinline__ void store_pair(float v0, float v1, float2 b, float slope, __nv_bfloat16 *out_hi, __nv_bfloat16 *out_lo,
                                            long long off) {
-  v0 += b.x;
-  v1 += b.y;
-  v0 = v0 > 0.f ? v0 : v0 * slope;
-  v1 = v1 > 0.f ? v1 : v1 * slope;
-  if (F16) {
-    *reinterpret_cast<uint32_t *>(out_hi + off) = pack2_f16(v0, v1);
-  } else {
-    const uint32_t h = pack2_bf16(v0, v1);
-    *reinterpret_cast<uint32_t *>(out_hi + off) = h;
-    if (SPLIT3)
-      *reinterpret_cast<uint32_t *>(out_lo + off) = pack2_bf16(v0 - __uint_as_float(h << 16), v1 - __uint_as_float(h & 0xFFFF0000u));
-  }
+  uint32_t h, l = 0;
+  epi_pack<SPLIT3, F16>(v0, v1, b.x, b.y, slope, h, l);
+  *reinterpret_cast<uint32_t *>(out_hi + off) = h;
+  if (SPLIT3) *reinterpret_cast<uint32_t *>(out_lo + off) = l;
 }
 
 // generic epilogue of the training-step kernels (see ConvKParams): two channels n, n + 1 of one output pixel
@@ -389,50 +428,75 @@ __global__ void __launch_bounds__(384, 1) conv_igemm_persistent_kernel(const __g
 }
 
 // ---------------------------------------------------------------------------------------------
-// conv1 (flow_conv1: 8 -> 64, 7x7 s2, i.e. 16 taps x 32 space-to-depth channels).  The generic path
-// fetches every tap's operand tile from L2 separately (16x re-read of the input).  Here one TMA box per filter row dh
-// brings the (BW+3)-pixel input strip into shared memory ONCE, in the un-swizzled K-major layout
-//     addr(pixel r, channel-chunk c) = base + c*LBO + 16*r          (8-channel chunks of 16 B)
-// in which the row index is linear in memory, so the four horizontal taps dw = 0..3 are the same
-// strip read through descriptors whose start address is shifted by dw*16 bytes.
-// Input buffer layout (written by the zoom kernel): [B*Hs rows][4 chunks][Ws cols][8 ch] bf16.
-// Tile = one output row x BW output columns (BW <= 128; MMA rows >= BW are don't-care and read past the strip into the
-// slack behind the ring).  Weights: the whole 64 x 512 matrix stays resident in shared memory (64B-swizzled, 16 tap tiles).
+// conv1 (flow_conv1: 8 -> 64, 7x7 s2, i.e. 16 taps x 32 space-to-depth channels), computed transposed:
+//     D^T [64 Cout x N px] = W [64 x K] . X [K x N px]
+// so the output pixels run along the wgmma N axis (N = 160 divides Wo = 320: no MMA column is wasted) and one m64nNk16 per K
+// step covers a whole column tile.
+//   A = the whole 64 x 512 weight matrix, resident in shared memory (64B-swizzled K-major, 16 tap tiles; conv1_kslot order).
+//   B = the (N+3)-pixel input strip of one input row, in the un-swizzled K-major layout
+//         addr(pixel r, channel-chunk c) = base + c*LBO + 16*r          (8-channel chunks of 16 B, LBO = (N+3)*16)
+//       in which the pixel index is linear in memory, so the four horizontal taps dw = 0..3 are the same strip read through
+//       descriptors whose start address is shifted by dw*16 bytes.  Input buffer layout (written by the zoom kernel):
+//       [B*Hs rows][4 chunks][Ws cols][8 ch], so a strip is four contiguous runs of (N+3)*16 bytes, one bulk copy each.
 //
 // Rolling strips: a CTA owns one column tile and a CONTIGUOUS run of output rows [g_lo, g_hi) and walks down it: output
 // row t uses the input strips t .. t+3 (one per filter row dh), so moving to the next row needs ONE new strip; every strip
-// travels L2 -> shared memory once (plus a 3-row halo per chunk).  The two consumer warpgroups take alternate rows (each
-// the full M = 128 as two m64 halves) so that one runs its epilogue while the other's wgmmas run.  Strip s is used by rows
-// s-3 .. s; the warpgroup of parity p is done with strips <= t+1 after its row t (its next row t+2 starts at strip t+2),
-// so after row t it releases strips t and t+1: every strip gets one arrival from each warpgroup (the parity-1 warpgroup
-// never uses strip 0 and releases it up front).
+// travels L2 -> shared memory once (plus a 3-row halo per run).  The two consumer warpgroups take alternate rows so that
+// one runs its epilogue while the other's wgmmas run.  Strip s is used by rows s-3 .. s; the warpgroup of parity p is done
+// with strips <= t+1 after its row t (its next row t+2 starts at strip t+2), so after row t it releases strips t and t+1:
+// every strip gets one arrival from each warpgroup (the parity-1 warpgroup never uses strip 0 and releases it up front).
 // Structurally-zero K steps are not issued: filter row 7 (dh = 3, odd input row) and filter column 7 (dw = 3, odd input
 // column) lie outside the 7 x 7 filter, so dh = 3 has no second K step and dw = 3 has ONE step over the input chunks
-// (0, 2) (weights packed in that order: conv1_kslot).
-template <int STAGES, bool SPLIT3, bool F16>
+// (0, 2) (weights packed in that order: conv1_kslot).  25 K steps per row, in the same order for every output element.
+//
+// Epilogue: bias + LeakyReLU + 16-bit pack in registers (epi_pack, the arithmetic of every forward epilogue), transposed
+// into a per-warpgroup [N px][64 ch] staging tile with stmatrix .trans (128B-swizzled: conflict-free), then TMA-stored in
+// boxes of kConv1StoreN pixels through a map that covers only the interior of the next layer's buffer, so the zero border
+// cannot be written.  Virtual rows (oh >= Ho) are not stored.
+//
+// N = 160 for fp16 / bf16 (2 column tiles at Wo = 320); bf16x3's hi + lo weights take 128 KB, which leaves room for N = 80
+// (4 column tiles) with a 5-deep hi + lo ring: a 6th stage would need 236 KB with the two warpgroups' hi + lo staging
+// tiles, over the 227 KB a CTA may use.
+//
+// The bulk copies are not bounds-checked by the hardware (a tensor map would clip them), so strips past the input's last
+// row are never loaded: the runs end 3 strips past their last output row, and at the end of the batch those 3 strips lie
+// past the buffer; they feed only the last image's virtual rows.
+constexpr int kConv1StoreN = 80;
+
+template <int N, int STAGES, bool SPLIT3>
+struct Conv1Smem {
+  static constexpr int NPREC = SPLIT3 ? 2 : 1;
+  static constexpr int TAP_BYTES = 64 * 32 * 2;                            // one 64 x 32 tap tile of the weights
+  static constexpr int RES_BYTES = 16 * TAP_BYTES * NPREC;
+  static constexpr int STG_BYTES = N * 128;                                // [N px][64 ch] 16-bit, per precision
+  static constexpr int PLANE_BYTES = (N + 3) * 16;                         // one chunk plane of a strip (= LBO)
+  static constexpr int STRIP_BYTES = (4 * PLANE_BYTES + 127) / 128 * 128;  // per precision
+  static constexpr int STAGE_BYTES = STRIP_BYTES * NPREC;
+  static constexpr int TOTAL = RES_BYTES + 2 * STG_BYTES * NPREC + STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(N % kConv1StoreN == 0 && N % 16 == 0 && STG_BYTES % 1024 == 0, "conv1 tile width");
+  static_assert(TOTAL <= 227 * 1024, "conv1 shared memory");
+};
+
+template <int N, int STAGES, bool SPLIT3, bool F16>
 __global__ void __launch_bounds__(384, 1) conv1_kernel(const __grid_constant__ ConvKParams p, const int rows_total,
-                                                       const int rows_per_chunk, const int chunks_per_col,
-                                                       const int strip_bytes /*per precision, multiple of 128*/) {
-  constexpr int NPREC = SPLIT3 ? 2 : 1;
-  constexpr int B_BYTES = 64 * 32 * 2, RES_BYTES = 16 * B_BYTES * NPREC;
+                                                       const int rows_per_chunk, const int chunks_per_col) {
+  using S = Conv1Smem<N, STAGES, SPLIT3>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t *res = smem;
-  uint8_t *ring = smem + RES_BYTES;
-  const int stage_bytes = strip_bytes * NPREC;
-  uint64_t *full_bar = reinterpret_cast<uint64_t *>(ring + STAGES * stage_bytes + kConv1Slack);
+  uint8_t *stg = res + S::RES_BYTES;  // consumer warpgroup w: hi tile at stg + w * NPREC * STG_BYTES, lo tile behind it
+  uint8_t *ring = stg + 2 * S::NPREC * S::STG_BYTES;
+  uint64_t *full_bar = reinterpret_cast<uint64_t *>(ring + STAGES * S::STAGE_BYTES);
   uint64_t *empty_bar = full_bar + STAGES;
   uint64_t *res_bar = empty_bar + STAGES;
 
   const int wgi = threadIdx.x >> 7, warp = threadIdx.x >> 5;
-  const int R = p.BW + 3;
-  const uint32_t LBO = (uint32_t)R * 16u;
   const int ct = blockIdx.x / chunks_per_col, ck = blockIdx.x - ct * chunks_per_col;
   const int g_lo = ck * rows_per_chunk;
   const int g_hi = min(rows_total, g_lo + rows_per_chunk);
-  const int n_rows = max(0, g_hi - g_lo);          // output rows (tiles) of this CTA
+  const int n_rows = max(0, g_hi - g_lo);          // output rows of this CTA
   const int n_strips = n_rows > 0 ? n_rows + 3 : 0;
-  const int ow0 = ct * p.BW;
+  const int ow0 = ct * N;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
@@ -442,7 +506,7 @@ __global__ void __launch_bounds__(384, 1) conv1_kernel(const __grid_constant__ C
     ptx::mbar_init(res_bar, 1);
     ptx::fence_barrier_init();
     ptx::prefetch_tmap(&p.b_map);
-    ptx::prefetch_tmap(&p.a_map[0]);
+    ptx::prefetch_tmap(&p.out_map[0]);
   }
   __syncthreads();
 
@@ -450,107 +514,133 @@ __global__ void __launch_bounds__(384, 1) conv1_kernel(const __grid_constant__ C
     ptx::regs_producer();
     if (warp == 0 && n_rows > 0) {
       if (ptx::elect_one()) {
-        ptx::mbar_expect_tx_raw(res_bar, (uint32_t)RES_BYTES);
+        ptx::mbar_expect_tx_raw(res_bar, (uint32_t)S::RES_BYTES);
         for (int kb = 0; kb < 16; ++kb) {
-          ptx::tma_load_2d_raw(res + kb * B_BYTES, &p.b_map, res_bar, kb * 32, 0);
-          if (SPLIT3) ptx::tma_load_2d_raw(res + (16 + kb) * B_BYTES, &p.b_lo_map, res_bar, kb * 32, 0);
+          ptx::tma_load_2d_raw(res + kb * S::TAP_BYTES, &p.b_map, res_bar, kb * 32, 0);
+          if (SPLIT3) ptx::tma_load_2d_raw(res + (16 + kb) * S::TAP_BYTES, &p.b_lo_map, res_bar, kb * 32, 0);
         }
       }
       __syncwarp();
-      const uint32_t tx = (uint32_t)(R * 64) * NPREC;
+      const size_t plane = (size_t)p.in_cols * 16;  // bytes between the chunk planes of one input row
+      const uint8_t *src_hi = reinterpret_cast<const uint8_t *>(p.in_hi) + (size_t)ow0 * 16;
+      const uint8_t *src_lo = reinterpret_cast<const uint8_t *>(p.in_lo) + (size_t)ow0 * 16;
       for (int s = 0; s < n_strips; ++s) {
         const int slot = s % STAGES;
         ptx::mbar_wait(&empty_bar[slot], (((uint32_t)(s / STAGES)) & 1u) ^ 1u);
-        uint8_t *st = ring + slot * stage_bytes;
-        ptx::mbar_expect_tx(&full_bar[slot], tx);
-        ptx::tma_load_4d(st, &p.a_map[0], &full_bar[slot], 0, ow0, 0, g_lo + s);
-        if (SPLIT3) ptx::tma_load_4d(st + strip_bytes, &p.a_lo_map[0], &full_bar[slot], 0, ow0, 0, g_lo + s);
+        uint8_t *st = ring + slot * S::STAGE_BYTES;
+        if (g_lo + s >= rows_total) {
+          // past the input's last row (the input has Hq = rows_total / B rows per image): the last run's final three
+          // strips feed only the last image's virtual rows, which are never stored, so nothing is read
+          if (ptx::elect_one()) ptx::mbar_arrive(&full_bar[slot]);
+        } else if (ptx::elect_one()) {
+          ptx::mbar_expect_tx_raw(&full_bar[slot], (uint32_t)(4 * S::PLANE_BYTES * S::NPREC));
+          const size_t row = (size_t)(g_lo + s) * 4 * plane;
+#pragma unroll
+          for (int c = 0; c < 4; ++c) {
+            ptx::bulk_load_raw(st + c * S::PLANE_BYTES, src_hi + row + c * plane, S::PLANE_BYTES, &full_bar[slot]);
+            if (SPLIT3)
+              ptx::bulk_load_raw(st + S::STRIP_BYTES + c * S::PLANE_BYTES, src_lo + row + c * plane, S::PLANE_BYTES, &full_bar[slot]);
+          }
+        }
+        __syncwarp();
       }
     }
   } else if (n_rows > 0) {
     ptx::regs_consumer();
-    const int set = wgi - 1, t = threadIdx.x & 127;
-    const bool arriver = t == 0;
-    const int r0 = frag_row(t), q2 = (t & 3) * 2;
-    float2 bias[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) bias[j] = make_float2(__ldg(p.bias + 8 * j + q2), __ldg(p.bias + 8 * j + q2 + 1));
+    const int set = wgi - 1, t = threadIdx.x & 127, lane = t & 31;
+    const bool leader = t == 0;
+    // this thread's accumulator rows are output channels co and co + 8
+    const int co = frag_row(t);
+    const float b0 = __ldg(p.bias + co), b1 = __ldg(p.bias + co + 8);
     const uint32_t ring_a = ptx::smem_u32(ring);
     // everything that does not depend on the row is formed once: ring-slot descriptor = dring + slot * slot_step
-    const uint64_t dring = ptx::gmma_desc(ring_a, LBO, 128, ptx::kNoSwizzle);
-    const uint64_t dring3 = ptx::gmma_desc(ring_a, 2u * LBO, 128, ptx::kNoSwizzle) + 3u;  // dw = 3: chunks 0 and 2, 3 pixels in
-    const uint64_t lo_step = (uint64_t)((uint32_t)strip_bytes >> 4);
-    const uint64_t slot_step = (uint64_t)((uint32_t)stage_bytes >> 4);
-    const uint64_t kstep = (uint64_t)(2u * LBO >> 4);
+    const uint64_t dring = ptx::gmma_desc(ring_a, S::PLANE_BYTES, 128, ptx::kNoSwizzle);
+    const uint64_t dring3 = ptx::gmma_desc(ring_a, 2u * S::PLANE_BYTES, 128, ptx::kNoSwizzle) + 3u;  // dw = 3: chunks 0, 2
+    const uint64_t lo_step = (uint64_t)(S::STRIP_BYTES >> 4);
+    const uint64_t slot_step = (uint64_t)(S::STAGE_BYTES >> 4);
+    const uint64_t kstep = (uint64_t)(2 * S::PLANE_BYTES >> 4);
     const uint64_t dres = ptx::gmma_desc(ptx::smem_u32(res), 16, 512, ptx::kSW64);
-    const uint64_t dres_lo = dres + (uint64_t)((16 * B_BYTES) >> 4);
-    const int n_cols_valid = min(p.BW, p.Wo - ow0);
+    const uint64_t dres_lo = dres + (uint64_t)((16 * S::TAP_BYTES) >> 4);
+    // stmatrix x4 of column groups (2i, 2i + 1): matrix m = lane / 8 is (column group 2i + m / 2, channels 16 * warp + 8 * (m & 1)
+    // .. +7); lane addresses row lane % 8 of it = pixel 16i + 8 * (m / 2) + lane % 8, 16-byte chunk 2 * warp + (m & 1), stored
+    // at chunk ^ (pixel % 8) of the pixel's 128-byte row (SW128, tiles 1024-byte aligned)
+    uint8_t *my_stg = stg + set * S::NPREC * S::STG_BYTES;
+    const int st_px = ((lane >> 4) << 3) + (lane & 7), st_chunk = 2 * (t >> 5) + ((lane >> 3) & 1);
+    const uint32_t st_addr = ptx::smem_u32(my_stg) + (uint32_t)(st_px * 128 + ((st_chunk ^ (lane & 7)) << 4));
     ptx::mbar_wait(res_bar, 0);
-    if (set == 1 && arriver) ptx::mbar_arrive(&empty_bar[0]);
+    if (set == 1 && leader) ptx::mbar_arrive(&empty_bar[0]);
     for (int row = set; row < n_rows; row += 2) {
-      float acc[2][32];
+      float acc[N / 2];
 #pragma unroll
       for (int dh = 0; dh < 4; ++dh) {
         const int s = row + dh;
         ptx::mbar_wait(&full_bar[s % STAGES], ((uint32_t)(s / STAGES)) & 1u);
       }
-      wg::fence_acc(acc[0]);
-      wg::fence_acc(acc[1]);
+      wg::fence_acc(acc);
       wg::fence();
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
+      for (int dh = 0; dh < 4; ++dh) {
+        const uint64_t so = (uint64_t)((row + dh) % STAGES) * slot_step;
 #pragma unroll
-        for (int dh = 0; dh < 4; ++dh) {
-          const uint64_t so = (uint64_t)((row + dh) % STAGES) * slot_step + (uint64_t)(h * 64);  // + 64 pixels of 16 B
+        for (int k = 0; k < 2; ++k) {
 #pragma unroll
-          for (int k = 0; k < 2; ++k) {
-#pragma unroll
-            for (int dw = 0; dw < 4; ++dw) {
-              if ((dh == 3 || dw == 3) && k == 1) continue;  // kh = 7 / kw = 7: outside the 7x7 filter, all-zero weights
-              const uint64_t da = (dw == 3 ? dring3 : dring + (uint64_t)dw + (uint64_t)k * kstep) + so;
-              const uint64_t wo = (uint64_t)((dh * 4 + dw) * (B_BYTES >> 4) + 2 * k);
-              wg::mma<64, F16, 0, 0>(acc[h], da, dres + wo, (dh | dw | k) ? 1u : 0u);
-              if (SPLIT3) {
-                wg::mma<64, false, 0, 0>(acc[h], da + lo_step, dres + wo, 1u);
-                wg::mma<64, false, 0, 0>(acc[h], da, dres_lo + wo, 1u);
-              }
+          for (int dw = 0; dw < 4; ++dw) {
+            if ((dh == 3 || dw == 3) && k == 1) continue;  // kh = 7 / kw = 7: outside the 7x7 filter, all-zero weights
+            const uint64_t db = (dw == 3 ? dring3 : dring + (uint64_t)dw + (uint64_t)k * kstep) + so;
+            const uint64_t wo = (uint64_t)((dh * 4 + dw) * (S::TAP_BYTES >> 4) + 2 * k);
+            wg::mma<N, F16, 0, 0>(acc, dres + wo, db, (dh | dw | k) ? 1u : 0u);
+            if (SPLIT3) {
+              wg::mma<N, false, 0, 0>(acc, dres + wo, db + lo_step, 1u);
+              wg::mma<N, false, 0, 0>(acc, dres_lo + wo, db, 1u);
             }
           }
         }
       }
       wg::commit();
       wg::wait<0>();
-      wg::fence_acc(acc[0]);
-      wg::fence_acc(acc[1]);
-      if (arriver) {
+      wg::fence_acc(acc);
+      if (leader) {
         ptx::mbar_arrive(&empty_bar[row % STAGES]);
         ptx::mbar_arrive(&empty_bar[(row + 1) % STAGES]);
       }
       const int g = g_lo + row;
       const int n_img = g / p.Hq, oh = g - n_img * p.Hq;
       if (n_img < p.Bn && oh < p.Ho) {
-        const long long row_off = (((long long)n_img * p.out_Hp + oh + p.out_py) * p.out_Wp + ow0 + p.out_px) * 64 + q2;
+        if (leader) ptx::bulk_wait_read0();  // this warpgroup's previous row has left the staging tile
+        ptx::named_bar_sync(1 + set, 128);
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+        for (int i = 0; i < N / 16; ++i) {
+          uint32_t h[4], l[4] = {0, 0, 0, 0};
+          epi_pack<SPLIT3, F16>(acc[8 * i + 0], acc[8 * i + 1], b0, b0, p.slope, h[0], l[0]);
+          epi_pack<SPLIT3, F16>(acc[8 * i + 2], acc[8 * i + 3], b1, b1, p.slope, h[1], l[1]);
+          epi_pack<SPLIT3, F16>(acc[8 * i + 4], acc[8 * i + 5], b0, b0, p.slope, h[2], l[2]);
+          epi_pack<SPLIT3, F16>(acc[8 * i + 6], acc[8 * i + 7], b1, b1, p.slope, h[3], l[3]);
+          ptx::stmatrix_x4_trans(st_addr + (uint32_t)(i * 16 * 128), h);
+          if (SPLIT3) ptx::stmatrix_x4_trans(st_addr + (uint32_t)(S::STG_BYTES + i * 16 * 128), l);
+        }
+        ptx::fence_proxy_async();  // the generic-proxy staging writes become visible to the TMA store
+        ptx::named_bar_sync(1 + set, 128);
+        if (leader) {
 #pragma unroll
-          for (int rr = 0; rr < 2; ++rr) {
-            const int m = h * 64 + r0 + rr * 8;
-            if (m < n_cols_valid) {
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                store_pair<SPLIT3, F16>(acc[h][4 * j + 2 * rr], acc[h][4 * j + 2 * rr + 1], bias[j], p.slope, p.out_hi, p.out_lo,
-                                        row_off + (long long)m * 64 + 8 * j);
-            }
+          for (int q = 0; q < N / kConv1StoreN; ++q) {
+            ptx::tma_store_4d(&p.out_map[0], my_stg + q * kConv1StoreN * 128, 0, ow0 + q * kConv1StoreN, oh, n_img);
+            if (SPLIT3)
+              ptx::tma_store_4d(&p.out_map[1], my_stg + S::STG_BYTES + q * kConv1StoreN * 128, 0, ow0 + q * kConv1StoreN, oh, n_img);
           }
+          ptx::bulk_commit();
+        }
       }
     }
+    if (leader) ptx::bulk_wait0();
   }
 }
 
 // ---------------------------------------------------------------------------------------------
 // conv1 of the RGB-D network (flow_conv1: 10 -> 64, 7x7 s2; deepIM_flownet.py:33-51 with INPUT_DEPTH).  Same rolling-strip
-// schedule as conv1_kernel; the space-to-depth input has 16-channel chunks: each of the four 2x2 phases (ph, pw) is a pair
-// of 8-channel chunk planes, channels 0-7 then 8-9 (+ 6 zero channels), so a strip is 8 chunk planes
+// schedule as conv1_kernel, but with the pixels on the MMA M axis: a tile is one output row x BW <= 128 columns (MMA rows
+// >= BW are don't-care and read past the strip into the slack behind the ring), each warpgroup issuing it as two m64 halves,
+// with the strips loaded as 4-D TMA boxes and the output stored straight from the fragments.  The space-to-depth input has
+// 16-channel chunks: each of the four 2x2 phases (ph, pw) is a pair of 8-channel chunk planes, channels 0-7 then 8-9 (+ 6 zero channels), so a strip is 8 chunk planes
 //     addr(pixel r, plane c) = base + c*LBO + 16*r,  plane c = (ph*2 + pw)*2 + half
 // and K step k (16 channels) of tap (dh, dw) is exactly phase k = ph*2 + pw: planes 2k, 2k + 1.  Phases with kh = 7
 // (dh = 3, ph = 1) or kw = 7 (dw = 3, pw = 1) lie outside the 7 x 7 filter and are not issued (49 of the 64 K steps run).

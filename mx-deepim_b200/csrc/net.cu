@@ -124,12 +124,7 @@ static int build_maps(NetState *ns, int B, bool f16, TensorMaps &tm) {
         if (int rc = encode_map(&maps[0], base, 4, dims, str, box4, 0)) return rc;
         maps[1] = maps[2] = maps[3] = maps[0];
       } else if (i == 0) {
-        // conv1 strip layout [B*rows][4 chunks][cols][8 ch]: box = 8 ch x (BW+3) cols x 4 chunks x 1 row
-        const uint64_t dims[4] = {8, (uint64_t)g.cols, 4, (uint64_t)B * g.rows};
-        const uint64_t str[3] = {16, (uint64_t)g.cols * 16, (uint64_t)g.cols * 64};
-        const uint32_t box4[4] = {8, (uint32_t)(g.BW + 3), 4, 1};
-        if (int rc = encode_map(&maps[0], base, 4, dims, str, box4, 0)) return rc;
-        maps[1] = maps[2] = maps[3] = maps[0];
+        // conv1_kernel reads its strips with plain bulk copies (kp.in_hi / in_lo): no activation map
       } else if (g.stride_eff == 1) {
         const uint64_t dims[3] = {(uint64_t)g.Cbuf, (uint64_t)g.cols, (uint64_t)B * g.rows};
         const uint64_t str[2] = {(uint64_t)g.Cbuf * 2, (uint64_t)g.cols * g.Cbuf * 2};
@@ -170,6 +165,20 @@ static int build_maps(NetState *ns, int B, bool f16, TensorMaps &tm) {
     kp.bias = ns->bias[i];
     kp.out_hi = ns->act_hi[i + 1];
     kp.out_lo = ns->act_lo[i + 1];
+    if (i == 0 && !ns->input_depth) {
+      // conv1_kernel: strips from the space-to-depth input, output tiles TMA-stored into conv2's buffer through a 4-D map
+      // (64 ch, Wo, Ho, B) whose origin is the interior's first pixel: the zero border lies outside every box
+      const LayerGeom &nx = ns->g[1];
+      kp.in_hi = ns->act_hi[0];
+      kp.in_lo = ns->act_lo[0];
+      kp.in_cols = g.cols;
+      const uint64_t dims[4] = {64, (uint64_t)g.Wo, (uint64_t)g.Ho, (uint64_t)B};
+      const uint64_t str[3] = {128, (uint64_t)nx.cols * 128, (uint64_t)nx.rows * nx.cols * 128};
+      const uint32_t box[4] = {64, (uint32_t)kConv1StoreN, 1, 1};
+      const size_t interior = ((size_t)nx.py * nx.cols + nx.px) * 64;
+      for (int lo = 0; lo < 2; ++lo)
+        if (int rc = encode_map(&kp.out_map[lo], (lo ? ns->act_lo[1] : ns->act_hi[1]) + interior, 4, dims, str, box, 64)) return rc;
+    }
   }
   return 0;
 }
@@ -501,16 +510,15 @@ static int launch_conv(const ConvKParams &kp, int total_tiles, int n_tiles, int 
   return 0;
 }
 
-template <int ST, bool S3, bool F16>
-static int launch_conv1(const ConvKParams &kp, int grid, int rows_total, int rpc, int chunks, int strip_bytes, cudaStream_t st) {
-  const int smem_bytes = (S3 ? 2 : 1) * 16 * 4096 + ST * (S3 ? 2 : 1) * strip_bytes + kConv1Slack + 1024 + 256;
-  DIM_REQUIRE(smem_bytes <= 227 * 1024, "conv1: image too wide for the rolling-strip ring");
-  static int set = 0;
-  if (set < smem_bytes) {
-    DIM_CHECK(cudaFuncSetAttribute(conv1_kernel<ST, S3, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-    set = smem_bytes;
+template <int N, int ST, bool S3, bool F16>
+static int launch_conv1(const ConvKParams &kp, int grid, int rows_total, int rpc, int chunks, cudaStream_t st) {
+  using S = Conv1Smem<N, ST, S3>;
+  static bool set = false;
+  if (!set) {
+    DIM_CHECK(cudaFuncSetAttribute(conv1_kernel<N, ST, S3, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+    set = true;
   }
-  conv1_kernel<ST, S3, F16><<<grid, 384, smem_bytes, st>>>(kp, rows_total, rpc, chunks, strip_bytes);
+  conv1_kernel<N, ST, S3, F16><<<grid, 384, S::TOTAL, st>>>(kp, rows_total, rpc, chunks);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -608,18 +616,22 @@ int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, fl
               : (f16 ? launch_conv1_rgbd<6, false, true, 64>(kp, grid, rows_total, rpc, chunks, strip_bytes, st)
                      : launch_conv1_rgbd<6, false, false, 64>(kp, grid, rows_total, rpc, chunks, strip_bytes, st));
     } else if (i == 0) {
-      // conv1: a CTA walks down a run of output rows of one column tile, one new input strip per row
+      // conv1: a CTA walks down a run of output rows of one column tile (N = 160 pixels, bf16x3: 80), one new input strip
+      // per row.  Built for the network's 480 x 640 input: Wo = 320 is a whole number of column tiles.
+      // The kernel skips the strips past the input's last row (row B * Hq): they must feed only virtual rows.
+      DIM_REQUIRE(g.Wo == 320 && g.cols >= g.Wo + 3 && g.Hq == g.rows && g.Hq == g.Ho + 3,
+                  "conv1_kernel is built for a 480x640 input (320 output columns)");
+      const int n_col = g.Wo / (s3 ? 80 : 160);
       const int rows_total = B * g.Hq;
-      int chunks = sms / g.n_col_tiles;
+      int chunks = sms / n_col;
       if (chunks > cdiv(rows_total, 16)) chunks = cdiv(rows_total, 16);  // keep the 3-row halo below ~20 %
       if (chunks < 1) chunks = 1;
       const int rpc = cdiv(rows_total, chunks);
       chunks = cdiv(rows_total, rpc);
-      const int strip_bytes = cdiv((g.BW + 3) * 64, 128) * 128;
-      const int grid = g.n_col_tiles * chunks;
-      rc = s3 ? launch_conv1<5, true, false>(kp, grid, rows_total, rpc, chunks, strip_bytes, st)
-              : (f16 ? launch_conv1<8, false, true>(kp, grid, rows_total, rpc, chunks, strip_bytes, st)
-                     : launch_conv1<8, false, false>(kp, grid, rows_total, rpc, chunks, strip_bytes, st));
+      const int grid = n_col * chunks;
+      rc = s3 ? launch_conv1<80, 5, true, false>(kp, grid, rows_total, rpc, chunks, st)
+              : (f16 ? launch_conv1<160, 8, false, true>(kp, grid, rows_total, rpc, chunks, st)
+                     : launch_conv1<160, 8, false, false>(kp, grid, rows_total, rpc, chunks, st));
     } else if (g.BLOCK_N == 128) {
       rc = s3 ? launch_conv<128, 3, true, false>(kp, total_tiles, n_tiles, sms, st)
               : (f16 ? launch_conv<128, 6, false, true>(kp, total_tiles, n_tiles, sms, st)
