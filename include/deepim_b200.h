@@ -486,8 +486,17 @@ DIM_API int32_t dim_train_get_config(dim_ctx *ctx, dim_train_config *cfg);
  * are frozen), then refreshes every bf16 operand pack of the context from the new master weights. */
 DIM_API int32_t dim_train_sgd_update(dim_ctx *ctx, const float *grads, float lr, float momentum, float wd,
                                      float rescale_grad, void *stream);
-/* Test hooks: intermediates of the training step (ids in train.cu) and their geometry
- * out7 = Hp, Wp, py, px, C, H, W. */
+/* Precision of this context's training step: DIM_PREC_BF16 (default; bf16 activations and activation gradients) or
+ * DIM_PREC_BF16X3 (every activation, activation gradient and operand pack a bf16 hi / lo pair, three tensor-core passes:
+ * gradients near the fp32 reference, about 2^-16 relative per stored value).  Gradients, master weights and momentum are
+ * fp32 in both.  Applies to dim_train_forward_backward(_rgbd), with and without gradients, and to the operand refresh of
+ * dim_train_sgd_update.  Any other value is refused (DIM_PREC_FP16 included).  Needs dim_train_create.  The first switch to
+ * DIM_PREC_BF16X3 allocates the lo halves; every switch to it synchronises the device and refreshes them from the master
+ * weights.  Switching back to DIM_PREC_BF16 leaves the bf16 step exactly as it was. */
+DIM_API int32_t dim_train_set_precision(dim_ctx *ctx, int32_t precision);
+DIM_API int32_t dim_train_get_precision(dim_ctx *ctx, int32_t *precision);
+/* Test hooks: intermediates of the training step (ids in train.cu; 100 + a bf16 buffer's id = its lo half after a
+ * DIM_PREC_BF16X3 step) and their geometry out7 = Hp, Wp, py, px, C, H, W. */
 DIM_API int32_t dim_train_debug_tensor(dim_ctx *ctx, int32_t id, void *host_dst, uint64_t bytes);
 DIM_API int32_t dim_train_debug_geometry(dim_ctx *ctx, int32_t id, int32_t *out7);
 /* ms7 = device time of the phases of the last dim_train_forward_backward (with gradients) on the caller's stream:

@@ -874,6 +874,17 @@ DIM_API int32_t dim_train_sgd_update(dim_ctx *ctx, const float *grads, float lr,
   DIM_REQUIRE(ctx && grads, "dim_train_sgd_update: NULL argument");
   return train_sgd_update(ctx, grads, lr, momentum, wd, rescale_grad, (cudaStream_t)stream);
 }
+DIM_API int32_t dim_train_set_precision(dim_ctx *ctx, int32_t precision) {
+  DIM_REQUIRE(ctx, "dim_train_set_precision: NULL context");
+  return train_set_precision(ctx, precision);
+}
+DIM_API int32_t dim_train_get_precision(dim_ctx *ctx, int32_t *precision) {
+  DIM_REQUIRE(ctx && precision, "dim_train_get_precision: NULL argument");
+  int p = 0;
+  if (int rc = train_get_precision(ctx, &p)) return rc;
+  *precision = p;
+  return 0;
+}
 DIM_API int32_t dim_train_debug_tensor(dim_ctx *ctx, int32_t id, void *host_dst, uint64_t bytes) {
   DIM_REQUIRE(ctx && host_dst, "dim_train_debug_tensor: NULL argument");
   return train_debug_tensor(ctx, id, host_dst, (size_t)bytes);

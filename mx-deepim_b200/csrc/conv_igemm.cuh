@@ -54,10 +54,11 @@ struct ConvKParams {
   //   interior pixel (oh*out_sy + out_oy, ow*out_sx + out_ox) of the output buffer when that is inside
   //   [0,out_H) x [0,out_W);  value = (acc + bias + addend) then LeakyReLU (mask.p == nullptr, slope 1 = none)
   //   or * (mask > 0 ? 1 : slope) for channels < mask_climit (LeakyReLU backward through the stored
-  //   activation).  All side buffers are bf16 NHWC with their own border / channel stride.
+  //   activation).  All side buffers are bf16 NHWC with their own border / channel stride.  SPLIT3: the addend is
+  //   read as hi + lo (lo at the same offset of addend.lo) and the result is stored as a hi / lo pair (out_hi, out_lo).
   int in_off_r, in_off_c;
   int out_sy, out_sx, out_oy, out_ox, out_H, out_W, out_cs, out_coff;
-  struct PixBuf { const __nv_bfloat16 *p; int Hp, Wp, py, px, cs, coff; } addend, mask;
+  struct PixBuf { const __nv_bfloat16 *p; int Hp, Wp, py, px, cs, coff; const __nv_bfloat16 *lo; } addend, mask;
   int mask_climit;
 };
 
@@ -220,6 +221,11 @@ constexpr int kConv1Slack = 2048;
 // Rows of the m64nN accumulator fragment owned by thread `t` of a warpgroup: row0 and row0 + 8; columns 8j + 2(t & 3) (+1).
 __device__ __forceinline__ int frag_row(int t) { return ((t >> 5) << 4) + ((t & 31) >> 2); }
 
+// the bf16 residuals (v - hi) of a packed bf16 pair hi = pack2_bf16(v0, v1): hi + lo carries ~16 significant bits
+__device__ __forceinline__ uint32_t pack2_bf16_lo(float v0, float v1, uint32_t hi) {
+  return pack2_bf16(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xFFFF0000u));
+}
+
 // The forward epilogue of two accumulator values: + bias, LeakyReLU, packed 16-bit pair (hi[, lo]; element 0 low).
 template <bool SPLIT3, bool F16>
 __device__ __forceinline__ void epi_pack(float v0, float v1, float b0, float b1, float slope, uint32_t &hi, uint32_t &lo) {
@@ -231,7 +237,7 @@ __device__ __forceinline__ void epi_pack(float v0, float v1, float b0, float b1,
     hi = pack2_f16(v0, v1);
   } else {
     hi = pack2_bf16(v0, v1);
-    if (SPLIT3) lo = pack2_bf16(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xFFFF0000u));
+    if (SPLIT3) lo = pack2_bf16_lo(v0, v1, hi);
   }
 }
 
@@ -245,7 +251,10 @@ __device__ __forceinline__ void store_pair(float v0, float v1, float2 b, float s
   if (SPLIT3) *reinterpret_cast<uint32_t *>(out_lo + off) = l;
 }
 
-// generic epilogue of the training-step kernels (see ConvKParams): two channels n, n + 1 of one output pixel
+// generic epilogue of the training-step kernels (see ConvKParams): two channels n, n + 1 of one output pixel.
+// SPLIT3: the addend is hi + lo (exact in fp32) and the result is stored as a hi / lo pair split like epi_pack.  The mask
+// reads the hi half only: its sign is the sign of hi + lo, because |lo| <= ulp(hi) / 2 and hi = 0 implies lo = 0.
+template <bool SPLIT3>
 __device__ __forceinline__ void store_pair_generic(float v0, float v1, const ConvKParams &p, int n, bool valid, long long off,
                                                    long long add_off, long long mask_off) {
   if (!valid || n >= p.Cout) return;
@@ -255,8 +264,14 @@ __device__ __forceinline__ void store_pair_generic(float v0, float v1, const Con
   }
   if (p.addend.p) {
     const __nv_bfloat162 a = *reinterpret_cast<const __nv_bfloat162 *>(p.addend.p + add_off);
-    v0 += __low2float(a);
-    v1 += __high2float(a);
+    if (SPLIT3) {
+      const __nv_bfloat162 al = *reinterpret_cast<const __nv_bfloat162 *>(p.addend.lo + add_off);
+      v0 += __low2float(a) + __low2float(al);
+      v1 += __high2float(a) + __high2float(al);
+    } else {
+      v0 += __low2float(a);
+      v1 += __high2float(a);
+    }
   }
   if (p.mask.p) {
     if (n < p.mask_climit) {
@@ -268,7 +283,13 @@ __device__ __forceinline__ void store_pair_generic(float v0, float v1, const Con
     v0 = v0 > 0.f ? v0 : v0 * p.slope;
     v1 = v1 > 0.f ? v1 : v1 * p.slope;
   }
-  *reinterpret_cast<__nv_bfloat162 *>(p.out_hi + off) = __floats2bfloat162_rn(v0, v1);
+  if (SPLIT3) {
+    const uint32_t h = pack2_bf16(v0, v1);
+    *reinterpret_cast<uint32_t *>(p.out_hi + off) = h;
+    *reinterpret_cast<uint32_t *>(p.out_lo + off) = pack2_bf16_lo(v0, v1, h);
+  } else {
+    *reinterpret_cast<__nv_bfloat162 *>(p.out_hi + off) = __floats2bfloat162_rn(v0, v1);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -283,6 +304,7 @@ struct ConvSmem2 {
   static constexpr int NPREC = SPLIT3 ? 2 : 1;
   static constexpr int STAGE_BYTES = (A_BYTES + B_BYTES) * NPREC;
   static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(TOTAL <= 227 * 1024, "conv_igemm shared memory");
 };
 
 template <int BLOCK_N, int STAGES, bool SPLIT3, bool F16, int EPI = 0>
@@ -409,7 +431,7 @@ __global__ void __launch_bounds__(384, 1) conv_igemm_persistent_kernel(const __g
               (((long long)n_img * p.mask.Hp + y + p.mask.py) * p.mask.Wp + x + p.mask.px) * p.mask.cs + p.mask.coff + n0 + q2;
 #pragma unroll
           for (int j = 0; j < BLOCK_N / 8; ++j)
-            store_pair_generic(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1], p, n0 + 8 * j + q2, valid, off + 8 * j,
+            store_pair_generic<SPLIT3>(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1], p, n0 + 8 * j + q2, valid, off + 8 * j,
                                add_off + 8 * j, mask_off + 8 * j);
         } else {
           const bool valid = (m < p.BW * p.BH) && (n_img < p.Bn) && (oh < p.Ho) && (ow < p.Wo);

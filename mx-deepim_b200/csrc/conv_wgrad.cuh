@@ -15,6 +15,9 @@
 // Work item = (K slice, tap, M tile, N tile); fp32 partial tiles are reduced (fixed order -> deterministic)
 // and re-laid out to the MXNet parameter layout by wgrad_reduce_kernel.
 // Warp roles as in conv_igemm.cuh: warp 0 loads, warpgroups 1 and 2 each own 64 of the 128 M rows.
+// SPLIT3 (bf16x3 training step): both operands are hi / lo pairs, a stage holds the hi set and the lo set behind it, and each
+// K step issues hi*hi + lo*hi + hi*lo into the same fp32 accumulator; the ring is shallower so that a stage of two operand
+// sets still fits (WgradSmem / Conv1WgradSmem assert the totals).
 #pragma once
 #include "conv_igemm.cuh"
 
@@ -23,6 +26,7 @@ namespace dim {
 struct WgradParams {
   CUtensorMap z_map;     // (C, cols, rows, B), box {64, BW, BH, 1}, SWIZZLE_128B
   CUtensorMap a_map[4];  // (C, cols, rows, B) views ((row parity, col parity) for stride 2), box {min(BN,64), BW, BH, 1}
+  CUtensorMap z_lo_map, a_lo_map[4];  // the same views of the lo halves (SPLIT3 only)
   int KH, KW, stride;
   int BW, BH, rects_x, rects_y, Bn;
   int z_off_r, z_off_c, a_off_r, a_off_c;
@@ -32,7 +36,8 @@ struct WgradParams {
 
 // consumer side shared by both wgrad kernels: K blocks [kb0, kb1) of the ring, then the fp32 tile rows of this warpgroup
 // (M rows 64*half .. +63) to dst (row stride ld floats).  a_off: byte offset of this warpgroup's M half in a stage.
-template <int BN, int STAGES, int STAGE_BYTES, int A_BYTES>
+// SPLIT3: the lo operands sit LO_BYTES behind the hi ones in every stage.
+template <int BN, int STAGES, int STAGE_BYTES, int A_BYTES, bool SPLIT3 = false, int LO_BYTES = 0>
 __device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full_bar, uint64_t *empty_bar, int kb0, int kb1, int half,
                                               uint64_t da_proto, uint32_t a_kstep, uint64_t db_proto, uint32_t b_kstep,
                                               float *dst, size_t ld) {
@@ -50,8 +55,14 @@ __device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full_bar,
     wg::fence_acc(acc);
     wg::fence();
 #pragma unroll
-    for (int k = 0; k < 4; ++k)  // 64 pixels = 4 x K 16
-      wg::mma<BN, false, 1, 1>(acc, da0 + (uint64_t)(k * a_kstep), db0 + (uint64_t)(k * b_kstep), 1u);
+    for (int k = 0; k < 4; ++k) {  // 64 pixels = 4 x K 16
+      const uint64_t da = da0 + (uint64_t)(k * a_kstep), db = db0 + (uint64_t)(k * b_kstep);
+      wg::mma<BN, false, 1, 1>(acc, da, db, 1u);
+      if (SPLIT3) {
+        wg::mma<BN, false, 1, 1>(acc, da + (uint64_t)(LO_BYTES >> 4), db, 1u);
+        wg::mma<BN, false, 1, 1>(acc, da, db + (uint64_t)(LO_BYTES >> 4), 1u);
+      }
+    }
     wg::commit();
     wg::wait<1>();
     wg::fence_acc(acc);
@@ -70,17 +81,19 @@ __device__ __forceinline__ void wgrad_consume(uint8_t *smem, uint64_t *full_bar,
   }
 }
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool SPLIT3 = false>
 struct WgradSmem {
   static constexpr int A_BYTES = 2 * 8192;                     // 128 channels x 64 pixels
   static constexpr int B_BYTES = BN >= 64 ? (BN / 64) * 8192 : 4096;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int SET_BYTES = A_BYTES + B_BYTES;          // one operand set (hi, or lo at + SET_BYTES)
+  static constexpr int STAGE_BYTES = SET_BYTES * (SPLIT3 ? 2 : 1);
   static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 + 256;
+  static_assert(TOTAL <= 227 * 1024, "conv_wgrad shared memory");
 };
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool SPLIT3 = false>
 __global__ void __launch_bounds__(384, 1) conv_wgrad_kernel(const __grid_constant__ WgradParams p) {
-  using S = WgradSmem<BN, STAGES>;
+  using S = WgradSmem<BN, STAGES, SPLIT3>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + STAGES * S::STAGE_BYTES);
@@ -138,6 +151,19 @@ __global__ void __launch_bounds__(384, 1) conv_wgrad_kernel(const __grid_constan
         } else {
           ptx::tma_load_4d(bs, &p.a_map[view], &full_bar[s], nt * BN, ox0 + dc + p.a_off_c, oy0 + dr + p.a_off_r, b);
         }
+        if (SPLIT3) {
+          uint8_t *sl = st + S::SET_BYTES;
+          ptx::tma_load_4d(sl, &p.z_lo_map, &full_bar[s], mt * 128, ox0 + p.z_off_c, oy0 + p.z_off_r, b);
+          ptx::tma_load_4d(sl + 8192, &p.z_lo_map, &full_bar[s], mt * 128 + 64, ox0 + p.z_off_c, oy0 + p.z_off_r, b);
+          if (BN >= 64) {
+#pragma unroll
+            for (int j = 0; j < BN / 64; ++j)
+              ptx::tma_load_4d(sl + S::A_BYTES + j * 8192, &p.a_lo_map[view], &full_bar[s], nt * BN + j * 64, ox0 + dc + p.a_off_c,
+                               oy0 + dr + p.a_off_r, b);
+          } else {
+            ptx::tma_load_4d(sl + S::A_BYTES, &p.a_lo_map[view], &full_bar[s], nt * BN, ox0 + dc + p.a_off_c, oy0 + dr + p.a_off_r, b);
+          }
+        }
         if (++s == STAGES) { s = 0; ph ^= 1u; }
       }
     }
@@ -149,8 +175,8 @@ __global__ void __launch_bounds__(384, 1) conv_wgrad_kernel(const __grid_constan
     // A: this warpgroup's 64 channels are one 8 KB box; per K step of 16 pixels both operands advance 16 rows
     const uint64_t da = ptx::gmma_desc(half * 8192, 8192, 1024, ptx::kSW128);
     const uint64_t db = BN >= 64 ? ptx::gmma_desc(0, 8192, 1024, ptx::kSW128) : ptx::gmma_desc(0, 4096, 512, ptx::kSW64);
-    wgrad_consume<BN, STAGES, S::STAGE_BYTES, S::A_BYTES>(smem, full_bar, empty_bar, kb0, kb1, half, da, 128, db,
-                                                          BN >= 64 ? 128 : 64, dst, Np);
+    wgrad_consume<BN, STAGES, S::STAGE_BYTES, S::A_BYTES, SPLIT3, S::SET_BYTES>(smem, full_bar, empty_bar, kb0, kb1, half, da, 128,
+                                                                                db, BN >= 64 ? 128 : 64, dst, Np);
   }
 }
 
@@ -197,15 +223,17 @@ __global__ void __launch_bounds__(256) wgrad_reduce_kernel(const float *__restri
 // 128 rows assembled from FOUR column-shifted TMA boxes of the NHWC-32 input copy (64-byte rows, SWIZZLE_64B, MN-major
 // groups LBO = 4 KB apart), N = 64 output channels of dZ (one SWIZZLE_128B box), K = 64 pixels: dZ is fetched 4x instead of
 // 16x and no MMA row is padding.
-template <int STAGES>
+template <int STAGES, bool SPLIT3 = false>
 struct Conv1WgradSmem {
-  static constexpr int A_BYTES = 4 * 4096, B_BYTES = 8192, STAGE_BYTES = A_BYTES + B_BYTES;
+  static constexpr int A_BYTES = 4 * 4096, B_BYTES = 8192, SET_BYTES = A_BYTES + B_BYTES;
+  static constexpr int STAGE_BYTES = SET_BYTES * (SPLIT3 ? 2 : 1);
   static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 + 256;
+  static_assert(TOTAL <= 227 * 1024, "conv1_wgrad shared memory");
 };
 
-template <int STAGES>
+template <int STAGES, bool SPLIT3 = false>
 __global__ void __launch_bounds__(384, 1) conv1_wgrad_kernel(const __grid_constant__ WgradParams p) {
-  using S = Conv1WgradSmem<STAGES>;
+  using S = Conv1WgradSmem<STAGES, SPLIT3>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + STAGES * S::STAGE_BYTES);
@@ -240,6 +268,12 @@ __global__ void __launch_bounds__(384, 1) conv1_wgrad_kernel(const __grid_consta
 #pragma unroll
         for (int dw = 0; dw < 4; ++dw) ptx::tma_load_4d(st + dw * 4096, &p.a_map[0], &full_bar[s], 0, ox0 + dw, oy0 + dh, b);
         ptx::tma_load_4d(st + S::A_BYTES, &p.z_map, &full_bar[s], 0, ox0 + p.z_off_c, oy0 + p.z_off_r, b);
+        if (SPLIT3) {
+#pragma unroll
+          for (int dw = 0; dw < 4; ++dw)
+            ptx::tma_load_4d(st + S::SET_BYTES + dw * 4096, &p.a_lo_map[0], &full_bar[s], 0, ox0 + dw, oy0 + dh, b);
+          ptx::tma_load_4d(st + S::SET_BYTES + S::A_BYTES, &p.z_lo_map, &full_bar[s], 0, ox0 + p.z_off_c, oy0 + p.z_off_r, b);
+        }
         if (++s == STAGES) { s = 0; ph ^= 1u; }
       }
     }
@@ -250,7 +284,8 @@ __global__ void __launch_bounds__(384, 1) conv1_wgrad_kernel(const __grid_consta
     // A: this warpgroup's 64 rows are two 32-channel boxes (dw = 2 half, 2 half + 1), 4 KB apart
     const uint64_t da = ptx::gmma_desc(half * 8192, 4096, 512, ptx::kSW64);
     const uint64_t db = ptx::gmma_desc(0, 8192, 1024, ptx::kSW128);
-    wgrad_consume<64, STAGES, S::STAGE_BYTES, S::A_BYTES>(smem, full_bar, empty_bar, kb0, kb1, half, da, 64, db, 128, dst, 64);
+    wgrad_consume<64, STAGES, S::STAGE_BYTES, S::A_BYTES, SPLIT3, S::SET_BYTES>(smem, full_bar, empty_bar, kb0, kb1, half, da, 64, db,
+                                                                                128, dst, 64);
   }
 }
 

@@ -98,6 +98,8 @@ size_t train_param_count(dim_ctx *ctx);
 int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel, bool input_depth = false);
 int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st);
 int train_sgd_update(dim_ctx *ctx, const float *grads, float lr, float momentum, float wd, float rescale, cudaStream_t st);
+int train_set_precision(dim_ctx *ctx, int precision);
+int train_get_precision(dim_ctx *ctx, int *precision);
 int train_debug_tensor(dim_ctx *ctx, int id, void *host, size_t bytes);
 int train_debug_phases(dim_ctx *ctx, float *ms7);
 void train_debug_geometry(dim_ctx *ctx, int id, int *out /*Hp, Wp, py, px, C, H, W*/);

@@ -16,6 +16,10 @@
 // Mixed precision: bf16 activations and activation gradients, fp32 accumulation, fp32 master weights /
 // momentum / gradients (the flat parameter vector uses the MXNet layouts, order = param table below, so that the
 // gradient all-reduce and checkpoints see the reference's tensors).
+// Precision of the step (dim_train_set_precision): DIM_PREC_BF16 (default) as above, or DIM_PREC_BF16X3, in which every
+// bf16 activation, activation gradient and operand pack is a hi / lo pair (x = hi + lo, ~16 significant bits): the
+// tensor-core kernels run their SPLIT3 form (hi*hi + lo*hi + hi*lo) and the CUDA-core kernels below, templated on S3,
+// read hi + lo and store pairs.  Their S3 = false instantiations are the bf16 step.
 #include <string.h>
 
 #include <algorithm>
@@ -47,9 +51,9 @@ enum { P_FC6 = 10, P_FC7 = 11, P_ROT = 12, P_TRANS = 13, P_CONV1D = 14, P_DECONV
 
 struct ParamOff { size_t w, b, wn, bn; };
 
-// bf16 NHWC buffer with border
+// bf16 NHWC buffer with border; lo: its bf16x3 lo half (same layout), allocated by the first switch to that precision
 struct Buf {
-  __nv_bfloat16 *p = nullptr;
+  __nv_bfloat16 *p = nullptr, *lo = nullptr;
   int H = 0, W = 0, Hp = 0, Wp = 0, py = 0, px = 0, C = 0;  // valid extent, allocated extent, border, channels
   size_t per_image() const { return (size_t)Hp * Wp * C; }
 };
@@ -86,7 +90,13 @@ struct TrainState {
   // bf16 operand packs
   __nv_bfloat16 *dg_pack[10][4] = {};  // data-gradient kernels of encoder layers 1..9 (per parity class)
   __nv_bfloat16 *d5_fwd[4] = {}, *d4_fwd[4] = {}, *d5_dg = nullptr, *d4_dg = nullptr;
-  std::map<int, TrainMaps> maps;
+  // bf16x3 step (dim_train_set_precision): the lo halves of the packs above, allocated with the buffers' lo halves by the
+  // first switch (fc6's lo pack is the inference one, NetState::fc6_w_lo)
+  __nv_bfloat16 *dg_pack_lo[10][4] = {};
+  __nv_bfloat16 *d5_fwd_lo[4] = {}, *d4_fwd_lo[4] = {}, *d5_dg_lo = nullptr, *d4_dg_lo = nullptr;
+  bool s3 = false;        // the step runs in DIM_PREC_BF16X3
+  bool lo_alloc = false;  // the lo halves exist
+  std::map<int, TrainMaps> maps;  // per batch size (+ kS3MapKey for the bf16x3 launch descriptors)
   int max_points = 0;
   // internal streams: [0..2] run parity classes 1..3 next to class 0 on the caller's stream; [3] runs the weight / bias
   // gradients next to the data-gradient chain (both only read the dZ buffers)
@@ -98,10 +108,25 @@ struct TrainState {
 static constexpr int LOSS_BLOCKS = 1024;
 static constexpr int THIN_CHUNKS = 256;
 static constexpr int BIAS_CHUNKS = 256;  // upper bound; the launch uses min(256, npix / 64) chunks
+static constexpr int kS3MapKey = 1 << 20;
 
 // ---------------------------------------------------------------------------------- small kernels
-__global__ void __launch_bounds__(256) strip_to_nhwc32_kernel(const __nv_bfloat16 *src, __nv_bfloat16 *dst, size_t n_chunks,
-                                                              int Ws) {
+// a bf16 value of the step: hi, plus lo in bf16x3 (hi + lo is exact in fp32)
+template <bool S3>
+__device__ __forceinline__ float ld_pair(const __nv_bfloat16 *hi, const __nv_bfloat16 *lo, size_t i) {
+  return S3 ? __bfloat162float(hi[i]) + __bfloat162float(lo[i]) : __bfloat162float(hi[i]);
+}
+// ... and its store: hi = bf16(v), in bf16x3 also lo = bf16(v - hi)
+template <bool S3>
+__device__ __forceinline__ void st_pair(__nv_bfloat16 *hi, __nv_bfloat16 *lo, size_t i, float v) {
+  const __nv_bfloat16 h = __float2bfloat16_rn(v);
+  hi[i] = h;
+  if (S3) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+}
+
+template <bool S3>
+__global__ void __launch_bounds__(256) strip_to_nhwc32_kernel(const __nv_bfloat16 *src, const __nv_bfloat16 *src_lo, __nv_bfloat16 *dst,
+                                                              __nv_bfloat16 *dst_lo, size_t n_chunks, int Ws) {
   // src [(b*Hs + r)][4][Ws][8] -> dst [(b*Hs + r)][Ws][32]; one 16-byte chunk per thread
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_chunks) return;
@@ -109,35 +134,44 @@ __global__ void __launch_bounds__(256) strip_to_nhwc32_kernel(const __nv_bfloat1
   const int chunk = (int)((i / Ws) % 4);
   const size_t row = i / ((size_t)Ws * 4);
   *reinterpret_cast<uint4 *>(dst + ((row * Ws + col) * 32 + chunk * 8)) = *reinterpret_cast<const uint4 *>(src + i * 8);
+  if (S3) *reinterpret_cast<uint4 *>(dst_lo + ((row * Ws + col) * 32 + chunk * 8)) = *reinterpret_cast<const uint4 *>(src_lo + i * 8);
 }
 
 // RGB-D conv1 input: src [(b*Hs + r)][8][Ws][8] -> dst [(b*Hs + r)][Ws][64] (channel = phase*16 + c); one 16-byte chunk per thread
-__global__ void __launch_bounds__(256) strip_to_nhwc64_kernel(const __nv_bfloat16 *src, __nv_bfloat16 *dst, size_t n_chunks,
-                                                              int Ws) {
+template <bool S3>
+__global__ void __launch_bounds__(256) strip_to_nhwc64_kernel(const __nv_bfloat16 *src, const __nv_bfloat16 *src_lo, __nv_bfloat16 *dst,
+                                                              __nv_bfloat16 *dst_lo, size_t n_chunks, int Ws) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_chunks) return;
   const int col = (int)(i % Ws);
   const int chunk = (int)((i / Ws) % 8);
   const size_t row = i / ((size_t)Ws * 8);
   *reinterpret_cast<uint4 *>(dst + ((row * Ws + col) * 64 + chunk * 8)) = *reinterpret_cast<const uint4 *>(src + i * 8);
+  if (S3) *reinterpret_cast<uint4 *>(dst_lo + ((row * Ws + col) * 64 + chunk * 8)) = *reinterpret_cast<const uint4 *>(src_lo + i * 8);
 }
 
 // copy channels [0,C) of an NHWC buffer's valid region into another buffer (different border / channel stride)
-__global__ void __launch_bounds__(256) copy_interior_kernel(const __nv_bfloat16 *src, int sHp, int sWp, int spy, int spx, int sC,
-                                                            __nv_bfloat16 *dst, int dHp, int dWp, int dpy, int dpx, int dC,
-                                                            int dcoff, int B, int H, int W, int C) {
+template <bool S3>
+__global__ void __launch_bounds__(256) copy_interior_kernel(const __nv_bfloat16 *src, const __nv_bfloat16 *src_lo, int sHp, int sWp, int spy,
+                                                            int spx, int sC, __nv_bfloat16 *dst, __nv_bfloat16 *dst_lo, int dHp, int dWp,
+                                                            int dpy, int dpx, int dC, int dcoff, int B, int H, int W, int C) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int c8n = C / 8;
   if (i >= (size_t)B * H * W * c8n) return;
   const int c8 = (int)(i % c8n);
   const int x = (int)((i / c8n) % W), y = (int)((i / ((size_t)c8n * W)) % H), b = (int)(i / ((size_t)c8n * W * H));
-  const uint4 v = *reinterpret_cast<const uint4 *>(src + (((size_t)b * sHp + y + spy) * sWp + x + spx) * sC + c8 * 8);
-  *reinterpret_cast<uint4 *>(dst + (((size_t)b * dHp + y + dpy) * dWp + x + dpx) * dC + dcoff + c8 * 8) = v;
+  const size_t si = (((size_t)b * sHp + y + spy) * sWp + x + spx) * sC + c8 * 8;
+  const size_t di = (((size_t)b * dHp + y + dpy) * dWp + x + dpx) * dC + dcoff + c8 * 8;
+  *reinterpret_cast<uint4 *>(dst + di) = *reinterpret_cast<const uint4 *>(src + si);
+  if (S3) *reinterpret_cast<uint4 *>(dst_lo + di) = *reinterpret_cast<const uint4 *>(src_lo + si);
 }
 
-// g[c] *= (a[c] > 0 ? 1 : slope) over channels [coff, coff+C) of the valid region (LeakyReLU backward in place)
-__global__ void __launch_bounds__(256) lrelu_mask_inplace_kernel(__nv_bfloat16 *g, const __nv_bfloat16 *a, int Hp, int Wp, int py,
-                                                                 int px, int cs, int coff, int B, int H, int W, int C, float slope) {
+// g[c] *= (a[c] > 0 ? 1 : slope) over channels [coff, coff+C) of the valid region (LeakyReLU backward in place).  bf16x3: g is a
+// pair; the activation's hi half alone decides the mask (hi + lo has the sign of hi, see store_pair_generic)
+template <bool S3>
+__global__ void __launch_bounds__(256) lrelu_mask_inplace_kernel(__nv_bfloat16 *g, __nv_bfloat16 *g_lo, const __nv_bfloat16 *a, int Hp,
+                                                                 int Wp, int py, int px, int cs, int coff, int B, int H, int W, int C,
+                                                                 float slope) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int c8n = C / 8;
   if (i >= (size_t)B * H * W * c8n) return;
@@ -145,21 +179,24 @@ __global__ void __launch_bounds__(256) lrelu_mask_inplace_kernel(__nv_bfloat16 *
   const int x = (int)((i / c8n) % W), y = (int)((i / ((size_t)c8n * W)) % H), b = (int)(i / ((size_t)c8n * W * H));
   const size_t o = (((size_t)b * Hp + y + py) * Wp + x + px) * cs + coff + c8 * 8;
   __align__(16) __nv_bfloat16 gv[8];
+  __align__(16) __nv_bfloat16 gl[8];
   __align__(16) __nv_bfloat16 av[8];
   *reinterpret_cast<uint4 *>(gv) = *reinterpret_cast<const uint4 *>(g + o);
+  if (S3) *reinterpret_cast<uint4 *>(gl) = *reinterpret_cast<const uint4 *>(g_lo + o);
   *reinterpret_cast<uint4 *>(av) = *reinterpret_cast<const uint4 *>(a + o);
 #pragma unroll
   for (int e = 0; e < 8; ++e)
-    if (!(__bfloat162float(av[e]) > 0.f)) gv[e] = __float2bfloat16_rn(__bfloat162float(gv[e]) * slope);
+    if (!(__bfloat162float(av[e]) > 0.f)) st_pair<S3>(gv, gl, e, ld_pair<S3>(gv, gl, e) * slope);
   *reinterpret_cast<uint4 *>(g + o) = *reinterpret_cast<const uint4 *>(gv);
+  if (S3) *reinterpret_cast<uint4 *>(g_lo + o) = *reinterpret_cast<const uint4 *>(gl);
 }
 
 // ---- thin 3x3 / pad 1 convolutions with <= 2 output channels (Convolution1/2/3, mask_conv3): CUDA cores
 // forward: one 128-thread block per output pixel; the 4 warps split the input channels (warp w takes ci = w*32 + lane,
 // + 128, ...) so the dependent-FMA chain per lane is 4x shorter than with one warp per pixel; fixed-order combine
-template <int CO>
-__global__ void __launch_bounds__(128) thin_conv_fwd_kernel(const __nv_bfloat16 *x, int Hp, int Wp, int cs, int Cin, int B, int H,
-                                                            int W, const float *w, const float *bias, float *out) {
+template <int CO, bool S3>
+__global__ void __launch_bounds__(128) thin_conv_fwd_kernel(const __nv_bfloat16 *x, const __nv_bfloat16 *x_lo, int Hp, int Wp, int cs,
+                                                            int Cin, int B, int H, int W, const float *w, const float *bias, float *out) {
   __shared__ float red[4][CO];
   const int pix = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int xx = pix % W, yy = (pix / W) % H, b = pix / (W * H);
@@ -168,9 +205,9 @@ __global__ void __launch_bounds__(128) thin_conv_fwd_kernel(const __nv_bfloat16 
   for (int co = 0; co < CO; ++co) acc[co] = 0.f;
   for (int ky = 0; ky < 3; ++ky)
     for (int kx = 0; kx < 3; ++kx) {
-      const __nv_bfloat16 *px = x + (((size_t)b * Hp + yy + ky) * Wp + xx + kx) * cs;  // border 1 == pad 1
+      const size_t px = (((size_t)b * Hp + yy + ky) * Wp + xx + kx) * cs;  // border 1 == pad 1
       for (int ci = threadIdx.x; ci < Cin; ci += 128) {
-        const float v = __bfloat162float(px[ci]);
+        const float v = ld_pair<S3>(x, x_lo, px + ci);
 #pragma unroll
         for (int co = 0; co < CO; ++co) acc[co] = fmaf(v, w[((ky * 3 + kx) * CO + co) * Cin + ci], acc[co]);  // w = [tap][co][ci]
       }
@@ -186,9 +223,9 @@ __global__ void __launch_bounds__(128) thin_conv_fwd_kernel(const __nv_bfloat16 
 }
 
 // weight gradient, stage 1: thread (ci, tap) x pixel chunk blockIdx.y -> part[chunk][co][ci*9 + tap]
-template <int CO>
-__global__ void __launch_bounds__(256) thin_conv_wgrad_kernel(const __nv_bfloat16 *x, int Hp, int Wp, int cs, int Cin, int B, int H,
-                                                              int W, const float *dy, float *part) {
+template <int CO, bool S3>
+__global__ void __launch_bounds__(256) thin_conv_wgrad_kernel(const __nv_bfloat16 *x, const __nv_bfloat16 *x_lo, int Hp, int Wp, int cs,
+                                                              int Cin, int B, int H, int W, const float *dy, float *part) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= Cin * 9) return;
   const int ci = i % Cin, tap = i / Cin, ky = tap / 3, kx = tap % 3;
@@ -199,7 +236,7 @@ __global__ void __launch_bounds__(256) thin_conv_wgrad_kernel(const __nv_bfloat1
   for (int co = 0; co < CO; ++co) acc[co] = 0.f;
   int xx = p0 % W, yy = (p0 / W) % H, b = p0 / (W * H);
   for (int p = p0; p < p1; ++p) {
-    const float v = __bfloat162float(x[(((size_t)b * Hp + yy + ky) * Wp + xx + kx) * cs + ci]);
+    const float v = ld_pair<S3>(x, x_lo, (((size_t)b * Hp + yy + ky) * Wp + xx + kx) * cs + ci);
     const float *d = dy + (size_t)p * CO;
 #pragma unroll
     for (int co = 0; co < CO; ++co) acc[co] = fmaf(v, d[co], acc[co]);
@@ -237,10 +274,10 @@ __global__ void __launch_bounds__(256) thin_conv_wgrad_final_kernel(const float 
 }
 
 // data gradient: one thread per (pixel, ci); writes (accumulate = 0) or adds to a bf16 NHWC buffer with border 1
-template <int CO>
+template <int CO, bool S3>
 __global__ void __launch_bounds__(256) thin_conv_dgrad_kernel(const float *dy, const float *w, int Cin, int B, int H, int W,
-                                                              __nv_bfloat16 *dx, int Hp, int Wp, int py, int px, int cs,
-                                                              int c_write, int accumulate) {
+                                                              __nv_bfloat16 *dx, __nv_bfloat16 *dx_lo, int Hp, int Wp, int py, int px,
+                                                              int cs, int c_write, int accumulate) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (size_t)B * H * W * c_write) return;
   const int ci = (int)(i % c_write);
@@ -258,15 +295,16 @@ __global__ void __launch_bounds__(256) thin_conv_dgrad_kernel(const float *dy, c
         for (int co = 0; co < CO; ++co) acc = fmaf(d[co], w[((ky * 3 + kx) * CO + co) * Cin + ci], acc);  // w = [tap][co][ci]
       }
     }
-  __nv_bfloat16 *o = dx + (((size_t)b * Hp + yy + py) * Wp + xx + px) * cs + ci;
-  if (accumulate) acc += __bfloat162float(*o);
-  *o = __float2bfloat16_rn(acc);
+  const size_t o = (((size_t)b * Hp + yy + py) * Wp + xx + px) * cs + ci;
+  if (accumulate) acc += ld_pair<S3>(dx, dx_lo, o);
+  st_pair<S3>(dx, dx_lo, o, acc);
 }
 
 // ---- thin 2 -> 2 deconvolution k4 s2 + Crop(offset 1) (upsample_flow6to5 / 5to4)
+template <bool S3>
 __global__ void __launch_bounds__(256) thin_deconv_fwd_kernel(const float *in, int B, int Hi, int Wi, const float *w, const float *bias,
-                                                              __nv_bfloat16 *out, int Hp, int Wp, int py, int px, int cs, int coff,
-                                                              int Ho, int Wo) {
+                                                              __nv_bfloat16 *out, __nv_bfloat16 *out_lo, int Hp, int Wp, int py, int px,
+                                                              int cs, int coff, int Ho, int Wo) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * Ho * Wo * 2) return;
   const int co = i & 1, ox = (i >> 1) % Wo, oy = ((i >> 1) / Wo) % Ho, b = (i >> 1) / (Wo * Ho);
@@ -282,18 +320,20 @@ __global__ void __launch_bounds__(256) thin_deconv_fwd_kernel(const float *in, i
       acc = fmaf(p[1], w[((1 * 2 + co) * 4 + ky) * 4 + kx], acc);
     }
   }
-  out[(((size_t)b * Hp + oy + py) * Wp + ox + px) * cs + coff + co] = __float2bfloat16_rn(acc);
+  st_pair<S3>(out, out_lo, (((size_t)b * Hp + oy + py) * Wp + ox + px) * cs + coff + co, acc);
 }
 
 // backward of the thin deconvolution: din (one thread per input pixel x ci)
-__device__ __forceinline__ float thin_dY(const __nv_bfloat16 *dout, int Hp, int Wp, int py, int px, int cs, int coff, int Ho, int Wo,
-                                         int b, int oy, int ox, int co) {
+template <bool S3>
+__device__ __forceinline__ float thin_dY(const __nv_bfloat16 *dout, const __nv_bfloat16 *dout_lo, int Hp, int Wp, int py, int px, int cs,
+                                         int coff, int Ho, int Wo, int b, int oy, int ox, int co) {
   if (oy < 0 || oy >= Ho || ox < 0 || ox >= Wo) return 0.f;
-  return __bfloat162float(dout[(((size_t)b * Hp + oy + py) * Wp + ox + px) * cs + coff + co]);
+  return ld_pair<S3>(dout, dout_lo, (((size_t)b * Hp + oy + py) * Wp + ox + px) * cs + coff + co);
 }
+template <bool S3>
 __global__ void __launch_bounds__(256) thin_deconv_bwd_kernel(const float *in, int B, int Hi, int Wi, const float *w,
-                                                              const __nv_bfloat16 *dout, int Hp, int Wp, int py, int px, int cs,
-                                                              int coff, int Ho, int Wo, float *din) {
+                                                              const __nv_bfloat16 *dout, const __nv_bfloat16 *dout_lo, int Hp, int Wp,
+                                                              int py, int px, int cs, int coff, int Ho, int Wo, float *din) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * Hi * Wi * 2) return;
   const int ci = i & 1, ix = (i >> 1) % Wi, iy = ((i >> 1) / Wi) % Hi, b = (i >> 1) / (Wi * Hi);
@@ -301,14 +341,15 @@ __global__ void __launch_bounds__(256) thin_deconv_bwd_kernel(const float *in, i
   for (int ky = 0; ky < 4; ++ky)
     for (int kx = 0; kx < 4; ++kx)
       for (int co = 0; co < 2; ++co)
-        acc = fmaf(thin_dY(dout, Hp, Wp, py, px, cs, coff, Ho, Wo, b, 2 * iy + ky - 1, 2 * ix + kx - 1, co),
+        acc = fmaf(thin_dY<S3>(dout, dout_lo, Hp, Wp, py, px, cs, coff, Ho, Wo, b, 2 * iy + ky - 1, 2 * ix + kx - 1, co),
                    w[((ci * 2 + co) * 4 + ky) * 4 + kx], acc);
   din[i] = acc;
 }
 // dw (64 values) and db (2 values): one block per output, threads stride over the pixels, fixed-order tree reduction
-__global__ void __launch_bounds__(256) thin_deconv_wgrad_kernel(const float *in, int B, int Hi, int Wi, const __nv_bfloat16 *dout, int Hp,
-                                                                int Wp, int py, int px, int cs, int coff, int Ho, int Wo, float *dw,
-                                                                float *db) {
+template <bool S3>
+__global__ void __launch_bounds__(256) thin_deconv_wgrad_kernel(const float *in, int B, int Hi, int Wi, const __nv_bfloat16 *dout,
+                                                                const __nv_bfloat16 *dout_lo, int Hp, int Wp, int py, int px, int cs,
+                                                                int coff, int Ho, int Wo, float *dw, float *db) {
   __shared__ float red[256];
   const int t = blockIdx.x;  // 0..63: dw[((ci*2+co)*4+ky)*4+kx], 64..65: db[co]
   float acc = 0.f;
@@ -316,13 +357,14 @@ __global__ void __launch_bounds__(256) thin_deconv_wgrad_kernel(const float *in,
     const int kx = t & 3, ky = (t >> 2) & 3, co = (t >> 4) & 1, ci = t >> 5;
     for (int p = threadIdx.x; p < B * Hi * Wi; p += 256) {
       const int ix = p % Wi, iy = (p / Wi) % Hi, b = p / (Wi * Hi);
-      acc = fmaf(in[(size_t)p * 2 + ci], thin_dY(dout, Hp, Wp, py, px, cs, coff, Ho, Wo, b, 2 * iy + ky - 1, 2 * ix + kx - 1, co), acc);
+      acc = fmaf(in[(size_t)p * 2 + ci], thin_dY<S3>(dout, dout_lo, Hp, Wp, py, px, cs, coff, Ho, Wo, b, 2 * iy + ky - 1, 2 * ix + kx - 1, co),
+                 acc);
     }
   } else {
     const int co = t - 64;
     for (int p = threadIdx.x; p < B * Ho * Wo; p += 256) {
       const int ox = p % Wo, oy = (p / Wo) % Ho, b = p / (Wo * Ho);
-      acc += thin_dY(dout, Hp, Wp, py, px, cs, coff, Ho, Wo, b, oy, ox, co);
+      acc += thin_dY<S3>(dout, dout_lo, Hp, Wp, py, px, cs, coff, Ho, Wo, b, oy, ox, co);
     }
   }
   red[threadIdx.x] = acc;
@@ -519,13 +561,22 @@ __global__ void __launch_bounds__(256) fc_wgrad_kernel(const float *dy, const fl
 
 // fc6 weight gradient; the flat vector keeps fc6_weight as (256, h*10+w, c) -- the NHWC order of ReLU10 -- so both the
 // activation reads and the gradient writes are coalesced (the host API permutes to MXNet's (256, c*80+hw) on load / get)
-__global__ void __launch_bounds__(256) fc6_wgrad_kernel(const float *dh6, const __nv_bfloat16 *a10, int B, float *dw) {
+template <bool S3>
+__global__ void __launch_bounds__(256) fc6_wgrad_kernel(const float *dh6, const __nv_bfloat16 *a10, const __nv_bfloat16 *a10_lo, int B,
+                                                        float *dw) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // over 81920 / 2 pairs of k
   if (i >= 81920 / 2) return;
   float2 a[16];
 #pragma unroll
   for (int b = 0; b < 16; ++b)
-    if (b < B) a[b] = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(a10 + (size_t)b * 81920 + 2 * i));
+    if (b < B) {
+      a[b] = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(a10 + (size_t)b * 81920 + 2 * i));
+      if (S3) {
+        const float2 l = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(a10_lo + (size_t)b * 81920 + 2 * i));
+        a[b].x += l.x;
+        a[b].y += l.y;
+      }
+    }
   for (int o = blockIdx.y * 32; o < blockIdx.y * 32 + 32; ++o) {
     float2 acc = make_float2(0.f, 0.f);
 #pragma unroll
@@ -536,9 +587,10 @@ __global__ void __launch_bounds__(256) fc6_wgrad_kernel(const float *dh6, const 
 }
 // fc6 data gradient, added to the bf16 partial gradient of ReLU10 ([B][80][1024]).  Block = 64 consecutive k (2 per lane),
 // warp w streams output rows o in [32w, 32w+32) of the packed bf16 weight matrix; the 8 partial sums per (b, k) are
-// combined through shared memory in fixed order.
-__global__ void __launch_bounds__(256) fc6_dgrad_kernel(const float *dh6, const __nv_bfloat16 *w_hi /*[256][81920] packed*/, int B,
-                                                        __nv_bfloat16 *dA) {
+// combined through shared memory in fixed order.  bf16x3: the weights are w_hi + w_lo and dA is a pair.
+template <bool S3>
+__global__ void __launch_bounds__(256) fc6_dgrad_kernel(const float *dh6, const __nv_bfloat16 *w_hi /*[256][81920] packed*/,
+                                                        const __nv_bfloat16 *w_lo, int B, __nv_bfloat16 *dA, __nv_bfloat16 *dA_lo) {
   __shared__ float red[8][16][64];
   __shared__ float dh[16][256];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -550,7 +602,12 @@ __global__ void __launch_bounds__(256) fc6_dgrad_kernel(const float *dh6, const 
   for (int b = 0; b < 16; ++b) acc[b] = make_float2(0.f, 0.f);
 #pragma unroll 4
   for (int o = warp * 32; o < warp * 32 + 32; ++o) {
-    const float2 w = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(w_hi + (size_t)o * 81920 + k0));
+    float2 w = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(w_hi + (size_t)o * 81920 + k0));
+    if (S3) {
+      const float2 l = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(w_lo + (size_t)o * 81920 + k0));
+      w.x += l.x;
+      w.y += l.y;
+    }
 #pragma unroll
     for (int b = 0; b < 16; ++b) {
       const float d = dh[b][o];
@@ -569,20 +626,22 @@ __global__ void __launch_bounds__(256) fc6_dgrad_kernel(const float *dh6, const 
     float s = 0.f;
 #pragma unroll
     for (int w8 = 0; w8 < 8; ++w8) s += red[w8][b][kk];
-    __nv_bfloat16 *o = dA + (size_t)b * 81920 + blockIdx.x * 64 + kk;
-    *o = __float2bfloat16_rn(__bfloat162float(*o) + s);
+    const size_t o = (size_t)b * 81920 + blockIdx.x * 64 + kk;
+    st_pair<S3>(dA, dA_lo, o, ld_pair<S3>(dA, dA_lo, o) + s);
   }
 }
 
 // bias gradient = per-channel sum over all pixels of a bf16 NHWC buffer (zero border included), two stages
-__global__ void __launch_bounds__(256) bias_partial_kernel(const __nv_bfloat16 *g, size_t npix, int cs, int coff, int C, float *part) {
+template <bool S3>
+__global__ void __launch_bounds__(256) bias_partial_kernel(const __nv_bfloat16 *g, const __nv_bfloat16 *g_lo, size_t npix, int cs, int coff,
+                                                           int C, float *part) {
   const int c = blockIdx.x * 64 + (threadIdx.x & 63), lanep = threadIdx.x >> 6, chunk = blockIdx.y;
   __shared__ float red[4][64];
   const size_t per = (npix + gridDim.y - 1) / gridDim.y;
   const size_t p0 = (size_t)chunk * per, p1 = p0 + per < npix ? p0 + per : npix;
   float a = 0.f;
   if (c < C)
-    for (size_t p = p0 + lanep; p < p1; p += 4) a += __bfloat162float(g[p * cs + coff + c]);
+    for (size_t p = p0 + lanep; p < p1; p += 4) a += ld_pair<S3>(g, g_lo, p * cs + coff + c);
   red[lanep][threadIdx.x & 63] = a;
   __syncthreads();
   if (threadIdx.x < 64 && c < C)
@@ -656,7 +715,8 @@ __global__ void __launch_bounds__(256) pack_conv1_kernel(const float *w, __nv_bf
 }
 // data-gradient packs of ALL parity classes of one layer: class (ry, rx) is [Cin][Ty][Tx][Cout] with ky = ry + s*(Ty-1-ty).
 // block = (ci, 64 output channels): reads 64 rows of k*k floats, writes 64 consecutive bf16 per (class, tap)
-struct DgradPackDst { __nv_bfloat16 *p[4]; };
+// lo[c] = nullptr: no lo half (bf16 step); otherwise the bf16x3 residual pack of class c
+struct DgradPackDst { __nv_bfloat16 *p[4], *lo[4]; };
 __global__ void __launch_bounds__(256) pack_dgrad_kernel(const float *w, int Cout, int Cin, int k, int s, DgradPackDst dst) {
   __shared__ float tile[64 * 25];
   const int ci = blockIdx.x, co0 = blockIdx.y * 64, kk = k * k;
@@ -672,7 +732,7 @@ __global__ void __launch_bounds__(256) pack_dgrad_kernel(const float *w, int Cou
     for (int i = threadIdx.x; i < Ty * Tx * 64; i += 256) {
       const int tt = i >> 6, col = i & 63;
       const int ky = ry + s * (Ty - 1 - tt / Tx), kx = rx + s * (Tx - 1 - tt % Tx);
-      dst.p[c][((size_t)ci * Ty * Tx + tt) * Cout + co0 + col] = __float2bfloat16_rn(tile[col * kk + ky * k + kx]);
+      store_split(dst.p[c], dst.lo[c], ((size_t)ci * Ty * Tx + tt) * Cout + co0 + col, tile[col * kk + ky * k + kx]);
     }
   }
 }
@@ -689,18 +749,19 @@ __global__ void __launch_bounds__(256) pack_deconv_fwd_kernel(const float *w, in
   for (int i = threadIdx.x; i < 4 * 4 * 64; i += 256) {
     const int cl = i & 63, t = (i >> 6) & 3, c = i >> 8;
     const int ky = (c >> 1) + 2 * (1 - t / 2), kx = (c & 1) + 2 * (1 - t % 2);
-    if (c0 + cl < Cin_eff) dst.p[c][((size_t)co * 4 + t) * Cin_eff + c0 + cl] = __float2bfloat16_rn(tile[cl * 16 + ky * 4 + kx]);
+    if (c0 + cl < Cin_eff) store_split(dst.p[c], dst.lo[c], ((size_t)co * 4 + t) * Cin_eff + c0 + cl, tile[cl * 16 + ky * 4 + kx]);
   }
 }
 // deconvolution data gradient = stride-2 4x4 convolution: [Cin_eff][4][4][Cout]; block = one ci: Cout*16 contiguous floats in
-__global__ void __launch_bounds__(256) pack_deconv_dgrad_kernel(const float *w, int Cin, int Cout, int Cin_eff, __nv_bfloat16 *dst) {
+__global__ void __launch_bounds__(256) pack_deconv_dgrad_kernel(const float *w, int Cin, int Cout, int Cin_eff, __nv_bfloat16 *dst,
+                                                                __nv_bfloat16 *dst_lo) {
   extern __shared__ float dtile[];  // [Cout][17] (padded: the transposed read below would otherwise hit 2 banks)
   const int ci = blockIdx.x;
   for (int i = threadIdx.x; i < Cout * 16; i += 256) dtile[(i >> 4) * 17 + (i & 15)] = ci < Cin ? w[(size_t)ci * Cout * 16 + i] : 0.f;
   __syncthreads();
   for (int i = threadIdx.x; i < Cout * 16; i += 256) {
     const int co = i % Cout, tap = i / Cout;
-    dst[((size_t)ci * 16 + tap) * Cout + co] = __float2bfloat16_rn(dtile[co * 17 + tap]);
+    store_split(dst, dst_lo, ((size_t)ci * 16 + tap) * Cout + co, dtile[co * 17 + tap]);
   }
 }
 // fc6 master (out, hw, c) fp32 -> bf16 hi/lo operand (same order)
@@ -845,20 +906,23 @@ void train_destroy(dim_ctx *ctx) {
   } while (0)
 
 // refresh every bf16 operand pack (and the fp32 head parameters of the inference net) from the master weights
-// with_lo = false skips the bf16 'lo' halves (only the bf16x3 inference mode reads them); they are then marked stale and
-// refreshed lazily by train_refresh_lo() the next time that mode runs
+// with_lo = false skips the bf16 'lo' halves (only the bf16x3 modes read them); they are then marked stale and refreshed
+// lazily by train_refresh_lo() the next time the bf16x3 inference mode runs, or by the switch of the step to bf16x3
 static int repack_all(dim_ctx *ctx, cudaStream_t st, bool with_lo) {
   NetState *ns = ctx->net;
   TrainState *ts = train_of(ctx);
   const float *M = ts->master;
   if (ts->input_depth) LAUNCH1D(pack_conv1_rgbd_kernel, 64 * 1024, st, M + ts->off[0].w, ns->w_hi[0], with_lo ? ns->w_lo[0] : nullptr);
   else LAUNCH1D(pack_conv1_kernel, 64 * 512, st, M + ts->off[0].w, ns->w_hi[0], with_lo ? ns->w_lo[0] : nullptr);
+  // the training packs' lo halves exist once the step has run in bf16x3 (nullptr before)
+  auto L = [with_lo](__nv_bfloat16 *lo) { return with_lo ? lo : nullptr; };
   for (int i = 1; i < 10; ++i) {
     const LayerSpec &s = kLayers[i];
     pack_conv_fwd_kernel<<<dim3(s.Cout, cdiv(s.Cin, 64)), 256, 0, st>>>(M + ts->off[i].w, s.Cout, s.Cin, s.k, ns->w_hi[i],
                                                                           with_lo ? ns->w_lo[i] : nullptr);
     DIM_LAUNCH_CHECK();
-    DgradPackDst d{{ts->dg_pack[i][0], ts->dg_pack[i][1], ts->dg_pack[i][2], ts->dg_pack[i][3]}};
+    DgradPackDst d{{ts->dg_pack[i][0], ts->dg_pack[i][1], ts->dg_pack[i][2], ts->dg_pack[i][3]},
+                   {L(ts->dg_pack_lo[i][0]), L(ts->dg_pack_lo[i][1]), L(ts->dg_pack_lo[i][2]), L(ts->dg_pack_lo[i][3])}};
     pack_dgrad_kernel<<<dim3(s.Cin, s.Cout / 64), 256, 0, st>>>(M + ts->off[i].w, s.Cout, s.Cin, s.k, s.stride, d);
     DIM_LAUNCH_CHECK();
   }
@@ -867,7 +931,10 @@ static int repack_all(dim_ctx *ctx, cudaStream_t st, bool with_lo) {
   ns->f16_stale = true;  // the fp16 packs of DIM_PREC_FP16 are re-derived from hi/lo when that mode next runs
   LAUNCH1D(transpose256_kernel, 65536, st, M + ts->off[P_FC7].w, ns->fc7_wT);
   {
-    DgradPackDst d5{{ts->d5_fwd[0], ts->d5_fwd[1], ts->d5_fwd[2], ts->d5_fwd[3]}}, d4{{ts->d4_fwd[0], ts->d4_fwd[1], ts->d4_fwd[2], ts->d4_fwd[3]}};
+    DgradPackDst d5{{ts->d5_fwd[0], ts->d5_fwd[1], ts->d5_fwd[2], ts->d5_fwd[3]},
+                    {L(ts->d5_fwd_lo[0]), L(ts->d5_fwd_lo[1]), L(ts->d5_fwd_lo[2]), L(ts->d5_fwd_lo[3])}};
+    DgradPackDst d4{{ts->d4_fwd[0], ts->d4_fwd[1], ts->d4_fwd[2], ts->d4_fwd[3]},
+                    {L(ts->d4_fwd_lo[0]), L(ts->d4_fwd_lo[1]), L(ts->d4_fwd_lo[2]), L(ts->d4_fwd_lo[3])}};
     pack_deconv_fwd_kernel<<<dim3(512, 1024 / 64), 256, 0, st>>>(M + ts->off[P_DECONV5].w, 1024, 512, 1024, d5);
     DIM_LAUNCH_CHECK();
     pack_deconv_fwd_kernel<<<dim3(256, 1088 / 64), 256, 0, st>>>(M + ts->off[P_DECONV4].w, 1026, 256, 1088, d4);
@@ -877,9 +944,9 @@ static int repack_all(dim_ctx *ctx, cudaStream_t st, bool with_lo) {
   LAUNCH1D(pack_thin_kernel, 2 * 1026 * 9, st, M + ts->off[P_CONV2D].w, 2, 1026, ts->thin_w[1]);
   LAUNCH1D(pack_thin_kernel, 2 * 770 * 9, st, M + ts->off[P_CONV3D].w, 2, 770, ts->thin_w[2]);
   LAUNCH1D(pack_thin_kernel, 1 * 770 * 9, st, M + ts->off[P_MASK3].w, 1, 770, ts->thin_w[3]);
-  pack_deconv_dgrad_kernel<<<1024, 256, 512 * 17 * 4, st>>>(M + ts->off[P_DECONV5].w, 1024, 512, 1024, ts->d5_dg);
+  pack_deconv_dgrad_kernel<<<1024, 256, 512 * 17 * 4, st>>>(M + ts->off[P_DECONV5].w, 1024, 512, 1024, ts->d5_dg, L(ts->d5_dg_lo));
   DIM_LAUNCH_CHECK();
-  pack_deconv_dgrad_kernel<<<1088, 256, 256 * 17 * 4, st>>>(M + ts->off[P_DECONV4].w, 1026, 256, 1088, ts->d4_dg);
+  pack_deconv_dgrad_kernel<<<1088, 256, 256 * 17 * 4, st>>>(M + ts->off[P_DECONV4].w, 1026, 256, 1088, ts->d4_dg, L(ts->d4_dg_lo));
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -913,6 +980,64 @@ int train_refresh_lo(dim_ctx *ctx, cudaStream_t st) {
   return repack_all(ctx, st, true);
 }
 
+// the lo halves of the step's bf16 buffers and of its operand packs (bf16x3); zero-filled, so borders and padding channels
+// start (and stay) zero in both halves
+static int alloc_lo(dim_ctx *ctx, TrainState *ts) {
+  const int B = ctx->max_batch;
+  int rc = 0;
+  Buf *bufs[] = {&ts->act10b, &ts->cat2, &ts->cat3, &ts->dcat2, &ts->dcat3, &ts->dA10p, ts->input_depth ? &ts->s2d64 : &ts->s2d32};
+  for (Buf *b : bufs) rc |= dev_alloc(ctx, &b->lo, b->per_image() * B, true);
+  for (int i = 0; i < 10; ++i) rc |= dev_alloc(ctx, &ts->gz[i].lo, ts->gz[i].per_image() * B, true);
+  for (int i = 1; i < 10; ++i) {
+    const LayerSpec &s = kLayers[i];
+    for (int c = 0; c < (s.stride == 2 ? 4 : 1); ++c) {
+      const int Ty = s.stride == 2 ? (s.k - (c >> 1) + 1) / 2 : s.k, Tx = s.stride == 2 ? (s.k - (c & 1) + 1) / 2 : s.k;
+      rc |= dev_alloc(ctx, &ts->dg_pack_lo[i][c], (size_t)s.Cin * Ty * Tx * s.Cout, true);  // exact class size
+    }
+  }
+  for (int c = 0; c < 4; ++c) {
+    rc |= dev_alloc(ctx, &ts->d5_fwd_lo[c], (size_t)512 * 4 * 1024, true);
+    rc |= dev_alloc(ctx, &ts->d4_fwd_lo[c], (size_t)256 * 4 * 1088, true);
+  }
+  rc |= dev_alloc(ctx, &ts->d5_dg_lo, (size_t)1024 * 16 * 512, true);
+  rc |= dev_alloc(ctx, &ts->d4_dg_lo, (size_t)1088 * 16 * 256, true);
+  if (rc) {
+    set_error("dim_train_set_precision: device allocation failed (%d)", rc);
+    return 12;
+  }
+  ts->lo_alloc = true;
+  return 0;
+}
+
+int train_set_precision(dim_ctx *ctx, int precision) {
+  TrainState *ts = train_of(ctx);
+  DIM_REQUIRE(ts != nullptr, "dim_train_set_precision: call dim_train_create first");
+  DIM_REQUIRE(precision == DIM_PREC_BF16 || precision == DIM_PREC_BF16X3,
+              "dim_train_set_precision: the training step runs in DIM_PREC_BF16 or DIM_PREC_BF16X3");
+  const bool s3 = precision == DIM_PREC_BF16X3;
+  if (s3 == ts->s3) return 0;
+  if (s3) {
+    // not on the hot path: wait for every stream of the context, allocate once, then bring every lo half up to the master
+    // weights (updates made in bf16 left them stale)
+    DIM_CHECK(cudaDeviceSynchronize());
+    if (!ts->lo_alloc)
+      if (int rc = alloc_lo(ctx, ts)) return rc;
+    if (ctx->net->loaded && ctx->net->train_aliased) {
+      if (int rc = repack_all(ctx, ts->side[3], true)) return rc;
+      DIM_CHECK(cudaStreamSynchronize(ts->side[3]));
+    }
+  }
+  ts->s3 = s3;
+  return 0;
+}
+
+int train_get_precision(dim_ctx *ctx, int *precision) {
+  TrainState *ts = train_of(ctx);
+  DIM_REQUIRE(ts != nullptr, "dim_train_get_precision: call dim_train_create first");
+  *precision = ts->s3 ? DIM_PREC_BF16X3 : DIM_PREC_BF16;
+  return 0;
+}
+
 int train_get_params(dim_ctx *ctx, float *flat_host, size_t n, int which, cudaStream_t st) {
   TrainState *ts = train_of(ctx);
   DIM_REQUIRE(ts != nullptr && n == ts->n_params, "dim_train_get_params: bad state or size");
@@ -944,26 +1069,31 @@ static void pick_tile(int W, int rows_total, int cap, int &BW, int &BH, int max_
   }
 }
 
-template <int BN, int ST>
+template <int BN, int ST, bool S3 = false>
 static int launch_generic(const ConvKParams &kp, int total_tiles, int n_tiles, int cap, cudaStream_t st) {
-  using S = ConvSmem2<BN, ST, false>;
+  using S = ConvSmem2<BN, ST, S3>;
   static bool attr_set = false;
   if (!attr_set) {
-    DIM_CHECK(cudaFuncSetAttribute(conv_igemm_persistent_kernel<BN, ST, false, false, 1>,
+    DIM_CHECK(cudaFuncSetAttribute(conv_igemm_persistent_kernel<BN, ST, S3, false, 1>,
                                    cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
     attr_set = true;
   }
   const int grid = total_tiles < cap ? total_tiles : cap;
-  conv_igemm_persistent_kernel<BN, ST, false, false, 1><<<grid, 384, S::TOTAL, st>>>(kp, total_tiles, n_tiles);
+  conv_igemm_persistent_kernel<BN, ST, S3, false, 1><<<grid, 384, S::TOTAL, st>>>(kp, total_tiles, n_tiles);
   DIM_LAUNCH_CHECK();
   return 0;
 }
 
-// one CTA per SM with the deepest ring that fits (STAGES x stage bytes <= 192 KB)
-static int run_generic(dim_ctx *ctx, const ConvKParams &kp, const LayerGeom &g, int B, cudaStream_t st) {
+// one CTA per SM with the deepest ring that fits (STAGES x stage bytes <= 192 KB; bf16x3 stages hold hi and lo operands)
+static int run_generic(dim_ctx *ctx, const ConvKParams &kp, const LayerGeom &g, int B, cudaStream_t st, bool s3) {
   const int n_tiles = cdiv(g.Cout, g.BLOCK_N);
   const int total = cdiv(B * g.Hq, g.BH) * g.n_col_tiles * n_tiles;
   const int sms = ctx->num_sms;
+  if (s3) {
+    if (g.BLOCK_N == 256) return launch_generic<256, 2, true>(kp, total, n_tiles, sms, st);
+    if (g.BLOCK_N == 128) return launch_generic<128, 3, true>(kp, total, n_tiles, sms, st);
+    return launch_generic<64, 4, true>(kp, total, n_tiles, sms, st);
+  }
   if (g.BLOCK_N == 256) return launch_generic<256, 4>(kp, total, n_tiles, sms, st);
   if (g.BLOCK_N == 128) return launch_generic<128, 6>(kp, total, n_tiles, sms, st);
   return launch_generic<64, 8>(kp, total, n_tiles, sms, st);
@@ -972,12 +1102,13 @@ static int run_generic(dim_ctx *ctx, const ConvKParams &kp, const LayerGeom &g, 
 // Describe one launch of the generic kernel.
 //   in      : bf16 NHWC input buffer (border included), channels [in_coff, in_coff + K_ch) are the K range
 //   stride2 : read through the 4 parity views (k4 s2 convolution), else stride-1 taps with (off_r, off_c)
-//   w       : [N][KH*KW][K_ch] bf16 pack
+//   w, w_lo : [N][KH*KW][K_ch] bf16 pack and its lo half
 //   out     : output buffer; virtual pixel (oh, ow) -> interior (oh*sy + oy, ow*sx + ox)
+//   s3      : bf16x3 (SPLIT3): also the lo maps of the input and the weights, the lo halves of out and addend
 static int make_generic(ConvKParams &kp, LayerGeom &g, int B, const Buf &in, int in_coff, int K_ch, bool stride2, int KH, int KW,
-                        int off_r, int off_c, int Ho, int Wo, const __nv_bfloat16 *w, int N, const float *bias, float slope,
-                        const Buf &out, int out_coff, int sy, int sx, int oy, int ox, const Buf *addend, int add_coff,
-                        const Buf *mask, int mask_coff, int mask_climit) {
+                        int off_r, int off_c, int Ho, int Wo, const __nv_bfloat16 *w, const __nv_bfloat16 *w_lo, int N,
+                        const float *bias, float slope, const Buf &out, int out_coff, int sy, int sx, int oy, int ox,
+                        const Buf *addend, int add_coff, const Buf *mask, int mask_coff, int mask_climit, bool s3) {
   memset(&kp, 0, sizeof(kp));
   memset(&g, 0, sizeof(g));
   g.Cout = N; g.KH = KH; g.KW = KW; g.BLOCK_K = 64;
@@ -987,53 +1118,55 @@ static int make_generic(ConvKParams &kp, LayerGeom &g, int B, const Buf &in, int
   g.n_col_tiles = cdiv(Wo, g.BW);
   g.kblocks = KH * KW * (K_ch / 64);
   const uint32_t box[3] = {64u, (uint32_t)g.BW, (uint32_t)g.BH};
-  if (!stride2) {
-    const uint64_t dims[3] = {(uint64_t)K_ch, (uint64_t)in.Wp, (uint64_t)B * in.Hp};
-    const uint64_t str[2] = {(uint64_t)in.C * 2, (uint64_t)in.Wp * in.C * 2};
-    if (int rc = encode_map(&kp.a_map[0], in.p + in_coff, 3, dims, str, box, 64)) return rc;
-    kp.a_map[1] = kp.a_map[2] = kp.a_map[3] = kp.a_map[0];
-  } else {
-    for (int ph = 0; ph < 2; ++ph)
-      for (int pw = 0; pw < 2; ++pw) {
-        const uint64_t dims[3] = {(uint64_t)K_ch, (uint64_t)in.Wp / 2, (uint64_t)B * in.Hp / 2};
-        const uint64_t str[2] = {(uint64_t)2 * in.C * 2, (uint64_t)2 * in.Wp * in.C * 2};
-        if (int rc = encode_map(&kp.a_map[(ph << 1) | pw], in.p + ((size_t)ph * in.Wp + pw) * in.C + in_coff, 3, dims, str, box, 64))
-          return rc;
-      }
-  }
-  {
+  for (int lo = 0; lo < (s3 ? 2 : 1); ++lo) {
+    __nv_bfloat16 *base = lo ? in.lo : in.p;
+    CUtensorMap *a_map = lo ? kp.a_lo_map : kp.a_map;
+    if (!stride2) {
+      const uint64_t dims[3] = {(uint64_t)K_ch, (uint64_t)in.Wp, (uint64_t)B * in.Hp};
+      const uint64_t str[2] = {(uint64_t)in.C * 2, (uint64_t)in.Wp * in.C * 2};
+      if (int rc = encode_map(&a_map[0], base + in_coff, 3, dims, str, box, 64)) return rc;
+      a_map[1] = a_map[2] = a_map[3] = a_map[0];
+    } else {
+      for (int ph = 0; ph < 2; ++ph)
+        for (int pw = 0; pw < 2; ++pw) {
+          const uint64_t dims[3] = {(uint64_t)K_ch, (uint64_t)in.Wp / 2, (uint64_t)B * in.Hp / 2};
+          const uint64_t str[2] = {(uint64_t)2 * in.C * 2, (uint64_t)2 * in.Wp * in.C * 2};
+          if (int rc = encode_map(&a_map[(ph << 1) | pw], base + ((size_t)ph * in.Wp + pw) * in.C + in_coff, 3, dims, str, box, 64))
+            return rc;
+        }
+    }
     const uint64_t Ktot = (uint64_t)KH * KW * K_ch;
     const uint64_t dims[2] = {Ktot, (uint64_t)N};
     const uint64_t str[1] = {Ktot * 2};
     const uint32_t boxw[2] = {64u, (uint32_t)g.BLOCK_N};
-    if (int rc = encode_map(&kp.b_map, const_cast<__nv_bfloat16 *>(w), 2, dims, str, boxw, 64)) return rc;
+    if (int rc = encode_map(lo ? &kp.b_lo_map : &kp.b_map, const_cast<__nv_bfloat16 *>(lo ? w_lo : w), 2, dims, str, boxw, 64)) return rc;
   }
   kp.KH = KH; kp.KW = KW; kp.stride = stride2 ? 2 : 1; kp.cchunks = K_ch / 64;
   kp.BW = g.BW; kp.BH = g.BH; kp.n_col_tiles = g.n_col_tiles;
   kp.Hq = g.Hq; kp.Ho = Ho; kp.Wo = Wo; kp.Bn = B;
   kp.out_Hp = out.Hp; kp.out_Wp = out.Wp; kp.out_py = out.py; kp.out_px = out.px; kp.Cout = N;
   kp.kblocks = g.kblocks;
-  kp.slope = slope; kp.bias = bias; kp.out_hi = out.p; kp.out_lo = nullptr;
+  kp.slope = slope; kp.bias = bias; kp.out_hi = out.p; kp.out_lo = s3 ? out.lo : nullptr;
   kp.in_off_r = off_r; kp.in_off_c = off_c;
   kp.out_sy = sy; kp.out_sx = sx; kp.out_oy = oy; kp.out_ox = ox; kp.out_H = out.H; kp.out_W = out.W;
   kp.out_cs = out.C; kp.out_coff = out_coff;
-  if (addend) kp.addend = {addend->p, addend->Hp, addend->Wp, addend->py, addend->px, addend->C, add_coff};
-  if (mask) kp.mask = {mask->p, mask->Hp, mask->Wp, mask->py, mask->px, mask->C, mask_coff};
+  if (addend) kp.addend = {addend->p, addend->Hp, addend->Wp, addend->py, addend->px, addend->C, add_coff, s3 ? addend->lo : nullptr};
+  if (mask) kp.mask = {mask->p, mask->Hp, mask->Wp, mask->py, mask->px, mask->C, mask_coff, nullptr};  // hi decides the sign
   kp.mask_climit = mask_climit;
   return 0;
 }
 
 // ------------------------------------------------------------------------------ wgrad launches
-template <int BN, int ST>
+template <int BN, int ST, bool S3 = false>
 static int launch_wgrad(const WgradParams &p, cudaStream_t st) {
-  using S = WgradSmem<BN, ST>;
+  using S = WgradSmem<BN, ST, S3>;
   static bool attr_set = false;
   if (!attr_set) {
-    DIM_CHECK(cudaFuncSetAttribute(conv_wgrad_kernel<BN, ST>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+    DIM_CHECK(cudaFuncSetAttribute(conv_wgrad_kernel<BN, ST, S3>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
     attr_set = true;
   }
   const int grid = p.KH * p.KW * p.m_tiles * p.n_tiles * p.kslices;
-  conv_wgrad_kernel<BN, ST><<<grid, 384, S::TOTAL, st>>>(p);
+  conv_wgrad_kernel<BN, ST, S3><<<grid, 384, S::TOTAL, st>>>(p);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -1047,7 +1180,7 @@ static int encode_map4(CUtensorMap *m, __nv_bfloat16 *base, uint64_t C, uint64_t
 }
 
 // Z: M-side buffer (channels [z_coff, z_coff+M)), iterated over its valid H x W region; A: N-side buffer, read at
-// (y*s + kh, x*s + kw) in ITS bordered coordinates (+ a_off)
+// (y*s + kh, x*s + kw) in ITS bordered coordinates (+ a_off); bf16x3 (ts->s3): also the maps of both lo halves
 static int make_wgrad(TrainState *ts, WgradParams &p, int &BN, int B, const Buf &Z, int z_coff, int M, int H, int W, const Buf &A,
                       int a_coff, int N, int stride, int KH, int KW, int a_off_r, int a_off_c, int sms) {
   memset(&p, 0, sizeof(p));
@@ -1074,28 +1207,38 @@ static int make_wgrad(TrainState *ts, WgradParams &p, int &BN, int B, const Buf 
   p.kb_per_slice = cdiv(p.kb_total, ks);
   p.kslices = cdiv(p.kb_total, p.kb_per_slice);
   p.partial = ts->wg_partial;
-  if (int rc = encode_map4(&p.z_map, Z.p + z_coff, M, Z.Wp, Z.Hp, B, Z.C, (uint64_t)Z.Wp * Z.C, (uint64_t)Z.Hp * Z.Wp * Z.C, 64, p.BW, p.BH))
-    return rc;
   const uint32_t boxc = BN >= 64 ? 64 : 32;
-  if (stride == 1) {
-    if (int rc = encode_map4(&p.a_map[0], A.p + a_coff, N, A.Wp, A.Hp, B, A.C, (uint64_t)A.Wp * A.C, (uint64_t)A.Hp * A.Wp * A.C, boxc,
-                             p.BW, p.BH))
+  for (int lo = 0; lo < (ts->s3 ? 2 : 1); ++lo) {
+    __nv_bfloat16 *zb = lo ? Z.lo : Z.p, *ab = lo ? A.lo : A.p;
+    CUtensorMap *a_map = lo ? p.a_lo_map : p.a_map;
+    if (int rc = encode_map4(lo ? &p.z_lo_map : &p.z_map, zb + z_coff, M, Z.Wp, Z.Hp, B, Z.C, (uint64_t)Z.Wp * Z.C,
+                             (uint64_t)Z.Hp * Z.Wp * Z.C, 64, p.BW, p.BH))
       return rc;
-    p.a_map[1] = p.a_map[2] = p.a_map[3] = p.a_map[0];
-  } else {
-    for (int ph = 0; ph < 2; ++ph)
-      for (int pw = 0; pw < 2; ++pw)
-        if (int rc = encode_map4(&p.a_map[(ph << 1) | pw], A.p + ((size_t)ph * A.Wp + pw) * A.C + a_coff, N, A.Wp / 2, A.Hp / 2, B,
-                                 (uint64_t)2 * A.C, (uint64_t)2 * A.Wp * A.C, (uint64_t)A.Hp * A.Wp * A.C, boxc, p.BW, p.BH))
-          return rc;
+    if (stride == 1) {
+      if (int rc = encode_map4(&a_map[0], ab + a_coff, N, A.Wp, A.Hp, B, A.C, (uint64_t)A.Wp * A.C, (uint64_t)A.Hp * A.Wp * A.C, boxc,
+                               p.BW, p.BH))
+        return rc;
+      a_map[1] = a_map[2] = a_map[3] = a_map[0];
+    } else {
+      for (int ph = 0; ph < 2; ++ph)
+        for (int pw = 0; pw < 2; ++pw)
+          if (int rc = encode_map4(&a_map[(ph << 1) | pw], ab + ((size_t)ph * A.Wp + pw) * A.C + a_coff, N, A.Wp / 2, A.Hp / 2, B,
+                                   (uint64_t)2 * A.C, (uint64_t)2 * A.Wp * A.C, (uint64_t)A.Hp * A.Wp * A.C, boxc, p.BW, p.BH))
+            return rc;
+    }
   }
   return 0;
 }
 
-static int run_wgrad(const WgradParams &p, int BN, int kind, int D0, int D1, int k, float *grad, cudaStream_t st) {
+static int run_wgrad(const WgradParams &p, int BN, bool s3, int kind, int D0, int D1, int k, float *grad, cudaStream_t st) {
   int rc;
-  // one CTA per SM, ring depth = what fits in ~192 KB of shared memory
-  if (BN == 256) rc = launch_wgrad<256, 4>(p, st);
+  // one CTA per SM, ring depth = what fits in ~192 KB of shared memory (bf16x3: a stage holds the hi and the lo operands)
+  if (s3) {
+    if (BN == 256) rc = launch_wgrad<256, 2, true>(p, st);
+    else if (BN == 128) rc = launch_wgrad<128, 3, true>(p, st);
+    else if (BN == 64) rc = launch_wgrad<64, 4, true>(p, st);
+    else rc = launch_wgrad<32, 5, true>(p, st);
+  } else if (BN == 256) rc = launch_wgrad<256, 4>(p, st);
   else if (BN == 128) rc = launch_wgrad<128, 6>(p, st);
   else if (BN == 64) rc = launch_wgrad<64, 8>(p, st);
   else rc = launch_wgrad<32, 8>(p, st);
@@ -1108,13 +1251,19 @@ static int run_wgrad(const WgradParams &p, int BN, int kind, int D0, int D1, int
 }
 
 // conv1: one GEMM per filter row (conv1_wgrad_kernel); p was built by make_wgrad for the 16-tap form, only the slicing differs
-static int run_wgrad_conv1(TrainState *ts, const WgradParams &p16, int sms, float *grad, cudaStream_t st) {
-  using S = Conv1WgradSmem<8>;
+template <int ST, bool S3>
+static int launch_wgrad_conv1(const WgradParams &p, cudaStream_t st) {
+  using S = Conv1WgradSmem<ST, S3>;
   static bool attr_set = false;
   if (!attr_set) {
-    DIM_CHECK(cudaFuncSetAttribute(conv1_wgrad_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+    DIM_CHECK(cudaFuncSetAttribute(conv1_wgrad_kernel<ST, S3>, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
     attr_set = true;
   }
+  conv1_wgrad_kernel<ST, S3><<<4 * p.kslices, 384, S::TOTAL, st>>>(p);
+  DIM_LAUNCH_CHECK();
+  return 0;
+}
+static int run_wgrad_conv1(TrainState *ts, const WgradParams &p16, int sms, float *grad, cudaStream_t st) {
   WgradParams p = p16;
   int ks = cdiv(2 * sms, 4);
   if (ks > p.kb_total / 2) ks = p.kb_total / 2;
@@ -1122,8 +1271,7 @@ static int run_wgrad_conv1(TrainState *ts, const WgradParams &p16, int sms, floa
   p.kb_per_slice = cdiv(p.kb_total, ks);
   p.kslices = cdiv(p.kb_total, p.kb_per_slice);
   DIM_REQUIRE((size_t)p.kslices * 4 * 128 * 64 <= ts->wg_partial_elems, "wgrad workspace too small");
-  conv1_wgrad_kernel<8><<<4 * p.kslices, 384, S::TOTAL, st>>>(p);
-  DIM_LAUNCH_CHECK();
+  if (int rc = ts->s3 ? launch_wgrad_conv1<4, true>(p, st) : launch_wgrad_conv1<8, false>(p, st)) return rc;
   const size_t total = (size_t)4 * 128 * 64;
   wgrad_reduce_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(p.partial, p.kslices, 4, 128, 64, WG_CONV1_ROW, 64, 8, 7, grad);
   DIM_LAUNCH_CHECK();
@@ -1134,7 +1282,8 @@ static int bias_grad(TrainState *ts, const Buf &g, int B, int coff, int C, float
   const size_t npix = (size_t)B * g.Hp * g.Wp;
   int chunks = (int)(npix / 64);
   chunks = chunks < 1 ? 1 : (chunks > BIAS_CHUNKS ? BIAS_CHUNKS : chunks);
-  bias_partial_kernel<<<dim3(cdiv(C, 64), chunks), 256, 0, st>>>(g.p, npix, g.C, coff, C, ts->bias_part);
+  (ts->s3 ? bias_partial_kernel<true> : bias_partial_kernel<false>)<<<dim3(cdiv(C, 64), chunks), 256, 0, st>>>(g.p, g.lo, npix, g.C, coff,
+                                                                                                            C, ts->bias_part);
   DIM_LAUNCH_CHECK();
   bias_final_kernel<<<cdiv(C, 256), 256, 0, st>>>(ts->bias_part, chunks, C, db);
   DIM_LAUNCH_CHECK();
@@ -1146,7 +1295,8 @@ static int thin_wgrad(TrainState *ts, const Buf &x, int Cin, int B, int H, int W
   const int npix = B * H * W;
   int chunks = npix / 32;
   chunks = chunks < 1 ? 1 : (chunks > THIN_CHUNKS ? THIN_CHUNKS : chunks);
-  thin_conv_wgrad_kernel<CO><<<dim3(cdiv(Cin * 9, 256), chunks), 256, 0, st>>>(x.p, x.Hp, x.Wp, x.C, Cin, B, H, W, dy, ts->thin_part);
+  (ts->s3 ? thin_conv_wgrad_kernel<CO, true> : thin_conv_wgrad_kernel<CO, false>)<<<dim3(cdiv(Cin * 9, 256), chunks), 256, 0, st>>>(
+      x.p, x.lo, x.Hp, x.Wp, x.C, Cin, B, H, W, dy, ts->thin_part);
   DIM_LAUNCH_CHECK();
   thin_conv_wgrad_final_kernel<CO><<<cdiv(CO * Cin * 9, 256) + 1, 256, 0, st>>>(ts->thin_part, chunks, Cin, dy, npix, dw, db);
   DIM_LAUNCH_CHECK();
@@ -1155,13 +1305,13 @@ static int thin_wgrad(TrainState *ts, const Buf &x, int Cin, int B, int H, int W
 
 static int thin_deconv_bwd(const float *in, int B, int Hi, int Wi, const float *w, const Buf &dout, int coff, int Ho, int Wo, float *din,
                            float *dw, float *db, cudaStream_t st, cudaStream_t sw, TrainState *ts) {
-  thin_deconv_bwd_kernel<<<cdiv(B * Hi * Wi * 2, 256), 256, 0, st>>>(in, B, Hi, Wi, w, dout.p, dout.Hp, dout.Wp, dout.py, dout.px, dout.C,
-                                                                      coff, Ho, Wo, din);
+  (ts->s3 ? thin_deconv_bwd_kernel<true> : thin_deconv_bwd_kernel<false>)<<<cdiv(B * Hi * Wi * 2, 256), 256, 0, st>>>(
+      in, B, Hi, Wi, w, dout.p, dout.lo, dout.Hp, dout.Wp, dout.py, dout.px, dout.C, coff, Ho, Wo, din);
   DIM_LAUNCH_CHECK();
   DIM_CHECK(cudaEventRecord(ts->ev_fork, st));  // dout is final on st; the weight gradient is off the critical path
   DIM_CHECK(cudaStreamWaitEvent(sw, ts->ev_fork, 0));
-  thin_deconv_wgrad_kernel<<<66, 256, 0, sw>>>(in, B, Hi, Wi, dout.p, dout.Hp, dout.Wp, dout.py, dout.px, dout.C, coff, Ho,
-                                                                Wo, dw, db);
+  (ts->s3 ? thin_deconv_wgrad_kernel<true> : thin_deconv_wgrad_kernel<false>)<<<66, 256, 0, sw>>>(
+      in, B, Hi, Wi, dout.p, dout.lo, dout.Hp, dout.Wp, dout.py, dout.px, dout.C, coff, Ho, Wo, dw, db);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -1171,10 +1321,10 @@ static Buf act_buf(const NetState *ns, int i) {  // act[i] as a Buf (input of en
   Buf b;
   if (i < 10) {
     const LayerGeom &g = ns->g[i];
-    b.p = ns->act_hi[i]; b.Hp = g.rows; b.Wp = g.cols; b.py = g.py; b.px = g.px; b.C = g.Cbuf; b.H = g.Hin; b.W = g.Win;
+    b.p = ns->act_hi[i]; b.lo = ns->act_lo[i]; b.Hp = g.rows; b.Wp = g.cols; b.py = g.py; b.px = g.px; b.C = g.Cbuf; b.H = g.Hin; b.W = g.Win;
   } else {
     const LayerGeom &g = ns->g[9];
-    b.p = ns->act_hi[10]; b.Hp = g.Ho; b.Wp = g.Wo; b.py = b.px = 0; b.C = g.Cout; b.H = g.Ho; b.W = g.Wo;
+    b.p = ns->act_hi[10]; b.lo = ns->act_lo[10]; b.Hp = g.Ho; b.Wp = g.Wo; b.py = b.px = 0; b.C = g.Cout; b.H = g.Ho; b.W = g.Wo;
   }
   return b;
 }
@@ -1184,26 +1334,27 @@ static int build_train_maps(dim_ctx *ctx, int B, TrainMaps &tm) {
   TrainState *ts = train_of(ctx);
   const float *M = ts->master;
   const int sms = ctx->num_sms;
+  const bool s3 = ts->s3;
   // decoder forward: 4 parity classes each; output pixel = 2q + r - 1 (Crop offset 1)
   for (int c = 0; c < 4; ++c) {
     const int ry = c >> 1, rx = c & 1;
     if (int rc = make_generic(tm.deconv5_fwd[c], tm.g_deconv5_fwd[c], B, ts->act10b, 0, 1024, false, 2, 2, 0, 0, ts->act10b.H + 1,
-                              ts->act10b.W + 1, ts->d5_fwd[c], 512, M + ts->off[P_DECONV5].b, 0.1f, ts->cat2, 512, 2, 2, ry - 1, rx - 1,
-                              nullptr, 0, nullptr, 0, 0))
+                              ts->act10b.W + 1, ts->d5_fwd[c], ts->d5_fwd_lo[c], 512, M + ts->off[P_DECONV5].b, 0.1f, ts->cat2, 512, 2, 2,
+                              ry - 1, rx - 1, nullptr, 0, nullptr, 0, 0, s3))
       return rc;
     if (int rc = make_generic(tm.deconv4_fwd[c], tm.g_deconv4_fwd[c], B, ts->cat2, 0, 1088, false, 2, 2, 0, 0, ts->cat2.H + 1,
-                              ts->cat2.W + 1, ts->d4_fwd[c], 256, M + ts->off[P_DECONV4].b, 0.1f, ts->cat3, 512, 2, 2, ry - 1, rx - 1,
-                              nullptr, 0, nullptr, 0, 0))
+                              ts->cat2.W + 1, ts->d4_fwd[c], ts->d4_fwd_lo[c], 256, M + ts->off[P_DECONV4].b, 0.1f, ts->cat3, 512, 2, 2,
+                              ry - 1, rx - 1, nullptr, 0, nullptr, 0, 0, s3))
       return rc;
   }
   // decoder data gradients (stride-2 4x4 convolutions of the bordered output-gradient canvases)
   {
     const Buf a10 = act_buf(ns, 10);
     if (int rc = make_generic(tm.deconv5_dgrad, tm.g_deconv5_dgrad, B, ts->dcat2, 512, 512, true, 4, 4, 0, 0, ts->act10b.H, ts->act10b.W,
-                              ts->d5_dg, 1024, nullptr, 0.1f, ts->gz[9], 0, 1, 1, 0, 0, &ts->dA10p, 0, &a10, 0, 1024))
+                              ts->d5_dg, ts->d5_dg_lo, 1024, nullptr, 0.1f, ts->gz[9], 0, 1, 1, 0, 0, &ts->dA10p, 0, &a10, 0, 1024, s3))
       return rc;
     if (int rc = make_generic(tm.deconv4_dgrad, tm.g_deconv4_dgrad, B, ts->dcat3, 512, 256, true, 4, 4, 0, 0, ts->cat2.H, ts->cat2.W,
-                              ts->d4_dg, 1088, nullptr, 1.0f, ts->dcat2, 0, 1, 1, 0, 0, nullptr, 0, nullptr, 0, 0))
+                              ts->d4_dg, ts->d4_dg_lo, 1088, nullptr, 1.0f, ts->dcat2, 0, 1, 1, 0, 0, nullptr, 0, nullptr, 0, 0, s3))
       return rc;
   }
   // encoder data gradients, layers 9..1 -> gz[i-1]
@@ -1227,7 +1378,8 @@ static int build_train_maps(dim_ctx *ctx, int B, TrainMaps &tm) {
         Ty = Tx = s.k; offr = offc = 0; oy = ox = 0; sy = 1; Jy = lg.Hin; Jx = lg.Win;
       }
       if (int rc = make_generic(tm.dgrad[i][c], tm.g_dgrad[i][c], B, ts->gz[i], 0, s.Cout, false, Ty, Tx, offr, offc, Jy, Jx,
-                                ts->dg_pack[i][c], s.Cin, nullptr, 0.1f, ts->gz[i - 1], 0, sy, sy, oy, ox, addend, 0, &ai, 0, s.Cin))
+                                ts->dg_pack[i][c], ts->dg_pack_lo[i][c], s.Cin, nullptr, 0.1f, ts->gz[i - 1], 0, sy, sy, oy, ox, addend, 0,
+                                &ai, 0, s.Cin, s3))
         return rc;
     }
   }
@@ -1254,10 +1406,10 @@ static int build_train_maps(dim_ctx *ctx, int B, TrainMaps &tm) {
   return 0;
 }
 
-static int copy_interior(const Buf &src, Buf &dst, int dcoff, int B, int C, cudaStream_t st) {
+static int copy_interior(const Buf &src, Buf &dst, int dcoff, int B, int C, cudaStream_t st, bool s3) {
   const size_t n = (size_t)B * src.H * src.W * (C / 8);
-  copy_interior_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(src.p, src.Hp, src.Wp, src.py, src.px, src.C, dst.p, dst.Hp, dst.Wp,
-                                                                     dst.py, dst.px, dst.C, dcoff, B, src.H, src.W, C);
+  (s3 ? copy_interior_kernel<true> : copy_interior_kernel<false>)<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+      src.p, src.lo, src.Hp, src.Wp, src.py, src.px, src.C, dst.p, dst.lo, dst.Hp, dst.Wp, dst.py, dst.px, dst.C, dcoff, B, src.H, src.W, C);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -1268,16 +1420,16 @@ static int run_classes(dim_ctx *ctx, TrainState *ts, const ConvKParams *kp, cons
   const int tiles0 = cdiv(B * g[0].Hq, g[0].BH) * g[0].n_col_tiles * cdiv(g[0].Cout, g[0].BLOCK_N);
   if (n == 1 || tiles0 >= ctx->num_sms) {
     for (int c = 0; c < n; ++c)
-      if (int rc = run_generic(ctx, kp[c], g[c], B, st)) return rc;
+      if (int rc = run_generic(ctx, kp[c], g[c], B, st, ts->s3)) return rc;
     return 0;
   }
   DIM_CHECK(cudaEventRecord(ts->ev_fork, st));
   for (int c = 1; c < n; ++c) {
     DIM_CHECK(cudaStreamWaitEvent(ts->side[c - 1], ts->ev_fork, 0));
-    if (int rc = run_generic(ctx, kp[c], g[c], B, ts->side[c - 1])) return rc;
+    if (int rc = run_generic(ctx, kp[c], g[c], B, ts->side[c - 1], ts->s3)) return rc;
     DIM_CHECK(cudaEventRecord(ts->ev_cls[c - 1], ts->side[c - 1]));
   }
-  if (int rc = run_generic(ctx, kp[0], g[0], B, st)) return rc;
+  if (int rc = run_generic(ctx, kp[0], g[0], B, st, ts->s3)) return rc;
   for (int c = 1; c < n; ++c) DIM_CHECK(cudaStreamWaitEvent(st, ts->ev_cls[c - 1], 0));
   return 0;
 }
@@ -1305,11 +1457,13 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
   const bool labels = io.zflow && io.zfw && io.zmask_gt && io.src_pose && io.pc_model && io.pc_weights && io.pc_observed && io.N >= 1;
   DIM_REQUIRE(labels || io.grads == nullptr, "dim_train_forward_backward: the backward pass needs every label");
   DIM_REQUIRE(labels || (!io.zflow && !io.zfw && !io.zmask_gt && !io.pc_model), "dim_train_forward_backward: pass all labels or none");
-  auto it = ts->maps.find(B);
+  const bool s3 = ts->s3;
+  const int key = B + (s3 ? kS3MapKey : 0);
+  auto it = ts->maps.find(key);
   if (it == ts->maps.end()) {
     TrainMaps tm;
     if (int rc = build_train_maps(ctx, B, tm)) return rc;
-    it = ts->maps.emplace(B, tm).first;
+    it = ts->maps.emplace(key, tm).first;
   }
   const TrainMaps &tm = it->second;
   const float *M = ts->master;
@@ -1327,34 +1481,38 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
               "dim_train_forward_backward: the RGB-D network takes both zoomed depths, the RGB network none");
   if (ts->input_depth) {
     if (int rc = pack_nhwc10_launch(ctx, io.zio, io.zir, io.zdo, io.zdr, io.zmo, io.zmr, B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0],
-                                    nullptr, st, 0))
+                                    s3 ? ns->act_lo[0] : nullptr, st, 0))
       return rc;
-  } else if (int rc = pack_nhwc8_launch(ctx, io.zio, io.zir, io.zmo, io.zmr, B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0], nullptr, st, 0)) {
+  } else if (int rc = pack_nhwc8_launch(ctx, io.zio, io.zir, io.zmo, io.zmr, B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0],
+                                        s3 ? ns->act_lo[0] : nullptr, st, 0)) {
     return rc;
   }
-  if (int rc = net_forward(ctx, B, DIM_PREC_BF16, nullptr, ts->rot_raw, ts->ztrans, nullptr, st, nullptr)) return rc;
+  if (int rc = net_forward(ctx, B, s3 ? DIM_PREC_BF16X3 : DIM_PREC_BF16, nullptr, ts->rot_raw, ts->ztrans, nullptr, st, nullptr)) return rc;
   DIM_CHECK(cudaEventRecord(ts->ev_phase[1], st));
   const Buf a10 = act_buf(ns, 10), a8 = act_buf(ns, 8), a6 = act_buf(ns, 6);
-  if (int rc = copy_interior(a10, ts->act10b, 0, B, 1024, st)) return rc;
-  thin_conv_fwd_kernel<2><<<B * h6 * w6, 128, 0, st>>>(ts->act10b.p, ts->act10b.Hp, ts->act10b.Wp, 1024, 1024, B, h6, w6,
-           ts->thin_w[0], M + ts->off[P_CONV1D].b, ts->flow6);
+  auto thin_fwd2 = s3 ? thin_conv_fwd_kernel<2, true> : thin_conv_fwd_kernel<2, false>;
+  auto thin_fwd1 = s3 ? thin_conv_fwd_kernel<1, true> : thin_conv_fwd_kernel<1, false>;
+  auto thin_deconv_fwd = s3 ? thin_deconv_fwd_kernel<true> : thin_deconv_fwd_kernel<false>;
+  if (int rc = copy_interior(a10, ts->act10b, 0, B, 1024, st, s3)) return rc;
+  thin_fwd2<<<B * h6 * w6, 128, 0, st>>>(ts->act10b.p, ts->act10b.lo, ts->act10b.Hp, ts->act10b.Wp, 1024, 1024, B, h6, w6, ts->thin_w[0],
+                                         M + ts->off[P_CONV1D].b, ts->flow6);
   DIM_LAUNCH_CHECK();
   if (int rc = run_classes(ctx, ts, tm.deconv5_fwd, tm.g_deconv5_fwd, 4, B, st)) return rc;
-  if (int rc = copy_interior(a8, ts->cat2, 0, B, 512, st)) return rc;
-  LAUNCH1D(thin_deconv_fwd_kernel, (size_t)B * h5 * w5 * 2, st, ts->flow6, B, h6, w6, M + ts->off[P_UP65].w, M + ts->off[P_UP65].b,
-           ts->cat2.p, ts->cat2.Hp, ts->cat2.Wp, 1, 1, 1088, 1024, h5, w5);
-  thin_conv_fwd_kernel<2><<<B * h5 * w5, 128, 0, st>>>(ts->cat2.p, ts->cat2.Hp, ts->cat2.Wp, 1088, 1026, B, h5, w5,
-           ts->thin_w[1], M + ts->off[P_CONV2D].b, ts->flow5);
+  if (int rc = copy_interior(a8, ts->cat2, 0, B, 512, st, s3)) return rc;
+  LAUNCH1D(thin_deconv_fwd, (size_t)B * h5 * w5 * 2, st, ts->flow6, B, h6, w6, M + ts->off[P_UP65].w, M + ts->off[P_UP65].b,
+           ts->cat2.p, ts->cat2.lo, ts->cat2.Hp, ts->cat2.Wp, 1, 1, 1088, 1024, h5, w5);
+  thin_fwd2<<<B * h5 * w5, 128, 0, st>>>(ts->cat2.p, ts->cat2.lo, ts->cat2.Hp, ts->cat2.Wp, 1088, 1026, B, h5, w5, ts->thin_w[1],
+                                         M + ts->off[P_CONV2D].b, ts->flow5);
   DIM_LAUNCH_CHECK();
   if (int rc = run_classes(ctx, ts, tm.deconv4_fwd, tm.g_deconv4_fwd, 4, B, st)) return rc;
-  if (int rc = copy_interior(a6, ts->cat3, 0, B, 512, st)) return rc;
-  LAUNCH1D(thin_deconv_fwd_kernel, (size_t)B * h4 * w4 * 2, st, ts->flow5, B, h5, w5, M + ts->off[P_UP54].w, M + ts->off[P_UP54].b,
-           ts->cat3.p, ts->cat3.Hp, ts->cat3.Wp, 1, 1, 832, 768, h4, w4);
-  thin_conv_fwd_kernel<2><<<B * h4 * w4, 128, 0, st>>>(ts->cat3.p, ts->cat3.Hp, ts->cat3.Wp, 832, 770, B, h4, w4,
-           ts->thin_w[2], M + ts->off[P_CONV3D].b, ts->flow4);
+  if (int rc = copy_interior(a6, ts->cat3, 0, B, 512, st, s3)) return rc;
+  LAUNCH1D(thin_deconv_fwd, (size_t)B * h4 * w4 * 2, st, ts->flow5, B, h5, w5, M + ts->off[P_UP54].w, M + ts->off[P_UP54].b,
+           ts->cat3.p, ts->cat3.lo, ts->cat3.Hp, ts->cat3.Wp, 1, 1, 832, 768, h4, w4);
+  thin_fwd2<<<B * h4 * w4, 128, 0, st>>>(ts->cat3.p, ts->cat3.lo, ts->cat3.Hp, ts->cat3.Wp, 832, 770, B, h4, w4, ts->thin_w[2],
+                                         M + ts->off[P_CONV3D].b, ts->flow4);
   DIM_LAUNCH_CHECK();
-  thin_conv_fwd_kernel<1><<<B * h4 * w4, 128, 0, st>>>(ts->cat3.p, ts->cat3.Hp, ts->cat3.Wp, 832, 770, B, h4, w4,
-           ts->thin_w[3], M + ts->off[P_MASK3].b, ts->mask4);
+  thin_fwd1<<<B * h4 * w4, 128, 0, st>>>(ts->cat3.p, ts->cat3.lo, ts->cat3.Hp, ts->cat3.Wp, 832, 770, B, h4, w4, ts->thin_w[3],
+                                         M + ts->off[P_MASK3].b, ts->mask4);
   DIM_LAUNCH_CHECK();
   DIM_CHECK(cudaEventRecord(ts->ev_phase[2], st));
   fullres_loss_kernel<<<LOSS_BLOCKS, 256, 0, st>>>(ts->flow4, ts->mask4, h4, w4, M + ts->off[P_UPS].w, M + ts->off[P_MUPS].w, io.zflow,
@@ -1396,7 +1554,8 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
   LAUNCH1D(fc_wgrad_kernel, 4 * 256, sw, ts->drot, ts->h7, B, 4, 256, G + ts->off[P_ROT].w, G + ts->off[P_ROT].b);
   LAUNCH1D(fc_wgrad_kernel, 3 * 256, sw, ts->dtrans, ts->h7, B, 3, 256, G + ts->off[P_TRANS].w, G + ts->off[P_TRANS].b);
   LAUNCH1D(fc_wgrad_kernel, 256 * 256, sw, ts->dh7, ts->h6, B, 256, 256, G + ts->off[P_FC7].w, G + ts->off[P_FC7].b);
-  fc6_wgrad_kernel<<<dim3(81920 / 2 / 256, 8), 256, 0, sw>>>(ts->dh6, ns->act_hi[10], B, G + ts->off[P_FC6].w);
+  (s3 ? fc6_wgrad_kernel<true> : fc6_wgrad_kernel<false>)<<<dim3(81920 / 2 / 256, 8), 256, 0, sw>>>(ts->dh6, ns->act_hi[10], ns->act_lo[10],
+                                                                                                     B, G + ts->off[P_FC6].w);
   DIM_LAUNCH_CHECK();
   LAUNCH1D(fc_wgrad_kernel, 256, sw, ts->dh6, ts->h6 /*unused for K=0*/, B, 256, 0, G + ts->off[P_FC6].w /*no write*/, G + ts->off[P_FC6].b);
   DIM_CHECK(cudaEventRecord(ts->ev_phase[4], st));
@@ -1407,49 +1566,53 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
   if (int rc = fork_side(ts, st)) return rc;
   if (int rc = thin_wgrad<2>(ts, ts->cat3, 770, B, h4, w4, ts->dflow4, G + ts->off[P_CONV3D].w, G + ts->off[P_CONV3D].b, sw)) return rc;
   if (int rc = thin_wgrad<1>(ts, ts->cat3, 770, B, h4, w4, ts->dmask4, G + ts->off[P_MASK3].w, G + ts->off[P_MASK3].b, sw)) return rc;
-  LAUNCH1D(thin_conv_dgrad_kernel<2>, (size_t)B * h4 * w4 * 832, st, ts->dflow4, ts->thin_w[2], 770, B, h4, w4, ts->dcat3.p,
+  auto thin_dgrad2 = s3 ? thin_conv_dgrad_kernel<2, true> : thin_conv_dgrad_kernel<2, false>;
+  auto thin_dgrad1 = s3 ? thin_conv_dgrad_kernel<1, true> : thin_conv_dgrad_kernel<1, false>;
+  auto lrelu_mask_inplace = s3 ? lrelu_mask_inplace_kernel<true> : lrelu_mask_inplace_kernel<false>;
+  LAUNCH1D(thin_dgrad2, (size_t)B * h4 * w4 * 832, st, ts->dflow4, ts->thin_w[2], 770, B, h4, w4, ts->dcat3.p, ts->dcat3.lo,
            ts->dcat3.Hp, ts->dcat3.Wp, 1, 1, 832, 832, 0);
-  LAUNCH1D(thin_conv_dgrad_kernel<1>, (size_t)B * h4 * w4 * 832, st, ts->dmask4, ts->thin_w[3], 770, B, h4, w4, ts->dcat3.p,
+  LAUNCH1D(thin_dgrad1, (size_t)B * h4 * w4 * 832, st, ts->dmask4, ts->thin_w[3], 770, B, h4, w4, ts->dcat3.p, ts->dcat3.lo,
            ts->dcat3.Hp, ts->dcat3.Wp, 1, 1, 832, 832, 1);
   // upsample_flow5to4
   if (int rc = thin_deconv_bwd(ts->flow5, B, h5, w5, M + ts->off[P_UP54].w, ts->dcat3, 768, h4, w4, ts->dflow5, G + ts->off[P_UP54].w,
                                G + ts->off[P_UP54].b, st, sw, ts))
     return rc;
   // deconv4: LeakyReLU backward on its slice, bias, weight and data gradients
-  LAUNCH1D(lrelu_mask_inplace_kernel, (size_t)B * h4 * w4 * 32, st, ts->dcat3.p, ts->cat3.p, ts->cat3.Hp, ts->cat3.Wp, 1, 1, 832, 512, B, h4,
-           w4, 256, 0.1f);
+  LAUNCH1D(lrelu_mask_inplace, (size_t)B * h4 * w4 * 32, st, ts->dcat3.p, ts->dcat3.lo, ts->cat3.p, ts->cat3.Hp, ts->cat3.Wp, 1, 1, 832,
+           512, B, h4, w4, 256, 0.1f);
   if (int rc = fork_side(ts, st)) return rc;
   if (int rc = bias_grad(ts, ts->dcat3, B, 512, 256, G + ts->off[P_DECONV4].b, sw)) return rc;
-  if (int rc = run_wgrad(tm.wg_deconv4, tm.wg_bn_d4, WG_DECONV, 1026, 256, 4, G + ts->off[P_DECONV4].w, sw)) return rc;
-  if (int rc = run_generic(ctx, tm.deconv4_dgrad, tm.g_deconv4_dgrad, B, st)) return rc;
+  if (int rc = run_wgrad(tm.wg_deconv4, tm.wg_bn_d4, s3, WG_DECONV, 1026, 256, 4, G + ts->off[P_DECONV4].w, sw)) return rc;
+  if (int rc = run_generic(ctx, tm.deconv4_dgrad, tm.g_deconv4_dgrad, B, st, s3)) return rc;
   // Convolution2 (adds to dcat2), upsample_flow6to5
   if (int rc = thin_wgrad<2>(ts, ts->cat2, 1026, B, h5, w5, ts->dflow5, G + ts->off[P_CONV2D].w, G + ts->off[P_CONV2D].b, sw)) return rc;  // dflow5 was final before the last fork
-  LAUNCH1D(thin_conv_dgrad_kernel<2>, (size_t)B * h5 * w5 * 1088, st, ts->dflow5, ts->thin_w[1], 1026, B, h5, w5, ts->dcat2.p,
+  LAUNCH1D(thin_dgrad2, (size_t)B * h5 * w5 * 1088, st, ts->dflow5, ts->thin_w[1], 1026, B, h5, w5, ts->dcat2.p, ts->dcat2.lo,
            ts->dcat2.Hp, ts->dcat2.Wp, 1, 1, 1088, 1088, 1);
   if (int rc = thin_deconv_bwd(ts->flow6, B, h6, w6, M + ts->off[P_UP65].w, ts->dcat2, 1024, h5, w5, ts->dflow6, G + ts->off[P_UP65].w,
                                G + ts->off[P_UP65].b, st, sw, ts))
     return rc;
   // deconv5
-  LAUNCH1D(lrelu_mask_inplace_kernel, (size_t)B * h5 * w5 * 64, st, ts->dcat2.p, ts->cat2.p, ts->cat2.Hp, ts->cat2.Wp, 1, 1, 1088, 512, B, h5,
-           w5, 512, 0.1f);
+  LAUNCH1D(lrelu_mask_inplace, (size_t)B * h5 * w5 * 64, st, ts->dcat2.p, ts->dcat2.lo, ts->cat2.p, ts->cat2.Hp, ts->cat2.Wp, 1, 1, 1088,
+           512, B, h5, w5, 512, 0.1f);
   if (int rc = fork_side(ts, st)) return rc;
   if (int rc = bias_grad(ts, ts->dcat2, B, 512, 512, G + ts->off[P_DECONV5].b, sw)) return rc;
-  if (int rc = run_wgrad(tm.wg_deconv5, tm.wg_bn_d5, WG_DECONV, 1024, 512, 4, G + ts->off[P_DECONV5].w, sw)) return rc;
+  if (int rc = run_wgrad(tm.wg_deconv5, tm.wg_bn_d5, s3, WG_DECONV, 1024, 512, 4, G + ts->off[P_DECONV5].w, sw)) return rc;
   // Convolution1 -> partial gradient of ReLU10, + fc6 data gradient, then deconv5's data gradient closes dZ of conv6_1
   if (int rc = thin_wgrad<2>(ts, ts->act10b, 1024, B, h6, w6, ts->dflow6, G + ts->off[P_CONV1D].w, G + ts->off[P_CONV1D].b, sw)) return rc;  // dflow6: before the last fork
-  LAUNCH1D(thin_conv_dgrad_kernel<2>, (size_t)B * h6 * w6 * 1024, st, ts->dflow6, ts->thin_w[0], 1024, B, h6, w6, ts->dA10p.p,
+  LAUNCH1D(thin_dgrad2, (size_t)B * h6 * w6 * 1024, st, ts->dflow6, ts->thin_w[0], 1024, B, h6, w6, ts->dA10p.p, ts->dA10p.lo,
            ts->dA10p.Hp, ts->dA10p.Wp, 0, 0, 1024, 1024, 0);
-  fc6_dgrad_kernel<<<81920 / 64, 256, 0, st>>>(ts->dh6, ns->fc6_w_hi, B, ts->dA10p.p);
+  (s3 ? fc6_dgrad_kernel<true> : fc6_dgrad_kernel<false>)<<<81920 / 64, 256, 0, st>>>(ts->dh6, ns->fc6_w_hi, ns->fc6_w_lo, B, ts->dA10p.p,
+                                                                                       ts->dA10p.lo);
   DIM_LAUNCH_CHECK();
-  if (int rc = run_generic(ctx, tm.deconv5_dgrad, tm.g_deconv5_dgrad, B, st)) return rc;
+  if (int rc = run_generic(ctx, tm.deconv5_dgrad, tm.g_deconv5_dgrad, B, st, s3)) return rc;
   DIM_CHECK(cudaEventRecord(ts->ev_phase[5], st));
   // encoder
   if (ts->input_depth)
-    LAUNCH1D(strip_to_nhwc64_kernel, (size_t)B * g[0].rows * 8 * g[0].cols, st, ns->act_hi[0], ts->s2d64.p,
-             (size_t)B * g[0].rows * 8 * g[0].cols, g[0].cols);
+    LAUNCH1D((s3 ? strip_to_nhwc64_kernel<true> : strip_to_nhwc64_kernel<false>), (size_t)B * g[0].rows * 8 * g[0].cols, st, ns->act_hi[0],
+             ns->act_lo[0], ts->s2d64.p, ts->s2d64.lo, (size_t)B * g[0].rows * 8 * g[0].cols, g[0].cols);
   else
-    LAUNCH1D(strip_to_nhwc32_kernel, (size_t)B * g[0].rows * 4 * g[0].cols, st, ns->act_hi[0], ts->s2d32.p,
-             (size_t)B * g[0].rows * 4 * g[0].cols, g[0].cols);
+    LAUNCH1D((s3 ? strip_to_nhwc32_kernel<true> : strip_to_nhwc32_kernel<false>), (size_t)B * g[0].rows * 4 * g[0].cols, st, ns->act_hi[0],
+             ns->act_lo[0], ts->s2d32.p, ts->s2d32.lo, (size_t)B * g[0].rows * 4 * g[0].cols, g[0].cols);
   for (int i = 9; i >= 0; --i) {
     const LayerSpec &s = kLayers[i];
     if (int rc = fork_side(ts, st)) return rc;  // gz[i] is complete on st
@@ -1457,10 +1620,10 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
       if (int rc = record_buckets(io, 10, 1 << 30, sw)) return rc;
     if (int rc = bias_grad(ts, ts->gz[i], B, 0, s.Cout, G + ts->off[i].b, sw)) return rc;
     if (i == 0 && ts->input_depth) {
-      if (int rc = run_wgrad(tm.wg[0], tm.wg_bn[0], WG_CONV1_RGBD, 64, 10, 7, G + ts->off[0].w, sw)) return rc;
+      if (int rc = run_wgrad(tm.wg[0], tm.wg_bn[0], s3, WG_CONV1_RGBD, 64, 10, 7, G + ts->off[0].w, sw)) return rc;
     } else if (i == 0) {
       if (int rc = run_wgrad_conv1(ts, tm.wg[0], ctx->num_sms, G + ts->off[0].w, sw)) return rc;
-    } else if (int rc = run_wgrad(tm.wg[i], tm.wg_bn[i], WG_CONV, s.Cout, s.Cin, s.k, G + ts->off[i].w, sw)) return rc;
+    } else if (int rc = run_wgrad(tm.wg[i], tm.wg_bn[i], s3, WG_CONV, s.Cout, s.Cin, s.k, G + ts->off[i].w, sw)) return rc;
     if (int rc = record_buckets(io, i, i + 1, sw)) return rc;
     if (i >= 1)
       if (int rc = run_classes(ctx, ts, tm.dgrad[i], tm.g_dgrad[i], tm.n_dgrad[i], B, st)) return rc;
@@ -1488,14 +1651,15 @@ int train_sgd_update(dim_ctx *ctx, const float *grads, float lr, float momentum,
   cudaStream_t sw = ts->side[3];
   DIM_CHECK(cudaEventRecord(ts->ev_fork, st));
   DIM_CHECK(cudaStreamWaitEvent(sw, ts->ev_fork, 0));
-  if (int rc = repack_all(ctx, sw, false)) return rc;
+  if (int rc = repack_all(ctx, sw, ts->s3)) return rc;  // the bf16x3 step reads the lo halves: refresh them too
   DIM_CHECK(cudaEventRecord(ts->ev_repack, sw));
   ctx->net->repack_done = ts->ev_repack;
   return 0;
 }
 
 // test / debugging hook: copy an intermediate to the host.  id: 0 flow6, 1 flow5, 2 flow4, 3 mask4 (fp32);
-// 10 cat2, 11 cat3, 12 dcat2, 13 dcat3, 14 dA10p, 15 act10b, 20+i gz[i] (bf16, whole bordered buffer)
+// 10 cat2, 11 cat3, 12 dcat2, 13 dcat3, 14 dA10p, 15 act10b, 20+i gz[i] (bf16, whole bordered buffer); 100 + one of the bf16 ids:
+// that buffer's lo half (exists once the step has run in bf16x3)
 int train_debug_tensor(dim_ctx *ctx, int id, void *host, size_t bytes) {
   TrainState *ts = train_of(ctx);
   DIM_REQUIRE(ts != nullptr, "no training state");
@@ -1503,8 +1667,10 @@ int train_debug_tensor(dim_ctx *ctx, int id, void *host, size_t bytes) {
   size_t have = 0;
   const int B = ctx->max_batch;
   const LayerGeom *g = ctx->net->g;
-  auto fb = [&](const Buf &b) { src = b.p; have = b.per_image() * B * 2; };
-  switch (id) {
+  const bool lo = id >= 100;
+  if (lo) id -= 100;
+  auto fb = [&](const Buf &b) { src = lo ? b.lo : b.p; have = b.per_image() * B * 2; };
+  switch (lo && id < 10 ? -1 : id) {
     case 0: src = ts->flow6; have = (size_t)B * g[9].Ho * g[9].Wo * 8; break;
     case 1: src = ts->flow5; have = (size_t)B * g[7].Ho * g[7].Wo * 8; break;
     case 2: src = ts->flow4; have = (size_t)B * g[5].Ho * g[5].Wo * 8; break;
@@ -1541,6 +1707,7 @@ int train_debug_phases(dim_ctx *ctx, float *ms7) {
 void train_debug_geometry(dim_ctx *ctx, int id, int *out /*Hp, Wp, py, px, C, H, W*/) {
   TrainState *ts = train_of(ctx);
   const Buf *b = nullptr;
+  if (id >= 100) id -= 100;  // a lo half has its buffer's geometry
   if (id == 10) b = &ts->cat2; else if (id == 11) b = &ts->cat3; else if (id == 12) b = &ts->dcat2; else if (id == 13) b = &ts->dcat3;
   else if (id == 14) b = &ts->dA10p; else if (id == 15) b = &ts->act10b; else if (id >= 20 && id < 30) b = &ts->gz[id - 20];
   if (!b) { for (int k = 0; k < 7; ++k) out[k] = 0; return; }

@@ -98,6 +98,8 @@ SIGNATURES = {
     "dim_train_set_config": (i32, [vp, C.POINTER(TrainConfig)]),
     "dim_train_get_config": (i32, [vp, C.POINTER(TrainConfig)]),
     "dim_train_sgd_update": (i32, [vp, vp, f32, f32, f32, f32, vp]),
+    "dim_train_set_precision": (i32, [vp, i32]),
+    "dim_train_get_precision": (i32, [vp, C.POINTER(i32)]),
     "dim_train_debug_tensor": (i32, [vp, i32, vp, C.c_uint64]),
     "dim_train_debug_phases": (i32, [vp, pf32]),
     "dim_train_debug_geometry": (i32, [vp, i32, C.POINTER(i32)]),

@@ -103,10 +103,13 @@ def _p(t):
 
 
 class Trainer:
-    def __init__(self, ctx, weights: dict, max_points=3000, lr=1e-4, momentum=0.975, wd=5e-4, bucket_mb=32.0, config=None):
+    def __init__(self, ctx, weights: dict, max_points=3000, lr=1e-4, momentum=0.975, wd=5e-4, bucket_mb=32.0, config=None,
+                 precision="bf16"):
         """config: optional dict overriding fields of dim_train_config (lw_flow, lw_mask, lw_pm, num_3d_sample,
         normalize_3d_point, normalize_flow, trans_means, trans_stds, rot_coord = 'MODEL' | 'CAMERA'): the yaml's train.LW_* /
-        NUM_3D_SAMPLE / NORMALIZE_* / network.TRANS_MEANS / TRANS_STDS / ROT_COORD.  Default: the shipped LM6d values."""
+        NUM_3D_SAMPLE / NORMALIZE_* / network.TRANS_MEANS / TRANS_STDS / ROT_COORD.  Default: the shipped LM6d values.
+        precision: 'bf16' (bf16 activations and activation gradients) or 'bf16x3' (hi / lo pairs, gradients near fp32) for
+        every step of this context -- forward_backward, fit_batch, test_forward_full and the updates (see set_precision)."""
         self.ctx, self.lr, self.momentum, self.wd = ctx, lr, momentum, wd
         self.input_depth = bool(getattr(ctx, "input_depth", False))  # Context(input_depth=True): the RGB-D network
         if _is_rgbd(weights) != self.input_depth:
@@ -122,10 +125,23 @@ class Trainer:
         self._shapes = {k: np.asarray(v).shape for k, v in weights.items()}
         check(lib.dim_train_load_params(ctx._h, flat.ctypes.data_as(C.c_void_p), self.n, self._stream()))
         torch.cuda.current_stream(ctx.device).synchronize()
+        self.set_precision(precision)
         self.grads = torch.zeros(self.n, dtype=torch.float32, device=ctx.device)
         self.buckets, self.bucket_first = make_buckets(bucket_mb, tensor_sizes(self.input_depth))
         self._events = None
         self._comm_stream = None
+
+    def set_precision(self, precision):
+        """'bf16' | 'bf16x3' (or DIM_PREC_BF16 / DIM_PREC_BF16X3): the precision of this context's training step
+        (dim_train_set_precision).  'fp16' is refused: there is no fp16 training step."""
+        torch.cuda.current_stream(self.ctx.device).synchronize()  # the switch synchronises the device, not torch's stream
+        check(lib.dim_train_set_precision(self.ctx._h, capi.precision_id(precision)))
+
+    @property
+    def precision(self) -> str:
+        p = C.c_int32()
+        check(lib.dim_train_get_precision(self.ctx._h, C.byref(p)))
+        return {capi.PREC_BF16: "bf16", capi.PREC_BF16X3: "bf16x3"}[p.value]
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.ctx.device).cuda_stream)

@@ -1,5 +1,6 @@
 """GPU diagnostic: the device training step (forward, losses, gradients, SGD) against the CPU training oracle,
-tensor by tensor.  Writes the report as JSON.  Usage: python tools/gpu_train_check.py [B [OUT.json]]  (default train_check.json)"""
+tensor by tensor.  Writes the report as JSON.
+Usage: python tools/gpu_train_check.py [B [OUT.json]] [--precision bf16|bf16x3]  (defaults 2, train_check.json, bf16)"""
 import json
 import os
 import sys
@@ -52,7 +53,13 @@ def cmp(a, b):
 
 
 def main():
-    B = int(sys.argv[1]) if len(sys.argv) > 1 and sys.argv[1].isdigit() else 2
+    argv = list(sys.argv[1:])
+    precision = "bf16"
+    if "--precision" in argv:
+        i = argv.index("--precision")
+        precision = argv[i + 1]
+        del argv[i:i + 2]
+    B = int(argv[0]) if argv and argv[0].isdigit() else 2
     meshes = [synth.make_cube(), synth.make_blob()]
     w = synth.make_train_weights(0)
     batch = make_batch(meshes, B, 11)
@@ -60,7 +67,7 @@ def main():
     out, g, zin, lab = T.forward_backward(w, batch, K, MEANS)
     t_cpu = time.time() - t0
     ctx = Context(0, max_batch=B, max_classes=2, max_verts=6000, max_faces=11000)
-    tr = Trainer(ctx, w)
+    tr = Trainer(ctx, w, precision=precision)
     dev = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.float32)).cuda()
     z = {"zoom_image_observed": dev(zin["zoom_image_observed"]), "zoom_image_rendered": dev(zin["zoom_image_rendered"]),
          "zoom_mask_observed": dev(zin["zoom_mask_observed"]), "zoom_mask_rendered": dev(zin["zoom_mask_rendered"]),
@@ -68,7 +75,7 @@ def main():
          "zoom_mask_gt_observed": dev(lab["zoom_mask_gt_observed"]), "src_pose": dev(lab["src_pose"]),
          "point_cloud_model": dev(lab["point_cloud_model"]), "point_cloud_weights": dev(lab["point_cloud_weights"]),
          "point_cloud_observed": dev(lab["point_cloud_observed"])}
-    rep = {"B": B, "cpu_oracle_s": t_cpu}
+    rep = {"B": B, "precision": precision, "cpu_oracle_s": t_cpu}
     res = tr.forward_backward(z)
     torch.cuda.synchronize()
     losses = res["losses"].cpu().numpy()
@@ -121,7 +128,7 @@ def main():
     torch.cuda.synchronize()
     rep["ms_per_step"] = e0.elapsed_time(e1) / 5
     rep["device"] = torch.cuda.get_device_name(0)
-    with open(sys.argv[2] if len(sys.argv) > 2 else "train_check.json", "w") as f:
+    with open(argv[1] if len(argv) > 1 else "train_check.json", "w") as f:
         json.dump(rep, f, indent=1)
     bad = [k for k, v in rep["grads"].items() if v["cos"] < 0.99 and v["ref_max"] > 0]
     print(json.dumps({"losses": rep["losses"], "ms_per_step": rep["ms_per_step"], "bad_grads": bad}, indent=1))

@@ -1,7 +1,7 @@
 """Training-step benchmark (BASELINE.json config C4: flow+mask+pose losses on synthetic rendered pairs, per-GPU batch 4,
 4 inner iterations per batch, NCCL gradient all-reduce when launched under torchrun).
 
-    python tools/train_bench.py [--batch 4] [--steps 10] [--warmup 3]
+    python tools/train_bench.py [--batch 4] [--steps 10] [--warmup 3] [--precision bf16|bf16x3]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P tools/train_bench.py
 
 One "step" = one data batch of Module.fit = 4 x (zoom front, forward, losses, backward, all-reduce, SGD update, re-render
@@ -30,6 +30,7 @@ def main():
     ap.add_argument("--out", default="")
     ap.add_argument("--bucket-mb", type=float, default=None, help="gradient bucket size of the overlapped all-reduce (default: Trainer's)")
     ap.add_argument("--no-overlap", action="store_true", help="all-reduce after the backward pass instead of bucket by bucket during it")
+    ap.add_argument("--precision", default="bf16", choices=["bf16", "bf16x3"], help="precision of the training step (Trainer)")
     a = ap.parse_args()
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank, local = int(os.environ.get("RANK", "0")), int(os.environ.get("LOCAL_RANK", "0"))
@@ -44,7 +45,7 @@ def main():
                   max_faces=max(len(m.faces) for m in meshes))
     for i, m in enumerate(meshes):
         ctx.upload_mesh(i, m)
-    tr = Trainer(ctx, synth.make_train_weights(0), **({"bucket_mb": a.bucket_mb} if a.bucket_mb else {}))
+    tr = Trainer(ctx, synth.make_train_weights(0), precision=a.precision, **({"bucket_mb": a.bucket_mb} if a.bucket_mb else {}))
     batch, cls, tgt, depth = make_device_batch(ctx, meshes, a.batch, 3 + rank, K, MEANS)
     if a.no_overlap:
         step0 = tr.step
@@ -83,7 +84,9 @@ def main():
             "ms_per_inner_iteration": float(ms) / 4, "split_ms": {"forward_backward": ev[0].elapsed_time(ev[1]),
                                                                    "allreduce": ev[1].elapsed_time(ev[2]), "sgd_update_repack": ev[2].elapsed_time(ev[3]),
                                                                    "host_enqueue_forward_backward": (c1 - c0) * 1e3, "host_enqueue_update": (c2 - c1) * 1e3},
-            "dtype": "bf16 activations/gradients, fp32 master", "data": "synthetic", "scaling": "weak",
+            "dtype": {"bf16": "bf16 activations/gradients, fp32 master",
+                      "bf16x3": "bf16 hi/lo activations/gradients (3 MMA passes), fp32 master"}[a.precision],
+            "precision": a.precision, "device": torch.cuda.get_device_name(local), "data": "synthetic", "scaling": "weak",
             "config": {"workload": "C4 training step", "allreduce_overlap": (not a.no_overlap) and world > 1, "per_gpu_batch": a.batch, "inner_iterations": 4, "grad_bytes": tr.n * 4,
                        "buckets_mb": [round((hi - lo) * 4 / 2 ** 20, 1) for lo, hi in tr.buckets]},
             "phases_ms": dict(zip(["encoder_fwd", "decoder_fwd", "losses_heads", "fc_bwd", "decoder_bwd", "encoder_dgrad_chain", "wait_wgrad_stream"], [round(float(x), 4) for x in ph])),
