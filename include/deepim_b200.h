@@ -354,6 +354,29 @@ DIM_API int32_t dim_net_fwd_rgbd(dim_ctx *ctx, const float *zoom_image_observed,
                                  const float *zoom_mask_rendered, int32_t B, int32_t precision,
                                  float *rot, float *trans, void *stream);
 
+/* Image-only network (config.network.INPUT_MASK: False, the reference's default; deepIM_flownet.py:53-62, tester.py:439): conv1
+ * sees concat(image_observed/255, image_rendered/255), so flow_conv1_weight is (64, 6, 7, 7), and the test graph zooms with
+ * ZoomImage (zoom_image.py:26-107, the boxes of sum_c(image + mean) > 0.01) instead of ZoomMask + ZoomImageWithFactor.
+ *
+ * dim_ctx_set_input_mask: enable = 0 switches the context to this network, 1 (the default) back.  Only before dim_net_load /
+ *   dim_train_create (an error afterwards); refused together with dim_ctx_set_input_depth (depth input without the mask
+ *   channels is not supported).  A context that never calls it is unchanged.
+ * On such a context the existing entries follow the network, with no argument change:
+ *   - dim_refine(_lit), dim_refine_host(_lit)(_async) run the image-only chain: the observed box is computed once per call,
+ *     the rendered box of every iteration from the render's colours; the zoom factor is ZoomImage's (ZoomMask's arithmetic
+ *     with the observed-centre fallback for an empty render).  dim_refine_status: bit 0 = the observed image has no valid
+ *     pixel (the reference raises; the fallback factor (1,1,0,0) was used), bit 2 = the rendered image has none (the zoom
+ *     centres on the observed box, as the reference does), bit 1 unchanged.
+ *   - dim_net_fwd needs zoom_mask_observed = zoom_mask_rendered = NULL; so does dim_train_forward_backward.
+ *   - dim_train_update(_lit) is unchanged: with PRED_MASK the reference's training graph still zooms with ZoomMask and learns
+ *     the mask; only the network input loses the mask channels.
+ *   - dim_net_load takes the (64, 6, 7, 7) flow_conv1 weight; the flat training vector is the table of
+ *     dim_train_param_info_nomask (flow_conv1 (64, 6, 7, 7): 6 272 floats fewer; every other entry as dim_train_param_info),
+ *     and dim_train_param_count reports its size. */
+DIM_API int32_t dim_ctx_set_input_mask(dim_ctx *ctx, int32_t enable);
+DIM_API int32_t dim_train_param_info_nomask(int32_t idx, const char **name, int64_t *weight_numel,
+                                            int64_t *bias_numel);
+
 /* BGR u8 HWC -> RGB-mean f32 CHW on device (lib/utils/image.py:583-594 transform). */
 DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int32_t B,
                                        const double *pixel_means_rgb_host, float *image,

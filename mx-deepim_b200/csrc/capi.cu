@@ -309,10 +309,24 @@ DIM_API int32_t dim_ctx_set_input_depth(dim_ctx *ctx, int32_t enable) {
   DIM_REQUIRE(ctx != nullptr, "dim_ctx_set_input_depth: NULL context");
   if (net_input_depth(ctx) == (enable != 0)) return 0;
   DIM_REQUIRE(train_param_count(ctx) == 0, "dim_ctx_set_input_depth: call it before dim_train_create (this context trains)");
+  DIM_REQUIRE(net_input_mask(ctx), "dim_ctx_set_input_depth: input_depth with input_mask = 0 (depth input without the mask "
+                                   "channels, INPUT_DEPTH without INPUT_MASK) is not supported");
   drop_graphs(ctx);
   if (enable && !ctx->depth_u16)
     if (dev_alloc(ctx, &ctx->depth_u16, (size_t)ctx->max_batch * ctx->H * ctx->W)) return 12;
   return net_set_input_depth(ctx, enable != 0);
+}
+
+DIM_API int32_t dim_ctx_set_input_mask(dim_ctx *ctx, int32_t enable) {
+  DIM_REQUIRE(ctx != nullptr, "dim_ctx_set_input_mask: NULL context");
+  if (net_input_mask(ctx) == (enable != 0)) return 0;
+  DIM_REQUIRE(train_param_count(ctx) == 0, "dim_ctx_set_input_mask: call it before dim_train_create (this context trains)");
+  DIM_REQUIRE(!net_input_depth(ctx), "dim_ctx_set_input_mask: input_mask = 0 with input_depth (depth input without the mask "
+                                     "channels, INPUT_DEPTH without INPUT_MASK) is not supported");
+  drop_graphs(ctx);
+  if (!enable && !ctx->bbox_obs)
+    if (dev_alloc(ctx, &ctx->bbox_obs, (size_t)ctx->max_batch * 4)) return 12;
+  return net_set_input_mask(ctx, enable != 0);
 }
 
 DIM_API int32_t dim_net_load(dim_ctx *ctx, const float *const *W, const float *const *Bv) {
@@ -323,8 +337,14 @@ DIM_API int32_t dim_net_load(dim_ctx *ctx, const float *const *W, const float *c
 
 DIM_API int32_t dim_net_fwd(dim_ctx *ctx, const float *zio, const float *zir, const float *zmo, const float *zmr,
                             int32_t B, int32_t precision, float *rot, float *trans, void *stream) {
-  DIM_REQUIRE(ctx && zio && zir && zmo && zmr && rot && trans, "dim_net_fwd: NULL argument");
+  DIM_REQUIRE(ctx && zio && zir && rot && trans, "dim_net_fwd: NULL argument");
   if (int rc = input_mode_check(ctx, false, "dim_net_fwd", "dim_net_fwd_rgbd")) return rc;
+  if (net_input_mask(ctx)) {
+    DIM_REQUIRE(zmo && zmr, "dim_net_fwd: NULL argument");
+  } else {
+    DIM_REQUIRE(!zmo && !zmr, "dim_net_fwd: this context's network takes no mask input (dim_ctx_set_input_mask): pass "
+                              "zoom_mask_observed = zoom_mask_rendered = NULL");
+  }
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_net_fwd: batch exceeds max_batch");
   cudaStream_t st = (cudaStream_t)stream;
   int rows, cols, pad; __nv_bfloat16 *hi, *lo;
@@ -363,6 +383,10 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
   int rows, cols, pad; __nv_bfloat16 *hi, *lo;
   net_input_geometry(ctx, &rows, &cols, &pad, &hi, &lo);
   const bool depth = net_input_depth(ctx);  // RGB-D network: ren4.w = depth, obs4.w = depth_observed
+  // image-only network (ZoomImage): both boxes come from the colours; the observed one once per call
+  const bool mask = net_input_mask(ctx);
+  if (!mask)
+    if (int rc = obs_colour_box_launch(ctx, a.obs4, a.B, ctx->bbox_obs, st)) return rc;
   const double *pose_src = a.pose_init;
   for (int it = 0; it < a.n_iter; ++it) {
     DimNvtxRange r_it("dim_refine iteration");
@@ -392,21 +416,27 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
       const LitParams lp = a.lit ? lit_params(ctx->light_pos, a.intensity + (size_t)it * a.B * 3, a.brightness_ratio)
                                  : LitParams{nullptr, nullptr, 0.f, 0.f};
       if (int rc = render_launch(ctx, a.cls_idx, ctx->pose_cur_f32, a.B, a.K9, a.zn, a.zf, a.means, 1, nullptr, nullptr,
-                                 nullptr, nullptr, nullptr, ctx->ren4, st, a.lit ? &lp : nullptr, depth))
+                                 nullptr, nullptr, nullptr, ctx->ren4, st, a.lit ? &lp : nullptr, depth, !mask))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[1], st));
     float *zf_it = a.zoom_factor ? a.zoom_factor + (size_t)it * a.B * 4 : ctx->zoom_factor;
     int *bbox_it = a.bbox ? a.bbox + (size_t)it * a.B * 8 : nullptr;
-    // per-iteration status (bit 0: rendered / observed mask empty -> fallback zoom factor; bit 1: bad class index)
+    // per-iteration status (bit 0: rendered / observed mask empty -> fallback zoom factor; bit 1: bad class index;
+    // image-only network: bit 0 = observed image empty, bit 2 = rendered image empty -> zoom centred on the observed box)
     {
       DimNvtxRange r("bbox + zoom");
-      if (int rc = zoom_factor_from_ren_launch(ctx, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it, bbox_it,
-                                               ctx->status_hist + (size_t)(it < 8 ? it : 7) * a.B, st))
+      int *status_it = ctx->status_hist + (size_t)(it < 8 ? it : 7) * a.B;
+      if (mask) {
+        if (int rc = zoom_factor_from_ren_launch(ctx, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it, bbox_it, status_it, st))
+          return rc;
+      } else if (int rc = zoom_factor_from_boxes_launch(ctx, ctx->bbox_obs, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it,
+                                                        bbox_it, status_it, st)) {
         return rc;
+      }
       if (int rc = zoom_fused_launch(ctx, a.obs4, ctx->ren4, zf_it, means_f, a.B, rows, cols, pad, hi,
                                      a.precision == DIM_PREC_BF16X3 ? lo : nullptr, st, a.precision == DIM_PREC_FP16, a.means,
-                                     depth))
+                                     depth, mask))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[2], st));
@@ -818,6 +848,13 @@ DIM_API int32_t dim_train_param_info_rgbd(int32_t idx, const char **name, int64_
   *w_numel = w; *b_numel = b;
   return 0;
 }
+DIM_API int32_t dim_train_param_info_nomask(int32_t idx, const char **name, int64_t *w_numel, int64_t *b_numel) {
+  long long w = 0, b = 0;
+  DIM_REQUIRE(name && w_numel && b_numel, "dim_train_param_info_nomask: NULL argument");
+  if (train_param_info(idx, name, &w, &b, false, false)) return 2;
+  *w_numel = w; *b_numel = b;
+  return 0;
+}
 DIM_API int32_t dim_train_load_params(dim_ctx *ctx, const float *flat_host, int64_t n, void *stream) {
   DIM_REQUIRE(ctx && flat_host && n > 0, "dim_train_load_params: bad argument");
   return train_load_params(ctx, flat_host, (size_t)n, (cudaStream_t)stream);
@@ -833,8 +870,14 @@ DIM_API int32_t dim_train_forward_backward(dim_ctx *ctx, const float *zio, const
                                            float *flow_est, float *mask_prob, float *losses4, float *grads, float *rot_raw,
                                            void *const *bucket_events, const int32_t *bucket_first_tensor, int32_t n_buckets,
                                            void *stream) {
-  DIM_REQUIRE(ctx && zio && zir && zmo && zmr && zoom_factor, "dim_train_forward_backward: NULL argument");
+  DIM_REQUIRE(ctx && zio && zir && zoom_factor, "dim_train_forward_backward: NULL argument");
   if (int rc = input_mode_check(ctx, false, "dim_train_forward_backward", "dim_train_forward_backward_rgbd")) return rc;
+  if (net_input_mask(ctx)) {
+    DIM_REQUIRE(zmo && zmr, "dim_train_forward_backward: NULL argument");
+  } else {
+    DIM_REQUIRE(!zmo && !zmr, "dim_train_forward_backward: this context's network takes no mask input "
+                              "(dim_ctx_set_input_mask): pass zoom_mask_observed = zoom_mask_rendered = NULL");
+  }
   TrainIO io{zio, zir, zmo, zmr, zoom_factor, zflow, zfw, zmask_gt, src_pose, pc_model, pc_weights, pc_observed, B, N,
              rot_est_norm, trans_est, flow_est, mask_prob, losses4, grads, rot_raw, bucket_events, bucket_first_tensor,
              (bucket_events && bucket_first_tensor) ? n_buckets : 0};

@@ -127,6 +127,7 @@ struct dim_ctx {
   float *light_pos = nullptr;      // [max_batch,3] lit chain / lit train update: light of the pose being rendered
   float *lit_intensity = nullptr;  // [8, max_batch, 3] dim_refine_host_lit: the caller's light intensities on the device
   uint16_t *depth_u16 = nullptr;   // [max_batch,H,W] dim_refine_host_rgbd: the caller's depth file values (RGB-D contexts)
+  int *bbox_obs = nullptr;         // [max_batch,4] image-only network: the observed image's colour-valid box (ZoomImage)
   dim::NetState *net = nullptr;
   // CUDA graphs of the fused refinement chain (capi.cu refine_graphed): one executable graph per distinct argument set
   struct RefineGraph {

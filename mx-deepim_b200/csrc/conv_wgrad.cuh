@@ -187,7 +187,8 @@ enum { WG_CONV = 0, WG_CONV1_S2D = 1, WG_DECONV = 2, WG_CONV1_ROW = 3, WG_CONV1_
 // partial tiles are read coalesced; the (Cout,Cin,kh,kw) destination is written with a k*k-element stride.
 //   WG_CONV      : m = co, n = ci            -> (Cout, Cin, k, k)
 //   WG_CONV1_S2D : m = co, n = ph*16+pw*8+c  -> (64, 8, 7, 7), kh = 2dh+ph, kw = 2dw+pw      (taps = 16)
-//   WG_CONV1_ROW : m = dw*32+ph*16+pw*8+c, n = co, tap = dh -> (64, 8, 7, 7)                  (conv1_wgrad_kernel, taps = 4)
+//   WG_CONV1_ROW : m = dw*32+ph*16+pw*8+c, n = co, tap = dh -> (64, D1, 7, 7)                 (conv1_wgrad_kernel, taps = 4;
+//                  D1 = 8, or 6 for the image-only network: its zero mask lanes c >= 6 are dropped)
 //   WG_DECONV    : m = ci, n = co            -> (Cin, Cout, k, k)
 //   WG_CONV1_RGBD: m = co, n = ph*32+pw*16+c -> (64, 10, 7, 7), kh = 2dh+ph, kw = 2dw+pw  (RGB-D conv1, taps = 16; c >= 10 and
 //                  taps outside the 7 x 7 filter are the layout's zero padding and are dropped)

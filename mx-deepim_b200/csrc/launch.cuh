@@ -23,7 +23,8 @@ struct TrainIO {
 // raster.cu
 int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
                   const double *means, int trunc_u8, float *out_image, float *out_depth, float *out_mask, float *out_bgr,
-                  int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit = nullptr, bool ren4_depth = false);
+                  int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit = nullptr, bool ren4_depth = false,
+                  bool colour_box = false);
 
 // zoom.cu
 int zoom_gather_launch(dim_ctx *ctx, int mode, const float *src, float *dst, const float *zoom_factor, int B, int C,
@@ -33,10 +34,13 @@ int zoom_factor_launch(dim_ctx *ctx, const float *mask_real, const float *mask_r
                        const float *img_means = nullptr);
 int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *src_pose, int B, const float *K9,
                                 float *zoom_factor, int *bbox_out, int *status, cudaStream_t st);
+int obs_colour_box_launch(dim_ctx *ctx, const float4 *obs4, int B, int *bbox_obs, cudaStream_t st);
+int zoom_factor_from_boxes_launch(dim_ctx *ctx, const int *bbox_obs, const int *bbox_ren, const float *src_pose, int B,
+                                  const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st);
 int box_mask_launch(dim_ctx *ctx, const int *bbox, int B, float *mask, cudaStream_t st);
 int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, const float *zoom_factor,
                       const float *means_rgb, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
-                      cudaStream_t st, int f16, const double *means_d, bool depth = false);
+                      cudaStream_t st, int f16, const double *means_d, bool depth = false, bool mask = true);
 int obs4_depth_launch(dim_ctx *ctx, float4 *obs4, int B, const float *depth, const uint16_t *depth_u16, float factor,
                       cudaStream_t st);
 int pack_nhwc10_launch(dim_ctx *ctx, const float *io, const float *ir, const float *dobs, const float *dren, const float *mo,
@@ -84,6 +88,8 @@ int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, fl
 bool net_graph_safe(dim_ctx *ctx);
 int net_set_input_depth(dim_ctx *ctx, bool enable);
 bool net_input_depth(dim_ctx *ctx);
+int net_set_input_mask(dim_ctx *ctx, bool enable);
+bool net_input_mask(dim_ctx *ctx);
 int net_layer_profile(dim_ctx *ctx, int enable, float *ms10);
 int net_debug_activation(dim_ctx *ctx, int idx, int lo, void *host_dst, size_t bytes);
 void net_layer_geometry(dim_ctx *ctx, int idx, int *out /*rows, cols, Cbuf, py, px, Ho, Wo, Cout*/);
@@ -95,7 +101,8 @@ int train_load_params(dim_ctx *ctx, const float *flat_host, size_t n, cudaStream
 int train_refresh_lo(dim_ctx *ctx, cudaStream_t st);
 int train_get_params(dim_ctx *ctx, float *flat_host, size_t n, int which, cudaStream_t st);
 size_t train_param_count(dim_ctx *ctx);
-int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel, bool input_depth = false);
+int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel, bool input_depth = false,
+                     bool input_mask = true);
 int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st);
 int train_sgd_update(dim_ctx *ctx, const float *grads, float lr, float momentum, float wd, float rescale, cudaStream_t st);
 int train_set_precision(dim_ctx *ctx, int precision);

@@ -442,17 +442,19 @@ int net_load(dim_ctx *ctx, const float *const *W, const float *const *Bv) {
                       w[(((size_t)co * 10 + c) * 7 + kh) * 7 + kw];
                 }
     } else if (i == 0) {
-      // space-to-depth repack: W'[co][dh][dw][conv1_kslot(dw,ph,pw)+c] = W[co][c][2dh+ph][2dw+pw] (0 beyond 7x7)
+      // space-to-depth repack: W'[co][dh][dw][conv1_kslot(dw,ph,pw)+c] = W[co][c][2dh+ph][2dw+pw] (0 beyond 7x7); the
+      // image-only network's W is (64, 6, 7, 7): its mask columns c = 6, 7 stay zero
+      const int cin = ns->input_mask ? 8 : 6;
       for (int co = 0; co < g.Cout; ++co)
         for (int dh = 0; dh < 4; ++dh)
           for (int dw = 0; dw < 4; ++dw)
             for (int ph = 0; ph < 2; ++ph)
               for (int pw = 0; pw < 2; ++pw)
-                for (int c = 0; c < 8; ++c) {
+                for (int c = 0; c < cin; ++c) {
                   const int kh = 2 * dh + ph, kw = 2 * dw + pw;
                   if (kh >= 7 || kw >= 7) continue;
                   packed[(size_t)co * Ktot + (size_t)(dh * 4 + dw) * 32 + conv1_kslot(dw, ph, pw) + c] =
-                      w[(((size_t)co * 8 + c) * 7 + kh) * 7 + kw];
+                      w[(((size_t)co * cin + c) * 7 + kh) * 7 + kw];
                 }
     } else {
       for (int co = 0; co < g.Cout; ++co)
@@ -563,6 +565,19 @@ int net_set_input_depth(dim_ctx *ctx, bool enable) {
 }
 
 bool net_input_depth(dim_ctx *ctx) { return ctx->net && ctx->net->input_depth; }
+
+// switches flow_conv1 between the 8-channel and the 6-channel (image-only) weight; only before any weights are loaded.
+// Nothing else changes: the input buffer, its geometry and conv1_kernel are the 8-channel ones.
+int net_set_input_mask(dim_ctx *ctx, bool enable) {
+  NetState *ns = ctx->net;
+  DIM_REQUIRE(ns != nullptr, "net not created");
+  if (ns->input_mask == enable) return 0;
+  DIM_REQUIRE(!ns->loaded, "dim_ctx_set_input_mask: call it before dim_net_load (this context's weights are loaded)");
+  ns->input_mask = enable;
+  return 0;
+}
+
+bool net_input_mask(dim_ctx *ctx) { return !ctx->net || ctx->net->input_mask; }
 
 // where conv1's input buffer expects pixel (i,j) of the 8-channel blob (space-to-depth, pad 3)
 void net_input_geometry(dim_ctx *ctx, int *rows, int *cols, int *pad, __nv_bfloat16 **hi, __nv_bfloat16 **lo) {

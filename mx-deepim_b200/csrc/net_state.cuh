@@ -57,6 +57,9 @@ struct NetState {
   // (conv1_rgbd_kernel); the 8-channel network's conv1 input buffers are kept for switching back
   bool input_depth = false;
   __nv_bfloat16 *act0_rgb_hi = nullptr, *act0_rgb_lo = nullptr, *act0_rgbd_hi = nullptr, *act0_rgbd_lo = nullptr;
+  // image-only network (dim_ctx_set_input_mask(ctx, 0)): flow_conv1 takes 6 channels; conv1_kernel and its 8-lane input are
+  // unchanged, the weight pack carries zero columns for lanes 6-7 and every producer writes zeros there
+  bool input_mask = true;
   float *save_h6 = nullptr, *save_h7 = nullptr;
   cudaEvent_t repack_done = nullptr;  // training: the operand packs are refreshed on an internal stream after an update;
                                       // every consumer (net_forward) orders itself behind this event

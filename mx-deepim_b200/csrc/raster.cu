@@ -263,7 +263,10 @@ __device__ __forceinline__ float colour_of(unsigned char c, int trunc_u8) {
 // LIT is a compile-time switch: the unlit instantiation (the refinement loop's renderer) carries none of the shading code.
 // REN4_DEPTH (the RGB-D network's loop): the w lane of out_ren4 holds the depth instead of the 0/1 mask; the zoom kernel
 // samples it as depth_rendered and re-derives the mask as depth > 0.2, which is how the mask is made here.
-template <bool LIT, bool REN4_DEPTH = false>
+// COLOUR_BOX (the image-only network's loop): bbox_ren is ZoomImage's rendered box (zoom_image.py:35-37), the pixels whose
+// ((x + y) + z) > 0.01f over the ren4 colours (image + mean): the float32 expression of zoom.cu's img_mode bbox, on the
+// very values ren4 holds.  Uncovered pixels hold background + mean = 0 and never pass, so only covered ones are tested.
+template <bool LIT, bool REN4_DEPTH = false, bool COLOUR_BOX = false>
 __global__ void __launch_bounds__(256) raster_resolve_kernel(RasterParams p) {
   const int b = blockIdx.y;
   const int W4 = p.W >> 2;
@@ -363,8 +366,11 @@ __global__ void __launch_bounds__(256) raster_resolve_kernel(RasterParams p) {
         bl[k] = c2 - (float)p.mean[2];
       }
       d[k] = z;
-      if (z > 0.2f) {  // mask = depth > 0.2 (deepim/core/tester.py:440)
-        mk[k] = 1.f;
+      if (z > 0.2f) mk[k] = 1.f;  // mask = depth > 0.2 (deepim/core/tester.py:440)
+      bool in_bbox = z > 0.2f;
+      if (COLOUR_BOX)
+        in_bbox = ((r[k] + (float)p.mean[0]) + (g[k] + (float)p.mean[1])) + (bl[k] + (float)p.mean[2]) > 0.01f;
+      if (in_bbox) {
         mx0 = min(mx0, j4 + k);
         mx1 = max(mx1, j4 + k);
         my0 = i;
@@ -426,7 +432,8 @@ __global__ void raster_finish_kernel(int *bbox_ren, int *out_bbox, int B) {
 
 int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
                   const double *means, int trunc_u8, float *out_image, float *out_depth, float *out_mask,
-                  float *out_bgr, int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit, bool ren4_depth) {
+                  float *out_bgr, int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit, bool ren4_depth,
+                  bool colour_box) {
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_render: batch exceeds max_batch");
   DIM_REQUIRE((ctx->W & 3) == 0, "dim_render: width must be a multiple of 4");
   RasterParams p;
@@ -456,7 +463,11 @@ int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const 
   raster_coverage_kernel<<<dim3(cdiv(maxF, 128), B), 128, 0, st>>>(p);
   DIM_LAUNCH_CHECK();
   const dim3 rgrid(cdiv((ctx->W / 4) * ctx->H, 256), B);
-  if (ren4_depth) {
+  DIM_REQUIRE(!(ren4_depth && colour_box), "dim_render: the colour bbox has no RGB-D variant");
+  if (colour_box) {
+    if (p.lit) raster_resolve_kernel<true, false, true><<<rgrid, 256, 0, st>>>(p);
+    else raster_resolve_kernel<false, false, true><<<rgrid, 256, 0, st>>>(p);
+  } else if (ren4_depth) {
     if (p.lit) raster_resolve_kernel<true, true><<<rgrid, 256, 0, st>>>(p);
     else raster_resolve_kernel<false, true><<<rgrid, 256, 0, st>>>(p);
   } else if (p.lit) {

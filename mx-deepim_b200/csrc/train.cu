@@ -76,6 +76,7 @@ struct TrainState {
   Buf act10b, cat2, cat3, dcat2, dcat3, dA10p, gz[10], s2d32;
   Buf s2d64;         // RGB-D network: conv1's input as NHWC-64 (weight gradient operand)
   bool input_depth = false;  // the table's flow_conv1 is (64, 10, 7, 7)
+  bool input_mask = true;    // false: the image-only network, the table's flow_conv1 is (64, 6, 7, 7)
   float *flow6 = nullptr, *flow5 = nullptr, *flow4 = nullptr, *mask4 = nullptr;
   float *dflow6 = nullptr, *dflow5 = nullptr, *dflow4 = nullptr, *dmask4 = nullptr;
   float *dfull = nullptr;        // [B][3][H][W] gradient wrt the full-resolution flow (2) / mask logit (1)
@@ -705,13 +706,15 @@ __global__ void __launch_bounds__(256) pack_conv1_rgbd_kernel(const float *w, __
   const int kh = 2 * (tap >> 2) + (phase >> 1), kw = 2 * (tap & 3) + (phase & 1);
   store_split(hi, lo, i, (c < 10 && kh < 7 && kw < 7) ? w[((co * 10 + c) * 7 + kh) * 7 + kw] : 0.f);
 }
-// conv1 space-to-depth pack [64][4][4][32]
-__global__ void __launch_bounds__(256) pack_conv1_kernel(const float *w, __nv_bfloat16 *hi, __nv_bfloat16 *lo) {
+// conv1 space-to-depth pack [64][4][4][32] of a (64, cin, 7, 7) master: cin = 8, or 6 for the image-only network, whose
+// mask lanes 6-7 get zero columns
+__global__ void __launch_bounds__(256) pack_conv1_kernel(const float *w, int cin, __nv_bfloat16 *hi, __nv_bfloat16 *lo) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= 64 * 512) return;
   const int c = i & 7, pw = (i >> 3) & 1, ph = (i >> 4) & 1, dw = (i >> 5) & 3, dh = (i >> 7) & 3, co = i >> 9;
   const int kh = 2 * dh + ph, kw = 2 * dw + pw;
-  store_split(hi, lo, (i & ~31) + conv1_kslot(dw, ph, pw) + c, (kh < 7 && kw < 7) ? w[((co * 8 + c) * 7 + kh) * 7 + kw] : 0.f);
+  store_split(hi, lo, (i & ~31) + conv1_kslot(dw, ph, pw) + c,
+              (c < cin && kh < 7 && kw < 7) ? w[((co * cin + c) * 7 + kh) * 7 + kw] : 0.f);
 }
 // data-gradient packs of ALL parity classes of one layer: class (ry, rx) is [Cin][Ty][Tx][Cout] with ky = ry + s*(Ty-1-ty).
 // block = (ci, 64 output channels): reads 64 rows of k*k floats, writes 64 consecutive bf16 per (class, tap)
@@ -784,10 +787,11 @@ __global__ void transpose256_kernel(const float *w, float *wT) {
 
 // ------------------------------------------------------------------------------------ host side
 static size_t param_numel(const ParamSpec &s) { return (size_t)s.d0 * s.d1 * s.k * s.k; }
-// the table entry of the RGB or the RGB-D network: they differ only in flow_conv1's input channels (8 / 10)
-static ParamSpec param_spec(int i, bool input_depth) {
+// the table entry of the RGB, the RGB-D or the image-only network: they differ only in flow_conv1's input channels (8 / 10 / 6)
+static ParamSpec param_spec(int i, bool input_depth, bool input_mask = true) {
   ParamSpec s = kParams[i];
   if (i == 0 && input_depth) s.d1 = 10;
+  if (i == 0 && !input_mask) s.d1 = 6;
   return s;
 }
 static size_t bias_numel(const ParamSpec &s) {
@@ -816,9 +820,10 @@ int train_create(dim_ctx *ctx, int max_points) {
   train_of(ctx) = ts;
   ts->max_points = max_points;
   ts->input_depth = ns->input_depth;
+  ts->input_mask = ns->input_mask;
   size_t off = 0;
   for (int i = 0; i < 24; ++i) {
-    ts->off[i].w = off; ts->off[i].wn = param_numel(param_spec(i, ts->input_depth)); off += ts->off[i].wn;
+    ts->off[i].w = off; ts->off[i].wn = param_numel(param_spec(i, ts->input_depth, ts->input_mask)); off += ts->off[i].wn;
     ts->off[i].b = off; ts->off[i].bn = bias_numel(kParams[i]); off += ts->off[i].bn;
   }
   ts->n_params = off;
@@ -913,7 +918,8 @@ static int repack_all(dim_ctx *ctx, cudaStream_t st, bool with_lo) {
   TrainState *ts = train_of(ctx);
   const float *M = ts->master;
   if (ts->input_depth) LAUNCH1D(pack_conv1_rgbd_kernel, 64 * 1024, st, M + ts->off[0].w, ns->w_hi[0], with_lo ? ns->w_lo[0] : nullptr);
-  else LAUNCH1D(pack_conv1_kernel, 64 * 512, st, M + ts->off[0].w, ns->w_hi[0], with_lo ? ns->w_lo[0] : nullptr);
+  else LAUNCH1D(pack_conv1_kernel, 64 * 512, st, M + ts->off[0].w, ts->input_mask ? 8 : 6, ns->w_hi[0],
+                with_lo ? ns->w_lo[0] : nullptr);
   // the training packs' lo halves exist once the step has run in bf16x3 (nullptr before)
   auto L = [with_lo](__nv_bfloat16 *lo) { return with_lo ? lo : nullptr; };
   for (int i = 1; i < 10; ++i) {
@@ -1047,9 +1053,9 @@ int train_get_params(dim_ctx *ctx, float *flat_host, size_t n, int which, cudaSt
 }
 
 size_t train_param_count(dim_ctx *ctx) { TrainState *ts = train_of(ctx); return ts ? ts->n_params : 0; }
-int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel, bool input_depth) {
+int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel, bool input_depth, bool input_mask) {
   if (idx < 0 || idx >= 24) return 1;
-  const ParamSpec s = param_spec(idx, input_depth);
+  const ParamSpec s = param_spec(idx, input_depth, input_mask);
   *name = s.name; *w_numel = (long long)param_numel(s); *b_numel = (long long)bias_numel(s);
   return 0;
 }
@@ -1273,7 +1279,9 @@ static int run_wgrad_conv1(TrainState *ts, const WgradParams &p16, int sms, floa
   DIM_REQUIRE((size_t)p.kslices * 4 * 128 * 64 <= ts->wg_partial_elems, "wgrad workspace too small");
   if (int rc = ts->s3 ? launch_wgrad_conv1<4, true>(p, st) : launch_wgrad_conv1<8, false>(p, st)) return rc;
   const size_t total = (size_t)4 * 128 * 64;
-  wgrad_reduce_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(p.partial, p.kslices, 4, 128, 64, WG_CONV1_ROW, 64, 8, 7, grad);
+  // the image-only network's gradient is (64, 6, 7, 7): D1 = 6 drops the rows of the zero mask lanes
+  wgrad_reduce_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(p.partial, p.kslices, 4, 128, 64, WG_CONV1_ROW, 64,
+                                                                       ts->input_mask ? 8 : 6, 7, grad);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -1483,7 +1491,8 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
     if (int rc = pack_nhwc10_launch(ctx, io.zio, io.zir, io.zdo, io.zdr, io.zmo, io.zmr, B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0],
                                     s3 ? ns->act_lo[0] : nullptr, st, 0))
       return rc;
-  } else if (int rc = pack_nhwc8_launch(ctx, io.zio, io.zir, io.zmo, io.zmr, B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0],
+  } else if (int rc = pack_nhwc8_launch(ctx, io.zio, io.zir, ts->input_mask ? io.zmo : nullptr, ts->input_mask ? io.zmr : nullptr,
+                                        B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0],
                                         s3 ? ns->act_lo[0] : nullptr, st, 0)) {
     return rc;
   }

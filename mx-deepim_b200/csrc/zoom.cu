@@ -59,11 +59,12 @@ __global__ void __launch_bounds__(160) mask_bbox_kernel(const float *mask_real, 
   }
 }
 
-// zoom factor, one thread per instance (zoom_mask.py:59-103).  Mixed precision as the reference's
-// numpy 1.x: c = K.t and c_x = c0/c2 in float32, everything after in float64, stored as float32.
+// zoom factor, one thread per instance (zoom_mask.py:59-103; ZoomImage's is the same code, zoom_image.py:41-86).  Mixed
+// precision as the reference's numpy 1.x: c = K.t and c_x = c0/c2 in float32, everything after in float64, stored as float32.
+// ren_empty_bit: status bit set where the rendered box is empty and the zoom centres on the observed box (0: none)
 __global__ void zoom_factor_kernel(int *bbox8, const float *src_pose, int B, int H, int W, float k0, float k1,
                                    float k2, float k3, float k4, float k5, float k6, float k7, float k8,
-                                   float *zoom_factor, int *bbox_out, int *status, const int *cls_flag) {
+                                   float *zoom_factor, int *bbox_out, int *status, const int *cls_flag, int ren_empty_bit) {
   int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
   const int cf = cls_flag ? cls_flag[b] : 0;  // rasteriser: bad class index (bit 1)
@@ -79,7 +80,7 @@ __global__ void zoom_factor_kernel(int *bbox8, const float *src_pose, int B, int
     if (status) status[b] = 1 | cf;
     return;
   }
-  if (status) status[b] = cf;
+  if (status) status[b] = cf | (bb[5] < 0 ? ren_empty_bit : 0);
   const double real_x0 = bb[0], real_x1 = bb[1], real_y0 = bb[2], real_y1 = bb[3];
   const float *sp = src_pose + 12 * b;
   const float t0 = sp[3], t1 = sp[7], t2 = sp[11];
@@ -242,7 +243,7 @@ int zoom_factor_launch(dim_ctx *ctx, const float *mask_real, const float *mask_r
                                                        img_means ? img_means[1] : 0.f, img_means ? img_means[2] : 0.f);
   DIM_LAUNCH_CHECK();
   zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
-                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, nullptr);
+                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, nullptr, 0);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -268,7 +269,72 @@ int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *
   zoom_factor_from_ren_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_ren, ctx->bbox8, B);
   DIM_LAUNCH_CHECK();
   zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
-                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag);
+                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag, 0);
+  DIM_LAUNCH_CHECK();
+  return 0;
+}
+
+// Image-only network (ZoomImage, zoom_image.py:33-37): the observed box of the fused loop, valid = sum_c(image + mean) > 0.01
+// over obs4's colours (which hold image + mean), the float32 sum of mask_bbox_kernel's img_mode in the same channel order.
+// Once per dim_refine call: the observed image does not change over the iterations.  One block per (row, instance).
+__global__ void __launch_bounds__(160) obs_colour_box_kernel(const float4 *obs4, int H, int W, int *bbox_obs) {
+  const int i = blockIdx.x, b = blockIdx.y;
+  const float4 *src = obs4 + ((size_t)b * H + i) * W;
+  int x0 = 0x7fffffff, x1 = -1;
+  for (int j = threadIdx.x; j < W; j += blockDim.x) {
+    const float4 v = src[j];
+    if (((v.x + v.y) + v.z) > 0.01f) {
+      x0 = min(x0, j);
+      x1 = max(x1, j);
+    }
+  }
+  x0 = __reduce_min_sync(0xffffffffu, x0);
+  x1 = __reduce_max_sync(0xffffffffu, x1);
+  if ((threadIdx.x & 31) == 0 && x1 >= 0) {
+    int *o = bbox_obs + 4 * b;
+    atomicMin(o + 0, x0);
+    atomicMax(o + 1, x1);
+    atomicMin(o + 2, i);
+    atomicMax(o + 3, i);
+  }
+}
+
+__global__ void box4_init_kernel(int *box, int B, int H, int W) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  box[4 * b + 0] = W;
+  box[4 * b + 1] = -1;
+  box[4 * b + 2] = H;
+  box[4 * b + 3] = -1;
+}
+
+int obs_colour_box_launch(dim_ctx *ctx, const float4 *obs4, int B, int *bbox_obs, cudaStream_t st) {
+  box4_init_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_obs, B, ctx->H, ctx->W);
+  DIM_LAUNCH_CHECK();
+  obs_colour_box_kernel<<<dim3(ctx->H, B), 160, 0, st>>>(obs4, ctx->H, ctx->W, bbox_obs);
+  DIM_LAUNCH_CHECK();
+  return 0;
+}
+
+// zoom factor of the image-only loop: the observed box from obs_colour_box_kernel, the rendered one from the rasteriser's
+// colour-valid bbox (raster.cu COLOUR_BOX), then ZoomImage's arithmetic -- zoom_factor_kernel, with the observed-centre
+// fallback for an empty render flagged as status bit 2 (the reference prints "NO POINT VALID IN rendered" and goes on); an
+// empty observed image is bit 0 with the (1,1,0,0) factor (the reference raises)
+__global__ void boxes_to_bbox8_kernel(const int *bbox_obs, const int *bbox_ren, int *bbox8, int B) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  for (int k = 0; k < 4; ++k) {
+    bbox8[8 * b + k] = bbox_obs[4 * b + k];
+    bbox8[8 * b + 4 + k] = bbox_ren[4 * b + k];
+  }
+}
+
+int zoom_factor_from_boxes_launch(dim_ctx *ctx, const int *bbox_obs, const int *bbox_ren, const float *src_pose, int B,
+                                  const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st) {
+  boxes_to_bbox8_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_obs, bbox_ren, ctx->bbox8, B);
+  DIM_LAUNCH_CHECK();
+  zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
+                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag, 4);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -375,7 +441,9 @@ __device__ __forceinline__ void pack_chunk(const float *v, uint4 &h, uint4 &l) {
 // The depths ride in the w lanes: obs4.w = depth_observed, ren4.w = the render's depth (0 = background, so the rendered
 // mask depth > 0.2 of tester.py:440 is the same binarisation at 0.2 as for the 0/1 mask).  ZoomDepth (zoom_depth.py:24-44)
 // is the plain bilinear sample, zero outside the frame: the image taps with no mean.
-template <bool LO, bool F16, bool DEPTH = false>
+// MASK = false (image-only network, INPUT_MASK: False, deepIM_flownet.py:53-62): channels 6 and 7 are exact zeros -- conv1's
+// weight pack carries zero columns there -- and neither the box mask nor the ren4.w taps are computed.
+template <bool LO, bool F16, bool DEPTH = false, bool MASK = true>
 __device__ __forceinline__ void zoom_fused_pixel(const FusedZoomParams &p, const float4 *__restrict__ ob,
                                                  const float4 *__restrict__ rn, const AxisTap &x, const AxisTap &y,
                                                  uint4 (&h)[DEPTH ? 2 : 1], uint4 (&l)[DEPTH ? 2 : 1]) {
@@ -413,15 +481,19 @@ __device__ __forceinline__ void zoom_fused_pixel(const FusedZoomParams &p, const
 #pragma unroll
     for (int c = 10; c < 16; ++c) v[c] = 0.f;
   }
-  {  // observed mask = rectangle (an empty box has m0 > m1 on both axes)
-    const float tl = (y.m0 && x.m0) ? 1.f : 0.f, tr = (y.m0 && x.m1) ? 1.f : 0.f;
-    const float bl = (y.m1 && x.m0) ? 1.f : 0.f, br = (y.m1 && x.m1) ? 1.f : 0.f;
-    v[MO] = roundf(fmaf(br, wd, fmaf(bl, wc, fmaf(tr, wb, tl * wa))));
-  }
-  {  // rendered mask, binarised at 0.2 (zoom_mask.py:39-41)
-    const float tl = R00.w > 0.2f ? 1.f : 0.f, tr = R01.w > 0.2f ? 1.f : 0.f;
-    const float bl = R10.w > 0.2f ? 1.f : 0.f, br = R11.w > 0.2f ? 1.f : 0.f;
-    v[MO + 1] = roundf(fmaf(br, wd, fmaf(bl, wc, fmaf(tr, wb, tl * wa))));
+  if constexpr (!MASK) {
+    v[MO] = v[MO + 1] = 0.f;
+  } else {
+    {  // observed mask = rectangle (an empty box has m0 > m1 on both axes)
+      const float tl = (y.m0 && x.m0) ? 1.f : 0.f, tr = (y.m0 && x.m1) ? 1.f : 0.f;
+      const float bl = (y.m1 && x.m0) ? 1.f : 0.f, br = (y.m1 && x.m1) ? 1.f : 0.f;
+      v[MO] = roundf(fmaf(br, wd, fmaf(bl, wc, fmaf(tr, wb, tl * wa))));
+    }
+    {  // rendered mask, binarised at 0.2 (zoom_mask.py:39-41)
+      const float tl = R00.w > 0.2f ? 1.f : 0.f, tr = R01.w > 0.2f ? 1.f : 0.f;
+      const float bl = R10.w > 0.2f ? 1.f : 0.f, br = R11.w > 0.2f ? 1.f : 0.f;
+      v[MO + 1] = roundf(fmaf(br, wd, fmaf(bl, wc, fmaf(tr, wb, tl * wa))));
+    }
   }
   pack_chunk<LO, F16>(v, h[0], l[0]);
   if constexpr (DEPTH) pack_chunk<LO, F16>(v + 8, h[1], l[1]);
@@ -432,14 +504,15 @@ __device__ __forceinline__ void zoom_fused_pixel(const FusedZoomParams &p, const
 // slots are rewritten with zeros.  Sources are the pixel-interleaved float4 images, so each tap is one 16-byte load
 // per image; the column taps of the quad's two columns and the row taps of its two rows are computed once each.
 // DEPTH: the RGB-D network's input, two chunk planes per quad slot: [B*Hs rows][8 planes = (slot, half)][Ws cols][8 ch]
-template <bool LO, bool F16, bool DEPTH = false>
+template <bool LO, bool F16, bool DEPTH = false, bool MASK = true>
 __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParams p) {
   const int b = blockIdx.y;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= p.Hs * p.Ws) return;
   const int sr = q / p.Ws, sc = q - sr * p.Ws;
   const float4 z = __ldg(reinterpret_cast<const float4 *>(p.zoom_factor) + b);
-  int4 bb = __ldg(reinterpret_cast<const int4 *>(p.bbox8) + 2 * b);  // observed box (inclusive); bb.y < 0: empty
+  int4 bb = make_int4(1, 0, 1, 0);  // observed box (inclusive); empty: m0 > m1
+  if (MASK) bb = __ldg(reinterpret_cast<const int4 *>(p.bbox8) + 2 * b);
   if (bb.y < 0) { bb.x = 1; bb.y = 0; bb.z = 1; bb.w = 0; }
   int4 vb = make_int4(0, p.W, 0, p.H);
   if (p.vbox) vb = __ldg(reinterpret_cast<const int4 *>(p.vbox) + b);
@@ -460,7 +533,7 @@ __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParam
     uint4 h[NC], l[NC];
 #pragma unroll
     for (int c = 0; c < NC; ++c) h[c] = l[c] = make_uint4(0u, 0u, 0u, 0u);  // zero bits are the same in both formats
-    if (i >= 0 && i < p.H && j >= 0 && j < p.W) zoom_fused_pixel<LO, F16, DEPTH>(p, ob, rn, xt[s & 1], yt[s >> 1], h, l);
+    if (i >= 0 && i < p.H && j >= 0 && j < p.W) zoom_fused_pixel<LO, F16, DEPTH, MASK>(p, ob, rn, xt[s & 1], yt[s >> 1], h, l);
 #pragma unroll
     for (int c = 0; c < NC; ++c) {
       const size_t o = ((((size_t)b * p.Hs + sr) * 4 * NC + s * NC + c) * p.Ws + sc) * 8;
@@ -472,7 +545,7 @@ __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParam
 
 int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, const float *zoom_factor,
                       const float *means_rgb, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
-                      cudaStream_t st, int f16, const double *means_d, bool depth) {
+                      cudaStream_t st, int f16, const double *means_d, bool depth, bool mask) {
   FusedZoomParams p;
   p.obs4 = obs4; p.ren4 = ren4;
   p.bbox8 = ctx->bbox8; p.zoom_factor = zoom_factor;
@@ -484,7 +557,12 @@ int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, cons
   p.stepy = (float)(2.0 / (double)(ctx->H - 1));
   p.hi = hi; p.lo = lo;
   dim3 grid(cdiv(Hs * Ws, 128), B);
-  if (depth) {
+  DIM_REQUIRE(mask || !depth, "zoom_fused: the image-only network has no depth input");
+  if (!mask) {
+    if (f16) zoom_fused_nhwc8_kernel<false, true, false, false><<<grid, 128, 0, st>>>(p);
+    else if (lo) zoom_fused_nhwc8_kernel<true, false, false, false><<<grid, 128, 0, st>>>(p);
+    else zoom_fused_nhwc8_kernel<false, false, false, false><<<grid, 128, 0, st>>>(p);
+  } else if (depth) {
     if (f16) zoom_fused_nhwc8_kernel<false, true, true><<<grid, 128, 0, st>>>(p);
     else if (lo) zoom_fused_nhwc8_kernel<true, false, true><<<grid, 128, 0, st>>>(p);
     else zoom_fused_nhwc8_kernel<false, false, true><<<grid, 128, 0, st>>>(p);
@@ -534,7 +612,8 @@ int pack_obs4_launch(dim_ctx *ctx, const float *img, int B, float4 *out, const d
   return 0;
 }
 
-// NCHW float32 zoomed blobs -> conv1 NHWC8 bf16 input (used by dim_net_fwd on the op surface)
+// NCHW float32 zoomed blobs -> conv1 NHWC8 bf16 input (used by dim_net_fwd on the op surface); mo = mr = nullptr: the
+// image-only network, whose channels 6-7 are zeros
 __global__ void __launch_bounds__(256) pack_nhwc8_kernel(const float *io, const float *ir, const float *mo,
                                                          const float *mr, int H, int W, int Hs, int Ws, int pad,
                                                          __nv_bfloat16 *hi, __nv_bfloat16 *lo, int f16) {
@@ -548,8 +627,8 @@ __global__ void __launch_bounds__(256) pack_nhwc8_kernel(const float *io, const 
     v[c] = io[((size_t)b * 3 + c) * P + q] / 255.0f;
     v[3 + c] = ir[((size_t)b * 3 + c) * P + q] / 255.0f;
   }
-  v[6] = mo[(size_t)b * P + q];
-  v[7] = mr[(size_t)b * P + q];
+  v[6] = mo ? mo[(size_t)b * P + q] : 0.f;
+  v[7] = mr ? mr[(size_t)b * P + q] : 0.f;
   __align__(16) __nv_bfloat16 h[8];
   __align__(16) __nv_bfloat16 l[8];
 #pragma unroll

@@ -75,6 +75,8 @@ SIGNATURES = {
     "dim_refine_host_rgbd_async": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32,
                                          C.POINTER(Lighting), vp]),
     "dim_net_fwd_rgbd": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp]),
+    "dim_ctx_set_input_mask": (i32, [vp, i32]),
+    "dim_train_param_info_nomask": (i32, [i32, C.POINTER(C.c_char_p), C.POINTER(i64), C.POINTER(i64)]),
     "dim_transform_image_u8": (i32, [vp, vp, i32, pf64, vp, vp]),
     "dim_debug_activation": (i32, [vp, i32, i32, vp, u64]),
     "dim_debug_layer_geometry": (i32, [vp, i32, C.POINTER(i32)]),

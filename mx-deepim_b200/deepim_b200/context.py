@@ -63,10 +63,13 @@ def _lighting_arg(lighting, shape, on_device):
 
 class Context:
     def __init__(self, device=0, max_batch=16, height=480, width=640, max_classes=16, max_verts=60000,
-                 max_faces=120000, input_depth=False):
+                 max_faces=120000, input_depth=False, input_mask=True):
         """input_depth=True: the RGB-D network (config.network.INPUT_DEPTH, deepIM_flownet.py:33-51).  Its input gains
         depth_observed/255 and depth_rendered/255 as channels 6 and 7, so flow_conv1_weight is (64, 10, 7, 7); refine /
-        refine_host then need the observed depth and net_forward the zoomed depths.  Training it is not supported."""
+        refine_host then need the observed depth and net_forward the zoomed depths.
+        input_mask=False: the image-only network (config.network.INPUT_MASK: False, deepIM_flownet.py:53-62): conv1 sees the
+        two images only, so flow_conv1_weight is (64, 6, 7, 7); refine / refine_host zoom with ZoomImage (boxes from the
+        images' colours) and net_forward takes no masks.  Not combinable with input_depth."""
         if not torch.cuda.is_available():
             raise capi.DeepIMError("deepim_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         self.device = torch.device("cuda", device)
@@ -77,8 +80,11 @@ class Context:
         self._h = h
         self.num_classes = 0
         self.input_depth = bool(input_depth)
+        self.input_mask = bool(input_mask)
         if self.input_depth:
             check(lib.dim_ctx_set_input_depth(h, 1))
+        if not self.input_mask:
+            check(lib.dim_ctx_set_input_mask(h, 0))
 
     def _stream(self):
         """torch's current stream OF THIS CONTEXT'S DEVICE (a process may hold contexts on several GPUs)"""
@@ -115,11 +121,11 @@ class Context:
         """weights: name_weight / name_bias float32 arrays with MXNet layouts
         (deepim/symbols/deepIM_flownet.py:63-116,716-717)."""
         shape = tuple(np.shape(weights["flow_conv1_weight"]))
-        want = (64, 10 if self.input_depth else 8, 7, 7)
+        want = (64, 10 if self.input_depth else (8 if self.input_mask else 6), 7, 7)
         if shape != want:
-            raise ValueError("flow_conv1_weight has shape %s: this context's network takes %s (Context(input_depth=%s)); "
-                             "(64, 8, 7, 7) belongs to Context(input_depth=False), (64, 10, 7, 7) to Context(input_depth=True)"
-                             % (shape, want, self.input_depth))
+            raise ValueError("flow_conv1_weight has shape %s: this context's network takes %s (Context(input_depth=%s, "
+                             "input_mask=%s)); (64, 8, 7, 7) belongs to Context(), (64, 10, 7, 7) to Context(input_depth=True), "
+                             "(64, 6, 7, 7) to Context(input_mask=False)" % (shape, want, self.input_depth, self.input_mask))
         keep = []
         W = (C.c_void_p * 14)()
         Bv = (C.c_void_p * 14)()
@@ -359,10 +365,10 @@ class Context:
         return out
 
     # --------------------------------------------------------------------------------- net
-    def net_forward(self, zoom_image_observed, zoom_image_rendered, zoom_mask_observed, zoom_mask_rendered,
+    def net_forward(self, zoom_image_observed, zoom_image_rendered, zoom_mask_observed=None, zoom_mask_rendered=None,
                     precision=capi.PREC_BF16X3, zoom_depth_observed=None, zoom_depth_rendered=None):
         """The network on already-zoomed blobs; an RGB-D context (input_depth=True) also takes the zoomed depths
-        f32 [B,1,H,W] (metres)."""
+        f32 [B,1,H,W] (metres); an image-only context (input_mask=False) takes no masks (None)."""
         B = zoom_image_observed.shape[0]
         rot, trans = self._new((B, 4)), self._new((B, 3))
         if zoom_depth_observed is None and zoom_depth_rendered is None:

@@ -170,18 +170,19 @@ class LM6DRefine:
 
 
 def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl", "cup"), n_iter=4, max_batch=16, device=0,
-             precision="fp16", input_depth=False):
+             precision="fp16", input_depth=False, input_mask=True):
     """Batched pred_eval (deepim/core/tester.py:50-527 without its batch = 1 limit): refine every pair of the image set
     and score it the way the reference's dataset class does: ADD / ADI accuracy + AUC (evaluate_pose_add), 5 cm 5 deg
     (evaluate_pose) and Proj. 2D (evaluate_pose_arp_2d); the last two under res["rot_trans"] / res["arp_2d"].
     input_depth=True refines with the RGB-D network (weights with a (64, 10, 7, 7) flow_conv1) and reads each observed frame's
     `-depth.png` as well (image.py:190-219; converted on the device with DEPTH_FACTOR).
+    input_mask=False refines with the image-only network (weights with a (64, 6, 7, 7) flow_conv1; ZoomImage).
     Returns (evaluate_pose_add result + the two extra tables, poses_est [n_iter,M,3,4], poses_gt)."""
     from . import pose_eval
     from .refiner import PoseRefiner
     meshes = [dataset.mesh(c) for c in dataset.classes]
     ref = PoseRefiner(meshes, weights, K=K, device=device, max_batch=max_batch, n_iter=n_iter, precision=precision,
-                      input_depth=input_depth, depth_factor=DEPTH_FACTOR)
+                      input_depth=input_depth, depth_factor=DEPTH_FACTOR, input_mask=input_mask)
     imgs, cls_idx, init, gt, depths = [], [], [], [], []
     for ci, c in enumerate(dataset.classes):
         for pair in dataset.pairs(c):

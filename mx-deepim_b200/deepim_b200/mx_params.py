@@ -139,6 +139,20 @@ def input_depth_of(arg_params) -> bool:
     raise ValueError("flow_conv1_weight has shape %s: expected (64, 8, 7, 7) (RGB) or (64, 10, 7, 7) (RGB-D)" % (shape,))
 
 
+def network_of(arg_params) -> dict:
+    """Which network a checkpoint belongs to, as Context keyword arguments, from its flow_conv1_weight: (64, 8, 7, 7) = RGB
+    (INPUT_MASK) -> {input_depth: False, input_mask: True}; (64, 10, 7, 7) = RGB-D (INPUT_DEPTH + INPUT_MASK) -> input_depth
+    True; (64, 6, 7, 7) = image-only (INPUT_MASK: False, deepIM_flownet.py:53-62, e.g. a FlowNetS-initialised model) ->
+    input_mask False.  Anything else raises ValueError."""
+    shape = tuple(np.shape(arg_params["flow_conv1_weight"]))
+    nets = {(64, 8, 7, 7): (False, True), (64, 10, 7, 7): (True, True), (64, 6, 7, 7): (False, False)}
+    if shape not in nets:
+        raise ValueError("flow_conv1_weight has shape %s: expected (64, 8, 7, 7) (RGB), (64, 10, 7, 7) (RGB-D) or (64, 6, 7, 7) "
+                         "(image-only)" % (shape,))
+    depth, mask = nets[shape]
+    return {"input_depth": depth, "input_mask": mask}
+
+
 # ----------------------------------------------------------------------------------------- <prefix>-symbol.json
 # MXNet writes the network graph next to the checkpoint (`Module.save_checkpoint` -> `<prefix>-symbol.json`): a JSON object
 # {"nodes": [{"op": "null" | "<Operator>", "name": ..., "attrs" (>= 1.0) | "attr" | "param" (older): {str: str},

@@ -12,7 +12,10 @@ carry `normals`, and each submit draws its light intensities [n_iter, n, 3] from
 
 input_depth=True runs the RGB-D network (config.network.INPUT_DEPTH; weights with a (64, 10, 7, 7) flow_conv1): submit /
 refine then also take the observed depth as the loader's uint16 file values [N,H,W] (LINEMOD's *-depth.png), converted on the
-device as float32(u16) / float32(depth_factor)."""
+device as float32(u16) / float32(depth_factor).
+
+input_mask=False runs the image-only network (config.network.INPUT_MASK: False; weights with a (64, 6, 7, 7) flow_conv1): the
+loop zooms with ZoomImage, boxes from the images' colours."""
 from __future__ import annotations
 
 import numpy as np
@@ -27,7 +30,7 @@ from .context import Context
 class PoseRefiner:
     def __init__(self, meshes, weights, K=synth.K_LINEMOD, device=0, max_batch=16, n_iter=4,
                  pixel_means_rgb=synth.PIXEL_MEANS_RGB, znear=synth.ZNEAR, zfar=synth.ZFAR, precision="fp16",
-                 n_slots=2, lighting=None, input_depth=False, depth_factor=1000.0):
+                 n_slots=2, lighting=None, input_depth=False, depth_factor=1000.0, input_mask=True):
         self.light = _lighting.LightSource.of(lighting)
         if self.light is not None:
             for i, m in enumerate(meshes):
@@ -40,10 +43,11 @@ class PoseRefiner:
         mf = max(len(m.faces) for m in meshes)
         self.max_batch = max_batch
         self.input_depth, self.depth_factor = bool(input_depth), float(depth_factor)
+        self.input_mask = bool(input_mask)
         self.slots = []
         for _ in range(n_slots):
             ctx = Context(device, max_batch=max_batch, max_classes=len(meshes), max_verts=mv, max_faces=mf,
-                          input_depth=self.input_depth)
+                          input_depth=self.input_depth, input_mask=self.input_mask)
             for i, m in enumerate(meshes):
                 ctx.upload_mesh(i, m)
             ctx.load_weights(weights)
@@ -107,16 +111,18 @@ class PoseRefiner:
     def result(self, ticket, strict=True):
         """Block until the batch is done; returns poses [n_iter, n, 3, 4] float64 (numpy copy).
         The per-iteration device status is checked: an instance whose object left the view frustum (empty rendered mask;
-        the reference crashes in ZoomMask there) or whose class index is invalid raises DeepIMError when strict, else the
-        flags are left in `self.last_status` ([n_iter, n] int32) for the caller."""
+        the reference crashes in ZoomMask there; image-only network: an observed image with no valid pixel) or whose class
+        index is invalid raises DeepIMError when strict, else the flags are left in `self.last_status` ([n_iter, n] int32) for
+        the caller.  Bit 2 (image-only network: empty render, the zoom centred on the observed box as the reference does) is
+        reported there but does not raise."""
         slot = self.slots[ticket]
         slot["stream"].synchronize()
         slot["busy"] = False
         n, B = slot["n"], self.max_batch
         ni = min(self.n_iter, 8)
         self.last_status = slot["status"][: ni * n].view(ni, n).numpy().copy()
-        if strict and self.last_status.any():
-            bad = sorted(set(np.nonzero(self.last_status)[1].tolist()))
+        if strict and (self.last_status & 3).any():
+            bad = sorted(set(np.nonzero(self.last_status & 3)[1].tolist()))
             raise capi.DeepIMError("PoseRefiner: instances %s of the batch have a non-zero device status (bit 0: empty rendered "
                                    "mask -- object left the frustum; bit 1: bad class index): %s"
                                    % (bad, self.last_status[:, bad].tolist()))

@@ -266,11 +266,16 @@ def bilinear_upsampling_kernel(k: int = 32) -> np.ndarray:
     return np.outer(v, v).astype(np.float32)
 
 
-def make_train_weights(seed: int = 0, input_depth: bool = False):
+def make_train_weights(seed: int = 0, input_depth: bool = False, input_mask: bool = True):
     """make_weights + the train-only decoder / flow / mask heads (deepIM_flownet.py:121-167,176-193,317-338):
     He-normal decoder convs/deconvs (a k4 s2 deconv sums Cin*4 taps per output), N(0, 0.01) mask_conv3
-    (init_weights l.811-813), frozen bilinear `upsampling` (2 groups) / `mask_upsampling` kernels."""
+    (init_weights l.811-813), frozen bilinear `upsampling` (2 groups) / `mask_upsampling` kernels.
+    input_mask=False: the image-only network, make_weights' flow_conv1 without its two mask columns (64, 6, 7, 7)."""
+    if input_depth and not input_mask:
+        raise ValueError("input_depth with input_mask=False is not supported")
     w = make_weights(seed, input_depth)
+    if not input_mask:
+        w["flow_conv1_weight"] = np.ascontiguousarray(w["flow_conv1_weight"][:, :6])
     rng = np.random.default_rng(seed + 1000003)
     gain = np.sqrt(2.0 / (1.0 + 0.1 ** 2))
     for name, kind, shp, nb in DECODER_SPECS:

@@ -19,7 +19,9 @@ from ._capi import check, lib
 NORMALIZE_FLOW = 20.0
 
 
-def _param_info(input_depth):
+def _param_info(input_depth, input_mask=True):
+    if not input_mask:
+        return lib.dim_train_param_info_nomask
     return lib.dim_train_param_info_rgbd if input_depth else lib.dim_train_param_info
 
 
@@ -27,13 +29,18 @@ def _is_rgbd(weights) -> bool:
     return np.shape(weights["flow_conv1_weight"])[1:2] == (10,)
 
 
-def param_table(input_depth=False):
+def _is_nomask(weights) -> bool:
+    return np.shape(weights["flow_conv1_weight"])[1:2] == (6,)
+
+
+def param_table(input_depth=False, input_mask=True):
     """[(tensor name, numel)] in flat order, as the library reports it (dim_train_param_info; input_depth: the RGB-D
-    network's table, dim_train_param_info_rgbd, whose flow_conv1 is (64, 10, 7, 7))."""
+    network's table, dim_train_param_info_rgbd, whose flow_conv1 is (64, 10, 7, 7); input_mask=False: the image-only
+    network's table, dim_train_param_info_nomask, whose flow_conv1 is (64, 6, 7, 7))."""
     out = []
     for i in range(64):
         name, wn, bn = C.c_char_p(), C.c_int64(), C.c_int64()
-        if _param_info(input_depth)(i, C.byref(name), C.byref(wn), C.byref(bn)) != 0:
+        if _param_info(input_depth, input_mask)(i, C.byref(name), C.byref(wn), C.byref(bn)) != 0:
             break
         out.append((name.value.decode() + "_weight", wn.value))
         if bn.value:
@@ -42,9 +49,10 @@ def param_table(input_depth=False):
 
 
 def flatten_params(weights: dict) -> np.ndarray:
-    """The flat vector of the table the weights belong to (RGB-D when flow_conv1_weight has 10 input channels)."""
+    """The flat vector of the table the weights belong to (RGB-D when flow_conv1_weight has 10 input channels, image-only
+    when it has 6)."""
     parts = []
-    for name, n in param_table(_is_rgbd(weights)):
+    for name, n in param_table(_is_rgbd(weights), not _is_nomask(weights)):
         a = np.asarray(weights[name], dtype=np.float32)
         if name == "fc6_weight":  # the flat vector keeps fc6 as (out, h*10+w, c): NHWC order of the conv6_1 activation
             a = a.reshape(256, 1024, 80).transpose(0, 2, 1)
@@ -57,7 +65,7 @@ def flatten_params(weights: dict) -> np.ndarray:
 
 def unflatten_params(flat: np.ndarray, like: dict) -> dict:
     out, off = {}, 0
-    for name, n in param_table(_is_rgbd(like)):
+    for name, n in param_table(_is_rgbd(like), not _is_nomask(like)):
         a = np.asarray(flat[off:off + n], np.float32)
         if name == "fc6_weight":  # back to MXNet's (out, c*80 + h*10 + w) (deepIM_flownet.py:110-112)
             a = a.reshape(256, 80, 1024).transpose(0, 2, 1)
@@ -66,12 +74,12 @@ def unflatten_params(flat: np.ndarray, like: dict) -> dict:
     return out
 
 
-def tensor_sizes(input_depth=False):
+def tensor_sizes(input_depth=False, input_mask=True):
     """[(table index, weight + bias numel)] of the tensors of the flat vector (dim_train_param_info order)."""
     out = []
     for i in range(64):
         nm, wn, bn = C.c_char_p(), C.c_int64(), C.c_int64()
-        if _param_info(input_depth)(i, C.byref(nm), C.byref(wn), C.byref(bn)) != 0:
+        if _param_info(input_depth, input_mask)(i, C.byref(nm), C.byref(wn), C.byref(bn)) != 0:
             break
         out.append((i, wn.value + bn.value))
     return out
@@ -112,14 +120,16 @@ class Trainer:
         every step of this context -- forward_backward, fit_batch, test_forward_full and the updates (see set_precision)."""
         self.ctx, self.lr, self.momentum, self.wd = ctx, lr, momentum, wd
         self.input_depth = bool(getattr(ctx, "input_depth", False))  # Context(input_depth=True): the RGB-D network
-        if _is_rgbd(weights) != self.input_depth:
+        self.input_mask = bool(getattr(ctx, "input_mask", True))  # Context(input_mask=False): the image-only network
+        if _is_rgbd(weights) != self.input_depth or _is_nomask(weights) == self.input_mask:
             raise ValueError("flow_conv1_weight has %d input channels; this context's network takes %d"
-                             % (np.shape(weights["flow_conv1_weight"])[1], 10 if self.input_depth else 8))
+                             % (np.shape(weights["flow_conv1_weight"])[1],
+                                10 if self.input_depth else (8 if self.input_mask else 6)))
         check(lib.dim_train_create(ctx._h, max_points))
         if config:
             ctx.set_config(**config)
         self.n = int(lib.dim_train_param_count(ctx._h))
-        self.table = param_table(self.input_depth)
+        self.table = param_table(self.input_depth, self.input_mask)
         flat = flatten_params(weights)
         assert flat.size == self.n
         self._shapes = {k: np.asarray(v).shape for k, v in weights.items()}
@@ -127,7 +137,7 @@ class Trainer:
         torch.cuda.current_stream(ctx.device).synchronize()
         self.set_precision(precision)
         self.grads = torch.zeros(self.n, dtype=torch.float32, device=ctx.device)
-        self.buckets, self.bucket_first = make_buckets(bucket_mb, tensor_sizes(self.input_depth))
+        self.buckets, self.bucket_first = make_buckets(bucket_mb, tensor_sizes(self.input_depth, self.input_mask))
         self._events = None
         self._comm_stream = None
 
@@ -167,17 +177,19 @@ class Trainer:
         """z: dict of device float32 tensors (the outputs of the zoom front of the train symbol + labels):
         zoom_image_observed/rendered (B,3,H,W), zoom_mask_observed/rendered (B,1,H,W), zoom_factor (B,4),
         zoom_flow, zoom_flow_weights (B,2,H,W), zoom_mask_gt_observed (B,1,H,W), src_pose (B,3,4),
-        point_cloud_model/weights/observed (B,3,N); RGB-D network: also zoom_depth_observed / zoom_depth_rendered (B,1,H,W)."""
+        point_cloud_model/weights/observed (B,3,N); RGB-D network: also zoom_depth_observed / zoom_depth_rendered (B,1,H,W).
+        The image-only network does not read zoom_mask_observed / zoom_mask_rendered (they may be absent); the GT mask
+        label still is."""
         ctx = self.ctx
         B, N = z["zoom_image_observed"].shape[0], z["point_cloud_model"].shape[2]
+        zmo, zmr = (z["zoom_mask_observed"], z["zoom_mask_rendered"]) if self.input_mask else (None, None)
         for k, t in z.items():
             if t.dtype != torch.float32 or not t.is_contiguous() or not t.is_cuda:
                 raise TypeError("%s must be a contiguous float32 CUDA tensor" % k)
         out = {"rot_est_norm": ctx._new((B, 4)), "trans_est": ctx._new((B, 3)), "losses": ctx._new((4,)),
                "flow_est": ctx._new((B, 2, ctx.H, ctx.W)) if want_maps else None,
                "mask_prob": ctx._new((B, 1, ctx.H, ctx.W)) if want_maps else None}
-        args = (ctx._h, _p(z["zoom_image_observed"]), _p(z["zoom_image_rendered"]), _p(z["zoom_mask_observed"]),
-                _p(z["zoom_mask_rendered"]), _p(z["zoom_factor"]), _p(z["zoom_flow"]), _p(z["zoom_flow_weights"]),
+        args = (ctx._h, _p(z["zoom_image_observed"]), _p(z["zoom_image_rendered"]), _p(zmo), _p(zmr), _p(z["zoom_factor"]), _p(z["zoom_flow"]), _p(z["zoom_flow_weights"]),
                 _p(z["zoom_mask_gt_observed"]), _p(z["src_pose"]), _p(z["point_cloud_model"]), _p(z["point_cloud_weights"]),
                 _p(z["point_cloud_observed"]), B, N, _p(out["rot_est_norm"]), _p(out["trans_est"]), _p(out["flow_est"]),
                 _p(out["mask_prob"]), _p(out["losses"]), _p(self.grads) if backward else None, None,
@@ -195,9 +207,14 @@ class Trainer:
         flow_est = invZoomFlow(upsampled flow x NORMALIZE_FLOW), plus the zoomed intermediates the graph also returns.
         batch: image_observed/rendered (B,3,H,W), mask_observed/rendered (B,1,H,W), src_pose (B,3,4), pixel_means_rgb."""
         ctx = self.ctx
-        zo, zg, zr, zf, bbox, status = ctx.zoom_mask(batch["mask_observed"], batch["mask_observed"], batch["mask_rendered"],
-                                                     batch["src_pose"], K)
-        zio, zir = ctx.zoom_image_with_factor(zf, batch["image_observed"], batch["image_rendered"], batch["pixel_means_rgb"])
+        if self.input_mask:
+            zo, zg, zr, zf, bbox, status = ctx.zoom_mask(batch["mask_observed"], batch["mask_observed"], batch["mask_rendered"],
+                                                         batch["src_pose"], K)
+            zio, zir = ctx.zoom_image_with_factor(zf, batch["image_observed"], batch["image_rendered"], batch["pixel_means_rgb"])
+        else:  # the image-only test graph zooms with ZoomImage and feeds no masks (deepIM_flownet.py:562-601)
+            zio, zir, zf, bbox, status = ctx.zoom_image(batch["image_observed"], batch["image_rendered"], batch["src_pose"], K,
+                                                        batch["pixel_means_rgb"])
+            zo = zr = None
         B = zio.shape[0]
         rot, trans = ctx._new((B, 4)), ctx._new((B, 3))
         zflow, zprob = ctx._new((B, 2, ctx.H, ctx.W)), ctx._new((B, 1, ctx.H, ctx.W))
