@@ -1666,7 +1666,8 @@ int train_sgd_update(dim_ctx *ctx, const float *grads, float lr, float momentum,
   return 0;
 }
 
-// test / debugging hook: copy an intermediate to the host.  id: 0 flow6, 1 flow5, 2 flow4, 3 mask4 (fp32);
+// test / debugging hook: copy an intermediate to the host.  id: 0 flow6, 1 flow5, 2 flow4, 3 mask4, 4 dflow4, 5 dmask4,
+// 6 dflow5, 7 dflow6, 8 h6 (the fc6 activation kept for the backward pass), 9 dh6 (gradient of fc6's pre-activation) (fp32);
 // 10 cat2, 11 cat3, 12 dcat2, 13 dcat3, 14 dA10p, 15 act10b, 20+i gz[i] (bf16, whole bordered buffer); 100 + one of the bf16 ids:
 // that buffer's lo half (exists once the step has run in bf16x3)
 int train_debug_tensor(dim_ctx *ctx, int id, void *host, size_t bytes) {
@@ -1688,6 +1689,8 @@ int train_debug_tensor(dim_ctx *ctx, int id, void *host, size_t bytes) {
     case 5: src = ts->dmask4; have = (size_t)B * g[5].Ho * g[5].Wo * 4; break;
     case 6: src = ts->dflow5; have = (size_t)B * g[7].Ho * g[7].Wo * 8; break;
     case 7: src = ts->dflow6; have = (size_t)B * g[9].Ho * g[9].Wo * 8; break;
+    case 8: src = ts->h6; have = (size_t)B * 256 * 4; break;
+    case 9: src = ts->dh6; have = (size_t)B * 256 * 4; break;
     case 10: fb(ts->cat2); break;
     case 11: fb(ts->cat3); break;
     case 12: fb(ts->dcat2); break;

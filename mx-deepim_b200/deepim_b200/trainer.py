@@ -285,12 +285,13 @@ class Trainer:
         return unflatten_params(flat, {k: np.empty(s, np.float32) for k, s in self._shapes.items()})
 
     def debug_tensor(self, tid):
-        """fp32 maps (id < 10) as [B,h,w,c]; bf16 buffers (id >= 10) as float32 [B,Hp,Wp,C] incl. border."""
+        """fp32 maps (id < 8) as [B,h,w,c], h6 / dh6 (8 / 9) as [B,256]; bf16 buffers (id >= 10) as float32 [B,Hp,Wp,C]
+        incl. border."""
         ctx = self.ctx
         B = ctx.max_batch
         if tid < 10:
             hw = {0: (8, 10, 2), 1: (15, 20, 2), 2: (30, 40, 2), 3: (30, 40, 1), 4: (30, 40, 2), 5: (30, 40, 1), 6: (15, 20, 2),
-                  7: (8, 10, 2)}[tid]
+                  7: (8, 10, 2), 8: (256,), 9: (256,)}[tid]
             a = np.empty((B,) + hw, np.float32)
             check(lib.dim_train_debug_tensor(ctx._h, tid, a.ctypes.data_as(C.c_void_p), a.nbytes))
             return a

@@ -36,6 +36,8 @@ NORMALIZE_FLOW, NORMALIZE_3D_POINT = 20.0, 0.1
 ENC = [("flow_conv1", 2, 3), ("conv2", 2, 2), ("conv3", 2, 2), ("conv3_1", 1, 1), ("conv4", 2, 1),
        ("conv4_1", 1, 1), ("conv5", 2, 1), ("conv5_1", 1, 1), ("conv6", 2, 1), ("conv6_1", 1, 1)]
 FROZEN = ("upsampling_weight", "mask_upsampling_weight")
+# deconv5 / deconv4 of the decoder below: 4x4, stride 2, output cropped to the skip connection's size from row / column 1
+DECONV_STRIDE, DECONV_CROP = 2, 1
 
 
 def bilinear_kernel(k=32):
@@ -102,12 +104,14 @@ def graph(weights, zin, labels, requires_grad=True, num_threads=None, emulate_bf
     ztrans = F.linear(h, P["trans_weight"], P["trans_bias"])
     # decoder (symbol:121-165)
     flow6 = F.conv2d(r10, P["Convolution1_weight"], P["Convolution1_bias"], padding=1)
-    d5 = F.conv_transpose2d(r10, P["deconv5_weight"], P["deconv5_bias"], stride=2)[:, :, 1:1 + r8.shape[2], 1:1 + r8.shape[3]]
+    d5 = F.conv_transpose2d(r10, P["deconv5_weight"], P["deconv5_bias"],
+                            stride=DECONV_STRIDE)[:, :, DECONV_CROP:DECONV_CROP + r8.shape[2], DECONV_CROP:DECONV_CROP + r8.shape[3]]
     up65 = F.conv_transpose2d(flow6, P["upsample_flow6to5_weight"], P["upsample_flow6to5_bias"], stride=2)
     up65 = store(up65[:, :, 1:1 + r8.shape[2], 1:1 + r8.shape[3]])
     cat2 = torch.cat([r8, lrelu(d5), up65], dim=1)
     flow5 = F.conv2d(cat2, P["Convolution2_weight"], P["Convolution2_bias"], padding=1)
-    d4 = F.conv_transpose2d(cat2, P["deconv4_weight"], P["deconv4_bias"], stride=2)[:, :, 1:1 + r6.shape[2], 1:1 + r6.shape[3]]
+    d4 = F.conv_transpose2d(cat2, P["deconv4_weight"], P["deconv4_bias"],
+                            stride=DECONV_STRIDE)[:, :, DECONV_CROP:DECONV_CROP + r6.shape[2], DECONV_CROP:DECONV_CROP + r6.shape[3]]
     up54 = F.conv_transpose2d(flow5, P["upsample_flow5to4_weight"], P["upsample_flow5to4_bias"], stride=2)
     up54 = store(up54[:, :, 1:1 + r6.shape[2], 1:1 + r6.shape[3]])
     cat3 = torch.cat([r6, lrelu(d4), up54], dim=1)

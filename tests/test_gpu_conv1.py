@@ -1,6 +1,10 @@
-"""flow_conv1 (conv1_kernel) on its own, in every precision, at batch sizes whose row runs end mid-image or leave a short
-last run: the stored activation against a torch conv2d of the same 16-bit input blob, the zero border and the images past
-the batch left untouched, every value finite."""
+"""The inference network's kernels one at a time, in every precision: each encoder layer (flow_conv1 through conv1_kernel,
+conv2 ... conv6_1 through conv_igemm_persistent_kernel) against a float64 convolution of exactly the 16-bit input the device
+stored (the seeded blob for conv1, act[i] for layer i), and fc6 (fc6_mma_kernel) + fc7 + the rot / trans heads against
+float64 from the stored act[10].  Batch sizes whose tiles span images and end mid-image; the zero border and the images past
+the batch left untouched; a full batch of a tight allocation.  Bound (tests/kernel_ref.py):
+|dev - ref| <= rho |ref| + kappa 2^-24 S element by element, rho the output storage (fp16 2^-11, bf16 2^-8, bf16x3 2^-15)."""
+import json
 import os
 import sys
 
@@ -14,6 +18,8 @@ for p in (ROOT, os.path.join(ROOT, "mx-deepim_b200")):
     if p not in sys.path:
         sys.path.insert(0, p)
 
+import kernel_ref as R  # noqa: E402
+from oracle.train_oracle import ENC  # noqa: E402
 from deepim_b200 import _capi as capi  # noqa: E402
 from deepim_b200 import synth  # noqa: E402
 from deepim_b200.context import Context  # noqa: E402
@@ -21,26 +27,46 @@ from deepim_b200.context import Context  # noqa: E402
 pytestmark = pytest.mark.gpu
 
 H, W, MAXB = 480, 640, 16
-# per precision: (mode, how the device rounds conv1's operands, bound on |act - ref| relative to max(1, |ref|max)).
-# The reference sees the same rounded operands, so what is left is the 16-bit output rounding and the fp32 summation order.
-MODES = {
-    "fp16": (capi.PREC_FP16, lambda t: t.half().double(), 2.5e-3),
-    "bf16": (capi.PREC_BF16, lambda t: t.bfloat16().double(), 8e-3),
-    "bf16x3": (capi.PREC_BF16X3, lambda t: t.double(), 2e-4),
+MODES = {"fp16": capi.PREC_FP16, "bf16": capi.PREC_BF16, "bf16x3": capi.PREC_BF16X3}
+# kappa per kernel family: 4 x the largest (|err| - rho |ref|) / (2^-24 S) observed over every case of this file, rounded
+# up to two digits and at least 1 ("obs"; measured on an H100 80GB HBM3 at a 400 W power limit).  Printed when the module ends (pytest -s).
+KAPPA = {
+    "conv1": 24,       # obs 5.9     conv1_kernel
+    "tower": 96,       # obs 24.0    conv_igemm_persistent_kernel, conv2 ... conv6_1
+    "fc6_head": 1,     # obs 0.0042  fc6_mma_kernel + head_kernel (fc7, rot, trans in fp32); S carried through fc7 and the heads
 }
+SIZES = [(H, W)]  # SIZES[i]: the interior of act[i], the input of encoder layer i (filled from the weights' kernel sizes)
 
 
 @pytest.fixture(scope="module")
 def weights():
-    return synth.make_weights(0)
+    w = synth.make_weights(0)
+    del SIZES[1:]
+    for name, s, p in ENC:
+        k = w[name + "_weight"].shape[-1]
+        SIZES.append(((SIZES[-1][0] + 2 * p - k) // s + 1, (SIZES[-1][1] + 2 * p - k) // s + 1))
+    return w
+
+
+def _open(weights, max_batch):
+    if not torch.cuda.is_available():
+        pytest.skip("needs a GPU")
+    c = Context(0, max_batch=max_batch)
+    c.load_weights(weights)
+    return c
 
 
 @pytest.fixture(scope="module")
 def ctx(weights):
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    c = Context(0, max_batch=MAXB)
-    c.load_weights(weights)
+    c = _open(weights, MAXB)
+    yield c
+    c.close()
+    print("\ninference kernels, largest kappa needed: " + json.dumps({k: float("%.4g" % v) for k, v in sorted(R.OBSERVED.items())}))
+
+
+@pytest.fixture(scope="module")
+def ctx5(weights):
+    c = _open(weights, 5)
     yield c
     c.close()
 
@@ -54,58 +80,97 @@ def _blobs(B, seed):
     return zio, zir, zmo, zmr
 
 
-def _act1(ctx, mode, n=MAXB):
-    """conv2's bordered input buffer for the first n images (hi + lo in bf16x3)."""
-    a, g = ctx.debug_activation(1, n, fp16=mode == "fp16")
-    if mode == "bf16x3":
-        a = a + ctx.debug_activation(1, n, lo=True)[0]
-    return a, g
-
-
-def _check_batch(ctx, weights, mode, B, n):
-    """runs conv1 on a seeded batch of B; checks the first n images of its output buffer, returns them."""
-    prec, rnd, tol = MODES[mode]
+def _forward(ctx, mode, B, seed):
     dev = torch.device("cuda", 0)
-    w = rnd(torch.from_numpy(np.asarray(weights["flow_conv1_weight"], np.float32))).to(dev)
-    b = torch.from_numpy(np.asarray(weights["flow_conv1_bias"], np.float32)).double().to(dev)
-    zio, zir, zmo, zmr = _blobs(B, B)
-    ctx.net_forward(zio.to(dev), zir.to(dev), zmo.to(dev), zmr.to(dev), prec)
-    act, g = _act1(ctx, mode, n)
-    py, px, Ho, Wo = g[3], g[4], 240, 320  # g[5:7] are conv2's output extent
-    assert np.isfinite(act).all(), (mode, B)
-    x = rnd(torch.cat([zio / 255.0, zir / 255.0, zmo, zmr], dim=1)).to(dev)
-    ref = F.leaky_relu(F.conv2d(x, w, b, stride=2, padding=3), 0.1).permute(0, 2, 3, 1).cpu().numpy()
-    inner = act[:B, py:py + Ho, px:px + Wo, :]
-    err = np.abs(inner - ref).max()
-    assert err < tol * max(1.0, np.abs(ref).max()), (mode, B, err)
-    border = act[:B].copy()
-    border[:, py:py + Ho, px:px + Wo, :] = 0
-    assert not border.any(), "conv1 wrote into the zero border (%s, B=%d)" % (mode, B)
-    return act
+    blobs = _blobs(B, seed)
+    rot, trans = ctx.net_forward(*[t.to(dev) for t in blobs], MODES[mode])
+    return blobs, rot, trans
 
 
+def _act(ctx, mode, idx, n):
+    """act[idx] as stored for the first n images: hi, lo (bf16x3; else None) float32 [n, rows, cols, C] incl. border, and
+    its interior (py, px, H, W)"""
+    hi, g = ctx.debug_activation(idx, n, fp16=mode == "fp16")
+    lo = ctx.debug_activation(idx, n, lo=True)[0] if mode == "bf16x3" else None
+    return hi, lo, (g[3], g[4]) + SIZES[idx]
+
+
+def _check_layer(ctx, weights, mode, layer, B, n, seed=None):
+    """runs the network on a seeded batch of B and checks layer `layer` from its stored input; returns the first n images of
+    its output buffer (hi, lo)"""
+    name, s, p = ENC[layer]
+    blobs = _forward(ctx, mode, B, B if seed is None else seed)[0]
+    hi, lo, geo = _act(ctx, mode, layer + 1, n)
+    assert np.isfinite(hi).all(), (name, mode, B)
+    if layer == 0:
+        zio, zir, zmo, zmr = blobs
+        x = R.operand(torch.cat([zio / 255.0, zir / 255.0, zmo, zmr], dim=1), mode)
+    else:
+        ihi, ilo, igeo = _act(ctx, mode, layer, B)
+        x = R.interior(ihi, igeo, B), R.interior(ilo, igeo, B)
+    w = R.operand(weights[name + "_weight"], mode)
+    b = R.gpu(weights[name + "_bias"])[None, :, None, None]
+    ref, S = R.products(lambda a, ww: F.conv2d(a, ww, stride=s, padding=p), x, w)
+    out = R.fused((R.interior(hi, geo, B), R.interior(lo, geo, B)))[0]
+    R.check("conv1" if layer == 0 else "tower", "%s (%s, B=%d)" % (name, mode, B), out, F.leaky_relu(ref + b, 0.1),
+            S + b.abs(), R.RHO[mode], KAPPA["conv1" if layer == 0 else "tower"], R.at_pixel)
+    for half in (hi, lo):
+        assert half is None or R.border_is_zero(half, geo, B), "%s wrote into the zero border (%s, B=%d)" % (name, mode, B)
+    return hi, lo
+
+
+LAYER_IDS = [name for name, _, _ in ENC]
+
+
+@pytest.mark.parametrize("layer", range(10), ids=LAYER_IDS)
 @pytest.mark.parametrize("mode", sorted(MODES))
-def test_conv1_matches_torch_and_keeps_borders(ctx, weights, mode):
-    dev = torch.device("cuda", 0)
+def test_layer_matches_float64_and_keeps_borders(ctx, weights, mode, layer):
+    """B = 1, 3, 16 on one context: row runs and tiles that end mid-image, span images, or leave a short last run"""
     # fill every image of the buffer first, so that a smaller batch writing past its last image would show
-    ctx.net_forward(*[t.to(dev) for t in _blobs(MAXB, 99)], MODES[mode][0])
-    before, _ = _act1(ctx, mode)
+    _forward(ctx, mode, MAXB, 99)
+    before = _act(ctx, mode, layer + 1, MAXB)[:2]
     for B in (1, 3, MAXB):
-        act = _check_batch(ctx, weights, mode, B, MAXB)
+        got = _check_layer(ctx, weights, mode, layer, B, MAXB)
         if B < MAXB:
-            assert np.array_equal(act[B:], before[B:]), "conv1 wrote past image %d (%s)" % (B - 1, mode)
+            for g, b0 in zip(got, before):
+                assert g is None or np.array_equal(g[B:], b0[B:]), "%s wrote past image %d (%s)" % (ENC[layer][0], B - 1, mode)
+
+
+@pytest.mark.parametrize("layer", range(10), ids=LAYER_IDS)
+@pytest.mark.parametrize("mode", sorted(MODES))
+def test_layer_full_batch_of_a_tight_allocation(ctx5, weights, mode, layer):
+    """A full batch (B = max_batch) ends its input buffer at the batch's last input row.  For conv1 the run of rows that ends
+    there is 3 strips longer than its output rows; max_batch = 5 puts that end 49 KB short of the 2 MiB granule the buffer's
+    allocation is rounded to, less than the 62 KB of 3 strips: conv1 reads none of them.  The other layers' tiles past the
+    last image are virtual rows, masked in the epilogue."""
+    _check_layer(ctx5, weights, mode, layer, 5, 5)
+
+
+def _fc6_nhwc(a):
+    """fc6 (256, c*80 + hw) in MXNet order -> (256, hw*1024 + c), the NHWC order of act[10] the kernel reads"""
+    return np.ascontiguousarray(np.asarray(a).reshape(256, 1024, 80).transpose(0, 2, 1)).reshape(256, 81920)
 
 
 @pytest.mark.parametrize("mode", sorted(MODES))
-def test_conv1_full_batch_of_a_tight_allocation(weights, mode):
-    """A full batch (B = max_batch) ends its input buffer at the batch's last input row, and the run of rows that ends
-    there is 3 strips longer than its output rows.  max_batch = 5 puts that end 49 KB short of the 2 MiB granule the
-    buffer's allocation is rounded to, less than the 62 KB of 3 strips: conv1 reads none of them."""
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    c = Context(0, max_batch=5)
-    try:
-        c.load_weights(weights)
-        _check_batch(c, weights, mode, 5, 5)
-    finally:
-        c.close()
+def test_fc6_and_heads_match_float64(ctx, weights, mode):
+    """rot / trans of net_forward against float64 fc6 -> fc7 -> heads from the stored act[10]: fc6's operands as its 16-bit
+    pack rounds them (fp16, bf16 or the bf16x3 hi / lo passes), fc7 / rot / trans from the fp32 weights.  B = 1, 3, 9, 16: the
+    batch is the M rows of mma.m16n8k16, B = 9 and 16 use both 8-row halves.  The error scale S of fc6 is carried through
+    fc7 and the heads by their absolute weights (LeakyReLU moves no difference up)."""
+    lrelu = lambda v: F.leaky_relu(v, 0.1)
+    W6 = R.operand(_fc6_nhwc(weights["fc6_weight"]), mode)
+    wb = {k: R.gpu(weights[k]) for k in ("fc6_bias", "fc7_weight", "fc7_bias", "rot_weight", "rot_bias", "trans_weight",
+                                         "trans_bias")}
+    for B in (1, 3, 9, MAXB):
+        _, rot, trans = _forward(ctx, mode, B, 50 + B)
+        hi, lo, _ = _act(ctx, mode, 10, B)
+        a = R.gpu(hi).reshape(B, 81920), (None if lo is None else R.gpu(lo).reshape(B, 81920))
+        z6, S6 = R.products(lambda x, w: x @ w.T, a, W6)
+        h6, E6 = lrelu(z6 + wb["fc6_bias"]), S6 + wb["fc6_bias"].abs()
+        w7 = wb["fc7_weight"]
+        h7 = lrelu(h6 @ w7.T + wb["fc7_bias"])
+        E7 = E6 @ w7.abs().T + h6.abs() @ w7.abs().T + wb["fc7_bias"].abs()
+        for name, dev in (("rot", rot), ("trans", trans)):
+            w, b = wb[name + "_weight"], wb[name + "_bias"]
+            R.check("fc6_head", "%s (%s, B=%d)" % (name, mode, B), dev, h7 @ w.T + b, E7 @ w.abs().T + h7.abs() @ w.abs().T + b.abs(),
+                    0.0, KAPPA["fc6_head"], lambda idx: "(image %d, output %d)" % idx)

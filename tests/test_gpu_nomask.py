@@ -17,6 +17,7 @@ if not torch.cuda.is_available():
     pytest.skip("no CUDA device", allow_module_level=True)
 
 import nomask_oracle  # noqa: E402
+from kernel_ref import s2d_decode  # noqa: E402
 from oracle import oracle as O  # noqa: E402
 from deepim_b200 import _capi as capi  # noqa: E402
 from deepim_b200 import lighting, synth  # noqa: E402
@@ -110,19 +111,16 @@ def test_conv1_input_is_the_zoomed_images(ctx, case, prec):
     hi, g = ctx.debug_activation(0, B, fp16=f16)
     rows, cols, ch, pad = g[0], g[1], g[2], g[3]
     assert ch == 32
-    xp = np.zeros((B, 8, 2 * rows, 2 * cols), np.float32)
-    xp[:, :6, pad:pad + H, pad:pad + W] = x
-    # chunk plane ph*2 + pw holds the 8 channels of pixel (2r + ph, 2c + pw)
-    exp = xp.reshape(B, 8, rows, 2, cols, 2).transpose(0, 2, 3, 5, 4, 1).reshape(B, rows, 4, cols, 8)
+    exp = np.zeros((B, 8, 2 * rows, 2 * cols), np.float32)
+    exp[:, :6, pad:pad + H, pad:pad + W] = x
     rnd = (lambda a: a.astype(np.float16).astype(np.float32)) if f16 else \
         (lambda a: torch.from_numpy(a).bfloat16().float().numpy())
-    got = hi.reshape(B, rows, 4, cols, 8)
+    got = s2d_decode(hi)
     assert np.array_equal(got, rnd(exp)), np.argwhere(got != rnd(exp))[:5]
-    assert not got[..., 6:].any()
+    assert not got[:, 6:].any()
     if prec == capi.PREC_BF16X3:
-        lo, _ = ctx.debug_activation(0, B, lo=True)
-        lo = lo.reshape(B, rows, 4, cols, 8)
-        assert np.array_equal(lo, rnd(exp - rnd(exp))) and not lo[..., 6:].any()
+        lo = s2d_decode(ctx.debug_activation(0, B, lo=True)[0])
+        assert np.array_equal(lo, rnd(exp - rnd(exp))) and not lo[:, 6:].any()
 
 
 def test_nomask_refine_teacher_forced_per_iteration(ctx, case):
