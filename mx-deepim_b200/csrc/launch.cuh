@@ -82,6 +82,8 @@ int pose_error_launch(const double *pose_est, const double *pose_gt, int M, cons
 int net_create(dim_ctx *ctx);
 void net_destroy(dim_ctx *ctx);
 int net_load(dim_ctx *ctx, const float *const *W, const float *const *Bv);
+int net_alloc_weights(dim_ctx *ctx);
+int net_pack_weights(dim_ctx *ctx, const float *const *w, cudaStream_t st, bool with_lo, bool with_f16);
 void net_input_geometry(dim_ctx *ctx, int *rows, int *cols, int *pad, __nv_bfloat16 **hi, __nv_bfloat16 **lo);
 int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, float *rot_out, float *trans_out,
                 float *se3_out, cudaStream_t st, cudaEvent_t after_conv);

@@ -9,6 +9,7 @@
 #include <cuda_fp16.h>
 #include <string.h>
 
+#include <memory>
 #include <mutex>
 
 #include "launch.cuh"
@@ -367,26 +368,108 @@ void net_destroy(dim_ctx *ctx) {
   ctx->net = nullptr;
 }
 
-static void split_bf16(const float *src, size_t n, std::vector<__nv_bfloat16> &hi, std::vector<__nv_bfloat16> &lo,
-                       std::vector<__nv_bfloat16> &f16) {
-  hi.resize(n);
-  lo.resize(n);
-  f16.resize(n);
-  for (size_t i = 0; i < n; ++i) {
-    hi[i] = __float2bfloat16_rn(src[i]);
-    lo[i] = __float2bfloat16_rn(src[i] - __bfloat162float(hi[i]));
-    const __half h = __float2half_rn(src[i]);  // He-scale weights are far inside the fp16 range; inf only for |w| > 65504
-    memcpy(&f16[i], &h, 2);
+// ------------------------------------------------------------------------------ weight packing
+// fp32 weights in the flat parameter vector's layouts -> 16-bit operand packs.  The same kernels serve dim_net_load (from a
+// staging copy of the checkpoint) and the training step (from the fp32 master after every update).
+//
+// forward pack [Cout][kh][kw][Cin] of conv2 ... conv6_1: block = (co, 64 input channels), which reads k*k-float rows
+// (contiguous) into shared memory and writes 64 consecutive 16-bit values per tap
+__global__ void __launch_bounds__(256) pack_conv_fwd_kernel(const float *w, int Cout, int Cin, int k, __nv_bfloat16 *hi,
+                                                            __nv_bfloat16 *lo, __nv_bfloat16 *f16) {
+  __shared__ float tile[64 * 25];
+  const int co = blockIdx.x, c0 = blockIdx.y * 64, kk = k * k;
+  const int nc = min(64, Cin - c0);
+  const float *src = w + ((size_t)co * Cin + c0) * kk;
+  for (int i = threadIdx.x; i < nc * kk; i += 256) tile[i] = src[i];
+  __syncthreads();
+#pragma unroll 2  // the compiler's 4 with the optional fp16 store takes 40 registers (6 blocks per SM instead of 8)
+  for (int i = threadIdx.x; i < nc * kk; i += 256) {
+    const int tap = i / nc, cl = i - tap * nc;
+    store_split(hi, lo, ((size_t)co * kk + tap) * Cin + c0 + cl, tile[cl * kk + tap], f16);
   }
 }
+// RGB-D conv1 space-to-depth pack [64][4][4][64]: W'[co][dh][dw][(ph*2 + pw)*16 + c] = W[co][c][2dh+ph][2dw+pw] for c < 10
+// (0 beyond 7x7 and for c >= 10)
+__global__ void __launch_bounds__(256) pack_conv1_rgbd_kernel(const float *w, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
+                                                              __nv_bfloat16 *f16) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 64 * 1024) return;
+  const int co = i >> 10, tap = (i >> 6) & 15, phase = (i >> 4) & 3, c = i & 15;
+  const int kh = 2 * (tap >> 2) + (phase >> 1), kw = 2 * (tap & 3) + (phase & 1);
+  store_split(hi, lo, i, (c < 10 && kh < 7 && kw < 7) ? w[((co * 10 + c) * 7 + kh) * 7 + kw] : 0.f, f16);
+}
+// conv1 space-to-depth pack [64][4][4][32] of a (64, cin, 7, 7) weight: W'[co][dh][dw][conv1_kslot(dw,ph,pw) + c] =
+// W[co][c][2dh+ph][2dw+pw] (0 beyond 7x7); cin = 8, or 6 for the image-only network, whose mask lanes 6-7 get zero columns
+__global__ void __launch_bounds__(256) pack_conv1_kernel(const float *w, int cin, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
+                                                         __nv_bfloat16 *f16) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 64 * 512) return;
+  const int c = i & 7, pw = (i >> 3) & 1, ph = (i >> 4) & 1, dw = (i >> 5) & 3, dh = (i >> 7) & 3, co = i >> 9;
+  const int kh = 2 * dh + ph, kw = 2 * dw + pw;
+  store_split(hi, lo, (i & ~31) + conv1_kslot(dw, ph, pw) + c,
+              (c < cin && kh < 7 && kw < 7) ? w[((co * cin + c) * 7 + kh) * 7 + kw] : 0.f, f16);
+}
+// fc6 (out, hw, c) fp32 -> 16-bit operand (same order)
+__global__ void __launch_bounds__(256) pack_fc6_kernel(const float *w, __nv_bfloat16 *hi, __nv_bfloat16 *lo, __nv_bfloat16 *f16) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)256 * FC6_K) return;
+  store_split(hi, lo, i, w[i], f16);
+}
+// fc7 (out, in) -> fp32 [in][out] for head_kernel
+__global__ void transpose256_kernel(const float *w, float *wT) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < 65536) wT[(i & 255) * 256 + (i >> 8)] = w[i];
+}
 
-// first call allocates, later calls (dim_net_load on a loaded context) overwrite in place: the tensor maps
-// cached in NetState::maps keep pointing at valid storage
-template <typename T>
-static int upload(dim_ctx *ctx, T **dst, const std::vector<T> &v) {
-  if (*dst == nullptr)
-    if (int rc = dev_alloc(ctx, dst, v.size(), false)) return rc;
-  DIM_CHECK(cudaMemcpy(*dst, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+// first call allocates, later calls return at once: a reload overwrites in place, so the tensor maps cached in
+// NetState::maps keep pointing at valid storage
+int net_alloc_weights(dim_ctx *ctx) {
+  NetState *ns = ctx->net;
+  if (ns->trans_b) return 0;  // allocated last
+  for (int i = 0; i < 10; ++i) {
+    const LayerGeom &g = ns->g[i];
+    const size_t n = (size_t)g.Cout * g.KH * g.KW * g.Ceff;
+    if (int rc = dev_alloc(ctx, &ns->w_hi[i], n)) return rc;
+    if (int rc = dev_alloc(ctx, &ns->w_lo[i], n)) return rc;
+    if (int rc = dev_alloc(ctx, &ns->w_f16[i], n)) return rc;
+    if (int rc = dev_alloc(ctx, &ns->bias[i], g.Cout)) return rc;
+  }
+  const size_t n6 = (size_t)256 * FC6_K;
+  if (int rc = dev_alloc(ctx, &ns->fc6_w_hi, n6)) return rc;
+  if (int rc = dev_alloc(ctx, &ns->fc6_w_lo, n6)) return rc;
+  if (int rc = dev_alloc(ctx, &ns->fc6_w_f16, n6)) return rc;
+  if (int rc = dev_alloc(ctx, &ns->fc6_b, 256)) return rc;
+  if (int rc = dev_alloc(ctx, &ns->fc7_wT, 256 * 256)) return rc;
+  if (int rc = dev_alloc(ctx, &ns->fc7_b, 256)) return rc;
+  if (int rc = dev_alloc(ctx, &ns->rot_w, 4 * 256)) return rc;
+  if (int rc = dev_alloc(ctx, &ns->rot_b, 4)) return rc;
+  if (int rc = dev_alloc(ctx, &ns->trans_w, 3 * 256)) return rc;
+  return dev_alloc(ctx, &ns->trans_b, 3);
+}
+
+// w[0..9]: conv1 ... conv6_1 (Cout, Cin, k, k), w[10]: fc6 (256, hw, c), w[11]: fc7 (out, in), device fp32.  Packs are
+// written on st; a pack left out (with_lo / with_f16 false) is marked stale.
+int net_pack_weights(dim_ctx *ctx, const float *const *w, cudaStream_t st, bool with_lo, bool with_f16) {
+  NetState *ns = ctx->net;
+  auto L = [with_lo](__nv_bfloat16 *p) { return with_lo ? p : nullptr; };
+  auto F = [with_f16](__nv_bfloat16 *p) { return with_f16 ? p : nullptr; };
+  if (ns->input_depth)
+    pack_conv1_rgbd_kernel<<<64 * 1024 / 256, 256, 0, st>>>(w[0], ns->w_hi[0], L(ns->w_lo[0]), F(ns->w_f16[0]));
+  else
+    pack_conv1_kernel<<<64 * 512 / 256, 256, 0, st>>>(w[0], ns->input_mask ? 8 : 6, ns->w_hi[0], L(ns->w_lo[0]), F(ns->w_f16[0]));
+  DIM_LAUNCH_CHECK();
+  for (int i = 1; i < 10; ++i) {
+    const LayerSpec &s = kLayers[i];
+    pack_conv_fwd_kernel<<<dim3(s.Cout, cdiv(s.Cin, 64)), 256, 0, st>>>(w[i], s.Cout, s.Cin, s.k, ns->w_hi[i], L(ns->w_lo[i]),
+                                                                          F(ns->w_f16[i]));
+    DIM_LAUNCH_CHECK();
+  }
+  pack_fc6_kernel<<<256 * FC6_K / 256, 256, 0, st>>>(w[10], ns->fc6_w_hi, L(ns->fc6_w_lo), F(ns->fc6_w_f16));
+  DIM_LAUNCH_CHECK();
+  transpose256_kernel<<<256, 256, 0, st>>>(w[11], ns->fc7_wT);
+  DIM_LAUNCH_CHECK();
+  ns->lo_stale = !with_lo;
+  ns->f16_stale = !with_f16;
   return 0;
 }
 
@@ -423,76 +506,44 @@ int net_load(dim_ctx *ctx, const float *const *W, const float *const *Bv) {
   DIM_REQUIRE(ns->net_ok, "dim_net_load: FlowNetS + fc6 (81920 inputs) needs a 480x640 context");
   DIM_REQUIRE(!ns->train_aliased, "dim_net_load: this context trains; use dim_train_load_params (it owns the weights)");
   if (ns->loaded) DIM_CHECK(cudaDeviceSynchronize());  // a reload must not race kernels still reading the old weights
+  if (int rc = net_alloc_weights(ctx)) return rc;
+  // the packed tensors W[0..11] are staged on the device as fp32 for net_pack_weights (~180 MB, freed on return)
+  size_t n[12], off[13] = {0};
   for (int i = 0; i < 10; ++i) {
     const LayerGeom &g = ns->g[i];
-    const size_t Ktot = (size_t)g.KH * g.KW * g.Ceff;
-    std::vector<float> packed((size_t)g.Cout * Ktot, 0.f);
-    const float *w = W[i];  // [Cout][Cin][k][k]
-    if (i == 0 && ns->input_depth) {
-      // W'[co][dh][dw][(ph*2 + pw)*16 + c] = W[co][c][2dh+ph][2dw+pw] for c < 10 (0 beyond 7x7 and for c >= 10)
-      for (int co = 0; co < g.Cout; ++co)
-        for (int dh = 0; dh < 4; ++dh)
-          for (int dw = 0; dw < 4; ++dw)
-            for (int ph = 0; ph < 2; ++ph)
-              for (int pw = 0; pw < 2; ++pw)
-                for (int c = 0; c < 10; ++c) {
-                  const int kh = 2 * dh + ph, kw = 2 * dw + pw;
-                  if (kh >= 7 || kw >= 7) continue;
-                  packed[(size_t)co * Ktot + (size_t)(dh * 4 + dw) * 64 + (ph * 2 + pw) * 16 + c] =
-                      w[(((size_t)co * 10 + c) * 7 + kh) * 7 + kw];
-                }
-    } else if (i == 0) {
-      // space-to-depth repack: W'[co][dh][dw][conv1_kslot(dw,ph,pw)+c] = W[co][c][2dh+ph][2dw+pw] (0 beyond 7x7); the
-      // image-only network's W is (64, 6, 7, 7): its mask columns c = 6, 7 stay zero
-      const int cin = ns->input_mask ? 8 : 6;
-      for (int co = 0; co < g.Cout; ++co)
-        for (int dh = 0; dh < 4; ++dh)
-          for (int dw = 0; dw < 4; ++dw)
-            for (int ph = 0; ph < 2; ++ph)
-              for (int pw = 0; pw < 2; ++pw)
-                for (int c = 0; c < cin; ++c) {
-                  const int kh = 2 * dh + ph, kw = 2 * dw + pw;
-                  if (kh >= 7 || kw >= 7) continue;
-                  packed[(size_t)co * Ktot + (size_t)(dh * 4 + dw) * 32 + conv1_kslot(dw, ph, pw) + c] =
-                      w[(((size_t)co * cin + c) * 7 + kh) * 7 + kw];
-                }
-    } else {
-      for (int co = 0; co < g.Cout; ++co)
-        for (int c = 0; c < g.Cin; ++c)
-          for (int kh = 0; kh < g.k; ++kh)
-            for (int kw = 0; kw < g.k; ++kw)
-              packed[(size_t)co * Ktot + (size_t)(kh * g.k + kw) * g.Cin + c] =
-                  w[(((size_t)co * g.Cin + c) * g.k + kh) * g.k + kw];
-    }
-    std::vector<__nv_bfloat16> hi, lo, hf;
-    split_bf16(packed.data(), packed.size(), hi, lo, hf);
-    if (int rc = upload(ctx, &ns->w_hi[i], hi)) return rc;
-    if (int rc = upload(ctx, &ns->w_lo[i], lo)) return rc;
-    if (int rc = upload(ctx, &ns->w_f16[i], hf)) return rc;
-    std::vector<float> bv(Bv[i], Bv[i] + g.Cout);
-    if (int rc = upload(ctx, &ns->bias[i], bv)) return rc;
+    const int cin = i == 0 && !ns->input_depth ? (ns->input_mask ? 8 : 6) : g.Cin;
+    n[i] = (size_t)g.Cout * cin * g.k * g.k;
+  }
+  n[10] = (size_t)256 * FC6_K;
+  n[11] = 256 * 256;
+  for (int i = 0; i < 12; ++i) off[i + 1] = off[i] + n[i];
+  float *stage_p = nullptr;
+  DIM_CHECK(cudaMalloc(&stage_p, off[12] * sizeof(float)));
+  std::unique_ptr<float, cudaError_t (*)(void *)> stage(stage_p, cudaFree);
+  auto put = [](float *dst, const float *src, size_t count) {
+    return cudaMemcpy(dst, src, count * sizeof(float), cudaMemcpyHostToDevice);
+  };
+  const float *w[12];
+  for (int i = 0; i < 12; ++i) {
+    w[i] = stage.get() + off[i];
+    if (i != 10) DIM_CHECK(put(stage.get() + off[i], W[i], n[i]));
   }
   {  // fc6: (out, c*80 + h*10 + w) -> (out, (h*10+w)*1024 + c)   (NCHW flatten, deepIM_flownet.py:110)
     std::vector<float> p((size_t)256 * FC6_K);
     for (int o = 0; o < 256; ++o)
       for (int c = 0; c < 1024; ++c)
         for (int hw = 0; hw < 80; ++hw) p[(size_t)o * FC6_K + (size_t)hw * 1024 + c] = W[10][(size_t)o * FC6_K + (size_t)c * 80 + hw];
-    std::vector<__nv_bfloat16> hb, lb, fb;
-    split_bf16(p.data(), p.size(), hb, lb, fb);
-    if (int rc = upload(ctx, &ns->fc6_w_hi, hb)) return rc;
-    if (int rc = upload(ctx, &ns->fc6_w_lo, lb)) return rc;
-    if (int rc = upload(ctx, &ns->fc6_w_f16, fb)) return rc;
-    if (int rc = upload(ctx, &ns->fc6_b, std::vector<float>(Bv[10], Bv[10] + 256))) return rc;
-    std::vector<float> t((size_t)256 * 256);
-    for (int o = 0; o < 256; ++o)
-      for (int k = 0; k < 256; ++k) t[(size_t)k * 256 + o] = W[11][(size_t)o * 256 + k];
-    if (int rc = upload(ctx, &ns->fc7_wT, t)) return rc;
-    if (int rc = upload(ctx, &ns->fc7_b, std::vector<float>(Bv[11], Bv[11] + 256))) return rc;
-    if (int rc = upload(ctx, &ns->rot_w, std::vector<float>(W[12], W[12] + 4 * 256))) return rc;
-    if (int rc = upload(ctx, &ns->rot_b, std::vector<float>(Bv[12], Bv[12] + 4))) return rc;
-    if (int rc = upload(ctx, &ns->trans_w, std::vector<float>(W[13], W[13] + 3 * 256))) return rc;
-    if (int rc = upload(ctx, &ns->trans_b, std::vector<float>(Bv[13], Bv[13] + 3))) return rc;
+    DIM_CHECK(put(stage.get() + off[10], p.data(), n[10]));
   }
+  for (int i = 0; i < 10; ++i) DIM_CHECK(put(ns->bias[i], Bv[i], ns->g[i].Cout));
+  DIM_CHECK(put(ns->fc6_b, Bv[10], 256));
+  DIM_CHECK(put(ns->fc7_b, Bv[11], 256));
+  DIM_CHECK(put(ns->rot_w, W[12], 4 * 256));
+  DIM_CHECK(put(ns->rot_b, Bv[12], 4));
+  DIM_CHECK(put(ns->trans_w, W[13], 3 * 256));
+  DIM_CHECK(put(ns->trans_b, Bv[13], 3));
+  if (int rc = net_pack_weights(ctx, w, 0, /*with_lo=*/true, /*with_f16=*/true)) return rc;
+  DIM_CHECK(cudaStreamSynchronize(0));
   ns->loaded = true;
   return 0;
 }

@@ -36,6 +36,16 @@ struct TensorMaps {
 // (the pw = 1 half is kw = 7, outside the filter): the kernels feed that K step from chunk planes 0 and 2 and drop the other.
 __host__ __device__ inline int conv1_kslot(int dw, int ph, int pw) { return dw == 3 ? pw * 16 + ph * 8 : ph * 16 + pw * 8; }
 
+// one element of an operand pack from its fp32 weight: hi = bf16(v); lo = bf16(v - hi) (the bf16x3 residual) and f16 =
+// half(v), each only where its destination is given
+__device__ __forceinline__ void store_split(__nv_bfloat16 *hi, __nv_bfloat16 *lo, size_t i, float v,
+                                            __nv_bfloat16 *f16 = nullptr) {
+  const __nv_bfloat16 h = __float2bfloat16_rn(v);
+  hi[i] = h;
+  if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+  if (f16) reinterpret_cast<__half *>(f16)[i] = __float2half_rn(v);  // inf only for |w| > 65504
+}
+
 struct NetState {
   LayerGeom g[10];
   __nv_bfloat16 *w_hi[10] = {}, *w_lo[10] = {};
@@ -60,10 +70,10 @@ struct NetState {
   // image-only network (dim_ctx_set_input_mask(ctx, 0)): flow_conv1 takes 6 channels; conv1_kernel and its 8-lane input are
   // unchanged, the weight pack carries zero columns for lanes 6-7 and every producer writes zeros there
   bool input_mask = true;
-  float *save_h6 = nullptr, *save_h7 = nullptr;
+  float *save_h6 = nullptr, *save_h7 = nullptr;  // training: fc6 / fc7 activations kept for the backward pass ([B][256])
   cudaEvent_t repack_done = nullptr;  // training: the operand packs are refreshed on an internal stream after an update;
                                       // every consumer (net_forward) orders itself behind this event
-  bool lo_stale = false;  // training updated the weights without refreshing the bf16 'lo' halves (bf16x3 mode refreshes lazily)  // training: fc6 / fc7 activations kept for the backward pass ([B][256])
+  bool lo_stale = false;  // training updated the weights without refreshing the bf16 'lo' halves (bf16x3 mode refreshes lazily)
   std::map<int, TensorMaps> maps;  // per batch size (+ kF16MapKey for the fp16 operand maps)
   int max_batch = 0, num_sms = 132;
 };

@@ -75,8 +75,6 @@ struct TrainState {
   float *master = nullptr, *mom = nullptr;
   Buf act10b, cat2, cat3, dcat2, dcat3, dA10p, gz[10], s2d32;
   Buf s2d64;         // RGB-D network: conv1's input as NHWC-64 (weight gradient operand)
-  bool input_depth = false;  // the table's flow_conv1 is (64, 10, 7, 7)
-  bool input_mask = true;    // false: the image-only network, the table's flow_conv1 is (64, 6, 7, 7)
   float *flow6 = nullptr, *flow5 = nullptr, *flow4 = nullptr, *mask4 = nullptr;
   float *dflow6 = nullptr, *dflow5 = nullptr, *dflow4 = nullptr, *dmask4 = nullptr;
   float *dfull = nullptr;        // [B][3][H][W] gradient wrt the full-resolution flow (2) / mask logit (1)
@@ -675,47 +673,11 @@ __global__ void __launch_bounds__(256) sgd_kernel(float *w, float *mom, const fl
   w[i] += m;
 }
 
-// ---- weight repacking (fp32 master, MXNet layouts -> bf16 operand packs)
-__device__ __forceinline__ void store_split(__nv_bfloat16 *hi, __nv_bfloat16 *lo, size_t i, float v) {
-  const __nv_bfloat16 h = __float2bfloat16_rn(v);
-  hi[i] = h;
-  if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-}
-// The packs are permutations of (Cout, Cin, k, k); a thread-per-destination gather reads the master with a k*k-float
-// stride (every 4-byte read in its own sector).  The tiled kernels below read k*k-float rows (contiguous) into shared
-// memory and write 64 consecutive bf16 per (tap, class): both sides coalesced.
+// ---- weight repacking (fp32 master, MXNet layouts -> bf16 operand packs); the inference network's packs are net.cu's
+// (net_pack_weights).  The packs are permutations of (Cout, Cin, k, k); a thread-per-destination gather reads the master
+// with a k*k-float stride (every 4-byte read in its own sector).  The tiled kernels below read k*k-float rows (contiguous)
+// into shared memory and write 64 consecutive bf16 per (tap, class): both sides coalesced.
 //
-// forward pack [Cout][kh][kw][Cin] (net.cu net_load): block = (co, 64 input channels)
-__global__ void __launch_bounds__(256) pack_conv_fwd_kernel(const float *w, int Cout, int Cin, int k, __nv_bfloat16 *hi, __nv_bfloat16 *lo) {
-  __shared__ float tile[64 * 25];
-  const int co = blockIdx.x, c0 = blockIdx.y * 64, kk = k * k;
-  const int nc = min(64, Cin - c0);
-  const float *src = w + ((size_t)co * Cin + c0) * kk;
-  for (int i = threadIdx.x; i < nc * kk; i += 256) tile[i] = src[i];
-  __syncthreads();
-  for (int i = threadIdx.x; i < nc * kk; i += 256) {
-    const int tap = i / nc, cl = i - tap * nc;
-    store_split(hi, lo, ((size_t)co * kk + tap) * Cin + c0 + cl, tile[cl * kk + tap]);
-  }
-}
-// RGB-D conv1 space-to-depth pack [64][4][4][64]: K = (ph*2 + pw)*16 + c within a tap (net.cu net_load)
-__global__ void __launch_bounds__(256) pack_conv1_rgbd_kernel(const float *w, __nv_bfloat16 *hi, __nv_bfloat16 *lo) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= 64 * 1024) return;
-  const int co = i >> 10, tap = (i >> 6) & 15, phase = (i >> 4) & 3, c = i & 15;
-  const int kh = 2 * (tap >> 2) + (phase >> 1), kw = 2 * (tap & 3) + (phase & 1);
-  store_split(hi, lo, i, (c < 10 && kh < 7 && kw < 7) ? w[((co * 10 + c) * 7 + kh) * 7 + kw] : 0.f);
-}
-// conv1 space-to-depth pack [64][4][4][32] of a (64, cin, 7, 7) master: cin = 8, or 6 for the image-only network, whose
-// mask lanes 6-7 get zero columns
-__global__ void __launch_bounds__(256) pack_conv1_kernel(const float *w, int cin, __nv_bfloat16 *hi, __nv_bfloat16 *lo) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= 64 * 512) return;
-  const int c = i & 7, pw = (i >> 3) & 1, ph = (i >> 4) & 1, dw = (i >> 5) & 3, dh = (i >> 7) & 3, co = i >> 9;
-  const int kh = 2 * dh + ph, kw = 2 * dw + pw;
-  store_split(hi, lo, (i & ~31) + conv1_kslot(dw, ph, pw) + c,
-              (c < cin && kh < 7 && kw < 7) ? w[((co * cin + c) * 7 + kh) * 7 + kw] : 0.f);
-}
 // data-gradient packs of ALL parity classes of one layer: class (ry, rx) is [Cin][Ty][Tx][Cout] with ky = ry + s*(Ty-1-ty).
 // block = (ci, 64 output channels): reads 64 rows of k*k floats, writes 64 consecutive bf16 per (class, tap)
 // lo[c] = nullptr: no lo half (bf16 step); otherwise the bf16x3 residual pack of class c
@@ -767,22 +729,12 @@ __global__ void __launch_bounds__(256) pack_deconv_dgrad_kernel(const float *w, 
     store_split(dst, dst_lo, ((size_t)ci * 16 + tap) * Cout + co, dtile[co * 17 + tap]);
   }
 }
-// fc6 master (out, hw, c) fp32 -> bf16 hi/lo operand (same order)
-__global__ void __launch_bounds__(256) pack_fc6_kernel(const float *w, __nv_bfloat16 *hi, __nv_bfloat16 *lo) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)256 * 81920) return;
-  store_split(hi, lo, i, w[i]);
-}
 // thin-conv weights (CO, Cin, 3, 3) -> [tap][co][ci] fp32 so that lanes striding over ci read consecutive words
 __global__ void __launch_bounds__(256) pack_thin_kernel(const float *w, int CO, int Cin, float *wt) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= CO * Cin * 9) return;
   const int ci = i % Cin, co = (i / Cin) % CO, tap = i / (Cin * CO);
   wt[i] = w[((size_t)(co * Cin + ci)) * 9 + tap];
-}
-__global__ void transpose256_kernel(const float *w, float *wT) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < 65536) wT[(i & 255) * 256 + (i >> 8)] = w[i];
 }
 
 // ------------------------------------------------------------------------------------ host side
@@ -819,11 +771,9 @@ int train_create(dim_ctx *ctx, int max_points) {
   TrainState *ts = new TrainState();
   train_of(ctx) = ts;
   ts->max_points = max_points;
-  ts->input_depth = ns->input_depth;
-  ts->input_mask = ns->input_mask;
   size_t off = 0;
   for (int i = 0; i < 24; ++i) {
-    ts->off[i].w = off; ts->off[i].wn = param_numel(param_spec(i, ts->input_depth, ts->input_mask)); off += ts->off[i].wn;
+    ts->off[i].w = off; ts->off[i].wn = param_numel(param_spec(i, ns->input_depth, ns->input_mask)); off += ts->off[i].wn;
     ts->off[i].b = off; ts->off[i].bn = bias_numel(kParams[i]); off += ts->off[i].bn;
   }
   ts->n_params = off;
@@ -839,7 +789,7 @@ int train_create(dim_ctx *ctx, int max_points) {
   rc |= alloc_buf(ctx, ts->dcat3, B, g[5].Ho, g[5].Wo, 832, 1, true);
   rc |= alloc_buf(ctx, ts->dA10p, B, g[9].Ho, g[9].Wo, 1024, 0, false);
   for (int i = 0; i < 10; ++i) rc |= alloc_buf(ctx, ts->gz[i], B, g[i].Ho, g[i].Wo, g[i].Cout, 1, false);
-  if (ts->input_depth) rc |= alloc_buf(ctx, ts->s2d64, B, g[0].rows, g[0].cols, 64, 0, false);
+  if (ns->input_depth) rc |= alloc_buf(ctx, ts->s2d64, B, g[0].rows, g[0].cols, 64, 0, false);
   else rc |= alloc_buf(ctx, ts->s2d32, B, g[0].rows, g[0].cols, 32, 0, false);
   const size_t n6 = (size_t)B * g[9].Ho * g[9].Wo, n5 = (size_t)B * g[7].Ho * g[7].Wo, n4 = (size_t)B * g[5].Ho * g[5].Wo;
   rc |= dev_alloc(ctx, &ts->flow6, n6 * 2, true); rc |= dev_alloc(ctx, &ts->dflow6, n6 * 2, true);
@@ -912,30 +862,23 @@ void train_destroy(dim_ctx *ctx) {
 
 // refresh every bf16 operand pack (and the fp32 head parameters of the inference net) from the master weights
 // with_lo = false skips the bf16 'lo' halves (only the bf16x3 modes read them); they are then marked stale and refreshed
-// lazily by train_refresh_lo() the next time the bf16x3 inference mode runs, or by the switch of the step to bf16x3
+// lazily by train_refresh_lo() the next time the bf16x3 inference mode runs, or by the switch of the step to bf16x3.  The
+// fp16 packs of DIM_PREC_FP16 are marked stale too: net_forward re-derives them from hi/lo when that mode next runs
 static int repack_all(dim_ctx *ctx, cudaStream_t st, bool with_lo) {
-  NetState *ns = ctx->net;
   TrainState *ts = train_of(ctx);
   const float *M = ts->master;
-  if (ts->input_depth) LAUNCH1D(pack_conv1_rgbd_kernel, 64 * 1024, st, M + ts->off[0].w, ns->w_hi[0], with_lo ? ns->w_lo[0] : nullptr);
-  else LAUNCH1D(pack_conv1_kernel, 64 * 512, st, M + ts->off[0].w, ts->input_mask ? 8 : 6, ns->w_hi[0],
-                with_lo ? ns->w_lo[0] : nullptr);
+  const float *w[12];
+  for (int i = 0; i < 12; ++i) w[i] = M + ts->off[i].w;
+  if (int rc = net_pack_weights(ctx, w, st, with_lo, /*with_f16=*/false)) return rc;
   // the training packs' lo halves exist once the step has run in bf16x3 (nullptr before)
   auto L = [with_lo](__nv_bfloat16 *lo) { return with_lo ? lo : nullptr; };
   for (int i = 1; i < 10; ++i) {
     const LayerSpec &s = kLayers[i];
-    pack_conv_fwd_kernel<<<dim3(s.Cout, cdiv(s.Cin, 64)), 256, 0, st>>>(M + ts->off[i].w, s.Cout, s.Cin, s.k, ns->w_hi[i],
-                                                                          with_lo ? ns->w_lo[i] : nullptr);
-    DIM_LAUNCH_CHECK();
     DgradPackDst d{{ts->dg_pack[i][0], ts->dg_pack[i][1], ts->dg_pack[i][2], ts->dg_pack[i][3]},
                    {L(ts->dg_pack_lo[i][0]), L(ts->dg_pack_lo[i][1]), L(ts->dg_pack_lo[i][2]), L(ts->dg_pack_lo[i][3])}};
     pack_dgrad_kernel<<<dim3(s.Cin, s.Cout / 64), 256, 0, st>>>(M + ts->off[i].w, s.Cout, s.Cin, s.k, s.stride, d);
     DIM_LAUNCH_CHECK();
   }
-  LAUNCH1D(pack_fc6_kernel, (size_t)256 * 81920, st, M + ts->off[P_FC6].w, ns->fc6_w_hi, with_lo ? ns->fc6_w_lo : nullptr);
-  ns->lo_stale = !with_lo;
-  ns->f16_stale = true;  // the fp16 packs of DIM_PREC_FP16 are re-derived from hi/lo when that mode next runs
-  LAUNCH1D(transpose256_kernel, 65536, st, M + ts->off[P_FC7].w, ns->fc7_wT);
   {
     DgradPackDst d5{{ts->d5_fwd[0], ts->d5_fwd[1], ts->d5_fwd[2], ts->d5_fwd[3]},
                     {L(ts->d5_fwd_lo[0]), L(ts->d5_fwd_lo[1]), L(ts->d5_fwd_lo[2]), L(ts->d5_fwd_lo[3])}};
@@ -962,11 +905,7 @@ int train_load_params(dim_ctx *ctx, const float *flat_host, size_t n, cudaStream
   NetState *ns = ctx->net;
   DIM_REQUIRE(ts != nullptr, "dim_train_load_params: dim_train_create has not been called");
   DIM_REQUIRE(n == ts->n_params, "dim_train_load_params: wrong parameter count");
-  if (!ns->loaded) {  // allocate the inference-side operand buffers through the regular loader
-    const float *W[14], *Bv[14];
-    for (int i = 0; i < 14; ++i) { W[i] = flat_host + ts->off[i].w; Bv[i] = flat_host + ts->off[i].b; }
-    if (int rc = net_load(ctx, W, Bv)) return rc;
-  }
+  if (int rc = net_alloc_weights(ctx)) return rc;
   DIM_CHECK(cudaMemcpyAsync(ts->master, flat_host, n * sizeof(float), cudaMemcpyHostToDevice, st));
   DIM_CHECK(cudaMemsetAsync(ts->mom, 0, n * sizeof(float), st));
   // fp32 parameters that the kernels read as they are (biases, rot / trans heads) now alias the master vector, so an
@@ -977,6 +916,7 @@ int train_load_params(dim_ctx *ctx, const float *flat_host, size_t n, cudaStream
   ns->rot_w = ts->master + ts->off[P_ROT].w; ns->rot_b = ts->master + ts->off[P_ROT].b;
   ns->trans_w = ts->master + ts->off[P_TRANS].w; ns->trans_b = ts->master + ts->off[P_TRANS].b;
   ns->maps.clear();
+  ns->loaded = true;
   return repack_all(ctx, st, true);
 }
 
@@ -991,7 +931,7 @@ int train_refresh_lo(dim_ctx *ctx, cudaStream_t st) {
 static int alloc_lo(dim_ctx *ctx, TrainState *ts) {
   const int B = ctx->max_batch;
   int rc = 0;
-  Buf *bufs[] = {&ts->act10b, &ts->cat2, &ts->cat3, &ts->dcat2, &ts->dcat3, &ts->dA10p, ts->input_depth ? &ts->s2d64 : &ts->s2d32};
+  Buf *bufs[] = {&ts->act10b, &ts->cat2, &ts->cat3, &ts->dcat2, &ts->dcat3, &ts->dA10p, ctx->net->input_depth ? &ts->s2d64 : &ts->s2d32};
   for (Buf *b : bufs) rc |= dev_alloc(ctx, &b->lo, b->per_image() * B, true);
   for (int i = 0; i < 10; ++i) rc |= dev_alloc(ctx, &ts->gz[i].lo, ts->gz[i].per_image() * B, true);
   for (int i = 1; i < 10; ++i) {
@@ -1269,9 +1209,9 @@ static int launch_wgrad_conv1(const WgradParams &p, cudaStream_t st) {
   DIM_LAUNCH_CHECK();
   return 0;
 }
-static int run_wgrad_conv1(TrainState *ts, const WgradParams &p16, int sms, float *grad, cudaStream_t st) {
+static int run_wgrad_conv1(dim_ctx *ctx, TrainState *ts, const WgradParams &p16, float *grad, cudaStream_t st) {
   WgradParams p = p16;
-  int ks = cdiv(2 * sms, 4);
+  int ks = cdiv(2 * ctx->num_sms, 4);
   if (ks > p.kb_total / 2) ks = p.kb_total / 2;
   if (ks < 1) ks = 1;
   p.kb_per_slice = cdiv(p.kb_total, ks);
@@ -1281,7 +1221,7 @@ static int run_wgrad_conv1(TrainState *ts, const WgradParams &p16, int sms, floa
   const size_t total = (size_t)4 * 128 * 64;
   // the image-only network's gradient is (64, 6, 7, 7): D1 = 6 drops the rows of the zero mask lanes
   wgrad_reduce_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(p.partial, p.kslices, 4, 128, 64, WG_CONV1_ROW, 64,
-                                                                       ts->input_mask ? 8 : 6, 7, grad);
+                                                                       ctx->net->input_mask ? 8 : 6, 7, grad);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -1394,7 +1334,7 @@ static int build_train_maps(dim_ctx *ctx, int B, TrainMaps &tm) {
   // weight gradients
   for (int i = 0; i < 10; ++i) {
     const LayerSpec &s = kLayers[i];
-    if (i == 0 && ts->input_depth) {  // generic kernel over the 16 taps of the NHWC-64 copy (SW128 boxes), WG_CONV1_RGBD reduce
+    if (i == 0 && ns->input_depth) {  // generic kernel over the 16 taps of the NHWC-64 copy (SW128 boxes), WG_CONV1_RGBD reduce
       if (int rc = make_wgrad(ts, tm.wg[0], tm.wg_bn[0], B, ts->gz[0], 0, 64, ns->g[0].Ho, ns->g[0].Wo, ts->s2d64, 0, 64, 1, 4, 4, 0, 0, sms))
         return rc;
     } else if (i == 0) {
@@ -1485,13 +1425,13 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
   // ---------------- forward
   DimNvtxRange r_fwd("dim_train forward + losses");
   DIM_CHECK(cudaEventRecord(ts->ev_phase[0], st));
-  DIM_REQUIRE((io.zdo && io.zdr) == ts->input_depth && (io.zdo == nullptr) == (io.zdr == nullptr),
+  DIM_REQUIRE((io.zdo && io.zdr) == ns->input_depth && (io.zdo == nullptr) == (io.zdr == nullptr),
               "dim_train_forward_backward: the RGB-D network takes both zoomed depths, the RGB network none");
-  if (ts->input_depth) {
+  if (ns->input_depth) {
     if (int rc = pack_nhwc10_launch(ctx, io.zio, io.zir, io.zdo, io.zdr, io.zmo, io.zmr, B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0],
                                     s3 ? ns->act_lo[0] : nullptr, st, 0))
       return rc;
-  } else if (int rc = pack_nhwc8_launch(ctx, io.zio, io.zir, ts->input_mask ? io.zmo : nullptr, ts->input_mask ? io.zmr : nullptr,
+  } else if (int rc = pack_nhwc8_launch(ctx, io.zio, io.zir, ns->input_mask ? io.zmo : nullptr, ns->input_mask ? io.zmr : nullptr,
                                         B, g[0].rows, g[0].cols, g[0].py, ns->act_hi[0],
                                         s3 ? ns->act_lo[0] : nullptr, st, 0)) {
     return rc;
@@ -1616,7 +1556,7 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
   if (int rc = run_generic(ctx, tm.deconv5_dgrad, tm.g_deconv5_dgrad, B, st, s3)) return rc;
   DIM_CHECK(cudaEventRecord(ts->ev_phase[5], st));
   // encoder
-  if (ts->input_depth)
+  if (ns->input_depth)
     LAUNCH1D((s3 ? strip_to_nhwc64_kernel<true> : strip_to_nhwc64_kernel<false>), (size_t)B * g[0].rows * 8 * g[0].cols, st, ns->act_hi[0],
              ns->act_lo[0], ts->s2d64.p, ts->s2d64.lo, (size_t)B * g[0].rows * 8 * g[0].cols, g[0].cols);
   else
@@ -1628,10 +1568,10 @@ int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st) {
     if (i == 9)  // heads, decoder (thin kernels on st, deconvolution wgrads on sw): tensors 10..23 are done
       if (int rc = record_buckets(io, 10, 1 << 30, sw)) return rc;
     if (int rc = bias_grad(ts, ts->gz[i], B, 0, s.Cout, G + ts->off[i].b, sw)) return rc;
-    if (i == 0 && ts->input_depth) {
+    if (i == 0 && ns->input_depth) {
       if (int rc = run_wgrad(tm.wg[0], tm.wg_bn[0], s3, WG_CONV1_RGBD, 64, 10, 7, G + ts->off[0].w, sw)) return rc;
     } else if (i == 0) {
-      if (int rc = run_wgrad_conv1(ts, tm.wg[0], ctx->num_sms, G + ts->off[0].w, sw)) return rc;
+      if (int rc = run_wgrad_conv1(ctx, ts, tm.wg[0], G + ts->off[0].w, sw)) return rc;
     } else if (int rc = run_wgrad(tm.wg[i], tm.wg_bn[i], s3, WG_CONV, s.Cout, s.Cin, s.k, G + ts->off[i].w, sw)) return rc;
     if (int rc = record_buckets(io, i, i + 1, sw)) return rc;
     if (i >= 1)
