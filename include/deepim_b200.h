@@ -382,6 +382,41 @@ DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int3
                                        const double *pixel_means_rgb_host, float *image,
                                        void *stream);
 
+/* Train-time augmentation of the observed inputs (the shipped training config: LM6D_REFINE + LM6D_REFINE_SYN, MASK_DILATE).
+ * The caller supplies every random draw (deepim_b200/augment.py draws them in the reference's order).
+ *
+ * Background bank: BGR u8 photos [h,w,3] of any size (h, w in [1, 16384]), uploaded once per context like meshes.
+ *   Capacity: indices 0 .. DIM_BG_MAX-1; each dim_bg_upload allocates h*w*3 bytes of device memory, held until the context
+ *   is destroyed; uploading to an index already used replaces its photo (frees the old one; synchronises the device).
+ *   A photo whose resized crop (below) does not fit the context's H x W canvas is refused at upload.
+ * dim_bg_geometry: host only, no context -- the crop and resize of image.py:108-145 + resize (image.py:552-572) in float64:
+ *   out4 = crop_h, crop_w, dst_h, dst_w; *scale = cv2.resize's fx = fy.  The crop is the photo's top-left crop_h x crop_w
+ *   (its H:W aspect), resized to dst_h x dst_w and placed at the canvas's top-left corner, black elsewhere.  A crop scaled
+ *   by exactly 1/2 with an odd side is refused (cv2 takes its INTER_AREA border path there, not reproduced).
+ * dim_replace_background (image.py:96-157): per instance b,
+ *   composite[b] = mask[b] != 0 ? observed_bgr[b] : background;  image_observed[b] = transform(composite[b])
+ *   with transform the float64 mean subtraction of dim_transform_image_u8.
+ *   observed_bgr f32 [B,H,W,3] BGR in [0,255] as dim_render's out_bgr writes it: that is the observed image the device
+ *     pipeline already has, so no conversion pass is needed; values are clamped to [0,255] and truncated to u8 as numpy's
+ *     store into the reference's uint8 canvas does (dim_render's truncating renders are whole numbers already);
+ *   mask f32 [B,1,H,W] (mask_gt_observed; != 0 keeps the observed pixel);
+ *   bg_index_host HOST i32 [B]: bank index, or -1 = keep the observed image (image_observed = transform(observed));
+ *   image_observed f32 [B,3,H,W] RGB - means; composite_u8 u8 [B,H,W,3] BGR (nullable).
+ *   The bilinear resize is OpenCV 4.x INTER_LINEAR on 8-bit images, bit for bit (pinned against cv2 4.13; augment.cu).
+ *   Refused: B outside [1, max_batch], an index >= 0 that names no uploaded photo (or any index >= 0 on an empty bank).
+ * dim_mask_dilate (lib/utils/mask_dilate.py:19-47): mask_in / mask_out f32 [B,1,H,W]; draws DEVICE i32 [B,5] = direction,
+ *   then the thickness of the down, up, right and left shift (<= 0: that side is skipped).  Each shift tests the ORIGINAL
+ *   mask, so a box grows into a cross; nonzero inputs stay as they are except values > 1, which become 1.  In place
+ *   (mask_in == mask_out) is refused. */
+#define DIM_BG_MAX 65536
+DIM_API int32_t dim_bg_upload(dim_ctx *ctx, int32_t idx, const uint8_t *bgr_u8_host, int32_t h, int32_t w);
+DIM_API int32_t dim_bg_geometry(int32_t H, int32_t W, int32_t bh, int32_t bw, int32_t *out4, double *scale);
+DIM_API int32_t dim_replace_background(dim_ctx *ctx, const float *observed_bgr, const float *mask,
+                                       const int32_t *bg_index_host, int32_t B, const double *pixel_means_rgb_host,
+                                       float *image_observed, uint8_t *composite_u8, void *stream);
+DIM_API int32_t dim_mask_dilate(dim_ctx *ctx, const float *mask_in, const int32_t *draws, int32_t B, float *mask_out,
+                                void *stream);
+
 /* Test hooks (not part of the drop-in surface): copy the bf16 NHWC activation buffer feeding conv
  * layer idx (10 = fc6 input) to the host, and its geometry
  * out8 = rows, cols, C, py, px, Ho, Wo, Cout. */

@@ -20,6 +20,7 @@ UNITS = {
     "raster.cu": ["-fmad=false"],
     "zoom.cu": ["-fmad=false"],
     "geom.cu": ["-fmad=false"],
+    "augment.cu": ["-fmad=false"],
     "net.cu": [],
     "train.cu": [],
     "capi.cu": [],

@@ -106,6 +106,7 @@ DIM_API void dim_ctx_destroy(dim_ctx *ctx) {
   for (auto &g : ctx->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   for (cudaEvent_t e : ctx->prof_events) cudaEventDestroy(e);
   for (void *p : ctx->owned) cudaFree(p);
+  for (auto &e : ctx->bg) if (e.data) cudaFree(e.data);
   delete ctx;
 }
 
@@ -374,6 +375,90 @@ DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr, int32_t
                                        void *stream) {
   DIM_REQUIRE(ctx && bgr && means && image, "dim_transform_image_u8: NULL argument");
   return transform_u8_launch(ctx, bgr, B, means, image, (cudaStream_t)stream);
+}
+
+// train-time augmentation of the observed inputs (augment.cu)
+DIM_API int32_t dim_bg_upload(dim_ctx *ctx, int32_t idx, const uint8_t *bgr, int32_t h, int32_t w) {
+  DIM_REQUIRE(ctx && bgr, "dim_bg_upload: NULL argument");
+  DIM_REQUIRE(idx >= 0 && idx < DIM_BG_MAX, "dim_bg_upload: bank index outside [0, DIM_BG_MAX)");
+  DIM_REQUIRE(h >= 1 && w >= 1 && h <= 16384 && w <= 16384, "dim_bg_upload: image size outside [1, 16384]");
+  BgGeom g;
+  if (int rc = bg_geometry(ctx->H, ctx->W, h, w, &g)) return rc;
+  if ((size_t)idx >= ctx->bg.size()) ctx->bg.resize(idx + 1);
+  dim_ctx::BgImage &e = ctx->bg[idx];
+  if (e.data) {  // replacing a photo: cudaFree waits for the device, so no enqueued replacement still reads it
+    DIM_CHECK(cudaFree(e.data));
+    e = dim_ctx::BgImage();
+  }
+  uint8_t *d = nullptr;
+  DIM_CHECK(cudaMalloc(&d, (size_t)h * w * 3));
+  e.data = d; e.h = h; e.w = w;
+  DIM_CHECK(cudaMemcpy(d, bgr, (size_t)h * w * 3, cudaMemcpyHostToDevice));
+  return 0;
+}
+
+DIM_API int32_t dim_bg_geometry(int32_t H, int32_t W, int32_t bh, int32_t bw, int32_t *out4, double *scale) {
+  DIM_REQUIRE(out4 && scale, "dim_bg_geometry: NULL argument");
+  DIM_REQUIRE(H >= 1 && W >= 1 && bh >= 1 && bw >= 1, "dim_bg_geometry: bad sizes");
+  BgGeom g;
+  if (int rc = bg_geometry(H, W, bh, bw, &g)) return rc;
+  out4[0] = g.crop_h; out4[1] = g.crop_w; out4[2] = g.dst_h; out4[3] = g.dst_w;
+  *scale = g.scale;
+  return 0;
+}
+
+DIM_API int32_t dim_replace_background(dim_ctx *ctx, const float *observed_bgr, const float *mask,
+                                       const int32_t *bg_index_host, int32_t B, const double *means,
+                                       float *image_observed, uint8_t *composite_u8, void *stream) {
+  DIM_REQUIRE(ctx && observed_bgr && mask && bg_index_host && means && image_observed,
+              "dim_replace_background: NULL argument");
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_replace_background: B outside [1, max_batch]");
+  BgLaunch L;
+  memset(&L, 0, sizeof(L));
+  for (int k = 0; k < 3; ++k) L.mean[k] = means[k];
+  for (int b0 = 0; b0 < B; b0 += BG_LAUNCH_MAX) {  // validate every index before the first launch
+    const int nb = B - b0 < BG_LAUNCH_MAX ? B - b0 : BG_LAUNCH_MAX;
+    for (int i = 0; i < nb; ++i) {
+      const int idx = bg_index_host[b0 + i];
+      if (idx < 0) continue;
+      if (ctx->bg.empty()) {
+        set_error("dim_replace_background: instance %d names photo %d but the background bank is empty", b0 + i, idx);
+        return 2;
+      }
+      if ((size_t)idx >= ctx->bg.size() || !ctx->bg[idx].data) {
+        set_error("dim_replace_background: instance %d names photo %d, which was not uploaded", b0 + i, idx);
+        return 2;
+      }
+      BgGeom g;
+      if (int rc = bg_geometry(ctx->H, ctx->W, ctx->bg[idx].h, ctx->bg[idx].w, &g)) return rc;
+    }
+  }
+  for (int b0 = 0; b0 < B; b0 += BG_LAUNCH_MAX) {
+    const int nb = B - b0 < BG_LAUNCH_MAX ? B - b0 : BG_LAUNCH_MAX;
+    L.b0 = b0;
+    for (int i = 0; i < nb; ++i) {
+      BgInst &in = L.inst[i];
+      in = BgInst{};
+      const int idx = bg_index_host[b0 + i];
+      if (idx < 0) continue;
+      const dim_ctx::BgImage &e = ctx->bg[idx];
+      BgGeom g;
+      bg_geometry(ctx->H, ctx->W, e.h, e.w, &g);
+      in.data = e.data; in.inv_scale = 1.0 / g.scale; in.stride = e.w;
+      in.crop_h = g.crop_h; in.crop_w = g.crop_w; in.dst_h = g.dst_h; in.dst_w = g.dst_w;
+    }
+    if (int rc = replace_bg_launch(ctx, L, nb, observed_bgr, mask, image_observed, composite_u8, (cudaStream_t)stream))
+      return rc;
+  }
+  return 0;
+}
+
+DIM_API int32_t dim_mask_dilate(dim_ctx *ctx, const float *mask_in, const int32_t *draws, int32_t B, float *mask_out,
+                                void *stream) {
+  DIM_REQUIRE(ctx && mask_in && draws && mask_out, "dim_mask_dilate: NULL argument");
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_mask_dilate: B outside [1, max_batch]");
+  DIM_REQUIRE(mask_in != mask_out, "dim_mask_dilate: in place (mask_in == mask_out) is not supported");
+  return mask_dilate_launch(ctx, mask_in, draws, B, mask_out, (cudaStream_t)stream);
 }
 
 static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {

@@ -128,6 +128,9 @@ struct dim_ctx {
   float *lit_intensity = nullptr;  // [8, max_batch, 3] dim_refine_host_lit: the caller's light intensities on the device
   uint16_t *depth_u16 = nullptr;   // [max_batch,H,W] dim_refine_host_rgbd: the caller's depth file values (RGB-D contexts)
   int *bbox_obs = nullptr;         // [max_batch,4] image-only network: the observed image's colour-valid box (ZoomImage)
+  // background bank of dim_replace_background (dim_bg_upload): BGR u8 photos, each allocated at its upload
+  struct BgImage { uint8_t *data = nullptr; int h = 0, w = 0; };
+  std::vector<BgImage> bg;
   dim::NetState *net = nullptr;
   // CUDA graphs of the fused refinement chain (capi.cu refine_graphed): one executable graph per distinct argument set
   struct RefineGraph {

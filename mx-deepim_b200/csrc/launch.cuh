@@ -78,6 +78,20 @@ int pose_error2d_launch(const double *pose_est, const double *pose_gt, int M, co
 int pose_error_launch(const double *pose_est, const double *pose_gt, int M, const double *pts, int N, int symmetric,
                       double *out, cudaStream_t st);
 
+// augment.cu
+struct BgGeom { int crop_h, crop_w, dst_h, dst_w; double scale; };  // scale = cv2.resize's fx = fy
+struct BgInst {  // one instance of dim_replace_background; data == nullptr keeps the observed image
+  const uint8_t *data;  // the bank photo, BGR u8 [h, stride, 3]; the crop is its top-left crop_h x crop_w
+  double inv_scale;     // 1 / scale
+  int stride, crop_h, crop_w, dst_h, dst_w, pad;
+};
+constexpr int BG_LAUNCH_MAX = 32;  // instances per launch (the per-instance table travels as a kernel argument)
+struct BgLaunch { BgInst inst[BG_LAUNCH_MAX]; double mean[3]; int b0, pad; };
+int bg_geometry(int H, int W, int bh, int bw, BgGeom *g);
+int replace_bg_launch(dim_ctx *ctx, const BgLaunch &L, int nb, const float *obs, const float *mask, float *image,
+                      uint8_t *comp, cudaStream_t st);
+int mask_dilate_launch(dim_ctx *ctx, const float *in, const int *draws, int B, float *out, cudaStream_t st);
+
 // net.cu
 int net_create(dim_ctx *ctx);
 void net_destroy(dim_ctx *ctx);

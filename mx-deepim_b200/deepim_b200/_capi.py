@@ -78,6 +78,10 @@ SIGNATURES = {
     "dim_ctx_set_input_mask": (i32, [vp, i32]),
     "dim_train_param_info_nomask": (i32, [i32, C.POINTER(C.c_char_p), C.POINTER(i64), C.POINTER(i64)]),
     "dim_transform_image_u8": (i32, [vp, vp, i32, pf64, vp, vp]),
+    "dim_bg_upload": (i32, [vp, i32, vp, i32, i32]),
+    "dim_bg_geometry": (i32, [i32, i32, i32, i32, C.POINTER(i32), pf64]),
+    "dim_replace_background": (i32, [vp, vp, vp, vp, i32, pf64, vp, vp, vp]),
+    "dim_mask_dilate": (i32, [vp, vp, vp, i32, vp, vp]),
     "dim_debug_activation": (i32, [vp, i32, i32, vp, u64]),
     "dim_debug_layer_geometry": (i32, [vp, i32, C.POINTER(i32)]),
     "dim_refine_status": (i32, [vp, i32, i32, vp, vp]),

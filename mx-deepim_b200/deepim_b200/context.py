@@ -364,6 +364,36 @@ class Context:
         check(lib.dim_transform_image_u8(self._h, _p(bgr_u8), B, farr(pixel_means_rgb, 3, C.c_double), _p(out), self._stream()))
         return out
 
+    # -------------------------------------------------------------------------- augmentation
+    def replace_background(self, observed_bgr, mask, bg_index, pixel_means_rgb, want_composite=False):
+        """dim_replace_background (image.py:96-157): observed_bgr float32 [B,H,W,3] BGR in [0,255] (render's "bgr"),
+        mask float32 [B,1,H,W] (!= 0 keeps the observed pixel), bg_index host int32 [B] photo of the context's background
+        bank (deepim_b200.augment.BackgroundBank) or -1 = keep.  Returns image_observed float32 [B,3,H,W] (RGB - means),
+        and with want_composite also the uint8 BGR composite [B,H,W,3]."""
+        B = observed_bgr.shape[0]
+        _chk(observed_bgr, torch.float32, (B, self.H, self.W, 3), "observed_bgr")
+        _chk(mask, torch.float32, (B, 1, self.H, self.W), "mask")
+        idx = np.ascontiguousarray(bg_index, np.int32)
+        if idx.shape != (B,):
+            raise ValueError("bg_index: expected shape (%d,), got %s" % (B, idx.shape))
+        out = self._new((B, 3, self.H, self.W))
+        comp = self._new((B, self.H, self.W, 3), torch.uint8) if want_composite else None
+        check(lib.dim_replace_background(self._h, _p(observed_bgr), _p(mask), idx.ctypes.data, B,
+                                         farr(pixel_means_rgb, 3, C.c_double), _p(out), _p(comp), self._stream()))
+        return (out, comp) if want_composite else out
+
+    def mask_dilate(self, mask, draws):
+        """dim_mask_dilate (mask_dilate.py:19-47): mask float32 [B,1,H,W]; draws int32 [B,5] (host or CUDA; see
+        deepim_b200.augment.mask_dilate_draws).  Returns the dilated mask (a new tensor)."""
+        B = mask.shape[0]
+        _chk(mask, torch.float32, (B, 1, self.H, self.W), "mask")
+        d = torch.as_tensor(np.asarray(draws, np.int32) if not isinstance(draws, torch.Tensor) else draws)
+        d = d.to(self.device).contiguous()
+        _chk(d, torch.int32, (B, 5), "draws")
+        out = self._new(mask.shape)
+        check(lib.dim_mask_dilate(self._h, _p(mask), _p(d), B, _p(out), self._stream()))
+        return out
+
     # --------------------------------------------------------------------------------- net
     def net_forward(self, zoom_image_observed, zoom_image_rendered, zoom_mask_observed=None, zoom_mask_rendered=None,
                     precision=capi.PREC_BF16X3, zoom_depth_observed=None, zoom_depth_rendered=None):

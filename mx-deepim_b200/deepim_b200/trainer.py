@@ -304,7 +304,7 @@ class Trainer:
 
 
 def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000, init_mask="box_gt", poses=None,
-                      image_observed=None, cls_np=None, lighting=None, input_depth=False):
+                      image_observed=None, cls_np=None, lighting=None, input_depth=False, background=None, mask_dilate=None):
     """Synthetic training batch built with the device kernels only (config C4: rendered pairs, labels from
     dim_train_update, INIT_MASK box_gt without dilation, 3000 sampled model points as get_point_cloud_model,
     lib/utils/image.py:452-478).  init_mask = "box_gt" (the reference's training config: mask_observed = box of the GT mask)
@@ -316,8 +316,15 @@ def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000,
     each with a fresh intensity draw.
     input_depth = True adds the RGB-D network's blobs: depth_observed = the observed render's depth, depth_rendered = the
     update's render depth (refined_depth_array, batch_updater_py_multi.py:269).
+    background = (augment.BackgroundBank, draws): the observed images are synthetic (data_syn), so each gets the background
+    photo the draws name (int32 [B] bank indices, -1 = keep; an int instead of an array seeds
+    augment.background_draws(B, RandomState(seed), len(bank))), composited under the GT mask (image.py:96-157).
+    mask_dilate = a np.random.RandomState or an int seed: mask_observed is dilated after the box is formed with
+    augment.mask_dilate_draws (TRAIN.MASK_DILATE, image.py:289-290).  Both stay fixed across fit_batch's inner iterations.
     Returns (batch dict of CUDA tensors, cls int32[B], tgt_pose f32[B,3,4], depth_gt)."""
-    from . import synth
+    from . import augment, synth
+    if background is not None and image_observed is not None:
+        raise ValueError("make_device_batch: background replaces the rendered observed image; image_observed would ignore it")
     obs, ini = synth.sample_pose_pairs(B, seed) if poses is None else poses
     dev = ctx.device
     cls_np = (np.arange(B) % len(meshes)).astype(np.int32) if cls_np is None else np.asarray(cls_np, np.int32)
@@ -325,12 +332,18 @@ def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000,
     tgt = torch.from_numpy(obs.astype(np.float32)).to(dev)
     src = torch.from_numpy(ini.astype(np.float32)).to(dev)
     light = _lighting.LightSource.of(lighting)
+    want = ("image", "depth", "mask") + (("bgr",) if background is not None else ())
     if light is None:
-        r = ctx.render(cls, tgt, K, pixel_means_rgb=pixel_means_rgb, trunc_u8=True)
+        r = ctx.render(cls, tgt, K, pixel_means_rgb=pixel_means_rgb, trunc_u8=True, want=want)
     else:
         lp = torch.from_numpy(_lighting.modelnet_light_position(obs)).to(dev)
         r = ctx.render_lit(cls, tgt, K, lp, torch.from_numpy(light.draw(B)).to(dev), light.brightness_ratio,
-                           pixel_means_rgb=pixel_means_rgb, want=("image", "depth", "mask"))
+                           pixel_means_rgb=pixel_means_rgb, want=want)
+    if background is not None:
+        bank, draws = background
+        if np.ndim(draws) == 0:
+            draws = augment.background_draws(B, np.random.RandomState(int(draws)), len(bank))
+        image_observed = ctx.replace_background(r["bgr"], r["mask"], draws, pixel_means_rgb)
     ident = torch.tensor([[1.0, 0, 0, 0]] * B, dtype=torch.float32, device=dev)
     upd = ctx.train_update(cls, src, ident, torch.zeros(B, 3, device=dev), tgt, r["depth"], K, pixel_means_rgb=pixel_means_rgb,
                            lighting=_device_lighting(light, B, dev))
@@ -343,7 +356,11 @@ def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000,
         pw[b, :, :len(keep)] = 1
     pobs = np.stack([obs[b, :, :3].astype(np.float32) @ pts[b] + obs[b, :, 3:4].astype(np.float32) for b in range(B)]).astype(np.float32)
     box = r["bbox"] if init_mask == "box_gt" else ctx.render(cls, upd["src_pose"], K, pixel_means_rgb=pixel_means_rgb, want=("mask",))["bbox"]
-    batch = {"image_observed": r["image"] if image_observed is None else image_observed, "image_rendered": upd["image_rendered"], "mask_observed": ctx.update_mask_box(box),
+    mask_observed = ctx.update_mask_box(box)
+    if mask_dilate is not None:
+        rs = mask_dilate if isinstance(mask_dilate, np.random.RandomState) else np.random.RandomState(int(mask_dilate))
+        mask_observed = ctx.mask_dilate(mask_observed, augment.mask_dilate_draws(B, rs))
+    batch = {"image_observed": r["image"] if image_observed is None else image_observed, "image_rendered": upd["image_rendered"], "mask_observed": mask_observed,
              "mask_gt_observed": r["mask"], "mask_rendered": upd["mask_rendered"], "src_pose": upd["src_pose"], "flow": upd["flow"],
              "flow_weights": upd["flow_weights"], "point_cloud_model": torch.from_numpy(pts).to(dev),
              "point_cloud_weights": torch.from_numpy(pw).to(dev), "point_cloud_observed": torch.from_numpy(pobs).to(dev),
