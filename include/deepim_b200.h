@@ -33,7 +33,7 @@ extern "C" {
 
 typedef struct dim_ctx dim_ctx;
 
-#define DIM_ABI_VERSION 2
+#define DIM_ABI_VERSION 3
 DIM_API int32_t dim_abi_version(void);
 DIM_API const char *dim_last_error(void);
 
@@ -175,6 +175,26 @@ DIM_API int32_t dim_transform3d_bwd(dim_ctx *ctx, const float *out_grad, const f
                                     int32_t rot_coord, float *rot_grad, float *trans_grad,
                                     void *stream);
 
+/* Lighting of the ModelNet / unseen-object configuration (config.dataset.dataset "ModelNet*": deepim/core/tester.py:114-133,
+ * 146-185; lib/pair_matching/batch_updater_py_multi.py:35-52,187-229).  The `lighting` argument of dim_train_update,
+ * dim_refine and dim_refine_host(_async): NULL = the unlit renderer; otherwise every render of the call is the Lambert-lit
+ * renderer of dim_render_lit.  The light follows the pose being rendered: in the GL camera frame
+ *   light_position = float32(offset[0] + t_x, offset[1] - t_y, offset[2] - t_z)
+ * computed from the float64 pose (the reference's hard-coded light index 2 gives offset = (0, 0.5, 0.5)).  The reference
+ * draws light_intensity from U(0.9, 1.1)^3 afresh for every render; here the caller supplies the draws.
+ *   intensity (non-NULL): device f32 [n_iter,B,3] for dim_refine (iteration it renders with intensity[it]), [B,3] for
+ *              dim_train_update, HOST f32 [n_iter,B,3] for dim_refine_host(_async) (n_iter <= 8; copied to the
+ *              context on `stream` before the call returns, so a pageable buffer may be reused at once).
+ *   brightness_ratio: colour = texel * ((1 - ratio) + ratio * brightness) * intensity (the reference: 0.7).
+ * Depth, masks, bboxes, zoom, labels and flow are those of the unlit calls; only the colours change.  Every uploaded mesh
+ * must have normals (dim_mesh_upload_normals).  Lit loops share dim_refine_status and are captured / replayed as CUDA
+ * graphs like unlit ones. */
+typedef struct dim_lighting {
+  const float *intensity; /* see above: device [n_iter,B,3] (refine) / [B,3] (train update); host for dim_refine_host */
+  double offset[3];       /* light at zero translation, GL frame; the reference: (0, 0.5, 0.5) */
+  float brightness_ratio; /* the reference: 0.7 */
+} dim_lighting;
+
 /* Train-time inter-iteration update (lib/pair_matching/batch_updater_py_multi.py:91-328,
  * batchUpdaterPyMulti.forward): compose the predicted delta onto src_pose, re-render WITHOUT uint8
  * truncation (float32 image - float32 means, l.184,234), recompute the labels rot (quaternion of
@@ -185,7 +205,9 @@ DIM_API int32_t dim_transform3d_bwd(dim_ctx *ctx, const float *out_grad, const f
  *        pixel_means_rgb host f64
  *   out: image_rendered f32[B,3,H,W], depth_rendered/mask_rendered f32[B,1,H,W], src_pose_new f32[B,3,4],
  *        rot_label f32[B,4], trans_label f32[B,3], flow f32[B,2,H,W], flow_weights f32[B,2,H,W]
- *        (flow, flow_weights may be NULL together). */
+ *        (flow, flow_weights may be NULL together).
+ *   lighting (nullable, see dim_lighting): the ModelNet re-render (l.187-235); the light follows the float64 refined pose,
+ *        image_rendered = float32 quantised lit colours - float32 means; every other output is the unlit one. */
 DIM_API int32_t dim_train_update(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose,
                                  const float *rot_est, const float *trans_est, const float *tgt_pose,
                                  const float *depth_gt_observed, int32_t B, const double *K9_host,
@@ -193,7 +215,41 @@ DIM_API int32_t dim_train_update(dim_ctx *ctx, const int32_t *cls_idx, const flo
                                  const double *T_means_host, const double *T_stds_host,
                                  int32_t rot_coord, float *image_rendered, float *depth_rendered,
                                  float *mask_rendered, float *src_pose_new, float *rot_label,
-                                 float *trans_label, float *flow, float *flow_weights, void *stream);
+                                 float *trans_label, float *flow, float *flow_weights,
+                                 const dim_lighting *lighting, void *stream);
+
+/* Network variants.  A context runs one of three networks, chosen before dim_net_load / dim_train_create (either switch
+ * is an error afterwards); a context that never switches runs the mask network.
+ *   - mask network (INPUT_MASK on): conv1 sees concat(image_observed/255, image_rendered/255, mask_observed,
+ *     mask_rendered), flow_conv1_weight (64, 8, 7, 7).
+ *   - RGB-D network (config.network.INPUT_DEPTH: deepIM_flownet.py:33-51, tester.py:437-438), dim_ctx_set_input_depth(ctx,
+ *     1): the input gains two channels, in the order image_observed/255, image_rendered/255, depth_observed/255,
+ *     depth_rendered/255, mask_observed, mask_rendered, so flow_conv1_weight is (64, 10, 7, 7).  The depths are metres,
+ *     divided by 255 as the reference does; depth_rendered is each iteration's render depth (0 = background), zoomed with
+ *     the iteration's zoom factor like every other input (ZoomDepth, zoom_depth.py:24-44).
+ *   - image-only network (config.network.INPUT_MASK: False, the reference's default; deepIM_flownet.py:53-62,
+ *     tester.py:439), dim_ctx_set_input_mask(ctx, 0): conv1 sees concat(image_observed/255, image_rendered/255), so
+ *     flow_conv1_weight is (64, 6, 7, 7), and the test graph zooms with ZoomImage (zoom_image.py:26-107, the boxes of
+ *     sum_c(image + mean) > 0.01) instead of ZoomMask + ZoomImageWithFactor.
+ * dim_ctx_set_input_depth: enable = 1 switches to the RGB-D network, 0 back.  dim_ctx_set_input_mask: enable = 0 switches
+ * to the image-only network, 1 back.  Depth input without the mask channels (INPUT_DEPTH without INPUT_MASK) is not
+ * supported: each switch refuses it.
+ * Every entry point follows the context's network, with these rules:
+ *   - depth inputs (depth_observed of dim_refine, depth_observed_u16_host of dim_refine_host(_async), zoom_depth_* of
+ *     dim_net_fwd and dim_train_forward_backward) are non-NULL exactly on an RGB-D context; otherwise the call fails with a
+ *     message naming the argument and dim_ctx_set_input_depth;
+ *   - mask inputs (zoom_mask_* of dim_net_fwd and dim_train_forward_backward) are NULL exactly on an image-only context;
+ *   - dim_net_load takes the network's flow_conv1 weight; the flat training vector is the network's table
+ *     (dim_train_param_info) and dim_train_param_count reports its size.
+ * On an image-only context dim_refine / dim_refine_host(_async) run the image-only chain: the observed box is computed once
+ * per call, the rendered box of every iteration from the render's colours; the zoom factor is ZoomImage's (ZoomMask's
+ * arithmetic with the observed-centre fallback for an empty render).  dim_refine_status: bit 0 = the observed image has no
+ * valid pixel (the reference raises; the fallback factor (1,1,0,0) was used), bit 2 = the rendered image has none (the
+ * zoom centres on the observed box, as the reference does), bit 1 unchanged.  dim_train_update is the same for every
+ * network: with PRED_MASK the reference's training graph still zooms with ZoomMask and learns the mask; only the network
+ * input loses the mask channels. */
+DIM_API int32_t dim_ctx_set_input_depth(dim_ctx *ctx, int32_t enable);
+DIM_API int32_t dim_ctx_set_input_mask(dim_ctx *ctx, int32_t enable);
 
 /* FlowNetS weights (deepim/symbols/deepIM_flownet.py:63-116,716-717; MXNet layouts: Convolution
  * (Cout,Cin,kh,kw), FullyConnected (out,in)).  Host float32 pointers, 14 (weight,bias) pairs in the
@@ -209,10 +265,11 @@ DIM_API int32_t dim_net_load(dim_ctx *ctx, const float *const *weights_host,
                              the single-pass mode that meets the 1e-4 rot / 1e-3 trans se3 tolerance (headline mode) */
 
 /* Encoder + fc + heads on already-zoomed blobs (get_convs, deepIM_flownet.py:53-116; heads
- * l.716-717): inputs f32 NCHW as the op surface produces them; rot f32[B,4] raw quaternion,
- * trans f32[B,3] zoomed translation. */
+ * l.716-717): inputs f32 NCHW as the op surface produces them (zoomed depths f32 [B,1,H,W] in metres, zoomed masks
+ * f32 [B,1,H,W]; NULL as the network variant says); rot f32[B,4] raw quaternion, trans f32[B,3] zoomed translation. */
 DIM_API int32_t dim_net_fwd(dim_ctx *ctx, const float *zoom_image_observed,
-                            const float *zoom_image_rendered, const float *zoom_mask_observed,
+                            const float *zoom_image_rendered, const float *zoom_depth_observed,
+                            const float *zoom_depth_rendered, const float *zoom_mask_observed,
                             const float *zoom_mask_rendered, int32_t B, int32_t precision,
                             float *rot, float *trans, void *stream);
 
@@ -224,24 +281,34 @@ DIM_API int32_t dim_net_fwd(dim_ctx *ctx, const float *zoom_image_observed,
  *   outputs (device): poses f64[n_iter,B,3,4], se3 f32[n_iter,B,7], zoom_factor f32[n_iter,B,4],
  *   bbox i32[n_iter,B,8]; any of the last three may be NULL.
  *   pose_override f64[n_iter,B,3,4] or NULL: when given, iteration `it` starts from
- *   pose_override[it] instead of the previous estimate (teacher forcing for parity tests). */
+ *   pose_override[it] instead of the previous estimate (teacher forcing for parity tests).
+ *   depth_observed: RGB-D network only, f32 [B,1,H,W] in metres (constant over the iterations).
+ *   lighting: nullable, see dim_lighting (device intensity [n_iter,B,3]).
+ * After one eager run of an argument set the chain is captured as a CUDA graph and replayed (keyed on every argument,
+ * the depth and intensity pointers included). */
 DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx,
                            const double *pose_init, int32_t B, int32_t n_iter, const float *K9_host,
                            float znear, float zfar, const double *pixel_means_rgb_host,
                            int32_t precision, const double *pose_override, double *poses,
-                           float *se3, float *zoom_factor, int32_t *bbox, void *stream);
+                           float *se3, float *zoom_factor, int32_t *bbox, const float *depth_observed,
+                           const dim_lighting *lighting, void *stream);
 
 /* Host-buffer convenience around dim_refine (what deepim/core/tester.py:pred_eval would call):
  * image_observed_u8 host u8[B,H,W,3] BGR (as cv2.imread returns; transformed on device as
  * lib/utils/image.py:583-594), cls_idx host, pose_init host f64; poses_out host f64[n_iter,B,3,4].
+ * depth_observed_u16_host: RGB-D network only, the host depth file values u16 [B,H,W], converted on the device as
+ * lib/utils/image.py:203,218 does: float32(u16) / float32(depth_factor) (LINEMOD: 1000; depth_factor is checked only
+ * when a depth is given).  lighting: nullable, see dim_lighting (HOST intensity [n_iter,B,3]).
  * Pinned buffers are recommended.  Synchronises the stream before returning. */
 DIM_API int32_t dim_refine_host(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
                                 const int32_t *cls_idx_host, const double *pose_init_host,
                                 int32_t B, int32_t n_iter, const float *K9_host, float znear,
                                 float zfar, const double *pixel_means_rgb_host, int32_t precision,
-                                double *poses_out_host, float *se3_out_host, void *stream);
+                                double *poses_out_host, float *se3_out_host,
+                                const uint16_t *depth_observed_u16_host, float depth_factor,
+                                const dim_lighting *lighting, void *stream);
 
-/* Per-iteration status of the LAST dim_refine(_lit) / dim_refine_host(_lit)(_async) call on this context, copied device -> host
+/* Per-iteration status of the LAST dim_refine / dim_refine_host(_async) call on this context, copied device -> host
  * asynchronously on `stream` (the stream that call ran on): [min(n_iter,8), B] int32.  0 = ok; bit 0 = the rendered mask
  * of that iteration was empty (the reference crashes there: np.min of an empty array, zoom_mask.py:55-58; here the
  * fallback zoom factor was used and the instance's pose is meaningless); bit 1 = class index out of range or no mesh
@@ -256,126 +323,8 @@ DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *image_observe
                                       int32_t B, int32_t n_iter, const float *K9_host, float znear,
                                       float zfar, const double *pixel_means_rgb_host,
                                       int32_t precision, double *poses_out_host, float *se3_out_host,
-                                      void *stream);
-
-/* ModelNet / unseen-object configuration (config.dataset.dataset "ModelNet*": deepim/core/tester.py:114-133,146-185;
- * lib/pair_matching/batch_updater_py_multi.py:35-52,187-229): every render of the loop is the Lambert-lit renderer of
- * dim_render_lit instead of the unlit one.  The light follows the pose being rendered: in the GL camera frame
- *   light_position = float32(offset[0] + t_x, offset[1] - t_y, offset[2] - t_z)
- * computed from the float64 pose (the reference's hard-coded light index 2 gives offset = (0, 0.5, 0.5)).  The reference
- * draws light_intensity from U(0.9, 1.1)^3 afresh for every render; here the caller supplies the draws.
- *   intensity: device f32 [n_iter,B,3] for dim_refine_lit (iteration it renders with intensity[it]), [B,3] for
- *              dim_train_update_lit, HOST f32 [n_iter,B,3] for dim_refine_host_lit(_async) (n_iter <= 8; copied to the
- *              context on `stream` before the call returns, so a pageable buffer may be reused at once).
- *   brightness_ratio: colour = texel * ((1 - ratio) + ratio * brightness) * intensity (the reference: 0.7).
- * Depth, masks, bboxes, zoom, labels and flow are those of the unlit calls; only the colours change.  Every uploaded mesh
- * must have normals (dim_mesh_upload_normals).  The lit calls take every argument of their unlit counterparts plus
- * `lighting`, share dim_refine_status, and are captured / replayed as CUDA graphs like dim_refine. */
-typedef struct dim_lighting {
-  const float *intensity; /* see above: device [n_iter,B,3] (refine) / [B,3] (train update); host for dim_refine_host_lit */
-  double offset[3];       /* light at zero translation, GL frame; the reference: (0, 0.5, 0.5) */
-  float brightness_ratio; /* the reference: 0.7 */
-} dim_lighting;
-DIM_API int32_t dim_refine_lit(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx,
-                               const double *pose_init, int32_t B, int32_t n_iter, const float *K9_host,
-                               float znear, float zfar, const double *pixel_means_rgb_host,
-                               int32_t precision, const double *pose_override, double *poses,
-                               float *se3, float *zoom_factor, int32_t *bbox, const dim_lighting *lighting,
-                               void *stream);
-DIM_API int32_t dim_refine_host_lit(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
-                                    const int32_t *cls_idx_host, const double *pose_init_host,
-                                    int32_t B, int32_t n_iter, const float *K9_host, float znear,
-                                    float zfar, const double *pixel_means_rgb_host, int32_t precision,
-                                    double *poses_out_host, float *se3_out_host,
-                                    const dim_lighting *lighting, void *stream);
-DIM_API int32_t dim_refine_host_lit_async(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
-                                          const int32_t *cls_idx_host, const double *pose_init_host,
-                                          int32_t B, int32_t n_iter, const float *K9_host, float znear,
-                                          float zfar, const double *pixel_means_rgb_host,
-                                          int32_t precision, double *poses_out_host, float *se3_out_host,
-                                          const dim_lighting *lighting, void *stream);
-
-/* dim_train_update for the ModelNet configuration (batch_updater_py_multi.py:187-235): the re-render is lit, the light
- * follows the float64 refined pose (dim_lighting above; intensity device f32 [B,3]); image_rendered = float32 quantised
- * lit colours - float32 means.  Every other output equals dim_train_update's. */
-DIM_API int32_t dim_train_update_lit(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose,
-                                     const float *rot_est, const float *trans_est, const float *tgt_pose,
-                                     const float *depth_gt_observed, int32_t B, const double *K9_host,
-                                     float znear, float zfar, const double *pixel_means_rgb_host,
-                                     const double *T_means_host, const double *T_stds_host,
-                                     int32_t rot_coord, float *image_rendered, float *depth_rendered,
-                                     float *mask_rendered, float *src_pose_new, float *rot_label,
-                                     float *trans_label, float *flow, float *flow_weights,
-                                     const dim_lighting *lighting, void *stream);
-
-/* RGB-D refinement (config.network.INPUT_DEPTH: deepIM_flownet.py:33-51, tester.py:437-438).  The network's input gains
- * two channels, in the order image_observed/255, image_rendered/255, depth_observed/255, depth_rendered/255,
- * mask_observed, mask_rendered: flow_conv1_weight is (64, 10, 7, 7), the depths (metres, divided by 255 as the reference
- * does) are channels 6 and 7.  depth_rendered is each iteration's render depth (0 = background), zoomed with the
- * iteration's zoom factor like every other input (ZoomDepth, zoom_depth.py:24-44).
- *
- * dim_ctx_set_input_depth: enable = 1 switches the context's network to the 10-channel input, 0 back to the 8-channel one.
- *   Only before dim_net_load / dim_train_create (an error afterwards); a context that never calls it is unchanged.  On an
- *   RGB-D context dim_net_load takes the (64,10,7,7) flow_conv1 weight and the training step is
- *   dim_train_forward_backward_rgbd (below).
- * The RGB network's entries (dim_refine(_lit), dim_refine_host(_lit)(_async), dim_net_fwd) refuse an RGB-D context and the
- * _rgbd entries an RGB one, with a message naming the call to use.
- * dim_refine_rgbd: dim_refine's arguments plus depth_observed, device f32 [B,1,H,W] in metres (constant over the
- *   iterations), and lighting (NULL: unlit; else as dim_refine_lit).  Shares dim_refine_status; captured / replayed as a
- *   CUDA graph like dim_refine, keyed on the depth pointer as well.
- * dim_refine_host_rgbd(_async): dim_refine_host's arguments plus the host depth file values u16 [B,H,W], converted on the
- *   device as lib/utils/image.py:203,218 does: float32(u16) / float32(depth_factor) (LINEMOD: 1000); lighting as above
- *   with a HOST intensity.
- * dim_net_fwd_rgbd: dim_net_fwd on already-zoomed blobs plus the zoomed depths f32 [B,1,H,W]. */
-DIM_API int32_t dim_ctx_set_input_depth(dim_ctx *ctx, int32_t enable);
-DIM_API int32_t dim_refine_rgbd(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx,
-                                const double *pose_init, int32_t B, int32_t n_iter, const float *K9_host,
-                                float znear, float zfar, const double *pixel_means_rgb_host,
-                                int32_t precision, const double *pose_override, double *poses,
-                                float *se3, float *zoom_factor, int32_t *bbox, const float *depth_observed,
-                                const dim_lighting *lighting, void *stream);
-DIM_API int32_t dim_refine_host_rgbd(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
-                                     const int32_t *cls_idx_host, const double *pose_init_host,
-                                     int32_t B, int32_t n_iter, const float *K9_host, float znear,
-                                     float zfar, const double *pixel_means_rgb_host, int32_t precision,
-                                     double *poses_out_host, float *se3_out_host,
-                                     const uint16_t *depth_observed_u16_host, float depth_factor,
-                                     const dim_lighting *lighting, void *stream);
-DIM_API int32_t dim_refine_host_rgbd_async(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
-                                           const int32_t *cls_idx_host, const double *pose_init_host,
-                                           int32_t B, int32_t n_iter, const float *K9_host, float znear,
-                                           float zfar, const double *pixel_means_rgb_host, int32_t precision,
-                                           double *poses_out_host, float *se3_out_host,
-                                           const uint16_t *depth_observed_u16_host, float depth_factor,
-                                           const dim_lighting *lighting, void *stream);
-DIM_API int32_t dim_net_fwd_rgbd(dim_ctx *ctx, const float *zoom_image_observed,
-                                 const float *zoom_image_rendered, const float *zoom_depth_observed,
-                                 const float *zoom_depth_rendered, const float *zoom_mask_observed,
-                                 const float *zoom_mask_rendered, int32_t B, int32_t precision,
-                                 float *rot, float *trans, void *stream);
-
-/* Image-only network (config.network.INPUT_MASK: False, the reference's default; deepIM_flownet.py:53-62, tester.py:439): conv1
- * sees concat(image_observed/255, image_rendered/255), so flow_conv1_weight is (64, 6, 7, 7), and the test graph zooms with
- * ZoomImage (zoom_image.py:26-107, the boxes of sum_c(image + mean) > 0.01) instead of ZoomMask + ZoomImageWithFactor.
- *
- * dim_ctx_set_input_mask: enable = 0 switches the context to this network, 1 (the default) back.  Only before dim_net_load /
- *   dim_train_create (an error afterwards); refused together with dim_ctx_set_input_depth (depth input without the mask
- *   channels is not supported).  A context that never calls it is unchanged.
- * On such a context the existing entries follow the network, with no argument change:
- *   - dim_refine(_lit), dim_refine_host(_lit)(_async) run the image-only chain: the observed box is computed once per call,
- *     the rendered box of every iteration from the render's colours; the zoom factor is ZoomImage's (ZoomMask's arithmetic
- *     with the observed-centre fallback for an empty render).  dim_refine_status: bit 0 = the observed image has no valid
- *     pixel (the reference raises; the fallback factor (1,1,0,0) was used), bit 2 = the rendered image has none (the zoom
- *     centres on the observed box, as the reference does), bit 1 unchanged.
- *   - dim_net_fwd needs zoom_mask_observed = zoom_mask_rendered = NULL; so does dim_train_forward_backward.
- *   - dim_train_update(_lit) is unchanged: with PRED_MASK the reference's training graph still zooms with ZoomMask and learns
- *     the mask; only the network input loses the mask channels.
- *   - dim_net_load takes the (64, 6, 7, 7) flow_conv1 weight; the flat training vector is the table of
- *     dim_train_param_info_nomask (flow_conv1 (64, 6, 7, 7): 6 272 floats fewer; every other entry as dim_train_param_info),
- *     and dim_train_param_count reports its size. */
-DIM_API int32_t dim_ctx_set_input_mask(dim_ctx *ctx, int32_t enable);
-DIM_API int32_t dim_train_param_info_nomask(int32_t idx, const char **name, int64_t *weight_numel,
-                                            int64_t *bias_numel);
+                                      const uint16_t *depth_observed_u16_host, float depth_factor,
+                                      const dim_lighting *lighting, void *stream);
 
 /* BGR u8 HWC -> RGB-mean f32 CHW on device (lib/utils/image.py:583-594 transform). */
 DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int32_t B,
@@ -470,15 +419,18 @@ DIM_API int32_t dim_flow_epe(dim_ctx *ctx, const float *flow_pred, const float *
  * returned by dim_train_param_info (flow_conv1 ... conv6_1, fc6, fc7, rot, trans, Convolution1, deconv5,
  * upsample_flow6to5, Convolution2, deconv4, upsample_flow5to4, Convolution3, mask_conv3) weight then bias,
  * followed by the frozen bilinear upsampling_weight (2,1,32,32) and mask_upsampling_weight (1,1,32,32):
- * 57 749 164 floats.  One tensor is permuted: fc6_weight is stored (256, h*10+w, c) -- the NHWC order of the
- * conv6_1 activation it multiplies -- instead of MXNet's (256, c*80 + h*10 + w) (the Python host permutes on
- * load / get; element-wise consumers such as the all-reduce and SGD do not care).  Gradients use the same layout (that is the buffer a data-parallel caller all-reduces
- * with NCCL between dim_train_forward_backward and dim_train_sgd_update; kvstore replacement,
- * deepim/core/module.py:616-635). */
+ * 57 749 164 floats for the mask network; the RGB-D network's flow_conv1 (64, 10, 7, 7) adds 6 272, the image-only
+ * network's (64, 6, 7, 7) removes 6 272, every other entry is the same.  One tensor is permuted: fc6_weight is stored
+ * (256, h*10+w, c) -- the NHWC order of the conv6_1 activation it multiplies -- instead of MXNet's (256, c*80 + h*10 + w)
+ * (the Python host permutes on load / get; element-wise consumers such as the all-reduce and SGD do not care).  Gradients
+ * use the same layout (that is the buffer a data-parallel caller all-reduces with NCCL between dim_train_forward_backward
+ * and dim_train_sgd_update; kvstore replacement, deepim/core/module.py:616-635).
+ * dim_train_param_info needs no context: entry idx of the table of the network (input_depth, input_mask) as the Network
+ * variants above; input_depth = 1 with input_mask = 0 is refused.  Non-zero past the last entry. */
 DIM_API int32_t dim_train_create(dim_ctx *ctx, int32_t max_points);
 DIM_API int64_t dim_train_param_count(dim_ctx *ctx);
-DIM_API int32_t dim_train_param_info(int32_t idx, const char **name, int64_t *weight_numel,
-                                     int64_t *bias_numel);
+DIM_API int32_t dim_train_param_info(int32_t input_depth, int32_t input_mask, int32_t idx, const char **name,
+                                     int64_t *weight_numel, int64_t *bias_numel);
 /* flat_host: host pointer.  Also (re)loads the inference network of this context. */
 DIM_API int32_t dim_train_load_params(dim_ctx *ctx, const float *flat_host, int64_t n, void *stream);
 /* which = 0: parameters, 1: momentum.  Synchronises the stream. */
@@ -486,6 +438,9 @@ DIM_API int32_t dim_train_get_params(dim_ctx *ctx, float *flat_host, int64_t n, 
                                      void *stream);
 /* Device pointers, fp32 NCHW: zoomed images (B,3,H,W), zoomed masks (B,1,H,W), zoom_factor (B,4), zoomed flow
  * label (B,2,H,W) and weights (B,2,H,W), zoomed GT mask (B,1,H,W), src_pose (B,3,4), point clouds (B,3,N).
+ * RGB-D network: zoom_depth_observed / zoom_depth_rendered (B,1,H,W), metres (the train-time update's depth_rendered,
+ * zoomed with the pair's zoom factor; deepIM_flownet.py:33-51, batch_updater l.269); conv1 has no data gradient, so only
+ * flow_conv1_weight's gradient widens.  Depth and mask inputs are NULL as the network variant says.
  * Outputs: rot_est_norm (B,4) = L2Normalization(rot), trans_est (B,3) = invZoomTrans, flow_est (B,2,H,W)
  * (= flow_est_crop * NORMALIZE_FLOW, nullable), mask_prob (B,1,H,W) (nullable), losses4 = [sum flow_loss,
  * sum point_matching_loss, sum mask BCE, weighted objective], grads (flat, see above; NULL = forward only:
@@ -497,23 +452,6 @@ DIM_API int32_t dim_train_get_params(dim_ctx *ctx, float *flat_host, int64_t n, 
  * caller can start the NCCL all-reduce of that slice of `grads` while the rest of the backward pass still runs.
  * All work is joined back into `stream` before the call's stream order ends. */
 DIM_API int32_t dim_train_forward_backward(
-    dim_ctx *ctx, const float *zoom_image_observed, const float *zoom_image_rendered,
-    const float *zoom_mask_observed, const float *zoom_mask_rendered, const float *zoom_factor,
-    const float *zoom_flow, const float *zoom_flow_weights, const float *zoom_mask_gt_observed,
-    const float *src_pose, const float *point_cloud_model, const float *point_cloud_weights,
-    const float *point_cloud_observed, int32_t B, int32_t N, float *rot_est_norm, float *trans_est,
-    float *flow_est, float *mask_prob, float *losses4, float *grads, float *rot_raw,
-    void *const *bucket_events,
-    const int32_t *bucket_first_tensor, int32_t n_buckets, void *stream);
-/* The training step of the RGB-D network (a context switched by dim_ctx_set_input_depth before dim_train_create):
- * dim_train_forward_backward's arguments plus the zoomed depth_observed and depth_rendered f32 (B,1,H,W), metres (the
- * train-time update's depth_rendered, zoomed with the pair's zoom factor; deepIM_flownet.py:33-51, batch_updater l.269).
- * conv1 has no data gradient, so only flow_conv1_weight's gradient widens.  The flat parameter vector of such a context is
- * the RGB-D table: dim_train_param_info_rgbd (flow_conv1 (64,10,7,7): 6 272 floats more; every other entry as
- * dim_train_param_info); dim_train_param_count reports its size.  Each network's entry refuses the other's context. */
-DIM_API int32_t dim_train_param_info_rgbd(int32_t idx, const char **name, int64_t *weight_numel,
-                                          int64_t *bias_numel);
-DIM_API int32_t dim_train_forward_backward_rgbd(
     dim_ctx *ctx, const float *zoom_image_observed, const float *zoom_image_rendered,
     const float *zoom_mask_observed, const float *zoom_mask_rendered, const float *zoom_factor,
     const float *zoom_flow, const float *zoom_flow_weights, const float *zoom_mask_gt_observed,
@@ -547,7 +485,7 @@ DIM_API int32_t dim_train_sgd_update(dim_ctx *ctx, const float *grads, float lr,
 /* Precision of this context's training step: DIM_PREC_BF16 (default; bf16 activations and activation gradients) or
  * DIM_PREC_BF16X3 (every activation, activation gradient and operand pack a bf16 hi / lo pair, three tensor-core passes:
  * gradients near the fp32 reference, about 2^-16 relative per stored value).  Gradients, master weights and momentum are
- * fp32 in both.  Applies to dim_train_forward_backward(_rgbd), with and without gradients, and to the operand refresh of
+ * fp32 in both.  Applies to dim_train_forward_backward, with and without gradients, and to the operand refresh of
  * dim_train_sgd_update.  Any other value is refused (DIM_PREC_FP16 included).  Needs dim_train_create.  The first switch to
  * DIM_PREC_BF16X3 allocates the lo halves; every switch to it synchronises the device and refreshes them from the master
  * weights.  Switching back to DIM_PREC_BF16 leaves the bf16 step exactly as it was. */

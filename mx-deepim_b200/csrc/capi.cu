@@ -160,10 +160,11 @@ static int normals_check(dim_ctx *ctx, const char *fn) {
     }
   return 0;
 }
-// the lit loop / update entry points: lighting and its intensities are given and every uploaded mesh has normals
+// lighting of the loop / update entry points: NULL = unlit; else its intensities are given and every uploaded mesh has normals
 static int lit_check(dim_ctx *ctx, const dim_lighting *lit, const char *fn) {
-  if (!ctx || !lit || !lit->intensity) {
-    set_error("%s: NULL context, lighting or lighting->intensity", fn);
+  if (!lit) return 0;
+  if (!lit->intensity) {
+    set_error("%s: NULL lighting->intensity", fn);
     return 2;
   }
   return normals_check(ctx, fn);
@@ -172,15 +173,15 @@ static LitParams lit_params(const float *light_pos, const float *intensity, floa
   return LitParams{light_pos, intensity, (float)(1.0 - (double)ratio), ratio};
 }
 
-// the RGB network's entries refuse an RGB-D context and the _rgbd entries an RGB one: never run conv1 on the wrong channels
-static int input_mode_check(dim_ctx *ctx, bool rgbd_entry, const char *fn, const char *use) {
-  if (!ctx) { set_error("%s: NULL context", fn); return 2; }
-  if (net_input_depth(ctx) == rgbd_entry) return 0;
-  if (rgbd_entry)
-    set_error("%s: this context's network takes no depth input; call %s, or switch the context with "
-              "dim_ctx_set_input_depth before loading weights", fn, use);
+// depth inputs are given exactly when the context's network is RGB-D: never run conv1 on the wrong channels.
+// d1: the second depth of a pair (the single-depth entries pass d0 twice); args names them in the message.
+static int depth_check(dim_ctx *ctx, const void *d0, const void *d1, const char *fn, const char *args) {
+  const bool rgbd = net_input_depth(ctx);
+  if (rgbd ? (d0 && d1) : (!d0 && !d1)) return 0;
+  if (rgbd)
+    set_error("%s: this context's network takes depth input (dim_ctx_set_input_depth): %s must not be NULL", fn, args);
   else
-    set_error("%s: this context's network takes depth input (dim_ctx_set_input_depth); call %s", fn, use);
+    set_error("%s: this context's network takes no depth input (dim_ctx_set_input_depth): pass %s = NULL", fn, args);
   return 2;
 }
 
@@ -336,10 +337,11 @@ DIM_API int32_t dim_net_load(dim_ctx *ctx, const float *const *W, const float *c
   return net_load(ctx, W, Bv);
 }
 
-DIM_API int32_t dim_net_fwd(dim_ctx *ctx, const float *zio, const float *zir, const float *zmo, const float *zmr,
-                            int32_t B, int32_t precision, float *rot, float *trans, void *stream) {
+DIM_API int32_t dim_net_fwd(dim_ctx *ctx, const float *zio, const float *zir, const float *zdo, const float *zdr,
+                            const float *zmo, const float *zmr, int32_t B, int32_t precision, float *rot, float *trans,
+                            void *stream) {
   DIM_REQUIRE(ctx && zio && zir && rot && trans, "dim_net_fwd: NULL argument");
-  if (int rc = input_mode_check(ctx, false, "dim_net_fwd", "dim_net_fwd_rgbd")) return rc;
+  if (int rc = depth_check(ctx, zdo, zdr, "dim_net_fwd", "zoom_depth_observed / zoom_depth_rendered")) return rc;
   if (net_input_mask(ctx)) {
     DIM_REQUIRE(zmo && zmr, "dim_net_fwd: NULL argument");
   } else {
@@ -350,23 +352,10 @@ DIM_API int32_t dim_net_fwd(dim_ctx *ctx, const float *zio, const float *zir, co
   cudaStream_t st = (cudaStream_t)stream;
   int rows, cols, pad; __nv_bfloat16 *hi, *lo;
   net_input_geometry(ctx, &rows, &cols, &pad, &hi, &lo);
-  if (int rc = pack_nhwc8_launch(ctx, zio, zir, zmo, zmr, B, rows, cols, pad, hi,
-                                 precision == DIM_PREC_BF16X3 ? lo : nullptr, st, precision == DIM_PREC_FP16))
-    return rc;
-  return net_forward(ctx, B, precision, nullptr, rot, trans, nullptr, st, nullptr);
-}
-
-DIM_API int32_t dim_net_fwd_rgbd(dim_ctx *ctx, const float *zio, const float *zir, const float *zdo, const float *zdr,
-                                 const float *zmo, const float *zmr, int32_t B, int32_t precision, float *rot, float *trans,
-                                 void *stream) {
-  DIM_REQUIRE(ctx && zio && zir && zdo && zdr && zmo && zmr && rot && trans, "dim_net_fwd_rgbd: NULL argument");
-  if (int rc = input_mode_check(ctx, true, "dim_net_fwd_rgbd", "dim_net_fwd")) return rc;
-  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_net_fwd_rgbd: batch exceeds max_batch");
-  cudaStream_t st = (cudaStream_t)stream;
-  int rows, cols, pad; __nv_bfloat16 *hi, *lo;
-  net_input_geometry(ctx, &rows, &cols, &pad, &hi, &lo);
-  if (int rc = pack_nhwc10_launch(ctx, zio, zir, zdo, zdr, zmo, zmr, B, rows, cols, pad, hi,
-                                  precision == DIM_PREC_BF16X3 ? lo : nullptr, st, precision == DIM_PREC_FP16))
+  __nv_bfloat16 *lo_or_null = precision == DIM_PREC_BF16X3 ? lo : nullptr;
+  const int f16 = precision == DIM_PREC_FP16;
+  if (int rc = zdo ? pack_nhwc10_launch(ctx, zio, zir, zdo, zdr, zmo, zmr, B, rows, cols, pad, hi, lo_or_null, st, f16)
+                   : pack_nhwc8_launch(ctx, zio, zir, zmo, zmr, B, rows, cols, pad, hi, lo_or_null, st, f16))
     return rc;
   return net_forward(ctx, B, precision, nullptr, rot, trans, nullptr, st, nullptr);
 }
@@ -602,12 +591,17 @@ static RefineArgs refine_args(int32_t B, int32_t n_iter, const float *K9, float 
   return a;
 }
 
-// dim_refine(_lit) after their argument checks
-static int refine_device(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
-                         int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
-                         int32_t precision, const double *pose_override, double *poses, float *se3, float *zoom_factor,
-                         int32_t *bbox, const dim_lighting *lit, cudaStream_t st, const float *depth_observed = nullptr) {
-  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lit);
+DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
+                           int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
+                           int32_t precision, const double *pose_override, double *poses, float *se3, float *zoom_factor,
+                           int32_t *bbox, const float *depth_observed, const dim_lighting *lighting, void *stream) {
+  DIM_REQUIRE(ctx && image_observed && cls_idx && pose_init && K9 && means && poses, "dim_refine: NULL argument");
+  if (int rc = depth_check(ctx, depth_observed, depth_observed, "dim_refine", "depth_observed")) return rc;
+  if (int rc = lit_check(ctx, lighting, "dim_refine")) return rc;
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine: batch exceeds max_batch");
+  DIM_REQUIRE(n_iter >= 1, "dim_refine: n_iter must be >= 1");
+  cudaStream_t st = (cudaStream_t)stream;
+  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
   a.obs4 = ctx->obs4; a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
   a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
   // the graph never reads depth_observed: it is packed into obs4.w below, outside the graph, like the image, so a replay is
@@ -619,53 +613,16 @@ static int refine_device(dim_ctx *ctx, const float *image_observed, const int32_
   return refine_graphed(ctx, a, st);
 }
 
-DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
-                           int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
-                           int32_t precision, const double *pose_override, double *poses, float *se3,
-                           float *zoom_factor, int32_t *bbox, void *stream) {
-  DIM_REQUIRE(ctx && image_observed && cls_idx && pose_init && K9 && means && poses, "dim_refine: NULL argument");
-  if (int rc = input_mode_check(ctx, false, "dim_refine", "dim_refine_rgbd")) return rc;
-  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine: batch exceeds max_batch");
-  DIM_REQUIRE(n_iter >= 1, "dim_refine: n_iter must be >= 1");
-  return refine_device(ctx, image_observed, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override,
-                       poses, se3, zoom_factor, bbox, nullptr, (cudaStream_t)stream);
-}
-
-DIM_API int32_t dim_refine_lit(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
-                               int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
-                               int32_t precision, const double *pose_override, double *poses, float *se3,
-                               float *zoom_factor, int32_t *bbox, const dim_lighting *lighting, void *stream) {
-  if (int rc = lit_check(ctx, lighting, "dim_refine_lit")) return rc;
-  if (int rc = input_mode_check(ctx, false, "dim_refine_lit", "dim_refine_rgbd")) return rc;
-  DIM_REQUIRE(image_observed && cls_idx && pose_init && K9 && means && poses, "dim_refine_lit: NULL argument");
-  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_lit: batch exceeds max_batch");
-  DIM_REQUIRE(n_iter >= 1, "dim_refine_lit: n_iter must be >= 1");
-  return refine_device(ctx, image_observed, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override,
-                       poses, se3, zoom_factor, bbox, lighting, (cudaStream_t)stream);
-}
-
-DIM_API int32_t dim_refine_rgbd(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
-                                int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
-                                int32_t precision, const double *pose_override, double *poses, float *se3, float *zoom_factor,
-                                int32_t *bbox, const float *depth_observed, const dim_lighting *lighting, void *stream) {
-  if (int rc = input_mode_check(ctx, true, "dim_refine_rgbd", "dim_refine / dim_refine_lit")) return rc;
-  if (lighting)
-    if (int rc = lit_check(ctx, lighting, "dim_refine_rgbd")) return rc;
-  DIM_REQUIRE(image_observed && depth_observed && cls_idx && pose_init && K9 && means && poses,
-              "dim_refine_rgbd: NULL argument (image_observed, depth_observed, cls_idx, pose_init, K9, means, poses)");
-  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_rgbd: batch exceeds max_batch");
-  DIM_REQUIRE(n_iter >= 1, "dim_refine_rgbd: n_iter must be >= 1");
-  return refine_device(ctx, image_observed, cls_idx, pose_init, B, n_iter, K9, zn, zf, means, precision, pose_override,
-                       poses, se3, zoom_factor, bbox, lighting, (cudaStream_t)stream, depth_observed);
-}
-
-// dim_refine_host(_lit)(_rgbd)_async; lit_host: the caller's lighting with HOST intensities [n_iter,B,3] (nullptr: unlit);
-// depth_u16: RGB-D network, the caller's host depth file values [B,H,W] (nullptr: RGB network)
-static int refine_host_impl(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host, int32_t B,
-                            int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
-                            double *poses_out, float *se3_out, const dim_lighting *lit_host, cudaStream_t st,
-                            const uint16_t *depth_u16 = nullptr, float depth_factor = 0.f) {
+// lighting: the caller's lighting with HOST intensities [n_iter,B,3]; depth_u16: the caller's host depth file values [B,H,W]
+DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host,
+                                      int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
+                                      int32_t precision, double *poses_out, float *se3_out, const uint16_t *depth_u16,
+                                      float depth_factor, const dim_lighting *lighting, void *stream) {
   DIM_REQUIRE(ctx && img_u8 && cls_host && pose_host && K9 && means && poses_out, "dim_refine_host: NULL argument");
+  if (int rc = depth_check(ctx, depth_u16, depth_u16, "dim_refine_host", "depth_observed_u16_host")) return rc;
+  if (depth_u16)
+    DIM_REQUIRE(depth_factor > 0.f && depth_factor < 3.0e38f, "dim_refine_host: depth_factor must be positive and finite");
+  if (int rc = lit_check(ctx, lighting, "dim_refine_host")) return rc;
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_host: batch exceeds max_batch");
   DIM_REQUIRE(n_iter >= 1 && n_iter <= 8, "dim_refine_host: n_iter must be in [1,8]");
   for (int32_t i = 0; i < B; ++i) {  // the class indices are on the host here: fail loudly (the reference indexes a python list)
@@ -676,16 +633,17 @@ static int refine_host_impl(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *
       return 2;
     }
   }
+  cudaStream_t st = (cudaStream_t)stream;
   const size_t P = (size_t)ctx->H * ctx->W;
   DIM_CHECK(cudaMemcpyAsync(ctx->image_observed_u8, img_u8, (size_t)B * 3 * P, cudaMemcpyHostToDevice, st));
   DIM_CHECK(cudaMemcpyAsync(ctx->cls_dev, cls_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
   DIM_CHECK(cudaMemcpyAsync(ctx->pose_cur, pose_host, sizeof(double) * B * 12, cudaMemcpyHostToDevice, st));
-  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lit_host);
+  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
   a.obs4 = ctx->obs4; a.cls_idx = ctx->cls_dev; a.pose_init = ctx->pose_cur; a.poses = ctx->poses_dev;
   a.se3 = ctx->se3_hist_dev;
-  if (lit_host) {  // the intensities move to the context's buffer (a fixed address: graphs)
+  if (lighting) {  // the intensities move to the context's buffer (a fixed address: graphs)
     a.intensity = ctx->lit_intensity;
-    DIM_CHECK(cudaMemcpyAsync(ctx->lit_intensity, lit_host->intensity, sizeof(float) * (size_t)n_iter * B * 3,
+    DIM_CHECK(cudaMemcpyAsync(ctx->lit_intensity, lighting->intensity, sizeof(float) * (size_t)n_iter * B * 3,
                               cudaMemcpyHostToDevice, st));
   }
   if (int rc = transform_u8_obs4_launch(ctx, ctx->image_observed_u8, B, means, ctx->obs4, st)) return rc;
@@ -700,56 +658,12 @@ static int refine_host_impl(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *
   return 0;
 }
 
-DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host,
-                                      const double *pose_host, int32_t B, int32_t n_iter, const float *K9, float zn,
-                                      float zf, const double *means, int32_t precision, double *poses_out,
-                                      float *se3_out, void *stream) {
-  if (int rc = input_mode_check(ctx, false, "dim_refine_host", "dim_refine_host_rgbd")) return rc;
-  return refine_host_impl(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out, se3_out,
-                          nullptr, (cudaStream_t)stream);
-}
-
-DIM_API int32_t dim_refine_host_lit_async(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host,
-                                          const double *pose_host, int32_t B, int32_t n_iter, const float *K9, float zn,
-                                          float zf, const double *means, int32_t precision, double *poses_out,
-                                          float *se3_out, const dim_lighting *lighting, void *stream) {
-  if (int rc = lit_check(ctx, lighting, "dim_refine_host_lit")) return rc;
-  if (int rc = input_mode_check(ctx, false, "dim_refine_host_lit", "dim_refine_host_rgbd")) return rc;
-  return refine_host_impl(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out, se3_out,
-                          lighting, (cudaStream_t)stream);
-}
-
-DIM_API int32_t dim_refine_host_lit(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host,
-                                    int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
-                                    int32_t precision, double *poses_out, float *se3_out, const dim_lighting *lighting,
-                                    void *stream) {
-  if (int rc = dim_refine_host_lit_async(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision,
-                                         poses_out, se3_out, lighting, stream))
-    return rc;
-  DIM_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
-  return 0;
-}
-
-DIM_API int32_t dim_refine_host_rgbd_async(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host,
-                                           const double *pose_host, int32_t B, int32_t n_iter, const float *K9, float zn,
-                                           float zf, const double *means, int32_t precision, double *poses_out,
-                                           float *se3_out, const uint16_t *depth_u16, float depth_factor,
-                                           const dim_lighting *lighting, void *stream) {
-  if (int rc = input_mode_check(ctx, true, "dim_refine_host_rgbd", "dim_refine_host / dim_refine_host_lit")) return rc;
-  if (lighting)
-    if (int rc = lit_check(ctx, lighting, "dim_refine_host_rgbd")) return rc;
-  DIM_REQUIRE(depth_u16 != nullptr, "dim_refine_host_rgbd: NULL depth");
-  DIM_REQUIRE(depth_factor > 0.f && depth_factor < 3.0e38f, "dim_refine_host_rgbd: depth_factor must be positive and finite");
-  return refine_host_impl(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out, se3_out,
-                          lighting, (cudaStream_t)stream, depth_u16, depth_factor);
-}
-
-DIM_API int32_t dim_refine_host_rgbd(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host,
-                                     int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
-                                     int32_t precision, double *poses_out, float *se3_out, const uint16_t *depth_u16,
-                                     float depth_factor, const dim_lighting *lighting, void *stream) {
-  if (int rc = dim_refine_host_rgbd_async(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision,
-                                          poses_out, se3_out, depth_u16, depth_factor, lighting, stream))
+DIM_API int32_t dim_refine_host(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host,
+                                int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
+                                int32_t precision, double *poses_out, float *se3_out, const uint16_t *depth_u16,
+                                float depth_factor, const dim_lighting *lighting, void *stream) {
+  if (int rc = dim_refine_host_async(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out,
+                                     se3_out, depth_u16, depth_factor, lighting, stream))
     return rc;
   DIM_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
   return 0;
@@ -767,29 +681,21 @@ DIM_API int32_t dim_refine_status(dim_ctx *ctx, int32_t B, int32_t n_iter, int32
   return 0;
 }
 
-DIM_API int32_t dim_refine_host(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host,
-                                int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
-                                int32_t precision, double *poses_out, float *se3_out, void *stream) {
-  if (int rc = dim_refine_host_async(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out,
-                                     se3_out, stream))
-    return rc;
-  DIM_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
-  return 0;
-}
-
-// dim_train_update(_lit); lit: nullptr = the unlit re-render
-static int train_update_impl(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose, const float *rot_est,
-                             const float *trans_est, const float *tgt_pose, const float *depth_gt_observed, int32_t B,
-                             const double *K9, float zn, float zf, const double *means, const double *Tm, const double *Ts,
-                             int32_t rot_coord, float *image_rendered, float *depth_rendered, float *mask_rendered,
-                             float *src_pose_new, float *rot_label, float *trans_label, float *flow, float *flow_weights,
-                             const dim_lighting *lit, cudaStream_t st) {
+// lighting: nullptr = the unlit re-render
+DIM_API int32_t dim_train_update(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose, const float *rot_est,
+                                 const float *trans_est, const float *tgt_pose, const float *depth_gt_observed, int32_t B,
+                                 const double *K9, float zn, float zf, const double *means, const double *Tm, const double *Ts,
+                                 int32_t rot_coord, float *image_rendered, float *depth_rendered, float *mask_rendered,
+                                 float *src_pose_new, float *rot_label, float *trans_label, float *flow, float *flow_weights,
+                                 const dim_lighting *lit, void *stream) {
   DIM_REQUIRE(ctx && cls_idx && src_pose && rot_est && trans_est && tgt_pose && K9 && means && Tm && Ts,
               "dim_train_update: NULL argument");
   DIM_REQUIRE(image_rendered && depth_rendered && mask_rendered && src_pose_new && rot_label && trans_label,
               "dim_train_update: NULL output");
+  if (int rc = lit_check(ctx, lit, "dim_train_update")) return rc;
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_train_update: batch exceeds max_batch");
   DIM_REQUIRE(rot_coord >= 0 && rot_coord <= 2, "dim_train_update: unknown rot_coord");
+  cudaStream_t st = (cudaStream_t)stream;
   float *KT = ctx->pose_cur_f32;  // [B,12] scratch
   if (int rc = train_pose_launch(src_pose, rot_est, trans_est, tgt_pose, B, Tm, Ts, rot_coord, K9, src_pose_new,
                                  rot_label, trans_label, KT, st, lit ? ctx->light_pos : nullptr, lit ? lit->offset : nullptr))
@@ -820,30 +726,6 @@ static int train_update_impl(dim_ctx *ctx, const int32_t *cls_idx, const float *
                                   P * sizeof(float), B, cudaMemcpyDeviceToDevice, st));
   }
   return 0;
-}
-
-DIM_API int32_t dim_train_update(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose, const float *rot_est,
-                                 const float *trans_est, const float *tgt_pose, const float *depth_gt_observed,
-                                 int32_t B, const double *K9, float zn, float zf, const double *means,
-                                 const double *Tm, const double *Ts, int32_t rot_coord, float *image_rendered,
-                                 float *depth_rendered, float *mask_rendered, float *src_pose_new, float *rot_label,
-                                 float *trans_label, float *flow, float *flow_weights, void *stream) {
-  return train_update_impl(ctx, cls_idx, src_pose, rot_est, trans_est, tgt_pose, depth_gt_observed, B, K9, zn, zf, means, Tm,
-                           Ts, rot_coord, image_rendered, depth_rendered, mask_rendered, src_pose_new, rot_label, trans_label,
-                           flow, flow_weights, nullptr, (cudaStream_t)stream);
-}
-
-DIM_API int32_t dim_train_update_lit(dim_ctx *ctx, const int32_t *cls_idx, const float *src_pose, const float *rot_est,
-                                     const float *trans_est, const float *tgt_pose, const float *depth_gt_observed,
-                                     int32_t B, const double *K9, float zn, float zf, const double *means,
-                                     const double *Tm, const double *Ts, int32_t rot_coord, float *image_rendered,
-                                     float *depth_rendered, float *mask_rendered, float *src_pose_new, float *rot_label,
-                                     float *trans_label, float *flow, float *flow_weights, const dim_lighting *lighting,
-                                     void *stream) {
-  if (int rc = lit_check(ctx, lighting, "dim_train_update_lit")) return rc;
-  return train_update_impl(ctx, cls_idx, src_pose, rot_est, trans_est, tgt_pose, depth_gt_observed, B, K9, zn, zf, means, Tm,
-                           Ts, rot_coord, image_rendered, depth_rendered, mask_rendered, src_pose_new, rot_label, trans_label,
-                           flow, flow_weights, lighting, (cudaStream_t)stream);
 }
 
 DIM_API int32_t dim_profile_enable(dim_ctx *ctx, int32_t enable) {
@@ -919,24 +801,13 @@ DIM_API int32_t dim_train_create(dim_ctx *ctx, int32_t max_points) {
   return train_create(ctx, max_points);
 }
 DIM_API int64_t dim_train_param_count(dim_ctx *ctx) { return ctx ? (int64_t)train_param_count(ctx) : 0; }
-DIM_API int32_t dim_train_param_info(int32_t idx, const char **name, int64_t *w_numel, int64_t *b_numel) {
-  long long w = 0, b = 0;
+DIM_API int32_t dim_train_param_info(int32_t input_depth, int32_t input_mask, int32_t idx, const char **name, int64_t *w_numel,
+                                     int64_t *b_numel) {
   DIM_REQUIRE(name && w_numel && b_numel, "dim_train_param_info: NULL argument");
-  if (train_param_info(idx, name, &w, &b)) return 2;
-  *w_numel = w; *b_numel = b;
-  return 0;
-}
-DIM_API int32_t dim_train_param_info_rgbd(int32_t idx, const char **name, int64_t *w_numel, int64_t *b_numel) {
+  DIM_REQUIRE(!input_depth || input_mask, "dim_train_param_info: input_depth with input_mask = 0 (depth input without the mask "
+                                          "channels, INPUT_DEPTH without INPUT_MASK) is not supported");
   long long w = 0, b = 0;
-  DIM_REQUIRE(name && w_numel && b_numel, "dim_train_param_info_rgbd: NULL argument");
-  if (train_param_info(idx, name, &w, &b, true)) return 2;
-  *w_numel = w; *b_numel = b;
-  return 0;
-}
-DIM_API int32_t dim_train_param_info_nomask(int32_t idx, const char **name, int64_t *w_numel, int64_t *b_numel) {
-  long long w = 0, b = 0;
-  DIM_REQUIRE(name && w_numel && b_numel, "dim_train_param_info_nomask: NULL argument");
-  if (train_param_info(idx, name, &w, &b, false, false)) return 2;
+  if (train_param_info(idx, name, &w, &b, input_depth != 0, input_mask != 0)) return 2;
   *w_numel = w; *b_numel = b;
   return 0;
 }
@@ -954,9 +825,9 @@ DIM_API int32_t dim_train_forward_backward(dim_ctx *ctx, const float *zio, const
                                            const float *pc_observed, int32_t B, int32_t N, float *rot_est_norm, float *trans_est,
                                            float *flow_est, float *mask_prob, float *losses4, float *grads, float *rot_raw,
                                            void *const *bucket_events, const int32_t *bucket_first_tensor, int32_t n_buckets,
-                                           void *stream) {
+                                           const float *zdo, const float *zdr, void *stream) {
   DIM_REQUIRE(ctx && zio && zir && zoom_factor, "dim_train_forward_backward: NULL argument");
-  if (int rc = input_mode_check(ctx, false, "dim_train_forward_backward", "dim_train_forward_backward_rgbd")) return rc;
+  if (int rc = depth_check(ctx, zdo, zdr, "dim_train_forward_backward", "zoom_depth_observed / zoom_depth_rendered")) return rc;
   if (net_input_mask(ctx)) {
     DIM_REQUIRE(zmo && zmr, "dim_train_forward_backward: NULL argument");
   } else {
@@ -965,21 +836,7 @@ DIM_API int32_t dim_train_forward_backward(dim_ctx *ctx, const float *zio, const
   }
   TrainIO io{zio, zir, zmo, zmr, zoom_factor, zflow, zfw, zmask_gt, src_pose, pc_model, pc_weights, pc_observed, B, N,
              rot_est_norm, trans_est, flow_est, mask_prob, losses4, grads, rot_raw, bucket_events, bucket_first_tensor,
-             (bucket_events && bucket_first_tensor) ? n_buckets : 0};
-  return train_forward_backward(ctx, io, (cudaStream_t)stream);
-}
-DIM_API int32_t dim_train_forward_backward_rgbd(
-    dim_ctx *ctx, const float *zio, const float *zir, const float *zmo, const float *zmr, const float *zoom_factor, const float *zflow,
-    const float *zfw, const float *zmask_gt, const float *src_pose, const float *pc_model, const float *pc_weights,
-    const float *pc_observed, int32_t B, int32_t N, float *rot_est_norm, float *trans_est, float *flow_est, float *mask_prob,
-    float *losses4, float *grads, float *rot_raw, void *const *bucket_events, const int32_t *bucket_first_tensor, int32_t n_buckets,
-    const float *zoom_depth_observed, const float *zoom_depth_rendered, void *stream) {
-  DIM_REQUIRE(ctx && zio && zir && zmo && zmr && zoom_factor && zoom_depth_observed && zoom_depth_rendered,
-              "dim_train_forward_backward_rgbd: NULL argument");
-  if (int rc = input_mode_check(ctx, true, "dim_train_forward_backward_rgbd", "dim_train_forward_backward")) return rc;
-  TrainIO io{zio, zir, zmo, zmr, zoom_factor, zflow, zfw, zmask_gt, src_pose, pc_model, pc_weights, pc_observed, B, N,
-             rot_est_norm, trans_est, flow_est, mask_prob, losses4, grads, rot_raw, bucket_events, bucket_first_tensor,
-             (bucket_events && bucket_first_tensor) ? n_buckets : 0, zoom_depth_observed, zoom_depth_rendered};
+             (bucket_events && bucket_first_tensor) ? n_buckets : 0, zdo, zdr};
   return train_forward_backward(ctx, io, (cudaStream_t)stream);
 }
 DIM_API int32_t dim_train_set_config(dim_ctx *ctx, const dim_train_config *cfg) {

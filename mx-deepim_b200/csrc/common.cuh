@@ -87,7 +87,7 @@ struct RefineArgs {
   float *se3, *zoom_factor;  // nullable: the context's scratch
   int32_t *bbox;             // nullable
   const float *intensity;    // lit: device [n_iter,B,3]; unlit: nullptr
-  const float *depth_observed;  // RGB-D network, dim_refine_rgbd: the caller's device depth; otherwise nullptr
+  const float *depth_observed;  // RGB-D network, dim_refine: the caller's device depth; otherwise nullptr
   double means[3], offset[3];  // offset: the light's (lit only)
   float K9[9], zn, zf, brightness_ratio;
   int32_t B, n_iter, precision, lit;
@@ -125,8 +125,8 @@ struct dim_ctx {
   double *poses_dev = nullptr;  // [8, max_batch, 12]
   float *se3_hist_dev = nullptr;
   float *light_pos = nullptr;      // [max_batch,3] lit chain / lit train update: light of the pose being rendered
-  float *lit_intensity = nullptr;  // [8, max_batch, 3] dim_refine_host_lit: the caller's light intensities on the device
-  uint16_t *depth_u16 = nullptr;   // [max_batch,H,W] dim_refine_host_rgbd: the caller's depth file values (RGB-D contexts)
+  float *lit_intensity = nullptr;  // [8, max_batch, 3] lit dim_refine_host: the caller's light intensities on the device
+  uint16_t *depth_u16 = nullptr;   // [max_batch,H,W] RGB-D dim_refine_host: the caller's depth file values
   int *bbox_obs = nullptr;         // [max_batch,4] image-only network: the observed image's colour-valid box (ZoomImage)
   // background bank of dim_replace_background (dim_bg_upload): BGR u8 photos, each allocated at its upload
   struct BgImage { uint8_t *data = nullptr; int h = 0, w = 0; };

@@ -117,8 +117,7 @@ int train_load_params(dim_ctx *ctx, const float *flat_host, size_t n, cudaStream
 int train_refresh_lo(dim_ctx *ctx, cudaStream_t st);
 int train_get_params(dim_ctx *ctx, float *flat_host, size_t n, int which, cudaStream_t st);
 size_t train_param_count(dim_ctx *ctx);
-int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel, bool input_depth = false,
-                     bool input_mask = true);
+int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel, bool input_depth, bool input_mask);
 int train_forward_backward(dim_ctx *ctx, const TrainIO &io, cudaStream_t st);
 int train_sgd_update(dim_ctx *ctx, const float *grads, float lr, float momentum, float wd, float rescale, cudaStream_t st);
 int train_set_precision(dim_ctx *ctx, int precision);

@@ -654,7 +654,7 @@ int pack_nhwc8_launch(dim_ctx *ctx, const float *io, const float *ir, const floa
   return 0;
 }
 
-// NCHW float32 zoomed blobs + zoomed depths -> the RGB-D network's conv1 input (dim_net_fwd_rgbd): channels
+// NCHW float32 zoomed blobs + zoomed depths -> the RGB-D network's conv1 input (dim_net_fwd, training step): channels
 // io/255, ir/255, do/255, dr/255, mo, mr in two 8-channel chunks per space-to-depth phase
 __global__ void __launch_bounds__(256) pack_nhwc10_kernel(const float *io, const float *ir, const float *dobs,
                                                           const float *dren, const float *mo, const float *mr, int H, int W,

@@ -31,6 +31,9 @@ class Lighting(C.Structure):
     _fields_ = [("intensity", vp), ("offset", C.c_double * 3), ("brightness_ratio", f32)]
 
 
+plit = C.POINTER(Lighting)
+
+
 # name -> (restype, argtypes); every symbol declared in include/deepim_b200.h
 SIGNATURES = {
     "dim_abi_version": (i32, []),
@@ -56,27 +59,14 @@ SIGNATURES = {
     "dim_transform3d_fwd": (i32, [vp, vp, vp, vp, vp, i32, i32, pf32, pf32, i32, vp, vp]),
     "dim_transform3d_bwd": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, pf32, pf32, i32, vp, vp, vp]),
     "dim_train_update": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, pf64, f32, f32, pf64, pf64, pf64, i32, vp, vp, vp, vp, vp,
-                               vp, vp, vp, vp]),
+                               vp, vp, vp, plit, vp]),
     "dim_net_load": (i32, [vp, C.POINTER(vp), C.POINTER(vp)]),
-    "dim_net_fwd": (i32, [vp, vp, vp, vp, vp, i32, i32, vp, vp, vp]),
-    "dim_refine": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, vp]),
-    "dim_refine_host": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp]),
-    "dim_refine_host_async": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp]),
-    "dim_refine_lit": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, C.POINTER(Lighting), vp]),
-    "dim_refine_host_lit": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, C.POINTER(Lighting), vp]),
-    "dim_refine_host_lit_async": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, C.POINTER(Lighting), vp]),
-    "dim_train_update_lit": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, pf64, f32, f32, pf64, pf64, pf64, i32, vp, vp, vp, vp, vp,
-                                   vp, vp, vp, C.POINTER(Lighting), vp]),
+    "dim_net_fwd": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp]),
+    "dim_refine": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, vp, plit, vp]),
+    "dim_refine_host": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32, plit, vp]),
+    "dim_refine_host_async": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32, plit, vp]),
     "dim_ctx_set_input_depth": (i32, [vp, i32]),
-    "dim_refine_rgbd": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, vp,
-                              C.POINTER(Lighting), vp]),
-    "dim_refine_host_rgbd": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32,
-                                   C.POINTER(Lighting), vp]),
-    "dim_refine_host_rgbd_async": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32,
-                                         C.POINTER(Lighting), vp]),
-    "dim_net_fwd_rgbd": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp]),
     "dim_ctx_set_input_mask": (i32, [vp, i32]),
-    "dim_train_param_info_nomask": (i32, [i32, C.POINTER(C.c_char_p), C.POINTER(i64), C.POINTER(i64)]),
     "dim_transform_image_u8": (i32, [vp, vp, i32, pf64, vp, vp]),
     "dim_bg_upload": (i32, [vp, i32, vp, i32, i32]),
     "dim_bg_geometry": (i32, [i32, i32, i32, i32, C.POINTER(i32), pf64]),
@@ -95,12 +85,10 @@ SIGNATURES = {
     "dim_flow_epe": (i32, [vp, vp, vp, vp, vp, i32, vp, vp]),
     "dim_train_create": (i32, [vp, i32]),
     "dim_train_param_count": (i64, [vp]),
-    "dim_train_param_info": (i32, [i32, C.POINTER(C.c_char_p), C.POINTER(i64), C.POINTER(i64)]),
+    "dim_train_param_info": (i32, [i32, i32, i32, C.POINTER(C.c_char_p), C.POINTER(i64), C.POINTER(i64)]),
     "dim_train_load_params": (i32, [vp, vp, i64, vp]),
     "dim_train_get_params": (i32, [vp, vp, i64, i32, vp]),
-    "dim_train_forward_backward": (i32, [vp] + [vp] * 12 + [i32, i32] + [vp] * 7 + [vp, vp, i32] + [vp]),
-    "dim_train_param_info_rgbd": (i32, [i32, C.POINTER(C.c_char_p), C.POINTER(i64), C.POINTER(i64)]),
-    "dim_train_forward_backward_rgbd": (i32, [vp] + [vp] * 12 + [i32, i32] + [vp] * 7 + [vp, vp, i32] + [vp, vp] + [vp]),
+    "dim_train_forward_backward": (i32, [vp] + [vp] * 12 + [i32, i32] + [vp] * 7 + [vp, vp, i32] + [vp, vp] + [vp]),
     "dim_train_set_config": (i32, [vp, C.POINTER(TrainConfig)]),
     "dim_train_get_config": (i32, [vp, C.POINTER(TrainConfig)]),
     "dim_train_sgd_update": (i32, [vp, vp, f32, f32, f32, f32, vp]),

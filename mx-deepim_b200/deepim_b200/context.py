@@ -343,18 +343,15 @@ class Context:
         }
         if want_flow:
             _chk(depth_gt_observed, torch.float32, (B, 1, self.H, self.W), "depth_gt_observed")
-        args = (self._h, _p(cls_idx), _p(src_pose), _p(rot_est), _p(trans_est), _p(tgt_pose),
-                _p(depth_gt_observed) if want_flow else None, B,
-                farr(np.asarray(K, np.float64).reshape(9), 9, C.c_double), znear, zfar,
-                farr(pixel_means_rgb, 3, C.c_double), farr(T_means, 3, C.c_double),
-                farr(T_stds, 3, C.c_double), capi.ROT_COORD[rot_coord.lower()],
-                _p(out["image_rendered"]), _p(out["depth_rendered"]), _p(out["mask_rendered"]),
-                _p(out["src_pose"]), _p(out["rot"]), _p(out["trans"]), _p(out["flow"]), _p(out["flow_weights"]))
-        if lighting is None:
-            check(lib.dim_train_update(*args, self._stream()))
-        else:
-            lit, _ = _lighting_arg(lighting, (B, 3), True)
-            check(lib.dim_train_update_lit(*args, C.byref(lit), self._stream()))
+        lit = None if lighting is None else C.byref(_lighting_arg(lighting, (B, 3), True)[0])
+        check(lib.dim_train_update(self._h, _p(cls_idx), _p(src_pose), _p(rot_est), _p(trans_est), _p(tgt_pose),
+                                   _p(depth_gt_observed) if want_flow else None, B,
+                                   farr(np.asarray(K, np.float64).reshape(9), 9, C.c_double), znear, zfar,
+                                   farr(pixel_means_rgb, 3, C.c_double), farr(T_means, 3, C.c_double),
+                                   farr(T_stds, 3, C.c_double), capi.ROT_COORD[rot_coord.lower()],
+                                   _p(out["image_rendered"]), _p(out["depth_rendered"]), _p(out["mask_rendered"]),
+                                   _p(out["src_pose"]), _p(out["rot"]), _p(out["trans"]), _p(out["flow"]),
+                                   _p(out["flow_weights"]), lit, self._stream()))
         return out
 
     def transform_image_u8(self, bgr_u8, pixel_means_rgb):
@@ -400,17 +397,13 @@ class Context:
         """The network on already-zoomed blobs; an RGB-D context (input_depth=True) also takes the zoomed depths
         f32 [B,1,H,W] (metres); an image-only context (input_mask=False) takes no masks (None)."""
         B = zoom_image_observed.shape[0]
+        for n, t in (("zoom_depth_observed", zoom_depth_observed), ("zoom_depth_rendered", zoom_depth_rendered)):
+            if t is not None:
+                _chk(t, torch.float32, (B, 1, self.H, self.W), n)
         rot, trans = self._new((B, 4)), self._new((B, 3))
-        if zoom_depth_observed is None and zoom_depth_rendered is None:
-            check(lib.dim_net_fwd(self._h, _p(zoom_image_observed), _p(zoom_image_rendered), _p(zoom_mask_observed),
-                                  _p(zoom_mask_rendered), B, precision, _p(rot), _p(trans), self._stream()))
-            return rot, trans
-        shp = (B, 1, self.H, self.W)
-        _chk(zoom_depth_observed, torch.float32, shp, "zoom_depth_observed")
-        _chk(zoom_depth_rendered, torch.float32, shp, "zoom_depth_rendered")
-        check(lib.dim_net_fwd_rgbd(self._h, _p(zoom_image_observed), _p(zoom_image_rendered), _p(zoom_depth_observed),
-                                   _p(zoom_depth_rendered), _p(zoom_mask_observed), _p(zoom_mask_rendered), B, precision,
-                                   _p(rot), _p(trans), self._stream()))
+        check(lib.dim_net_fwd(self._h, _p(zoom_image_observed), _p(zoom_image_rendered), _p(zoom_depth_observed),
+                              _p(zoom_depth_rendered), _p(zoom_mask_observed), _p(zoom_mask_rendered), B, precision,
+                              _p(rot), _p(trans), self._stream()))
         return rot, trans
 
     def debug_activation(self, idx, B, lo=False, fp16=False):
@@ -479,17 +472,13 @@ class Context:
             bbox = self._new((n_iter, B, 8), torch.int32)
         if pose_override is not None:
             _chk(pose_override, torch.float64, (n_iter, B, 3, 4), "pose_override")
-        args = (self._h, _p(image_observed), _p(cls_idx), _p(pose_init), B, n_iter,
-                farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
-                farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses), _p(se3), _p(zf), _p(bbox))
-        lit = None if lighting is None else _lighting_arg(lighting, (n_iter, B, 3), True)[0]
         if depth_observed is not None:
             _chk(depth_observed, torch.float32, (B, 1, self.H, self.W), "depth_observed")
-            check(lib.dim_refine_rgbd(*args, _p(depth_observed), None if lit is None else C.byref(lit), self._stream()))
-        elif lit is None:
-            check(lib.dim_refine(*args, self._stream()))
-        else:
-            check(lib.dim_refine_lit(*args, C.byref(lit), self._stream()))
+        lit = None if lighting is None else C.byref(_lighting_arg(lighting, (n_iter, B, 3), True)[0])
+        check(lib.dim_refine(self._h, _p(image_observed), _p(cls_idx), _p(pose_init), B, n_iter,
+                             farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
+                             farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses), _p(se3), _p(zf),
+                             _p(bbox), _p(depth_observed), lit, self._stream()))
         return {"poses": poses, "se3": se3, "zoom_factor": zf, "bbox": bbox}
 
     def refine_host(self, image_observed_u8, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
@@ -510,9 +499,7 @@ class Context:
             poses_out = np.empty((n_iter, B, 3, 4), np.float64)
         if se3_out is None:
             se3_out = np.empty((n_iter, B, 7), np.float32)
-        args = (self._h, hptr(image_observed_u8), hptr(cls_idx), hptr(pose_init), B, n_iter,
-                farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
-                farr(pixel_means_rgb, 3, C.c_double), precision, hptr(poses_out), hptr(se3_out))
+        dkeep = None
         if depth_observed_u16 is not None:
             if isinstance(depth_observed_u16, torch.Tensor):
                 if depth_observed_u16.is_cuda or depth_observed_u16.dtype != torch.uint16:
@@ -522,17 +509,12 @@ class Context:
                 dkeep = np.ascontiguousarray(depth_observed_u16, np.uint16)
             if tuple(dkeep.shape) != (B, self.H, self.W):
                 raise ValueError("depth_observed_u16: expected shape %s, got %s" % ((B, self.H, self.W), tuple(dkeep.shape)))
-            lit, _keep = (None, None) if lighting is None else _lighting_arg(lighting, (n_iter, B, 3), False)
-            fn = lib.dim_refine_host_rgbd if sync else lib.dim_refine_host_rgbd_async
-            check(fn(*args, hptr(dkeep), float(np.float32(depth_factor)), None if lit is None else C.byref(lit),
-                     self._stream()))
-        elif lighting is None:
-            fn = lib.dim_refine_host if sync else lib.dim_refine_host_async
-            check(fn(*args, self._stream()))
-        else:
-            lit, _keep = _lighting_arg(lighting, (n_iter, B, 3), False)
-            fn = lib.dim_refine_host_lit if sync else lib.dim_refine_host_lit_async
-            check(fn(*args, C.byref(lit), self._stream()))
+        lit, _keep = (None, None) if lighting is None else _lighting_arg(lighting, (n_iter, B, 3), False)
+        fn = lib.dim_refine_host if sync else lib.dim_refine_host_async
+        check(fn(self._h, hptr(image_observed_u8), hptr(cls_idx), hptr(pose_init), B, n_iter,
+                 farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision,
+                 hptr(poses_out), hptr(se3_out), None if dkeep is None else hptr(dkeep), float(np.float32(depth_factor)),
+                 None if lit is None else C.byref(lit), self._stream()))
         return poses_out, se3_out
 
 

@@ -19,12 +19,6 @@ from ._capi import check, lib
 NORMALIZE_FLOW = 20.0
 
 
-def _param_info(input_depth, input_mask=True):
-    if not input_mask:
-        return lib.dim_train_param_info_nomask
-    return lib.dim_train_param_info_rgbd if input_depth else lib.dim_train_param_info
-
-
 def _is_rgbd(weights) -> bool:
     return np.shape(weights["flow_conv1_weight"])[1:2] == (10,)
 
@@ -35,12 +29,12 @@ def _is_nomask(weights) -> bool:
 
 def param_table(input_depth=False, input_mask=True):
     """[(tensor name, numel)] in flat order, as the library reports it (dim_train_param_info; input_depth: the RGB-D
-    network's table, dim_train_param_info_rgbd, whose flow_conv1 is (64, 10, 7, 7); input_mask=False: the image-only
-    network's table, dim_train_param_info_nomask, whose flow_conv1 is (64, 6, 7, 7))."""
+    network's table, whose flow_conv1 is (64, 10, 7, 7); input_mask=False: the image-only network's table, whose
+    flow_conv1 is (64, 6, 7, 7))."""
     out = []
     for i in range(64):
         name, wn, bn = C.c_char_p(), C.c_int64(), C.c_int64()
-        if _param_info(input_depth, input_mask)(i, C.byref(name), C.byref(wn), C.byref(bn)) != 0:
+        if lib.dim_train_param_info(int(input_depth), int(input_mask), i, C.byref(name), C.byref(wn), C.byref(bn)) != 0:
             break
         out.append((name.value.decode() + "_weight", wn.value))
         if bn.value:
@@ -79,7 +73,7 @@ def tensor_sizes(input_depth=False, input_mask=True):
     out = []
     for i in range(64):
         nm, wn, bn = C.c_char_p(), C.c_int64(), C.c_int64()
-        if _param_info(input_depth, input_mask)(i, C.byref(nm), C.byref(wn), C.byref(bn)) != 0:
+        if lib.dim_train_param_info(int(input_depth), int(input_mask), i, C.byref(nm), C.byref(wn), C.byref(bn)) != 0:
             break
         out.append((i, wn.value + bn.value))
     return out
@@ -183,22 +177,21 @@ class Trainer:
         ctx = self.ctx
         B, N = z["zoom_image_observed"].shape[0], z["point_cloud_model"].shape[2]
         zmo, zmr = (z["zoom_mask_observed"], z["zoom_mask_rendered"]) if self.input_mask else (None, None)
+        zdo, zdr = (z["zoom_depth_observed"], z["zoom_depth_rendered"]) if self.input_depth else (None, None)
         for k, t in z.items():
             if t.dtype != torch.float32 or not t.is_contiguous() or not t.is_cuda:
                 raise TypeError("%s must be a contiguous float32 CUDA tensor" % k)
         out = {"rot_est_norm": ctx._new((B, 4)), "trans_est": ctx._new((B, 3)), "losses": ctx._new((4,)),
                "flow_est": ctx._new((B, 2, ctx.H, ctx.W)) if want_maps else None,
                "mask_prob": ctx._new((B, 1, ctx.H, ctx.W)) if want_maps else None}
-        args = (ctx._h, _p(z["zoom_image_observed"]), _p(z["zoom_image_rendered"]), _p(zmo), _p(zmr), _p(z["zoom_factor"]), _p(z["zoom_flow"]), _p(z["zoom_flow_weights"]),
-                _p(z["zoom_mask_gt_observed"]), _p(z["src_pose"]), _p(z["point_cloud_model"]), _p(z["point_cloud_weights"]),
-                _p(z["point_cloud_observed"]), B, N, _p(out["rot_est_norm"]), _p(out["trans_est"]), _p(out["flow_est"]),
-                _p(out["mask_prob"]), _p(out["losses"]), _p(self.grads) if backward else None, None,
-                *((self._bucket_events() + (len(self.buckets),)) if (backward and overlap) else (None, None, 0)))
-        if self.input_depth:
-            check(lib.dim_train_forward_backward_rgbd(*args, _p(z["zoom_depth_observed"]), _p(z["zoom_depth_rendered"]),
-                                                      self._stream()))
-        else:
-            check(lib.dim_train_forward_backward(*args, self._stream()))
+        check(lib.dim_train_forward_backward(
+            ctx._h, _p(z["zoom_image_observed"]), _p(z["zoom_image_rendered"]), _p(zmo), _p(zmr), _p(z["zoom_factor"]),
+            _p(z["zoom_flow"]), _p(z["zoom_flow_weights"]), _p(z["zoom_mask_gt_observed"]), _p(z["src_pose"]),
+            _p(z["point_cloud_model"]), _p(z["point_cloud_weights"]), _p(z["point_cloud_observed"]), B, N,
+            _p(out["rot_est_norm"]), _p(out["trans_est"]), _p(out["flow_est"]), _p(out["mask_prob"]), _p(out["losses"]),
+            _p(self.grads) if backward else None, None,
+            *((self._bucket_events() + (len(self.buckets),)) if (backward and overlap) else (None, None, 0)),
+            _p(zdo), _p(zdr), self._stream()))
         return out
 
     def test_forward_full(self, batch, K):
@@ -220,7 +213,7 @@ class Trainer:
         zflow, zprob = ctx._new((B, 2, ctx.H, ctx.W)), ctx._new((B, 1, ctx.H, ctx.W))
         check(lib.dim_train_forward_backward(ctx._h, _p(zio), _p(zir), _p(zo), _p(zr), _p(zf), None, None, None, None, None, None,
                                              None, B, 0, None, _p(trans), _p(zflow), _p(zprob), None, None, _p(rot), None, None, 0,
-                                             self._stream()))
+                                             None, None, self._stream()))
         mask_pred = torch.round(ctx.zoom_mask_with_factor(zf, zprob, True))
         flow_est, _ = ctx.zoom_flow(zf, zflow, None, True)
         return {"se3": torch.cat([rot, trans], dim=1), "zoom_factor": zf, "mask_observed_pred": mask_pred, "flow_est": flow_est,

@@ -15,7 +15,7 @@ def declared_symbols(root):
     return sorted(set(re.findall(r"DIM_API\s+[\w\s\*]+?\b(dim_\w+)\s*\(", txt)))
 
 
-def test_library_exports_every_declared_symbol(root):
+def test_library_exports_every_declared_symbol_at_abi_3(root):
     so = os.path.join(root, "mx-deepim_b200", "libdeepim_b200.so")
     assert os.path.exists(so), "run python __graft_entry__.py (build) first"
     lib = ctypes.CDLL(so)
@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol(root):
     for s in syms:
         assert hasattr(lib, s), "symbol %s declared in the header but not exported" % s
     lib.dim_abi_version.restype = ctypes.c_int32
-    assert lib.dim_abi_version() == 2
+    assert lib.dim_abi_version() == 3
 
 
 def test_library_is_sm90a_native_wgmma_and_tma(root):
@@ -79,6 +79,43 @@ def test_train_config_struct_layout_matches_the_header(root, tmp_path):
 def test_ctypes_binding_covers_the_header(root):
     from deepim_b200 import _capi
     assert sorted(_capi.SIGNATURES) == declared_symbols(root)
+
+
+def header_prototypes(root):
+    """{name: (return type, [parameter declarations])} of every function the header declares"""
+    txt = open(os.path.join(root, "include", "deepim_b200.h")).read()
+    txt = re.sub(r"/\*.*?\*/", "", txt, flags=re.S)
+    return {m.group(2): (" ".join(m.group(1).split()), [" ".join(p.split()) for p in m.group(3).split(",")])
+            for m in re.finditer(r"DIM_API\s+([\w\s\*]+?)\b(dim_\w+)\s*\(([^)]*)\)", txt)}
+
+
+@pytest.mark.parametrize("fn", declared_symbols(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+def test_ctypes_prototypes_match_the_header(root, fn):
+    """Return kind, argument count and argument kinds (pointer / 32-bit int / 64-bit int / 64-bit unsigned / float) of each
+    entry in _capi.SIGNATURES equal the header's prototype: a wrong argtypes list would misread the call's arguments
+    without any error."""
+    import ctypes as C
+    from deepim_b200 import _capi
+    ret, params = header_prototypes(root)[fn]
+    restype, argtypes = _capi.SIGNATURES[fn]
+    if params == ["void"]:
+        params = []
+
+    def kind_c(decl):
+        if "*" in decl:
+            return "ptr"
+        return {"void": "void", "int32_t": "i32", "int64_t": "i64", "uint64_t": "u64", "float": "f32"}[decl.split()[0]]
+
+    def kind_py(t):
+        if t is None:
+            return "void"
+        if t in (C.c_void_p, C.c_char_p) or issubclass(t, C._Pointer):
+            return "ptr"
+        return {C.c_int32: "i32", C.c_int64: "i64", C.c_uint64: "u64", C.c_float: "f32"}[t]
+
+    assert kind_c(ret) == kind_py(restype), (fn, ret)
+    assert len(argtypes) == len(params), (fn, params)
+    assert [kind_c(p) for p in params] == [kind_py(t) for t in argtypes], fn
 
 
 def test_no_cpu_fallback_ctx_create_fails_loudly_without_gpu(root):
@@ -233,6 +270,11 @@ def test_trainer_flat_parameter_layout():
             f6 = flat[off:off + n].reshape(256, 80, 1024)
             assert f6[5, 17, 300] == w["fc6_weight"][5, 300 * 80 + 17]
         off += n
+    # depth input without the mask channels is no network of this library: its table is refused, as the context switches are
+    from deepim_b200 import _capi
+    name, wn, bn = ctypes.c_char_p(), ctypes.c_int64(), ctypes.c_int64()
+    assert _capi.lib.dim_train_param_info(1, 0, 0, ctypes.byref(name), ctypes.byref(wn), ctypes.byref(bn)) != 0
+    assert b"input_mask = 0" in _capi.lib.dim_last_error()
 
 
 def test_simpson_rule_and_obj_parser(tmp_path):

@@ -1,5 +1,5 @@
 """GPU: the ModelNet (unseen-object) branch of the test and train loops -- the fused refinement loop and the train-time
-batch update with the Lambert-lit renderer (dim_refine_lit, dim_refine_host_lit, dim_train_update_lit) against the lit CPU
+batch update with the Lambert-lit renderer (dim_refine, dim_refine_host, dim_train_update with a dim_lighting) against the lit CPU
 checker (tests/lit_oracle.py, built on the oracle), against the unlit calls where the light is neutral, and through the
 Python layers (PoseRefiner, trainer)."""
 import numpy as np
@@ -100,8 +100,8 @@ def test_lit_refine_free_running_fp16(ctx, case):
 
 
 def test_neutral_light_gives_the_unlit_loop_bit_for_bit(ctx, case):
-    """brightness_ratio 0 and unit intensity: round(texel) = the uint8-truncated unlit colour, so dim_refine_lit computes what
-    dim_refine computes, bit for bit."""
+    """brightness_ratio 0 and unit intensity: round(texel) = the uint8-truncated unlit colour, so the lit dim_refine computes what
+    the unlit one computes, bit for bit."""
     c = case
     args = (dev(c["img"]), dev(c["cls"]), dev(c["ini"]), K, N_ITER)
     unlit = ctx.refine(*args, pixel_means_rgb=MEANS)
@@ -210,7 +210,7 @@ def test_lit_train_update_matches_oracle(ctx, meshes):
     assert np.abs(out["flow"].cpu().numpy() - ref["flow"])[np.repeat(both, 2, 1)].max() < 2e-3
 
 
-def test_lit_calls_refuse_missing_normals_and_null_intensity(ctx, case):
+def test_lighting_refuses_missing_normals_and_null_intensity(ctx, case):
     import ctypes as C
     from deepim_b200._capi import lib
     c = case
@@ -228,20 +228,19 @@ def test_lit_calls_refuse_missing_normals_and_null_intensity(ctx, case):
                               lighting=lit(torch.ones(2, 3, device=DEV)))
     finally:
         bare.close()
-    # NULL lighting / NULL intensity through the C ABI
+    # NULL intensity through the C ABI (NULL lighting is the unlit loop)
     B = c["B"]
     img, cls, ini = dev(c["img"]), dev(c["cls"]), dev(c["ini"])
     poses = torch.empty(N_ITER, B, 3, 4, dtype=torch.float64, device=DEV)
     K9 = capi.farr(K.reshape(9), 9)
     means = capi.farr(MEANS, 3, C.c_double)
     null_int = capi.Lighting(None, (C.c_double * 3)(0.0, 0.5, 0.5), 0.7)
-    for lp in (None, C.byref(null_int)):
-        rc = lib.dim_refine_lit(ctx._h, C.c_void_p(img.data_ptr()), C.c_void_p(cls.data_ptr()), C.c_void_p(ini.data_ptr()), B,
-                                N_ITER, K9, 0.25, 6.0, means, capi.PREC_FP16, None, C.c_void_p(poses.data_ptr()), None, None, None,
-                                lp, None)
-        assert rc != 0 and b"NULL" in lib.dim_last_error()
-        with pytest.raises(capi.DeepIMError):
-            capi.check(rc)
+    rc = lib.dim_refine(ctx._h, C.c_void_p(img.data_ptr()), C.c_void_p(cls.data_ptr()), C.c_void_p(ini.data_ptr()), B, N_ITER,
+                        K9, 0.25, 6.0, means, capi.PREC_FP16, None, C.c_void_p(poses.data_ptr()), None, None, None, None,
+                        C.byref(null_int), None)
+    assert rc != 0 and b"NULL" in lib.dim_last_error()
+    with pytest.raises(capi.DeepIMError):
+        capi.check(rc)
     with pytest.raises(ValueError):
         ctx.refine(img, cls, ini, K, N_ITER, lighting={"offset": (0, 0.5, 0.5)})  # no intensity
 

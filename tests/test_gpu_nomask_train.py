@@ -118,13 +118,13 @@ def test_gradients_equal_the_eight_channel_step_with_zero_mask_columns(setup):
         c8.close()
 
 
-def test_nomask_training_entry_refuses_masks(setup):
+def test_nomask_training_step_refuses_masks(setup):
     meshes, w, batch, ctx, tr = setup
     z = tr.zoom_front(device_batch(batch), K)
     args = [ctx._h] + [capi.C.c_void_p(z[k].data_ptr()) for k in
                        ("zoom_image_observed", "zoom_image_rendered", "zoom_mask_observed", "zoom_mask_rendered", "zoom_factor")]
     args += [None] * 7 + [B, 0] + [None] * 7 + [None, None, 0]
-    rc = capi.lib.dim_train_forward_backward(*args, None)
+    rc = capi.lib.dim_train_forward_backward(*args, None, None, None)
     assert rc != 0 and b"takes no mask input" in capi.lib.dim_last_error()
     with pytest.raises(ValueError, match="input channels"):
         Trainer(ctx, synth.make_train_weights(0))

@@ -1,5 +1,5 @@
-"""GPU: the RGB-D network (config.network.INPUT_DEPTH) in the fused refinement loop and on the op surface -- dim_refine_rgbd,
-dim_refine_host_rgbd and dim_net_fwd_rgbd against the RGB-D CPU checker (tests/depth_oracle.py), against the RGB context
+"""GPU: the RGB-D network (config.network.INPUT_DEPTH) in the fused refinement loop and on the op surface -- dim_refine,
+dim_refine_host and dim_net_fwd of an RGB-D context against the RGB-D CPU checker (tests/depth_oracle.py), against the RGB context
 where the depth weights are zero, and the error paths of the mode switch."""
 import ctypes as C
 
@@ -231,25 +231,31 @@ def test_net_fwd_rgbd_matches_the_checker(ctx, weights, case, prec):
     assert np.abs(trans.cpu().numpy() - tr).max() < 1e-3
 
 
-def test_error_paths(meshes, weights, case):
+def test_depth_arguments_follow_the_network_error_paths(meshes, weights, case):
     c = case
     w8 = synth.make_weights(0)
     rgb = make_ctx(meshes, w8, False)
     rgbd = make_ctx(meshes, weights)
     try:
         args = (dev(c["img"][:2]), dev(c["cls"][:2]), dev(c["ini"][:2]), K, 1)
-        with pytest.raises(capi.DeepIMError, match="dim_refine_rgbd"):
+        with pytest.raises(capi.DeepIMError, match="takes depth input.*depth_observed"):
             rgbd.refine(*args, pixel_means_rgb=MEANS)
         with pytest.raises(capi.DeepIMError, match="takes no depth input"):
             rgb.refine(*args, pixel_means_rgb=MEANS, depth_observed=dev(c["depth"][:2]))
-        with pytest.raises(capi.DeepIMError, match="dim_refine_host_rgbd"):
+        with pytest.raises(capi.DeepIMError, match="takes depth input.*depth_observed_u16_host"):
             rgbd.refine_host(c["u8"][:2], c["cls"][:2], c["ini"][:2], K, 1, pixel_means_rgb=MEANS)
-        with pytest.raises(capi.DeepIMError, match="dim_net_fwd_rgbd"):
-            z = c["ref"]["inputs"][0]
+        with pytest.raises(capi.DeepIMError, match="takes no depth input"):
+            rgb.refine_host(c["u8"][:2], c["cls"][:2], c["ini"][:2], K, 1, pixel_means_rgb=MEANS,
+                            depth_observed_u16=c["u16"][:2])
+        z = c["ref"]["inputs"][0]
+        with pytest.raises(capi.DeepIMError, match="takes depth input.*zoom_depth_observed"):
             rgbd.net_forward(dev(z["zio"][:2]), dev(z["zir"][:2]), dev(z["zmo"][:2]), dev(z["zmr"][:2]))
+        with pytest.raises(capi.DeepIMError, match="takes no depth input"):
+            rgb.net_forward(dev(z["zio"][:2]), dev(z["zir"][:2]), dev(z["zmo"][:2]), dev(z["zmr"][:2]),
+                            zoom_depth_observed=dev(z["zdo"][:2]), zoom_depth_rendered=dev(z["zdr"][:2]))
         # NULL depth
         poses = torch.empty((1, 2, 3, 4), dtype=torch.float64, device=DEV)
-        rc = capi.lib.dim_refine_rgbd(rgbd._h, C.c_void_p(args[0].data_ptr()), C.c_void_p(args[1].data_ptr()),
+        rc = capi.lib.dim_refine(rgbd._h, C.c_void_p(args[0].data_ptr()), C.c_void_p(args[1].data_ptr()),
                                       C.c_void_p(args[2].data_ptr()), 2, 1, capi.farr(np.asarray(K, np.float32).reshape(9), 9),
                                       0.25, 6.0, capi.farr(MEANS, 3, C.c_double), capi.PREC_FP16, None,
                                       C.c_void_p(poses.data_ptr()), None, None, None, None, None, None)
@@ -266,8 +272,8 @@ def test_error_paths(meshes, weights, case):
         z1 = torch.zeros((2, 1, H, W), device=DEV)
         zf = torch.tensor([[1.0, 1.0, 0.0, 0.0]] * 2, device=DEV)
         p = lambda t: C.c_void_p(t.data_ptr())
-        rc = capi.lib.dim_train_forward_backward_rgbd(rgb._h, p(zb), p(zb), p(z1), p(z1), p(zf), *([None] * 7), 2, 0,
-                                                      *([None] * 7), None, None, 0, p(z1), p(z1), None)
+        rc = capi.lib.dim_train_forward_backward(rgb._h, p(zb), p(zb), p(z1), p(z1), p(zf), *([None] * 7), 2, 0,
+                                                 *([None] * 7), None, None, 0, p(z1), p(z1), None)
         assert rc != 0 and b"takes no depth input" in capi.lib.dim_last_error()
         # and the switch is refused once the context trains
         t = Context(0, max_batch=2, max_classes=1, max_verts=6000, max_faces=11000)

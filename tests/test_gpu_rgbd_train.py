@@ -1,4 +1,4 @@
-"""GPU: the training step of the RGB-D network (dim_train_forward_backward_rgbd) against the RGB-D train checker
+"""GPU: the training step of the RGB-D network (dim_train_forward_backward on an RGB-D context) against the RGB-D train checker
 (tests/depth_oracle.train_forward_backward, train_oracle.graph with the 10-channel input), its parameter table, and
 fit_batch carrying the re-render's depth.  Bounds as tests/test_gpu_train.py (bf16 mixed-precision step, fp32 checker)."""
 import os
@@ -92,7 +92,7 @@ def test_rgbd_training_step_matches_the_checker(setup):
     assert c["cos"] > 0.995 and np.abs(g["flow_conv1_weight"][:, 6:8]).max() > 0, c
 
 
-def test_rgbd_and_rgb_training_entries_refuse_the_other_network(setup):
+def test_training_step_refuses_depth_the_network_does_not_take(setup):
     meshes, w, batch, ctx, tr = setup
     b = {k: dev(v) for k, v in batch.items()}
     b["pixel_means_rgb"] = MEANS.astype(np.float32)
@@ -100,8 +100,8 @@ def test_rgbd_and_rgb_training_entries_refuse_the_other_network(setup):
     args = [ctx._h] + [capi.C.c_void_p(z[k].data_ptr()) for k in
                        ("zoom_image_observed", "zoom_image_rendered", "zoom_mask_observed", "zoom_mask_rendered", "zoom_factor")]
     args += [None] * 7 + [B, 0] + [None] * 7 + [None, None, 0]
-    rc = capi.lib.dim_train_forward_backward(*args, None)
-    assert rc != 0 and b"dim_train_forward_backward_rgbd" in capi.lib.dim_last_error()
+    rc = capi.lib.dim_train_forward_backward(*args, None, None, None)
+    assert rc != 0 and b"takes depth input" in capi.lib.dim_last_error()
     with pytest.raises(ValueError, match="input channels"):
         Trainer(ctx, synth.make_train_weights(0))
 

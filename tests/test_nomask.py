@@ -1,9 +1,7 @@
 """CPU: the image-only network's host-side pieces (config.network.INPUT_MASK: False) -- the CPU checker's ZoomImage against the
-reference operator's fixture, its 6-channel tower, the parameter table, the 6-channel checkpoint and weight helpers, and the
-ctypes prototypes of the new entries."""
+reference operator's fixture, its 6-channel tower, the parameter table, the 6-channel checkpoint and weight helpers."""
 import hashlib
 import os
-import re
 import sys
 
 import numpy as np
@@ -73,7 +71,7 @@ def test_weights_and_six_channel_checkpoint_round_trip(tmp_path):
 
 
 def test_library_reports_the_nomask_parameter_table():
-    """dim_train_param_info_nomask: the RGB table with flow_conv1_weight (64, 6, 7, 7), 6 272 floats fewer: 57 742 892."""
+    """dim_train_param_info(input_mask=0): the RGB table with flow_conv1_weight (64, 6, 7, 7), 6 272 floats fewer: 57 742 892."""
     from deepim_b200.trainer import flatten_params, param_table, tensor_sizes, unflatten_params
     rgb, nm = param_table(), param_table(input_mask=False)
     assert [k for k, _ in rgb] == [k for k, _ in nm]
@@ -88,22 +86,3 @@ def test_library_reports_the_nomask_parameter_table():
     for k in w:
         assert np.array_equal(back[k], w[k]), k
 
-
-def _c_params(root, fn):
-    txt = open(os.path.join(root, "include", "deepim_b200.h")).read()
-    txt = re.sub(r"/\*.*?\*/", "", txt, flags=re.S)
-    m = re.search(r"DIM_API\s+[\w\s\*]+?\b%s\s*\(([^)]*)\)" % fn, txt)
-    assert m, fn
-    return [" ".join(p.split()) for p in m.group(1).split(",")]
-
-
-@pytest.mark.parametrize("fn", ["dim_ctx_set_input_mask", "dim_train_param_info_nomask"])
-def test_nomask_ctypes_prototypes_match_the_header(root, fn):
-    import ctypes as C
-    from deepim_b200 import _capi
-    params = _c_params(root, fn)
-    _, argtypes = _capi.SIGNATURES[fn]
-    assert len(argtypes) == len(params), (fn, params)
-    kind_c = lambda p: "ptr" if "*" in p else {"int32_t": "i32", "int64_t": "i64", "float": "f32"}[p.split()[0]]
-    kind_py = lambda t: {C.c_int32: "i32", C.c_int64: "i64", C.c_float: "f32"}.get(t, "ptr")
-    assert [kind_c(p) for p in params] == [kind_py(t) for t in argtypes], fn

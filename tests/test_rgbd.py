@@ -111,7 +111,7 @@ def test_rgbd_conv1_kernel_is_wgmma_and_tma(root):
 
 
 def test_library_reports_the_rgbd_parameter_table():
-    """dim_train_param_info_rgbd: the RGB table with flow_conv1_weight (64, 10, 7, 7), 6 272 floats more."""
+    """dim_train_param_info(input_depth=1): the RGB table with flow_conv1_weight (64, 10, 7, 7), 6 272 floats more."""
     from deepim_b200.trainer import param_table, flatten_params, unflatten_params
     rgb, rgbd = param_table(False), param_table(True)
     assert [k for k, _ in rgb] == [k for k, _ in rgbd]
@@ -125,38 +125,3 @@ def test_library_reports_the_rgbd_parameter_table():
     for k in w:
         assert np.array_equal(back[k], w[k]), k
 
-
-def _c_params(root, fn):
-    txt = open(os.path.join(root, "include", "deepim_b200.h")).read()
-    txt = re.sub(r"/\*.*?\*/", "", txt, flags=re.S)
-    m = re.search(r"DIM_API\s+[\w\s\*]+?\b%s\s*\(([^)]*)\)" % fn, txt)
-    assert m, fn
-    return [" ".join(p.split()) for p in m.group(1).split(",")]
-
-
-@pytest.mark.parametrize("fn", ["dim_ctx_set_input_depth", "dim_refine_rgbd", "dim_refine_host_rgbd", "dim_refine_host_rgbd_async",
-                                "dim_net_fwd_rgbd", "dim_train_param_info_rgbd", "dim_train_forward_backward_rgbd"])
-def test_rgbd_ctypes_prototypes_match_the_header(root, fn):
-    """Argument count and kind (pointer / 32-bit int / 64-bit int / float) of each RGB-D entry in _capi.SIGNATURES equal the
-    header's prototype."""
-    import ctypes as C
-    from deepim_b200 import _capi
-    params = _c_params(root, fn)
-    _, argtypes = _capi.SIGNATURES[fn]
-    assert len(argtypes) == len(params), (fn, params)
-
-    def kind_c(p):
-        if "*" in p:
-            return "ptr"
-        return {"int32_t": "i32", "int64_t": "i64", "float": "f32"}[p.split()[0]]
-
-    def kind_py(t):
-        if t in (C.c_int32,):
-            return "i32"
-        if t in (C.c_int64,):
-            return "i64"
-        if t in (C.c_float,):
-            return "f32"
-        return "ptr"
-
-    assert [kind_c(p) for p in params] == [kind_py(t) for t in argtypes], fn

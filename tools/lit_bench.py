@@ -3,8 +3,8 @@
     python tools/lit_bench.py [--steps 10] [--warmup 2] [--rounds 2] [--batch 16] [--slots 4]
 
 Same inputs, pass shape and precision (fp16) as bench.py's device-resident `value`: one step = 32 device batches of `batch`
-instances, `slots` batches in flight on as many contexts / streams, 3 rotating input sets.  The lit loop is dim_refine_lit
-(Lambert-lit render; light = (0, .5, .5) + (t_x, -t_y, -t_z) of the float64 pose, brightness ratio 0.7), normals from
+instances, `slots` batches in flight on as many contexts / streams, 3 rotating input sets.  The lit loop is dim_refine with
+a dim_lighting (Lambert-lit render; light = (0, .5, .5) + (t_x, -t_y, -t_z) of the float64 pose, brightness ratio 0.7), normals from
 synth.vertex_normals, light intensities [4, batch, 3] drawn once from default_rng(2024).  The unlit and lit passes alternate
 `rounds` times so that clock drift under a power cap hits both alike; the best round of each is reported, plus the stage
 times (render / zoom / conv / head) of a single-stream pass with CUDA events between the stages.  Random-init weights: the

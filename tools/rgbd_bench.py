@@ -4,8 +4,8 @@
 
 Same inputs, pass shape and precision (fp16) as bench.py's device-resident `value`: one step = 32 device batches of `batch`
 instances, `slots` batches in flight on as many contexts / streams, 3 rotating input sets.  The RGB passes run dim_refine on
-RGB contexts, the RGB-D passes dim_refine_rgbd on RGB-D contexts (Context(input_depth=True)) with a fixed observed depth
-per input set.  The two alternate `rounds` times so that clock drift under a power cap hits both alike; the best round of
+RGB contexts, the RGB-D passes dim_refine on RGB-D contexts (Context(input_depth=True)) with a fixed observed depth per
+input set.  The two alternate `rounds` times so that clock drift under a power cap hits both alike; the best round of
 each is reported, plus the stage times (render / zoom / conv / head) of a single-stream pass with CUDA events between the
 stages and the per-layer conv times of one forward pass.  Random-init weights: the timed work does not depend on the weight
 or depth values.  Prints one JSON line."""
