@@ -5,10 +5,15 @@ deepim_oracle.c), the FlowNetS forward in torch-CPU fp32 and the test-time itera
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference leg may
 import this module.  The product package never does (tests/test_no_oracle_in_product.py).
 
+The network variants are arguments, as on the device: the lit render of the ModelNet branch (`lighting`), the RGB-D
+network (the depths) and the image-only network (no masks).  The light and depth helpers restate the reference
+independently of the product's deepim_b200.lighting; tests/test_lighting.py compares the two.
+
 Reference anchors:
   net            deepim/symbols/deepIM_flownet.py:32-118 (get_convs), 715-726 (heads)
   iteration glue deepim/core/tester.py:340-485, lib/pair_matching/data_pair.py:66-129,
                  lib/utils/image.py:583-594
+  lit render     deepim/core/tester.py:146-188, lib/pair_matching/batch_updater_py_multi.py:187-235
   ADD / ADI      lib/utils/pose_error.py:72-108
 """
 from __future__ import annotations
@@ -63,6 +68,12 @@ def lib():
 
 
 ROT_COORD = {"model": 0, "camera": 1, "camera_new": 2}
+# FlowNetS encoder (deepIM_flownet.py:32-105): name, stride, padding
+ENC = [("flow_conv1", 2, 3), ("conv2", 2, 2), ("conv3", 2, 2), ("conv3_1", 1, 1), ("conv4", 2, 1),
+       ("conv4_1", 1, 1), ("conv5", 2, 1), ("conv5_1", 1, 1), ("conv6", 2, 1), ("conv6_1", 1, 1)]
+# the ModelNet branch's light: offset of light index 2 and Render_Py_Light_ModelNet_Multi's brightness ratio
+OFFSET = (0.0, 0.5, 0.5)
+BRIGHTNESS_RATIO = 0.7
 
 
 def _ptr(a):
@@ -114,6 +125,31 @@ def render_lit(mesh, normals, pose, K, light_position, light_intensity, brightne
                          _ptr(out["bgr"]), _ptr(out["depth"]), _ptr(out["image"]), _ptr(out["mask"]), _ptr(bbox))
     out["bbox"] = bbox
     return out
+
+
+def light_position(pose, offset=OFFSET):
+    """The light of the ModelNet branch's renders (tester.py:146-160) on the float64 pose being rendered, cast to float32
+    at the end like the glumpy uniform:
+        light_position = np.array([0, 1, 1]) * 0.5
+        light_position[0] += pose[0, 3]; light_position[1] -= pose[1, 3]; light_position[2] -= pose[2, 3]"""
+    light = np.array(offset, dtype=np.float64)
+    pose = np.asarray(pose, dtype=np.float64)
+    light[0] += pose[0, 3]
+    light[1] -= pose[1, 3]
+    light[2] -= pose[2, 3]
+    return light.astype(np.float32)
+
+
+def _render_lit(mesh, pose, K, intensity, lighting, zn, zf, H, W, means_rgb, want):
+    """render_lit at the light of `pose`; lighting = {"offset", "brightness_ratio"} (defaults OFFSET, BRIGHTNESS_RATIO),
+    the mesh carries `normals`."""
+    return render_lit(mesh, mesh.normals, pose, K, light_position(pose, lighting.get("offset", OFFSET)), intensity,
+                      lighting.get("brightness_ratio", BRIGHTNESS_RATIO), zn, zf, H, W, means_rgb, want)
+
+
+def depth_from_u16(u16, depth_factor=1000.0):
+    """lib/utils/image.py:203,218: a float32 array divided by a Python float stays float32 (float32-rounded factor)."""
+    return np.asarray(u16).astype(np.float32) / depth_factor
 
 
 # -------------------------------------------------------------------------------------------- zoom
@@ -279,10 +315,23 @@ def flow(depth_src, depth_tgt, KT, Kinv):
 
 
 # --------------------------------------------------------------------------------------------- net
-def net_forward(weights, zoom_image_observed, zoom_image_rendered, zoom_mask_observed, zoom_mask_rendered,
-                num_threads=None, return_features=False, emulate_bf16=False, emulate_fp16=False):
-    """FlowNetS encoder + fc + heads, torch-CPU fp32 (deepIM_flownet.py:53-116, 716-717).
-    Returns rot (B,4) raw quaternion, trans (B,3) zoomed translation.
+def conv1_input(zio, zir, zdo=None, zdr=None, zmo=None, zmr=None):
+    """conv1's input (B,C,H,W) float32 numpy in the symbol's channel order (deepIM_flownet.py:33-62): the zoomed images
+    / 255, the zoomed depths / 255 (INPUT_DEPTH), the zoomed masks (INPUT_MASK); a blob the network does not take is None.
+    The divisions are the graph's correctly rounded float32 ones, done by torch's multithreaded CPU kernel (numpy's
+    single-threaded division would add ~1 ms to each batch-1 forward of bench.py's reference leg)."""
+    import torch
+
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))
+    scaled = [t(a) / 255.0 for a in (zio, zir, zdo, zdr) if a is not None]
+    return torch.cat(scaled + [t(a) for a in (zmo, zmr) if a is not None], dim=1).numpy()
+
+
+def net_forward(weights, zio, zir, zmo=None, zmr=None, num_threads=None, return_features=False, emulate_bf16=False,
+                emulate_fp16=False, *, zdo=None, zdr=None):
+    """FlowNetS encoder + fc + heads, torch-CPU fp32 (deepIM_flownet.py:53-116, 716-717) on the zoomed blobs:
+    without masks the image-only network, with depths the RGB-D network (flow_conv1_weight must have conv1_input's
+    channels).  Returns rot (B,4) raw quaternion, trans (B,3) zoomed translation.
     emulate_bf16=True rounds what the device's throughput mode (DIM_PREC_BF16) stores in bf16 -- the conv / fc6 operand
     weights and every conv activation -- keeping fp32 accumulation: calibrates that mode's tolerance (tests).
     emulate_fp16=True does the same for DIM_PREC_FP16 (IEEE half storage, 11 significant bits)."""
@@ -294,12 +343,9 @@ def net_forward(weights, zoom_image_observed, zoom_image_rendered, zoom_mask_obs
     from_np = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))
     with torch.no_grad():
         rb = (lambda t: t.bfloat16().float()) if emulate_bf16 else ((lambda t: t.half().float()) if emulate_fp16 else (lambda t: t))
-        x = rb(torch.cat([from_np(zoom_image_observed) / 255.0, from_np(zoom_image_rendered) / 255.0,
-                          from_np(zoom_mask_observed), from_np(zoom_mask_rendered)], dim=1))
+        x = rb(torch.from_numpy(conv1_input(zio, zir, zdo, zdr, zmo, zmr)))
         feats = {}
-        specs = [("flow_conv1", 2, 3), ("conv2", 2, 2), ("conv3", 2, 2), ("conv3_1", 1, 1), ("conv4", 2, 1),
-                 ("conv4_1", 1, 1), ("conv5", 2, 1), ("conv5_1", 1, 1), ("conv6", 2, 1), ("conv6_1", 1, 1)]
-        for name, s, p in specs:
+        for name, s, p in ENC:
             x = F.conv2d(x, rb(from_np(weights[name + "_weight"])), from_np(weights[name + "_bias"]), stride=s, padding=p)
             x = rb(F.leaky_relu(x, 0.1))
             if return_features:
@@ -319,46 +365,79 @@ def net_forward(weights, zoom_image_observed, zoom_image_rendered, zoom_mask_obs
 
 
 # ------------------------------------------------------------------------------------------- chain
-def test_forward(weights, image_observed, image_rendered, mask_observed, mask_rendered, src_pose, K, means_rgb):
-    """One pass of the FAST_TEST graph (get_test_symbol_share, deepIM_flownet.py:548-735):
-    returns se3 (B,7), zoom_factor (B,4), bbox (B,8)."""
-    zmo, _, zmr, zf, bbox = zoom_mask(mask_observed, mask_observed, mask_rendered, src_pose, K)
-    zio, zir = zoom_image_with_factor(zf, image_observed, image_rendered, means_rgb)
-    rot, trans_z = net_forward(weights, zio, zir, zmo, zmr)
-    trans = zoom_trans(zf, trans_z, True)
-    return np.concatenate([rot, trans], axis=1).astype(np.float32), zf, bbox
+def test_forward(weights, image_observed, image_rendered, mask_observed, mask_rendered, src_pose, K, means_rgb,
+                 depth_observed=None, depth_rendered=None, return_inputs=False):
+    """One pass of the FAST_TEST graph (get_test_symbol_share, deepIM_flownet.py:548-735): returns se3 (B,7),
+    zoom_factor (B,4), bbox (B,8) and, with return_inputs, the zoomed blobs: dict zio, zir, zoom_factor, bbox, plus
+    zdo, zdr and zmo, zmr where the network takes them.
+    With masks the zoom is ZoomMask + ZoomImageWithFactor; without (image-only network, masks None) it is ZoomImage
+    (symbol:562-601).  Depths (RGB-D network) are zoomed with ZoomDepth (zoom_depth.py:24-44) by the same factor."""
+    z = {}
+    if mask_observed is None:
+        z["zio"], z["zir"], zf, bbox = zoom_image(image_observed, image_rendered, src_pose, K, means_rgb)
+    else:
+        z["zmo"], _, z["zmr"], zf, bbox = zoom_mask(mask_observed, mask_observed, mask_rendered, src_pose, K)
+        z["zio"], z["zir"] = zoom_image_with_factor(zf, image_observed, image_rendered, means_rgb)
+    if depth_observed is not None:
+        z["zdo"], z["zdr"] = zoom_depth(zf, depth_observed), zoom_depth(zf, depth_rendered)
+    rot, trans_z = net_forward(weights, z["zio"], z["zir"], z.get("zmo"), z.get("zmr"), zdo=z.get("zdo"), zdr=z.get("zdr"))
+    se3 = np.concatenate([rot, zoom_trans(zf, trans_z, True)], axis=1).astype(np.float32)
+    if return_inputs:
+        return se3, zf, bbox, dict(z, zoom_factor=zf, bbox=bbox)
+    return se3, zf, bbox
 
 
 def refine(weights, meshes, cls_idx, image_observed, pose_init, K, n_iter=4, means_rgb=None, zn=0.25, zf=6.0,
-           poses_override=None):
+           poses_override=None, *, lighting=None, depth_observed=None, input_mask=True, return_inputs=False):
     """Test-time refinement loop restated from deepim/core/tester.py:340-485 (SURVEY Appendix A).
     image_observed (B,3,H,W) float32 RGB-mean; pose_init (B,3,4).  The initial rendered blobs are the
     render at pose_init (the reference loads the same thing pre-rendered from disk).
     poses_override[it] (B,3,4), if given, replaces the pose fed to iteration `it` (teacher forcing for
     per-iteration parity tests).
-    Returns dict poses (n_iter,B,3,4) f64, se3 (n_iter,B,7) f32, zoom_factor (n_iter,B,4), bbox (n_iter,B,8)."""
+    lighting = {"intensity": float32 [n_iter,B,3], "offset", "brightness_ratio"}: the ModelNet branch's lit render, instance b
+    of iteration `it` with intensity[it, b] and the light of its float64 pose (every mesh carries `normals`).
+    depth_observed (B,1,H,W) float32 metres: the RGB-D network, fed the render's depth at the pose being refined
+    (tester.py:427,437-438; the depth of the lit render is the unlit one).
+    input_mask=False: the image-only network, zoomed with ZoomImage; the loop carries no masks (tester.py:439).
+    Returns dict poses (n_iter,B,3,4) f64, se3 (n_iter,B,7) f32, zoom_factor (n_iter,B,4), bbox (n_iter,B,8) and, with
+    return_inputs, "inputs": test_forward's zoomed blobs of each iteration."""
     B, _, H, W = image_observed.shape
     if means_rgb is None:
         means_rgb = np.array([103.939, 116.779, 123.68], np.float32)
+    want = ("image",) + (("depth",) if depth_observed is not None else ()) + (("mask",) if input_mask else ())
+    inten = None if lighting is None else np.asarray(lighting["intensity"], np.float32)
     pose = np.array(pose_init, dtype=np.float64)
     res = {"poses": np.zeros((n_iter, B, 3, 4)), "se3": np.zeros((n_iter, B, 7), np.float32),
            "zoom_factor": np.zeros((n_iter, B, 4), np.float32), "bbox": np.zeros((n_iter, B, 8), np.int32)}
+    if return_inputs:
+        res["inputs"] = []
     for it in range(n_iter):
         if poses_override is not None and poses_override[it] is not None:
             pose = np.array(poses_override[it], dtype=np.float64)
         img_r = np.empty((B, 3, H, W), np.float32)
-        m_r = np.empty((B, 1, H, W), np.float32)
-        m_o = np.empty((B, 1, H, W), np.float32)
+        d_r = np.empty((B, 1, H, W), np.float32) if depth_observed is not None else None
+        m_r, m_o = (np.empty((B, 1, H, W), np.float32), np.empty((B, 1, H, W), np.float32)) if input_mask else (None, None)
         for b in range(B):
-            r = render(meshes[int(cls_idx[b])], pose[b], K, zn, zf, H, W, means_rgb, True, want=("image", "mask"))
-            img_r[b], m_r[b, 0] = r["image"], r["mask"]
-            m_o[b, 0] = box_mask(r["bbox"], H, W)  # data_pair.py:93-105 (end-exclusive rectangle)
-        src_pose32 = pose.astype(np.float32)
-        se3, zfac, bbox = test_forward(weights, image_observed, img_r, m_o, m_r, src_pose32, K, means_rgb)
+            mesh = meshes[int(cls_idx[b])]
+            if lighting is None:
+                r = render(mesh, pose[b], K, zn, zf, H, W, means_rgb, True, want=want)
+            else:
+                r = _render_lit(mesh, pose[b], K, inten[it, b], lighting, zn, zf, H, W, means_rgb, want)
+            img_r[b] = r["image"]
+            if d_r is not None:
+                d_r[b, 0] = r["depth"]
+            if input_mask:
+                m_r[b, 0] = r["mask"]
+                m_o[b, 0] = box_mask(r["bbox"], H, W)  # data_pair.py:93-105 (end-exclusive rectangle)
+        out = test_forward(weights, image_observed, img_r, m_o, m_r, pose.astype(np.float32), K, means_rgb, depth_observed, d_r,
+                           return_inputs)
+        se3, zfac, bbox = out[:3]
         new_pose = np.zeros_like(pose)
         for b in range(B):
             new_pose[b] = rt_transform(pose[b], se3[b, :4], se3[b, 4:], (0, 0, 0), (1, 1, 1), "camera")
         res["poses"][it], res["se3"][it], res["zoom_factor"][it], res["bbox"][it] = new_pose, se3, zfac, bbox
+        if return_inputs:
+            res["inputs"].append(out[3])
         pose = new_pose
     return res
 
@@ -515,20 +594,30 @@ def calc_se3_f32(pose_src, pose_tgt):
 
 
 def train_update(meshes, cls_idx, src_pose, rot_est, trans_est, tgt_pose, depth_gt_observed, K, means_rgb,
-                 T_means=(0, 0, 0), T_stds=(1, 1, 1), rot_coord="camera", zn=0.25, zf=6.0):
+                 T_means=(0, 0, 0), T_stds=(1, 1, 1), rot_coord="camera", zn=0.25, zf=6.0, lighting=None):
     """batchUpdaterPyMulti.forward (lib/pair_matching/batch_updater_py_multi.py:91-328) for one context.
-    src_pose / tgt_pose / rot_est / trans_est are float32 (they come out of NDArrays)."""
+    src_pose / tgt_pose / rot_est / trans_est are float32 (they come out of NDArrays).
+    lighting = {"intensity": float32 [B,3], "offset", "brightness_ratio"}: the ModelNet branch, whose re-render is lit at the
+    float64 refined pose (l.187-229) and whose image is refined_image[:, :, [2,1,0]].transpose([2,0,1]).astype(np.float32)
+    - pixel_means in float32 (l.234-235); the unlit image is the render's, its means subtracted in float64."""
     B = len(cls_idx)
     H, W = depth_gt_observed.shape[-2:]
     out = {"image_rendered": np.zeros((B, 3, H, W), np.float32), "depth_rendered": np.zeros((B, 1, H, W), np.float32),
            "mask_rendered": np.zeros((B, 1, H, W), np.float32), "src_pose": np.zeros((B, 3, 4), np.float32),
            "rot": np.zeros((B, 4), np.float32), "trans": np.zeros((B, 3), np.float32)}
     KT = np.zeros((B, 3, 4), np.float32)
+    if lighting is not None:
+        inten, m32 = np.asarray(lighting["intensity"], np.float32), np.asarray(means_rgb, np.float32)
     for b in range(B):
         refined = rt_transform(src_pose[b].astype(np.float64), rot_est[b], trans_est[b], T_means, T_stds, rot_coord)
-        r = render(meshes[int(cls_idx[b])], refined, K, zn, zf, H, W, means_rgb, trunc_u8=False,
-                   want=("image", "depth", "mask"))
-        out["image_rendered"][b], out["depth_rendered"][b, 0], out["mask_rendered"][b, 0] = r["image"], r["depth"], r["mask"]
+        mesh = meshes[int(cls_idx[b])]
+        if lighting is None:
+            r = render(mesh, refined, K, zn, zf, H, W, means_rgb, trunc_u8=False, want=("image", "depth", "mask"))
+            out["image_rendered"][b] = r["image"]
+        else:
+            r = _render_lit(mesh, refined, K, inten[b], lighting, zn, zf, H, W, means_rgb, ("bgr", "depth", "mask"))
+            out["image_rendered"][b] = r["bgr"][:, :, [2, 1, 0]].transpose([2, 0, 1]).astype(np.float32) - m32[:, None, None]
+        out["depth_rendered"][b, 0], out["mask_rendered"][b, 0] = r["depth"], r["mask"]
         Rd, Td = rt_delta_f32tgt(refined, tgt_pose[b], T_means, T_stds, rot_coord)
         out["rot"][b], out["trans"][b] = mat2quat(Rd), Td
         out["src_pose"][b] = refined

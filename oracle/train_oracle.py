@@ -30,11 +30,10 @@ from __future__ import annotations
 import numpy as np
 
 from . import oracle as O
+from .oracle import ENC
 
 LW_PM, NUM_3D_SAMPLE, LW_FLOW, LW_MASK = 0.1, 3000, 0.25, 0.03
 NORMALIZE_FLOW, NORMALIZE_3D_POINT = 20.0, 0.1
-ENC = [("flow_conv1", 2, 3), ("conv2", 2, 2), ("conv3", 2, 2), ("conv3_1", 1, 1), ("conv4", 2, 1),
-       ("conv4_1", 1, 1), ("conv5", 2, 1), ("conv5_1", 1, 1), ("conv6", 2, 1), ("conv6_1", 1, 1)]
 FROZEN = ("upsampling_weight", "mask_upsampling_weight")
 # deconv5 / deconv4 of the decoder below: 4x4, stride 2, output cropped to the skip connection's size from row / column 1
 DECONV_STRIDE, DECONV_CROP = 2, 1
@@ -57,7 +56,8 @@ def _t(a):
 
 def graph(weights, zin, labels, requires_grad=True, num_threads=None, emulate_bf16=False):
     """The network part of the train symbol on already-zoomed inputs.
-    zin: zoom_image_observed, zoom_image_rendered (B,3,H,W), zoom_mask_observed, zoom_mask_rendered (B,1,H,W)
+    zin: zoom_image_observed, zoom_image_rendered (B,3,H,W); zoom_depth_observed, zoom_depth_rendered (B,1,H,W) for the
+         RGB-D network; zoom_mask_observed, zoom_mask_rendered (B,1,H,W) unless the network is image-only (O.conv1_input)
     labels: zoom_factor (B,4), zoom_flow (B,2,H,W), zoom_flow_weights (B,2,H,W), zoom_mask_gt_observed (B,1,H,W),
             src_pose (B,3,4), point_cloud_model / point_cloud_weights / point_cloud_observed (B,3,N)
     Returns (outputs dict of numpy arrays, grads dict name -> numpy) ; grads is {} when requires_grad=False.
@@ -87,8 +87,8 @@ def graph(weights, zin, labels, requires_grad=True, num_threads=None, emulate_bf
             if k.endswith("_weight") and k[:-7] in tc and requires_grad:
                 v.retain_grad()
     lrelu = lambda x: store(F.leaky_relu(x, 0.1))
-    x = rb(torch.cat([_t(zin["zoom_image_observed"]) / 255.0, _t(zin["zoom_image_rendered"]) / 255.0,
-                      _t(zin["zoom_mask_observed"]), _t(zin["zoom_mask_rendered"])], dim=1))
+    x = rb(torch.from_numpy(O.conv1_input(zin["zoom_image_observed"], zin["zoom_image_rendered"], zin.get("zoom_depth_observed"),
+                            zin.get("zoom_depth_rendered"), zin.get("zoom_mask_observed"), zin.get("zoom_mask_rendered"))))
     feat, pre = {}, {}
     for name, s, p in ENC:
         z = F.conv2d(x, P[name + "_weight"], P[name + "_bias"], stride=s, padding=p)
@@ -178,13 +178,17 @@ def graph(weights, zin, labels, requires_grad=True, num_threads=None, emulate_bf
 
 
 def zoom_inputs(batch, K, means_rgb):
-    """The zoom front of get_train_symbol (symbol:391-489) via the numpy/C oracle."""
+    """The zoom front of get_train_symbol (symbol:391-489) via the numpy/C oracle; a batch that carries depth_observed and
+    depth_rendered (B,1,H,W metres: the RGB-D network) also gets them zoomed with ZoomDepth by the pair's zoom factor."""
     zo, zg, zr, zf, bbox = O.zoom_mask(batch["mask_observed"], batch["mask_gt_observed"], batch["mask_rendered"],
                                        batch["src_pose"].astype(np.float32), K)
     zio, zir = O.zoom_image_with_factor(zf, batch["image_observed"], batch["image_rendered"],
                                         np.asarray(means_rgb, np.float32))
     zfl, zfw = O.zoom_flow(zf, batch["flow"], batch["flow_weights"], False)
     zin = {"zoom_image_observed": zio, "zoom_image_rendered": zir, "zoom_mask_observed": zo, "zoom_mask_rendered": zr}
+    if "depth_observed" in batch:
+        zin["zoom_depth_observed"] = O.zoom_depth(zf, batch["depth_observed"])
+        zin["zoom_depth_rendered"] = O.zoom_depth(zf, batch["depth_rendered"])
     labels = {"zoom_factor": zf, "zoom_flow": zfl, "zoom_flow_weights": zfw, "zoom_mask_gt_observed": zg,
               "src_pose": batch["src_pose"].astype(np.float32), "bbox": bbox,
               "point_cloud_model": batch["point_cloud_model"], "point_cloud_weights": batch["point_cloud_weights"],
@@ -193,9 +197,13 @@ def zoom_inputs(batch, K, means_rgb):
     return zin, labels
 
 
-def forward_backward(weights, batch, K, means_rgb, requires_grad=True, num_threads=None):
+def forward_backward(weights, batch, K, means_rgb, requires_grad=True, num_threads=None, input_mask=True):
+    """The train symbol on a batch: zoom front, graph, unzoomed mask prediction.  input_mask=False is the image-only
+    network with PRED_MASK (deepIM_flownet.py:391): the ZoomMask front and the mask labels stay, only conv1's input
+    loses the masks.  Returns (outputs, grads, zin, labels); zin holds every zoomed blob, masks included."""
     zin, labels = zoom_inputs(batch, K, means_rgb)
-    out, grads = graph(weights, zin, labels, requires_grad, num_threads)
+    net_in = zin if input_mask else {k: v for k, v in zin.items() if not k.startswith("zoom_mask_")}
+    out, grads = graph(weights, net_in, labels, requires_grad, num_threads)
     out["zoom_factor"] = labels["zoom_factor"]
     out["mask_pred_bin"] = np.round(out["mask_prob"])  # mx.sym.round: half away from zero; prob in (0,1)
     out["unzoomed_mask_pred"] = O.zoom_mask_with_factor(labels["zoom_factor"], out["mask_pred_bin"], True)

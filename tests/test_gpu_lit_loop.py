@@ -1,7 +1,7 @@
 """GPU: the ModelNet (unseen-object) branch of the test and train loops -- the fused refinement loop and the train-time
-batch update with the Lambert-lit renderer (dim_refine, dim_refine_host, dim_train_update with a dim_lighting) against the lit CPU
-checker (tests/lit_oracle.py, built on the oracle), against the unlit calls where the light is neutral, and through the
-Python layers (PoseRefiner, trainer)."""
+batch update with the Lambert-lit renderer (dim_refine, dim_refine_host, dim_train_update with a dim_lighting) against the
+oracle's lit loops (oracle.refine / oracle.train_update with lighting), against the unlit calls where the light is neutral,
+and through the Python layers (PoseRefiner, trainer)."""
 import numpy as np
 import pytest
 
@@ -11,7 +11,6 @@ torch = pytest.importorskip("torch")
 if not torch.cuda.is_available():
     pytest.skip("no CUDA device", allow_module_level=True)
 
-import lit_oracle  # noqa: E402
 from oracle import oracle as O  # noqa: E402
 from deepim_b200 import _capi as capi  # noqa: E402
 from deepim_b200 import lighting, synth  # noqa: E402
@@ -63,13 +62,13 @@ def case(meshes, weights):
     cls = np.array([0, 1, 1, 0], np.int32)
     u8 = []
     for b in range(B):
-        r = O.render_lit(meshes[cls[b]], meshes[cls[b]].normals, obs[b], K, lit_oracle.light_position(obs[b]),
+        r = O.render_lit(meshes[cls[b]], meshes[cls[b]].normals, obs[b], K, O.light_position(obs[b]),
                          np.array([1.02, 0.97, 1.0], np.float32), 0.7)
         u8.append(synth.composite_observed(r["bgr"], r["mask"], b))
     u8 = np.stack(u8)
     img = np.stack([synth.transform_image(u8[b]) for b in range(B)])
     inten = lighting.sample_intensity(np.random.default_rng(11), (N_ITER, B))
-    ref = lit_oracle.refine(weights, meshes, cls, img, ini, K, lit(inten), N_ITER, MEANS32)
+    ref = O.refine(weights, meshes, cls, img, ini, K, N_ITER, MEANS32, lighting=lit(inten))
     return dict(B=B, obs=obs, ini=ini, cls=cls, u8=u8, img=img, inten=inten, ref=ref)
 
 
@@ -193,7 +192,7 @@ def test_lit_train_update_matches_oracle(ctx, meshes):
     for k in ("depth_rendered", "mask_rendered", "src_pose", "rot", "trans", "flow", "flow_weights"):
         assert torch.equal(out[k], unlit[k]), k
     assert not torch.equal(out["image_rendered"], unlit["image_rendered"])
-    ref = lit_oracle.train_update(meshes, cls, src32, rot_est, trans_est, tgt32, depth_gt, K, MEANS, lit(inten))
+    ref = O.train_update(meshes, cls, src32, rot_est, trans_est, tgt32, depth_gt, K, MEANS, lighting=lit(inten))
     sp = out["src_pose"].cpu().numpy()
     assert np.abs(sp - ref["src_pose"]).max() < 1e-6
     assert np.abs(out["rot"].cpu().numpy() - ref["rot"]).max() < 1e-6     # Jacobi vs LAPACK eigh, float32 store

@@ -1,6 +1,7 @@
 """GPU: the image-only network (config.network.INPUT_MASK: False) in the fused refinement loop and on the op surface --
-dim_refine(_lit), dim_refine_host and dim_net_fwd of a dim_ctx_set_input_mask(ctx, 0) context against the CPU checker
-(tests/nomask_oracle.py), against the 8-channel context with zero mask columns, and the error paths of the switch.
+dim_refine(_lit), dim_refine_host and dim_net_fwd of a dim_ctx_set_input_mask(ctx, 0) context against the oracle's
+image-only loop (oracle.refine with input_mask=False), against the 8-channel context with zero mask columns, and the error
+paths of the switch.
 
 B = 16 observed frames: eight renders on a black background (the observed box is the object's) and eight composited over
 noise (the observed box is the full frame).  Instance 5 refines a black-textured cube: its render has no colour-valid pixel,
@@ -16,7 +17,6 @@ torch = pytest.importorskip("torch")
 if not torch.cuda.is_available():
     pytest.skip("no CUDA device", allow_module_level=True)
 
-import nomask_oracle  # noqa: E402
 from kernel_ref import s2d_decode  # noqa: E402
 from oracle import oracle as O  # noqa: E402
 from deepim_b200 import _capi as capi  # noqa: E402
@@ -81,7 +81,7 @@ def case(meshes, weights):
             u8.append(synth.composite_observed(r["bgr"], r["mask"], b))
     u8 = np.stack(u8)
     img = np.stack([synth.transform_image(u8[b]) for b in range(B)])
-    ref = nomask_oracle.refine(weights, meshes, cls, img, ini, K, N_ITER, MEANS)
+    ref = O.refine(weights, meshes, cls, img, ini, K, N_ITER, MEANS, input_mask=False, return_inputs=True)
     return dict(obs=obs, ini=ini, cls=cls, u8=u8, img=img, ref=ref)
 
 
@@ -106,7 +106,7 @@ def test_conv1_input_is_the_zoomed_images(ctx, case, prec):
     ctx.refine(dev(c["img"]), dev(c["cls"]), dev(c["ini"]), K, 1, pixel_means_rgb=MEANS, precision=prec)
     torch.cuda.synchronize()
     z = c["ref"]["inputs"][0]
-    x = nomask_oracle.conv1_input(z["zio"], z["zir"])  # [B,6,H,W]
+    x = O.conv1_input(z["zio"], z["zir"])  # [B,6,H,W]
     f16 = prec == capi.PREC_FP16
     hi, g = ctx.debug_activation(0, B, fp16=f16)
     rows, cols, ch, pad = g[0], g[1], g[2], g[3]
@@ -142,7 +142,8 @@ def test_nomask_refine_lit_teacher_forced(ctx, meshes, weights, case):
     inten = lighting.sample_intensity(np.random.default_rng(3), (N_ITER, B))
     lit = {"intensity": inten, "offset": lighting.OFFSET, "brightness_ratio": 0.7}
     po = [c["ini"]] + [c["ref"]["poses"][i] for i in range(N_ITER - 1)]
-    ref = nomask_oracle.refine(weights, meshes, c["cls"], c["img"], c["ini"], K, N_ITER, MEANS, poses_override=po, lighting=lit)
+    ref = O.refine(weights, meshes, c["cls"], c["img"], c["ini"], K, N_ITER, MEANS, poses_override=po, lighting=lit,
+                   input_mask=False)
     res = ctx.refine(dev(c["img"]), dev(c["cls"]), dev(c["ini"]), K, N_ITER, pixel_means_rgb=MEANS, precision=capi.PREC_FP16,
                      pose_override=teacher(c), lighting=dict(lit, intensity=dev(inten)))
     assert np.array_equal(res["bbox"].cpu().numpy(), ref["bbox"])
@@ -167,7 +168,7 @@ def test_net_fwd_equals_the_eight_channel_network_with_zero_mask_columns(meshes,
         r8, t8 = c8.net_forward(dev(z["zio"]), dev(z["zir"]), dev(m), dev(1 - m), precision=prec)
         assert torch.equal(r6, r8) and torch.equal(t6, t8)
         if prec == capi.PREC_FP16:
-            rr, tr = nomask_oracle.net_forward(weights, z["zio"], z["zir"])
+            rr, tr = O.net_forward(weights, z["zio"], z["zir"])
             assert np.abs(r6.cpu().numpy() - rr).max() < 1e-4 and np.abs(t6.cpu().numpy() - tr).max() < 1e-3
     finally:
         c6.close()

@@ -1,5 +1,5 @@
-"""GPU: the training step of the image-only network (a dim_ctx_set_input_mask(ctx, 0) context) against the train checker with
-the 6-channel input (tests/nomask_oracle.train_forward_backward), against the 8-channel step with zero mask columns, its
+"""GPU: the training step of the image-only network (a dim_ctx_set_input_mask(ctx, 0) context) against the train oracle with
+the 6-channel input (train_oracle.forward_backward(input_mask=False)), against the 8-channel step with zero mask columns, its
 parameter table, and fit_batch in bf16 and bf16x3.  With PRED_MASK the training graph still zooms with ZoomMask and learns
 the mask; only the network input loses the mask channels."""
 import os
@@ -17,7 +17,6 @@ if not torch.cuda.is_available():
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-import nomask_oracle  # noqa: E402
 from oracle import train_oracle as T  # noqa: E402
 from deepim_b200 import _capi as capi  # noqa: E402
 from deepim_b200 import synth  # noqa: E402
@@ -69,7 +68,7 @@ def test_nomask_training_step_matches_the_checker(setup, precision):
     (measured on an H100), an accuracy of the bf16 step itself, which is the 8-channel step bit for bit (test below) and is
     bounded by tests/test_gpu_train.py."""
     meshes, w, batch, ctx, tr = setup
-    out, g, zin, lab = nomask_oracle.train_forward_backward(w, batch, K, MEANS)
+    out, g, zin, lab = T.forward_backward(w, batch, K, MEANS, input_mask=False)
     try:
         tr.set_precision(precision)
         z = tr.zoom_front(device_batch(batch), K)

@@ -1,5 +1,6 @@
 """GPU: the RGB-D network (config.network.INPUT_DEPTH) in the fused refinement loop and on the op surface -- dim_refine,
-dim_refine_host and dim_net_fwd of an RGB-D context against the RGB-D CPU checker (tests/depth_oracle.py), against the RGB context
+dim_refine_host and dim_net_fwd of an RGB-D context against the oracle's RGB-D loop (oracle.refine with depth_observed), against
+the RGB context
 where the depth weights are zero, and the error paths of the mode switch."""
 import ctypes as C
 
@@ -12,8 +13,6 @@ torch = pytest.importorskip("torch")
 if not torch.cuda.is_available():
     pytest.skip("no CUDA device", allow_module_level=True)
 
-import depth_oracle  # noqa: E402
-import lit_oracle  # noqa: E402
 from oracle import oracle as O  # noqa: E402
 from deepim_b200 import _capi as capi  # noqa: E402
 from deepim_b200 import lighting, synth  # noqa: E402
@@ -74,9 +73,9 @@ def case(meshes, weights):
         dep.append(np.clip(np.rint(d * 1000.0), 0, 65535).astype(np.uint16))
     u8, u16 = np.stack(u8), np.stack(dep)
     img = np.stack([synth.transform_image(u8[b]) for b in range(B)])
-    depth = depth_oracle.depth_from_u16(u16, 1000.0)[:, None]
+    depth = O.depth_from_u16(u16, 1000.0)[:, None]
     # float64 means, as the device gets them: the checker's render subtracts them in float64 like the device's
-    ref = depth_oracle.refine(weights, meshes, cls, img, depth, ini, K, N_ITER, MEANS)
+    ref = O.refine(weights, meshes, cls, img, ini, K, N_ITER, MEANS, depth_observed=depth, return_inputs=True)
     return dict(obs=obs, ini=ini, cls=cls, u8=u8, u16=u16, img=img, depth=depth, ref=ref)
 
 
@@ -93,7 +92,7 @@ def test_conv1_input_equals_the_checker_blob(ctx, case, prec):
                depth_observed=dev(c["depth"]))
     torch.cuda.synchronize()
     z = c["ref"]["inputs"][0]
-    x = depth_oracle.conv1_input(z["zio"], z["zir"], z["zdo"], z["zdr"], z["zmo"], z["zmr"])  # [B,10,H,W]
+    x = O.conv1_input(z["zio"], z["zir"], z["zdo"], z["zdr"], z["zmo"], z["zmr"])  # [B,10,H,W]
     f16 = prec == capi.PREC_FP16
     hi, g = ctx.debug_activation(0, B, fp16=f16)
     rows, cols, ch, pad = g[0], g[1], g[2], g[3]
@@ -209,8 +208,9 @@ def test_lit_and_depth_together(ctx, meshes, weights, case):
     c = case
     inten = lighting.sample_intensity(np.random.default_rng(3), (N_ITER, B))
     lit = {"intensity": inten, "offset": lighting.OFFSET, "brightness_ratio": 0.7}
-    ref = depth_oracle.refine(weights, meshes, c["cls"], c["img"], c["depth"], c["ini"], K, N_ITER, MEANS,
-                              poses_override=[c["ini"]] + [c["ref"]["poses"][i] for i in range(N_ITER - 1)], lighting=lit)
+    ref = O.refine(weights, meshes, c["cls"], c["img"], c["ini"], K, N_ITER, MEANS,
+                   poses_override=[c["ini"]] + [c["ref"]["poses"][i] for i in range(N_ITER - 1)], lighting=lit,
+                   depth_observed=c["depth"])
     res = ctx.refine(dev(c["img"]), dev(c["cls"]), dev(c["ini"]), K, N_ITER, pixel_means_rgb=MEANS, precision=capi.PREC_FP16,
                      pose_override=teacher(c), depth_observed=dev(c["depth"]), lighting=dict(lit, intensity=dev(inten)))
     assert np.array_equal(res["bbox"].cpu().numpy(), ref["bbox"])
@@ -226,7 +226,7 @@ def test_net_fwd_rgbd_matches_the_checker(ctx, weights, case, prec):
     z = case["ref"]["inputs"][0]
     rot, trans = ctx.net_forward(dev(z["zio"]), dev(z["zir"]), dev(z["zmo"]), dev(z["zmr"]), precision=prec,
                                  zoom_depth_observed=dev(z["zdo"]), zoom_depth_rendered=dev(z["zdr"]))
-    rr, tr = depth_oracle.net_forward(weights, z["zio"], z["zir"], z["zdo"], z["zdr"], z["zmo"], z["zmr"])
+    rr, tr = O.net_forward(weights, z["zio"], z["zir"], z["zmo"], z["zmr"], zdo=z["zdo"], zdr=z["zdr"])
     assert np.abs(rot.cpu().numpy() - rr).max() < 1e-4
     assert np.abs(trans.cpu().numpy() - tr).max() < 1e-3
 

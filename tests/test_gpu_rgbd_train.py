@@ -1,5 +1,5 @@
-"""GPU: the training step of the RGB-D network (dim_train_forward_backward on an RGB-D context) against the RGB-D train checker
-(tests/depth_oracle.train_forward_backward, train_oracle.graph with the 10-channel input), its parameter table, and
+"""GPU: the training step of the RGB-D network (dim_train_forward_backward on an RGB-D context) against the train oracle
+(train_oracle.forward_backward on a batch with depths: train_oracle.graph with the 10-channel input), its parameter table, and
 fit_batch carrying the re-render's depth.  Bounds as tests/test_gpu_train.py (bf16 mixed-precision step, fp32 checker)."""
 import os
 import sys
@@ -16,7 +16,6 @@ if not torch.cuda.is_available():
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-import depth_oracle  # noqa: E402
 from oracle import oracle as O, train_oracle as T  # noqa: E402
 from deepim_b200 import _capi as capi  # noqa: E402
 from deepim_b200 import synth  # noqa: E402
@@ -67,7 +66,7 @@ def test_rgbd_param_table(setup):
 
 def test_rgbd_training_step_matches_the_checker(setup):
     meshes, w, batch, ctx, tr = setup
-    out, g, zin, lab = depth_oracle.train_forward_backward(w, batch, K, MEANS)
+    out, g, zin, lab = T.forward_backward(w, batch, K, MEANS)
     b = {k: dev(v) for k, v in batch.items()}
     b["pixel_means_rgb"] = MEANS.astype(np.float32)
     z = tr.zoom_front(b, K)

@@ -22,7 +22,6 @@ if not torch.cuda.is_available():
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-import depth_oracle  # noqa: E402
 from oracle import oracle as O, train_oracle as T  # noqa: E402
 from deepim_b200 import _capi as capi  # noqa: E402
 from deepim_b200 import synth  # noqa: E402
@@ -193,7 +192,7 @@ def test_bf16x3_rgbd_step_matches_the_checker(setup):
     noise = np.random.default_rng(4).normal(0, 0.002, depth_gt.shape).astype(np.float32)
     batch["depth_observed"] = np.where(depth_gt > 0, depth_gt + noise, 0).astype(np.float32)
     batch["depth_rendered"] = upd["depth_rendered"]
-    out, g, _, _ = depth_oracle.train_forward_backward(w, batch, K, MEANS)
+    out, g, _, _ = T.forward_backward(w, batch, K, MEANS)
     ctx = Context(0, max_batch=B, max_classes=2, max_verts=6000, max_faces=11000, input_depth=True)
     try:
         for i, m in enumerate(meshes):

@@ -1,13 +1,13 @@
 """CPU: the ModelNet branch's lighting -- the dim_lighting ABI struct, the light helpers against the reference's own
-statements, and the lit CPU loop (tests/lit_oracle.py) against the oracle's unlit one where the lighting is neutral."""
+statements, and the oracle's lit loop against its unlit one where the lighting is neutral."""
 import ctypes
 import os
 
 import numpy as np
 import pytest
 
-import lit_oracle
 from deepim_b200 import lighting, synth
+from oracle import oracle as O
 
 
 def test_lighting_struct_layout_matches_the_header(root, tmp_path):
@@ -65,7 +65,7 @@ def test_light_position_rounds_once_from_float64():
         pose[:, 3] = (rng.uniform(-0.1, 0.1), rng.uniform(-0.1, 0.1), rng.uniform(0.4, 1.2))
         ref = _reference_light(pose)
         assert np.array_equal(lighting.modelnet_light_position(pose), ref)
-        assert np.array_equal(lit_oracle.light_position(pose), ref)
+        assert np.array_equal(O.light_position(pose), ref)
         p32 = pose.astype(np.float32)
         f32_first = np.array([np.float32(0) + p32[0, 3], np.float32(0.5) - p32[1, 3], np.float32(0.5) - p32[2, 3]], np.float32)
         differs += int(not np.array_equal(f32_first, ref))
@@ -88,10 +88,9 @@ def test_sample_intensity_is_seeded_uniform_float32():
         lighting.LightSource.of({"seed": 1, "ratio": 0.5})
 
 
-def test_lit_checker_loop_with_neutral_light_equals_the_unlit_oracle_loop():
+def test_oracle_lit_loop_with_neutral_light_equals_its_unlit_loop():
     """brightness_ratio 0 and unit intensity: every lit colour is round(texel) = the unlit (uint8-truncated) colour, so the
     lit CPU loop reproduces the oracle's unlit one exactly."""
-    from oracle import oracle as O
     mesh = synth.make_cube()
     mesh.normals = synth.vertex_normals(mesh)
     K, means = synth.K_LINEMOD, synth.PIXEL_MEANS_RGB.astype(np.float32)
@@ -101,15 +100,14 @@ def test_lit_checker_loop_with_neutral_light_equals_the_unlit_oracle_loop():
     img = synth.transform_image(synth.composite_observed(r["bgr"], r["mask"], 0))[None]
     cls = np.zeros(1, np.int32)
     unlit = O.refine(weights, [mesh], cls, img, ini, K, 2, means)
-    lit = lit_oracle.refine(weights, [mesh], cls, img, ini, K,
-                            {"intensity": np.ones((2, 1, 3), np.float32), "offset": (0.0, 0.5, 0.5), "brightness_ratio": 0.0},
-                            2, means)
+    lit = O.refine(weights, [mesh], cls, img, ini, K, 2, means,
+                   lighting={"intensity": np.ones((2, 1, 3), np.float32), "offset": (0.0, 0.5, 0.5), "brightness_ratio": 0.0})
     for k in ("poses", "se3", "zoom_factor", "bbox"):
         assert np.array_equal(lit[k], unlit[k]), k
     # and a real light changes the colours but not the geometry of the render
     pose = ini[0]
     li = np.array([1.05, 0.95, 1.0], np.float32)
     a = O.render(mesh, pose, K, means_rgb=means)
-    b = O.render_lit(mesh, mesh.normals, pose, K, lit_oracle.light_position(pose), li, 0.7, means_rgb=means)
+    b = O.render_lit(mesh, mesh.normals, pose, K, O.light_position(pose), li, 0.7, means_rgb=means)
     assert np.array_equal(a["mask"], b["mask"]) and np.array_equal(a["depth"], b["depth"])
     assert not np.array_equal(a["image"], b["image"])

@@ -1,4 +1,4 @@
-"""CPU: the image-only network's host-side pieces (config.network.INPUT_MASK: False) -- the CPU checker's ZoomImage against the
+"""CPU: the image-only network's host-side pieces (config.network.INPUT_MASK: False) -- the oracle's ZoomImage against the
 reference operator's fixture, its 6-channel tower, the parameter table, the 6-channel checkpoint and weight helpers."""
 import hashlib
 import os
@@ -7,7 +7,6 @@ import sys
 import numpy as np
 import pytest
 
-import nomask_oracle
 from oracle import oracle as O
 from deepim_b200 import mx_params, synth
 
@@ -15,35 +14,35 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def test_checker_zoom_image_reproduces_the_reference_operator():
-    """nomask_oracle's ZoomImage step against ref_mx_zoom_small.npz (the reference's unmodified ZoomImage operator): the zoom
+    """The oracle's ZoomImage step against ref_mx_zoom_small.npz (the reference's unmodified ZoomImage operator): the zoom
     factor and both zoomed images bit for bit."""
     sys.path.insert(0, os.path.join(HERE, "golden"))
     import mx_cases as C
     g = np.load(os.path.join(HERE, "golden", "ref_mx_zoom_small.npz"))
     c = C.zoom_case(int(g["seed"]), int(g["B"]), int(g["H"]), int(g["W"]))
-    z = nomask_oracle.zoom_inputs(c["img_o"], c["img_r"], c["pose"], c["K"], C.PIXEL_MEANS_RGB)
-    assert np.array_equal(z["zoom_factor"], g["zimg_factor"])
-    assert hashlib.sha256(z["zio"].tobytes()).digest() == g["zimg_o_sha"].tobytes()
-    assert hashlib.sha256(z["zir"].tobytes()).digest() == g["zimg_r_sha"].tobytes()
+    zio, zir, zf, _ = O.zoom_image(c["img_o"], c["img_r"], c["pose"], c["K"], C.PIXEL_MEANS_RGB)
+    assert np.array_equal(zf, g["zimg_factor"])
+    assert hashlib.sha256(zio.tobytes()).digest() == g["zimg_o_sha"].tobytes()
+    assert hashlib.sha256(zir.tobytes()).digest() == g["zimg_r_sha"].tobytes()
 
 
 def test_conv1_input_is_the_two_images():
     """deepIM_flownet.py:53-62 without INPUT_MASK: observed/255 then rendered/255, nothing else."""
     rng = np.random.default_rng(0)
     zio, zir = rng.uniform(-120, 150, (2, 3, 4, 5)).astype(np.float32), rng.uniform(-120, 150, (2, 3, 4, 5)).astype(np.float32)
-    x = nomask_oracle.conv1_input(zio, zir)
+    x = O.conv1_input(zio, zir)
     assert x.shape == (2, 6, 4, 5) and x.dtype == np.float32
     assert np.array_equal(x[:, :3], zio / np.float32(255)) and np.array_equal(x[:, 3:], zir / np.float32(255))
 
 
 def test_six_channel_tower_is_the_eight_channel_one_with_zero_mask_columns():
-    """The checker's tower with W6 equals oracle.net_forward with W6 plus zero mask columns, whatever the masks hold."""
+    """The oracle's tower with W6 and no masks equals it with W6 plus zero mask columns, whatever the masks hold."""
     w6 = synth.make_train_weights(2, input_mask=False)
     w8 = dict(w6, flow_conv1_weight=np.concatenate([w6["flow_conv1_weight"], np.zeros((64, 2, 7, 7), np.float32)], axis=1))
     rng = np.random.default_rng(1)
     zio, zir = rng.uniform(-120, 150, (1, 3, 480, 640)).astype(np.float32), rng.uniform(-120, 150, (1, 3, 480, 640)).astype(np.float32)
     m = (rng.uniform(size=(1, 1, 480, 640)) > 0.5).astype(np.float32)
-    r6, t6 = nomask_oracle.net_forward(w6, zio, zir)
+    r6, t6 = O.net_forward(w6, zio, zir)
     r8, t8 = O.net_forward(w8, zio, zir, m, 1 - m)
     assert np.abs(r6 - r8).max() < 1e-5 and np.abs(t6 - t8).max() < 1e-5
 

@@ -1,12 +1,11 @@
-"""CPU: the RGB-D network's host-side pieces -- the loader's depth conversion, the RGB-D CPU checker against the oracle's
-RGB loop, the 10-channel checkpoint and weight helpers, and the HGMMA / TMA code of its conv1 kernel."""
+"""CPU: the RGB-D network's host-side pieces -- the loader's depth conversion, the oracle's RGB-D loop against its RGB
+loop, the 10-channel checkpoint and weight helpers, and the HGMMA / TMA code of its conv1 kernel."""
 import os
 import re
 
 import numpy as np
 import pytest
 
-import depth_oracle
 from oracle import oracle as O
 from deepim_b200 import mx_params, synth
 
@@ -15,13 +14,13 @@ def test_depth_conversion_matches_the_reference_expression():
     """image.py:203,218: float32(u16) / DEPTH_FACTOR with a Python float is float32 division by the float32 factor."""
     u16 = np.arange(0, 65536, dtype=np.uint16).reshape(256, 256)
     for factor in (1000.0, 10000.0, 999.9, 1.0 / 3.0):
-        got = depth_oracle.depth_from_u16(u16, factor)
+        got = O.depth_from_u16(u16, factor)
         ref = u16.astype(np.float32) / np.float32(factor)
         assert got.dtype == np.float32
         assert np.array_equal(got.view(np.uint32), ref.view(np.uint32)), factor
     # and not float64 division rounded afterwards (the two differ for some inputs)
     f64 = (u16.astype(np.float64) / 999.9).astype(np.float32)
-    assert not np.array_equal(depth_oracle.depth_from_u16(u16, 999.9), f64)
+    assert not np.array_equal(O.depth_from_u16(u16, 999.9), f64)
 
 
 def test_conv1_input_channel_order():
@@ -31,7 +30,7 @@ def test_conv1_input_channel_order():
     zio, zir = rng.uniform(-120, 150, (B, 3, H, W)).astype(np.float32), rng.uniform(-120, 150, (B, 3, H, W)).astype(np.float32)
     zdo, zdr = rng.uniform(0, 2, (B, 1, H, W)).astype(np.float32), rng.uniform(0, 2, (B, 1, H, W)).astype(np.float32)
     zmo, zmr = (rng.uniform(size=(B, 1, H, W)) > 0.5).astype(np.float32), (rng.uniform(size=(B, 1, H, W)) > 0.5).astype(np.float32)
-    x = depth_oracle.conv1_input(zio, zir, zdo, zdr, zmo, zmr)
+    x = O.conv1_input(zio, zir, zdo, zdr, zmo, zmr)
     assert x.shape == (B, 10, H, W) and x.dtype == np.float32
     assert np.array_equal(x[:, 6:7], zdo / np.float32(255)) and np.array_equal(x[:, 7:8], zdr / np.float32(255))
     assert np.array_equal(x[:, 8:9], zmo) and np.array_equal(x[:, 9:], zmr)
@@ -48,15 +47,15 @@ def test_checker_with_zero_depth_columns_reproduces_the_rgb_loop():
     depth = (r["depth"] + np.float32(0.5) * (r["depth"] == 0)).astype(np.float32)[None, None]
     cls = np.zeros(1, np.int32)
     ref = O.refine(weights, [m], cls, img, ini, synth.K_LINEMOD, 2, synth.PIXEL_MEANS_RGB.astype(np.float32))
-    got = depth_oracle.refine(synth.with_depth_channels(weights), [m], cls, img, depth, ini, synth.K_LINEMOD, 2,
-                              synth.PIXEL_MEANS_RGB.astype(np.float32))
+    got = O.refine(synth.with_depth_channels(weights), [m], cls, img, ini, synth.K_LINEMOD, 2,
+                   synth.PIXEL_MEANS_RGB.astype(np.float32), depth_observed=depth)
     assert np.array_equal(got["bbox"], ref["bbox"])
     assert np.array_equal(got["zoom_factor"], ref["zoom_factor"])
     assert np.abs(got["se3"] - ref["se3"]).max() < 1e-6
     assert np.abs(got["poses"] - ref["poses"]).max() < 1e-6
     # a real depth column changes the output
     w = synth.make_weights(0, input_depth=True)
-    moved = depth_oracle.refine(w, [m], cls, img, depth, ini, synth.K_LINEMOD, 1, synth.PIXEL_MEANS_RGB.astype(np.float32))
+    moved = O.refine(w, [m], cls, img, ini, synth.K_LINEMOD, 1, synth.PIXEL_MEANS_RGB.astype(np.float32), depth_observed=depth)
     assert np.abs(moved["se3"][0] - ref["se3"][0]).max() > 1e-6
 
 
