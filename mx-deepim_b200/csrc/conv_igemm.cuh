@@ -15,8 +15,16 @@
 //
 // Warp roles (384 threads = 3 warpgroups): warp 0 = TMA producer (elected lane), warpgroups 1 and 2 = consumers.  Each
 // consumer issues the wgmmas of 64 of the tile's 128 rows (M = 64 per instruction) into its own register accumulator and
-// runs the epilogue for them (bias + LeakyReLU -> bf16 NHWC stores into the next layer's bordered buffer).  The producer
+// runs the epilogue for them (bias + LeakyReLU -> 16-bit NHWC into the next layer's bordered buffer).  The producer
 // keeps loading the next tile while the consumers drain the current one.
+//
+// Forward layers (EPI = 0) load each stage's activation tile as two boxes of BW x BH/2 pixels, one per consumer
+// (shared-memory rows 0 and 64), so a consumer's rows are whole output rows even when BW does not divide 64 (BW = 20,
+// 10: rows 60-63 of each half are never stored).  In fp16 / bf16 a consumer writes its packed results with stmatrix into a
+// 128B-swizzled [64 px][64 ch] staging block per 64-channel group and one thread TMA-stores each block as one box through
+// out_map, whose extent keeps the zero border, the virtual rows and images >= B from being written; the few boxes that run
+// into the next image store those rows from the fragments.  The TMA stores drain while the next tile's wgmmas run.
+// bf16x3 stores from the fragments: its hi + lo ring leaves no room for a staging tile.
 //
 // SPLIT3 = bf16x3 precision mode: operands are hi/lo bf16 pairs (x = hi + lo); each K step issues
 // hi*hi + lo*hi + hi*lo into the same fp32 accumulator (error ~2^-16 relative, near-fp32).
@@ -36,8 +44,9 @@ struct ConvKParams {
   CUtensorMap a_lo_map[4];  // activation views (lo), SPLIT3 only
   CUtensorMap b_map;        // weights hi (fp16 pack in F16 mode)
   CUtensorMap b_lo_map;     // weights lo
-  // conv1_kernel only: output store maps (hi, lo) over the INTERIOR of the next layer's bordered buffer, box = 64 ch x
-  // kConv1StoreN px, SW128; and the space-to-depth input it reads with plain bulk copies ([rows][4 chunks][in_cols][8 ch])
+  // output store maps (Cout, Wo, Ho, B) over the INTERIOR of the next layer's bordered buffer, box = 64 ch x a pixel
+  // rectangle, SW128: conv1_kernel (hi, lo; kConv1StoreN x 1 px) and the fp16 / bf16 EPI = 0 conv_igemm kernels ([0];
+  // BW x BH/2 px).  conv1_kernel also reads the space-to-depth input with plain bulk copies ([rows][4 chunks][in_cols][8 ch])
   CUtensorMap out_map[2];
   const __nv_bfloat16 *in_hi, *in_lo;
   int in_cols;
@@ -166,6 +175,12 @@ __device__ __forceinline__ void named_bar_sync(int id, int threads) {
 __device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, const uint32_t (&r)[4]) {
   asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
                "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+// ... stored as they are: fragment row r becomes the 16-byte row at lane (8 * matrix + r)'s address
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
+               "r"(r[3])
                : "memory");
 }
 
@@ -297,25 +312,36 @@ __device__ __forceinline__ void store_pair_generic(float v0, float v1, const Con
 // m*Nn + n, n fastest so CTAs that share an activation tile run side by side and hit it in L2 together).  The smem ring
 // runs across tile boundaries: the producer is already loading tile t+1 while the consumers store tile t.  A consumer
 // keeps one K block of wgmmas in flight (wait_group 1) and hands the stage of the previous block back to the producer.
-template <int BLOCK_N, int STAGES, bool SPLIT3>
+// Layout: the ring, then (TMA_EPI) the two consumers' staging tiles, then the barriers.  A staging tile holds STG_GROUPS
+// [64 px][64 ch] blocks of 8 KB: all of BLOCK_N when that fits beside the ring, else half of it, and the tile is stored in
+// two rounds.
+template <int BLOCK_N, int STAGES, bool SPLIT3, int EPI>
 struct ConvSmem2 {
   static constexpr int A_BYTES = 128 * 64 * 2;
   static constexpr int B_BYTES = BLOCK_N * 64 * 2;
   static constexpr int NPREC = SPLIT3 ? 2 : 1;
   static constexpr int STAGE_BYTES = (A_BYTES + B_BYTES) * NPREC;
-  static constexpr int TOTAL = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(TOTAL <= 227 * 1024, "conv_igemm shared memory");
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  static constexpr int LIMIT = 227 * 1024, FIXED = 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr bool TMA_EPI = EPI == 0 && !SPLIT3;
+  static constexpr int STG_GROUPS =
+      !TMA_EPI ? 0 : (RING_BYTES + 2 * BLOCK_N * 128 + FIXED <= LIMIT ? BLOCK_N / 64 : BLOCK_N / 128);
+  static constexpr int STG_ROUNDS = TMA_EPI ? BLOCK_N / 64 / STG_GROUPS : 0;
+  static constexpr int STG_BYTES = STG_GROUPS * 8192;  // per consumer warpgroup
+  static constexpr int TOTAL = RING_BYTES + 2 * STG_BYTES + FIXED;
+  static_assert(TOTAL <= LIMIT, "conv_igemm shared memory");
 };
 
 template <int BLOCK_N, int STAGES, bool SPLIT3, bool F16, int EPI = 0>
 __global__ void __launch_bounds__(384, 1) conv_igemm_persistent_kernel(const __grid_constant__ ConvKParams p,
                                                                        const int total_tiles, const int n_tiles) {
-  using S = ConvSmem2<BLOCK_N, STAGES, SPLIT3>;
+  using S = ConvSmem2<BLOCK_N, STAGES, SPLIT3, EPI>;
   constexpr uint32_t SBO = 1024u;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + STAGES * S::STAGE_BYTES);
+  uint8_t *stg = smem + S::RING_BYTES;
+  uint64_t *full_bar = reinterpret_cast<uint64_t *>(stg + 2 * S::STG_BYTES);
   uint64_t *empty_bar = full_bar + STAGES;
 
   const int wgi = threadIdx.x >> 7, warp = threadIdx.x >> 5;
@@ -328,6 +354,7 @@ __global__ void __launch_bounds__(384, 1) conv_igemm_persistent_kernel(const __g
     ptx::fence_barrier_init();
     ptx::prefetch_tmap(&p.b_map);
     ptx::prefetch_tmap(&p.a_map[0]);
+    if (S::TMA_EPI) ptx::prefetch_tmap(&p.out_map[0]);
   }
   __syncthreads();
 
@@ -356,11 +383,12 @@ __global__ void __launch_bounds__(384, 1) conv_igemm_persistent_kernel(const __g
           if (EPI) { dr += p.in_off_r; dc += p.in_off_c; }
           if (ptx::elect_one()) {
             ptx::mbar_expect_tx_raw(&full_bar[s], tx);
-            ptx::tma_load_3d_raw(st, &p.a_map[view], &full_bar[s], cc * 64, ow0 + dc, g0 + dr);
-            ptx::tma_load_2d_raw(st + S::A_BYTES, &p.b_map, &full_bar[s], kb * 64, n0);
-            if (SPLIT3) {
-              ptx::tma_load_3d_raw(st + S::A_BYTES + S::B_BYTES, &p.a_lo_map[view], &full_bar[s], cc * 64, ow0 + dc, g0 + dr);
-              ptx::tma_load_2d_raw(st + 2 * S::A_BYTES + S::B_BYTES, &p.b_lo_map, &full_bar[s], kb * 64, n0);
+            for (int pr = 0; pr < S::NPREC; ++pr) {
+              uint8_t *sa = st + pr * (S::A_BYTES + S::B_BYTES);
+              const CUtensorMap *am = pr ? &p.a_lo_map[view] : &p.a_map[view];
+              ptx::tma_load_3d_raw(sa, am, &full_bar[s], cc * 64, ow0 + dc, g0 + dr);
+              if (EPI == 0) ptx::tma_load_3d_raw(sa + S::A_BYTES / 2, am, &full_bar[s], cc * 64, ow0 + dc, g0 + dr + (p.BH >> 1));
+              ptx::tma_load_2d_raw(sa + S::A_BYTES, pr ? &p.b_lo_map : &p.b_map, &full_bar[s], kb * 64, n0);
             }
           }
           __syncwarp();
@@ -373,9 +401,16 @@ __global__ void __launch_bounds__(384, 1) conv_igemm_persistent_kernel(const __g
     // ------------------------------------------------------------------ consumers: rows 64*(wgi-1) .. +63 of the M tile
     const int t = threadIdx.x & 127;
     const int half = wgi - 1;
-    const int r0 = half * 64 + frag_row(t), q2 = (t & 3) * 2;
+    const int q2 = (t & 3) * 2;
     const bool arriver = t == 0;
     const uint32_t base = ptx::smem_u32(smem);
+    // TMA_EPI staging: stmatrix x4 of 8-channel groups (j, j + 1): matrix mi = lane / 8 is (pixels 16 * warp + 8 * (mi & 1)
+    // .. +7, group j + mi / 2); lane addresses pixel 16 * warp + 8 * (mi & 1) + lane % 8, whose 16-byte chunk c of a 128-byte
+    // row sits at c ^ (pixel % 8) (SW128, blocks 1024-byte aligned)
+    uint8_t *my_stg = stg + half * S::STG_BYTES;
+    const int lane = t & 31;
+    const uint32_t st_addr = ptx::smem_u32(my_stg) + (uint32_t)((16 * (t >> 5) + 8 * ((lane >> 3) & 1) + (lane & 7)) * 128);
+    const uint32_t st_sw = (uint32_t)(((lane >> 4) & 1) ^ (lane & 7));
     float acc[BLOCK_N / 2];
     int s = 0;
     uint32_t ph = 0;
@@ -412,40 +447,93 @@ __global__ void __launch_bounds__(384, 1) conv_igemm_persistent_kernel(const __g
       const int nt = tile % n_tiles, mt = tile / n_tiles;
       const int col_tile = mt % p.n_col_tiles, row_tile = mt / p.n_col_tiles;
       const int n0 = nt * BLOCK_N;
+      if constexpr (S::TMA_EPI) {
+        // this warpgroup's box: output rows gs .. gs + BH/2 - 1 (virtual rows over the batch, BH/2 <= Hq: at most two
+        // images), columns ow0 .. ow0 + BW - 1
+        const int gs = row_tile * p.BH + half * (p.BH >> 1), ow0 = col_tile * p.BW;
+        const int n_img = gs / p.Hq, oh = gs - n_img * p.Hq;
+        const bool store0 = n_img < p.Bn && oh < p.Ho, store1 = n_img + 1 < p.Bn && oh + (p.BH >> 1) > p.Hq;
 #pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {
-        const int m = r0 + rr * 8;
-        const int bh = m / p.BW, bw = m - bh * p.BW;
-        const int g = row_tile * p.BH + bh, ow = col_tile * p.BW + bw;
-        const int n_img = g / p.Hq, oh = g - n_img * p.Hq;
-        if (EPI == 1) {
-          const int y = oh * p.out_sy + p.out_oy, x = ow * p.out_sx + p.out_ox;
-          const bool valid = (m < p.BW * p.BH) && (n_img < p.Bn) && (oh < p.Ho) && (ow < p.Wo) && y >= 0 && y < p.out_H &&
-                             x >= 0 && x < p.out_W;
-          const long long off =
-              (((long long)n_img * p.out_Hp + y + p.out_py) * p.out_Wp + x + p.out_px) * p.out_cs + p.out_coff + n0 + q2;
-          const long long add_off =
-              (((long long)n_img * p.addend.Hp + y + p.addend.py) * p.addend.Wp + x + p.addend.px) * p.addend.cs + p.addend.coff +
-              n0 + q2;
-          const long long mask_off =
-              (((long long)n_img * p.mask.Hp + y + p.mask.py) * p.mask.Wp + x + p.mask.px) * p.mask.cs + p.mask.coff + n0 + q2;
+        for (int rd = 0; rd < S::STG_ROUNDS; ++rd) {
+          if (arriver) ptx::bulk_wait_read0();  // the previous stores have left the staging tile
+          ptx::named_bar_sync(1 + half, 128);
 #pragma unroll
-          for (int j = 0; j < BLOCK_N / 8; ++j)
-            store_pair_generic<SPLIT3>(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1], p, n0 + 8 * j + q2, valid, off + 8 * j,
-                               add_off + 8 * j, mask_off + 8 * j);
-        } else {
-          const bool valid = (m < p.BW * p.BH) && (n_img < p.Bn) && (oh < p.Ho) && (ow < p.Wo);
-          if (valid) {
-            const long long off = (((long long)n_img * p.out_Hp + oh + p.out_py) * p.out_Wp + ow + p.out_px) * p.Cout + n0 + q2;
+          for (int i = 0; i < S::STG_GROUPS * 4; ++i) {  // 8-channel groups j, j + 1 = chunks 2 (i & 3) (+1) of block i / 4
+            const int j = rd * S::STG_GROUPS * 8 + 2 * i;
+            const float *bj = p.bias + n0 + 8 * j + q2;
+            const float b0 = __ldg(bj), b1 = __ldg(bj + 1), b2 = __ldg(bj + 8), b3 = __ldg(bj + 9);
+            uint32_t h[4], unused;
+            epi_pack<false, F16>(acc[4 * j + 0], acc[4 * j + 1], b0, b1, p.slope, h[0], unused);
+            epi_pack<false, F16>(acc[4 * j + 2], acc[4 * j + 3], b0, b1, p.slope, h[1], unused);
+            epi_pack<false, F16>(acc[4 * j + 4], acc[4 * j + 5], b2, b3, p.slope, h[2], unused);
+            epi_pack<false, F16>(acc[4 * j + 6], acc[4 * j + 7], b2, b3, p.slope, h[3], unused);
+            ptx::stmatrix_x4(st_addr + (uint32_t)((i >> 2) * 8192) + (((uint32_t)(2 * (i & 3)) ^ st_sw) << 4), h);
+          }
+          ptx::fence_proxy_async();  // the generic-proxy staging writes become visible to the TMA store
+          ptx::named_bar_sync(1 + half, 128);
+          if (arriver && store0) {
+            for (int q = 0; q < S::STG_GROUPS; ++q)
+              ptx::tma_store_4d(&p.out_map[0], my_stg + q * 8192, n0 + (rd * S::STG_GROUPS + q) * 64, ow0, oh, n_img);
+            ptx::bulk_commit();
+          }
+        }
+        if (store1) {
+          // the box's rows past image n_img's virtual rows are rows of image n_img + 1; a box there would start at a negative
+          // row, so they are stored from the fragments
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            const int lr = frag_row(t) + rr * 8, bh = lr / p.BW;
+            const int oh1 = oh + bh - p.Hq, ow = ow0 + lr - bh * p.BW;
+            if (lr < p.BW * (p.BH >> 1) && oh1 >= 0 && oh1 < p.Ho) {
+              const long long off =
+                  (((long long)(n_img + 1) * p.out_Hp + oh1 + p.out_py) * p.out_Wp + ow + p.out_px) * p.Cout + n0 + q2;
+#pragma unroll
+              for (int j = 0; j < BLOCK_N / 8; ++j)
+                store_pair<false, F16>(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1],
+                                       make_float2(__ldg(p.bias + n0 + 8 * j + q2), __ldg(p.bias + n0 + 8 * j + q2 + 1)), p.slope,
+                                       p.out_hi, p.out_lo, off + 8 * j);
+            }
+          }
+        }
+      } else {
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          // EPI = 0: row lr of this warpgroup's BW x BH/2 box; EPI = 1: row m of the BW x BH tile
+          const int lr = frag_row(t) + rr * 8, m = EPI ? half * 64 + lr : lr;
+          const bool in_tile = EPI ? m < p.BW * p.BH : lr < p.BW * (p.BH >> 1);
+          const int bh = m / p.BW, bw = m - bh * p.BW;
+          const int g = row_tile * p.BH + (EPI ? 0 : half * (p.BH >> 1)) + bh, ow = col_tile * p.BW + bw;
+          const int n_img = g / p.Hq, oh = g - n_img * p.Hq;
+          if (EPI == 1) {
+            const int y = oh * p.out_sy + p.out_oy, x = ow * p.out_sx + p.out_ox;
+            const bool valid = in_tile && (n_img < p.Bn) && (oh < p.Ho) && (ow < p.Wo) && y >= 0 && y < p.out_H &&
+                               x >= 0 && x < p.out_W;
+            const long long off =
+                (((long long)n_img * p.out_Hp + y + p.out_py) * p.out_Wp + x + p.out_px) * p.out_cs + p.out_coff + n0 + q2;
+            const long long add_off =
+                (((long long)n_img * p.addend.Hp + y + p.addend.py) * p.addend.Wp + x + p.addend.px) * p.addend.cs + p.addend.coff +
+                n0 + q2;
+            const long long mask_off =
+                (((long long)n_img * p.mask.Hp + y + p.mask.py) * p.mask.Wp + x + p.mask.px) * p.mask.cs + p.mask.coff + n0 + q2;
 #pragma unroll
             for (int j = 0; j < BLOCK_N / 8; ++j)
-              store_pair<SPLIT3, F16>(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1],
-                                      make_float2(__ldg(p.bias + n0 + 8 * j + q2), __ldg(p.bias + n0 + 8 * j + q2 + 1)), p.slope, p.out_hi,
-                                      p.out_lo, off + 8 * j);
+              store_pair_generic<SPLIT3>(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1], p, n0 + 8 * j + q2, valid, off + 8 * j,
+                                 add_off + 8 * j, mask_off + 8 * j);
+          } else {
+            const bool valid = in_tile && (n_img < p.Bn) && (oh < p.Ho) && (ow < p.Wo);
+            if (valid) {
+              const long long off = (((long long)n_img * p.out_Hp + oh + p.out_py) * p.out_Wp + ow + p.out_px) * p.Cout + n0 + q2;
+#pragma unroll
+              for (int j = 0; j < BLOCK_N / 8; ++j)
+                store_pair<SPLIT3, F16>(acc[4 * j + 2 * rr], acc[4 * j + 2 * rr + 1],
+                                        make_float2(__ldg(p.bias + n0 + 8 * j + q2), __ldg(p.bias + n0 + 8 * j + q2 + 1)), p.slope, p.out_hi,
+                                        p.out_lo, off + 8 * j);
+            }
           }
         }
       }
     }
+    if (S::TMA_EPI && arriver) ptx::bulk_wait0();
   }
 }
 

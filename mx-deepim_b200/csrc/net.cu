@@ -116,7 +116,8 @@ static int build_maps(NetState *ns, int B, bool f16, TensorMaps &tm) {
     for (int lo = 0; lo < 2; ++lo) {
       __nv_bfloat16 *base = lo ? ns->act_lo[i] : ns->act_hi[i];
       CUtensorMap *maps = lo ? kp.a_lo_map : kp.a_map;
-      const uint32_t box[3] = {(uint32_t)g.BLOCK_K, (uint32_t)g.BW, (uint32_t)g.BH};
+      // conv2 ... conv6_1: one box per consumer warpgroup (BW x BH/2 pixels; conv_igemm.cuh)
+      const uint32_t box[3] = {(uint32_t)g.BLOCK_K, (uint32_t)g.BW, (uint32_t)(g.BH / 2)};
       if (i == 0 && ns->input_depth) {
         // RGB-D conv1 strip layout [B*rows][8 chunks][cols][8 ch]: box = 8 ch x (BW+3) cols x 8 chunks x 1 row
         const uint64_t dims[4] = {8, (uint64_t)g.cols, 8, (uint64_t)B * g.rows};
@@ -167,18 +168,25 @@ static int build_maps(NetState *ns, int B, bool f16, TensorMaps &tm) {
     kp.out_hi = ns->act_hi[i + 1];
     kp.out_lo = ns->act_lo[i + 1];
     if (i == 0 && !ns->input_depth) {
-      // conv1_kernel: strips from the space-to-depth input, output tiles TMA-stored into conv2's buffer through a 4-D map
-      // (64 ch, Wo, Ho, B) whose origin is the interior's first pixel: the zero border lies outside every box
-      const LayerGeom &nx = ns->g[1];
+      // conv1_kernel: strips from the space-to-depth input
       kp.in_hi = ns->act_hi[0];
       kp.in_lo = ns->act_lo[0];
       kp.in_cols = g.cols;
-      const uint64_t dims[4] = {64, (uint64_t)g.Wo, (uint64_t)g.Ho, (uint64_t)B};
-      const uint64_t str[3] = {128, (uint64_t)nx.cols * 128, (uint64_t)nx.rows * nx.cols * 128};
-      const uint32_t box[4] = {64, (uint32_t)kConv1StoreN, 1, 1};
-      const size_t interior = ((size_t)nx.py * nx.cols + nx.px) * 64;
-      for (int lo = 0; lo < 2; ++lo)
-        if (int rc = encode_map(&kp.out_map[lo], (lo ? ns->act_lo[1] : ns->act_hi[1]) + interior, 4, dims, str, box, 64)) return rc;
+    }
+    if (i > 0 || !ns->input_depth) {
+      // output tiles TMA-stored into the next layer's buffer through a 4-D map (Cout, Wo, Ho, B) whose origin is the
+      // interior's first pixel: the zero border lies outside every box.  conv1_kernel stores hi and lo rows of kConv1StoreN
+      // pixels; conv_igemm a warpgroup's BW x BH/2 pixels, which must not span more than two images
+      DIM_REQUIRE(i == 0 || (g.BH % 2 == 0 && g.BH / 2 <= g.Hq && g.BW * (g.BH / 2) <= 64),
+                  "conv_igemm: a consumer warpgroup's box must be whole output rows within two images");
+      const uint64_t cb = (uint64_t)g.Cout * 2;
+      const uint64_t dims[4] = {(uint64_t)g.Cout, (uint64_t)g.Wo, (uint64_t)g.Ho, (uint64_t)B};
+      const uint64_t str[3] = {cb, (uint64_t)kp.out_Wp * cb, (uint64_t)kp.out_Hp * kp.out_Wp * cb};
+      const uint32_t box[4] = {64, (uint32_t)(i == 0 ? kConv1StoreN : g.BW), (uint32_t)(i == 0 ? 1 : g.BH / 2), 1};
+      const size_t interior = ((size_t)kp.out_py * kp.out_Wp + kp.out_px) * g.Cout;
+      for (int lo = 0; lo < (i == 0 ? 2 : 1); ++lo)
+        if (int rc = encode_map(&kp.out_map[lo], (lo ? ns->act_lo[i + 1] : ns->act_hi[i + 1]) + interior, 4, dims, str, box, 64))
+          return rc;
     }
   }
   return 0;
@@ -550,7 +558,7 @@ int net_load(dim_ctx *ctx, const float *const *W, const float *const *Bv) {
 
 template <int BN, int ST, bool S3, bool F16>
 static int launch_conv(const ConvKParams &kp, int total_tiles, int n_tiles, int cap, cudaStream_t st) {
-  using S = ConvSmem2<BN, ST, S3>;
+  using S = ConvSmem2<BN, ST, S3, 0>;
   static bool attr_set = false;
   if (!attr_set) {
     DIM_CHECK(cudaFuncSetAttribute(conv_igemm_persistent_kernel<BN, ST, S3, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,

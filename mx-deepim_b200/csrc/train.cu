@@ -1017,7 +1017,7 @@ static void pick_tile(int W, int rows_total, int cap, int &BW, int &BH, int max_
 
 template <int BN, int ST, bool S3 = false>
 static int launch_generic(const ConvKParams &kp, int total_tiles, int n_tiles, int cap, cudaStream_t st) {
-  using S = ConvSmem2<BN, ST, S3>;
+  using S = ConvSmem2<BN, ST, S3, 1>;
   static bool attr_set = false;
   if (!attr_set) {
     DIM_CHECK(cudaFuncSetAttribute(conv_igemm_persistent_kernel<BN, ST, S3, false, 1>,

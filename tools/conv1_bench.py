@@ -5,7 +5,8 @@
 Runs dim_net_fwd on fixed seeded zoomed blobs (random-init weights: the timed work does not depend on the values) with
 the per-layer events of dim_debug_layer_profile, and averages each layer's time over `forwards` passes.  conv1's
 executed FLOP count is what conv1_kernel issues (every virtual row, 25 K steps of 16 per row and column tile, three
-wgmmas per K step in bf16x3), the useful count is 2 * B * Ho * Wo * 64 * 8 * 7 * 7.  Both rates are set against the dense fp16 / bf16 tensor rate at the SM clock
+wgmmas per K step in bf16x3), the useful count is 2 * B * Ho * Wo * 64 * 8 * 7 * 7.  conv2 ... conv6_1 get the same executed / useful counts (igemm_flops)
+and rates.  All rates are set against the dense fp16 / bf16 tensor rate at the SM clock
 sampled during the timed passes (132 SMs x 4096 FLOP per clock).  The card's name, power limit and clocks are read in the
 same run.  Prints one JSON line."""
 import argparse
@@ -32,6 +33,28 @@ from deepim_b200.context import Context  # noqa: E402
 H, W, HO, WO, HQ = 480, 640, 240, 320, 243  # conv1 output rows per image incl. the 3 virtual rows of the strip schedule
 NAMES = ["flow_conv1", "conv2", "conv3", "conv3_1", "conv4", "conv4_1", "conv5", "conv5_1", "conv6", "conv6_1"]
 PREC = {"fp16": capi.PREC_FP16, "bf16": capi.PREC_BF16, "bf16x3": capi.PREC_BF16X3}
+# (Cout, Cin, k, stride, pad) of conv2 ... conv6_1 (deepIM_flownet.py:63-107)
+IGEMM = [(128, 64, 5, 2, 2), (256, 128, 5, 2, 2), (256, 256, 3, 1, 1), (512, 256, 3, 2, 1), (512, 512, 3, 1, 1),
+         (512, 512, 3, 2, 1), (512, 512, 3, 1, 1), (1024, 512, 3, 2, 1), (1024, 1024, 3, 1, 1)]
+
+
+def igemm_flops(B, passes):
+    """(executed, useful) FLOP of conv2 ... conv6_1 per forward.  Executed is what conv_igemm_persistent_kernel issues: every
+    128-row M tile over the virtual rows of the batch (net.cu build_geometry: BW x BH pixels, BW | Wo, unused tile rows and
+    rows past the batch included) x BLOCK_N x the whole K."""
+    h, w, out = HO, WO, []
+    for cout, cin, k, s, pad in IGEMM:
+        ho, wo = (h + 2 * pad - k) // s + 1, (w + 2 * pad - k) // s + 1
+        hp = h + 2 * pad
+        hp += hp & 1 if s == 2 else 0
+        hq = hp // 2 if s == 2 else hp
+        bw = max((d for d in range(8, min(wo, 128) + 1) if wo % d == 0), key=lambda d: d * (128 // d) * 1000 + d)
+        bh = 128 // bw
+        bn = 256 if cout >= 256 else 128
+        tiles = -(-B * hq // bh) * (wo // bw) * (cout // bn)
+        out.append((2.0 * tiles * 128 * bn * k * k * cin * passes, 2.0 * B * ho * wo * cout * cin * k * k))
+        h, w = ho, wo
+    return out
 
 
 def card():
@@ -94,11 +117,18 @@ def main():
            "conv1": {"ms": round(float(layers[0]), 4), "executed_gflop": round(executed / 1e9, 2),
                      "useful_gflop": round(useful / 1e9, 2),
                      "executed_tflops": round(executed / c1 / 1e12, 1), "useful_tflops": round(useful / c1 / 1e12, 1)}}
-    if clocks and clocks.get("sm_mhz"):
-        peak = 132 * 4096 * clocks["sm_mhz"] * 1e6
+    peak = 132 * 4096 * clocks["sm_mhz"] * 1e6 if clocks and clocks.get("sm_mhz") else None
+    if peak:
         res["conv1"]["dense_peak_tflops_at_sampled_clock"] = round(peak / 1e12, 1)
         res["conv1"]["executed_share_of_peak"] = round(executed / c1 / peak, 3)
         res["conv1"]["useful_share_of_peak"] = round(useful / c1 / peak, 3)
+    res["igemm"] = {}
+    for name, ms, (ex, us) in zip(NAMES[1:], layers[1:], igemm_flops(B, passes)):
+        r = {"ms": round(float(ms), 4), "executed_gflop": round(ex / 1e9, 2), "useful_gflop": round(us / 1e9, 2),
+             "executed_tflops": round(ex / (ms * 1e-3) / 1e12, 1)}
+        if peak:
+            r["executed_share_of_peak"] = round(ex / (ms * 1e-3) / peak, 3)
+        res["igemm"][name] = r
     ctx.close()
     print(json.dumps(res), flush=True)
 
