@@ -308,11 +308,13 @@ DIM_API int32_t dim_refine_host(dim_ctx *ctx, const uint8_t *image_observed_u8_h
                                 const uint16_t *depth_observed_u16_host, float depth_factor,
                                 const dim_lighting *lighting, void *stream);
 
-/* Per-iteration status of the LAST dim_refine / dim_refine_host(_async) call on this context, copied device -> host
- * asynchronously on `stream` (the stream that call ran on): [min(n_iter,8), B] int32.  0 = ok; bit 0 = the rendered mask
- * of that iteration was empty (the reference crashes there: np.min of an empty array, zoom_mask.py:55-58; here the
- * fallback zoom factor was used and the instance's pose is meaningless); bit 1 = class index out of range or no mesh
- * uploaded for that class (the reference indexes a python list and raises). */
+/* Per-iteration status of the LAST dim_refine / dim_refine_host(_async) / dim_refine_frames(_host(_async)) call on this
+ * context, copied device -> host asynchronously on `stream` (the stream that call ran on): [min(n_iter,8), B] int32.
+ * 0 = ok; bit 0 = the rendered mask of that iteration was empty (the reference crashes there: np.min of an empty array,
+ * zoom_mask.py:55-58; here the fallback zoom factor was used and the instance's pose is meaningless); bit 1 = class index
+ * out of range or no mesh uploaded for that class (the reference indexes a python list and raises); bit 2 = image-only
+ * network, empty render (see the network variants); bit 3 = dim_refine_frames only: the instance's frame index lies
+ * outside [0, F), so it observed frame 0 instead (its pose is meaningless). */
 DIM_API int32_t dim_refine_status(dim_ctx *ctx, int32_t B, int32_t n_iter, int32_t *status_host, void *stream);
 
 /* Same as dim_refine_host but returns right after enqueueing the copies and kernels on `stream`
@@ -325,6 +327,41 @@ DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *image_observe
                                       int32_t precision, double *poses_out_host, float *se3_out_host,
                                       const uint16_t *depth_observed_u16_host, float depth_factor,
                                       const dim_lighting *lighting, void *stream);
+
+/* Frame-indexed fused loop: several instances refined against one copy of their observed frame (several objects of one
+ * image, or several initial hypotheses of one object).  F frames, B instances; instance b observes frame frame_idx[b].
+ * Every other argument has dim_refine's / dim_refine_host(_async)'s meaning, and instance b's results equal those of
+ * dim_refine with frame frame_idx[b] as its image_observed[b], bit for bit.  Each frame is uploaded (host entries) and
+ * packed once per call, however many instances observe it; 1 <= F <= max_batch.
+ *   dim_refine_frames: image_frames f32[F,3,H,W] RGB - mean (device), frame_idx i32[B] (device), depth_frames f32
+ *     [F,1,H,W] metres (RGB-D network only).  The indices are not checked on the host: one outside [0, F) makes the
+ *     instance observe frame 0 and sets status bit 3 (dim_refine_status) in every iteration; nothing is read outside the
+ *     F frames.  The CUDA graph of the chain reads frame_idx at replay: new indices in the same buffer need no re-capture.
+ *   dim_refine_frames_host(_async): frames_u8_host u8[F,H,W,3] BGR, frame_idx_host i32[B], depth_frames_u16_host u16
+ *     [F,H,W] (RGB-D network only).  Every index is checked before anything is enqueued: one outside [0, F) fails the call
+ *     with a message naming the instance.
+ * Image-only network: the observed box is computed once per frame; instance b's is the box of its frame. */
+DIM_API int32_t dim_refine_frames(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx,
+                                  const int32_t *cls_idx, const double *pose_init, int32_t B, int32_t n_iter,
+                                  const float *K9_host, float znear, float zfar, const double *pixel_means_rgb_host,
+                                  int32_t precision, const double *pose_override, double *poses, float *se3,
+                                  float *zoom_factor, int32_t *bbox, const float *depth_frames,
+                                  const dim_lighting *lighting, void *stream);
+DIM_API int32_t dim_refine_frames_host_async(dim_ctx *ctx, const uint8_t *frames_u8_host, int32_t F,
+                                             const int32_t *frame_idx_host, const int32_t *cls_idx_host,
+                                             const double *pose_init_host, int32_t B, int32_t n_iter,
+                                             const float *K9_host, float znear, float zfar,
+                                             const double *pixel_means_rgb_host, int32_t precision,
+                                             double *poses_out_host, float *se3_out_host,
+                                             const uint16_t *depth_frames_u16_host, float depth_factor,
+                                             const dim_lighting *lighting, void *stream);
+DIM_API int32_t dim_refine_frames_host(dim_ctx *ctx, const uint8_t *frames_u8_host, int32_t F,
+                                       const int32_t *frame_idx_host, const int32_t *cls_idx_host,
+                                       const double *pose_init_host, int32_t B, int32_t n_iter, const float *K9_host,
+                                       float znear, float zfar, const double *pixel_means_rgb_host, int32_t precision,
+                                       double *poses_out_host, float *se3_out_host,
+                                       const uint16_t *depth_frames_u16_host, float depth_factor,
+                                       const dim_lighting *lighting, void *stream);
 
 /* BGR u8 HWC -> RGB-mean f32 CHW on device (lib/utils/image.py:583-594 transform). */
 DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int32_t B,

@@ -80,6 +80,7 @@ DIM_API int32_t dim_ctx_create(int32_t device, int32_t max_batch, int32_t H, int
   rc |= dev_alloc(ctx, &ctx->obs4, Bm * P);
   rc |= dev_alloc(ctx, &ctx->image_observed_u8, Bm * 3 * P);
   rc |= dev_alloc(ctx, &ctx->cls_dev, Bm);
+  rc |= dev_alloc(ctx, &ctx->frame_dev, Bm);
   rc |= dev_alloc(ctx, &ctx->poses_dev, 8 * Bm * 12);
   rc |= dev_alloc(ctx, &ctx->se3_hist_dev, 8 * Bm * 7);
   rc |= dev_alloc(ctx, &ctx->light_pos, Bm * 3);
@@ -457,10 +458,10 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
   int rows, cols, pad; __nv_bfloat16 *hi, *lo;
   net_input_geometry(ctx, &rows, &cols, &pad, &hi, &lo);
   const bool depth = net_input_depth(ctx);  // RGB-D network: ren4.w = depth, obs4.w = depth_observed
-  // image-only network (ZoomImage): both boxes come from the colours; the observed one once per call
+  // image-only network (ZoomImage): both boxes come from the colours; the observed one once per call and frame
   const bool mask = net_input_mask(ctx);
   if (!mask)
-    if (int rc = obs_colour_box_launch(ctx, a.obs4, a.B, ctx->bbox_obs, st)) return rc;
+    if (int rc = obs_colour_box_launch(ctx, a.obs4, a.n_frames, ctx->bbox_obs, st)) return rc;
   const double *pose_src = a.pose_init;
   for (int it = 0; it < a.n_iter; ++it) {
     DimNvtxRange r_it("dim_refine iteration");
@@ -497,20 +498,22 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
     float *zf_it = a.zoom_factor ? a.zoom_factor + (size_t)it * a.B * 4 : ctx->zoom_factor;
     int *bbox_it = a.bbox ? a.bbox + (size_t)it * a.B * 8 : nullptr;
     // per-iteration status (bit 0: rendered / observed mask empty -> fallback zoom factor; bit 1: bad class index;
-    // image-only network: bit 0 = observed image empty, bit 2 = rendered image empty -> zoom centred on the observed box)
+    // image-only network: bit 0 = observed image empty, bit 2 = rendered image empty -> zoom centred on the observed box;
+    // bit 3: frame index out of range -> frame 0 observed)
     {
       DimNvtxRange r("bbox + zoom");
       int *status_it = ctx->status_hist + (size_t)(it < 8 ? it : 7) * a.B;
       if (mask) {
-        if (int rc = zoom_factor_from_ren_launch(ctx, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it, bbox_it, status_it, st))
+        if (int rc = zoom_factor_from_ren_launch(ctx, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it, bbox_it, status_it, st,
+                                                 a.frame_idx, a.n_frames))
           return rc;
       } else if (int rc = zoom_factor_from_boxes_launch(ctx, ctx->bbox_obs, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it,
-                                                        bbox_it, status_it, st)) {
+                                                        bbox_it, status_it, st, a.frame_idx, a.n_frames)) {
         return rc;
       }
       if (int rc = zoom_fused_launch(ctx, a.obs4, ctx->ren4, zf_it, means_f, a.B, rows, cols, pad, hi,
                                      a.precision == DIM_PREC_BF16X3 ? lo : nullptr, st, a.precision == DIM_PREC_FP16, a.means,
-                                     depth, mask))
+                                     depth, mask, a.frame_idx, a.n_frames))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[2], st));
@@ -591,6 +594,20 @@ static RefineArgs refine_args(int32_t B, int32_t n_iter, const float *K9, float 
   return a;
 }
 
+// dim_refine / dim_refine_frames once the arguments are checked: the F observed frames (and their depths) packed into obs4
+// outside the graph, then the chain; frame_idx nullptr = instance b observes frame b (F == B)
+static int refine_device(dim_ctx *ctx, RefineArgs &a, const float *frames, int32_t F, const int32_t *frame_idx,
+                         const float *depth, cudaStream_t st) {
+  a.obs4 = ctx->obs4; a.frame_idx = frame_idx; a.n_frames = F;
+  // the graph never reads the depth: it is packed into obs4.w below, outside the graph, like the image, so a replay is
+  // correct whatever the key holds; keying on it only costs one capture per distinct depth buffer
+  a.depth_observed = depth;
+  if (int rc = pack_obs4_launch(ctx, frames, F, ctx->obs4, a.means, st)) return rc;
+  if (depth)
+    if (int rc = obs4_depth_launch(ctx, ctx->obs4, F, depth, nullptr, 0.f, st)) return rc;
+  return refine_graphed(ctx, a, st);
+}
+
 DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
                            int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
                            int32_t precision, const double *pose_override, double *poses, float *se3, float *zoom_factor,
@@ -600,17 +617,75 @@ DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int3
   if (int rc = lit_check(ctx, lighting, "dim_refine")) return rc;
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine: batch exceeds max_batch");
   DIM_REQUIRE(n_iter >= 1, "dim_refine: n_iter must be >= 1");
-  cudaStream_t st = (cudaStream_t)stream;
   RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
-  a.obs4 = ctx->obs4; a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
+  a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
   a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
-  // the graph never reads depth_observed: it is packed into obs4.w below, outside the graph, like the image, so a replay is
-  // correct whatever the key holds; keying on it only costs one capture per distinct depth buffer
-  a.depth_observed = depth_observed;
-  if (int rc = pack_obs4_launch(ctx, image_observed, B, ctx->obs4, means, st)) return rc;
-  if (depth_observed)
-    if (int rc = obs4_depth_launch(ctx, ctx->obs4, B, depth_observed, nullptr, 0.f, st)) return rc;
-  return refine_graphed(ctx, a, st);
+  return refine_device(ctx, a, image_observed, B, nullptr, depth_observed, (cudaStream_t)stream);
+}
+
+// frame-indexed dim_refine: F observed frames, instance b observes frame frame_idx[b] (device; checked in the kernels)
+DIM_API int32_t dim_refine_frames(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx,
+                                  const int32_t *cls_idx, const double *pose_init, int32_t B, int32_t n_iter, const float *K9,
+                                  float zn, float zf, const double *means, int32_t precision, const double *pose_override,
+                                  double *poses, float *se3, float *zoom_factor, int32_t *bbox, const float *depth_frames,
+                                  const dim_lighting *lighting, void *stream) {
+  DIM_REQUIRE(ctx && image_frames && frame_idx && cls_idx && pose_init && K9 && means && poses,
+              "dim_refine_frames: NULL argument");
+  if (int rc = depth_check(ctx, depth_frames, depth_frames, "dim_refine_frames", "depth_frames")) return rc;
+  if (int rc = lit_check(ctx, lighting, "dim_refine_frames")) return rc;
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_frames: batch exceeds max_batch");
+  DIM_REQUIRE(F >= 1 && F <= ctx->max_batch, "dim_refine_frames: frame count F outside [1, max_batch]");
+  DIM_REQUIRE(n_iter >= 1, "dim_refine_frames: n_iter must be >= 1");
+  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
+  a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
+  a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
+  return refine_device(ctx, a, image_frames, F, frame_idx, depth_frames, (cudaStream_t)stream);
+}
+
+// the host entries once their scalar arguments are checked: the class and frame indices are checked here, before anything
+// is enqueued; fn names the entry point in the messages.  frame_host nullptr = instance b observes frame b (F == B)
+static int refine_host_enqueue(dim_ctx *ctx, const char *fn, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
+                               const int32_t *cls_host, const double *pose_host, int32_t B, int32_t n_iter, const float *K9,
+                               float zn, float zf, const double *means, int32_t precision, double *poses_out, float *se3_out,
+                               const uint16_t *depth_u16, float depth_factor, const dim_lighting *lighting, cudaStream_t st) {
+  for (int32_t i = 0; i < B; ++i) {  // the class indices are on the host here: fail loudly (the reference indexes a python list)
+    const int32_t c = cls_host[i];
+    if (c < 0 || c >= ctx->max_classes || ctx->meshes_host[c].V <= 0) {
+      set_error("%s: instance %d has class index %d: out of range [0,%d) or no mesh uploaded for it", fn, (int)i, (int)c,
+                (int)ctx->max_classes);
+      return 2;
+    }
+  }
+  if (frame_host)  // so are the frame indices: nothing is enqueued when one is out of range
+    for (int32_t i = 0; i < B; ++i)
+      if (frame_host[i] < 0 || frame_host[i] >= F) {
+        set_error("%s: instance %d has frame index %d: out of range [0,%d)", fn, (int)i, (int)frame_host[i], (int)F);
+        return 2;
+      }
+  const size_t P = (size_t)ctx->H * ctx->W;
+  DIM_CHECK(cudaMemcpyAsync(ctx->image_observed_u8, frames_u8, (size_t)F * 3 * P, cudaMemcpyHostToDevice, st));
+  DIM_CHECK(cudaMemcpyAsync(ctx->cls_dev, cls_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
+  DIM_CHECK(cudaMemcpyAsync(ctx->pose_cur, pose_host, sizeof(double) * B * 12, cudaMemcpyHostToDevice, st));
+  if (frame_host) DIM_CHECK(cudaMemcpyAsync(ctx->frame_dev, frame_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
+  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
+  a.obs4 = ctx->obs4; a.cls_idx = ctx->cls_dev; a.pose_init = ctx->pose_cur; a.poses = ctx->poses_dev;
+  a.se3 = ctx->se3_hist_dev;
+  a.frame_idx = frame_host ? ctx->frame_dev : nullptr; a.n_frames = F;
+  if (lighting) {  // the intensities move to the context's buffer (a fixed address: graphs)
+    a.intensity = ctx->lit_intensity;
+    DIM_CHECK(cudaMemcpyAsync(ctx->lit_intensity, lighting->intensity, sizeof(float) * (size_t)n_iter * B * 3,
+                              cudaMemcpyHostToDevice, st));
+  }
+  if (int rc = transform_u8_obs4_launch(ctx, ctx->image_observed_u8, F, means, ctx->obs4, st)) return rc;
+  if (depth_u16) {  // the converted depth lands in obs4 outside the graph, like the image
+    DIM_CHECK(cudaMemcpyAsync(ctx->depth_u16, depth_u16, sizeof(uint16_t) * F * P, cudaMemcpyHostToDevice, st));
+    if (int rc = obs4_depth_launch(ctx, ctx->obs4, F, nullptr, ctx->depth_u16, depth_factor, st)) return rc;
+  }
+  if (int rc = refine_graphed(ctx, a, st)) return rc;
+  DIM_CHECK(cudaMemcpyAsync(poses_out, ctx->poses_dev, sizeof(double) * (size_t)n_iter * B * 12, cudaMemcpyDeviceToHost, st));
+  if (se3_out)
+    DIM_CHECK(cudaMemcpyAsync(se3_out, ctx->se3_hist_dev, sizeof(float) * (size_t)n_iter * B * 7, cudaMemcpyDeviceToHost, st));
+  return 0;
 }
 
 // lighting: the caller's lighting with HOST intensities [n_iter,B,3]; depth_u16: the caller's host depth file values [B,H,W]
@@ -625,36 +700,38 @@ DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *img_u8, const
   if (int rc = lit_check(ctx, lighting, "dim_refine_host")) return rc;
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_host: batch exceeds max_batch");
   DIM_REQUIRE(n_iter >= 1 && n_iter <= 8, "dim_refine_host: n_iter must be in [1,8]");
-  for (int32_t i = 0; i < B; ++i) {  // the class indices are on the host here: fail loudly (the reference indexes a python list)
-    const int32_t c = cls_host[i];
-    if (c < 0 || c >= ctx->max_classes || ctx->meshes_host[c].V <= 0) {
-      set_error("dim_refine_host: instance %d has class index %d: out of range [0,%d) or no mesh uploaded for it", (int)i, (int)c,
-                (int)ctx->max_classes);
-      return 2;
-    }
-  }
-  cudaStream_t st = (cudaStream_t)stream;
-  const size_t P = (size_t)ctx->H * ctx->W;
-  DIM_CHECK(cudaMemcpyAsync(ctx->image_observed_u8, img_u8, (size_t)B * 3 * P, cudaMemcpyHostToDevice, st));
-  DIM_CHECK(cudaMemcpyAsync(ctx->cls_dev, cls_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
-  DIM_CHECK(cudaMemcpyAsync(ctx->pose_cur, pose_host, sizeof(double) * B * 12, cudaMemcpyHostToDevice, st));
-  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
-  a.obs4 = ctx->obs4; a.cls_idx = ctx->cls_dev; a.pose_init = ctx->pose_cur; a.poses = ctx->poses_dev;
-  a.se3 = ctx->se3_hist_dev;
-  if (lighting) {  // the intensities move to the context's buffer (a fixed address: graphs)
-    a.intensity = ctx->lit_intensity;
-    DIM_CHECK(cudaMemcpyAsync(ctx->lit_intensity, lighting->intensity, sizeof(float) * (size_t)n_iter * B * 3,
-                              cudaMemcpyHostToDevice, st));
-  }
-  if (int rc = transform_u8_obs4_launch(ctx, ctx->image_observed_u8, B, means, ctx->obs4, st)) return rc;
-  if (depth_u16) {  // the converted depth lands in obs4 outside the graph, like the image
-    DIM_CHECK(cudaMemcpyAsync(ctx->depth_u16, depth_u16, sizeof(uint16_t) * B * P, cudaMemcpyHostToDevice, st));
-    if (int rc = obs4_depth_launch(ctx, ctx->obs4, B, nullptr, ctx->depth_u16, depth_factor, st)) return rc;
-  }
-  if (int rc = refine_graphed(ctx, a, st)) return rc;
-  DIM_CHECK(cudaMemcpyAsync(poses_out, ctx->poses_dev, sizeof(double) * (size_t)n_iter * B * 12, cudaMemcpyDeviceToHost, st));
-  if (se3_out)
-    DIM_CHECK(cudaMemcpyAsync(se3_out, ctx->se3_hist_dev, sizeof(float) * (size_t)n_iter * B * 7, cudaMemcpyDeviceToHost, st));
+  return refine_host_enqueue(ctx, "dim_refine_host", img_u8, B, nullptr, cls_host, pose_host, B, n_iter, K9, zn, zf, means,
+                             precision, poses_out, se3_out, depth_u16, depth_factor, lighting, (cudaStream_t)stream);
+}
+
+// frame-indexed dim_refine_host_async: F host frames [F,H,W,3] (depth [F,H,W]), frame_host [B] checked before any enqueue
+DIM_API int32_t dim_refine_frames_host_async(dim_ctx *ctx, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
+                                             const int32_t *cls_host, const double *pose_host, int32_t B, int32_t n_iter,
+                                             const float *K9, float zn, float zf, const double *means, int32_t precision,
+                                             double *poses_out, float *se3_out, const uint16_t *depth_u16, float depth_factor,
+                                             const dim_lighting *lighting, void *stream) {
+  DIM_REQUIRE(ctx && frames_u8 && frame_host && cls_host && pose_host && K9 && means && poses_out,
+              "dim_refine_frames_host: NULL argument");
+  if (int rc = depth_check(ctx, depth_u16, depth_u16, "dim_refine_frames_host", "depth_frames_u16_host")) return rc;
+  if (depth_u16)
+    DIM_REQUIRE(depth_factor > 0.f && depth_factor < 3.0e38f, "dim_refine_frames_host: depth_factor must be positive and finite");
+  if (int rc = lit_check(ctx, lighting, "dim_refine_frames_host")) return rc;
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_frames_host: batch exceeds max_batch");
+  DIM_REQUIRE(F >= 1 && F <= ctx->max_batch, "dim_refine_frames_host: frame count F outside [1, max_batch]");
+  DIM_REQUIRE(n_iter >= 1 && n_iter <= 8, "dim_refine_frames_host: n_iter must be in [1,8]");
+  return refine_host_enqueue(ctx, "dim_refine_frames_host", frames_u8, F, frame_host, cls_host, pose_host, B, n_iter, K9, zn, zf,
+                             means, precision, poses_out, se3_out, depth_u16, depth_factor, lighting, (cudaStream_t)stream);
+}
+
+DIM_API int32_t dim_refine_frames_host(dim_ctx *ctx, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
+                                       const int32_t *cls_host, const double *pose_host, int32_t B, int32_t n_iter,
+                                       const float *K9, float zn, float zf, const double *means, int32_t precision,
+                                       double *poses_out, float *se3_out, const uint16_t *depth_u16, float depth_factor,
+                                       const dim_lighting *lighting, void *stream) {
+  if (int rc = dim_refine_frames_host_async(ctx, frames_u8, F, frame_host, cls_host, pose_host, B, n_iter, K9, zn, zf, means,
+                                            precision, poses_out, se3_out, depth_u16, depth_factor, lighting, stream))
+    return rc;
+  DIM_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
   return 0;
 }
 
@@ -669,11 +746,11 @@ DIM_API int32_t dim_refine_host(dim_ctx *ctx, const uint8_t *img_u8, const int32
   return 0;
 }
 
-// status of the LAST dim_refine / dim_refine_host(_async) call on this context: [min(n_iter, 8), B] int32, device -> host
-// (asynchronous on `stream`, which must be the stream that call ran on).  0 = ok; bit 0 = the rendered mask of that
-// iteration was empty (object left the frustum: the reference crashes in ZoomMask, np.min of an empty array; here the
-// fallback zoom factor (1,1,0,0) was used and the pose of that instance is meaningless); bit 1 = class index out of range
-// or no mesh uploaded for it.
+// status of the LAST dim_refine / dim_refine_host(_async) / dim_refine_frames(_host(_async)) call on this context:
+// [min(n_iter, 8), B] int32, device -> host (asynchronous on `stream`, which must be the stream that call ran on).  0 = ok;
+// bit 0 = the rendered mask of that iteration was empty (object left the frustum: the reference crashes in ZoomMask, np.min
+// of an empty array; here the fallback zoom factor (1,1,0,0) was used and the pose of that instance is meaningless); bit 1 =
+// class index out of range or no mesh uploaded for it; bit 3 = dim_refine_frames: frame index out of range (frame 0 used).
 DIM_API int32_t dim_refine_status(dim_ctx *ctx, int32_t B, int32_t n_iter, int32_t *status_host, void *stream) {
   DIM_REQUIRE(ctx && status_host && B >= 1 && B <= ctx->max_batch && n_iter >= 1, "dim_refine_status: bad argument");
   const int n = n_iter < 8 ? n_iter : 8;

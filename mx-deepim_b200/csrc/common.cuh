@@ -80,7 +80,8 @@ struct NetState;  // net_state.cuh
 // no padding).  Not in the key, because drop_graphs discards every graph when they change: ctx->cfg (trans means / stds,
 // rot_coord), mesh uploads, network weights and the "graph" option.
 struct RefineArgs {
-  const float4 *obs4;
+  const float4 *obs4;        // n_frames observed frames
+  const int32_t *frame_idx;  // device [B]: the frame instance b observes (read at replay); nullptr = frame b (dim_refine)
   const int32_t *cls_idx;
   const double *pose_init, *pose_override;  // pose_override: nullable [n_iter,B,3,4] source pose of every iteration
   double *poses;
@@ -91,8 +92,10 @@ struct RefineArgs {
   double means[3], offset[3];  // offset: the light's (lit only)
   float K9[9], zn, zf, brightness_ratio;
   int32_t B, n_iter, precision, lit;
+  int32_t n_frames;  // frames in obs4 (dim_refine: B)
+  int32_t zero;      // always 0: fills what would otherwise be tail padding
 };
-static_assert(sizeof(RefineArgs) == 10 * sizeof(void *) + 6 * sizeof(double) + 12 * sizeof(float) + 4 * sizeof(int32_t),
+static_assert(sizeof(RefineArgs) == 11 * sizeof(void *) + 6 * sizeof(double) + 12 * sizeof(float) + 6 * sizeof(int32_t),
               "RefineArgs must have no padding: its bytes are the graph key");
 
 }  // namespace dim
@@ -122,6 +125,7 @@ struct dim_ctx {
   float4 *ren4 = nullptr, *obs4 = nullptr;  // [max_batch,H,W] pixel-interleaved images of the fused loop
   uint8_t *image_observed_u8 = nullptr;
   int *cls_dev = nullptr;
+  int *frame_dev = nullptr;     // [max_batch] dim_refine_frames_host: the caller's frame index of every instance
   double *poses_dev = nullptr;  // [8, max_batch, 12]
   float *se3_hist_dev = nullptr;
   float *light_pos = nullptr;      // [max_batch,3] lit chain / lit train update: light of the pose being rendered

@@ -32,15 +32,19 @@ int zoom_gather_launch(dim_ctx *ctx, int mode, const float *src, float *dst, con
 int zoom_factor_launch(dim_ctx *ctx, const float *mask_real, const float *mask_ren, int C, const float *src_pose, int B,
                        const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
                        const float *img_means = nullptr);
+// frame_idx / n_frames: the fused loop's map from instance to observed frame (RefineArgs); nullptr = frame b
 int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *src_pose, int B, const float *K9,
-                                float *zoom_factor, int *bbox_out, int *status, cudaStream_t st);
-int obs_colour_box_launch(dim_ctx *ctx, const float4 *obs4, int B, int *bbox_obs, cudaStream_t st);
+                                float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
+                                const int32_t *frame_idx = nullptr, int n_frames = 0);
+int obs_colour_box_launch(dim_ctx *ctx, const float4 *obs4, int F, int *bbox_obs, cudaStream_t st);
 int zoom_factor_from_boxes_launch(dim_ctx *ctx, const int *bbox_obs, const int *bbox_ren, const float *src_pose, int B,
-                                  const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st);
+                                  const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
+                                  const int32_t *frame_idx = nullptr, int n_frames = 0);
 int box_mask_launch(dim_ctx *ctx, const int *bbox, int B, float *mask, cudaStream_t st);
 int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, const float *zoom_factor,
                       const float *means_rgb, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
-                      cudaStream_t st, int f16, const double *means_d, bool depth = false, bool mask = true);
+                      cudaStream_t st, int f16, const double *means_d, bool depth = false, bool mask = true,
+                      const int32_t *frame_idx = nullptr, int n_frames = 0);
 int obs4_depth_launch(dim_ctx *ctx, float4 *obs4, int B, const float *depth, const uint16_t *depth_u16, float factor,
                       cudaStream_t st);
 int pack_nhwc10_launch(dim_ctx *ctx, const float *io, const float *ir, const float *dobs, const float *dren, const float *mo,

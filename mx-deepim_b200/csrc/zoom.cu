@@ -59,15 +59,32 @@ __global__ void __launch_bounds__(160) mask_bbox_kernel(const float *mask_real, 
   }
 }
 
+// The observed frame of instance b in the fused loop (dim_refine_frames): frame_idx[b], or frame 0 when that lies outside
+// [0, n_frames) -- a bad index never reads outside the packed frames; the zoom factor flags it as status bit 3.
+// frame_idx == nullptr: instance b observes frame b (dim_refine).
+__device__ __forceinline__ int frame_of(const int32_t *frame_idx, int n_frames, int b) {
+  if (!frame_idx) return b;
+  const int f = __ldg(frame_idx + b);
+  return (f >= 0 && f < n_frames) ? f : 0;
+}
+__device__ __forceinline__ bool frame_bad(const int32_t *frame_idx, int n_frames, int b) {
+  if (!frame_idx) return false;
+  const int f = __ldg(frame_idx + b);
+  return f < 0 || f >= n_frames;
+}
+
 // zoom factor, one thread per instance (zoom_mask.py:59-103; ZoomImage's is the same code, zoom_image.py:41-86).  Mixed
 // precision as the reference's numpy 1.x: c = K.t and c_x = c0/c2 in float32, everything after in float64, stored as float32.
 // ren_empty_bit: status bit set where the rendered box is empty and the zoom centres on the observed box (0: none)
+// frame_idx / n_frames (fused loop, nullable): an instance whose frame index is out of range gets status bit 3
 __global__ void zoom_factor_kernel(int *bbox8, const float *src_pose, int B, int H, int W, float k0, float k1,
                                    float k2, float k3, float k4, float k5, float k6, float k7, float k8,
-                                   float *zoom_factor, int *bbox_out, int *status, const int *cls_flag, int ren_empty_bit) {
+                                   float *zoom_factor, int *bbox_out, int *status, const int *cls_flag, int ren_empty_bit,
+                                   const int32_t *frame_idx, int n_frames) {
   int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  const int cf = cls_flag ? cls_flag[b] : 0;  // rasteriser: bad class index (bit 1)
+  // rasteriser: bad class index (bit 1); frame index out of range (bit 3)
+  const int cf = (cls_flag ? cls_flag[b] : 0) | (frame_bad(frame_idx, n_frames, b) ? 8 : 0);
   int *bb = bbox8 + 8 * b;
   if (bb[1] < 0) bb[0] = bb[1] = bb[2] = bb[3] = -1;
   if (bb[5] < 0) bb[4] = bb[5] = bb[6] = bb[7] = -1;
@@ -243,7 +260,8 @@ int zoom_factor_launch(dim_ctx *ctx, const float *mask_real, const float *mask_r
                                                        img_means ? img_means[1] : 0.f, img_means ? img_means[2] : 0.f);
   DIM_LAUNCH_CHECK();
   zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
-                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, nullptr, 0);
+                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, nullptr, 0,
+                                                  nullptr, 0);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -265,18 +283,21 @@ __global__ void zoom_factor_from_ren_kernel(const int *bbox_ren, int *bbox8, int
 }
 
 int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *src_pose, int B, const float *K9,
-                                float *zoom_factor, int *bbox_out, int *status, cudaStream_t st) {
+                                float *zoom_factor, int *bbox_out, int *status, cudaStream_t st, const int32_t *frame_idx,
+                                int n_frames) {
   zoom_factor_from_ren_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_ren, ctx->bbox8, B);
   DIM_LAUNCH_CHECK();
   zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
-                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag, 0);
+                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag, 0,
+                                                  frame_idx, n_frames);
   DIM_LAUNCH_CHECK();
   return 0;
 }
 
 // Image-only network (ZoomImage, zoom_image.py:33-37): the observed box of the fused loop, valid = sum_c(image + mean) > 0.01
 // over obs4's colours (which hold image + mean), the float32 sum of mask_bbox_kernel's img_mode in the same channel order.
-// Once per dim_refine call: the observed image does not change over the iterations.  One block per (row, instance).
+// Once per dim_refine call: the observed image does not change over the iterations.  One block per (row, frame): with
+// dim_refine_frames each frame's box is reduced once, however many instances observe it.
 __global__ void __launch_bounds__(160) obs_colour_box_kernel(const float4 *obs4, int H, int W, int *bbox_obs) {
   const int i = blockIdx.x, b = blockIdx.y;
   const float4 *src = obs4 + ((size_t)b * H + i) * W;
@@ -308,10 +329,10 @@ __global__ void box4_init_kernel(int *box, int B, int H, int W) {
   box[4 * b + 3] = -1;
 }
 
-int obs_colour_box_launch(dim_ctx *ctx, const float4 *obs4, int B, int *bbox_obs, cudaStream_t st) {
-  box4_init_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_obs, B, ctx->H, ctx->W);
+int obs_colour_box_launch(dim_ctx *ctx, const float4 *obs4, int F, int *bbox_obs, cudaStream_t st) {
+  box4_init_kernel<<<cdiv(F, 64), 64, 0, st>>>(bbox_obs, F, ctx->H, ctx->W);
   DIM_LAUNCH_CHECK();
-  obs_colour_box_kernel<<<dim3(ctx->H, B), 160, 0, st>>>(obs4, ctx->H, ctx->W, bbox_obs);
+  obs_colour_box_kernel<<<dim3(ctx->H, F), 160, 0, st>>>(obs4, ctx->H, ctx->W, bbox_obs);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -319,22 +340,27 @@ int obs_colour_box_launch(dim_ctx *ctx, const float4 *obs4, int B, int *bbox_obs
 // zoom factor of the image-only loop: the observed box from obs_colour_box_kernel, the rendered one from the rasteriser's
 // colour-valid bbox (raster.cu COLOUR_BOX), then ZoomImage's arithmetic -- zoom_factor_kernel, with the observed-centre
 // fallback for an empty render flagged as status bit 2 (the reference prints "NO POINT VALID IN rendered" and goes on); an
-// empty observed image is bit 0 with the (1,1,0,0) factor (the reference raises)
-__global__ void boxes_to_bbox8_kernel(const int *bbox_obs, const int *bbox_ren, int *bbox8, int B) {
+// empty observed image is bit 0 with the (1,1,0,0) factor (the reference raises).
+// bbox_obs holds one box per frame; the instance's observed box is gathered here from its frame (frame_of).
+__global__ void boxes_to_bbox8_kernel(const int *bbox_obs, const int *bbox_ren, int *bbox8, int B, const int32_t *frame_idx,
+                                      int n_frames) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
+  const int f = frame_of(frame_idx, n_frames, b);
   for (int k = 0; k < 4; ++k) {
-    bbox8[8 * b + k] = bbox_obs[4 * b + k];
+    bbox8[8 * b + k] = bbox_obs[4 * f + k];
     bbox8[8 * b + 4 + k] = bbox_ren[4 * b + k];
   }
 }
 
 int zoom_factor_from_boxes_launch(dim_ctx *ctx, const int *bbox_obs, const int *bbox_ren, const float *src_pose, int B,
-                                  const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st) {
-  boxes_to_bbox8_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_obs, bbox_ren, ctx->bbox8, B);
+                                  const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
+                                  const int32_t *frame_idx, int n_frames) {
+  boxes_to_bbox8_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_obs, bbox_ren, ctx->bbox8, B, frame_idx, n_frames);
   DIM_LAUNCH_CHECK();
   zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
-                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag, 4);
+                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag, 4,
+                                                  frame_idx, n_frames);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -367,7 +393,9 @@ int box_mask_launch(dim_ctx *ctx, const int *bbox, int B, float *mask, cudaStrea
 // The two source images already hold (image + mean) -- the sampler's first step, done once by their producers with the
 // same float32 addition -- so a tap costs no arithmetic before its weight.
 struct FusedZoomParams {
-  const float4 *obs4;   // [B,H,W,4] observed (RGB - mean) + mean, w unused (RGB-D network: w = depth_observed)
+  const float4 *obs4;   // [F,H,W,4] observed frames (RGB - mean) + mean, w unused (RGB-D network: w = depth_observed)
+  const int32_t *frame_idx;  // [B] frame of each instance (frame_of); nullptr: frame b
+  int n_frames;
   const float4 *ren4;   // [B,H,W,4] rendered (RGB - mean) + mean, w = mask_rendered (0/1) (RGB-D network: w = depth)
   const int *bbox8;     // observed box = bb[0..3] (inclusive)
   const int *vbox;      // [B,4] x0,x1,y0,y1: ren4 is only valid inside this box (rasteriser), background outside; nullable
@@ -504,6 +532,7 @@ __device__ __forceinline__ void zoom_fused_pixel(const FusedZoomParams &p, const
 // slots are rewritten with zeros.  Sources are the pixel-interleaved float4 images, so each tap is one 16-byte load
 // per image; the column taps of the quad's two columns and the row taps of its two rows are computed once each.
 // DEPTH: the RGB-D network's input, two chunk planes per quad slot: [B*Hs rows][8 planes = (slot, half)][Ws cols][8 ch]
+// Instance b's observed taps come from frame frame_of(b) of obs4 (dim_refine_frames), its rendered taps from ren4[b].
 template <bool LO, bool F16, bool DEPTH = false, bool MASK = true>
 __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParams p) {
   const int b = blockIdx.y;
@@ -523,8 +552,8 @@ __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParam
     xt[k] = axis_tap(j0 + k, z.x, z.z, p.W, p.stepx, vb.x, vb.y, bb.x, bb.y);
     yt[k] = axis_tap(i0 + k, z.y, z.w, p.H, p.stepy, vb.z, vb.w, bb.z, bb.w);
   }
-  const size_t base = (size_t)b * p.H * p.W;
-  const float4 *ob = p.obs4 + base, *rn = p.ren4 + base;
+  const size_t P = (size_t)p.H * p.W;
+  const float4 *ob = p.obs4 + (size_t)frame_of(p.frame_idx, p.n_frames, b) * P, *rn = p.ren4 + (size_t)b * P;
   // conv1 strip layout: [B*Hs rows][4 chunks (= quad slot)][Ws cols][8 ch] (DEPTH: 2 chunks per slot)
   constexpr int NC = DEPTH ? 2 : 1;
 #pragma unroll
@@ -545,9 +574,11 @@ __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParam
 
 int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, const float *zoom_factor,
                       const float *means_rgb, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
-                      cudaStream_t st, int f16, const double *means_d, bool depth, bool mask) {
+                      cudaStream_t st, int f16, const double *means_d, bool depth, bool mask, const int32_t *frame_idx,
+                      int n_frames) {
   FusedZoomParams p;
   p.obs4 = obs4; p.ren4 = ren4;
+  p.frame_idx = frame_idx; p.n_frames = n_frames;
   p.bbox8 = ctx->bbox8; p.zoom_factor = zoom_factor;
   p.vbox = means_d ? ctx->vbox : nullptr;  // means_d given: ren4 comes from the fused loop's box-only render
   for (int c = 0; c < 3; ++c) p.bg[c] = (means_d ? (float)(0.0 - means_d[c]) : 0.f) + means_rgb[c];

@@ -517,11 +517,90 @@ class Context:
                  None if lit is None else C.byref(lit), self._stream()))
         return poses_out, se3_out
 
+    def refine_frames(self, frames, frame_idx, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
+                      pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, pose_override=None, out=None,
+                      lighting=None, depth_frames=None):
+        """refine() against F shared observed frames: frames f32[F,3,H,W] (RGB - mean), frame_idx i32[B] CUDA (instance b
+        observes frames[frame_idx[b]]), 1 <= F <= max_batch.  Instance b's results equal refine(frames[frame_idx], ...)'s, bit
+        for bit; each frame is packed once.  An index outside [0, F) is not an error here: that instance observes frame 0
+        and refine_status() reports bit 3.  Writing new indices into the same frame_idx tensor replays the captured graph.
+        depth_frames: f32 [F,1,H,W] CUDA, metres -- required on an RGB-D context, refused otherwise.  Every other argument
+        as refine()."""
+        F, B = frames.shape[0], cls_idx.shape[0]
+        _chk(frames, torch.float32, (F, 3, self.H, self.W), "frames")
+        _chk(frame_idx, torch.int32, (B,), "frame_idx")
+        _chk(cls_idx, torch.int32, (B,), "cls_idx")
+        _chk(pose_init, torch.float64, (B, 3, 4), "pose_init")
+        if out is not None:
+            poses, se3, zf, bbox = out["poses"], out["se3"], out["zoom_factor"], out["bbox"]
+            _chk(poses, torch.float64, (n_iter, B, 3, 4), "out['poses']")
+            _chk(se3, torch.float32, (n_iter, B, 7), "out['se3']")
+            _chk(zf, torch.float32, (n_iter, B, 4), "out['zoom_factor']")
+            _chk(bbox, torch.int32, (n_iter, B, 8), "out['bbox']")
+        else:
+            poses = self._new((n_iter, B, 3, 4), torch.float64)
+            se3 = self._new((n_iter, B, 7))
+            zf = self._new((n_iter, B, 4))
+            bbox = self._new((n_iter, B, 8), torch.int32)
+        if pose_override is not None:
+            _chk(pose_override, torch.float64, (n_iter, B, 3, 4), "pose_override")
+        if depth_frames is not None:
+            _chk(depth_frames, torch.float32, (F, 1, self.H, self.W), "depth_frames")
+        lit = None if lighting is None else C.byref(_lighting_arg(lighting, (n_iter, B, 3), True)[0])
+        check(lib.dim_refine_frames(self._h, _p(frames), F, _p(frame_idx), _p(cls_idx), _p(pose_init), B, n_iter,
+                                    farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
+                                    farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses), _p(se3),
+                                    _p(zf), _p(bbox), _p(depth_frames), lit, self._stream()))
+        return {"poses": poses, "se3": se3, "zoom_factor": zf, "bbox": bbox}
+
+    def refine_frames_host(self, frames_u8, frame_idx, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
+                           pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, poses_out=None,
+                           se3_out=None, sync=True, lighting=None, depth_frames_u16=None, depth_factor=1000.0):
+        """refine_host() against F shared observed frames: frames_u8 uint8 [F,H,W,3] BGR, frame_idx int32 [B] (host; every
+        index is checked: one outside [0, F) raises before anything is enqueued), depth_frames_u16 uint16 [F,H,W] on an
+        RGB-D context.  Each frame is uploaded once.  Every other argument as refine_host()."""
+        def hptr(a):
+            return C.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else C.c_void_p(a.ctypes.data)
+
+        def host(a, dtype, tdtype, name):
+            if isinstance(a, torch.Tensor):
+                if a.is_cuda or a.dtype != tdtype:
+                    raise ValueError("%s must be a host %s array" % (name, np.dtype(dtype).name))
+                return a.contiguous()
+            return np.ascontiguousarray(a, dtype)
+        F = frames_u8.shape[0]
+        fidx = host(frame_idx, np.int32, torch.int32, "frame_idx")
+        cls = host(cls_idx, np.int32, torch.int32, "cls_idx")
+        pose = host(pose_init, np.float64, torch.float64, "pose_init")
+        B = cls.shape[0]
+        if tuple(fidx.shape) != (B,):
+            raise ValueError("frame_idx: expected shape %s, got %s" % ((B,), tuple(fidx.shape)))
+        if tuple(frames_u8.shape) != (F, self.H, self.W, 3):
+            raise ValueError("frames_u8: expected shape %s, got %s" % ((F, self.H, self.W, 3), tuple(frames_u8.shape)))
+        if poses_out is None:
+            poses_out = np.empty((n_iter, B, 3, 4), np.float64)
+        if se3_out is None:
+            se3_out = np.empty((n_iter, B, 7), np.float32)
+        dkeep = None
+        if depth_frames_u16 is not None:
+            dkeep = host(depth_frames_u16, np.uint16, torch.uint16, "depth_frames_u16")
+            if tuple(dkeep.shape) != (F, self.H, self.W):
+                raise ValueError("depth_frames_u16: expected shape %s, got %s" % ((F, self.H, self.W), tuple(dkeep.shape)))
+        frames = frames_u8 if isinstance(frames_u8, torch.Tensor) else np.ascontiguousarray(frames_u8, np.uint8)
+        lit, _keep = (None, None) if lighting is None else _lighting_arg(lighting, (n_iter, B, 3), False)
+        fn = lib.dim_refine_frames_host if sync else lib.dim_refine_frames_host_async
+        check(fn(self._h, hptr(frames), F, hptr(fidx), hptr(cls), hptr(pose), B, n_iter,
+                 farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision,
+                 hptr(poses_out), hptr(se3_out), None if dkeep is None else hptr(dkeep), float(np.float32(depth_factor)),
+                 None if lit is None else C.byref(lit), self._stream()))
+        return poses_out, se3_out
+
 
 def _refine_status(self, B, n_iter, out=None, sync=True):
-    """Per-iteration status of the last refine / refine_host call: int32 [min(n_iter,8), B]; 0 = ok, bit 0 = empty rendered
-    mask in that iteration (pose meaningless; the reference crashes there), bit 1 = bad class index.  `out`: pinned int32
-    tensor for an asynchronous copy on the current stream (sync=False)."""
+    """Per-iteration status of the last refine / refine_host / refine_frames(_host) call: int32 [min(n_iter,8), B]; 0 = ok,
+    bit 0 = empty rendered mask in that iteration (pose meaningless; the reference crashes there), bit 1 = bad class index,
+    bit 3 = refine_frames: frame index out of range (frame 0 observed).  `out`: pinned int32 tensor for an asynchronous copy
+    on the current stream (sync=False)."""
     n = min(int(n_iter), 8)
     if out is None:
         out = torch.empty((n, B), dtype=torch.int32).pin_memory()

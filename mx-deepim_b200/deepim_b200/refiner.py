@@ -15,7 +15,10 @@ refine then also take the observed depth as the loader's uint16 file values [N,H
 device as float32(u16) / float32(depth_factor).
 
 input_mask=False runs the image-only network (config.network.INPUT_MASK: False; weights with a (64, 6, 7, 7) flow_conv1): the
-loop zooms with ZoomImage, boxes from the images' colours."""
+loop zooms with ZoomImage, boxes from the images' colours.
+
+refine_frames / submit_frames refine instances that share observed frames (several objects in one image, several initial
+hypotheses of one object) against one uploaded copy of each frame (dim_refine_frames_host)."""
 from __future__ import annotations
 
 import numpy as np
@@ -25,6 +28,25 @@ from . import _capi as capi
 from . import lighting as _lighting
 from . import sharding, synth
 from .context import Context
+
+
+def plan_frame_batches(frame_of, n_frames: int, max_batch: int, lo: int = 0, hi=None):
+    """Device batches of PoseRefiner.refine_frames for instances [lo, hi) (default: all) of frame_of (instance i observes
+    frame frame_of[i] of n_frames): the contiguous slices of at most max_batch instances that refine() uses (sharding.chunks),
+    each with the frames it observes.  Returns [(a, b, frames, local)]: instances a..b-1, frames = the sorted global indices
+    of their frames (at most b - a <= max_batch of them), local int32 [b - a] = each instance's index into `frames`, so
+    frames[local[i]] == frame_of[a + i].  Raises ValueError naming the first instance whose frame index is outside
+    [0, n_frames)."""
+    f = np.asarray(frame_of).reshape(-1)
+    hi = len(f) if hi is None else hi
+    bad = np.nonzero((f < 0) | (f >= n_frames))[0]
+    if len(bad):
+        raise ValueError("instance %d has frame index %d: out of range [0,%d)" % (bad[0], f[bad[0]], n_frames))
+    out = []
+    for a, b in sharding.chunks(lo, hi, max_batch):
+        frames, local = np.unique(f[a:b], return_inverse=True)
+        out.append((a, b, frames, local.astype(np.int32).reshape(-1)))
+    return out
 
 
 class PoseRefiner:
@@ -56,7 +78,7 @@ class PoseRefiner:
                 "poses": torch.empty((n_iter, max_batch, 3, 4), dtype=torch.float64).pin_memory(),
                 "se3": torch.empty((n_iter, max_batch, 7), dtype=torch.float32).pin_memory(),
                 "status": torch.zeros((min(n_iter, 8) * max_batch,), dtype=torch.int32).pin_memory(),
-                "img": None, "cls": None, "pose": None, "depth": None,
+                "img": None, "cls": None, "pose": None, "depth": None, "frame": None,
                 "intensity": torch.empty((n_iter, max_batch, 3), dtype=torch.float32).pin_memory() if self.light else None,
             })
         self.ctx = self.slots[0]["ctx"]
@@ -80,6 +102,15 @@ class PoseRefiner:
         """Enqueue one batch (<= max_batch instances, host arrays; pinned torch tensors are used in place).
         depths_u16: uint16 [n,H,W], required with input_depth=True.
         Returns a ticket for result().  At most len(slots) batches may be in flight."""
+        return self._submit(images_bgr_u8, None, cls_idx, poses_init, depths_u16)
+
+    def submit_frames(self, frames_bgr_u8, frame_idx, cls_idx, poses_init, depths_u16=None):
+        """submit() against shared frames: frames_bgr_u8 uint8 [f,H,W,3] (f <= max_batch), frame_idx int [n] (instance i
+        observes frames_bgr_u8[frame_idx[i]]; checked before anything is enqueued), depths_u16 uint16 [f,H,W] with
+        input_depth=True.  Each frame is uploaded once."""
+        return self._submit(frames_bgr_u8, frame_idx, cls_idx, poses_init, depths_u16)
+
+    def _submit(self, images_bgr_u8, frame_idx, cls_idx, poses_init, depths_u16):
         i = self._next
         slot = self.slots[i]
         if slot["busy"]:
@@ -87,6 +118,8 @@ class PoseRefiner:
         n = len(cls_idx)
         if n > self.max_batch:
             raise ValueError("batch larger than max_batch")
+        if len(images_bgr_u8) > self.max_batch:
+            raise ValueError("more frames than max_batch")
         img = self._pinned(slot, "img", images_bgr_u8, torch.uint8)
         cls = self._pinned(slot, "cls", cls_idx, torch.int32)
         pose = self._pinned(slot, "pose", poses_init, torch.float64)
@@ -100,9 +133,15 @@ class PoseRefiner:
             inten.copy_(torch.from_numpy(self.light.draw((self.n_iter, n))))
             lit = self.light.lighting(inten)
         with torch.cuda.stream(slot["stream"]):
-            slot["ctx"].refine_host(img, cls, pose, self.K, self.n_iter, self.zn, self.zf, self.means, self.precision,
-                                    poses_out=slot["poses"], se3_out=slot["se3"], sync=False, lighting=lit,
-                                    depth_observed_u16=depth, depth_factor=self.depth_factor)
+            if frame_idx is None:
+                slot["ctx"].refine_host(img, cls, pose, self.K, self.n_iter, self.zn, self.zf, self.means, self.precision,
+                                        poses_out=slot["poses"], se3_out=slot["se3"], sync=False, lighting=lit,
+                                        depth_observed_u16=depth, depth_factor=self.depth_factor)
+            else:
+                fidx = self._pinned(slot, "frame", frame_idx, torch.int32)
+                slot["ctx"].refine_frames_host(img, fidx, cls, pose, self.K, self.n_iter, self.zn, self.zf, self.means,
+                                               self.precision, poses_out=slot["poses"], se3_out=slot["se3"], sync=False,
+                                               lighting=lit, depth_frames_u16=depth, depth_factor=self.depth_factor)
             slot["ctx"].refine_status(n, self.n_iter, out=slot["status"], sync=False)
         slot["busy"], slot["n"] = True, n
         self._next = (i + 1) % len(self.slots)
@@ -147,6 +186,30 @@ class PoseRefiner:
                 out[:, pa - lo:pb - lo] = self.result(t)
             d = None if depths_u16 is None else depths_u16[a:b]
             pending.append((self.submit(images_bgr_u8[a:b], cls_idx[a:b], poses_init[a:b], d), (a, b)))
+        for t, (pa, pb) in pending:
+            out[:, pa - lo:pb - lo] = self.result(t)
+        return sharding.gather_results(out, n, axis=1, dist=dist, device=self.ctx.device if world > 1 else None)
+
+    def refine_frames(self, frames_bgr_u8, frame_of, cls_idx, poses_init, dist=None, depths_u16=None):
+        """refine() with instances that share observed frames (several objects of one image, several initial hypotheses of
+        one object): frames_bgr_u8 [F,H,W,3] uint8, frame_of [N] int (instance i observes frames_bgr_u8[frame_of[i]]),
+        cls_idx [N], poses_init [N,3,4] float64; depths_u16 [F,H,W] uint16 with input_depth=True.
+        The device batches are refine()'s (plan_frame_batches), each uploading only the frames its instances observe, so the
+        result equals refine(frames_bgr_u8[frame_of], ...) bit for bit; keeping the instances of a frame next to each other
+        uploads each frame once.  Sharded over instances like refine(): a rank uploads the frames of its slice only."""
+        n = len(cls_idx)
+        if len(frame_of) != n:
+            raise ValueError("frame_of has %d entries for %d instances" % (len(frame_of), n))
+        rank, world = (dist.get_rank(), dist.get_world_size()) if dist is not None and dist.is_initialized() else (0, 1)
+        lo, hi = sharding.shard_range(n, rank, world)
+        out = np.zeros((self.n_iter, hi - lo, 3, 4), np.float64)
+        pending = []
+        for a, b, frames, local in plan_frame_batches(frame_of, len(frames_bgr_u8), self.max_batch, lo, hi):
+            if len(pending) == len(self.slots):
+                t, (pa, pb) = pending.pop(0)
+                out[:, pa - lo:pb - lo] = self.result(t)
+            d = None if depths_u16 is None else depths_u16[frames]
+            pending.append((self.submit_frames(frames_bgr_u8[frames], local, cls_idx[a:b], poses_init[a:b], d), (a, b)))
         for t, (pa, pb) in pending:
             out[:, pa - lo:pb - lo] = self.result(t)
         return sharding.gather_results(out, n, axis=1, dist=dist, device=self.ctx.device if world > 1 else None)
