@@ -411,11 +411,18 @@ DIM_API int32_t dim_debug_activation(dim_ctx *ctx, int32_t idx, int32_t lo, void
 DIM_API int32_t dim_debug_layer_geometry(dim_ctx *ctx, int32_t idx, int32_t *out8);
 /* tuning hooks (not part of the drop-in surface).
  * dim_debug_set_option: run-time switch.  Key "graph": 1 (default) = replay the refinement chain as a CUDA graph,
- *   0 = enqueue it launch by launch.  Drops the captured graphs; any other key is an error.
+ *   0 = enqueue it launch by launch.  Key "sms": the SM count the library sizes its launches for (the persistent conv
+ *   grids, conv1's row runs, the training step's parity-class streams and weight-gradient K slices): 1 ... the device's
+ *   count, or 0 = the device's count (the default); other values are refused.  It changes no device setting: the
+ *   kernels simply run on fewer CTAs, which lets the tests exercise the schedules of smaller parts (H100 PCIe: 114 SMs).
+ *   Every key drops the captured graphs; the "sms" key also the training step's cached launch descriptors.  Any other
+ *   key is an error.
  * dim_debug_layer_profile: enable = 1 records CUDA events around each conv layer of every dim_net_fwd / dim_refine
  *   iteration; ms10 (nullable) receives the 10 layer times of the LAST forward pass; enable = 0 stops. */
 DIM_API int32_t dim_debug_set_option(dim_ctx *ctx, const char *key, int32_t value);
 DIM_API int32_t dim_debug_layer_profile(dim_ctx *ctx, int32_t enable, float *ms10);
+/* dim_debug_graph_count: how many refinement chains this context holds captured as CUDA graphs (-1: NULL ctx). */
+DIM_API int32_t dim_debug_graph_count(dim_ctx *ctx);
 
 /* Stage profiling of dim_refine with CUDA events on the launching stream (used by bench.py for the
  * live roofline numbers).  enable=1 starts recording; dim_profile_read synchronises the device and
@@ -532,6 +539,10 @@ DIM_API int32_t dim_train_get_precision(dim_ctx *ctx, int32_t *precision);
  * DIM_PREC_BF16X3 step) and their geometry out7 = Hp, Wp, py, px, C, H, W. */
 DIM_API int32_t dim_train_debug_tensor(dim_ctx *ctx, int32_t id, void *host_dst, uint64_t bytes);
 DIM_API int32_t dim_train_debug_geometry(dim_ctx *ctx, int32_t id, int32_t *out7);
+/* Test hook: the K slicing of the 12 weight gradients (flow_conv1, conv2 ... conv6_1, deconv5, deconv4) of a B-image step
+ * at the current SM count (dim_debug_set_option "sms") and precision: out36[3 g], [3 g + 1], [3 g + 2] = slices, pixel
+ * blocks per slice (the K range one fp32 accumulator sums; 64 pixels a block), pixel blocks in all. */
+DIM_API int32_t dim_train_debug_wgrad_slices(dim_ctx *ctx, int32_t B, int32_t *out36);
 /* ms7 = device time of the phases of the last dim_train_forward_backward (with gradients) on the caller's stream:
  * encoder fwd, decoder fwd, losses + pose heads, fc/head backward, decoder backward, encoder data-gradient chain,
  * wait for the weight-gradient stream.  Synchronises the device. */

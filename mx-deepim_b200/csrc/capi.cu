@@ -60,7 +60,7 @@ DIM_API int32_t dim_ctx_create(int32_t device, int32_t max_batch, int32_t H, int
   dim_ctx *ctx = new dim_ctx();
   ctx->device = device; ctx->max_batch = max_batch; ctx->H = H; ctx->W = W;
   ctx->max_classes = max_classes; ctx->max_verts = max_verts; ctx->max_faces = max_faces;
-  ctx->num_sms = prop.multiProcessorCount;
+  ctx->num_sms = ctx->device_sms = prop.multiProcessorCount;
   const size_t P = (size_t)H * W, Bm = (size_t)max_batch;
   int rc = 0;
   rc |= dev_alloc(ctx, &ctx->meshes, (size_t)max_classes);
@@ -843,8 +843,26 @@ DIM_API int32_t dim_debug_set_option(dim_ctx *ctx, const char *key, int32_t valu
   DIM_REQUIRE(ctx && key, "dim_debug_set_option: NULL argument");
   drop_graphs(ctx);  // captured graphs hold the old kernel choice
   if (!strcmp(key, "graph")) { ctx->use_graph = value != 0; return 0; }
+  if (!strcmp(key, "sms")) {
+    // the SM count the launch schedules are sized for: the persistent conv grids, conv1's row runs, the training step's
+    // parity-class streams and weight-gradient K slices.  The device is not touched.
+    if (value < 0 || value > ctx->device_sms) {
+      set_error("dim_debug_set_option: \"sms\" must be in [1, %d] (the device's SM count), or 0 for the device's count; got %d",
+                ctx->device_sms, value);
+      return 2;
+    }
+    ctx->num_sms = value ? value : ctx->device_sms;
+    train_drop_maps(ctx);  // the cached training launch descriptors hold the old weight-gradient K-slice counts
+    return 0;
+  }
   set_error("dim_debug_set_option: unknown key '%s'", key);
   return 2;
+}
+DIM_API int32_t dim_debug_graph_count(dim_ctx *ctx) {
+  if (!ctx) return -1;
+  int32_t n = 0;
+  for (const auto &g : ctx->graphs) n += g.exec != nullptr;
+  return n;
 }
 DIM_API int32_t dim_debug_layer_profile(dim_ctx *ctx, int32_t enable, float *ms10) {
   DIM_REQUIRE(ctx, "dim_debug_layer_profile: NULL ctx");
@@ -959,5 +977,9 @@ DIM_API int32_t dim_train_debug_geometry(dim_ctx *ctx, int32_t id, int32_t *out7
   DIM_REQUIRE(ctx && out7, "dim_train_debug_geometry: NULL argument");
   train_debug_geometry(ctx, id, out7);
   return 0;
+}
+DIM_API int32_t dim_train_debug_wgrad_slices(dim_ctx *ctx, int32_t B, int32_t *out36) {
+  DIM_REQUIRE(ctx && out36, "dim_train_debug_wgrad_slices: NULL argument");
+  return train_debug_wgrad_slices(ctx, B, out36);
 }
 }  // extern "C"

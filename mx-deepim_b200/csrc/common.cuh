@@ -102,7 +102,8 @@ static_assert(sizeof(RefineArgs) == 11 * sizeof(void *) + 6 * sizeof(double) + 1
 
 struct dim_ctx {
   int device = 0, max_batch = 0, H = 0, W = 0, max_classes = 0, max_verts = 0, max_faces = 0;
-  int num_sms = 132;
+  int num_sms = 132;         // the SM count every launch decision uses (dim_debug_set_option "sms"; 0 restores device_sms)
+  int device_sms = 132;      // the device's multiProcessorCount
   // meshes
   std::vector<dim::MeshDev> meshes_host;
   dim::MeshDev *meshes = nullptr;  // device table [max_classes]

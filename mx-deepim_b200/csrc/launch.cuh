@@ -119,6 +119,7 @@ int train_create(dim_ctx *ctx, int max_points);
 void train_destroy(dim_ctx *ctx);
 int train_load_params(dim_ctx *ctx, const float *flat_host, size_t n, cudaStream_t st);
 int train_refresh_lo(dim_ctx *ctx, cudaStream_t st);
+void train_drop_maps(dim_ctx *ctx);
 int train_get_params(dim_ctx *ctx, float *flat_host, size_t n, int which, cudaStream_t st);
 size_t train_param_count(dim_ctx *ctx);
 int train_param_info(int idx, const char **name, long long *w_numel, long long *b_numel, bool input_depth, bool input_mask);
@@ -129,5 +130,6 @@ int train_get_precision(dim_ctx *ctx, int *precision);
 int train_debug_tensor(dim_ctx *ctx, int id, void *host, size_t bytes);
 int train_debug_phases(dim_ctx *ctx, float *ms7);
 void train_debug_geometry(dim_ctx *ctx, int id, int *out /*Hp, Wp, py, px, C, H, W*/);
+int train_debug_wgrad_slices(dim_ctx *ctx, int B, int *out36);
 
 }  // namespace dim

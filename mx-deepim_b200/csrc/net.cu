@@ -350,7 +350,6 @@ int net_create(dim_ctx *ctx) {
   NetState *ns = new NetState();
   ctx->net = ns;
   ns->max_batch = ctx->max_batch;
-  ns->num_sms = ctx->num_sms;
   build_geometry(ns, ctx->H, ctx->W);
   if ((size_t)ns->g[9].Ho * ns->g[9].Wo * ns->g[9].Cout != (size_t)FC6_K) return 0;  // geometry-only context
   for (int i = 0; i <= 10; ++i) {
@@ -673,7 +672,7 @@ int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, fl
     const ConvKParams &kp = tm.kp[i];
     const int n_tiles = g.Cout / g.BLOCK_N;
     const int total_tiles = cdiv(B * g.Hq, g.BH) * g.n_col_tiles * n_tiles;
-    const int sms = ns->num_sms;
+    const int sms = ctx->num_sms;
     int rc;
     if (i == 0 && ns->input_depth) {
       // RGB-D conv1: the same rolling strips, 8 chunk planes per strip; bf16x3 splits the output channels four ways

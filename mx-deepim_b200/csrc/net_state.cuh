@@ -74,8 +74,10 @@ struct NetState {
   cudaEvent_t repack_done = nullptr;  // training: the operand packs are refreshed on an internal stream after an update;
                                       // every consumer (net_forward) orders itself behind this event
   bool lo_stale = false;  // training updated the weights without refreshing the bf16 'lo' halves (bf16x3 mode refreshes lazily)
-  std::map<int, TensorMaps> maps;  // per batch size (+ kF16MapKey for the fp16 operand maps)
-  int max_batch = 0, num_sms = 132;
+  // per batch size (+ kF16MapKey for the fp16 operand maps).  Tensor maps and layer parameters only: the launch schedule
+  // comes from dim_ctx::num_sms at every net_forward, so a change of the SM count leaves these valid
+  std::map<int, TensorMaps> maps;
+  int max_batch = 0;
 };
 
 static constexpr int FC6_K = 1024 * 8 * 10;

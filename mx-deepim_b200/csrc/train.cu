@@ -920,6 +920,12 @@ int train_load_params(dim_ctx *ctx, const float *flat_host, size_t n, cudaStream
   return repack_all(ctx, st, true);
 }
 
+// the per-batch-size launch descriptors are rebuilt on the next step (they hold the weight-gradient K-slice counts chosen
+// for dim_ctx::num_sms); host-side parameter blocks only, so kernels already enqueued are unaffected
+void train_drop_maps(dim_ctx *ctx) {
+  if (TrainState *ts = train_of(ctx)) ts->maps.clear();
+}
+
 // called by net_forward before a bf16x3 pass when the training step left the lo halves stale
 int train_refresh_lo(dim_ctx *ctx, cudaStream_t st) {
   if (train_of(ctx) == nullptr) return 0;
@@ -1209,13 +1215,18 @@ static int launch_wgrad_conv1(const WgradParams &p, cudaStream_t st) {
   DIM_LAUNCH_CHECK();
   return 0;
 }
-static int run_wgrad_conv1(dim_ctx *ctx, TrainState *ts, const WgradParams &p16, float *grad, cudaStream_t st) {
+// conv1_wgrad_kernel's K slicing of the batch's pixel blocks: cdiv(2 sms, 4) slices of 4 filter-row CTAs each
+static WgradParams conv1_slicing(const dim_ctx *ctx, const WgradParams &p16) {
   WgradParams p = p16;
   int ks = cdiv(2 * ctx->num_sms, 4);
   if (ks > p.kb_total / 2) ks = p.kb_total / 2;
   if (ks < 1) ks = 1;
   p.kb_per_slice = cdiv(p.kb_total, ks);
   p.kslices = cdiv(p.kb_total, p.kb_per_slice);
+  return p;
+}
+static int run_wgrad_conv1(dim_ctx *ctx, TrainState *ts, const WgradParams &p16, float *grad, cudaStream_t st) {
+  const WgradParams p = conv1_slicing(ctx, p16);
   DIM_REQUIRE((size_t)p.kslices * 4 * 128 * 64 <= ts->wg_partial_elems, "wgrad workspace too small");
   if (int rc = ts->s3 ? launch_wgrad_conv1<4, true>(p, st) : launch_wgrad_conv1<8, false>(p, st)) return rc;
   const size_t total = (size_t)4 * 128 * 64;
@@ -1393,6 +1404,29 @@ static int record_buckets(const TrainIO &io, int lo_inclusive, int hi_exclusive,
   for (int k = 0; k < io.n_buckets; ++k)
     if (io.bucket_first_tensor[k] >= lo_inclusive && io.bucket_first_tensor[k] < hi_exclusive)
       DIM_CHECK(cudaEventRecord((cudaEvent_t)io.bucket_events[k], s));
+  return 0;
+}
+
+// test hook: the K slicing of the 12 weight gradients (flow_conv1, conv2 ... conv6_1, deconv5, deconv4) of a B-image step at
+// the current SM count and precision; out36[3 g ...] = slices, pixel blocks per slice (the K range one fp32 accumulator sums,
+// 64 pixels a block), pixel blocks in all
+int train_debug_wgrad_slices(dim_ctx *ctx, int B, int *out36) {
+  TrainState *ts = train_of(ctx);
+  DIM_REQUIRE(ts != nullptr && ctx->net->loaded, "dim_train_debug_wgrad_slices: call dim_train_create / dim_train_load_params first");
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_train_debug_wgrad_slices: bad batch size");
+  const int key = B + (ts->s3 ? kS3MapKey : 0);
+  auto it = ts->maps.find(key);
+  if (it == ts->maps.end()) {
+    TrainMaps tm;
+    if (int rc = build_train_maps(ctx, B, tm)) return rc;
+    it = ts->maps.emplace(key, tm).first;
+  }
+  const TrainMaps &tm = it->second;
+  for (int g = 0; g < 12; ++g) {
+    WgradParams p = g < 10 ? tm.wg[g] : (g == 10 ? tm.wg_deconv5 : tm.wg_deconv4);
+    if (g == 0 && !ctx->net->input_depth) p = conv1_slicing(ctx, p);
+    out36[3 * g] = p.kslices; out36[3 * g + 1] = p.kb_per_slice; out36[3 * g + 2] = p.kb_total;
+  }
   return 0;
 }
 

@@ -81,6 +81,7 @@ SIGNATURES = {
     "dim_debug_layer_geometry": (i32, [vp, i32, C.POINTER(i32)]),
     "dim_refine_status": (i32, [vp, i32, i32, vp, vp]),
     "dim_debug_set_option": (i32, [vp, C.c_char_p, i32]),
+    "dim_debug_graph_count": (i32, [vp]),
     "dim_debug_layer_profile": (i32, [vp, i32, pf32]),
     "dim_profile_enable": (i32, [vp, i32]),
     "dim_profile_read": (i32, [vp, pf32, C.POINTER(i32)]),
@@ -102,6 +103,7 @@ SIGNATURES = {
     "dim_train_debug_tensor": (i32, [vp, i32, vp, C.c_uint64]),
     "dim_train_debug_phases": (i32, [vp, pf32]),
     "dim_train_debug_geometry": (i32, [vp, i32, C.POINTER(i32)]),
+    "dim_train_debug_wgrad_slices": (i32, [vp, i32, C.POINTER(i32)]),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

@@ -168,3 +168,201 @@ def check(family, name, dev, ref, S, rho, kappa, where=lambda idx: str(idx), sla
             % (name, int(bad.sum()), dev.numel(), kappa, where(idx), dev.flatten()[i].item(), ref.flatten()[i].item(),
                S.flatten()[i].item(), obs, "; bad entries in: " + ", ".join(places[:12]) if len(places) > 1 else ""))
     return obs
+
+
+# ------------------------------------------------------------------------------------- inference network
+# kappa per inference kernel family: 4 x the largest (|err| - rho |ref|) / (2^-24 S) observed over every case of
+# tests/test_gpu_conv1.py, rounded up to two digits and at least 1 ("obs"; measured on an H100 80GB HBM3 at a 400 W power
+# limit).  The same bounds hold at every SM count (tests/test_gpu_schedule.py): each output's K order is fixed by the kernel.
+KAPPA_INFER = {
+    "conv1": 24,       # obs 5.9     conv1_kernel
+    "tower": 96,       # obs 24.0    conv_igemm_persistent_kernel, conv2 ... conv6_1
+    "fc6_head": 1,     # obs 0.0042  fc6_mma_kernel + head_kernel (fc7, rot, trans in fp32); S carried through fc7 and the heads
+}
+
+
+def fc6_nhwc(a):
+    """fc6 (256, c*80 + hw) in MXNet order -> (256, hw*1024 + c), the NHWC order of act[10] the kernels read"""
+    return np.ascontiguousarray(np.asarray(a).reshape(256, 1024, 80).transpose(0, 2, 1)).reshape(256, 81920)
+
+
+def check_fc6_heads(weights, mode, B, act10, rot, trans, tag=""):
+    """rot / trans of net_forward against float64 fc6 -> fc7 -> heads from the stored act[10] = (hi, lo) float32 numpy
+    [>= B, 8, 10, 1024]: fc6's operands as its 16-bit pack rounds them, fc7 / rot / trans from the fp32 weights.  The error
+    scale S of fc6 is carried through fc7 and the heads by their absolute weights (LeakyReLU moves no difference up)."""
+    lrelu = lambda v: F.leaky_relu(v, 0.1)
+    W6 = operand(fc6_nhwc(weights["fc6_weight"]), mode)
+    wb = {k: gpu(weights[k]) for k in ("fc6_bias", "fc7_weight", "fc7_bias", "rot_weight", "rot_bias", "trans_weight",
+                                       "trans_bias")}
+    hi, lo = act10
+    a = gpu(hi[:B]).reshape(B, 81920), (None if lo is None else gpu(lo[:B]).reshape(B, 81920))
+    z6, S6 = products(lambda x, w: x @ w.T, a, W6)
+    h6, E6 = lrelu(z6 + wb["fc6_bias"]), S6 + wb["fc6_bias"].abs()
+    w7 = wb["fc7_weight"]
+    h7 = lrelu(h6 @ w7.T + wb["fc7_bias"])
+    E7 = E6 @ w7.abs().T + h6.abs() @ w7.abs().T + wb["fc7_bias"].abs()
+    for name, dev in (("rot", rot), ("trans", trans)):
+        w, b = wb[name + "_weight"], wb[name + "_bias"]
+        check("fc6_head", "%s (%s, B=%d%s)" % (name, mode, B, tag), dev, h7 @ w.T + b, E7 @ w.abs().T + h7.abs() @ w.abs().T + b.abs(),
+              0.0, KAPPA_INFER["fc6_head"], lambda idx: "(image %d, output %d)" % idx)
+
+
+def check_conv_layer(weights, mode, layer, B, x, out, geo, tag=""):
+    """encoder layer `layer` (ENC order) against float64 from its stored input x = (hi, lo) float64 [B, Cin, H, W] (the
+    interior; conv1: the decoded space-to-depth canvas, pad included) and its stored output buffer out = (hi, lo) float32
+    numpy [>= B, rows, cols, C] with interior geo = (py, px, H, W).  Returns the largest kappa an element needed."""
+    from oracle.train_oracle import ENC
+    name, s, p = ENC[layer]
+    w = operand(weights[name + "_weight"], mode)
+    b = gpu(weights[name + "_bias"])[None, :, None, None]
+    ref, S = products(lambda a, ww: F.conv2d(a, ww, stride=s, padding=p), x, w)
+    dev = fused((interior(out[0], geo, B), interior(out[1], geo, B)))[0]
+    fam = "conv1" if layer == 0 else "tower"
+    return check(fam, "%s (%s, B=%d%s)" % (name, mode, B, tag), dev, F.leaky_relu(ref + b, 0.1), S + b.abs(), RHO[mode],
+                 KAPPA_INFER[fam], at_pixel)
+
+
+# ------------------------------------------------------------------------------------- training step
+# kappa of the weight-gradient families (conv_wgrad_kernel / conv1_wgrad_kernel + wgrad_reduce), shared by
+# tests/test_gpu_train_kernels.py and tests/test_gpu_schedule.py; see DESIGN.md section 6 for what each K-slice count needed
+KAPPA_WGRAD = {
+    "wgrad": 1300,          # obs 302.3  conv_wgrad_kernel + wgrad_reduce (WG_CONV, WG_DECONV)
+    "conv1_wgrad": 190,     # obs 45.8   conv1_wgrad_kernel + WG_CONV1_ROW; RGB-D: conv_wgrad_kernel + WG_CONV1_RGBD
+}
+
+
+# the weight gradients whose fp32 reduction order follows the SM count (make_wgrad / run_wgrad_conv1 K slices)
+SM_DEPENDENT_GRADS = ("flow_conv1_weight", "conv2_weight", "conv3_weight", "conv3_1_weight", "conv4_weight", "conv4_1_weight",
+                      "conv5_weight", "conv5_1_weight", "conv6_weight", "conv6_1_weight", "deconv5_weight", "deconv4_weight")
+
+
+def wgrad_slices(ctx, B):
+    """{gradient: (K slices, pixel blocks per slice, pixel blocks)} of a B-image training step at the context's current SM
+    count and precision (dim_train_debug_wgrad_slices; the order of SM_DEPENDENT_GRADS)"""
+    import ctypes as C
+    from deepim_b200 import _capi as capi
+    out = (C.c_int32 * 36)()
+    capi.check(capi.lib.dim_train_debug_wgrad_slices(ctx._h, B, out))
+    return {n: tuple(out[3 * g:3 * g + 3]) for g, n in enumerate(SM_DEPENDENT_GRADS)}
+
+
+def wgrad_slice_growth(slices, calibrated):
+    """{gradient: how much longer the K range one fp32 accumulator sums is under `slices` than under `calibrated` (the
+    schedule KAPPA_WGRAD was calibrated at: the device's SM count)}, at least 1.  The tensor cores' fp32 accumulation does
+    not round to nearest, so its error grows with the number of K steps one accumulator takes, linearly as measured
+    (DESIGN.md section 6); a weight gradient's kappa is scaled by this factor."""
+    return {n: max(1.0, slices[n][1] / calibrated[n][1]) for n in slices}
+
+
+class Run:
+    """the device state of a training context after one forward_backward of B images; buffers are read lazily and cached"""
+
+    def __init__(self, net, prec, B, ctx, tr):
+        from oracle.train_oracle import ENC
+        self.net, self.prec, self.B, self.ctx, self.tr = net, prec, B, ctx, tr
+        self.s3 = prec == "bf16x3"
+        self.grads = tr.grads_dict()
+        self.params = tr.get_params()
+        self.sizes = [(ctx.H, ctx.W)]  # sizes[i]: the interior of act[i] (the input of encoder layer i)
+        for name, s, p in ENC:
+            k = self.params[name + "_weight"].shape[-1]
+            h, w = self.sizes[-1]
+            self.sizes.append(((h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1))
+        self._c = {}
+
+    def _cached(self, key, f):
+        if key not in self._c:
+            self._c[key] = f()
+        return self._c[key]
+
+    def act_raw(self, i, lo=False):
+        """act[i] as stored ([max_batch, rows, cols, C] float32 incl. border) and its interior (py, px, H, W)"""
+        def f():
+            buf, g = self.ctx.debug_activation(i, self.ctx.max_batch, lo=lo)
+            return buf, (g[3], g[4]) + self.sizes[i]
+        return self._cached(("act", i, lo), f)
+
+    def act(self, i):
+        """(hi, lo) interior of act[i] as float64 [B, C, H, W]; act[0] decoded from conv1's space-to-depth buffer"""
+        def f():
+            out = []
+            for lo in ((False, True) if self.s3 else (False,)):
+                buf, (py, px, H, W) = self.act_raw(i, lo)
+                if i == 0:
+                    out.append(gpu(s2d_decode(buf[:self.B])[:, :, py:py + H, px:px + W]))
+                else:
+                    out.append(interior(buf, (py, px, H, W), self.B))
+            return out[0], (out[1] if self.s3 else None)
+        return self._cached(("actp", i), f)
+
+    def tbuf(self, tid, lo=False):
+        return self._cached(("t", tid, lo), lambda: self.tr.debug_tensor(tid + (100 if lo else 0)))
+
+    def pair(self, tid, c0=0, c1=None):
+        """(hi, lo) interior of a bf16 training buffer as float64 [B, C, H, W]"""
+        hi, geo = self.tbuf(tid)
+        lo = self.tbuf(tid, True)[0] if self.s3 else None
+        return interior(hi, geo, self.B, c0, c1), interior(lo, geo, self.B, c0, c1)
+
+    def fp32(self, tid):
+        """an fp32 training map [B, h, w, c] as float64 [B, c, h, w] (dh6 / h6: [B, 256])"""
+        a = gpu(self.tbuf(tid)[:self.B])
+        return a if a.dim() == 2 else a.permute(0, 3, 1, 2)
+
+    def w(self, name):
+        return operand(self.params[name], self.prec)
+
+    def w_fc6(self):
+        """fc6's operand pack, (256, hw*1024 + c): the NHWC order of ReLU10 the kernels read"""
+        return operand(fc6_nhwc(self.params["fc6_weight"]), self.prec)
+
+    def w32(self, name):
+        return gpu(self.params[name]), None
+
+    @property
+    def rho(self):
+        return RHO[self.prec]
+
+
+def check_conv_wgrad(run, i, tag="", growth=1.0):
+    """conv_wgrad_kernel + wgrad_reduce (WG_CONV) of encoder layer i = 1 ... 9: dW = conv2d_weight(act[i], gz[i])"""
+    from oracle.train_oracle import ENC
+    name, s, p = ENC[i]
+    k = run.params[name + "_weight"].shape[-1]
+    ref, S = conv_wgrad(run.act(i), run.pair(20 + i), k, s, p)
+    return check("wgrad", "%s_weight (B=%d, %s%s)" % (name, run.B, run.prec, tag), run.grads[name + "_weight"], ref, S, 0.0,
+                 KAPPA_WGRAD["wgrad"] * growth, wgrad_tiles(k, wgrad_bn(ref.shape[1])))
+
+
+def check_conv1_wgrad(run, tag="", growth=1.0):
+    """flow_conv1's weight gradient from the decoded space-to-depth input act[0] (stride 2, pad 3) and gz[0]: the
+    row-GEMM kernel with WG_CONV1_ROW (D1 = 8, or 6 for the image-only network) or, RGB-D, the generic kernel with
+    WG_CONV1_RGBD (D1 = 10).  The lanes past D1 hold exact zeros in the input and are absent from the gradient."""
+    from oracle.train_oracle import ENC
+    name, s, p = ENC[0]
+    x = run.act(0)
+    D1 = {"nomask": 6, "rgbd": 10}.get(run.net, 8)
+    dev = run.grads[name + "_weight"]
+    assert dev.shape == (64, D1, 7, 7)
+    assert x[0].shape[1] == (16 if run.net == "rgbd" else 8)
+    for half in x:
+        assert half is None or not half[:, D1:].any(), "conv1 input lanes %d+ are not zero" % D1
+    ref, S = conv_wgrad(x, run.pair(20), 7, s, p)
+
+    def where(idx):
+        co, ci, kh, kw = idx
+        if run.net == "rgbd":
+            return "(%d, %d, %d, %d) = tap %d" % (co, ci, kh, kw, (kh // 2) * 4 + kw // 2)
+        return "(%d, %d, %d, %d) = filter row %d, M row %d" % (co, ci, kh, kw, kh // 2, (kw // 2) * 32 + (kh % 2) * 16 + (kw % 2) * 8 + ci)
+    return check("conv1_wgrad", "flow_conv1_weight (%s, B=%d, %s%s)" % (run.net, run.B, run.prec, tag), dev, ref[:, :D1], S[:, :D1],
+                 0.0, KAPPA_WGRAD["conv1_wgrad"] * growth, where)
+
+
+def check_deconv_wgrad(run, name, tag="", growth=1.0):
+    """conv_wgrad_kernel + WG_DECONV: deconv5 from act10b and the final dcat2[512:1024], deconv4 from cat2[:1026] and the
+    final dcat3[512:768]"""
+    x, d = {"deconv5_weight": (run.pair(15, 0, 1024), run.pair(12, 512, 1024)),
+            "deconv4_weight": (run.pair(10, 0, 1026), run.pair(13, 512, 768))}[name]
+    ref, S = deconv_wgrad(x, d)
+    return check("wgrad", "%s (B=%d, %s%s)" % (name, run.B, run.prec, tag), run.grads[name], ref, S, 0.0, KAPPA_WGRAD["wgrad"] * growth,
+                 wgrad_tiles(4, wgrad_bn(ref.shape[1])))

@@ -11,7 +11,6 @@ import sys
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in (ROOT, os.path.join(ROOT, "mx-deepim_b200")):
@@ -28,13 +27,7 @@ pytestmark = pytest.mark.gpu
 
 H, W, MAXB = 480, 640, 16
 MODES = {"fp16": capi.PREC_FP16, "bf16": capi.PREC_BF16, "bf16x3": capi.PREC_BF16X3}
-# kappa per kernel family: 4 x the largest (|err| - rho |ref|) / (2^-24 S) observed over every case of this file, rounded
-# up to two digits and at least 1 ("obs"; measured on an H100 80GB HBM3 at a 400 W power limit).  Printed when the module ends (pytest -s).
-KAPPA = {
-    "conv1": 24,       # obs 5.9     conv1_kernel
-    "tower": 96,       # obs 24.0    conv_igemm_persistent_kernel, conv2 ... conv6_1
-    "fc6_head": 1,     # obs 0.0042  fc6_mma_kernel + head_kernel (fc7, rot, trans in fp32); S carried through fc7 and the heads
-}
+KAPPA = R.KAPPA_INFER  # kappa per kernel family (tests/kernel_ref.py); printed when the module ends (pytest -s)
 SIZES = [(H, W)]  # SIZES[i]: the interior of act[i], the input of encoder layer i (filled from the weights' kernel sizes)
 
 
@@ -98,7 +91,7 @@ def _act(ctx, mode, idx, n):
 def _check_layer(ctx, weights, mode, layer, B, n, seed=None):
     """runs the network on a seeded batch of B and checks layer `layer` from its stored input; returns the first n images of
     its output buffer (hi, lo)"""
-    name, s, p = ENC[layer]
+    name = ENC[layer][0]
     blobs = _forward(ctx, mode, B, B if seed is None else seed)[0]
     hi, lo, geo = _act(ctx, mode, layer + 1, n)
     assert np.isfinite(hi).all(), (name, mode, B)
@@ -108,12 +101,7 @@ def _check_layer(ctx, weights, mode, layer, B, n, seed=None):
     else:
         ihi, ilo, igeo = _act(ctx, mode, layer, B)
         x = R.interior(ihi, igeo, B), R.interior(ilo, igeo, B)
-    w = R.operand(weights[name + "_weight"], mode)
-    b = R.gpu(weights[name + "_bias"])[None, :, None, None]
-    ref, S = R.products(lambda a, ww: F.conv2d(a, ww, stride=s, padding=p), x, w)
-    out = R.fused((R.interior(hi, geo, B), R.interior(lo, geo, B)))[0]
-    R.check("conv1" if layer == 0 else "tower", "%s (%s, B=%d)" % (name, mode, B), out, F.leaky_relu(ref + b, 0.1),
-            S + b.abs(), R.RHO[mode], KAPPA["conv1" if layer == 0 else "tower"], R.at_pixel)
+    R.check_conv_layer(weights, mode, layer, B, x, (hi, lo), geo)
     for half in (hi, lo):
         assert half is None or R.border_is_zero(half, geo, B), "%s wrote into the zero border (%s, B=%d)" % (name, mode, B)
     return hi, lo
@@ -146,31 +134,29 @@ def test_layer_full_batch_of_a_tight_allocation(ctx5, weights, mode, layer):
     _check_layer(ctx5, weights, mode, layer, 5, 5)
 
 
-def _fc6_nhwc(a):
-    """fc6 (256, c*80 + hw) in MXNet order -> (256, hw*1024 + c), the NHWC order of act[10] the kernel reads"""
-    return np.ascontiguousarray(np.asarray(a).reshape(256, 1024, 80).transpose(0, 2, 1)).reshape(256, 81920)
+@pytest.fixture(scope="module")
+def ctx33(weights):
+    c = _open(weights, 33)
+    yield c
+    c.close()
+
+
+def _fc6_cases(ctx, weights, mode, batches):
+    for B in batches:
+        _, rot, trans = _forward(ctx, mode, B, 50 + B)
+        hi, lo, _ = _act(ctx, mode, 10, B)
+        R.check_fc6_heads(weights, mode, B, (hi, lo), rot, trans)
 
 
 @pytest.mark.parametrize("mode", sorted(MODES))
 def test_fc6_and_heads_match_float64(ctx, weights, mode):
-    """rot / trans of net_forward against float64 fc6 -> fc7 -> heads from the stored act[10]: fc6's operands as its 16-bit
-    pack rounds them (fp16, bf16 or the bf16x3 hi / lo passes), fc7 / rot / trans from the fp32 weights.  B = 1, 3, 9, 16: the
-    batch is the M rows of mma.m16n8k16, B = 9 and 16 use both 8-row halves.  The error scale S of fc6 is carried through
-    fc7 and the heads by their absolute weights (LeakyReLU moves no difference up)."""
-    lrelu = lambda v: F.leaky_relu(v, 0.1)
-    W6 = R.operand(_fc6_nhwc(weights["fc6_weight"]), mode)
-    wb = {k: R.gpu(weights[k]) for k in ("fc6_bias", "fc7_weight", "fc7_bias", "rot_weight", "rot_bias", "trans_weight",
-                                         "trans_bias")}
-    for B in (1, 3, 9, MAXB):
-        _, rot, trans = _forward(ctx, mode, B, 50 + B)
-        hi, lo, _ = _act(ctx, mode, 10, B)
-        a = R.gpu(hi).reshape(B, 81920), (None if lo is None else R.gpu(lo).reshape(B, 81920))
-        z6, S6 = R.products(lambda x, w: x @ w.T, a, W6)
-        h6, E6 = lrelu(z6 + wb["fc6_bias"]), S6 + wb["fc6_bias"].abs()
-        w7 = wb["fc7_weight"]
-        h7 = lrelu(h6 @ w7.T + wb["fc7_bias"])
-        E7 = E6 @ w7.abs().T + h6.abs() @ w7.abs().T + wb["fc7_bias"].abs()
-        for name, dev in (("rot", rot), ("trans", trans)):
-            w, b = wb[name + "_weight"], wb[name + "_bias"]
-            R.check("fc6_head", "%s (%s, B=%d)" % (name, mode, B), dev, h7 @ w.T + b, E7 @ w.abs().T + h7.abs() @ w.abs().T + b.abs(),
-                    0.0, KAPPA["fc6_head"], lambda idx: "(image %d, output %d)" % idx)
+    """rot / trans of net_forward against float64 fc6 -> fc7 -> heads from the stored act[10] (kernel_ref.check_fc6_heads).
+    B = 1, 3, 9, 16: the batch is the M rows of mma.m16n8k16, B = 9 and 16 use both 8-row halves."""
+    _fc6_cases(ctx, weights, mode, (1, 3, 9, MAXB))
+
+
+@pytest.mark.parametrize("mode", sorted(MODES))
+def test_fc6_and_heads_match_float64_above_16_instances(ctx33, weights, mode):
+    """The same check past one M chunk of fc6_mma_kernel (bench.py's C5 configuration batches 128 instances): B = 17 (a
+    one-row second chunk), 24, 32 (two full chunks) and 33 (three chunks, a one-row tail) on a max_batch = 33 context."""
+    _fc6_cases(ctx33, weights, mode, (17, 24, 32, 33))

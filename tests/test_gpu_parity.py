@@ -434,14 +434,15 @@ def test_refine_is_deterministic_and_batch_consistent(ctx, loop_case):
                    precision=capi.PREC_FP16)
     assert torch.equal(p["bbox"], a["bbox"][:, perm])
     assert (p["poses"] - a["poses"][:, perm]).abs().max().item() < 1e-5
-    # a single instance alone: the launch shapes change with the batch size, so rounding-level differences in se3 are
-    # allowed, and 4 FREE-RUNNING render-and-compare iterations amplify them
-    # (one silhouette pixel of the uint8 re-render).  Not a parity bound: those are the teacher-forced tests.
-    for prec, tol in ((capi.PREC_BF16X3, 5e-4), (capi.PREC_FP16, 5e-4), (capi.PREC_BF16, 2e-3)):
+    # a single instance alone: every output of the chain is reduced in an order fixed per instance (the conv tiles' K steps,
+    # fc6's mma rows and its split partials summed in order), whatever the batch size and the launch shapes it picks, so
+    # the instance's results are the same bits (tests/test_gpu_schedule.py holds this across SM counts and past B = 16)
+    for prec in (capi.PREC_BF16X3, capi.PREC_FP16, capi.PREC_BF16):
         full = ctx.refine(*args, pixel_means_rgb=MEANS, precision=prec)
         s = ctx.refine(dev(c["img"][1:2]), dev(c["cls"][1:2]), dev(c["ini"][1:2]), K, 4, pixel_means_rgb=MEANS,
                        precision=prec)
-        assert (s["poses"][:, 0] - full["poses"][:, 1]).abs().max().item() < tol
+        for k in ("poses", "se3", "bbox", "zoom_factor"):
+            assert torch.equal(s[k][:, 0], full[k][:, 1]), (prec, k)
 
 
 def test_refine_cuda_graph_replay_equals_eager(ctx, loop_case):

@@ -12,7 +12,6 @@ full batch); the image-only and the RGB-D network at B = 3 (conv1's weight gradi
 data gradient: their other kernels are the mask network's)."""
 import json
 
-import numpy as np
 import pytest
 
 pytestmark = pytest.mark.gpu
@@ -35,8 +34,7 @@ K, MEANS = synth.K_LINEMOD, synth.PIXEL_MEANS_RGB
 # rounded up to two digits and at least 1 ("obs"; measured on an H100 80GB HBM3 at a 400 W power limit).  The module prints what each
 # family needed when it finishes (pytest -s).
 KAPPA = {
-    "wgrad": 1300,          # obs 302.3  conv_wgrad_kernel + wgrad_reduce (WG_CONV, WG_DECONV)
-    "conv1_wgrad": 190,     # obs 45.8   conv1_wgrad_kernel + WG_CONV1_ROW; RGB-D: conv_wgrad_kernel + WG_CONV1_RGBD
+    **R.KAPPA_WGRAD,        # "wgrad", "conv1_wgrad": shared with tests/test_gpu_schedule.py
     "bias": 23,             # obs 5.5    bias_partial / bias_final
     "dgrad": 410,           # obs 100.9  conv_igemm_persistent_kernel, data-gradient parity classes (EPI = 1)
     "deconv_fwd": 70,       # obs 17.4   conv_igemm_persistent_kernel, deconvolution forward parity classes
@@ -88,75 +86,6 @@ def nets():
     print("\nkernel families, largest kappa needed: " + json.dumps({k: float("%.4g" % v) for k, v in sorted(R.OBSERVED.items())}))
 
 
-class Run:
-    """the device state after one forward_backward of B images; buffers are read lazily and cached"""
-
-    def __init__(self, net, prec, B, ctx, tr):
-        self.net, self.prec, self.B, self.ctx, self.tr = net, prec, B, ctx, tr
-        self.s3 = prec == "bf16x3"
-        self.grads = tr.grads_dict()
-        self.params = tr.get_params()
-        self.sizes = [(ctx.H, ctx.W)]  # sizes[i]: the interior of act[i] (the input of encoder layer i)
-        for name, s, p in LAYERS:
-            k = self.params[name + "_weight"].shape[-1]
-            h, w = self.sizes[-1]
-            self.sizes.append(((h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1))
-        self._c = {}
-
-    def _cached(self, key, f):
-        if key not in self._c:
-            self._c[key] = f()
-        return self._c[key]
-
-    def act_raw(self, i, lo=False):
-        """act[i] as stored ([max_batch, rows, cols, C] float32 incl. border) and its interior (py, px, H, W)"""
-        def f():
-            buf, g = self.ctx.debug_activation(i, self.ctx.max_batch, lo=lo)
-            return buf, (g[3], g[4]) + self.sizes[i]
-        return self._cached(("act", i, lo), f)
-
-    def act(self, i):
-        """(hi, lo) interior of act[i] as float64 [B, C, H, W]; act[0] decoded from conv1's space-to-depth buffer"""
-        def f():
-            out = []
-            for lo in ((False, True) if self.s3 else (False,)):
-                buf, (py, px, H, W) = self.act_raw(i, lo)
-                if i == 0:
-                    out.append(R.gpu(R.s2d_decode(buf[:self.B])[:, :, py:py + H, px:px + W]))
-                else:
-                    out.append(R.interior(buf, (py, px, H, W), self.B))
-            return out[0], (out[1] if self.s3 else None)
-        return self._cached(("actp", i), f)
-
-    def tbuf(self, tid, lo=False):
-        return self._cached(("t", tid, lo), lambda: self.tr.debug_tensor(tid + (100 if lo else 0)))
-
-    def pair(self, tid, c0=0, c1=None):
-        """(hi, lo) interior of a bf16 training buffer as float64 [B, C, H, W]"""
-        hi, geo = self.tbuf(tid)
-        lo = self.tbuf(tid, True)[0] if self.s3 else None
-        return R.interior(hi, geo, self.B, c0, c1), R.interior(lo, geo, self.B, c0, c1)
-
-    def fp32(self, tid):
-        """an fp32 training map [B, h, w, c] as float64 [B, c, h, w] (dh6 / h6: [B, 256])"""
-        a = R.gpu(self.tbuf(tid)[:self.B])
-        return a if a.dim() == 2 else a.permute(0, 3, 1, 2)
-
-    def w(self, name):
-        return R.operand(self.params[name], self.prec)
-
-    def w_fc6(self):
-        """fc6's operand pack, (256, hw*1024 + c): the NHWC order of ReLU10 the kernels read"""
-        return R.operand(_fc6_nhwc(self.params["fc6_weight"]), self.prec)
-
-    def w32(self, name):
-        return R.gpu(self.params[name]), None
-
-    @property
-    def rho(self):
-        return R.RHO[self.prec]
-
-
 @pytest.fixture(scope="module", params=CASES, ids=["%s-%s-B%s" % (n, p, "-".join(map(str, s))) for n, p, s in CASES])
 def run(request, nets):
     net, prec, sched = request.param
@@ -166,7 +95,7 @@ def run(request, nets):
         batch = make_device_batch(ctx, nets.meshes, B, 11 + B, K, MEANS, input_depth=net == "rgbd")[0]
         tr.forward_backward(tr.zoom_front(batch, K))
         torch.cuda.synchronize()
-    yield Run(net, prec, sched[-1], ctx, tr)
+    yield R.Run(net, prec, sched[-1], ctx, tr)
     tr.set_precision("bf16")
 
 
@@ -190,37 +119,13 @@ def mask_only(run):
 def test_conv_weight_gradients(run):
     """conv_wgrad_kernel + wgrad_reduce (WG_CONV), conv2 ... conv6_1: dW = conv2d_weight(act[i], gz[i])"""
     mask_only(run)
-
-    def one(i):
-        name, s, p = LAYERS[i]
-        k = run.params[name + "_weight"].shape[-1]
-        ref, S = R.conv_wgrad(run.act(i), run.pair(20 + i), k, s, p)
-        R.check("wgrad", "%s_weight (B=%d, %s)" % (name, run.B, run.prec), run.grads[name + "_weight"], ref, S, 0.0,
-                KAPPA["wgrad"], R.wgrad_tiles(k, R.wgrad_bn(ref.shape[1])))
-    collect([lambda i=i: one(i) for i in range(1, 10)])
+    collect([lambda i=i: R.check_conv_wgrad(run, i) for i in range(1, 10)])
 
 
 def test_conv1_weight_gradient(run):
-    """flow_conv1's weight gradient from the decoded space-to-depth input act[0] (stride 2, pad 3) and gz[0]: the
-    row-GEMM kernel with WG_CONV1_ROW (D1 = 8, or 6 for the image-only network) or, RGB-D, the generic kernel with
-    WG_CONV1_RGBD (D1 = 10).  The lanes past D1 hold exact zeros in the input and are absent from the gradient."""
-    name, s, p = LAYERS[0]
-    x = run.act(0)
-    D1 = {"nomask": 6, "rgbd": 10}.get(run.net, 8)
-    dev = run.grads[name + "_weight"]
-    assert dev.shape == (64, D1, 7, 7)
-    assert x[0].shape[1] == (16 if run.net == "rgbd" else 8)
-    for half in x:
-        assert half is None or not half[:, D1:].any(), "conv1 input lanes %d+ are not zero" % D1
-    ref, S = R.conv_wgrad(x, run.pair(20), 7, s, p)
-
-    def where(idx):
-        co, ci, kh, kw = idx
-        if run.net == "rgbd":
-            return "(%d, %d, %d, %d) = tap %d" % (co, ci, kh, kw, (kh // 2) * 4 + kw // 2)
-        return "(%d, %d, %d, %d) = filter row %d, M row %d" % (co, ci, kh, kw, kh // 2, (kw // 2) * 32 + (kh % 2) * 16 + (kw % 2) * 8 + ci)
-    R.check("conv1_wgrad", "flow_conv1_weight (%s, B=%d, %s)" % (run.net, run.B, run.prec), dev, ref[:, :D1], S[:, :D1], 0.0,
-            KAPPA["conv1_wgrad"], where)
+    """flow_conv1's weight gradient (kernel_ref.check_conv1_wgrad): the row-GEMM kernel with WG_CONV1_ROW or, RGB-D, the
+    generic kernel with WG_CONV1_RGBD"""
+    R.check_conv1_wgrad(run)
 
 
 def test_bias_gradients(run):
@@ -241,13 +146,7 @@ def test_deconv_weight_gradients(run):
     """conv_wgrad_kernel + WG_DECONV: deconv5 from act10b and the final dcat2[512:1024], deconv4 from cat2[:1026] and the
     final dcat3[512:768]"""
     mask_only(run)
-
-    def one(name, x, d):
-        ref, S = R.deconv_wgrad(x, d)
-        R.check("wgrad", "%s (B=%d, %s)" % (name, run.B, run.prec), run.grads[name], ref, S, 0.0, KAPPA["wgrad"],
-                R.wgrad_tiles(4, R.wgrad_bn(ref.shape[1])))
-    collect([lambda: one("deconv5_weight", run.pair(15, 0, 1024), run.pair(12, 512, 1024)),
-             lambda: one("deconv4_weight", run.pair(10, 0, 1026), run.pair(13, 512, 768))])
+    collect([lambda n=n: R.check_deconv_wgrad(run, n) for n in ("deconv5_weight", "deconv4_weight")])
 
 
 def test_thin_weight_gradients(run):
@@ -264,11 +163,6 @@ def test_thin_weight_gradients(run):
              lambda: one("Convolution2", run.pair(10, 0, 1026), run.fp32(6)),
              lambda: one("Convolution3", run.pair(11, 0, 770), run.fp32(4)),
              lambda: one("mask_conv3", run.pair(11, 0, 770), run.fp32(5))])
-
-
-def _fc6_nhwc(a):
-    """fc6 (256, c*80 + hw) in MXNet order -> (256, hw*1024 + c), the order of the NHWC ReLU10 the kernels read"""
-    return np.ascontiguousarray(np.asarray(a).reshape(256, 1024, 80).transpose(0, 2, 1)).reshape(256, 81920)
 
 
 def test_fc6_gradients(run):
@@ -292,7 +186,7 @@ def test_fc6_gradients(run):
         return "(out %d, y %d, x %d, channel %d)" % (o, kk // 10240, (kk // 1024) % 10, kk % 1024)
 
     def wgrad():
-        R.check("fc6", "fc6_weight" + tag, _fc6_nhwc(run.grads["fc6_weight"]), dh6.T @ a10, dh6.abs().T @ a10.abs(), 0.0,
+        R.check("fc6", "fc6_weight" + tag, R.fc6_nhwc(run.grads["fc6_weight"]), dh6.T @ a10, dh6.abs().T @ a10.abs(), 0.0,
                 KAPPA["fc6"], where_w)
 
     def bias():
