@@ -535,8 +535,10 @@ DIM_API int32_t dim_train_sgd_update(dim_ctx *ctx, const float *grads, float lr,
  * weights.  Switching back to DIM_PREC_BF16 leaves the bf16 step exactly as it was. */
 DIM_API int32_t dim_train_set_precision(dim_ctx *ctx, int32_t precision);
 DIM_API int32_t dim_train_get_precision(dim_ctx *ctx, int32_t *precision);
-/* Test hooks: intermediates of the training step (ids in train.cu; 100 + a bf16 buffer's id = its lo half after a
- * DIM_PREC_BF16X3 step) and their geometry out7 = Hp, Wp, py, px, C, H, W. */
+/* Test hooks: intermediates of the training step and their geometry out7 = Hp, Wp, py, px, C, H, W (ids in train.cu):
+ * 0-9 the fp32 flow / mask maps, their gradients, h6 and dh6; 10-15 and 20-29 the bf16 decoder, gradient and gz buffers
+ * (100 + one of these ids = its lo half after a DIM_PREC_BF16X3 step); 30-41 the fp32 pose heads and losses (h7, rot_raw,
+ * ztrans, rot_n, trans_est, pts_est, dpts, drot_n, dtrans, drot, dh7, dfull), which have no lo half and zero geometry. */
 DIM_API int32_t dim_train_debug_tensor(dim_ctx *ctx, int32_t id, void *host_dst, uint64_t bytes);
 DIM_API int32_t dim_train_debug_geometry(dim_ctx *ctx, int32_t id, int32_t *out7);
 /* Test hook: the K slicing of the 12 weight gradients (flow_conv1, conv2 ... conv6_1, deconv5, deconv4) of a B-image step

@@ -1643,7 +1643,8 @@ int train_sgd_update(dim_ctx *ctx, const float *grads, float lr, float momentum,
 // test / debugging hook: copy an intermediate to the host.  id: 0 flow6, 1 flow5, 2 flow4, 3 mask4, 4 dflow4, 5 dmask4,
 // 6 dflow5, 7 dflow6, 8 h6 (the fc6 activation kept for the backward pass), 9 dh6 (gradient of fc6's pre-activation) (fp32);
 // 10 cat2, 11 cat3, 12 dcat2, 13 dcat3, 14 dA10p, 15 act10b, 20+i gz[i] (bf16, whole bordered buffer); 100 + one of the bf16 ids:
-// that buffer's lo half (exists once the step has run in bf16x3)
+// that buffer's lo half (exists once the step has run in bf16x3); the pose heads (fp32): 30 h7 [B][256], 31 rot_raw [B][4],
+// 32 ztrans [B][3], 33 rot_n [B][4], 34 trans_est [B][3], 35 pts_est and 36 dpts [B][3][N] (N of the last step), 37 drot_n [B][4], 38 dtrans [B][3], 39 drot [B][4], 40 dh7 [B][256], 41 dfull [B][3][H][W]
 int train_debug_tensor(dim_ctx *ctx, int id, void *host, size_t bytes) {
   TrainState *ts = train_of(ctx);
   DIM_REQUIRE(ts != nullptr, "no training state");
@@ -1654,7 +1655,8 @@ int train_debug_tensor(dim_ctx *ctx, int id, void *host, size_t bytes) {
   const bool lo = id >= 100;
   if (lo) id -= 100;
   auto fb = [&](const Buf &b) { src = lo ? b.lo : b.p; have = b.per_image() * B * 2; };
-  switch (lo && id < 10 ? -1 : id) {
+  const bool bf16_id = (id >= 10 && id < 16) || (id >= 20 && id < 30);  // only these have lo halves
+  switch (lo && !bf16_id ? -1 : id) {
     case 0: src = ts->flow6; have = (size_t)B * g[9].Ho * g[9].Wo * 8; break;
     case 1: src = ts->flow5; have = (size_t)B * g[7].Ho * g[7].Wo * 8; break;
     case 2: src = ts->flow4; have = (size_t)B * g[5].Ho * g[5].Wo * 8; break;
@@ -1671,6 +1673,18 @@ int train_debug_tensor(dim_ctx *ctx, int id, void *host, size_t bytes) {
     case 13: fb(ts->dcat3); break;
     case 14: fb(ts->dA10p); break;
     case 15: fb(ts->act10b); break;
+    case 30: src = ts->h7; have = (size_t)B * 256 * 4; break;
+    case 31: src = ts->rot_raw; have = (size_t)B * 4 * 4; break;
+    case 32: src = ts->ztrans; have = (size_t)B * 3 * 4; break;
+    case 33: src = ts->rot_n; have = (size_t)B * 4 * 4; break;
+    case 34: src = ts->trans_est; have = (size_t)B * 3 * 4; break;
+    case 35: src = ts->pts_est; have = (size_t)B * 3 * ts->max_points * 4; break;
+    case 36: src = ts->dpts; have = (size_t)B * 3 * ts->max_points * 4; break;
+    case 37: src = ts->drot_n; have = (size_t)B * 4 * 4; break;
+    case 38: src = ts->dtrans; have = (size_t)B * 3 * 4; break;
+    case 39: src = ts->drot; have = (size_t)B * 4 * 4; break;
+    case 40: src = ts->dh7; have = (size_t)B * 256 * 4; break;
+    case 41: src = ts->dfull; have = (size_t)B * 3 * ctx->H * ctx->W * 4; break;
     default:
       if (id >= 20 && id < 30) fb(ts->gz[id - 20]);
   }

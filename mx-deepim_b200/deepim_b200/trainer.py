@@ -134,6 +134,7 @@ class Trainer:
         self.buckets, self.bucket_first = make_buckets(bucket_mb, tensor_sizes(self.input_depth, self.input_mask))
         self._events = None
         self._comm_stream = None
+        self._last_n = 0
 
     def set_precision(self, precision):
         """'bf16' | 'bf16x3' (or DIM_PREC_BF16 / DIM_PREC_BF16X3): the precision of this context's training step
@@ -176,6 +177,7 @@ class Trainer:
         label still is."""
         ctx = self.ctx
         B, N = z["zoom_image_observed"].shape[0], z["point_cloud_model"].shape[2]
+        self._last_n = N  # the point count of debug_tensor's pts_est / dpts
         zmo, zmr = (z["zoom_mask_observed"], z["zoom_mask_rendered"]) if self.input_mask else (None, None)
         zdo, zdr = (z["zoom_depth_observed"], z["zoom_depth_rendered"]) if self.input_depth else (None, None)
         for k, t in z.items():
@@ -278,13 +280,16 @@ class Trainer:
         return unflatten_params(flat, {k: np.empty(s, np.float32) for k, s in self._shapes.items()})
 
     def debug_tensor(self, tid):
-        """fp32 maps (id < 8) as [B,h,w,c], h6 / dh6 (8 / 9) as [B,256]; bf16 buffers (id >= 10) as float32 [B,Hp,Wp,C]
-        incl. border."""
+        """fp32 maps (id < 8) as [B,h,w,c], h6 / dh6 (8 / 9) as [B,256]; bf16 buffers (10 ... 29) as float32 [B,Hp,Wp,C]
+        incl. border; the pose heads (30 ... 40) as [B,256] (h7, dh7), [B,4] / [B,3] (rot_raw, ztrans, rot_n, trans_est,
+        drot_n, dtrans, drot) and [B,3,N] (pts_est, dpts, N of the last forward_backward); 41 dfull as [B,3,H,W].
+        B is the context's max_batch: images past the last step's batch hold whatever an earlier step left."""
         ctx = self.ctx
         B = ctx.max_batch
-        if tid < 10:
+        if tid < 10 or 30 <= tid < 42:
             hw = {0: (8, 10, 2), 1: (15, 20, 2), 2: (30, 40, 2), 3: (30, 40, 1), 4: (30, 40, 2), 5: (30, 40, 1), 6: (15, 20, 2),
-                  7: (8, 10, 2), 8: (256,), 9: (256,)}[tid]
+                  7: (8, 10, 2), 8: (256,), 9: (256,), 30: (256,), 31: (4,), 32: (3,), 33: (4,), 34: (3,), 35: (3, self._last_n),
+                  36: (3, self._last_n), 37: (4,), 38: (3,), 39: (4,), 40: (256,), 41: (3, ctx.H, ctx.W)}[tid]
             a = np.empty((B,) + hw, np.float32)
             check(lib.dim_train_debug_tensor(ctx._h, tid, a.ctypes.data_as(C.c_void_p), a.nbytes))
             return a

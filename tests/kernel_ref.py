@@ -124,6 +124,131 @@ def deconv_dgrad(d, w, Hi, Wi):
     return products(lambda g, ww: F.conv2d(deconv_canvas(g, Hi, Wi), ww, stride=DECONV_STRIDE), d, w)
 
 
+# the heads' fixed bilinear upsampling (deepIM_flownet.py:184-199, 329-344): a Deconvolution k32 s16 with one group per
+# channel, then Crop(offset (8, 8)) to the image size
+UP_K, UP_STRIDE, UP_CROP = 32, 16, 8
+
+
+def upsample_fwd(x, w, H, W):
+    """the upsampled, cropped map [B, C, H, W] of x [B, C, h, w]; w (C, 1, 32, 32).  Device-agnostic, like the other
+    references below (float64 in, float64 out)."""
+    c = UP_CROP
+    return F.conv_transpose2d(x, w, stride=UP_STRIDE, groups=x.shape[1])[:, :, c:c + H, c:c + W]
+
+
+def upsample_bwd(d, w, h, wd):
+    """the adjoint of upsample_fwd: the gradient [B, C, h, wd] of the low-resolution map from the gradient d [B, C, H, W]
+    of the cropped output (d placed on the uncropped canvas, then the stride-16 convolution with the same kernel)"""
+    B, C, H, W = d.shape
+    c = UP_CROP
+    canvas = d.new_zeros(B, C, UP_STRIDE * (h - 1) + UP_K, UP_STRIDE * (wd - 1) + UP_K)
+    canvas[:, :, c:c + H, c:c + W] = d
+    return F.conv2d(canvas, w, stride=UP_STRIDE, groups=C)
+
+
+L2_EPS = 1e-10  # L2Normalization(mode=instance): x / sqrt(sum x^2 + eps)
+
+
+def l2_normalize(x):
+    """L2Normalization of the rotation head, rows of x [B, 4]"""
+    return x / torch.sqrt((x * x).sum(1, keepdim=True) + L2_EPS)
+
+
+def l2_normalize_bwd(x, g):
+    """its backward: d x from the output gradient g, (g - y (y . g)) / n with y = x / n, n = sqrt(sum x^2 + eps)"""
+    n = torch.sqrt((x * x).sum(1, keepdim=True) + L2_EPS)
+    y = x / n
+    return (g - y * (y * g).sum(1, keepdim=True)) / n
+
+
+def pm_loss(est, obs, pw, norm):
+    """the L1 point-matching loss per element (deepIM_flownet.py:290-296): pw |(est - obs) / norm|"""
+    return pw * ((est - obs) / norm).abs()
+
+
+def pm_loss_grad(est, obs, pw, norm, gs):
+    """its gradient under MakeLoss(grad_scale = gs): gs pw sign(d) / norm, sign(0) = 0 as MXNet's abs backward"""
+    return gs * pw * torch.sign((est - obs) / norm) / norm
+
+
+def quat2mat_t3d(q):
+    """Transform3D's quat2mat_forward (transform3d.py:185-212) of q [B, 4] -> [B, 3, 3]: the identity where
+    |Nq - 1| >= 1e-2"""
+    w, x, y, z = q.unbind(1)
+    Nq = (q * q).sum(1)
+    s = 2.0 / Nq
+    X, Y, Z = x * s, y * s, z * s
+    M = torch.stack([1 - (y * Y + z * Z), x * Y - w * Z, x * Z + w * Y,
+                     x * Y + w * Z, 1 - (x * X + z * Z), y * Z - w * X,
+                     x * Z - w * Y, y * Z + w * X, 1 - (x * X + y * Y)], 1).reshape(-1, 3, 3)
+    eye = torch.eye(3, dtype=q.dtype, device=q.device).expand_as(M)
+    return torch.where(((Nq - 1).abs() < 1e-2)[:, None, None], M, eye)
+
+
+def _t3d_common(t, pose_src, Tm, Ts):
+    """T_transform (rot_coord model / camera): d = t Ts + Tm, z2 = src_z / exp(d_z), a_k = d_k + src_k / src_z, and
+    the error scales of z2 (relative, in units of 2^-24: exp, the division and d_z's own rounding) and of a_k"""
+    Tm, Ts = (torch.as_tensor(v, dtype=t.dtype, device=t.device) for v in (Tm, Ts))
+    src = pose_src[:, :, 3]
+    d = t * Ts + Tm
+    z2 = src[:, 2] / torch.exp(d[:, 2])
+    a = d[:, :2] + src[:, :2] / src[:, 2:3]
+    e2 = 3 + (t[:, 2] * Ts[2]).abs() + Tm[2].abs()
+    Sa = (t[:, :2] * Ts[:2]).abs() + Tm[:2].abs() + (src[:, :2] / src[:, 2:3]).abs()
+    return Ts, z2, a, e2, Sa
+
+
+def transform3d_fwd(P, q, t, pose_src, Tm, Ts, rot_coord):
+    """Transform3D forward (transform3d.py:34-97; rot_coord 'MODEL' or 'CAMERA'): points P [B, 3, N] under the rotation
+    q [B, 4] and the translation t [B, 3] relative to pose_src [B, 3, 4] -> (ref, S), S bounding the fp32 evaluation"""
+    Rd, Rs = quat2mat_t3d(q), pose_src[:, :, :3]
+    model = rot_coord.lower() == "model"
+    Rt, SRt = (Rs @ Rd, Rs.abs() @ Rd.abs()) if model else (Rd @ Rs, Rd.abs() @ Rs.abs())
+    _, z2, a, e2, Sa = _t3d_common(t, pose_src, Tm, Ts)
+    Tt = torch.cat([z2[:, None] * a, z2[:, None]], 1)
+    STt = z2.abs()[:, None] * torch.cat([e2[:, None] * a.abs() + Sa, e2[:, None]], 1)
+    return Rt @ P + Tt[:, :, None], SRt @ P.abs() + STt[:, :, None]
+
+
+def _quat2mat_bwd_coef(qn):
+    """[B, 4, 9]: (w', x', y', z') of quat2mat_backward (transform3d.py:214-275) as a linear map of the row-major 3x3
+    matrix gradient, for the normalised quaternion qn"""
+    w, x, y, z = qn.unbind(1)
+    o = torch.zeros_like(w)
+    rows = [[o, -z, y, z, o, -x, -y, x, o],
+            [o, y, z, y, -2 * x, -w, z, w, -2 * x],
+            [-2 * y, x, w, x, o, z, -w, z, -2 * y],
+            [-2 * z, -w, x, w, -2 * z, y, x, y, o]]
+    return 2 * torch.stack([torch.stack(r, 1) for r in rows], 1)
+
+
+def transform3d_bwd(D, P, q, t, pose_src, Tm, Ts, rot_coord):
+    """Transform3D's hand-written backward (transform3d.py:99-281) of the output gradient D [B, 3, N] ->
+    ((d rotation [B, 4], S), (d translation [B, 3], S)); the rotation gradient is zero where |Nq - 1| >= 1e-4"""
+    Ts, z2, a, e2, Sa = _t3d_common(t, pose_src, Tm, Ts)
+    Dt, SDt = D.sum(2), D.abs().sum(2)
+    share = -Ts[2] * z2
+    tg = torch.stack([Dt[:, 0] * Ts[0] * z2, Dt[:, 1] * Ts[1] * z2, Dt[:, 0] * share * a[:, 0] + Dt[:, 1] * share * a[:, 1]
+                      + Dt[:, 2] * share], 1)
+    Stg = e2[:, None] * torch.stack([SDt[:, 0] * (Ts[0] * z2).abs(), SDt[:, 1] * (Ts[1] * z2).abs(),
+                                     share.abs() * (SDt[:, 0] * Sa[:, 0] + SDt[:, 1] * Sa[:, 1] + SDt[:, 2])], 1)
+    RtD, SRtD = D @ P.transpose(1, 2), D.abs() @ P.abs().transpose(1, 2)
+    Rs = pose_src[:, :, :3]
+    if rot_coord.lower() == "model":
+        Dm, SDm = Rs.transpose(1, 2) @ RtD, Rs.abs().transpose(1, 2) @ SRtD
+    else:
+        Dm, SDm = RtD @ Rs.transpose(1, 2), SRtD @ Rs.abs().transpose(1, 2)
+    Nq = (q * q).sum(1)
+    Ns = torch.sqrt(Nq)[:, None]
+    C = _quat2mat_bwd_coef(q / Ns)
+    dq, Sdq = (C @ Dm.reshape(-1, 9, 1))[..., 0], (C.abs() @ SDm.reshape(-1, 9, 1))[..., 0]
+    sh = Ns ** 3 * (q * dq).sum(1, keepdim=True)
+    rg = Ns * dq - q * sh
+    Srg = Ns * Sdq + q.abs() * Ns ** 3 * (q.abs() * Sdq).sum(1, keepdim=True)
+    ok = ((Nq - 1).abs() < 1e-4)[:, None]
+    return (torch.where(ok, rg, torch.zeros_like(rg)), torch.where(ok, Srg, torch.zeros_like(Srg))), (tg, Stg)
+
+
 # ------------------------------------------------------------------------------------- the bound
 def at_pixel(idx):
     b, c, y, x = idx

@@ -481,6 +481,51 @@ def test_refine_cuda_graph_replay_equals_eager(ctx, loop_case):
     torch.cuda.synchronize()
 
 
+def test_refine_follows_config_pose_parameterisation(ctx, loop_case):
+    """dim_refine composes each iteration's pose under the context's trans_means / trans_stds / rot_coord: poses[i+1] =
+    rt_transform(poses[i], se3[i]) in float64 with the values set, eagerly and on graph replay; a second set_config with the
+    same buffers reaches the replay (set_config drops the captured chains)."""
+    from deepim_b200._capi import check, lib
+    c = loop_case
+    img, cls, ini = dev(c["img"]), dev(c["cls"]), dev(c["ini"])
+    cfg0 = ctx.get_config()
+
+    def holds(out, cfg, what):
+        poses, se3 = out["poses"].cpu().numpy(), out["se3"].cpu().numpy()
+        src = c["ini"]
+        for it in range(poses.shape[0]):
+            for b in range(c["B"]):
+                ref = O.rt_transform(src[b], se3[it, b, :4], se3[it, b, 4:], cfg["trans_means"], cfg["trans_stds"], cfg["rot_coord"])
+                assert np.abs(poses[it, b] - ref).max() <= 1e-12 * np.abs(ref).max(), (what, it, b)
+            src = poses[it]
+
+    side = torch.cuda.Stream(device=DEV)
+    try:
+        default = ctx.refine(img, cls, ini, K, 4, pixel_means_rgb=MEANS)
+        out = None
+        for new in ({"trans_means": (0.0625, -0.125, 0.03125), "trans_stds": (0.5, 2.0, 0.75), "rot_coord": "MODEL"},
+                    {"trans_means": (-0.03125, 0.0625, -0.0625), "trans_stds": (1.5, 0.25, 2.0), "rot_coord": "MODEL"}):
+            torch.cuda.synchronize()
+            ctx.set_config(**new)
+            cfg = ctx.get_config()
+            check(lib.dim_debug_set_option(ctx._h, b"graph", 0))
+            eager = ctx.refine(img, cls, ini, K, 4, pixel_means_rgb=MEANS)
+            holds(eager, cfg, "eager")
+            assert not torch.equal(eager["poses"], default["poses"])
+            torch.cuda.synchronize()
+            check(lib.dim_debug_set_option(ctx._h, b"graph", 1))
+            for it in range(3):  # eager warm-up, capture + launch, replay -- on the buffers of the previous config's graph
+                with torch.cuda.stream(side):
+                    out = ctx.refine(img, cls, ini, K, 4, pixel_means_rgb=MEANS, out=out)
+                side.synchronize()
+                holds(out, cfg, "graph %d" % it)
+                assert torch.equal(out["poses"], eager["poses"]), it
+    finally:
+        torch.cuda.synchronize()
+        check(lib.dim_debug_set_option(ctx._h, b"graph", 1))
+        ctx.set_config(**cfg0)
+
+
 def test_refine_host_matches_device_path(ctx, meshes, loop_case):
     c = loop_case
     B = c["B"]
