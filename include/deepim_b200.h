@@ -363,6 +363,32 @@ DIM_API int32_t dim_refine_frames_host(dim_ctx *ctx, const uint8_t *frames_u8_ho
                                        const uint16_t *depth_frames_u16_host, float depth_factor,
                                        const dim_lighting *lighting, void *stream);
 
+/* Frame-indexed fused loop with one camera per frame (a batch across several cameras; the reference's per-pair
+ * `<observed>-K.txt`, tester.py:424-427): K_frames [F,9] row-major f32 in place of K9, and instance b is rendered and
+ * zoomed with the intrinsics of its frame, K_frames[frame_of(b)] -- the frame whose taps it observes, frame 0 for a device
+ * index outside [0, F) (status bit 3).  One K serves both the render and the zoom centre K . t (the reference zooms with
+ * the config's K even when the pair has its own).  Instance b's results equal dim_refine_frames' with
+ * K9 = K_frames[frame_idx[b]], bit for bit.  Every other argument is dim_refine_frames' / dim_refine_frames_host_async's.
+ *   dim_refine_frames_k: K_frames device f32 [F,9], read as given (not checked, like frame_idx).  The CUDA graph of the
+ *     chain reads it at replay: new intrinsics in the same buffer need no re-capture; another buffer is another graph.
+ *   dim_refine_frames_k_host_async: K_frames_host f32 [F,9].  Every row is checked before anything is enqueued: one that is
+ *     not a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]] with fx, fy > 0 fails the call with a message naming the
+ *     frame.  The rows are copied into the context (no allocation); the outputs are valid once `stream` is synchronised. */
+DIM_API int32_t dim_refine_frames_k(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx,
+                                    const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B,
+                                    int32_t n_iter, float znear, float zfar, const double *pixel_means_rgb_host,
+                                    int32_t precision, const double *pose_override, double *poses, float *se3,
+                                    float *zoom_factor, int32_t *bbox, const float *depth_frames,
+                                    const dim_lighting *lighting, void *stream);
+DIM_API int32_t dim_refine_frames_k_host_async(dim_ctx *ctx, const uint8_t *frames_u8_host, int32_t F,
+                                               const int32_t *frame_idx_host, const float *K_frames_host,
+                                               const int32_t *cls_idx_host, const double *pose_init_host, int32_t B,
+                                               int32_t n_iter, float znear, float zfar,
+                                               const double *pixel_means_rgb_host, int32_t precision,
+                                               double *poses_out_host, float *se3_out_host,
+                                               const uint16_t *depth_frames_u16_host, float depth_factor,
+                                               const dim_lighting *lighting, void *stream);
+
 /* BGR u8 HWC -> RGB-mean f32 CHW on device (lib/utils/image.py:583-594 transform). */
 DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int32_t B,
                                        const double *pixel_means_rgb_host, float *image,

@@ -2,6 +2,8 @@
 #include <stdarg.h>
 #include <string.h>
 
+#include <cmath>
+
 #include "launch.cuh"
 
 namespace dim {
@@ -81,6 +83,7 @@ DIM_API int32_t dim_ctx_create(int32_t device, int32_t max_batch, int32_t H, int
   rc |= dev_alloc(ctx, &ctx->image_observed_u8, Bm * 3 * P);
   rc |= dev_alloc(ctx, &ctx->cls_dev, Bm);
   rc |= dev_alloc(ctx, &ctx->frame_dev, Bm);
+  rc |= dev_alloc(ctx, &ctx->K_dev, Bm * 9);
   rc |= dev_alloc(ctx, &ctx->poses_dev, 8 * Bm * 12);
   rc |= dev_alloc(ctx, &ctx->se3_hist_dev, 8 * Bm * 7);
   rc |= dev_alloc(ctx, &ctx->light_pos, Bm * 3);
@@ -491,7 +494,8 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
       const LitParams lp = a.lit ? lit_params(ctx->light_pos, a.intensity + (size_t)it * a.B * 3, a.brightness_ratio)
                                  : LitParams{nullptr, nullptr, 0.f, 0.f};
       if (int rc = render_launch(ctx, a.cls_idx, ctx->pose_cur_f32, a.B, a.K9, a.zn, a.zf, a.means, 1, nullptr, nullptr,
-                                 nullptr, nullptr, nullptr, ctx->ren4, st, a.lit ? &lp : nullptr, depth, !mask))
+                                 nullptr, nullptr, nullptr, ctx->ren4, st, a.lit ? &lp : nullptr, depth, !mask, a.K_frames,
+                                 a.frame_idx, a.n_frames))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[1], st));
@@ -505,10 +509,10 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
       int *status_it = ctx->status_hist + (size_t)(it < 8 ? it : 7) * a.B;
       if (mask) {
         if (int rc = zoom_factor_from_ren_launch(ctx, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it, bbox_it, status_it, st,
-                                                 a.frame_idx, a.n_frames))
+                                                 a.frame_idx, a.n_frames, a.K_frames))
           return rc;
       } else if (int rc = zoom_factor_from_boxes_launch(ctx, ctx->bbox_obs, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it,
-                                                        bbox_it, status_it, st, a.frame_idx, a.n_frames)) {
+                                                        bbox_it, status_it, st, a.frame_idx, a.n_frames, a.K_frames)) {
         return rc;
       }
       if (int rc = zoom_fused_launch(ctx, a.obs4, ctx->ren4, zf_it, means_f, a.B, rows, cols, pad, hi,
@@ -578,12 +582,13 @@ static int refine_graphed(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
   return 0;
 }
 
-// the loop's host values; the caller sets the pointers (lit: nullptr = unlit)
+// the loop's host values; the caller sets the pointers (lit: nullptr = unlit; K9 nullptr = per-frame intrinsics, K9 all zero
+// so that the graph key holds only the K_frames pointer)
 static RefineArgs refine_args(int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
                               int32_t precision, const dim_lighting *lit) {
   RefineArgs a{};
   a.B = B; a.n_iter = n_iter; a.precision = precision; a.zn = zn; a.zf = zf;
-  memcpy(a.K9, K9, sizeof(a.K9));
+  if (K9) memcpy(a.K9, K9, sizeof(a.K9));
   memcpy(a.means, means, sizeof(a.means));
   if (lit) {
     a.lit = 1;
@@ -623,31 +628,73 @@ DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int3
   return refine_device(ctx, a, image_observed, B, nullptr, depth_observed, (cudaStream_t)stream);
 }
 
+static int refuse(const char *fn, const char *msg) {
+  set_error("%s: %s", fn, msg);
+  return 2;
+}
+
+// dim_refine_frames (K9: one camera) and dim_refine_frames_k (K_frames: device [F,9], one camera per frame; K9 nullptr)
+static int refine_frames_device(dim_ctx *ctx, const char *fn, const float *image_frames, int32_t F, const int32_t *frame_idx,
+                                const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B,
+                                int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
+                                const double *pose_override, double *poses, float *se3, float *zoom_factor, int32_t *bbox,
+                                const float *depth_frames, const dim_lighting *lighting, cudaStream_t st) {
+  if (!(ctx && image_frames && frame_idx && cls_idx && pose_init && (K9 || K_frames) && means && poses))
+    return refuse(fn, "NULL argument");
+  if (int rc = depth_check(ctx, depth_frames, depth_frames, fn, "depth_frames")) return rc;
+  if (int rc = lit_check(ctx, lighting, fn)) return rc;
+  if (B < 1 || B > ctx->max_batch) return refuse(fn, "batch exceeds max_batch");
+  if (F < 1 || F > ctx->max_batch) return refuse(fn, "frame count F outside [1, max_batch]");
+  if (n_iter < 1) return refuse(fn, "n_iter must be >= 1");
+  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
+  a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
+  a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
+  a.K_frames = K_frames;
+  return refine_device(ctx, a, image_frames, F, frame_idx, depth_frames, st);
+}
+
 // frame-indexed dim_refine: F observed frames, instance b observes frame frame_idx[b] (device; checked in the kernels)
 DIM_API int32_t dim_refine_frames(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx,
                                   const int32_t *cls_idx, const double *pose_init, int32_t B, int32_t n_iter, const float *K9,
                                   float zn, float zf, const double *means, int32_t precision, const double *pose_override,
                                   double *poses, float *se3, float *zoom_factor, int32_t *bbox, const float *depth_frames,
                                   const dim_lighting *lighting, void *stream) {
-  DIM_REQUIRE(ctx && image_frames && frame_idx && cls_idx && pose_init && K9 && means && poses,
-              "dim_refine_frames: NULL argument");
-  if (int rc = depth_check(ctx, depth_frames, depth_frames, "dim_refine_frames", "depth_frames")) return rc;
-  if (int rc = lit_check(ctx, lighting, "dim_refine_frames")) return rc;
-  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_frames: batch exceeds max_batch");
-  DIM_REQUIRE(F >= 1 && F <= ctx->max_batch, "dim_refine_frames: frame count F outside [1, max_batch]");
-  DIM_REQUIRE(n_iter >= 1, "dim_refine_frames: n_iter must be >= 1");
-  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
-  a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
-  a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
-  return refine_device(ctx, a, image_frames, F, frame_idx, depth_frames, (cudaStream_t)stream);
+  return refine_frames_device(ctx, "dim_refine_frames", image_frames, F, frame_idx, nullptr, cls_idx, pose_init, B, n_iter,
+                              K9, zn, zf, means, precision, pose_override, poses, se3, zoom_factor, bbox, depth_frames,
+                              lighting, (cudaStream_t)stream);
 }
 
-// the host entries once their scalar arguments are checked: the class and frame indices are checked here, before anything
-// is enqueued; fn names the entry point in the messages.  frame_host nullptr = instance b observes frame b (F == B)
+// dim_refine_frames with one camera per frame: K_frames device f32 [F,9], read as given (like frame_idx) and at replay
+DIM_API int32_t dim_refine_frames_k(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx,
+                                    const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B,
+                                    int32_t n_iter, float zn, float zf, const double *means, int32_t precision,
+                                    const double *pose_override, double *poses, float *se3, float *zoom_factor, int32_t *bbox,
+                                    const float *depth_frames, const dim_lighting *lighting, void *stream) {
+  if (!K_frames) return refuse("dim_refine_frames_k", "NULL argument (K_frames)");
+  return refine_frames_device(ctx, "dim_refine_frames_k", image_frames, F, frame_idx, K_frames, cls_idx, pose_init, B, n_iter,
+                              nullptr, zn, zf, means, precision, pose_override, poses, se3, zoom_factor, bbox, depth_frames,
+                              lighting, (cudaStream_t)stream);
+}
+
+// why the host intrinsics K (row-major 3x3) are not a finite pinhole matrix [[fx, 0, cx], [0, fy, cy], [0, 0, 1]] with
+// fx, fy > 0, or nullptr when they are
+static const char *pinhole_defect(const float *K) {
+  for (int k = 0; k < 9; ++k)
+    if (!std::isfinite(K[k])) return "a value is not finite";
+  if (!(K[0] > 0.f && K[4] > 0.f)) return "fx and fy must be > 0";
+  if (K[1] != 0.f || K[3] != 0.f) return "K[0][1] (skew) and K[1][0] must be 0";
+  if (K[6] != 0.f || K[7] != 0.f || K[8] != 1.f) return "the last row must be (0, 0, 1)";
+  return nullptr;
+}
+
+// the host entries once their scalar arguments are checked: the class and frame indices (and intrinsics) are checked here,
+// before anything is enqueued; fn names the entry point in the messages.  frame_host nullptr = instance b observes frame b
+// (F == B).  K_host: nullptr = K9 for every instance; else host [F,9], one camera per frame (K9 nullptr)
 static int refine_host_enqueue(dim_ctx *ctx, const char *fn, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
-                               const int32_t *cls_host, const double *pose_host, int32_t B, int32_t n_iter, const float *K9,
-                               float zn, float zf, const double *means, int32_t precision, double *poses_out, float *se3_out,
-                               const uint16_t *depth_u16, float depth_factor, const dim_lighting *lighting, cudaStream_t st) {
+                               const float *K_host, const int32_t *cls_host, const double *pose_host, int32_t B,
+                               int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
+                               double *poses_out, float *se3_out, const uint16_t *depth_u16, float depth_factor,
+                               const dim_lighting *lighting, cudaStream_t st) {
   for (int32_t i = 0; i < B; ++i) {  // the class indices are on the host here: fail loudly (the reference indexes a python list)
     const int32_t c = cls_host[i];
     if (c < 0 || c >= ctx->max_classes || ctx->meshes_host[c].V <= 0) {
@@ -662,12 +709,21 @@ static int refine_host_enqueue(dim_ctx *ctx, const char *fn, const uint8_t *fram
         set_error("%s: instance %d has frame index %d: out of range [0,%d)", fn, (int)i, (int)frame_host[i], (int)F);
         return 2;
       }
+  if (K_host)  // and the cameras
+    for (int32_t f = 0; f < F; ++f)
+      if (const char *why = pinhole_defect(K_host + 9 * f)) {
+        set_error("%s: frame %d has intrinsics that are not a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]]: %s", fn,
+                  (int)f, why);
+        return 2;
+      }
   const size_t P = (size_t)ctx->H * ctx->W;
   DIM_CHECK(cudaMemcpyAsync(ctx->image_observed_u8, frames_u8, (size_t)F * 3 * P, cudaMemcpyHostToDevice, st));
   DIM_CHECK(cudaMemcpyAsync(ctx->cls_dev, cls_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
   DIM_CHECK(cudaMemcpyAsync(ctx->pose_cur, pose_host, sizeof(double) * B * 12, cudaMemcpyHostToDevice, st));
   if (frame_host) DIM_CHECK(cudaMemcpyAsync(ctx->frame_dev, frame_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
+  if (K_host) DIM_CHECK(cudaMemcpyAsync(ctx->K_dev, K_host, sizeof(float) * 9 * F, cudaMemcpyHostToDevice, st));
   RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
+  a.K_frames = K_host ? ctx->K_dev : nullptr;
   a.obs4 = ctx->obs4; a.cls_idx = ctx->cls_dev; a.pose_init = ctx->pose_cur; a.poses = ctx->poses_dev;
   a.se3 = ctx->se3_hist_dev;
   a.frame_idx = frame_host ? ctx->frame_dev : nullptr; a.n_frames = F;
@@ -700,8 +756,27 @@ DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *img_u8, const
   if (int rc = lit_check(ctx, lighting, "dim_refine_host")) return rc;
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_host: batch exceeds max_batch");
   DIM_REQUIRE(n_iter >= 1 && n_iter <= 8, "dim_refine_host: n_iter must be in [1,8]");
-  return refine_host_enqueue(ctx, "dim_refine_host", img_u8, B, nullptr, cls_host, pose_host, B, n_iter, K9, zn, zf, means,
-                             precision, poses_out, se3_out, depth_u16, depth_factor, lighting, (cudaStream_t)stream);
+  return refine_host_enqueue(ctx, "dim_refine_host", img_u8, B, nullptr, nullptr, cls_host, pose_host, B, n_iter, K9, zn, zf,
+                             means, precision, poses_out, se3_out, depth_u16, depth_factor, lighting, (cudaStream_t)stream);
+}
+
+// dim_refine_frames_host(_async) (K9: one camera) and dim_refine_frames_k_host_async (K_host: host [F,9], one camera per
+// frame; K9 nullptr): the scalar checks, then refine_host_enqueue
+static int refine_frames_host(dim_ctx *ctx, const char *fn, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
+                              const float *K_host, const int32_t *cls_host, const double *pose_host, int32_t B, int32_t n_iter,
+                              const float *K9, float zn, float zf, const double *means, int32_t precision, double *poses_out,
+                              float *se3_out, const uint16_t *depth_u16, float depth_factor, const dim_lighting *lighting,
+                              cudaStream_t st) {
+  if (!(ctx && frames_u8 && frame_host && cls_host && pose_host && (K9 || K_host) && means && poses_out))
+    return refuse(fn, "NULL argument");
+  if (int rc = depth_check(ctx, depth_u16, depth_u16, fn, "depth_frames_u16_host")) return rc;
+  if (depth_u16 && !(depth_factor > 0.f && depth_factor < 3.0e38f)) return refuse(fn, "depth_factor must be positive and finite");
+  if (int rc = lit_check(ctx, lighting, fn)) return rc;
+  if (B < 1 || B > ctx->max_batch) return refuse(fn, "batch exceeds max_batch");
+  if (F < 1 || F > ctx->max_batch) return refuse(fn, "frame count F outside [1, max_batch]");
+  if (n_iter < 1 || n_iter > 8) return refuse(fn, "n_iter must be in [1,8]");
+  return refine_host_enqueue(ctx, fn, frames_u8, F, frame_host, K_host, cls_host, pose_host, B, n_iter, K9, zn, zf, means,
+                             precision, poses_out, se3_out, depth_u16, depth_factor, lighting, st);
 }
 
 // frame-indexed dim_refine_host_async: F host frames [F,H,W,3] (depth [F,H,W]), frame_host [B] checked before any enqueue
@@ -710,17 +785,22 @@ DIM_API int32_t dim_refine_frames_host_async(dim_ctx *ctx, const uint8_t *frames
                                              const float *K9, float zn, float zf, const double *means, int32_t precision,
                                              double *poses_out, float *se3_out, const uint16_t *depth_u16, float depth_factor,
                                              const dim_lighting *lighting, void *stream) {
-  DIM_REQUIRE(ctx && frames_u8 && frame_host && cls_host && pose_host && K9 && means && poses_out,
-              "dim_refine_frames_host: NULL argument");
-  if (int rc = depth_check(ctx, depth_u16, depth_u16, "dim_refine_frames_host", "depth_frames_u16_host")) return rc;
-  if (depth_u16)
-    DIM_REQUIRE(depth_factor > 0.f && depth_factor < 3.0e38f, "dim_refine_frames_host: depth_factor must be positive and finite");
-  if (int rc = lit_check(ctx, lighting, "dim_refine_frames_host")) return rc;
-  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_frames_host: batch exceeds max_batch");
-  DIM_REQUIRE(F >= 1 && F <= ctx->max_batch, "dim_refine_frames_host: frame count F outside [1, max_batch]");
-  DIM_REQUIRE(n_iter >= 1 && n_iter <= 8, "dim_refine_frames_host: n_iter must be in [1,8]");
-  return refine_host_enqueue(ctx, "dim_refine_frames_host", frames_u8, F, frame_host, cls_host, pose_host, B, n_iter, K9, zn, zf,
-                             means, precision, poses_out, se3_out, depth_u16, depth_factor, lighting, (cudaStream_t)stream);
+  return refine_frames_host(ctx, "dim_refine_frames_host", frames_u8, F, frame_host, nullptr, cls_host, pose_host, B, n_iter,
+                            K9, zn, zf, means, precision, poses_out, se3_out, depth_u16, depth_factor, lighting,
+                            (cudaStream_t)stream);
+}
+
+// dim_refine_frames_host_async with one camera per frame: K_host [F,9], every row checked before any enqueue
+DIM_API int32_t dim_refine_frames_k_host_async(dim_ctx *ctx, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
+                                               const float *K_host, const int32_t *cls_host, const double *pose_host,
+                                               int32_t B, int32_t n_iter, float zn, float zf, const double *means,
+                                               int32_t precision, double *poses_out, float *se3_out,
+                                               const uint16_t *depth_u16, float depth_factor, const dim_lighting *lighting,
+                                               void *stream) {
+  if (!K_host) return refuse("dim_refine_frames_k_host", "NULL argument (K_frames_host)");
+  return refine_frames_host(ctx, "dim_refine_frames_k_host", frames_u8, F, frame_host, K_host, cls_host, pose_host, B, n_iter,
+                            nullptr, zn, zf, means, precision, poses_out, se3_out, depth_u16, depth_factor, lighting,
+                            (cudaStream_t)stream);
 }
 
 DIM_API int32_t dim_refine_frames_host(dim_ctx *ctx, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,

@@ -76,12 +76,28 @@ struct MeshDev {
 
 struct NetState;  // net_state.cuh
 
+// The observed frame of instance b in the fused loop (dim_refine_frames): frame_idx[b], or frame 0 when that lies outside
+// [0, n_frames) -- a bad index never reads outside the packed frames (or the per-frame intrinsics); the zoom factor flags it
+// as status bit 3.  frame_idx == nullptr: instance b observes frame b (dim_refine).
+__device__ __forceinline__ int frame_of(const int32_t *frame_idx, int n_frames, int b) {
+  if (!frame_idx) return b;
+  const int f = __ldg(frame_idx + b);
+  return (f >= 0 && f < n_frames) ? f : 0;
+}
+__device__ __forceinline__ bool frame_bad(const int32_t *frame_idx, int n_frames, int b) {
+  if (!frame_idx) return false;
+  const int f = __ldg(frame_idx + b);
+  return f < 0 || f >= n_frames;
+}
+
 // Everything the fused refinement loop reads from its caller, and the key of its CUDA graphs, compared byte for byte (so
 // no padding).  Not in the key, because drop_graphs discards every graph when they change: ctx->cfg (trans means / stds,
 // rot_coord), mesh uploads, network weights and the "graph" option.
 struct RefineArgs {
   const float4 *obs4;        // n_frames observed frames
   const int32_t *frame_idx;  // device [B]: the frame instance b observes (read at replay); nullptr = frame b (dim_refine)
+  const float *K_frames;     // device [n_frames,9]: the camera of every frame (read at replay; K9 is then all zero);
+                             // nullptr = K9 for every instance (dim_refine, dim_refine_frames)
   const int32_t *cls_idx;
   const double *pose_init, *pose_override;  // pose_override: nullable [n_iter,B,3,4] source pose of every iteration
   double *poses;
@@ -95,7 +111,7 @@ struct RefineArgs {
   int32_t n_frames;  // frames in obs4 (dim_refine: B)
   int32_t zero;      // always 0: fills what would otherwise be tail padding
 };
-static_assert(sizeof(RefineArgs) == 11 * sizeof(void *) + 6 * sizeof(double) + 12 * sizeof(float) + 6 * sizeof(int32_t),
+static_assert(sizeof(RefineArgs) == 12 * sizeof(void *) + 6 * sizeof(double) + 12 * sizeof(float) + 6 * sizeof(int32_t),
               "RefineArgs must have no padding: its bytes are the graph key");
 
 }  // namespace dim
@@ -127,6 +143,7 @@ struct dim_ctx {
   uint8_t *image_observed_u8 = nullptr;
   int *cls_dev = nullptr;
   int *frame_dev = nullptr;     // [max_batch] dim_refine_frames_host: the caller's frame index of every instance
+  float *K_dev = nullptr;       // [max_batch,9] dim_refine_frames_k_host: the caller's intrinsics of every frame
   double *poses_dev = nullptr;  // [8, max_batch, 12]
   float *se3_hist_dev = nullptr;
   float *light_pos = nullptr;      // [max_batch,3] lit chain / lit train update: light of the pose being rendered

@@ -21,10 +21,13 @@ struct TrainIO {
 };
 
 // raster.cu
+// K_frames / frame_idx / n_frames (fused loop, RefineArgs): instance b projects with row frame_of(b) of the per-frame
+// intrinsics [n_frames,9]; K_frames nullptr = K9 for every instance
 int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
                   const double *means, int trunc_u8, float *out_image, float *out_depth, float *out_mask, float *out_bgr,
                   int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit = nullptr, bool ren4_depth = false,
-                  bool colour_box = false);
+                  bool colour_box = false, const float *K_frames = nullptr, const int32_t *frame_idx = nullptr,
+                  int n_frames = 0);
 
 // zoom.cu
 int zoom_gather_launch(dim_ctx *ctx, int mode, const float *src, float *dst, const float *zoom_factor, int B, int C,
@@ -33,13 +36,14 @@ int zoom_factor_launch(dim_ctx *ctx, const float *mask_real, const float *mask_r
                        const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
                        const float *img_means = nullptr);
 // frame_idx / n_frames: the fused loop's map from instance to observed frame (RefineArgs); nullptr = frame b
+// K_frames: the fused loop's per-frame intrinsics [n_frames,9] (RefineArgs); nullptr = K9 for every instance
 int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *src_pose, int B, const float *K9,
                                 float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
-                                const int32_t *frame_idx = nullptr, int n_frames = 0);
+                                const int32_t *frame_idx = nullptr, int n_frames = 0, const float *K_frames = nullptr);
 int obs_colour_box_launch(dim_ctx *ctx, const float4 *obs4, int F, int *bbox_obs, cudaStream_t st);
 int zoom_factor_from_boxes_launch(dim_ctx *ctx, const int *bbox_obs, const int *bbox_ren, const float *src_pose, int B,
                                   const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
-                                  const int32_t *frame_idx = nullptr, int n_frames = 0);
+                                  const int32_t *frame_idx = nullptr, int n_frames = 0, const float *K_frames = nullptr);
 int box_mask_launch(dim_ctx *ctx, const int *bbox, int B, float *mask, cudaStream_t st);
 int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, const float *zoom_factor,
                       const float *means_rgb, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo,

@@ -38,6 +38,9 @@ struct RasterParams {
   int num_classes;  // size of the mesh table: class indices are range-checked on the device (mesh_for)
   int *cls_flag;    // [B] 0 ok / 2 = class index out of range or no mesh uploaded for it (renders nothing); nullable
   float fx, fy, cx, cy, zn, zf;
+  const float *K_frames;     // fused loop, nullable: [n_frames,9] intrinsics; instance b projects with row frame_of(b) of them
+  const int32_t *frame_idx;  // instead of fx, fy, cx, cy (RefineArgs)
+  int n_frames;
   double mean[3];
   float bg[3];  // (float)(0.0 - mean)
   int trunc_u8;
@@ -84,6 +87,11 @@ __global__ void __launch_bounds__(256) raster_vertex_kernel(RasterParams p) {
   if (p.cls_flag && v == 0) p.cls_flag[b] = m.V > 0 ? 0 : 2;
   const float *pose = p.pose + 12 * b;
   int ok = 0, X = 0, Y = 0;
+  float fx = p.fx, fy = p.fy, cx = p.cx, cy = p.cy;
+  if (p.K_frames) {
+    const float *k = p.K_frames + 9 * frame_of(p.frame_idx, p.n_frames, b);
+    fx = __ldg(k + 0); cx = __ldg(k + 2); fy = __ldg(k + 4); cy = __ldg(k + 5);
+  }
   if (v < m.V) {
     float x = m.verts[3 * v], y = m.verts[3 * v + 1], z = m.verts[3 * v + 2];
     float xc = ((pose[0] * x + pose[1] * y) + pose[2] * z) + pose[3];
@@ -92,8 +100,8 @@ __global__ void __launch_bounds__(256) raster_vertex_kernel(RasterParams p) {
     ok = zc > 1e-6f;
     float sx = 0.f, sy = 0.f, iz = 0.f;
     if (ok) {
-      sx = (p.fx * xc) / zc + p.cx;
-      sy = (p.fy * yc) / zc + p.cy;
+      sx = (fx * xc) / zc + cx;
+      sy = (fy * yc) / zc + cy;
       ok = (fabsf(sx) <= 1e6f) && (fabsf(sy) <= 1e6f);
       iz = 1.0f / zc;
     }
@@ -433,7 +441,7 @@ __global__ void raster_finish_kernel(int *bbox_ren, int *out_bbox, int B) {
 int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
                   const double *means, int trunc_u8, float *out_image, float *out_depth, float *out_mask,
                   float *out_bgr, int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit, bool ren4_depth,
-                  bool colour_box) {
+                  bool colour_box, const float *K_frames, const int32_t *frame_idx, int n_frames) {
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_render: batch exceeds max_batch");
   DIM_REQUIRE((ctx->W & 3) == 0, "dim_render: width must be a multiple of 4");
   RasterParams p;
@@ -442,6 +450,7 @@ int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const 
   p.max_verts = ctx->max_verts; p.max_faces = ctx->max_faces; p.H = ctx->H; p.W = ctx->W;
   p.num_classes = ctx->max_classes; p.cls_flag = ctx->cls_flag;
   p.fx = K9[0]; p.fy = K9[4]; p.cx = K9[2]; p.cy = K9[5]; p.zn = zn; p.zf = zf;
+  p.K_frames = K_frames; p.frame_idx = frame_idx; p.n_frames = n_frames;
   for (int c = 0; c < 3; ++c) {
     p.mean[c] = means ? means[c] : 0.0;
     p.bg[c] = trunc_u8 ? (float)(0.0 - p.mean[c]) : 0.0f - (float)p.mean[c];

@@ -59,30 +59,23 @@ __global__ void __launch_bounds__(160) mask_bbox_kernel(const float *mask_real, 
   }
 }
 
-// The observed frame of instance b in the fused loop (dim_refine_frames): frame_idx[b], or frame 0 when that lies outside
-// [0, n_frames) -- a bad index never reads outside the packed frames; the zoom factor flags it as status bit 3.
-// frame_idx == nullptr: instance b observes frame b (dim_refine).
-__device__ __forceinline__ int frame_of(const int32_t *frame_idx, int n_frames, int b) {
-  if (!frame_idx) return b;
-  const int f = __ldg(frame_idx + b);
-  return (f >= 0 && f < n_frames) ? f : 0;
-}
-__device__ __forceinline__ bool frame_bad(const int32_t *frame_idx, int n_frames, int b) {
-  if (!frame_idx) return false;
-  const int f = __ldg(frame_idx + b);
-  return f < 0 || f >= n_frames;
-}
-
 // zoom factor, one thread per instance (zoom_mask.py:59-103; ZoomImage's is the same code, zoom_image.py:41-86).  Mixed
 // precision as the reference's numpy 1.x: c = K.t and c_x = c0/c2 in float32, everything after in float64, stored as float32.
 // ren_empty_bit: status bit set where the rendered box is empty and the zoom centres on the observed box (0: none)
 // frame_idx / n_frames (fused loop, nullable): an instance whose frame index is out of range gets status bit 3
+// K_frames (fused loop, nullable): [n_frames,9] intrinsics; instance b uses its frame's row (frame_of) instead of k0 ... k8
 __global__ void zoom_factor_kernel(int *bbox8, const float *src_pose, int B, int H, int W, float k0, float k1,
                                    float k2, float k3, float k4, float k5, float k6, float k7, float k8,
                                    float *zoom_factor, int *bbox_out, int *status, const int *cls_flag, int ren_empty_bit,
-                                   const int32_t *frame_idx, int n_frames) {
+                                   const int32_t *frame_idx, int n_frames, const float *K_frames) {
   int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
+  if (K_frames) {
+    const float *k = K_frames + 9 * frame_of(frame_idx, n_frames, b);
+    k0 = __ldg(k + 0); k1 = __ldg(k + 1); k2 = __ldg(k + 2);
+    k3 = __ldg(k + 3); k4 = __ldg(k + 4); k5 = __ldg(k + 5);
+    k6 = __ldg(k + 6); k7 = __ldg(k + 7); k8 = __ldg(k + 8);
+  }
   // rasteriser: bad class index (bit 1); frame index out of range (bit 3)
   const int cf = (cls_flag ? cls_flag[b] : 0) | (frame_bad(frame_idx, n_frames, b) ? 8 : 0);
   int *bb = bbox8 + 8 * b;
@@ -261,7 +254,7 @@ int zoom_factor_launch(dim_ctx *ctx, const float *mask_real, const float *mask_r
   DIM_LAUNCH_CHECK();
   zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
                                                   K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, nullptr, 0,
-                                                  nullptr, 0);
+                                                  nullptr, 0, nullptr);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -284,12 +277,12 @@ __global__ void zoom_factor_from_ren_kernel(const int *bbox_ren, int *bbox8, int
 
 int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *src_pose, int B, const float *K9,
                                 float *zoom_factor, int *bbox_out, int *status, cudaStream_t st, const int32_t *frame_idx,
-                                int n_frames) {
+                                int n_frames, const float *K_frames) {
   zoom_factor_from_ren_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_ren, ctx->bbox8, B);
   DIM_LAUNCH_CHECK();
   zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
                                                   K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag, 0,
-                                                  frame_idx, n_frames);
+                                                  frame_idx, n_frames, K_frames);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -355,12 +348,12 @@ __global__ void boxes_to_bbox8_kernel(const int *bbox_obs, const int *bbox_ren, 
 
 int zoom_factor_from_boxes_launch(dim_ctx *ctx, const int *bbox_obs, const int *bbox_ren, const float *src_pose, int B,
                                   const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
-                                  const int32_t *frame_idx, int n_frames) {
+                                  const int32_t *frame_idx, int n_frames, const float *K_frames) {
   boxes_to_bbox8_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_obs, bbox_ren, ctx->bbox8, B, frame_idx, n_frames);
   DIM_LAUNCH_CHECK();
   zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
                                                   K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag, 4,
-                                                  frame_idx, n_frames);
+                                                  frame_idx, n_frames, K_frames);
   DIM_LAUNCH_CHECK();
   return 0;
 }

@@ -61,6 +61,17 @@ def _lighting_arg(lighting, shape, on_device):
     return capi.Lighting(ptr, (C.c_double * 3)(*offset), float(np.float32(ratio))), keep
 
 
+def _per_frame_k(K, F):
+    """True when K holds one camera per frame ([F,3,3]), False for one camera ([3,3], or anything of 9 values as before);
+    raises on an [n,3,3] whose n is not F"""
+    shape = tuple(K.shape) if isinstance(K, torch.Tensor) else np.shape(K)
+    if len(shape) != 3:
+        return False
+    if shape != (F, 3, 3):
+        raise ValueError("K: expected [3,3] (one camera) or [F,3,3] = %s (one camera per frame), got %s" % ((F, 3, 3), shape))
+    return True
+
+
 class Context:
     def __init__(self, device=0, max_batch=16, height=480, width=640, max_classes=16, max_verts=60000,
                  max_faces=120000, input_depth=False, input_mask=True):
@@ -524,8 +535,11 @@ class Context:
         observes frames[frame_idx[b]]), 1 <= F <= max_batch.  Instance b's results equal refine(frames[frame_idx], ...)'s, bit
         for bit; each frame is packed once.  An index outside [0, F) is not an error here: that instance observes frame 0
         and refine_status() reports bit 3.  Writing new indices into the same frame_idx tensor replays the captured graph.
-        depth_frames: f32 [F,1,H,W] CUDA, metres -- required on an RGB-D context, refused otherwise.  Every other argument
-        as refine()."""
+        depth_frames: f32 [F,1,H,W] CUDA, metres -- required on an RGB-D context, refused otherwise.
+        K: [3,3], one camera for every instance, or [F,3,3], one camera per frame (dim_refine_frames_k): instance b is rendered
+        and zoomed with K[frame_idx[b]], and its results equal refine_frames(..., K=K[frame_idx[b]]) bit for bit.  A float32
+        CUDA tensor [F,3,3] is read in place, also at graph replay: new intrinsics written into it need no re-capture; any
+        other [F,3,3] array is copied to the device first.  Every other argument as refine()."""
         F, B = frames.shape[0], cls_idx.shape[0]
         _chk(frames, torch.float32, (F, 3, self.H, self.W), "frames")
         _chk(frame_idx, torch.int32, (B,), "frame_idx")
@@ -547,10 +561,18 @@ class Context:
         if depth_frames is not None:
             _chk(depth_frames, torch.float32, (F, 1, self.H, self.W), "depth_frames")
         lit = None if lighting is None else C.byref(_lighting_arg(lighting, (n_iter, B, 3), True)[0])
-        check(lib.dim_refine_frames(self._h, _p(frames), F, _p(frame_idx), _p(cls_idx), _p(pose_init), B, n_iter,
-                                    farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
-                                    farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses), _p(se3),
-                                    _p(zf), _p(bbox), _p(depth_frames), lit, self._stream()))
+        if _per_frame_k(K, F):
+            if not (isinstance(K, torch.Tensor) and K.device == self.device and K.dtype == torch.float32 and K.is_contiguous()):
+                K = torch.as_tensor(np.ascontiguousarray(K if not isinstance(K, torch.Tensor) else K.cpu(), np.float32),
+                                    device=self.device)
+            check(lib.dim_refine_frames_k(self._h, _p(frames), F, _p(frame_idx), _p(K), _p(cls_idx), _p(pose_init), B, n_iter,
+                                          znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override),
+                                          _p(poses), _p(se3), _p(zf), _p(bbox), _p(depth_frames), lit, self._stream()))
+        else:
+            check(lib.dim_refine_frames(self._h, _p(frames), F, _p(frame_idx), _p(cls_idx), _p(pose_init), B, n_iter,
+                                        farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
+                                        farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses), _p(se3),
+                                        _p(zf), _p(bbox), _p(depth_frames), lit, self._stream()))
         return {"poses": poses, "se3": se3, "zoom_factor": zf, "bbox": bbox}
 
     def refine_frames_host(self, frames_u8, frame_idx, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
@@ -558,7 +580,11 @@ class Context:
                            se3_out=None, sync=True, lighting=None, depth_frames_u16=None, depth_factor=1000.0):
         """refine_host() against F shared observed frames: frames_u8 uint8 [F,H,W,3] BGR, frame_idx int32 [B] (host; every
         index is checked: one outside [0, F) raises before anything is enqueued), depth_frames_u16 uint16 [F,H,W] on an
-        RGB-D context.  Each frame is uploaded once.  Every other argument as refine_host()."""
+        RGB-D context.  Each frame is uploaded once.
+        K: [3,3], or [F,3,3] host float32, one camera per frame (dim_refine_frames_k_host_async; see refine_frames): every
+        row must be a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]] with fx, fy > 0, else the call raises naming the
+        frame before anything is enqueued.  With sync=False a pinned K is copied asynchronously: keep it untouched until the
+        stream is synchronised.  Every other argument as refine_host()."""
         def hptr(a):
             return C.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else C.c_void_p(a.ctypes.data)
 
@@ -588,11 +614,20 @@ class Context:
                 raise ValueError("depth_frames_u16: expected shape %s, got %s" % ((F, self.H, self.W), tuple(dkeep.shape)))
         frames = frames_u8 if isinstance(frames_u8, torch.Tensor) else np.ascontiguousarray(frames_u8, np.uint8)
         lit, _keep = (None, None) if lighting is None else _lighting_arg(lighting, (n_iter, B, 3), False)
+        tail = (hptr(poses_out), hptr(se3_out), None if dkeep is None else hptr(dkeep), float(np.float32(depth_factor)),
+                None if lit is None else C.byref(lit), self._stream())
+        if _per_frame_k(K, F):
+            kf = host(K, np.float32, torch.float32, "K")
+            check(lib.dim_refine_frames_k_host_async(self._h, hptr(frames), F, hptr(fidx), hptr(kf), hptr(cls), hptr(pose), B,
+                                                     n_iter, znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision,
+                                                     *tail))
+            if sync:
+                torch.cuda.current_stream(self.device).synchronize()
+            return poses_out, se3_out
         fn = lib.dim_refine_frames_host if sync else lib.dim_refine_frames_host_async
         check(fn(self._h, hptr(frames), F, hptr(fidx), hptr(cls), hptr(pose), B, n_iter,
                  farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision,
-                 hptr(poses_out), hptr(se3_out), None if dkeep is None else hptr(dkeep), float(np.float32(depth_factor)),
-                 None if lit is None else C.byref(lit), self._stream()))
+                 *tail))
         return poses_out, se3_out
 
 

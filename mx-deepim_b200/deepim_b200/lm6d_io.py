@@ -6,6 +6,7 @@ Readers (and, for synthetic fixtures, writers) for what lib/dataset/LM6D_REFINE.
     <root>/models/models_info.txt            "<cls_idx> diameter <mm> ..."                   (LM6D_REFINE.py:112-126)
     <root>/image_set/<set>.txt               "<observed index> <rendered index>" per line   (l.128-138)
     <root>/data/observed/<index>-color.png | -depth.png (uint16, metres * DEPTH_FACTOR 1000) | -label.png   (l.140-182)
+    <root>/data/observed/<index>-K.txt       optional: the frame's own 3x3 intrinsics, np.loadtxt   (tester.py:424-427)
     <root>/data/gt_observed/<cls>/<idx>-pose.txt | -depth.png            (1 header line + 3x4, np.loadtxt(skiprows=1), l.184-196)
     <root>/data/rendered/<index>-color.png | -depth.png | -label.png | -pose.txt
 
@@ -158,15 +159,21 @@ class LM6DRefine:
             return [tuple(x.strip().split(" ")) for x in f if x.strip()]
 
     def load_pair(self, cls, pair):
-        """What load_render_annotation + the test loader read for one pair (LM6D_REFINE.py:226-262, image.py:297-399)."""
+        """What load_render_annotation + the test loader read for one pair (LM6D_REFINE.py:226-262, image.py:297-399), and
+        "K" (3x3 float64) from `data/observed/<observed index>-K.txt` where that file exists (tester.py:424-427); a pair
+        without one has no "K" and is taken with the dataset's K."""
         obs, ren = pair
         d = os.path.join(self.root, "data")
-        return {
+        rec = {
             "image_observed": read_color(os.path.join(d, "observed", obs + "-color.png")),
             "pose_observed": read_pose(os.path.join(d, "gt_observed", cls, obs.split("/")[1] + "-pose.txt")),
             "pose_rendered": read_pose(os.path.join(d, "rendered", ren + "-pose.txt")),
             "depth_rendered": read_depth(os.path.join(d, "rendered", ren + "-depth.png")),
         }
+        k_path = os.path.join(d, "observed", obs + "-K.txt")
+        if os.path.exists(k_path):
+            rec["K"] = np.loadtxt(k_path).reshape(3, 3)
+        return rec
 
 
 def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl", "cup"), n_iter=4, max_batch=16, device=0,
@@ -177,16 +184,20 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
     input_depth=True refines with the RGB-D network (weights with a (64, 10, 7, 7) flow_conv1) and reads each observed frame's
     `-depth.png` as well (image.py:190-219; converted on the device with DEPTH_FACTOR).
     input_mask=False refines with the image-only network (weights with a (64, 6, 7, 7) flow_conv1; ZoomImage).
+    A pair whose observed frame has a `-K.txt` (load_pair) is refined with that camera, for the render and the zoom, and the
+    other pairs with K, in one set of batches (PoseRefiner.refine with a K per instance).  Proj. 2D projects with K for every
+    pair, as the reference's evaluate_pose_arp_2d does with config.dataset.INTRINSIC_MATRIX (LM6D_REFINE.py:526).
     Returns (evaluate_pose_add result + the two extra tables, poses_est [n_iter,M,3,4], poses_gt)."""
     from . import pose_eval
     from .refiner import PoseRefiner
     meshes = [dataset.mesh(c) for c in dataset.classes]
     ref = PoseRefiner(meshes, weights, K=K, device=device, max_batch=max_batch, n_iter=n_iter, precision=precision,
                       input_depth=input_depth, depth_factor=DEPTH_FACTOR, input_mask=input_mask)
-    imgs, cls_idx, init, gt, depths = [], [], [], [], []
+    imgs, cls_idx, init, gt, depths, Ks = [], [], [], [], [], []
     for ci, c in enumerate(dataset.classes):
         for pair in dataset.pairs(c):
             rec = dataset.load_pair(c, pair)
+            Ks.append(rec.get("K"))
             imgs.append(rec["image_observed"])
             cls_idx.append(ci)
             init.append(rec["pose_rendered"])
@@ -195,7 +206,10 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
                 depths.append(read_depth_u16(os.path.join(dataset.root, "data", "observed", pair[0] + "-depth.png")))
     imgs, cls_idx = np.stack(imgs), np.asarray(cls_idx, np.int32)
     init, gt = np.stack(init).astype(np.float64), np.stack(gt).astype(np.float64)
-    poses = ref.refine(imgs, cls_idx, init, depths_u16=np.stack(depths).astype(np.uint16) if input_depth else None)
+    K_pairs = None  # one camera for every pair unless some pair has its own
+    if any(k is not None for k in Ks):
+        K_pairs = np.stack([np.asarray(K if k is None else k, np.float32).reshape(3, 3) for k in Ks])
+    poses = ref.refine(imgs, cls_idx, init, depths_u16=np.stack(depths).astype(np.uint16) if input_depth else None, K=K_pairs)
     res = pose_eval.evaluate_pose_add(ref.ctx, poses, gt, cls_idx, [dataset.points(c) for c in dataset.classes],
                                       [dataset.diameters[c] for c in dataset.classes], [c in symmetric for c in dataset.classes])
     pts_all = [dataset.points(c) for c in dataset.classes]

@@ -18,7 +18,12 @@ input_mask=False runs the image-only network (config.network.INPUT_MASK: False; 
 loop zooms with ZoomImage, boxes from the images' colours.
 
 refine_frames / submit_frames refine instances that share observed frames (several objects in one image, several initial
-hypotheses of one object) against one uploaded copy of each frame (dim_refine_frames_host)."""
+hypotheses of one object) against one uploaded copy of each frame (dim_refine_frames_host).
+
+Several cameras in one batch: refine_frames(..., K_frames=[F,3,3]) / submit_frames(..., K_frames=[f,3,3]) give every frame
+its own intrinsics, refine(..., K=[N,3,3]) / submit(..., K=[n,3,3]) every instance (the frame path with an identity map);
+dim_refine_frames_k_host_async renders and zooms each instance with its frame's K.  Without them the refiner's K serves
+every instance."""
 from __future__ import annotations
 
 import numpy as np
@@ -30,22 +35,29 @@ from . import sharding, synth
 from .context import Context
 
 
-def plan_frame_batches(frame_of, n_frames: int, max_batch: int, lo: int = 0, hi=None):
+def plan_frame_batches(frame_of, n_frames: int, max_batch: int, lo: int = 0, hi=None, K_frames=None):
     """Device batches of PoseRefiner.refine_frames for instances [lo, hi) (default: all) of frame_of (instance i observes
     frame frame_of[i] of n_frames): the contiguous slices of at most max_batch instances that refine() uses (sharding.chunks),
     each with the frames it observes.  Returns [(a, b, frames, local)]: instances a..b-1, frames = the sorted global indices
     of their frames (at most b - a <= max_batch of them), local int32 [b - a] = each instance's index into `frames`, so
     frames[local[i]] == frame_of[a + i].  Raises ValueError naming the first instance whose frame index is outside
-    [0, n_frames)."""
+    [0, n_frames).
+    K_frames [n_frames,3,3] (one camera per frame): each entry gains a fifth element, the cameras of its frames
+    K_frames[frames] (float32 [len(frames),3,3]), so that row local[i] is instance a + i's camera."""
     f = np.asarray(frame_of).reshape(-1)
     hi = len(f) if hi is None else hi
     bad = np.nonzero((f < 0) | (f >= n_frames))[0]
     if len(bad):
         raise ValueError("instance %d has frame index %d: out of range [0,%d)" % (bad[0], f[bad[0]], n_frames))
+    if K_frames is not None:
+        K_frames = np.asarray(K_frames, np.float32)
+        if K_frames.shape != (n_frames, 3, 3):
+            raise ValueError("K_frames: expected shape %s, got %s" % ((n_frames, 3, 3), K_frames.shape))
     out = []
     for a, b in sharding.chunks(lo, hi, max_batch):
         frames, local = np.unique(f[a:b], return_inverse=True)
-        out.append((a, b, frames, local.astype(np.int32).reshape(-1)))
+        e = (a, b, frames, local.astype(np.int32).reshape(-1))
+        out.append(e if K_frames is None else e + (np.ascontiguousarray(K_frames[frames]),))
     return out
 
 
@@ -78,7 +90,7 @@ class PoseRefiner:
                 "poses": torch.empty((n_iter, max_batch, 3, 4), dtype=torch.float64).pin_memory(),
                 "se3": torch.empty((n_iter, max_batch, 7), dtype=torch.float32).pin_memory(),
                 "status": torch.zeros((min(n_iter, 8) * max_batch,), dtype=torch.int32).pin_memory(),
-                "img": None, "cls": None, "pose": None, "depth": None, "frame": None,
+                "img": None, "cls": None, "pose": None, "depth": None, "frame": None, "K": None,
                 "intensity": torch.empty((n_iter, max_batch, 3), dtype=torch.float32).pin_memory() if self.light else None,
             })
         self.ctx = self.slots[0]["ctx"]
@@ -98,19 +110,23 @@ class PoseRefiner:
         buf[: t.shape[0]].copy_(t)
         return buf[: t.shape[0]]
 
-    def submit(self, images_bgr_u8, cls_idx, poses_init, depths_u16=None):
+    def submit(self, images_bgr_u8, cls_idx, poses_init, depths_u16=None, K=None):
         """Enqueue one batch (<= max_batch instances, host arrays; pinned torch tensors are used in place).
-        depths_u16: uint16 [n,H,W], required with input_depth=True.
+        depths_u16: uint16 [n,H,W], required with input_depth=True.  K: None = the refiner's K; float32 [n,3,3] = each
+        instance's own camera (submit_frames with an identity map).
         Returns a ticket for result().  At most len(slots) batches may be in flight."""
-        return self._submit(images_bgr_u8, None, cls_idx, poses_init, depths_u16)
+        if K is None:
+            return self._submit(images_bgr_u8, None, cls_idx, poses_init, depths_u16, None)
+        return self._submit(images_bgr_u8, np.arange(len(cls_idx), dtype=np.int32), cls_idx, poses_init, depths_u16, K)
 
-    def submit_frames(self, frames_bgr_u8, frame_idx, cls_idx, poses_init, depths_u16=None):
+    def submit_frames(self, frames_bgr_u8, frame_idx, cls_idx, poses_init, depths_u16=None, K_frames=None):
         """submit() against shared frames: frames_bgr_u8 uint8 [f,H,W,3] (f <= max_batch), frame_idx int [n] (instance i
         observes frames_bgr_u8[frame_idx[i]]; checked before anything is enqueued), depths_u16 uint16 [f,H,W] with
-        input_depth=True.  Each frame is uploaded once."""
-        return self._submit(frames_bgr_u8, frame_idx, cls_idx, poses_init, depths_u16)
+        input_depth=True.  Each frame is uploaded once.  K_frames: None = the refiner's K; float32 [f,3,3] = each frame's
+        camera (checked before anything is enqueued)."""
+        return self._submit(frames_bgr_u8, frame_idx, cls_idx, poses_init, depths_u16, K_frames)
 
-    def _submit(self, images_bgr_u8, frame_idx, cls_idx, poses_init, depths_u16):
+    def _submit(self, images_bgr_u8, frame_idx, cls_idx, poses_init, depths_u16, K_frames):
         i = self._next
         slot = self.slots[i]
         if slot["busy"]:
@@ -139,7 +155,8 @@ class PoseRefiner:
                                         depth_observed_u16=depth, depth_factor=self.depth_factor)
             else:
                 fidx = self._pinned(slot, "frame", frame_idx, torch.int32)
-                slot["ctx"].refine_frames_host(img, fidx, cls, pose, self.K, self.n_iter, self.zn, self.zf, self.means,
+                K = self.K if K_frames is None else self._pinned(slot, "K", np.asarray(K_frames, np.float32), torch.float32)
+                slot["ctx"].refine_frames_host(img, fidx, cls, pose, K, self.n_iter, self.zn, self.zf, self.means,
                                                self.precision, poses_out=slot["poses"], se3_out=slot["se3"], sync=False,
                                                lighting=lit, depth_frames_u16=depth, depth_factor=self.depth_factor)
             slot["ctx"].refine_status(n, self.n_iter, out=slot["status"], sync=False)
@@ -170,12 +187,17 @@ class PoseRefiner:
         return p.numpy().copy()
 
     # ------------------------------------------------------------------------------ convenience
-    def refine(self, images_bgr_u8, cls_idx, poses_init, dist=None, depths_u16=None):
+    def refine(self, images_bgr_u8, cls_idx, poses_init, dist=None, depths_u16=None, K=None):
         """images_bgr_u8 [N,H,W,3] uint8 (cv2 layout), cls_idx [N] int, poses_init [N,3,4] float64 (host); depths_u16 [N,H,W]
-        uint16 with input_depth=True.
+        uint16 with input_depth=True; K: None = the refiner's K for every instance, [N,3,3] = each instance's own camera
+        (several cameras in one batch; instance i's poses equal refine() by a refiner built with K[i], bit for bit).
         Returns poses [n_iter,N,3,4] float64 (host).  With torch.distributed initialised each rank
         processes its contiguous slice and the poses are all-gathered."""
         n = len(cls_idx)
+        if K is not None:
+            K = np.asarray(K, np.float32)
+            if K.shape != (n, 3, 3):
+                raise ValueError("K: expected one camera per instance %s, got %s" % ((n, 3, 3), K.shape))
         rank, world = (dist.get_rank(), dist.get_world_size()) if dist is not None and dist.is_initialized() else (0, 1)
         lo, hi = sharding.shard_range(n, rank, world)
         out = np.zeros((self.n_iter, hi - lo, 3, 4), np.float64)
@@ -185,18 +207,21 @@ class PoseRefiner:
                 t, (pa, pb) = pending.pop(0)
                 out[:, pa - lo:pb - lo] = self.result(t)
             d = None if depths_u16 is None else depths_u16[a:b]
-            pending.append((self.submit(images_bgr_u8[a:b], cls_idx[a:b], poses_init[a:b], d), (a, b)))
+            k = None if K is None else K[a:b]
+            pending.append((self.submit(images_bgr_u8[a:b], cls_idx[a:b], poses_init[a:b], d, k), (a, b)))
         for t, (pa, pb) in pending:
             out[:, pa - lo:pb - lo] = self.result(t)
         return sharding.gather_results(out, n, axis=1, dist=dist, device=self.ctx.device if world > 1 else None)
 
-    def refine_frames(self, frames_bgr_u8, frame_of, cls_idx, poses_init, dist=None, depths_u16=None):
+    def refine_frames(self, frames_bgr_u8, frame_of, cls_idx, poses_init, dist=None, depths_u16=None, K_frames=None):
         """refine() with instances that share observed frames (several objects of one image, several initial hypotheses of
         one object): frames_bgr_u8 [F,H,W,3] uint8, frame_of [N] int (instance i observes frames_bgr_u8[frame_of[i]]),
         cls_idx [N], poses_init [N,3,4] float64; depths_u16 [F,H,W] uint16 with input_depth=True.
         The device batches are refine()'s (plan_frame_batches), each uploading only the frames its instances observe, so the
         result equals refine(frames_bgr_u8[frame_of], ...) bit for bit; keeping the instances of a frame next to each other
-        uploads each frame once.  Sharded over instances like refine(): a rank uploads the frames of its slice only."""
+        uploads each frame once.  Sharded over instances like refine(): a rank uploads the frames of its slice only.
+        K_frames: None = the refiner's K; [F,3,3] = each frame's camera, carried into every device batch with its frames
+        (plan_frame_batches), so instance i's poses equal a refiner built with K_frames[frame_of[i]], bit for bit."""
         n = len(cls_idx)
         if len(frame_of) != n:
             raise ValueError("frame_of has %d entries for %d instances" % (len(frame_of), n))
@@ -204,12 +229,12 @@ class PoseRefiner:
         lo, hi = sharding.shard_range(n, rank, world)
         out = np.zeros((self.n_iter, hi - lo, 3, 4), np.float64)
         pending = []
-        for a, b, frames, local in plan_frame_batches(frame_of, len(frames_bgr_u8), self.max_batch, lo, hi):
+        for a, b, frames, local, *k in plan_frame_batches(frame_of, len(frames_bgr_u8), self.max_batch, lo, hi, K_frames):
             if len(pending) == len(self.slots):
                 t, (pa, pb) = pending.pop(0)
                 out[:, pa - lo:pb - lo] = self.result(t)
             d = None if depths_u16 is None else depths_u16[frames]
-            pending.append((self.submit_frames(frames_bgr_u8[frames], local, cls_idx[a:b], poses_init[a:b], d), (a, b)))
+            pending.append((self.submit_frames(frames_bgr_u8[frames], local, cls_idx[a:b], poses_init[a:b], d, *k), (a, b)))
         for t, (pa, pb) in pending:
             out[:, pa - lo:pb - lo] = self.result(t)
         return sharding.gather_results(out, n, axis=1, dist=dist, device=self.ctx.device if world > 1 else None)
