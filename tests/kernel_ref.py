@@ -311,10 +311,12 @@ def fc6_nhwc(a):
     return np.ascontiguousarray(np.asarray(a).reshape(256, 1024, 80).transpose(0, 2, 1)).reshape(256, 81920)
 
 
-def check_fc6_heads(weights, mode, B, act10, rot, trans, tag=""):
+def check_fc6_heads(weights, mode, B, act10, rot, trans, tag="", zoom_factor=None):
     """rot / trans of net_forward against float64 fc6 -> fc7 -> heads from the stored act[10] = (hi, lo) float32 numpy
     [>= B, 8, 10, 1024]: fc6's operands as its 16-bit pack rounds them, fc7 / rot / trans from the fp32 weights.  The error
-    scale S of fc6 is carried through fc7 and the heads by their absolute weights (LeakyReLU moves no difference up)."""
+    scale S of fc6 is carried through fc7 and the heads by their absolute weights (LeakyReLU moves no difference up).
+    zoom_factor [>= B, 4] (the refinement loop's se3): trans x and y are the head's outputs times wx in float32
+    (invZoomTrans), so ref and S of those two are scaled by wx and the product's rounding, 2^-24 relative, is allowed."""
     lrelu = lambda v: F.leaky_relu(v, 0.1)
     W6 = operand(fc6_nhwc(weights["fc6_weight"]), mode)
     wb = {k: gpu(weights[k]) for k in ("fc6_bias", "fc7_weight", "fc7_bias", "rot_weight", "rot_bias", "trans_weight",
@@ -328,8 +330,15 @@ def check_fc6_heads(weights, mode, B, act10, rot, trans, tag=""):
     E7 = E6 @ w7.abs().T + h6.abs() @ w7.abs().T + wb["fc7_bias"].abs()
     for name, dev in (("rot", rot), ("trans", trans)):
         w, b = wb[name + "_weight"], wb[name + "_bias"]
-        check("fc6_head", "%s (%s, B=%d%s)" % (name, mode, B, tag), dev, h7 @ w.T + b, E7 @ w.abs().T + h7.abs() @ w.abs().T + b.abs(),
-              0.0, KAPPA_INFER["fc6_head"], lambda idx: "(image %d, output %d)" % idx)
+        ref, S, slack = h7 @ w.T + b, E7 @ w.abs().T + h7.abs() @ w.abs().T + b.abs(), None
+        if name == "trans" and zoom_factor is not None:
+            s = torch.ones_like(ref)
+            s[:, :2] = gpu(np.asarray(zoom_factor)[:B, :1])
+            ref, S = ref * s, S * s.abs()
+            slack = torch.zeros_like(ref)
+            slack[:, :2] = U * ref[:, :2].abs()
+        check("fc6_head", "%s (%s, B=%d%s)" % (name, mode, B, tag), dev, ref, S, 0.0, KAPPA_INFER["fc6_head"],
+              lambda idx: "(image %d, output %d)" % idx, slack=slack)
 
 
 def check_conv_layer(weights, mode, layer, B, x, out, geo, tag=""):

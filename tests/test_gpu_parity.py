@@ -166,8 +166,24 @@ def test_zoom_image_flow_depth_mask_ops_bit_exact(ctx, zoom_inputs):
     zio, zir = ctx.zoom_image_with_factor(zf, dev(z["img_o"]), dev(z["img_r"]), MEANS32)
     ozio, ozir = O.zoom_image_with_factor(ozf, z["img_o"], z["img_r"], MEANS32)
     assert np.array_equal(zio.cpu().numpy(), ozio) and np.array_equal(zir.cpu().numpy(), ozir)
-    # out-of-frame samples come back as -mean (black), quirk App.B-6
-    assert np.isclose(zio.cpu().numpy().min(), -MEANS32.max(), atol=1e-4) or True
+    # out-of-frame samples come back as -mean (black), quirk App.B-6: with a crop wider than the frame (wx = 2) every output
+    # whose four taps lie outside the frame is the sampler's 0 minus the float32 mean, exactly
+    wide = np.array([[2.0, 2.0, 0.1, -0.05], [2.0, 2.0, -0.3, 0.2], [2.0, 2.0, 0.0, 0.0]], np.float32)
+    zio2, zir2 = ctx.zoom_image_with_factor(dev(wide), dev(z["img_o"]), dev(z["img_r"]), MEANS32)
+    one = np.float32(1)
+
+    def taps_out(n, w, t):
+        """outputs of one axis whose two taps c0, c0 + 1 both lie outside [0, n - 1] (src_coord's float32 sequence)"""
+        ct = -one + np.arange(n, dtype=np.float32) * np.float32(2.0 / (n - 1))
+        cr = ((w * ct + t + one) * np.float32(n - 1)) / np.float32(2)
+        f0 = np.floor(cr)
+        return (f0 + 1 < 0) | (f0 > n - 1)
+    for b in range(z["B"]):
+        out = taps_out(H, wide[b, 1], wide[b, 3])[:, None] | taps_out(W, wide[b, 0], wide[b, 2])[None, :]
+        assert 0.2 * H * W < out.sum() < H * W
+        for img in (zio2, zir2):
+            for c in range(3):
+                assert (img[b, c].cpu().numpy()[out] == -MEANS32[c]).all(), (b, c)
     for inv in (False, True):
         got = ctx.zoom_mask_with_factor(zf, dev(z["depth"]), inv)
         assert np.array_equal(got.cpu().numpy(), O.zoom_mask_with_factor(ozf, z["depth"], inv))
