@@ -105,7 +105,9 @@ int net_create(dim_ctx *ctx);
 void net_destroy(dim_ctx *ctx);
 int net_load(dim_ctx *ctx, const float *const *W, const float *const *Bv);
 int net_alloc_weights(dim_ctx *ctx);
-int net_pack_weights(dim_ctx *ctx, const float *const *w, cudaStream_t st, bool with_lo, bool with_f16);
+// net_pack_weights' `packs`: the bf16 hi packs (with fc7^T), the bf16x3 lo halves, the fp16 packs
+enum : unsigned { PACK_HI = 1, PACK_LO = 2, PACK_F16 = 4 };
+int net_pack_weights(dim_ctx *ctx, const float *const *w, cudaStream_t st, unsigned packs);
 void net_input_geometry(dim_ctx *ctx, int *rows, int *cols, int *pad, __nv_bfloat16 **hi, __nv_bfloat16 **lo);
 int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, float *rot_out, float *trans_out,
                 float *se3_out, cudaStream_t st, cudaEvent_t after_conv);
@@ -123,6 +125,7 @@ int train_create(dim_ctx *ctx, int max_points);
 void train_destroy(dim_ctx *ctx);
 int train_load_params(dim_ctx *ctx, const float *flat_host, size_t n, cudaStream_t st);
 int train_refresh_lo(dim_ctx *ctx, cudaStream_t st);
+int train_refresh_f16(dim_ctx *ctx, cudaStream_t st);
 void train_drop_maps(dim_ctx *ctx);
 int train_get_params(dim_ctx *ctx, float *flat_host, size_t n, int which, cudaStream_t st);
 size_t train_param_count(dim_ctx *ctx);

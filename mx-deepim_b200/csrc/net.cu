@@ -455,55 +455,34 @@ int net_alloc_weights(dim_ctx *ctx) {
 }
 
 // w[0..9]: conv1 ... conv6_1 (Cout, Cin, k, k), w[10]: fc6 (256, hw, c), w[11]: fc7 (out, in), device fp32.  Packs are
-// written on st; a pack left out (with_lo / with_f16 false) is marked stale.
-int net_pack_weights(dim_ctx *ctx, const float *const *w, cudaStream_t st, bool with_lo, bool with_f16) {
+// written on st, each rounded once from w.  `packs` (PACK_*) names the packs to write: PACK_HI means new weights, so every
+// pack left out goes stale; without it only the packs named are brought up to w (a lazy refresh from an unchanged master).
+int net_pack_weights(dim_ctx *ctx, const float *const *w, cudaStream_t st, unsigned packs) {
   NetState *ns = ctx->net;
-  auto L = [with_lo](__nv_bfloat16 *p) { return with_lo ? p : nullptr; };
-  auto F = [with_f16](__nv_bfloat16 *p) { return with_f16 ? p : nullptr; };
+  auto H = [packs](__nv_bfloat16 *p) { return packs & PACK_HI ? p : nullptr; };
+  auto L = [packs](__nv_bfloat16 *p) { return packs & PACK_LO ? p : nullptr; };
+  auto F = [packs](__nv_bfloat16 *p) { return packs & PACK_F16 ? p : nullptr; };
   if (ns->input_depth)
-    pack_conv1_rgbd_kernel<<<64 * 1024 / 256, 256, 0, st>>>(w[0], ns->w_hi[0], L(ns->w_lo[0]), F(ns->w_f16[0]));
+    pack_conv1_rgbd_kernel<<<64 * 1024 / 256, 256, 0, st>>>(w[0], H(ns->w_hi[0]), L(ns->w_lo[0]), F(ns->w_f16[0]));
   else
-    pack_conv1_kernel<<<64 * 512 / 256, 256, 0, st>>>(w[0], ns->input_mask ? 8 : 6, ns->w_hi[0], L(ns->w_lo[0]), F(ns->w_f16[0]));
+    pack_conv1_kernel<<<64 * 512 / 256, 256, 0, st>>>(w[0], ns->input_mask ? 8 : 6, H(ns->w_hi[0]), L(ns->w_lo[0]),
+                                                      F(ns->w_f16[0]));
   DIM_LAUNCH_CHECK();
   for (int i = 1; i < 10; ++i) {
     const LayerSpec &s = kLayers[i];
-    pack_conv_fwd_kernel<<<dim3(s.Cout, cdiv(s.Cin, 64)), 256, 0, st>>>(w[i], s.Cout, s.Cin, s.k, ns->w_hi[i], L(ns->w_lo[i]),
-                                                                          F(ns->w_f16[i]));
+    pack_conv_fwd_kernel<<<dim3(s.Cout, cdiv(s.Cin, 64)), 256, 0, st>>>(w[i], s.Cout, s.Cin, s.k, H(ns->w_hi[i]),
+                                                                          L(ns->w_lo[i]), F(ns->w_f16[i]));
     DIM_LAUNCH_CHECK();
   }
-  pack_fc6_kernel<<<256 * FC6_K / 256, 256, 0, st>>>(w[10], ns->fc6_w_hi, L(ns->fc6_w_lo), F(ns->fc6_w_f16));
+  pack_fc6_kernel<<<256 * FC6_K / 256, 256, 0, st>>>(w[10], H(ns->fc6_w_hi), L(ns->fc6_w_lo), F(ns->fc6_w_f16));
   DIM_LAUNCH_CHECK();
-  transpose256_kernel<<<256, 256, 0, st>>>(w[11], ns->fc7_wT);
-  DIM_LAUNCH_CHECK();
-  ns->lo_stale = !with_lo;
-  ns->f16_stale = !with_f16;
-  return 0;
-}
-
-// fp16 operand packs re-derived on the device from the bf16 hi/lo pair (hi + lo carries 16 significant bits): used
-// after a training update refreshed hi/lo from the fp32 master weights (train.cu repack_all)
-__global__ void __launch_bounds__(256) f16_from_hilo_kernel(const __nv_bfloat16 *hi, const __nv_bfloat16 *lo, size_t n,
-                                                            __nv_bfloat16 *out) {
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const __half h = __float2half_rn(__bfloat162float(hi[i]) + __bfloat162float(lo[i]));
-  reinterpret_cast<__half *>(out)[i] = h;
-}
-
-static int net_refresh_f16(dim_ctx *ctx, cudaStream_t st) {
-  NetState *ns = ctx->net;
-  if (ns->lo_stale)
-    if (int rc = train_refresh_lo(ctx, st)) return rc;
-  for (int i = 0; i < 10; ++i) {
-    const LayerGeom &g = ns->g[i];
-    const size_t n = (size_t)g.Cout * g.KH * g.KW * g.Ceff;
-    f16_from_hilo_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ns->w_hi[i], ns->w_lo[i], n, ns->w_f16[i]);
+  if (packs & PACK_HI) {
+    transpose256_kernel<<<256, 256, 0, st>>>(w[11], ns->fc7_wT);
     DIM_LAUNCH_CHECK();
+    ns->lo_stale = ns->f16_stale = true;
   }
-  const size_t n6 = (size_t)256 * FC6_K;
-  f16_from_hilo_kernel<<<(unsigned)((n6 + 255) / 256), 256, 0, st>>>(ns->fc6_w_hi, ns->fc6_w_lo, n6, ns->fc6_w_f16);
-  DIM_LAUNCH_CHECK();
-  ns->f16_stale = false;
+  if (packs & PACK_LO) ns->lo_stale = false;
+  if (packs & PACK_F16) ns->f16_stale = false;
   return 0;
 }
 
@@ -549,7 +528,7 @@ int net_load(dim_ctx *ctx, const float *const *W, const float *const *Bv) {
   DIM_CHECK(put(ns->rot_b, Bv[12], 4));
   DIM_CHECK(put(ns->trans_w, W[13], 3 * 256));
   DIM_CHECK(put(ns->trans_b, Bv[13], 3));
-  if (int rc = net_pack_weights(ctx, w, 0, /*with_lo=*/true, /*with_f16=*/true)) return rc;
+  if (int rc = net_pack_weights(ctx, w, 0, PACK_HI | PACK_LO | PACK_F16)) return rc;
   DIM_CHECK(cudaStreamSynchronize(0));
   ns->loaded = true;
   return 0;
@@ -665,7 +644,7 @@ int net_forward(dim_ctx *ctx, int B, int precision, const float *zoom_factor, fl
   if (s3 && ns->lo_stale)
     if (int rc = train_refresh_lo(ctx, st)) return rc;
   if (f16 && ns->f16_stale)
-    if (int rc = net_refresh_f16(ctx, st)) return rc;
+    if (int rc = train_refresh_f16(ctx, st)) return rc;
   if (ns->layer_events) DIM_CHECK(cudaEventRecord(ns->layer_events[0], st));
   for (int i = 0; i < 10; ++i) {
     const LayerGeom &g = ns->g[i];

@@ -41,7 +41,7 @@ __host__ __device__ inline int conv1_kslot(int dw, int ph, int pw) { return dw =
 __device__ __forceinline__ void store_split(__nv_bfloat16 *hi, __nv_bfloat16 *lo, size_t i, float v,
                                             __nv_bfloat16 *f16 = nullptr) {
   const __nv_bfloat16 h = __float2bfloat16_rn(v);
-  hi[i] = h;
+  if (hi) hi[i] = h;
   if (lo) lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
   if (f16) reinterpret_cast<__half *>(f16)[i] = __float2half_rn(v);  // inf only for |w| > 65504
 }
@@ -57,7 +57,7 @@ struct NetState {
   __nv_bfloat16 *fc6_w_hi = nullptr, *fc6_w_lo = nullptr;  // [256][81920] in (h,w,c) order
   __nv_bfloat16 *fc6_w_f16 = nullptr;
   bool train_aliased = false;  // dim_train_load_params made biases / head parameters alias the fp32 master vector
-  bool f16_stale = false;  // training updated the weights: the fp16 packs are re-derived lazily (net_refresh_f16)
+  bool f16_stale = false;  // training updated the weights: the fp16 packs are packed lazily from the master (train_refresh_f16)
   float *fc6_b = nullptr, *fc7_wT = nullptr, *fc7_b = nullptr, *rot_w = nullptr, *rot_b = nullptr,
         *trans_w = nullptr, *trans_b = nullptr;
   float *fc6_partial = nullptr;  // [FC6_SPLITS][max_batch][256]
@@ -72,7 +72,9 @@ struct NetState {
   bool input_mask = true;
   float *save_h6 = nullptr, *save_h7 = nullptr;  // training: fc6 / fc7 activations kept for the backward pass ([B][256])
   cudaEvent_t repack_done = nullptr;  // training: the operand packs are refreshed on an internal stream after an update;
-                                      // every consumer (net_forward) orders itself behind this event
+                                      // every consumer (net_forward) orders itself behind this event.  A lazy refresh in
+                                      // net_forward moves it to the caller's stream, so that the next update's SGD waits
+                                      // until that refresh has read the master too
   bool lo_stale = false;  // training updated the weights without refreshing the bf16 'lo' halves (bf16x3 mode refreshes lazily)
   // per batch size (+ kF16MapKey for the fp16 operand maps).  Tensor maps and layer parameters only: the launch schedule
   // comes from dim_ctx::num_sms at every net_forward, so a change of the SM count leaves these valid

@@ -860,16 +860,22 @@ void train_destroy(dim_ctx *ctx) {
     DIM_LAUNCH_CHECK();                                                           \
   } while (0)
 
+// the master's conv1 ... conv6_1, fc6 and fc7 weights in net_pack_weights' order
+static void master_weights(const TrainState *ts, const float *w[12]) {
+  for (int i = 0; i < 12; ++i) w[i] = ts->master + ts->off[i].w;
+}
+
 // refresh every bf16 operand pack (and the fp32 head parameters of the inference net) from the master weights
 // with_lo = false skips the bf16 'lo' halves (only the bf16x3 modes read them); they are then marked stale and refreshed
 // lazily by train_refresh_lo() the next time the bf16x3 inference mode runs, or by the switch of the step to bf16x3.  The
-// fp16 packs of DIM_PREC_FP16 are marked stale too: net_forward re-derives them from hi/lo when that mode next runs
+// fp16 packs of DIM_PREC_FP16 are marked stale too: only that inference mode reads them, and train_refresh_f16() packs them
+// from the master when it next runs
 static int repack_all(dim_ctx *ctx, cudaStream_t st, bool with_lo) {
   TrainState *ts = train_of(ctx);
   const float *M = ts->master;
   const float *w[12];
-  for (int i = 0; i < 12; ++i) w[i] = M + ts->off[i].w;
-  if (int rc = net_pack_weights(ctx, w, st, with_lo, /*with_f16=*/false)) return rc;
+  master_weights(ts, w);
+  if (int rc = net_pack_weights(ctx, w, st, PACK_HI | (with_lo ? PACK_LO : 0u))) return rc;
   // the training packs' lo halves exist once the step has run in bf16x3 (nullptr before)
   auto L = [with_lo](__nv_bfloat16 *lo) { return with_lo ? lo : nullptr; };
   for (int i = 1; i < 10; ++i) {
@@ -926,10 +932,30 @@ void train_drop_maps(dim_ctx *ctx) {
   if (TrainState *ts = train_of(ctx)) ts->maps.clear();
 }
 
+// a lazy refresh on the caller's stream st read the master: the next update's SGD must wait for it as for its own repack
+static int refreshed_on(dim_ctx *ctx, TrainState *ts, cudaStream_t st) {
+  DIM_CHECK(cudaEventRecord(ts->ev_repack, st));
+  ctx->net->repack_done = ts->ev_repack;
+  return 0;
+}
+
 // called by net_forward before a bf16x3 pass when the training step left the lo halves stale
 int train_refresh_lo(dim_ctx *ctx, cudaStream_t st) {
-  if (train_of(ctx) == nullptr) return 0;
-  return repack_all(ctx, st, true);
+  TrainState *ts = train_of(ctx);
+  if (ts == nullptr) return 0;
+  if (int rc = repack_all(ctx, st, true)) return rc;
+  return refreshed_on(ctx, ts, st);
+}
+
+// called by net_forward before an fp16 pass after an update: the fp16 packs from the master, rounded once as dim_net_load
+// rounds them, so a training context and an inference context loaded with its weights run the same fp16 network
+int train_refresh_f16(dim_ctx *ctx, cudaStream_t st) {
+  TrainState *ts = train_of(ctx);
+  if (ts == nullptr) return 0;
+  const float *w[12];
+  master_weights(ts, w);
+  if (int rc = net_pack_weights(ctx, w, st, PACK_F16)) return rc;
+  return refreshed_on(ctx, ts, st);
 }
 
 // the lo halves of the step's bf16 buffers and of its operand packs (bf16x3); zero-filled, so borders and padding channels

@@ -1,7 +1,8 @@
 """GPU: the two ways weights reach the inference network build the same operand packs.  One context loads a checkpoint with
 Context.load_weights (dim_net_load), another with Trainer (dim_train_load_params, whose flat vector holds fc6 permuted to
-(256, hw, c)); net_forward on the same zoomed inputs must return bit-identical rot / trans in bf16 (the hi packs) and bf16x3
-(hi and lo), for the mask, image-only and RGB-D networks."""
+(256, hw, c)); net_forward on the same zoomed inputs must return bit-identical rot / trans in bf16 (the hi packs), bf16x3
+(hi and lo) and fp16 (the fp16 packs: each weight rounded once from fp32, also on a training context), for the mask,
+image-only and RGB-D networks."""
 import numpy as np
 import pytest
 
@@ -39,7 +40,7 @@ def test_net_load_and_train_load_build_the_same_packs(net):
         a.load_weights(w)
         Trainer(b, w)
         args, depths = _inputs(net, 7)
-        for prec in (capi.PREC_BF16, capi.PREC_BF16X3):
+        for prec in (capi.PREC_BF16, capi.PREC_BF16X3, capi.PREC_FP16):
             ra, ta = a.net_forward(*args, precision=prec, **depths)
             rb, tb = b.net_forward(*args, precision=prec, **depths)
             torch.cuda.synchronize()
