@@ -33,7 +33,7 @@ extern "C" {
 
 typedef struct dim_ctx dim_ctx;
 
-#define DIM_ABI_VERSION 3
+#define DIM_ABI_VERSION 4
 DIM_API int32_t dim_abi_version(void);
 DIM_API const char *dim_last_error(void);
 
@@ -177,20 +177,20 @@ DIM_API int32_t dim_transform3d_bwd(dim_ctx *ctx, const float *out_grad, const f
 
 /* Lighting of the ModelNet / unseen-object configuration (config.dataset.dataset "ModelNet*": deepim/core/tester.py:114-133,
  * 146-185; lib/pair_matching/batch_updater_py_multi.py:35-52,187-229).  The `lighting` argument of dim_train_update,
- * dim_refine and dim_refine_host(_async): NULL = the unlit renderer; otherwise every render of the call is the Lambert-lit
+ * dim_refine and dim_refine_host_async: NULL = the unlit renderer; otherwise every render of the call is the Lambert-lit
  * renderer of dim_render_lit.  The light follows the pose being rendered: in the GL camera frame
  *   light_position = float32(offset[0] + t_x, offset[1] - t_y, offset[2] - t_z)
  * computed from the float64 pose (the reference's hard-coded light index 2 gives offset = (0, 0.5, 0.5)).  The reference
  * draws light_intensity from U(0.9, 1.1)^3 afresh for every render; here the caller supplies the draws.
  *   intensity (non-NULL): device f32 [n_iter,B,3] for dim_refine (iteration it renders with intensity[it]), [B,3] for
- *              dim_train_update, HOST f32 [n_iter,B,3] for dim_refine_host(_async) (n_iter <= 8; copied to the
+ *              dim_train_update, HOST f32 [n_iter,B,3] for dim_refine_host_async (n_iter <= 8; copied to the
  *              context on `stream` before the call returns, so a pageable buffer may be reused at once).
  *   brightness_ratio: colour = texel * ((1 - ratio) + ratio * brightness) * intensity (the reference: 0.7).
  * Depth, masks, bboxes, zoom, labels and flow are those of the unlit calls; only the colours change.  Every uploaded mesh
  * must have normals (dim_mesh_upload_normals).  Lit loops share dim_refine_status and are captured / replayed as CUDA
  * graphs like unlit ones. */
 typedef struct dim_lighting {
-  const float *intensity; /* see above: device [n_iter,B,3] (refine) / [B,3] (train update); host for dim_refine_host */
+  const float *intensity; /* see above: device [n_iter,B,3] (refine) / [B,3] (train update); host for dim_refine_host_async */
   double offset[3];       /* light at zero translation, GL frame; the reference: (0, 0.5, 0.5) */
   float brightness_ratio; /* the reference: 0.7 */
 } dim_lighting;
@@ -235,13 +235,13 @@ DIM_API int32_t dim_train_update(dim_ctx *ctx, const int32_t *cls_idx, const flo
  * to the image-only network, 1 back.  Depth input without the mask channels (INPUT_DEPTH without INPUT_MASK) is not
  * supported: each switch refuses it.
  * Every entry point follows the context's network, with these rules:
- *   - depth inputs (depth_observed of dim_refine, depth_observed_u16_host of dim_refine_host(_async), zoom_depth_* of
+ *   - depth inputs (depth_frames of dim_refine, depth_frames_u16_host of dim_refine_host_async, zoom_depth_* of
  *     dim_net_fwd and dim_train_forward_backward) are non-NULL exactly on an RGB-D context; otherwise the call fails with a
  *     message naming the argument and dim_ctx_set_input_depth;
  *   - mask inputs (zoom_mask_* of dim_net_fwd and dim_train_forward_backward) are NULL exactly on an image-only context;
  *   - dim_net_load takes the network's flow_conv1 weight; the flat training vector is the network's table
  *     (dim_train_param_info) and dim_train_param_count reports its size.
- * On an image-only context dim_refine / dim_refine_host(_async) run the image-only chain: the observed box is computed once
+ * On an image-only context dim_refine / dim_refine_host_async run the image-only chain: the observed box is computed once
  * per call, the rendered box of every iteration from the render's colours; the zoom factor is ZoomImage's (ZoomMask's
  * arithmetic with the observed-centre fallback for an empty render).  dim_refine_status: bit 0 = the observed image has no
  * valid pixel (the reference raises; the fallback factor (1,1,0,0) was used), bit 2 = the rendered image has none (the
@@ -275,119 +275,71 @@ DIM_API int32_t dim_net_fwd(dim_ctx *ctx, const float *zoom_image_observed,
 
 /* The fused test-time loop (deepim/core/tester.py:340-485 with FAST_TEST / UPDATE_MASK
  * box_rendered): n_iter x (render -> bbox+zoom -> FlowNetS -> ZoomTrans^-1 -> RT_transform),
- * everything on the device, no host sync.
- *   image_observed f32[B,3,H,W] RGB-mean (constant over iterations)
- *   cls_idx i32[B]; pose_init f64[B,3,4]
- *   outputs (device): poses f64[n_iter,B,3,4], se3 f32[n_iter,B,7], zoom_factor f32[n_iter,B,4],
+ * everything on the device, no host sync.  Two entries run it: dim_refine on device buffers, dim_refine_host_async on host
+ * buffers.  Both take B instances observing F frames, 1 <= B, F <= max_batch; each frame is uploaded (host entry) and
+ * packed once per call, however many instances observe it.
+ *   frame_idx i32[B] or NULL: instance b observes frame frame_idx[b] (several objects of one image, or several initial
+ *     hypotheses of one object); its results equal those of a call with frame frame_idx[b] as frame b, bit for bit.
+ *     NULL: instance b observes frame b, and F must equal B (the call is refused otherwise).
+ *   K9_host f32[9] (one camera for every instance) or K_frames f32[F,9] (one camera per frame, row-major): exactly one is
+ *     non-NULL (the call is refused otherwise).  K_frames is read through the frame map: instance b is rendered and zoomed
+ *     with K_frames[frame_of(b)] -- the frame whose taps it observes; row b without a map.  One K serves both the render
+ *     and the zoom centre K . t (the reference's per-pair `<observed>-K.txt`, tester.py:424-427, zooms with the config's K
+ *     even when the pair has its own).  Instance b's results equal those of K9 = K_frames[frame_of(b)], bit for bit.
+ *   cls_idx i32[B]; pose_init f64[B,3,4].
+ *   lighting: nullable, see dim_lighting.  Image-only network: the observed box is computed once per frame.
+ *
+ * dim_refine: every pointer but K9_host / pixel_means_rgb_host is a device pointer.
+ *   image_frames f32[F,3,H,W] RGB-mean (constant over iterations); depth_frames: RGB-D network only, f32 [F,1,H,W] in
+ *   metres; lighting->intensity device [n_iter,B,3].
+ *   frame_idx is not checked on the host: an index outside [0, F) makes the instance observe frame 0 (and use K_frames
+ *   row 0) and sets status bit 3 (dim_refine_status) in every iteration; nothing is read outside the F frames.  K_frames
+ *   is read as given (not checked).
+ *   outputs: poses f64[n_iter,B,3,4], se3 f32[n_iter,B,7], zoom_factor f32[n_iter,B,4],
  *   bbox i32[n_iter,B,8]; any of the last three may be NULL.
  *   pose_override f64[n_iter,B,3,4] or NULL: when given, iteration `it` starts from
  *   pose_override[it] instead of the previous estimate (teacher forcing for parity tests).
- *   depth_observed: RGB-D network only, f32 [B,1,H,W] in metres (constant over the iterations).
- *   lighting: nullable, see dim_lighting (device intensity [n_iter,B,3]).
- * After one eager run of an argument set the chain is captured as a CUDA graph and replayed (keyed on every argument,
- * the depth and intensity pointers included). */
-DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx,
-                           const double *pose_init, int32_t B, int32_t n_iter, const float *K9_host,
-                           float znear, float zfar, const double *pixel_means_rgb_host,
-                           int32_t precision, const double *pose_override, double *poses,
-                           float *se3, float *zoom_factor, int32_t *bbox, const float *depth_observed,
-                           const dim_lighting *lighting, void *stream);
+ *   After one eager run of an argument set the chain is captured as a CUDA graph and replayed (keyed on every argument,
+ *   the depth, intensity, frame_idx and K_frames pointers included).  The graph reads frame_idx and K_frames at replay:
+ *   new indices or intrinsics written into the same buffers need no re-capture; another buffer is another graph.
+ *
+ * dim_refine_host_async: host buffers (what deepim/core/tester.py:pred_eval would call).  frames_u8_host u8[F,H,W,3] BGR
+ *   (as cv2.imread returns; transformed on device as lib/utils/image.py:583-594), frame_idx_host / K_frames_host /
+ *   cls_idx_host / pose_init_host on the host; poses_out_host f64[n_iter,B,3,4], se3_out_host f32[n_iter,B,7] (nullable);
+ *   n_iter in [1, 8].
+ *   depth_frames_u16_host: RGB-D network only, the host depth file values u16 [F,H,W], converted on the device as
+ *   lib/utils/image.py:203,218 does: float32(u16) / float32(depth_factor) (LINEMOD: 1000; depth_factor is checked only
+ *   when a depth is given).  lighting->intensity HOST [n_iter,B,3] (copied to the context on `stream` before the call
+ *   returns, so a pageable buffer may be reused at once).
+ *   Every class index, frame index and K_frames_host row is checked before anything is enqueued: a class index without a
+ *   mesh, a frame index outside [0, F) or a row that is not a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]] with
+ *   fx, fy > 0 fails the call with a message naming the instance or frame.  K9_host is not checked.
+ *   Returns right after enqueueing the copies and kernels on `stream` (no synchronisation): the host output buffers are
+ *   valid once the stream has been synchronised.  Pinned buffers are recommended; they let a caller overlap the H2D copy
+ *   of batch k+1 (second context / stream) with the compute of k. */
+DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx,
+                           const float *K9_host, const float *K_frames, const int32_t *cls_idx,
+                           const double *pose_init, int32_t B, int32_t n_iter, float znear, float zfar,
+                           const double *pixel_means_rgb_host, int32_t precision, const double *pose_override,
+                           double *poses, float *se3, float *zoom_factor, int32_t *bbox,
+                           const float *depth_frames, const dim_lighting *lighting, void *stream);
+DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *frames_u8_host, int32_t F,
+                                      const int32_t *frame_idx_host, const float *K9_host,
+                                      const float *K_frames_host, const int32_t *cls_idx_host,
+                                      const double *pose_init_host, int32_t B, int32_t n_iter, float znear,
+                                      float zfar, const double *pixel_means_rgb_host, int32_t precision,
+                                      double *poses_out_host, float *se3_out_host,
+                                      const uint16_t *depth_frames_u16_host, float depth_factor,
+                                      const dim_lighting *lighting, void *stream);
 
-/* Host-buffer convenience around dim_refine (what deepim/core/tester.py:pred_eval would call):
- * image_observed_u8 host u8[B,H,W,3] BGR (as cv2.imread returns; transformed on device as
- * lib/utils/image.py:583-594), cls_idx host, pose_init host f64; poses_out host f64[n_iter,B,3,4].
- * depth_observed_u16_host: RGB-D network only, the host depth file values u16 [B,H,W], converted on the device as
- * lib/utils/image.py:203,218 does: float32(u16) / float32(depth_factor) (LINEMOD: 1000; depth_factor is checked only
- * when a depth is given).  lighting: nullable, see dim_lighting (HOST intensity [n_iter,B,3]).
- * Pinned buffers are recommended.  Synchronises the stream before returning. */
-DIM_API int32_t dim_refine_host(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
-                                const int32_t *cls_idx_host, const double *pose_init_host,
-                                int32_t B, int32_t n_iter, const float *K9_host, float znear,
-                                float zfar, const double *pixel_means_rgb_host, int32_t precision,
-                                double *poses_out_host, float *se3_out_host,
-                                const uint16_t *depth_observed_u16_host, float depth_factor,
-                                const dim_lighting *lighting, void *stream);
-
-/* Per-iteration status of the LAST dim_refine / dim_refine_host(_async) / dim_refine_frames(_host(_async)) call on this
- * context, copied device -> host asynchronously on `stream` (the stream that call ran on): [min(n_iter,8), B] int32.
+/* Per-iteration status of the LAST dim_refine / dim_refine_host_async call on this context, copied device -> host
+ * asynchronously on `stream` (the stream that call ran on): [min(n_iter,8), B] int32.
  * 0 = ok; bit 0 = the rendered mask of that iteration was empty (the reference crashes there: np.min of an empty array,
  * zoom_mask.py:55-58; here the fallback zoom factor was used and the instance's pose is meaningless); bit 1 = class index
  * out of range or no mesh uploaded for that class (the reference indexes a python list and raises); bit 2 = image-only
- * network, empty render (see the network variants); bit 3 = dim_refine_frames only: the instance's frame index lies
- * outside [0, F), so it observed frame 0 instead (its pose is meaningless). */
+ * network, empty render (see the network variants); bit 3 = dim_refine with a frame map only: the instance's frame index
+ * lies outside [0, F), so it observed frame 0 instead (its pose is meaningless). */
 DIM_API int32_t dim_refine_status(dim_ctx *ctx, int32_t B, int32_t n_iter, int32_t *status_host, void *stream);
-
-/* Same as dim_refine_host but returns right after enqueueing the copies and kernels on `stream`
- * (no synchronisation): the host output buffers are valid once the stream has been synchronised.
- * Lets a caller overlap the H2D copy of batch k+1 (second context / stream) with the compute of k. */
-DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *image_observed_u8_host,
-                                      const int32_t *cls_idx_host, const double *pose_init_host,
-                                      int32_t B, int32_t n_iter, const float *K9_host, float znear,
-                                      float zfar, const double *pixel_means_rgb_host,
-                                      int32_t precision, double *poses_out_host, float *se3_out_host,
-                                      const uint16_t *depth_observed_u16_host, float depth_factor,
-                                      const dim_lighting *lighting, void *stream);
-
-/* Frame-indexed fused loop: several instances refined against one copy of their observed frame (several objects of one
- * image, or several initial hypotheses of one object).  F frames, B instances; instance b observes frame frame_idx[b].
- * Every other argument has dim_refine's / dim_refine_host(_async)'s meaning, and instance b's results equal those of
- * dim_refine with frame frame_idx[b] as its image_observed[b], bit for bit.  Each frame is uploaded (host entries) and
- * packed once per call, however many instances observe it; 1 <= F <= max_batch.
- *   dim_refine_frames: image_frames f32[F,3,H,W] RGB - mean (device), frame_idx i32[B] (device), depth_frames f32
- *     [F,1,H,W] metres (RGB-D network only).  The indices are not checked on the host: one outside [0, F) makes the
- *     instance observe frame 0 and sets status bit 3 (dim_refine_status) in every iteration; nothing is read outside the
- *     F frames.  The CUDA graph of the chain reads frame_idx at replay: new indices in the same buffer need no re-capture.
- *   dim_refine_frames_host(_async): frames_u8_host u8[F,H,W,3] BGR, frame_idx_host i32[B], depth_frames_u16_host u16
- *     [F,H,W] (RGB-D network only).  Every index is checked before anything is enqueued: one outside [0, F) fails the call
- *     with a message naming the instance.
- * Image-only network: the observed box is computed once per frame; instance b's is the box of its frame. */
-DIM_API int32_t dim_refine_frames(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx,
-                                  const int32_t *cls_idx, const double *pose_init, int32_t B, int32_t n_iter,
-                                  const float *K9_host, float znear, float zfar, const double *pixel_means_rgb_host,
-                                  int32_t precision, const double *pose_override, double *poses, float *se3,
-                                  float *zoom_factor, int32_t *bbox, const float *depth_frames,
-                                  const dim_lighting *lighting, void *stream);
-DIM_API int32_t dim_refine_frames_host_async(dim_ctx *ctx, const uint8_t *frames_u8_host, int32_t F,
-                                             const int32_t *frame_idx_host, const int32_t *cls_idx_host,
-                                             const double *pose_init_host, int32_t B, int32_t n_iter,
-                                             const float *K9_host, float znear, float zfar,
-                                             const double *pixel_means_rgb_host, int32_t precision,
-                                             double *poses_out_host, float *se3_out_host,
-                                             const uint16_t *depth_frames_u16_host, float depth_factor,
-                                             const dim_lighting *lighting, void *stream);
-DIM_API int32_t dim_refine_frames_host(dim_ctx *ctx, const uint8_t *frames_u8_host, int32_t F,
-                                       const int32_t *frame_idx_host, const int32_t *cls_idx_host,
-                                       const double *pose_init_host, int32_t B, int32_t n_iter, const float *K9_host,
-                                       float znear, float zfar, const double *pixel_means_rgb_host, int32_t precision,
-                                       double *poses_out_host, float *se3_out_host,
-                                       const uint16_t *depth_frames_u16_host, float depth_factor,
-                                       const dim_lighting *lighting, void *stream);
-
-/* Frame-indexed fused loop with one camera per frame (a batch across several cameras; the reference's per-pair
- * `<observed>-K.txt`, tester.py:424-427): K_frames [F,9] row-major f32 in place of K9, and instance b is rendered and
- * zoomed with the intrinsics of its frame, K_frames[frame_of(b)] -- the frame whose taps it observes, frame 0 for a device
- * index outside [0, F) (status bit 3).  One K serves both the render and the zoom centre K . t (the reference zooms with
- * the config's K even when the pair has its own).  Instance b's results equal dim_refine_frames' with
- * K9 = K_frames[frame_idx[b]], bit for bit.  Every other argument is dim_refine_frames' / dim_refine_frames_host_async's.
- *   dim_refine_frames_k: K_frames device f32 [F,9], read as given (not checked, like frame_idx).  The CUDA graph of the
- *     chain reads it at replay: new intrinsics in the same buffer need no re-capture; another buffer is another graph.
- *   dim_refine_frames_k_host_async: K_frames_host f32 [F,9].  Every row is checked before anything is enqueued: one that is
- *     not a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]] with fx, fy > 0 fails the call with a message naming the
- *     frame.  The rows are copied into the context (no allocation); the outputs are valid once `stream` is synchronised. */
-DIM_API int32_t dim_refine_frames_k(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx,
-                                    const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B,
-                                    int32_t n_iter, float znear, float zfar, const double *pixel_means_rgb_host,
-                                    int32_t precision, const double *pose_override, double *poses, float *se3,
-                                    float *zoom_factor, int32_t *bbox, const float *depth_frames,
-                                    const dim_lighting *lighting, void *stream);
-DIM_API int32_t dim_refine_frames_k_host_async(dim_ctx *ctx, const uint8_t *frames_u8_host, int32_t F,
-                                               const int32_t *frame_idx_host, const float *K_frames_host,
-                                               const int32_t *cls_idx_host, const double *pose_init_host, int32_t B,
-                                               int32_t n_iter, float znear, float zfar,
-                                               const double *pixel_means_rgb_host, int32_t precision,
-                                               double *poses_out_host, float *se3_out_host,
-                                               const uint16_t *depth_frames_u16_host, float depth_factor,
-                                               const dim_lighting *lighting, void *stream);
 
 /* BGR u8 HWC -> RGB-mean f32 CHW on device (lib/utils/image.py:583-594 transform). */
 DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int32_t B,
@@ -536,7 +488,7 @@ DIM_API int32_t dim_train_forward_backward(
  * (0.25, 0.03, 0.1, 3000, 0.1, 20, means 0, stds 1, CAMERA).  The MakeLoss grad_scale of the point-matching loss is
  * lw_pm / num_3d_sample whatever the number of points passed per call (deepIM_flownet.py:330-336).
  * dim_train_set_config applies to dim_train_forward_backward of this context; trans_means / trans_stds / rot_coord also
- * drive dim_refine / dim_refine_host (RT_transform with T_means / T_stds / rot_coord, tester.py:452-461) and may be set
+ * drive dim_refine / dim_refine_host_async (RT_transform with T_means / T_stds / rot_coord, tester.py:452-461) and may be set
  * without dim_train_create (the other fields are then stored and used once a training state exists). */
 typedef struct dim_train_config {
   float lw_flow, lw_mask, lw_pm;

@@ -599,8 +599,33 @@ static RefineArgs refine_args(int32_t B, int32_t n_iter, const float *K9, float 
   return a;
 }
 
-// dim_refine / dim_refine_frames once the arguments are checked: the F observed frames (and their depths) packed into obs4
-// outside the graph, then the chain; frame_idx nullptr = instance b observes frame b (F == B)
+static int refuse(const char *fn, const char *msg) {
+  set_error("%s: %s", fn, msg);
+  return 2;
+}
+
+// the argument checks both loop entries share; fn names the entry in every message.  host: dim_refine_host_async (its
+// depth argument's name, n_iter <= 8).  A NULL frame_idx means instance b observes frame b, so F must equal B.
+static int refine_check(dim_ctx *ctx, const char *fn, bool host, const void *frames, int32_t F, const int32_t *frame_idx,
+                        const float *K9, const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B,
+                        int32_t n_iter, const double *means, const void *poses, const void *depth,
+                        const dim_lighting *lighting) {
+  if (!(ctx && frames && cls_idx && pose_init && means && poses)) return refuse(fn, "NULL argument");
+  if (!K9 == !K_frames)
+    return refuse(fn, host ? "exactly one of K9_host and K_frames_host must be non-NULL"
+                           : "exactly one of K9_host and K_frames must be non-NULL");
+  if (int rc = depth_check(ctx, depth, depth, fn, host ? "depth_frames_u16_host" : "depth_frames")) return rc;
+  if (int rc = lit_check(ctx, lighting, fn)) return rc;
+  if (B < 1 || B > ctx->max_batch) return refuse(fn, "batch exceeds max_batch");
+  if (F < 1 || F > ctx->max_batch) return refuse(fn, "frame count F outside [1, max_batch]");
+  if (!frame_idx && F != B) return refuse(fn, "frame_idx is NULL (instance b observes frame b): F must equal B");
+  if (host ? (n_iter < 1 || n_iter > 8) : n_iter < 1)
+    return refuse(fn, host ? "n_iter must be in [1,8]" : "n_iter must be >= 1");
+  return 0;
+}
+
+// dim_refine once the arguments are checked: the F observed frames (and their depths) packed into obs4 outside the graph,
+// then the chain
 static int refine_device(dim_ctx *ctx, RefineArgs &a, const float *frames, int32_t F, const int32_t *frame_idx,
                          const float *depth, cudaStream_t st) {
   a.obs4 = ctx->obs4; a.frame_idx = frame_idx; a.n_frames = F;
@@ -613,67 +638,19 @@ static int refine_device(dim_ctx *ctx, RefineArgs &a, const float *frames, int32
   return refine_graphed(ctx, a, st);
 }
 
-DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_observed, const int32_t *cls_idx, const double *pose_init,
-                           int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
-                           int32_t precision, const double *pose_override, double *poses, float *se3, float *zoom_factor,
-                           int32_t *bbox, const float *depth_observed, const dim_lighting *lighting, void *stream) {
-  DIM_REQUIRE(ctx && image_observed && cls_idx && pose_init && K9 && means && poses, "dim_refine: NULL argument");
-  if (int rc = depth_check(ctx, depth_observed, depth_observed, "dim_refine", "depth_observed")) return rc;
-  if (int rc = lit_check(ctx, lighting, "dim_refine")) return rc;
-  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine: batch exceeds max_batch");
-  DIM_REQUIRE(n_iter >= 1, "dim_refine: n_iter must be >= 1");
-  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
-  a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
-  a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
-  return refine_device(ctx, a, image_observed, B, nullptr, depth_observed, (cudaStream_t)stream);
-}
-
-static int refuse(const char *fn, const char *msg) {
-  set_error("%s: %s", fn, msg);
-  return 2;
-}
-
-// dim_refine_frames (K9: one camera) and dim_refine_frames_k (K_frames: device [F,9], one camera per frame; K9 nullptr)
-static int refine_frames_device(dim_ctx *ctx, const char *fn, const float *image_frames, int32_t F, const int32_t *frame_idx,
-                                const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B,
-                                int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
-                                const double *pose_override, double *poses, float *se3, float *zoom_factor, int32_t *bbox,
-                                const float *depth_frames, const dim_lighting *lighting, cudaStream_t st) {
-  if (!(ctx && image_frames && frame_idx && cls_idx && pose_init && (K9 || K_frames) && means && poses))
-    return refuse(fn, "NULL argument");
-  if (int rc = depth_check(ctx, depth_frames, depth_frames, fn, "depth_frames")) return rc;
-  if (int rc = lit_check(ctx, lighting, fn)) return rc;
-  if (B < 1 || B > ctx->max_batch) return refuse(fn, "batch exceeds max_batch");
-  if (F < 1 || F > ctx->max_batch) return refuse(fn, "frame count F outside [1, max_batch]");
-  if (n_iter < 1) return refuse(fn, "n_iter must be >= 1");
+DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx, const float *K9,
+                           const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B, int32_t n_iter,
+                           float zn, float zf, const double *means, int32_t precision, const double *pose_override,
+                           double *poses, float *se3, float *zoom_factor, int32_t *bbox, const float *depth_frames,
+                           const dim_lighting *lighting, void *stream) {
+  if (int rc = refine_check(ctx, "dim_refine", false, image_frames, F, frame_idx, K9, K_frames, cls_idx, pose_init, B, n_iter,
+                            means, poses, depth_frames, lighting))
+    return rc;
   RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
   a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
   a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
   a.K_frames = K_frames;
-  return refine_device(ctx, a, image_frames, F, frame_idx, depth_frames, st);
-}
-
-// frame-indexed dim_refine: F observed frames, instance b observes frame frame_idx[b] (device; checked in the kernels)
-DIM_API int32_t dim_refine_frames(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx,
-                                  const int32_t *cls_idx, const double *pose_init, int32_t B, int32_t n_iter, const float *K9,
-                                  float zn, float zf, const double *means, int32_t precision, const double *pose_override,
-                                  double *poses, float *se3, float *zoom_factor, int32_t *bbox, const float *depth_frames,
-                                  const dim_lighting *lighting, void *stream) {
-  return refine_frames_device(ctx, "dim_refine_frames", image_frames, F, frame_idx, nullptr, cls_idx, pose_init, B, n_iter,
-                              K9, zn, zf, means, precision, pose_override, poses, se3, zoom_factor, bbox, depth_frames,
-                              lighting, (cudaStream_t)stream);
-}
-
-// dim_refine_frames with one camera per frame: K_frames device f32 [F,9], read as given (like frame_idx) and at replay
-DIM_API int32_t dim_refine_frames_k(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx,
-                                    const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B,
-                                    int32_t n_iter, float zn, float zf, const double *means, int32_t precision,
-                                    const double *pose_override, double *poses, float *se3, float *zoom_factor, int32_t *bbox,
-                                    const float *depth_frames, const dim_lighting *lighting, void *stream) {
-  if (!K_frames) return refuse("dim_refine_frames_k", "NULL argument (K_frames)");
-  return refine_frames_device(ctx, "dim_refine_frames_k", image_frames, F, frame_idx, K_frames, cls_idx, pose_init, B, n_iter,
-                              nullptr, zn, zf, means, precision, pose_override, poses, se3, zoom_factor, bbox, depth_frames,
-                              lighting, (cudaStream_t)stream);
+  return refine_device(ctx, a, image_frames, F, frame_idx, depth_frames, (cudaStream_t)stream);
 }
 
 // why the host intrinsics K (row-major 3x3) are not a finite pinhole matrix [[fx, 0, cx], [0, fy, cy], [0, 0, 1]] with
@@ -687,9 +664,9 @@ static const char *pinhole_defect(const float *K) {
   return nullptr;
 }
 
-// the host entries once their scalar arguments are checked: the class and frame indices (and intrinsics) are checked here,
-// before anything is enqueued; fn names the entry point in the messages.  frame_host nullptr = instance b observes frame b
-// (F == B).  K_host: nullptr = K9 for every instance; else host [F,9], one camera per frame (K9 nullptr)
+// dim_refine_host_async once its scalar arguments are checked: the class and frame indices (and intrinsics) are checked
+// here, before anything is enqueued.  frame_host nullptr = instance b observes frame b (F == B).  K_host: nullptr = K9 for
+// every instance; else host [F,9], one camera per frame (K9 nullptr)
 static int refine_host_enqueue(dim_ctx *ctx, const char *fn, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
                                const float *K_host, const int32_t *cls_host, const double *pose_host, int32_t B,
                                int32_t n_iter, const float *K9, float zn, float zf, const double *means, int32_t precision,
@@ -744,93 +721,26 @@ static int refine_host_enqueue(dim_ctx *ctx, const char *fn, const uint8_t *fram
   return 0;
 }
 
-// lighting: the caller's lighting with HOST intensities [n_iter,B,3]; depth_u16: the caller's host depth file values [B,H,W]
-DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host,
-                                      int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
-                                      int32_t precision, double *poses_out, float *se3_out, const uint16_t *depth_u16,
-                                      float depth_factor, const dim_lighting *lighting, void *stream) {
-  DIM_REQUIRE(ctx && img_u8 && cls_host && pose_host && K9 && means && poses_out, "dim_refine_host: NULL argument");
-  if (int rc = depth_check(ctx, depth_u16, depth_u16, "dim_refine_host", "depth_observed_u16_host")) return rc;
-  if (depth_u16)
-    DIM_REQUIRE(depth_factor > 0.f && depth_factor < 3.0e38f, "dim_refine_host: depth_factor must be positive and finite");
-  if (int rc = lit_check(ctx, lighting, "dim_refine_host")) return rc;
-  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_refine_host: batch exceeds max_batch");
-  DIM_REQUIRE(n_iter >= 1 && n_iter <= 8, "dim_refine_host: n_iter must be in [1,8]");
-  return refine_host_enqueue(ctx, "dim_refine_host", img_u8, B, nullptr, nullptr, cls_host, pose_host, B, n_iter, K9, zn, zf,
-                             means, precision, poses_out, se3_out, depth_u16, depth_factor, lighting, (cudaStream_t)stream);
-}
-
-// dim_refine_frames_host(_async) (K9: one camera) and dim_refine_frames_k_host_async (K_host: host [F,9], one camera per
-// frame; K9 nullptr): the scalar checks, then refine_host_enqueue
-static int refine_frames_host(dim_ctx *ctx, const char *fn, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
-                              const float *K_host, const int32_t *cls_host, const double *pose_host, int32_t B, int32_t n_iter,
-                              const float *K9, float zn, float zf, const double *means, int32_t precision, double *poses_out,
-                              float *se3_out, const uint16_t *depth_u16, float depth_factor, const dim_lighting *lighting,
-                              cudaStream_t st) {
-  if (!(ctx && frames_u8 && frame_host && cls_host && pose_host && (K9 || K_host) && means && poses_out))
-    return refuse(fn, "NULL argument");
-  if (int rc = depth_check(ctx, depth_u16, depth_u16, fn, "depth_frames_u16_host")) return rc;
+// lighting: the caller's lighting with HOST intensities [n_iter,B,3]; depth_u16: the caller's host depth file values [F,H,W]
+DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
+                                      const float *K9, const float *K_host, const int32_t *cls_host, const double *pose_host,
+                                      int32_t B, int32_t n_iter, float zn, float zf, const double *means, int32_t precision,
+                                      double *poses_out, float *se3_out, const uint16_t *depth_u16, float depth_factor,
+                                      const dim_lighting *lighting, void *stream) {
+  const char *fn = "dim_refine_host_async";
+  if (int rc = refine_check(ctx, fn, true, frames_u8, F, frame_host, K9, K_host, cls_host, pose_host, B, n_iter, means,
+                            poses_out, depth_u16, lighting))
+    return rc;
   if (depth_u16 && !(depth_factor > 0.f && depth_factor < 3.0e38f)) return refuse(fn, "depth_factor must be positive and finite");
-  if (int rc = lit_check(ctx, lighting, fn)) return rc;
-  if (B < 1 || B > ctx->max_batch) return refuse(fn, "batch exceeds max_batch");
-  if (F < 1 || F > ctx->max_batch) return refuse(fn, "frame count F outside [1, max_batch]");
-  if (n_iter < 1 || n_iter > 8) return refuse(fn, "n_iter must be in [1,8]");
   return refine_host_enqueue(ctx, fn, frames_u8, F, frame_host, K_host, cls_host, pose_host, B, n_iter, K9, zn, zf, means,
-                             precision, poses_out, se3_out, depth_u16, depth_factor, lighting, st);
+                             precision, poses_out, se3_out, depth_u16, depth_factor, lighting, (cudaStream_t)stream);
 }
 
-// frame-indexed dim_refine_host_async: F host frames [F,H,W,3] (depth [F,H,W]), frame_host [B] checked before any enqueue
-DIM_API int32_t dim_refine_frames_host_async(dim_ctx *ctx, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
-                                             const int32_t *cls_host, const double *pose_host, int32_t B, int32_t n_iter,
-                                             const float *K9, float zn, float zf, const double *means, int32_t precision,
-                                             double *poses_out, float *se3_out, const uint16_t *depth_u16, float depth_factor,
-                                             const dim_lighting *lighting, void *stream) {
-  return refine_frames_host(ctx, "dim_refine_frames_host", frames_u8, F, frame_host, nullptr, cls_host, pose_host, B, n_iter,
-                            K9, zn, zf, means, precision, poses_out, se3_out, depth_u16, depth_factor, lighting,
-                            (cudaStream_t)stream);
-}
-
-// dim_refine_frames_host_async with one camera per frame: K_host [F,9], every row checked before any enqueue
-DIM_API int32_t dim_refine_frames_k_host_async(dim_ctx *ctx, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
-                                               const float *K_host, const int32_t *cls_host, const double *pose_host,
-                                               int32_t B, int32_t n_iter, float zn, float zf, const double *means,
-                                               int32_t precision, double *poses_out, float *se3_out,
-                                               const uint16_t *depth_u16, float depth_factor, const dim_lighting *lighting,
-                                               void *stream) {
-  if (!K_host) return refuse("dim_refine_frames_k_host", "NULL argument (K_frames_host)");
-  return refine_frames_host(ctx, "dim_refine_frames_k_host", frames_u8, F, frame_host, K_host, cls_host, pose_host, B, n_iter,
-                            nullptr, zn, zf, means, precision, poses_out, se3_out, depth_u16, depth_factor, lighting,
-                            (cudaStream_t)stream);
-}
-
-DIM_API int32_t dim_refine_frames_host(dim_ctx *ctx, const uint8_t *frames_u8, int32_t F, const int32_t *frame_host,
-                                       const int32_t *cls_host, const double *pose_host, int32_t B, int32_t n_iter,
-                                       const float *K9, float zn, float zf, const double *means, int32_t precision,
-                                       double *poses_out, float *se3_out, const uint16_t *depth_u16, float depth_factor,
-                                       const dim_lighting *lighting, void *stream) {
-  if (int rc = dim_refine_frames_host_async(ctx, frames_u8, F, frame_host, cls_host, pose_host, B, n_iter, K9, zn, zf, means,
-                                            precision, poses_out, se3_out, depth_u16, depth_factor, lighting, stream))
-    return rc;
-  DIM_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
-  return 0;
-}
-
-DIM_API int32_t dim_refine_host(dim_ctx *ctx, const uint8_t *img_u8, const int32_t *cls_host, const double *pose_host,
-                                int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
-                                int32_t precision, double *poses_out, float *se3_out, const uint16_t *depth_u16,
-                                float depth_factor, const dim_lighting *lighting, void *stream) {
-  if (int rc = dim_refine_host_async(ctx, img_u8, cls_host, pose_host, B, n_iter, K9, zn, zf, means, precision, poses_out,
-                                     se3_out, depth_u16, depth_factor, lighting, stream))
-    return rc;
-  DIM_CHECK(cudaStreamSynchronize((cudaStream_t)stream));
-  return 0;
-}
-
-// status of the LAST dim_refine / dim_refine_host(_async) / dim_refine_frames(_host(_async)) call on this context:
-// [min(n_iter, 8), B] int32, device -> host (asynchronous on `stream`, which must be the stream that call ran on).  0 = ok;
-// bit 0 = the rendered mask of that iteration was empty (object left the frustum: the reference crashes in ZoomMask, np.min
-// of an empty array; here the fallback zoom factor (1,1,0,0) was used and the pose of that instance is meaningless); bit 1 =
-// class index out of range or no mesh uploaded for it; bit 3 = dim_refine_frames: frame index out of range (frame 0 used).
+// status of the LAST dim_refine / dim_refine_host_async call on this context: [min(n_iter, 8), B] int32, device -> host
+// (asynchronous on `stream`, which must be the stream that call ran on).  0 = ok; bit 0 = the rendered mask of that iteration
+// was empty (object left the frustum: the reference crashes in ZoomMask, np.min of an empty array; here the fallback zoom
+// factor (1,1,0,0) was used and the pose of that instance is meaningless); bit 1 = class index out of range or no mesh
+// uploaded for it; bit 3 = dim_refine with a frame map: frame index out of range (frame 0 used).
 DIM_API int32_t dim_refine_status(dim_ctx *ctx, int32_t B, int32_t n_iter, int32_t *status_host, void *stream) {
   DIM_REQUIRE(ctx && status_host && B >= 1 && B <= ctx->max_batch && n_iter >= 1, "dim_refine_status: bad argument");
   const int n = n_iter < 8 ? n_iter : 8;

@@ -76,9 +76,9 @@ struct MeshDev {
 
 struct NetState;  // net_state.cuh
 
-// The observed frame of instance b in the fused loop (dim_refine_frames): frame_idx[b], or frame 0 when that lies outside
+// The observed frame of instance b in the fused loop (dim_refine's frame map): frame_idx[b], or frame 0 when that lies outside
 // [0, n_frames) -- a bad index never reads outside the packed frames (or the per-frame intrinsics); the zoom factor flags it
-// as status bit 3.  frame_idx == nullptr: instance b observes frame b (dim_refine).
+// as status bit 3.  frame_idx == nullptr: instance b observes frame b (no frame map).
 __device__ __forceinline__ int frame_of(const int32_t *frame_idx, int n_frames, int b) {
   if (!frame_idx) return b;
   const int f = __ldg(frame_idx + b);
@@ -95,9 +95,9 @@ __device__ __forceinline__ bool frame_bad(const int32_t *frame_idx, int n_frames
 // rot_coord), mesh uploads, network weights and the "graph" option.
 struct RefineArgs {
   const float4 *obs4;        // n_frames observed frames
-  const int32_t *frame_idx;  // device [B]: the frame instance b observes (read at replay); nullptr = frame b (dim_refine)
+  const int32_t *frame_idx;  // device [B]: the frame instance b observes (read at replay); nullptr = frame b (no frame map)
   const float *K_frames;     // device [n_frames,9]: the camera of every frame (read at replay; K9 is then all zero);
-                             // nullptr = K9 for every instance (dim_refine, dim_refine_frames)
+                             // nullptr = K9 for every instance
   const int32_t *cls_idx;
   const double *pose_init, *pose_override;  // pose_override: nullable [n_iter,B,3,4] source pose of every iteration
   double *poses;
@@ -142,13 +142,13 @@ struct dim_ctx {
   float4 *ren4 = nullptr, *obs4 = nullptr;  // [max_batch,H,W] pixel-interleaved images of the fused loop
   uint8_t *image_observed_u8 = nullptr;
   int *cls_dev = nullptr;
-  int *frame_dev = nullptr;     // [max_batch] dim_refine_frames_host: the caller's frame index of every instance
-  float *K_dev = nullptr;       // [max_batch,9] dim_refine_frames_k_host: the caller's intrinsics of every frame
+  int *frame_dev = nullptr;     // [max_batch] dim_refine_host_async: the caller's frame index of every instance
+  float *K_dev = nullptr;       // [max_batch,9] dim_refine_host_async: the caller's intrinsics of every frame
   double *poses_dev = nullptr;  // [8, max_batch, 12]
   float *se3_hist_dev = nullptr;
   float *light_pos = nullptr;      // [max_batch,3] lit chain / lit train update: light of the pose being rendered
-  float *lit_intensity = nullptr;  // [8, max_batch, 3] lit dim_refine_host: the caller's light intensities on the device
-  uint16_t *depth_u16 = nullptr;   // [max_batch,H,W] RGB-D dim_refine_host: the caller's depth file values
+  float *lit_intensity = nullptr;  // [8, max_batch, 3] lit dim_refine_host_async: the caller's light intensities on the device
+  uint16_t *depth_u16 = nullptr;   // [max_batch,H,W] RGB-D dim_refine_host_async: the caller's depth file values
   int *bbox_obs = nullptr;         // [max_batch,4] image-only network: the observed image's colour-valid box (ZoomImage)
   // background bank of dim_replace_background (dim_bg_upload): BGR u8 photos, each allocated at its upload
   struct BgImage { uint8_t *data = nullptr; int h = 0, w = 0; };

@@ -529,7 +529,7 @@ int transform_u8_launch(dim_ctx *ctx, const uint8_t *bgr, int B, const double *m
   return 0;
 }
 
-// u8 BGR HWC -> pixel-interleaved float4 (RGB - mean) + mean (w = 0): dim_refine_host's input transform (float64 subtraction
+// u8 BGR HWC -> pixel-interleaved float4 (RGB - mean) + mean (w = 0): dim_refine_host_async's input transform (float64 subtraction
 // cast to float32, lib/utils/image.py:583-594) followed by the zoom sampler's float32 "+ mean" (zoom_image_with_factor.py:44)
 __global__ void __launch_bounds__(256) transform_u8_obs4_kernel(const uint8_t *bgr, int P, double m0, double m1,
                                                                 double m2, float4 *out) {

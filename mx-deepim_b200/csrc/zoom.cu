@@ -290,7 +290,7 @@ int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *
 // Image-only network (ZoomImage, zoom_image.py:33-37): the observed box of the fused loop, valid = sum_c(image + mean) > 0.01
 // over obs4's colours (which hold image + mean), the float32 sum of mask_bbox_kernel's img_mode in the same channel order.
 // Once per dim_refine call: the observed image does not change over the iterations.  One block per (row, frame): with
-// dim_refine_frames each frame's box is reduced once, however many instances observe it.
+// a frame map each frame's box is reduced once, however many instances observe it.
 __global__ void __launch_bounds__(160) obs_colour_box_kernel(const float4 *obs4, int H, int W, int *bbox_obs) {
   const int i = blockIdx.x, b = blockIdx.y;
   const float4 *src = obs4 + ((size_t)b * H + i) * W;
@@ -525,7 +525,7 @@ __device__ __forceinline__ void zoom_fused_pixel(const FusedZoomParams &p, const
 // slots are rewritten with zeros.  Sources are the pixel-interleaved float4 images, so each tap is one 16-byte load
 // per image; the column taps of the quad's two columns and the row taps of its two rows are computed once each.
 // DEPTH: the RGB-D network's input, two chunk planes per quad slot: [B*Hs rows][8 planes = (slot, half)][Ws cols][8 ch]
-// Instance b's observed taps come from frame frame_of(b) of obs4 (dim_refine_frames), its rendered taps from ren4[b].
+// Instance b's observed taps come from frame frame_of(b) of obs4 (dim_refine's frame map), its rendered taps from ren4[b].
 template <bool LO, bool F16, bool DEPTH = false, bool MASK = true>
 __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParams p) {
   const int b = blockIdx.y;

@@ -62,18 +62,9 @@ SIGNATURES = {
                                vp, vp, vp, plit, vp]),
     "dim_net_load": (i32, [vp, C.POINTER(vp), C.POINTER(vp)]),
     "dim_net_fwd": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, vp]),
-    "dim_refine": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, vp, plit, vp]),
-    "dim_refine_host": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32, plit, vp]),
-    "dim_refine_host_async": (i32, [vp, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32, plit, vp]),
-    "dim_refine_frames": (i32, [vp, vp, i32, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, vp, plit,
-                                vp]),
-    "dim_refine_frames_host": (i32, [vp, vp, i32, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32, plit, vp]),
-    "dim_refine_frames_host_async": (i32, [vp, vp, i32, vp, vp, vp, i32, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, f32, plit,
-                                           vp]),
-    "dim_refine_frames_k": (i32, [vp, vp, i32, vp, vp, vp, vp, i32, i32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, vp, plit,
-                                  vp]),
-    "dim_refine_frames_k_host_async": (i32, [vp, vp, i32, vp, vp, vp, vp, i32, i32, f32, f32, pf64, i32, vp, vp, vp, f32,
-                                             plit, vp]),
+    "dim_refine": (i32, [vp, vp, i32, vp, pf32, vp, vp, vp, i32, i32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, vp, plit, vp]),
+    "dim_refine_host_async": (i32, [vp, vp, i32, vp, pf32, vp, vp, vp, i32, i32, f32, f32, pf64, i32, vp, vp, vp, f32, plit,
+                                    vp]),
     "dim_ctx_set_input_depth": (i32, [vp, i32]),
     "dim_ctx_set_input_mask": (i32, [vp, i32]),
     "dim_transform_image_u8": (i32, [vp, vp, i32, pf64, vp, vp]),

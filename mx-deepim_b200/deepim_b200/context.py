@@ -36,6 +36,20 @@ def _chk(t, dtype, shape=None, name="tensor"):
     return t
 
 
+def hptr(a):
+    """host pointer of a numpy array or a CPU torch tensor"""
+    return C.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else C.c_void_p(a.ctypes.data)
+
+
+def _host(a, dtype, tdtype, name):
+    """a as a contiguous host array of dtype (a CPU torch tensor must already have it)"""
+    if isinstance(a, torch.Tensor):
+        if a.is_cuda or a.dtype != tdtype:
+            raise ValueError("%s must be a host %s array" % (name, np.dtype(dtype).name))
+        return a.contiguous()
+    return np.ascontiguousarray(a, dtype)
+
+
 def _lighting_arg(lighting, shape, on_device):
     """dim_lighting for a lighting dict (see deepim_b200.lighting): intensity float32 `shape`, a contiguous CUDA tensor when
     on_device, else a host array (numpy or CPU torch tensor).  Returns (struct, host array to keep alive)."""
@@ -466,31 +480,9 @@ class Context:
         = the ModelNet branch's lit loop (see deepim_b200.lighting).  Reusing the same intensity tensor lets the lit chain
         replay its graph as well.
         depth_observed: f32 [B,1,H,W] CUDA, metres -- required on an RGB-D context (input_depth=True), refused otherwise."""
-        B = image_observed.shape[0]
-        _chk(image_observed, torch.float32, (B, 3, self.H, self.W), "image_observed")
-        _chk(cls_idx, torch.int32, (B,), "cls_idx")
-        _chk(pose_init, torch.float64, (B, 3, 4), "pose_init")
-        if out is not None:
-            poses, se3, zf, bbox = out["poses"], out["se3"], out["zoom_factor"], out["bbox"]
-            _chk(poses, torch.float64, (n_iter, B, 3, 4), "out['poses']")
-            _chk(se3, torch.float32, (n_iter, B, 7), "out['se3']")
-            _chk(zf, torch.float32, (n_iter, B, 4), "out['zoom_factor']")
-            _chk(bbox, torch.int32, (n_iter, B, 8), "out['bbox']")
-        else:
-            poses = self._new((n_iter, B, 3, 4), torch.float64)
-            se3 = self._new((n_iter, B, 7))
-            zf = self._new((n_iter, B, 4))
-            bbox = self._new((n_iter, B, 8), torch.int32)
-        if pose_override is not None:
-            _chk(pose_override, torch.float64, (n_iter, B, 3, 4), "pose_override")
-        if depth_observed is not None:
-            _chk(depth_observed, torch.float32, (B, 1, self.H, self.W), "depth_observed")
-        lit = None if lighting is None else C.byref(_lighting_arg(lighting, (n_iter, B, 3), True)[0])
-        check(lib.dim_refine(self._h, _p(image_observed), _p(cls_idx), _p(pose_init), B, n_iter,
-                             farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
-                             farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses), _p(se3), _p(zf),
-                             _p(bbox), _p(depth_observed), lit, self._stream()))
-        return {"poses": poses, "se3": se3, "zoom_factor": zf, "bbox": bbox}
+        return self._refine(image_observed, None, cls_idx, pose_init, np.asarray(K, np.float32).reshape(3, 3), n_iter, znear,
+                            zfar, pixel_means_rgb, precision, pose_override, out, lighting, depth_observed,
+                            ("image_observed", "depth_observed"))
 
     def refine_host(self, image_observed_u8, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
                     pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, poses_out=None,
@@ -503,30 +495,9 @@ class Context:
         depth_observed_u16: RGB-D context only, host uint16 [B,H,W] depth file values (the *-depth.png of the observed
         frame); the device converts them as the reference's loader does, float32(u16) / float32(depth_factor).  With
         sync=False a pinned depth array is copied asynchronously too: keep it untouched until the stream is synchronised."""
-        def hptr(a):
-            return C.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else C.c_void_p(a.ctypes.data)
-        B = image_observed_u8.shape[0]
-        if poses_out is None:
-            poses_out = np.empty((n_iter, B, 3, 4), np.float64)
-        if se3_out is None:
-            se3_out = np.empty((n_iter, B, 7), np.float32)
-        dkeep = None
-        if depth_observed_u16 is not None:
-            if isinstance(depth_observed_u16, torch.Tensor):
-                if depth_observed_u16.is_cuda or depth_observed_u16.dtype != torch.uint16:
-                    raise ValueError("depth_observed_u16 must be a host uint16 array")
-                dkeep = depth_observed_u16.contiguous()
-            else:
-                dkeep = np.ascontiguousarray(depth_observed_u16, np.uint16)
-            if tuple(dkeep.shape) != (B, self.H, self.W):
-                raise ValueError("depth_observed_u16: expected shape %s, got %s" % ((B, self.H, self.W), tuple(dkeep.shape)))
-        lit, _keep = (None, None) if lighting is None else _lighting_arg(lighting, (n_iter, B, 3), False)
-        fn = lib.dim_refine_host if sync else lib.dim_refine_host_async
-        check(fn(self._h, hptr(image_observed_u8), hptr(cls_idx), hptr(pose_init), B, n_iter,
-                 farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision,
-                 hptr(poses_out), hptr(se3_out), None if dkeep is None else hptr(dkeep), float(np.float32(depth_factor)),
-                 None if lit is None else C.byref(lit), self._stream()))
-        return poses_out, se3_out
+        return self._refine_host(image_observed_u8, None, cls_idx, pose_init, np.asarray(K, np.float32).reshape(3, 3), n_iter,
+                                 znear, zfar, pixel_means_rgb, precision, poses_out, se3_out, sync, lighting,
+                                 depth_observed_u16, depth_factor, ("image_observed_u8", "depth_observed_u16"))
 
     def refine_frames(self, frames, frame_idx, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
                       pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, pose_override=None, out=None,
@@ -536,13 +507,36 @@ class Context:
         for bit; each frame is packed once.  An index outside [0, F) is not an error here: that instance observes frame 0
         and refine_status() reports bit 3.  Writing new indices into the same frame_idx tensor replays the captured graph.
         depth_frames: f32 [F,1,H,W] CUDA, metres -- required on an RGB-D context, refused otherwise.
-        K: [3,3], one camera for every instance, or [F,3,3], one camera per frame (dim_refine_frames_k): instance b is rendered
-        and zoomed with K[frame_idx[b]], and its results equal refine_frames(..., K=K[frame_idx[b]]) bit for bit.  A float32
-        CUDA tensor [F,3,3] is read in place, also at graph replay: new intrinsics written into it need no re-capture; any
-        other [F,3,3] array is copied to the device first.  Every other argument as refine()."""
-        F, B = frames.shape[0], cls_idx.shape[0]
-        _chk(frames, torch.float32, (F, 3, self.H, self.W), "frames")
-        _chk(frame_idx, torch.int32, (B,), "frame_idx")
+        K: [3,3], one camera for every instance, or [F,3,3], one camera per frame: instance b is rendered and zoomed with
+        K[frame_idx[b]], and its results equal refine_frames(..., K=K[frame_idx[b]]) bit for bit.  A float32 CUDA tensor
+        [F,3,3] is read in place, also at graph replay: new intrinsics written into it need no re-capture; any other [F,3,3]
+        array is copied to the device first.  Every other argument as refine()."""
+        return self._refine(frames, frame_idx, cls_idx, pose_init, K, n_iter, znear, zfar, pixel_means_rgb, precision,
+                            pose_override, out, lighting, depth_frames, ("frames", "depth_frames"))
+
+    def refine_frames_host(self, frames_u8, frame_idx, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
+                           pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, poses_out=None,
+                           se3_out=None, sync=True, lighting=None, depth_frames_u16=None, depth_factor=1000.0):
+        """refine_host() against F shared observed frames: frames_u8 uint8 [F,H,W,3] BGR, frame_idx int32 [B] (host; every
+        index is checked: one outside [0, F) raises before anything is enqueued), depth_frames_u16 uint16 [F,H,W] on an
+        RGB-D context.  Each frame is uploaded once.
+        K: [3,3], or [F,3,3] host float32, one camera per frame (see refine_frames): every row must be a finite pinhole
+        matrix [[fx,0,cx],[0,fy,cy],[0,0,1]] with fx, fy > 0, else the call raises naming the frame before anything is
+        enqueued.  With sync=False a pinned K is copied asynchronously: keep it untouched until the stream is synchronised.
+        Every other argument as refine_host()."""
+        return self._refine_host(frames_u8, frame_idx, cls_idx, pose_init, K, n_iter, znear, zfar, pixel_means_rgb,
+                                 precision, poses_out, se3_out, sync, lighting, depth_frames_u16, depth_factor,
+                                 ("frames_u8", "depth_frames_u16"))
+
+    def _refine(self, frames, frame_idx, cls_idx, pose_init, K, n_iter, znear, zfar, pixel_means_rgb, precision,
+                pose_override, out, lighting, depth, names):
+        """refine / refine_frames: one dim_refine call.  frame_idx None = instance b observes frames[b]; K [3,3] or [F,3,3]
+        (_per_frame_k); names = the caller's names of the frames and depth arguments, for the messages."""
+        F = frames.shape[0]
+        B = F if frame_idx is None else cls_idx.shape[0]
+        _chk(frames, torch.float32, (F, 3, self.H, self.W), names[0])
+        if frame_idx is not None:
+            _chk(frame_idx, torch.int32, (B,), "frame_idx")
         _chk(cls_idx, torch.int32, (B,), "cls_idx")
         _chk(pose_init, torch.float64, (B, 3, 4), "pose_init")
         if out is not None:
@@ -558,76 +552,59 @@ class Context:
             bbox = self._new((n_iter, B, 8), torch.int32)
         if pose_override is not None:
             _chk(pose_override, torch.float64, (n_iter, B, 3, 4), "pose_override")
-        if depth_frames is not None:
-            _chk(depth_frames, torch.float32, (F, 1, self.H, self.W), "depth_frames")
+        if depth is not None:
+            _chk(depth, torch.float32, (F, 1, self.H, self.W), names[1])
         lit = None if lighting is None else C.byref(_lighting_arg(lighting, (n_iter, B, 3), True)[0])
+        K9 = K_frames = None
         if _per_frame_k(K, F):
+            K_frames = K
             if not (isinstance(K, torch.Tensor) and K.device == self.device and K.dtype == torch.float32 and K.is_contiguous()):
-                K = torch.as_tensor(np.ascontiguousarray(K if not isinstance(K, torch.Tensor) else K.cpu(), np.float32),
-                                    device=self.device)
-            check(lib.dim_refine_frames_k(self._h, _p(frames), F, _p(frame_idx), _p(K), _p(cls_idx), _p(pose_init), B, n_iter,
-                                          znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override),
-                                          _p(poses), _p(se3), _p(zf), _p(bbox), _p(depth_frames), lit, self._stream()))
+                K_frames = torch.as_tensor(np.ascontiguousarray(K if not isinstance(K, torch.Tensor) else K.cpu(), np.float32),
+                                           device=self.device)
         else:
-            check(lib.dim_refine_frames(self._h, _p(frames), F, _p(frame_idx), _p(cls_idx), _p(pose_init), B, n_iter,
-                                        farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar,
-                                        farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses), _p(se3),
-                                        _p(zf), _p(bbox), _p(depth_frames), lit, self._stream()))
+            K9 = farr(np.asarray(K, np.float32).reshape(9), 9)
+        check(lib.dim_refine(self._h, _p(frames), F, _p(frame_idx), K9, _p(K_frames), _p(cls_idx), _p(pose_init), B, n_iter,
+                             znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses),
+                             _p(se3), _p(zf), _p(bbox), _p(depth), lit, self._stream()))
         return {"poses": poses, "se3": se3, "zoom_factor": zf, "bbox": bbox}
 
-    def refine_frames_host(self, frames_u8, frame_idx, cls_idx, pose_init, K, n_iter=4, znear=0.25, zfar=6.0,
-                           pixel_means_rgb=(103.939, 116.779, 123.68), precision=capi.PREC_FP16, poses_out=None,
-                           se3_out=None, sync=True, lighting=None, depth_frames_u16=None, depth_factor=1000.0):
-        """refine_host() against F shared observed frames: frames_u8 uint8 [F,H,W,3] BGR, frame_idx int32 [B] (host; every
-        index is checked: one outside [0, F) raises before anything is enqueued), depth_frames_u16 uint16 [F,H,W] on an
-        RGB-D context.  Each frame is uploaded once.
-        K: [3,3], or [F,3,3] host float32, one camera per frame (dim_refine_frames_k_host_async; see refine_frames): every
-        row must be a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]] with fx, fy > 0, else the call raises naming the
-        frame before anything is enqueued.  With sync=False a pinned K is copied asynchronously: keep it untouched until the
-        stream is synchronised.  Every other argument as refine_host()."""
-        def hptr(a):
-            return C.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else C.c_void_p(a.ctypes.data)
-
-        def host(a, dtype, tdtype, name):
-            if isinstance(a, torch.Tensor):
-                if a.is_cuda or a.dtype != tdtype:
-                    raise ValueError("%s must be a host %s array" % (name, np.dtype(dtype).name))
-                return a.contiguous()
-            return np.ascontiguousarray(a, dtype)
+    def _refine_host(self, frames_u8, frame_idx, cls_idx, pose_init, K, n_iter, znear, zfar, pixel_means_rgb, precision,
+                     poses_out, se3_out, sync, lighting, depth_u16, depth_factor, names):
+        """refine_host / refine_frames_host / PoseRefiner: one dim_refine_host_async call, then (sync) a synchronise of the
+        stream.  frame_idx None = instance b observes frames_u8[b]; K [3,3] or [F,3,3] (_per_frame_k); names = the caller's
+        names of the frames and depth arguments, for the messages."""
         F = frames_u8.shape[0]
-        fidx = host(frame_idx, np.int32, torch.int32, "frame_idx")
-        cls = host(cls_idx, np.int32, torch.int32, "cls_idx")
-        pose = host(pose_init, np.float64, torch.float64, "pose_init")
-        B = cls.shape[0]
-        if tuple(fidx.shape) != (B,):
+        fidx = None if frame_idx is None else _host(frame_idx, np.int32, torch.int32, "frame_idx")
+        cls = _host(cls_idx, np.int32, torch.int32, "cls_idx")
+        pose = _host(pose_init, np.float64, torch.float64, "pose_init")
+        B = F if fidx is None else cls.shape[0]
+        if fidx is not None and tuple(fidx.shape) != (B,):
             raise ValueError("frame_idx: expected shape %s, got %s" % ((B,), tuple(fidx.shape)))
         if tuple(frames_u8.shape) != (F, self.H, self.W, 3):
-            raise ValueError("frames_u8: expected shape %s, got %s" % ((F, self.H, self.W, 3), tuple(frames_u8.shape)))
+            raise ValueError("%s: expected shape %s, got %s" % (names[0], (F, self.H, self.W, 3), tuple(frames_u8.shape)))
         if poses_out is None:
             poses_out = np.empty((n_iter, B, 3, 4), np.float64)
         if se3_out is None:
             se3_out = np.empty((n_iter, B, 7), np.float32)
         dkeep = None
-        if depth_frames_u16 is not None:
-            dkeep = host(depth_frames_u16, np.uint16, torch.uint16, "depth_frames_u16")
+        if depth_u16 is not None:
+            dkeep = _host(depth_u16, np.uint16, torch.uint16, names[1])
             if tuple(dkeep.shape) != (F, self.H, self.W):
-                raise ValueError("depth_frames_u16: expected shape %s, got %s" % ((F, self.H, self.W), tuple(dkeep.shape)))
+                raise ValueError("%s: expected shape %s, got %s" % (names[1], (F, self.H, self.W), tuple(dkeep.shape)))
         frames = frames_u8 if isinstance(frames_u8, torch.Tensor) else np.ascontiguousarray(frames_u8, np.uint8)
         lit, _keep = (None, None) if lighting is None else _lighting_arg(lighting, (n_iter, B, 3), False)
-        tail = (hptr(poses_out), hptr(se3_out), None if dkeep is None else hptr(dkeep), float(np.float32(depth_factor)),
-                None if lit is None else C.byref(lit), self._stream())
+        K9 = K_frames = None
         if _per_frame_k(K, F):
-            kf = host(K, np.float32, torch.float32, "K")
-            check(lib.dim_refine_frames_k_host_async(self._h, hptr(frames), F, hptr(fidx), hptr(kf), hptr(cls), hptr(pose), B,
-                                                     n_iter, znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision,
-                                                     *tail))
-            if sync:
-                torch.cuda.current_stream(self.device).synchronize()
-            return poses_out, se3_out
-        fn = lib.dim_refine_frames_host if sync else lib.dim_refine_frames_host_async
-        check(fn(self._h, hptr(frames), F, hptr(fidx), hptr(cls), hptr(pose), B, n_iter,
-                 farr(np.asarray(K, np.float32).reshape(9), 9), znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision,
-                 *tail))
+            K_frames = _host(K, np.float32, torch.float32, "K")
+        else:
+            K9 = farr(np.asarray(K, np.float32).reshape(9), 9)
+        check(lib.dim_refine_host_async(self._h, hptr(frames), F, None if fidx is None else hptr(fidx), K9,
+                                        None if K_frames is None else hptr(K_frames), hptr(cls), hptr(pose), B, n_iter, znear,
+                                        zfar, farr(pixel_means_rgb, 3, C.c_double), precision, hptr(poses_out),
+                                        hptr(se3_out), None if dkeep is None else hptr(dkeep), float(np.float32(depth_factor)),
+                                        None if lit is None else C.byref(lit), self._stream()))
+        if sync:
+            torch.cuda.current_stream(self.device).synchronize()
         return poses_out, se3_out
 
 

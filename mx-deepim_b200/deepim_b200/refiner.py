@@ -18,12 +18,12 @@ input_mask=False runs the image-only network (config.network.INPUT_MASK: False; 
 loop zooms with ZoomImage, boxes from the images' colours.
 
 refine_frames / submit_frames refine instances that share observed frames (several objects in one image, several initial
-hypotheses of one object) against one uploaded copy of each frame (dim_refine_frames_host).
+hypotheses of one object) against one uploaded copy of each frame (dim_refine_host_async with a frame map).
 
 Several cameras in one batch: refine_frames(..., K_frames=[F,3,3]) / submit_frames(..., K_frames=[f,3,3]) give every frame
-its own intrinsics, refine(..., K=[N,3,3]) / submit(..., K=[n,3,3]) every instance (the frame path with an identity map);
-dim_refine_frames_k_host_async renders and zooms each instance with its frame's K.  Without them the refiner's K serves
-every instance."""
+its own intrinsics, refine(..., K=[N,3,3]) / submit(..., K=[n,3,3]) every instance (no frame map: instance i uses row i);
+dim_refine_host_async renders and zooms each instance with its frame's K.  Without them the refiner's K serves every
+instance."""
 from __future__ import annotations
 
 import numpy as np
@@ -113,11 +113,9 @@ class PoseRefiner:
     def submit(self, images_bgr_u8, cls_idx, poses_init, depths_u16=None, K=None):
         """Enqueue one batch (<= max_batch instances, host arrays; pinned torch tensors are used in place).
         depths_u16: uint16 [n,H,W], required with input_depth=True.  K: None = the refiner's K; float32 [n,3,3] = each
-        instance's own camera (submit_frames with an identity map).
+        instance's own camera.
         Returns a ticket for result().  At most len(slots) batches may be in flight."""
-        if K is None:
-            return self._submit(images_bgr_u8, None, cls_idx, poses_init, depths_u16, None)
-        return self._submit(images_bgr_u8, np.arange(len(cls_idx), dtype=np.int32), cls_idx, poses_init, depths_u16, K)
+        return self._submit(images_bgr_u8, None, cls_idx, poses_init, depths_u16, K)
 
     def submit_frames(self, frames_bgr_u8, frame_idx, cls_idx, poses_init, depths_u16=None, K_frames=None):
         """submit() against shared frames: frames_bgr_u8 uint8 [f,H,W,3] (f <= max_batch), frame_idx int [n] (instance i
@@ -148,17 +146,12 @@ class PoseRefiner:
             inten = slot["intensity"].view(-1)[: self.n_iter * n * 3].view(self.n_iter, n, 3)
             inten.copy_(torch.from_numpy(self.light.draw((self.n_iter, n))))
             lit = self.light.lighting(inten)
+        fidx = None if frame_idx is None else self._pinned(slot, "frame", frame_idx, torch.int32)
+        K = self.K if K_frames is None else self._pinned(slot, "K", np.asarray(K_frames, np.float32), torch.float32)
         with torch.cuda.stream(slot["stream"]):
-            if frame_idx is None:
-                slot["ctx"].refine_host(img, cls, pose, self.K, self.n_iter, self.zn, self.zf, self.means, self.precision,
-                                        poses_out=slot["poses"], se3_out=slot["se3"], sync=False, lighting=lit,
-                                        depth_observed_u16=depth, depth_factor=self.depth_factor)
-            else:
-                fidx = self._pinned(slot, "frame", frame_idx, torch.int32)
-                K = self.K if K_frames is None else self._pinned(slot, "K", np.asarray(K_frames, np.float32), torch.float32)
-                slot["ctx"].refine_frames_host(img, fidx, cls, pose, K, self.n_iter, self.zn, self.zf, self.means,
-                                               self.precision, poses_out=slot["poses"], se3_out=slot["se3"], sync=False,
-                                               lighting=lit, depth_frames_u16=depth, depth_factor=self.depth_factor)
+            slot["ctx"]._refine_host(img, fidx, cls, pose, K, self.n_iter, self.zn, self.zf, self.means, self.precision,
+                                     slot["poses"], slot["se3"], False, lit, depth, self.depth_factor,
+                                     ("images_bgr_u8", "depths_u16"))
             slot["ctx"].refine_status(n, self.n_iter, out=slot["status"], sync=False)
         slot["busy"], slot["n"] = True, n
         self._next = (i + 1) % len(self.slots)

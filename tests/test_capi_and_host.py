@@ -15,7 +15,7 @@ def declared_symbols(root):
     return sorted(set(re.findall(r"DIM_API\s+[\w\s\*]+?\b(dim_\w+)\s*\(", txt)))
 
 
-def test_library_exports_every_declared_symbol_at_abi_3(root):
+def test_library_exports_every_declared_symbol_at_abi_4(root):
     so = os.path.join(root, "mx-deepim_b200", "libdeepim_b200.so")
     assert os.path.exists(so), "run python __graft_entry__.py (build) first"
     lib = ctypes.CDLL(so)
@@ -24,7 +24,20 @@ def test_library_exports_every_declared_symbol_at_abi_3(root):
     for s in syms:
         assert hasattr(lib, s), "symbol %s declared in the header but not exported" % s
     lib.dim_abi_version.restype = ctypes.c_int32
-    assert lib.dim_abi_version() == 3
+    assert lib.dim_abi_version() == 4
+
+
+def test_library_exports_no_undeclared_symbol(root):
+    """Every dim_ symbol the library exports is declared in the header: an entry point removed from the header but left
+    in the library would otherwise go unnoticed."""
+    import shutil
+    import subprocess
+    if shutil.which("nm") is None:
+        pytest.skip("nm not on PATH")
+    so = os.path.join(root, "mx-deepim_b200", "libdeepim_b200.so")
+    out = subprocess.run(["nm", "-D", "--defined-only", so], capture_output=True, text=True, check=True).stdout
+    exported = sorted({line.split()[-1] for line in out.splitlines() if line.split() and line.split()[-1].startswith("dim_")})
+    assert exported == declared_symbols(root)
 
 
 def test_library_is_sm90a_native_wgmma_and_tma(root):

@@ -1,5 +1,5 @@
 """GPU: the ModelNet (unseen-object) branch of the test and train loops -- the fused refinement loop and the train-time
-batch update with the Lambert-lit renderer (dim_refine, dim_refine_host, dim_train_update with a dim_lighting) against the
+batch update with the Lambert-lit renderer (dim_refine, dim_refine_host_async, dim_train_update with a dim_lighting) against the
 oracle's lit loops (oracle.refine / oracle.train_update with lighting), against the unlit calls where the light is neutral,
 and through the Python layers (PoseRefiner, trainer)."""
 import numpy as np
@@ -234,9 +234,9 @@ def test_lighting_refuses_missing_normals_and_null_intensity(ctx, case):
     K9 = capi.farr(K.reshape(9), 9)
     means = capi.farr(MEANS, 3, C.c_double)
     null_int = capi.Lighting(None, (C.c_double * 3)(0.0, 0.5, 0.5), 0.7)
-    rc = lib.dim_refine(ctx._h, C.c_void_p(img.data_ptr()), C.c_void_p(cls.data_ptr()), C.c_void_p(ini.data_ptr()), B, N_ITER,
-                        K9, 0.25, 6.0, means, capi.PREC_FP16, None, C.c_void_p(poses.data_ptr()), None, None, None, None,
-                        C.byref(null_int), None)
+    rc = lib.dim_refine(ctx._h, C.c_void_p(img.data_ptr()), B, None, K9, None, C.c_void_p(cls.data_ptr()),
+                        C.c_void_p(ini.data_ptr()), B, N_ITER, 0.25, 6.0, means, capi.PREC_FP16, None, C.c_void_p(poses.data_ptr()),
+                        None, None, None, None, C.byref(null_int), None)
     assert rc != 0 and b"NULL" in lib.dim_last_error()
     with pytest.raises(capi.DeepIMError):
         capi.check(rc)

@@ -355,7 +355,7 @@ def test_smaller_batch_on_the_same_context(ctxs, scene, expected):
 
 
 def test_frames_from_several_cameras(meshes, weights, scene):
-    """one dim_refine_frames_k call: 3 frames from 3 cameras, a non-identity frame map; each instance's expectation is built
+    """one dim_refine call with K_frames: 3 frames from 3 cameras, a non-identity frame map; each instance's expectation is built
     with its frame and its frame's camera"""
     Kf = np.stack([K, K.copy(), K.copy()]).astype(np.float32)
     Kf[1, 0, 0] *= 1.1

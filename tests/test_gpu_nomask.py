@@ -1,5 +1,5 @@
 """GPU: the image-only network (config.network.INPUT_MASK: False) in the fused refinement loop and on the op surface --
-dim_refine(_lit), dim_refine_host and dim_net_fwd of a dim_ctx_set_input_mask(ctx, 0) context against the oracle's
+dim_refine(_lit), dim_refine_host_async and dim_net_fwd of a dim_ctx_set_input_mask(ctx, 0) context against the oracle's
 image-only loop (oracle.refine with input_mask=False), against the 8-channel context with zero mask columns, and the error
 paths of the switch.
 

@@ -1,9 +1,9 @@
-"""GPU: one camera per frame in the frame-indexed fused loop (dim_refine_frames_k, dim_refine_frames_k_host_async,
+"""GPU: one camera per frame in the frame-indexed fused loop (dim_refine / dim_refine_host_async with K_frames,
 Context.refine_frames(K=[F,3,3]), PoseRefiner.refine_frames(K_frames=...) / refine(K=...), lm6d_io's per-pair `-K.txt`).
 
-Instance b is rendered and zoomed with the camera of its frame, so its results must equal dim_refine_frames with
+Instance b is rendered and zoomed with the camera of its frame, so its results must equal dim_refine's with
 K9 = K_frames[frame_idx[b]], bit for bit -- poses, se3, zoom factors, bboxes and status -- for every network and precision.
-dim_refine_frames' own parity with the oracle is covered elsewhere; the teacher-forced oracle check below holds each camera
+dim_refine's own parity with the oracle is covered elsewhere; the teacher-forced oracle check below holds each camera
 to the float restatement directly.
 
 The case: F = 6 frames at 480x640 from three cameras (LINEMOD, YCB-Video camera 1, and an off-centre one; frames 0 / 3 the
@@ -133,7 +133,7 @@ def mixed_vs_per_camera(ctx, c, idx, prec=capi.PREC_FP16, lit=None, depth=False)
     return a, sa
 
 
-# ------------------------------------------------------------------------ 1. mixed batch = per-camera dim_refine_frames
+# ---------------------------------------------------------------------------- 1. mixed batch = per-camera K9 batches
 @pytest.mark.parametrize("prec", [capi.PREC_FP16, capi.PREC_BF16, capi.PREC_BF16X3], ids=["fp16", "bf16", "bf16x3"])
 def test_mask_network_mixed_batch_equals_per_camera_batches(ctx, case, prec):
     a, sa = mixed_vs_per_camera(ctx, case, IDX, prec)
@@ -225,7 +225,7 @@ def test_teacher_forced_against_the_oracle_per_camera(ctx, meshes, case):
 # -------------------------------------------------------------------------------------------------- 4. graph replay
 def test_graph_replay_intrinsics_rewrite_and_interleaving(ctx, case):
     """On a side stream (the legacy default stream cannot be captured): new intrinsics in a captured K buffer take effect at
-    the next replay without a new capture, a second K buffer is a second graph, and dim_refine_frames interleaves."""
+    the next replay without a new capture, a second K buffer is a second graph, and a call with K9 interleaves."""
     s = torch.cuda.Stream(device=DEV)
     s.wait_stream(torch.cuda.current_stream(DEV))
     with torch.cuda.stream(s):
@@ -252,7 +252,7 @@ def graph_replay_body(ctx, case):
     n0 = count()
     kbuf, kbuf2 = dev(KF), dev(KF)
     out = out2 = out1 = None
-    for rep in range(3):  # eager, capture, replay -- two K buffers and dim_refine_frames interleaved
+    for rep in range(3):  # eager, capture, replay -- two K buffers and a K9 call interleaved
         out = ctx.refine_frames(frames, *args, kbuf, N_ITER, pixel_means_rgb=MEANS, out=out)
         same(out, want["a"])
         out2 = ctx.refine_frames(frames, *args, kbuf2, N_ITER, pixel_means_rgb=MEANS, out=out2)
@@ -364,12 +364,27 @@ def test_error_paths(ctx, case):
     means = capi.farr(MEANS, 3, capi.C.c_double)
     poses = torch.full((N_ITER, B, 3, 4), 7.0, dtype=torch.float64, device=DEV)
     p = capi.C.c_void_p
-    rc = capi.lib.dim_refine_frames_k(ctx._h, p(frames.data_ptr()), F, p(fidx.data_ptr()), None, p(cls.data_ptr()),
-                                      p(ini.data_ptr()), B, N_ITER, 0.25, 6.0, means, capi.PREC_FP16, None,
-                                      p(poses.data_ptr()), None, None, None, None, None, ctx._stream())
-    assert rc == 2 and b"NULL argument" in capi.lib.dim_last_error()
+    kf, K9 = dev(KF.astype(np.float32)), capi.farr(KF[0].astype(np.float32).reshape(9), 9)
+    hposes = np.full((N_ITER, B, 3, 4), 7.0)
+    hu8, hidx, hkf, hcls, hini = (np.ascontiguousarray(a) for a in (c["u8"], IDX, KF.astype(np.float32), c["cls"], c["ini"]))
+
+    def dev_call(F_=F, iptr=p(fidx.data_ptr()), k9=None, kptr=p(kf.data_ptr())):
+        return capi.lib.dim_refine(ctx._h, p(frames.data_ptr()), F_, iptr, k9, kptr, p(cls.data_ptr()), p(ini.data_ptr()), B,
+                                   N_ITER, 0.25, 6.0, means, capi.PREC_FP16, None, p(poses.data_ptr()), None, None, None, None,
+                                   None, ctx._stream())
+
+    def host_call(F_=F, iptr=p(hidx.ctypes.data), k9=None, kptr=p(hkf.ctypes.data)):
+        return capi.lib.dim_refine_host_async(ctx._h, p(hu8.ctypes.data), F_, iptr, k9, kptr, p(hcls.ctypes.data),
+                                              p(hini.ctypes.data), B, N_ITER, 0.25, 6.0, means, capi.PREC_FP16,
+                                              p(hposes.ctypes.data), None, None, 1000.0, None, ctx._stream())
+    for call, entry, kptr in ((dev_call, b"dim_refine: ", p(kf.data_ptr())),
+                              (host_call, b"dim_refine_host_async: ", p(hkf.ctypes.data))):
+        for k9, kp in ((None, None), (K9, kptr)):   # neither K, both K
+            assert call(k9=k9, kptr=kp) == 2 and entry + b"exactly one of K9_host and K_frames" in capi.lib.dim_last_error()
+        assert call(iptr=None) == 2 and entry + b"frame_idx is NULL" in capi.lib.dim_last_error()   # F = 6, B = 16
+        assert b"F must equal B" in capi.lib.dim_last_error()
     torch.cuda.synchronize()
-    assert (poses == 7.0).all()
+    assert (poses == 7.0).all() and (hposes == 7.0).all()
 
     def bad(f, r, col, v):
         k = KF.copy()
@@ -381,7 +396,7 @@ def test_error_paths(ctx, case):
                           (bad(5, 2, 2, 2.0), 5, "last row"), (bad(0, 2, 0, 1e-3), 0, "last row")):
         out_p = np.full((N_ITER, B, 3, 4), 7.0)
         out_s = np.full((N_ITER, B, 7), 7.0, np.float32)
-        with pytest.raises(capi.DeepIMError, match=r"dim_refine_frames_k_host: frame %d has intrinsics .*%s" % (frame, why)):
+        with pytest.raises(capi.DeepIMError, match=r"dim_refine_host_async: frame %d has intrinsics .*%s" % (frame, why)):
             ctx.refine_frames_host(c["u8"], IDX, c["cls"], c["ini"], k, N_ITER, pixel_means_rgb=MEANS, poses_out=out_p,
                                    se3_out=out_s)
         torch.cuda.synchronize()
@@ -390,10 +405,10 @@ def test_error_paths(ctx, case):
         ctx.refine_frames(frames, fidx, cls, ini, dev(KF[:-1]), N_ITER, pixel_means_rgb=MEANS)
     with pytest.raises(ValueError, match="one camera per frame"):
         ctx.refine_frames_host(c["u8"], IDX, c["cls"], c["ini"], np.concatenate([KF, KF[:1]]), N_ITER, pixel_means_rgb=MEANS)
-    # the checks of dim_refine_frames_host hold for the per-frame entry too
+    # the frame index checks hold with per-frame intrinsics too
     wrong = IDX.copy()
     wrong[3] = F
-    with pytest.raises(capi.DeepIMError, match="dim_refine_frames_k_host: instance 3 has frame index 6"):
+    with pytest.raises(capi.DeepIMError, match="dim_refine_host_async: instance 3 has frame index 6"):
         ctx.refine_frames_host(c["u8"], wrong, c["cls"], c["ini"], KF, N_ITER, pixel_means_rgb=MEANS)
     with pytest.raises(capi.DeepIMError, match="depth_frames_u16_host"):
         ctx.refine_frames_host(c["u8"], IDX, c["cls"], c["ini"], KF, N_ITER, pixel_means_rgb=MEANS,

@@ -1,7 +1,7 @@
-"""GPU: the frame-indexed fused loop (dim_refine_frames, dim_refine_frames_host(_async), PoseRefiner.refine_frames).
+"""GPU: the frame-indexed fused loop (dim_refine and dim_refine_host_async with a frame map, PoseRefiner.refine_frames).
 
-Instance b of dim_refine_frames(frames, idx) observes frames[idx[b]]; its results must equal dim_refine(frames[idx]) bit for
-bit -- poses, se3, zoom factors, bboxes and status -- for every network and precision.  dim_refine's own parity with the
+Instance b of dim_refine(frames, idx) observes frames[idx[b]]; its results must equal dim_refine(frames[idx]) without a map,
+bit for bit -- poses, se3, zoom factors, bboxes and status -- for every network and precision.  dim_refine's own parity with the
 oracle is covered elsewhere, so the equality carries it over.
 
 The case: F = 3 frames of the C2 mesh composited over noise, B = 16 instances observing them 10 / 5 / 1 (not contiguous; frame
@@ -174,8 +174,8 @@ def test_one_frame_for_every_instance(ctx, meshes):
 
 # -------------------------------------------------------------------------------------------------- 3. graph replay
 def test_graph_replay_index_rewrite_and_interleaving(ctx, case):
-    """On a side stream (the legacy default stream cannot be captured): eager run, capture and replay of dim_refine_frames
-    equal the launch-by-launch run, with two index buffers and dim_refine interleaved on one context; new indices written
+    """On a side stream (the legacy default stream cannot be captured): eager run, capture and replay of dim_refine with a
+    frame map equal the launch-by-launch run, with two index buffers and dim_refine without a map interleaved on one context; new indices written
     into a captured index buffer take effect at the next replay."""
     s = torch.cuda.Stream(device=DEV)
     s.wait_stream(torch.cuda.current_stream(DEV))
@@ -199,7 +199,7 @@ def graph_replay_body(ctx, case):
     capi.check(capi.lib.dim_debug_set_option(ctx._h, b"graph", 1))
     fidx, fidx2, gathered = dev(IDX), dev(IDX), frames[dev(IDX).long()].contiguous()
     out = out2 = outr = None
-    for rep in range(3):  # eager, capture, replay -- interleaved with a second index buffer and with dim_refine
+    for rep in range(3):  # eager, capture, replay -- interleaved with a second index buffer and with no frame map
         out = ctx.refine_frames(frames, fidx, cls, ini, K, N_ITER, pixel_means_rgb=MEANS, out=out)
         assert_same(out, want["a"])
         out2 = ctx.refine_frames(frames, fidx2, cls, ini, K, N_ITER, pixel_means_rgb=MEANS, out=out2)
@@ -259,14 +259,31 @@ def test_error_paths(ctx, meshes, case):
     st = ctx._stream()
     p = capi.C.c_void_p
 
-    def dev_call(F_, fptr=p(frames.data_ptr()), iptr=p(fidx.data_ptr()), depth=None):
-        return capi.lib.dim_refine_frames(h, fptr, F_, iptr, p(cls.data_ptr()), p(ini.data_ptr()), B, N_ITER, K9, 0.25, 6.0,
-                                          means, capi.PREC_FP16, None, p(poses.data_ptr()), None, None, None, depth, None, st)
-    for F_ in (0, B + 1):
-        assert dev_call(F_) == 2 and b"frame count F" in capi.lib.dim_last_error()
+    kf = dev(np.stack([np.asarray(K, np.float32)] * F))
+    hu8, hidx, hcls, hini = (np.ascontiguousarray(a) for a in (c["u8"], IDX, c["cls"], c["ini"]))
+    hposes = np.full((N_ITER, B, 3, 4), 7.0)
+
+    def dev_call(F_, fptr=p(frames.data_ptr()), iptr=p(fidx.data_ptr()), depth=None, k9=K9, kptr=None):
+        return capi.lib.dim_refine(h, fptr, F_, iptr, k9, kptr, p(cls.data_ptr()), p(ini.data_ptr()), B, N_ITER, 0.25, 6.0,
+                                   means, capi.PREC_FP16, None, p(poses.data_ptr()), None, None, None, depth, None, st)
+
+    def host_call(F_, iptr=p(hidx.ctypes.data), k9=K9, kptr=None):
+        return capi.lib.dim_refine_host_async(h, p(hu8.ctypes.data), F_, iptr, k9, kptr, p(hcls.ctypes.data),
+                                              p(hini.ctypes.data), B, N_ITER, 0.25, 6.0, means, capi.PREC_FP16,
+                                              p(hposes.ctypes.data), None, None, 1000.0, None, st)
+    for call, entry in ((dev_call, b"dim_refine: "), (host_call, b"dim_refine_host_async: ")):
+        for F_ in (0, B + 1):
+            assert call(F_) == 2 and entry + b"frame count F" in capi.lib.dim_last_error()
+        # no frame map: instance b observes frame b, so F must equal B
+        assert call(F, iptr=None) == 2 and entry + b"frame_idx is NULL" in capi.lib.dim_last_error()
+        assert b"F must equal B" in capi.lib.dim_last_error()
+        # exactly one of K9 and K_frames
+        for k9, kptr in ((K9, p(kf.data_ptr())), (None, None)):
+            assert call(F, k9=k9, kptr=kptr) == 2 and entry + b"exactly one of K9_host and K_frames" in capi.lib.dim_last_error()
     assert dev_call(F, fptr=None) == 2 and b"NULL argument" in capi.lib.dim_last_error()
-    assert dev_call(F, iptr=None) == 2 and b"NULL argument" in capi.lib.dim_last_error()
     assert dev_call(F, depth=p(frames.data_ptr())) == 2 and b"takes no depth input" in capi.lib.dim_last_error()
+    torch.cuda.synchronize()
+    assert (hposes == 7.0).all()
 
     host = dict(pixel_means_rgb=MEANS)
     bad = IDX.copy()

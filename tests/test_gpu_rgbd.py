@@ -1,5 +1,5 @@
 """GPU: the RGB-D network (config.network.INPUT_DEPTH) in the fused refinement loop and on the op surface -- dim_refine,
-dim_refine_host and dim_net_fwd of an RGB-D context against the oracle's RGB-D loop (oracle.refine with depth_observed), against
+dim_refine_host_async and dim_net_fwd of an RGB-D context against the oracle's RGB-D loop (oracle.refine with depth_observed), against
 the RGB context
 where the depth weights are zero, and the error paths of the mode switch."""
 import ctypes as C
@@ -238,11 +238,11 @@ def test_depth_arguments_follow_the_network_error_paths(meshes, weights, case):
     rgbd = make_ctx(meshes, weights)
     try:
         args = (dev(c["img"][:2]), dev(c["cls"][:2]), dev(c["ini"][:2]), K, 1)
-        with pytest.raises(capi.DeepIMError, match="takes depth input.*depth_observed"):
+        with pytest.raises(capi.DeepIMError, match="takes depth input.*depth_frames must not be NULL"):
             rgbd.refine(*args, pixel_means_rgb=MEANS)
         with pytest.raises(capi.DeepIMError, match="takes no depth input"):
             rgb.refine(*args, pixel_means_rgb=MEANS, depth_observed=dev(c["depth"][:2]))
-        with pytest.raises(capi.DeepIMError, match="takes depth input.*depth_observed_u16_host"):
+        with pytest.raises(capi.DeepIMError, match="takes depth input.*depth_frames_u16_host"):
             rgbd.refine_host(c["u8"][:2], c["cls"][:2], c["ini"][:2], K, 1, pixel_means_rgb=MEANS)
         with pytest.raises(capi.DeepIMError, match="takes no depth input"):
             rgb.refine_host(c["u8"][:2], c["cls"][:2], c["ini"][:2], K, 1, pixel_means_rgb=MEANS,
@@ -255,10 +255,10 @@ def test_depth_arguments_follow_the_network_error_paths(meshes, weights, case):
                             zoom_depth_observed=dev(z["zdo"][:2]), zoom_depth_rendered=dev(z["zdr"][:2]))
         # NULL depth
         poses = torch.empty((1, 2, 3, 4), dtype=torch.float64, device=DEV)
-        rc = capi.lib.dim_refine(rgbd._h, C.c_void_p(args[0].data_ptr()), C.c_void_p(args[1].data_ptr()),
-                                      C.c_void_p(args[2].data_ptr()), 2, 1, capi.farr(np.asarray(K, np.float32).reshape(9), 9),
-                                      0.25, 6.0, capi.farr(MEANS, 3, C.c_double), capi.PREC_FP16, None,
-                                      C.c_void_p(poses.data_ptr()), None, None, None, None, None, None)
+        rc = capi.lib.dim_refine(rgbd._h, C.c_void_p(args[0].data_ptr()), 2, None,
+                                 capi.farr(np.asarray(K, np.float32).reshape(9), 9), None, C.c_void_p(args[1].data_ptr()),
+                                 C.c_void_p(args[2].data_ptr()), 2, 1, 0.25, 6.0, capi.farr(MEANS, 3, C.c_double),
+                                 capi.PREC_FP16, None, C.c_void_p(poses.data_ptr()), None, None, None, None, None, None)
         assert rc != 0 and b"NULL" in capi.lib.dim_last_error()
         # the switch is refused once weights are loaded, and a weight of the other network is refused
         with pytest.raises(capi.DeepIMError, match="before dim_net_load"):

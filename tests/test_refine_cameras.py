@@ -42,9 +42,9 @@ def test_context_per_frame_camera_shapes():
     torch = pytest.importorskip("torch")
     from deepim_b200.context import _per_frame_k
     one = np.eye(3, dtype=np.float32)
-    assert _per_frame_k(one, 4) is False                      # [3,3]: one camera, dim_refine_frames
+    assert _per_frame_k(one, 4) is False                      # [3,3]: one camera, K9
     assert _per_frame_k(one.reshape(9), 4) is False           # nine values, as before
-    assert _per_frame_k(np.stack([one] * 4), 4) is True       # [F,3,3]: dim_refine_frames_k
+    assert _per_frame_k(np.stack([one] * 4), 4) is True       # [F,3,3]: K_frames
     assert _per_frame_k(torch.from_numpy(np.stack([one] * 2)), 2) is True
     for bad in (np.stack([one] * 3), np.zeros((4, 3, 4), np.float32), np.zeros((4, 9, 1), np.float32)):
         with pytest.raises(ValueError, match=r"one camera per frame\), got"):

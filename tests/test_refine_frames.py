@@ -1,33 +1,6 @@
-"""CPU: the frame-indexed refinement entry points are exported with the prototypes the ctypes binding declares, and
-PoseRefiner.refine_frames' batch plan (plan_frame_batches) is right."""
-import ctypes
-import os
-
+"""CPU: PoseRefiner.refine_frames' batch plan (plan_frame_batches) is right."""
 import numpy as np
 import pytest
-
-FRAME_FNS = ("dim_refine_frames", "dim_refine_frames_host", "dim_refine_frames_host_async")
-
-
-def test_frame_entry_points_are_exported(root):
-    lib = ctypes.CDLL(os.path.join(root, "mx-deepim_b200", "libdeepim_b200.so"))
-    for fn in FRAME_FNS:
-        assert hasattr(lib, fn), fn
-
-
-def test_frame_entry_point_prototypes():
-    """Argument order of the three entries: dim_refine's / dim_refine_host(_async)'s with (frames, F, frame_idx) in place of
-    the image argument, and dim_refine's depth argument in the same place."""
-    import ctypes as C
-    from deepim_b200 import _capi
-    S = _capi.SIGNATURES
-    refine, frames = S["dim_refine"][1], S["dim_refine_frames"][1]
-    assert S["dim_refine_frames"][0] is C.c_int32
-    assert frames[:4] == [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p] and frames[4:] == refine[2:]
-    for host, fr in (("dim_refine_host", "dim_refine_frames_host"), ("dim_refine_host_async", "dim_refine_frames_host_async")):
-        h, f = S[host][1], S[fr][1]
-        assert S[fr][0] is C.c_int32
-        assert f[:4] == [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p] and f[4:] == h[2:], fr
 
 
 @pytest.mark.parametrize("n,n_frames,max_batch,seed", [(37, 11, 16, 0), (16, 3, 16, 1), (5, 1, 16, 2), (64, 64, 8, 3),

@@ -7,15 +7,16 @@ C2 inputs (the 5k-vert blob, 4 iterations, fp16, random-init weights), device ba
 in flight through PoseRefiner (as bench.py's e2e arm), pinned host u8 frames.  Every device batch observes batch / k frames,
 k instances per frame (an initial hypothesis each: the frame's object pose perturbed as synth.sample_pose_pairs does), over
 3 rotating input sets.  Three passes alternate `rounds` times:
-  dup       dim_refine_host_async with each frame copied once per instance (k = 8): `batch` frames uploaded and packed
-  frames8   dim_refine_frames_host_async, k = 8: batch / 8 frames uploaded and packed
-  frames2   dim_refine_frames_host_async, k = 2: batch / 2 frames
-  cams_mixed  dim_refine_frames_k_host_async: `batch` instances, 2 per frame, over batch / 2 frames from 4 cameras (each
-              frame rendered with its own camera), one batch with one K per frame
-  cams_split  the same instances split by camera into 4 batches of batch / 4 through dim_refine_frames_host_async, what a
-              caller without per-frame intrinsics has to do
+  dup       dim_refine_host_async without a frame map, each frame copied once per instance (k = 8): `batch` frames
+            uploaded and packed
+  frames8   dim_refine_host_async with a frame map, k = 8: batch / 8 frames uploaded and packed
+  frames2   dim_refine_host_async with a frame map, k = 2: batch / 2 frames
+  cams_mixed  dim_refine_host_async with a frame map and K_frames: `batch` instances, 2 per frame, over batch / 2 frames
+              from 4 cameras (each frame rendered with its own camera), one batch with one K per frame
+  cams_split  the same instances split by camera into 4 batches of batch / 4 through dim_refine_host_async with a frame
+              map and K9, what a caller without per-frame intrinsics has to do
   cams_one    the same poses, every frame rendered with the first camera: one batch of `batch` through
-              dim_refine_frames_host_async
+              dim_refine_host_async with a frame map and K9
 Reported per pass: refinements/s end to end (host wall clock around `steps` x 32 batches of `batch` instances, results
 consumed; best round), host-to-device bytes per batch (computed from the shapes), and for dup / frames8 / frames2, from a
 pass of one batch at a time on one context with the stage events on (dim_profile_enable) the batch time, the chain's four
@@ -170,13 +171,13 @@ def main():
     # same frames, same instances: the duplicated and the frame-indexed upload refine identically
     p_dup = run("dup", 1)
     p_fr = run("frames8", 1)
-    assert np.array_equal(p_dup, p_fr), "dim_refine_frames_host differs from dim_refine_host on duplicated frames"
+    assert np.array_equal(p_dup, p_fr), "a frame map differs from duplicated frames (dim_refine_host_async)"
     p_mixed = run("cams_mixed", 1)
     p_split = []
     for sub in cam_sets[0]["split"]:
         p_split.append(ref.result(passes["cams_split"][1](sub)))
     assert np.array_equal(p_mixed, np.concatenate(p_split, axis=1)), \
-        "dim_refine_frames_k_host differs from dim_refine_frames_host on the per-camera batches"
+        "K_frames differs from K9 on the per-camera batches (dim_refine_host_async)"
     for name in passes:  # every (slot, input set) argument set: eager run, then graph capture
         run(name, 2 * N_SETS * N_CAMS * len(ref.slots))
         e2e(name, a.warmup)
