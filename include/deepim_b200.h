@@ -100,6 +100,24 @@ DIM_API int32_t dim_render_lit(dim_ctx *ctx, const int32_t *cls_idx, const float
                                float *out_depth, float *out_mask, float *out_bgr, int32_t *out_bbox,
                                void *stream);
 
+/* Data-preparation render (toolkit/LM6d_ds_1 .. ds_4, LM6d_0_gen_gt_observed.py): what the dataset files hold, from one
+ * rasterisation of B instances.
+ *   lit_bgr   u8[B,H,W,3]  Render_Py_Light colour (lib/render_glumpy/render_py_light.py get_fragment):
+ *                          texel * ((1 - ratio) + (ratio * brightness) * light_intensity), brightness as dim_render_lit,
+ *                          quantised to 8 bits.  The light colour scales only the diffuse term (dim_render_lit scales
+ *                          both);
+ *   bgr       u8[B,H,W,3]  unlit colour, Render_Py.render(...).astype('uint8');
+ *   depth_u16 u16[B,H,W]   (uint16)(depth * depth_factor), truncated like numpy's astype(np.uint16);
+ *   label     u8[B,H,W]    depth != 0.
+ * Every output may be NULL.  light_position / light_intensity f32[B,3] and brightness_ratio f32[B] are device arrays,
+ * given exactly when lit_bgr is (the call is refused otherwise); a lit call needs normals for every uploaded mesh
+ * (dim_mesh_upload_normals). */
+DIM_API int32_t dim_render_dataset(dim_ctx *ctx, const int32_t *cls_idx, const float *pose, int32_t B,
+                                   const float *K9_host, float znear, float zfar, float depth_factor,
+                                   const float *light_position, const float *light_intensity,
+                                   const float *brightness_ratio, uint8_t *lit_bgr, uint8_t *bgr,
+                                   uint16_t *depth_u16, uint8_t *label, void *stream);
+
 /* ZoomImage forward (zoom_image.py:26-107, the INPUT_MASK: False front end): the two boxes come from the
  * images themselves, valid = sum_c(image + pixel_mean_c) > 0.01; centre / crop / sampling as ZoomMask +
  * ZoomImageWithFactor.  pixel_means_rgb_host = the op's (already reversed) pixel_means attr.

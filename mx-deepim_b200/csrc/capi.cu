@@ -200,6 +200,27 @@ DIM_API int32_t dim_render_lit(dim_ctx *ctx, const int32_t *cls_idx, const float
                        (cudaStream_t)stream, &lit);
 }
 
+// data-preparation render (toolkit/LM6d_ds_1, ds_2, ds_4, LM6d_0): Render_Py_Light and Render_Py outputs of one pass
+DIM_API int32_t dim_render_dataset(dim_ctx *ctx, const int32_t *cls_idx, const float *pose, int32_t B, const float *K9,
+                                   float zn, float zf, float depth_factor, const float *light_position,
+                                   const float *light_intensity, const float *brightness_ratio, uint8_t *lit_bgr,
+                                   uint8_t *bgr, uint16_t *depth_u16, uint8_t *label, void *stream) {
+  DIM_REQUIRE(ctx && cls_idx && pose && K9, "dim_render_dataset: NULL argument");
+  const char *lit_args[3] = {"light_position", "light_intensity", "brightness_ratio"};
+  const void *lit_ptrs[3] = {light_position, light_intensity, brightness_ratio};
+  for (int k = 0; k < 3; ++k)
+    if ((lit_ptrs[k] != nullptr) != (lit_bgr != nullptr)) {
+      set_error(lit_bgr ? "dim_render_dataset: lit_bgr needs %s (NULL given)"
+                        : "dim_render_dataset: %s is given but lit_bgr is NULL (the light is used only for lit_bgr)",
+                lit_args[k]);
+      return 2;
+    }
+  if (lit_bgr)
+    if (int rc = normals_check(ctx, "dim_render_dataset")) return rc;
+  const DatasetOut o{lit_bgr, bgr, depth_u16, label, brightness_ratio, depth_factor};
+  return render_dataset_launch(ctx, cls_idx, pose, B, K9, zn, zf, light_position, light_intensity, o, (cudaStream_t)stream);
+}
+
 DIM_API int32_t dim_zoom_mask_fwd(dim_ctx *ctx, const float *mo, const float *mgt, const float *mr,
                                   const float *src_pose, int32_t B, const float *K9, float *zmo, float *zmgt,
                                   float *zmr, float *zoom_factor, int32_t *bbox, int32_t *status, void *stream) {

@@ -28,6 +28,17 @@ int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const 
                   int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit = nullptr, bool ren4_depth = false,
                   bool colour_box = false, const float *K_frames = nullptr, const int32_t *frame_idx = nullptr,
                   int n_frames = 0);
+// the data-preparation render (dim_render_dataset): file-ready outputs of one visibility pass, each nullable; ratio and the
+// light arrays of LitParams are per instance and used only for lit_bgr
+struct DatasetOut {
+  uint8_t *lit_bgr, *bgr;  // [B,H,W,3] BGR
+  uint16_t *depth;         // [B,H,W] (uint16)(depth * depth_factor)
+  uint8_t *label;          // [B,H,W] depth != 0
+  const float *ratio;      // device [B] brightness ratio
+  float depth_factor;
+};
+int render_dataset_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
+                          const float *light_pos, const float *light_int, const DatasetOut &o, cudaStream_t st);
 
 // zoom.cu
 int zoom_gather_launch(dim_ctx *ctx, int mode, const float *src, float *dst, const float *zoom_factor, int B, int C,

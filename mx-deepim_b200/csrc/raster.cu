@@ -268,6 +268,54 @@ __device__ __forceinline__ float colour_of(unsigned char c, int trunc_u8) {
   return f;
 }
 
+// The two lit renderers of the reference share the Lambert term and differ in where the light colour enters:
+//   SHADE_MODELNET  (render_py_light_modelnet_multi.py)  colour_c = texel_c * ((a0 + a1 * brightness) * I_c)
+//   SHADE_PY_LIGHT  (render_py_light.py, get_fragment)   colour_c = texel_c * (a0 + (a1 * brightness) * I_c)
+// with a0 = 1 - ratio, a1 = ratio; the fragment (b0, b1, b2, iz) is winner triangle f of instance b.  Returns the colours
+// quantised like the 8-bit framebuffer the reference reads back.
+enum Shade { SHADE_MODELNET, SHADE_PY_LIGHT };
+
+template <Shade S>
+__device__ __forceinline__ void shade_lit(const RasterParams &p, const MeshDev &m, const PVert *pv, int b, int f, float b0,
+                                          float b1, float b2, float iz, const PVert &A, const PVert &Bv, const PVert &Cv,
+                                          const unsigned char *tp, float a0, float a1, float q[3]) {
+  // Lambert shading, same float32 sequence as the CPU checker (see DESIGN.md "lit renderer")
+  const int iA = m.faces[3 * f];
+  int iB = m.faces[3 * f + 1], iC = m.faces[3 * f + 2];
+  if (edge_fn(pv[iA].X, pv[iA].Y, pv[iB].X, pv[iB].Y, pv[iC].X, pv[iC].Y) < 0) { const int tmp = iB; iB = iC; iC = tmp; }
+  const float w0 = b0 * A.iz, w1 = b1 * Bv.iz, w2 = b2 * Cv.iz;
+  const float *ps = p.pose + 12 * b;
+  float pm[3], nm[3], pc[3], nc[3];
+#pragma unroll
+  for (int e = 0; e < 3; ++e) {
+    pm[e] = ((w0 * m.verts[3 * iA + e] + w1 * m.verts[3 * iB + e]) + w2 * m.verts[3 * iC + e]) / iz;
+    nm[e] = ((w0 * m.normals[3 * iA + e] + w1 * m.normals[3 * iB + e]) + w2 * m.normals[3 * iC + e]) / iz;
+  }
+#pragma unroll
+  for (int rr = 0; rr < 3; ++rr) {
+    pc[rr] = ((ps[4 * rr] * pm[0] + ps[4 * rr + 1] * pm[1]) + ps[4 * rr + 2] * pm[2]) + ps[4 * rr + 3];
+    nc[rr] = (ps[4 * rr] * nm[0] + ps[4 * rr + 1] * nm[1]) + ps[4 * rr + 2] * nm[2];
+  }
+  const float *lp = p.light_pos + 3 * b, *li = p.light_int + 3 * b;
+  const float s0 = lp[0] - pc[0], s1 = lp[1] - (0.f - pc[1]), s2 = lp[2] - (0.f - pc[2]);
+  const float g0 = nc[0], g1 = 0.f - nc[1], g2 = 0.f - nc[2];
+  const float dot = (g0 * s0 + g1 * s1) + g2 * s2;
+  const float ls = sqrtf((s0 * s0 + s1 * s1) + s2 * s2), ln = sqrtf((g0 * g0 + g1 * g1) + g2 * g2);
+  const float den = ls * ln;
+  float br = 0.f;
+  if (den > 0.f) br = dot / den;
+  br = br < 1.f ? br : 1.f;
+  br = br > 0.f ? br : 0.f;
+  const float scale = S == SHADE_MODELNET ? a0 + a1 * br : a1 * br;
+#pragma unroll
+  for (int e = 0; e < 3; ++e) {
+    float col = S == SHADE_MODELNET ? ((float)tp[e] / 255.0f) * (scale * li[e]) : ((float)tp[e] / 255.0f) * (a0 + scale * li[e]);
+    col = col < 1.f ? col : 1.f;
+    col = col > 0.f ? col : 0.f;
+    q[e] = rintf(col * 255.0f);
+  }
+}
+
 // LIT is a compile-time switch: the unlit instantiation (the refinement loop's renderer) carries none of the shading code.
 // REN4_DEPTH (the RGB-D network's loop): the w lane of out_ren4 holds the depth instead of the 0/1 mask; the zoom kernel
 // samples it as depth_rendered and re-derives the mask as depth > 0.2, which is how the mask is made here.
@@ -322,42 +370,8 @@ __global__ void __launch_bounds__(256) raster_resolve_kernel(RasterParams p) {
       const unsigned char *tp = m.tex + ((size_t)ty * m.Tw + tx) * 3;
       float c0, c1, c2;
       if (LIT) {
-        // Lambert shading, same float32 sequence as the CPU checker (see DESIGN.md "lit renderer")
-        const int iA = m.faces[3 * f];
-        int iB = m.faces[3 * f + 1], iC = m.faces[3 * f + 2];
-        if (edge_fn(pv[iA].X, pv[iA].Y, pv[iB].X, pv[iB].Y, pv[iC].X, pv[iC].Y) < 0) { const int tmp = iB; iB = iC; iC = tmp; }
-        const float w0 = b0 * A.iz, w1 = b1 * Bv.iz, w2 = b2 * Cv.iz;
-        const float *ps = p.pose + 12 * b;
-        float pm[3], nm[3], pc[3], nc[3];
-#pragma unroll
-        for (int e = 0; e < 3; ++e) {
-          pm[e] = ((w0 * m.verts[3 * iA + e] + w1 * m.verts[3 * iB + e]) + w2 * m.verts[3 * iC + e]) / iz;
-          nm[e] = ((w0 * m.normals[3 * iA + e] + w1 * m.normals[3 * iB + e]) + w2 * m.normals[3 * iC + e]) / iz;
-        }
-#pragma unroll
-        for (int rr = 0; rr < 3; ++rr) {
-          pc[rr] = ((ps[4 * rr] * pm[0] + ps[4 * rr + 1] * pm[1]) + ps[4 * rr + 2] * pm[2]) + ps[4 * rr + 3];
-          nc[rr] = (ps[4 * rr] * nm[0] + ps[4 * rr + 1] * nm[1]) + ps[4 * rr + 2] * nm[2];
-        }
-        const float *lp = p.light_pos + 3 * b, *li = p.light_int + 3 * b;
-        const float s0 = lp[0] - pc[0], s1 = lp[1] - (0.f - pc[1]), s2 = lp[2] - (0.f - pc[2]);
-        const float g0 = nc[0], g1 = 0.f - nc[1], g2 = 0.f - nc[2];
-        const float dot = (g0 * s0 + g1 * s1) + g2 * s2;
-        const float ls = sqrtf((s0 * s0 + s1 * s1) + s2 * s2), ln = sqrtf((g0 * g0 + g1 * g1) + g2 * g2);
-        const float den = ls * ln;
-        float br = 0.f;
-        if (den > 0.f) br = dot / den;
-        br = br < 1.f ? br : 1.f;
-        br = br > 0.f ? br : 0.f;
-        const float scale = p.a0 + p.a1 * br;
         float q[3];
-#pragma unroll
-        for (int e = 0; e < 3; ++e) {
-          float col = ((float)tp[e] / 255.0f) * (scale * li[e]);
-          col = col < 1.f ? col : 1.f;
-          col = col > 0.f ? col : 0.f;
-          q[e] = rintf(col * 255.0f);
-        }
+        shade_lit<SHADE_MODELNET>(p, m, pv, b, f, b0, b1, b2, iz, A, Bv, Cv, tp, p.a0, p.a1, q);
         c0 = q[0]; c1 = q[1]; c2 = q[2];
       } else {
         c0 = colour_of(tp[0], p.trunc_u8); c1 = colour_of(tp[1], p.trunc_u8); c2 = colour_of(tp[2], p.trunc_u8);
@@ -438,6 +452,90 @@ __global__ void raster_finish_kernel(int *bbox_ren, int *out_bbox, int B) {
   }
 }
 
+// The data-preparation render (toolkit/LM6d_ds_1, ds_2, ds_4, LM6d_0): from one visibility pass, the Render_Py_Light colour
+// (SHADE_PY_LIGHT, ratio per instance), the unlit colour rgb_gl.astype('uint8') (Render_Py), the depth file's
+// (depth * depth_factor).astype(uint16) and the label depth != 0, as u8 / u16 planes ready for the PNG encoder.
+template <bool LIT>
+__global__ void __launch_bounds__(256) raster_dataset_kernel(RasterParams p, DatasetOut o) {
+  const int b = blockIdx.y;
+  const int W4 = p.W >> 2;
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= W4 * p.H) return;
+  const int i = q / W4, j4 = (q % W4) << 2;
+  const size_t P = (size_t)p.H * p.W;
+  const int vx0 = p.vbox[4 * b + 0], vx1 = p.vbox[4 * b + 1], vy0 = p.vbox[4 * b + 2], vy1 = p.vbox[4 * b + 3];
+  unsigned long long *vis = p.vis + (size_t)b * P + (size_t)i * p.W + j4;
+
+  unsigned lit[3] = {0u, 0u, 0u}, un[3] = {0u, 0u, 0u};  // 4 BGR pixels = 12 bytes, little-endian
+  unsigned dep[2] = {0u, 0u}, lab = 0u;
+  if (i >= vy0 && i <= vy1 && j4 + 3 >= vx0 && j4 <= vx1) {
+    ulonglong2 k01 = *reinterpret_cast<const ulonglong2 *>(vis);
+    ulonglong2 k23 = *reinterpret_cast<const ulonglong2 *>(vis + 2);
+    unsigned long long keys[4] = {k01.x, k01.y, k23.x, k23.y};
+    bool any = false;
+    const MeshDev m = mesh_for(p, b);
+    const PVert *pv = p.pverts + (size_t)b * p.max_verts;
+    const float a1 = LIT ? o.ratio[b] : 0.f, a0 = 1.f - a1;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (keys[k] == VIS_EMPTY) continue;
+      any = true;
+      const int f = (int)(unsigned)(keys[k] & 0xffffffffull);
+      PVert A = pv[m.faces[3 * f]], Bv = pv[m.faces[3 * f + 1]], Cv = pv[m.faces[3 * f + 2]];
+      TriSetup t;
+      tri_setup(A, Bv, Cv, t);
+      float b0 = 0.f, b1 = 0.f, b2 = 0.f, iz = 1.f, z = 0.f;
+      tri_fragment(t, i, j4 + k, p.zn, p.zf, b0, b1, b2, iz, z);
+      float un_ = (b0 * A.uz + b1 * Bv.uz) + b2 * Cv.uz;
+      float vn_ = (b0 * A.vz + b1 * Bv.vz) + b2 * Cv.vz;
+      float u = un_ / iz, v = vn_ / iz;
+      int tx = (int)floorf(u * (float)m.Tw), ty = (int)floorf(v * (float)m.Th);
+      tx = min(max(tx, 0), m.Tw - 1);
+      ty = min(max(ty, 0), m.Th - 1);
+      const unsigned char *tp = m.tex + ((size_t)ty * m.Tw + tx) * 3;
+#pragma unroll
+      for (int e = 0; e < 3; ++e) {  // BGR byte 3k + e of the 12 holds channel 2 - e
+        const int byte = 3 * k + e;
+        un[byte >> 2] |= (unsigned)(unsigned char)colour_of(tp[2 - e], 0) << ((byte & 3) * 8);
+      }
+      if (LIT) {
+        float c[3];
+        shade_lit<SHADE_PY_LIGHT>(p, m, pv, b, f, b0, b1, b2, iz, A, Bv, Cv, tp, a0, a1, c);
+#pragma unroll
+        for (int e = 0; e < 3; ++e) {
+          const int byte = 3 * k + e;
+          lit[byte >> 2] |= (unsigned)c[2 - e] << ((byte & 3) * 8);
+        }
+      }
+      dep[k >> 1] |= (unsigned)(unsigned short)(z * o.depth_factor) << ((k & 1) * 16);
+      if (z != 0.f) lab |= 1u << (k * 8);
+    }
+    if (any) {  // hand the visibility buffer back empty for the next render
+      *reinterpret_cast<ulonglong2 *>(vis) = make_ulonglong2(VIS_EMPTY, VIS_EMPTY);
+      *reinterpret_cast<ulonglong2 *>(vis + 2) = make_ulonglong2(VIS_EMPTY, VIS_EMPTY);
+    }
+  }
+  const size_t px = (size_t)b * P + (size_t)i * p.W + j4;
+  if (LIT && o.lit_bgr) *reinterpret_cast<uint3 *>(o.lit_bgr + 3 * px) = make_uint3(lit[0], lit[1], lit[2]);
+  if (o.bgr) *reinterpret_cast<uint3 *>(o.bgr + 3 * px) = make_uint3(un[0], un[1], un[2]);
+  if (o.depth) *reinterpret_cast<uint2 *>(o.depth + px) = make_uint2(dep[0], dep[1]);
+  if (o.label) *reinterpret_cast<unsigned *>(o.label + px) = lab;
+}
+
+// raster_init + raster_vertex + raster_coverage: the visibility buffer of every instance, for one resolve kernel
+static int raster_front(dim_ctx *ctx, const RasterParams &p, int B, cudaStream_t st) {
+  int maxV = 0, maxF = 0;
+  for (auto &m : ctx->meshes_host) { maxV = maxV > m.V ? maxV : m.V; maxF = maxF > m.F ? maxF : m.F; }
+  DIM_REQUIRE(maxV > 0 && maxF > 0, "dim_render: no mesh uploaded");
+  raster_init_kernel<<<cdiv(B, 128), 128, 0, st>>>(ctx->vbox, ctx->bbox_ren, B, ctx->H, ctx->W);
+  DIM_LAUNCH_CHECK();
+  raster_vertex_kernel<<<dim3(cdiv(maxV, 256), B), 256, 0, st>>>(p);
+  DIM_LAUNCH_CHECK();
+  raster_coverage_kernel<<<dim3(cdiv(maxF, 128), B), 128, 0, st>>>(p);
+  DIM_LAUNCH_CHECK();
+  return 0;
+}
+
 int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
                   const double *means, int trunc_u8, float *out_image, float *out_depth, float *out_mask,
                   float *out_bgr, int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit, bool ren4_depth,
@@ -462,15 +560,7 @@ int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const 
   p.lit = lit ? 1 : 0;
   p.light_pos = lit ? lit->light_pos : nullptr; p.light_int = lit ? lit->light_int : nullptr;
   p.a0 = lit ? lit->a0 : 0.f; p.a1 = lit ? lit->a1 : 0.f;
-  int maxV = 0, maxF = 0;
-  for (auto &m : ctx->meshes_host) { maxV = maxV > m.V ? maxV : m.V; maxF = maxF > m.F ? maxF : m.F; }
-  DIM_REQUIRE(maxV > 0 && maxF > 0, "dim_render: no mesh uploaded");
-  raster_init_kernel<<<cdiv(B, 128), 128, 0, st>>>(ctx->vbox, ctx->bbox_ren, B, ctx->H, ctx->W);
-  DIM_LAUNCH_CHECK();
-  raster_vertex_kernel<<<dim3(cdiv(maxV, 256), B), 256, 0, st>>>(p);
-  DIM_LAUNCH_CHECK();
-  raster_coverage_kernel<<<dim3(cdiv(maxF, 128), B), 128, 0, st>>>(p);
-  DIM_LAUNCH_CHECK();
+  if (int rc = raster_front(ctx, p, B, st)) return rc;
   const dim3 rgrid(cdiv((ctx->W / 4) * ctx->H, 256), B);
   DIM_REQUIRE(!(ren4_depth && colour_box), "dim_render: the colour bbox has no RGB-D variant");
   if (colour_box) {
@@ -486,6 +576,26 @@ int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const 
   }
   DIM_LAUNCH_CHECK();
   raster_finish_kernel<<<cdiv(B, 128), 128, 0, st>>>(ctx->bbox_ren, out_bbox, B);
+  DIM_LAUNCH_CHECK();
+  return 0;
+}
+
+int render_dataset_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
+                          const float *light_pos, const float *light_int, const DatasetOut &o, cudaStream_t st) {
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_render_dataset: batch exceeds max_batch");
+  DIM_REQUIRE((ctx->W & 3) == 0, "dim_render_dataset: width must be a multiple of 4");
+  RasterParams p = {};
+  p.meshes = ctx->meshes; p.cls = cls; p.pose = pose; p.pverts = ctx->pverts; p.vis = ctx->vis;
+  p.vbox = ctx->vbox; p.bbox_ren = ctx->bbox_ren;
+  p.max_verts = ctx->max_verts; p.max_faces = ctx->max_faces; p.H = ctx->H; p.W = ctx->W;
+  p.num_classes = ctx->max_classes; p.cls_flag = ctx->cls_flag;
+  p.fx = K9[0]; p.fy = K9[4]; p.cx = K9[2]; p.cy = K9[5]; p.zn = zn; p.zf = zf;
+  p.lit = o.lit_bgr ? 1 : 0;
+  p.light_pos = light_pos; p.light_int = light_int;
+  if (int rc = raster_front(ctx, p, B, st)) return rc;
+  const dim3 rgrid(cdiv((ctx->W / 4) * ctx->H, 256), B);
+  if (o.lit_bgr) raster_dataset_kernel<true><<<rgrid, 256, 0, st>>>(p, o);
+  else raster_dataset_kernel<false><<<rgrid, 256, 0, st>>>(p, o);
   DIM_LAUNCH_CHECK();
   return 0;
 }

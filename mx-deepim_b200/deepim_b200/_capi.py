@@ -46,6 +46,7 @@ SIGNATURES = {
     "dim_zoom_image_with_factor_fwd": (i32, [vp, vp, vp, vp, i32, pf32, vp, vp, vp]),
     "dim_mesh_upload_normals": (i32, [vp, i32, vp, i32]),
     "dim_render_lit": (i32, [vp, vp, vp, i32, pf32, f32, f32, pf64, vp, vp, f32, vp, vp, vp, vp, vp, vp]),
+    "dim_render_dataset": (i32, [vp, vp, vp, i32, pf32, f32, f32, f32, vp, vp, vp, vp, vp, vp, vp, vp]),
     "dim_zoom_image_fwd": (i32, [vp, vp, vp, vp, i32, pf32, pf32, vp, vp, vp, vp, vp, vp]),
     "dim_group_picker": (i32, [vp, vp, vp, i32, i32, i32, i64, i32, vp, vp]),
     "dim_zoom_mask_with_factor_fwd": (i32, [vp, vp, vp, i32, i32, vp, vp]),

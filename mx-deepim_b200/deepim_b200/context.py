@@ -206,6 +206,33 @@ class Context:
                                  _p(out["bgr"]), _p(out["bbox"]), self._stream()))
         return out
 
+    def render_dataset(self, cls_idx, pose, K, znear=0.25, zfar=6.0, depth_factor=1000.0, light_position=None,
+                       light_intensity=None, brightness_ratio=None, want=("bgr", "depth", "label")):
+        """dim_render_dataset: the dataset files' images from one rasterisation (toolkit/LM6d_ds_1, ds_2, ds_4, LM6d_0).
+        want names the outputs: "lit_bgr" uint8 [B,H,W,3] (Render_Py_Light colour; needs light_position / light_intensity
+        float32 [B,3] (GL camera frame) and brightness_ratio float32 [B], CUDA tensors), "bgr" uint8 [B,H,W,3] (unlit
+        Render_Py colour), "depth" uint16 [B,H,W] (depth * depth_factor, truncated), "label" uint8 [B,H,W] (depth != 0)."""
+        B = pose.shape[0]
+        _chk(pose, torch.float32, (B, 3, 4), "pose")
+        _chk(cls_idx, torch.int32, (B,), "cls_idx")
+        lit = "lit_bgr" in want
+        if lit:
+            _chk(light_position, torch.float32, (B, 3), "light_position")
+            _chk(light_intensity, torch.float32, (B, 3), "light_intensity")
+            _chk(brightness_ratio, torch.float32, (B,), "brightness_ratio")
+        elif light_position is not None or light_intensity is not None or brightness_ratio is not None:
+            raise ValueError("render_dataset: the light arguments are used only for 'lit_bgr', which `want` does not name")
+        out = {
+            "lit_bgr": self._new((B, self.H, self.W, 3), torch.uint8) if lit else None,
+            "bgr": self._new((B, self.H, self.W, 3), torch.uint8) if "bgr" in want else None,
+            "depth": self._new((B, self.H, self.W), torch.uint16) if "depth" in want else None,
+            "label": self._new((B, self.H, self.W), torch.uint8) if "label" in want else None,
+        }
+        check(lib.dim_render_dataset(self._h, _p(cls_idx), _p(pose), B, farr(np.asarray(K, np.float32).reshape(9), 9), znear,
+                                     zfar, float(depth_factor), _p(light_position), _p(light_intensity), _p(brightness_ratio),
+                                     _p(out["lit_bgr"]), _p(out["bgr"]), _p(out["depth"]), _p(out["label"]), self._stream()))
+        return {k: v for k, v in out.items() if v is not None}
+
     # -------------------------------------------------------------------------------- zoom
     def zoom_mask(self, mask_observed, mask_gt_observed, mask_rendered, src_pose, K):
         B = mask_observed.shape[0]
