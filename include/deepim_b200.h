@@ -359,6 +359,34 @@ DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *frames_u8_hos
  * lies outside [0, F), so it observed frame 0 instead (its pose is meaningless). */
 DIM_API int32_t dim_refine_status(dim_ctx *ctx, int32_t B, int32_t n_iter, int32_t *status_host, void *stream);
 
+/* Projective point-to-plane ICP against the observed depth: polishes B poses (typically dim_refine's last estimate) against
+ * the depth sensor.  Not in the reference (its evaluation only reads ICP poses computed by another program); the contract
+ * is oracle/icp.py, restated on the device in float64.  Per call the model surface is rendered once, at float32(pose_in),
+ * by the refinement loop's rasteriser; each iteration associates every model pixel with the observed pixel it projects
+ * to, builds the 6x6 point-to-plane normal equations of the inliers (|model depth - observed depth| < max_dist) and takes
+ * one Gauss-Newton step.  The results are identical run to run (no atomics in any sum).
+ *   depth_frames f32 [F,H,W] device, metres (0 = hole); frame_idx / F / K9_host / K_frames as dim_refine (a device index
+ *   outside [0, F) means frame 0 and status bit 3; K_frames is read as given; K9_host must be a finite pinhole matrix).
+ *   cls_idx i32[B], pose_in f64[B,3,4] device; 1 <= B, F <= max_batch; n_iter >= 1; max_dist > 0 (metres) also bounds the
+ *   depth step between a model pixel and its neighbours (silhouette and self-occlusion edges); min_points >= 6.
+ *   outputs (device): poses_out f64[n_iter,B,3,4] (the pose after each iteration), inliers i32[n_iter,B] and rms
+ *   f32[n_iter,B] (sqrt(mean r^2) of the inliers, 0 without any), both measured before that iteration's update, and
+ *   status i32[n_iter,B]: 0 = ok; bit 0 = no model pixel (empty render), bit 1 = bad class index, bit 3 = frame index out
+ *   of range, bit 4 = fewer than min_points inliers or a singular system.  With bit 0 or 4 the pose is left unchanged.
+ * Never reads the network: runs on every context variant.  A refused call enqueues nothing and leaves the outputs untouched.
+ * The call overwrites the context's render scratch; refinement graphs captured before it replay unchanged after it.
+ * With dim_profile_enable on, each call adds one record to dim_profile_read: ms4[0] = render, ms4[1] = association + solve. */
+DIM_API int32_t dim_icp(dim_ctx *ctx, const float *depth_frames, int32_t F, const int32_t *frame_idx,
+                        const float *K9_host, const float *K_frames, const int32_t *cls_idx,
+                        const double *pose_in, int32_t B, int32_t n_iter, float znear, float zfar,
+                        float max_dist, int32_t min_points, double *poses_out, int32_t *inliers,
+                        float *rms, int32_t *status, void *stream);
+
+/* The depth files' u16 values [F,H,W] (device) -> metres f32 [F,H,W] (device), as lib/utils/image.py:203,218 converts them:
+ * float32(u16) / float32(depth_factor) (LINEMOD: 1000). */
+DIM_API int32_t dim_depth_from_u16(dim_ctx *ctx, const uint16_t *depth_u16, int32_t F, float depth_factor,
+                                   float *depth, void *stream);
+
 /* BGR u8 HWC -> RGB-mean f32 CHW on device (lib/utils/image.py:583-594 transform). */
 DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int32_t B,
                                        const double *pixel_means_rgb_host, float *image,

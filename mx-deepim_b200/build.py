@@ -2,8 +2,8 @@
 
     python mx-deepim_b200/build.py [--force] [--verbose]
 
-raster.cu / zoom.cu / geom.cu are compiled with -fmad=false: their float32 sequences are specified
-operation by operation (the CPU checker used by tests/ is built with -ffp-contract=off) so that integer
+raster.cu / zoom.cu / geom.cu / icp.cu are compiled with -fmad=false: their float32 (icp.cu: float64)
+sequences are specified operation by operation (the CPU checker used by tests/ is built with -ffp-contract=off) so that integer
 outputs (bbox, masks, coverage) and the rendered images are bit-exact against the oracle.
 """
 import os
@@ -21,6 +21,7 @@ UNITS = {
     "zoom.cu": ["-fmad=false"],
     "geom.cu": ["-fmad=false"],
     "augment.cu": ["-fmad=false"],
+    "icp.cu": ["-fmad=false"],
     "net.cu": [],
     "train.cu": [],
     "capi.cu": [],

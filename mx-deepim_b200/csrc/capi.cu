@@ -88,6 +88,7 @@ DIM_API int32_t dim_ctx_create(int32_t device, int32_t max_batch, int32_t H, int
   rc |= dev_alloc(ctx, &ctx->se3_hist_dev, 8 * Bm * 7);
   rc |= dev_alloc(ctx, &ctx->light_pos, Bm * 3);
   rc |= dev_alloc(ctx, &ctx->lit_intensity, 8 * Bm * 3);
+  rc |= dev_alloc(ctx, &ctx->icp_partial, Bm * (size_t)cdiv(H, ICP_ROWS) * ICP_SLOT);
   if (rc) { dim_ctx_destroy(ctx); return 12; }
   ctx->meshes_host.assign(max_classes, MeshDev{nullptr, nullptr, nullptr, nullptr, 0, 0, 0, 0, nullptr});
   DIM_CHECK(cudaMemset(ctx->meshes, 0, sizeof(MeshDev) * max_classes));
@@ -755,6 +756,41 @@ DIM_API int32_t dim_refine_host_async(dim_ctx *ctx, const uint8_t *frames_u8, in
   if (depth_u16 && !(depth_factor > 0.f && depth_factor < 3.0e38f)) return refuse(fn, "depth_factor must be positive and finite");
   return refine_host_enqueue(ctx, fn, frames_u8, F, frame_host, K_host, cls_host, pose_host, B, n_iter, K9, zn, zf, means,
                              precision, poses_out, se3_out, depth_u16, depth_factor, lighting, (cudaStream_t)stream);
+}
+
+// projective point-to-plane ICP against the observed depth (icp.cu; the contract is oracle/icp.py).  Refused calls enqueue
+// nothing.  The call writes ren4, vbox, bbox_ren, cls_flag and pose_cur_f32, which every refinement iteration rewrites
+// before reading, so refinement graphs captured before it replay unchanged.
+DIM_API int32_t dim_icp(dim_ctx *ctx, const float *depth_frames, int32_t F, const int32_t *frame_idx, const float *K9_host,
+                        const float *K_frames, const int32_t *cls_idx, const double *pose_in, int32_t B, int32_t n_iter,
+                        float znear, float zfar, float max_dist, int32_t min_points, double *poses_out, int32_t *inliers,
+                        float *rms, int32_t *status, void *stream) {
+  const char *fn = "dim_icp";
+  if (!(ctx && depth_frames && cls_idx && pose_in && poses_out && inliers && rms && status)) return refuse(fn, "NULL argument");
+  if (!K9_host == !K_frames) return refuse(fn, "exactly one of K9_host and K_frames must be non-NULL");
+  if (B < 1 || B > ctx->max_batch) return refuse(fn, "batch exceeds max_batch");
+  if (F < 1 || F > ctx->max_batch) return refuse(fn, "frame count F outside [1, max_batch]");
+  if (!frame_idx && F != B) return refuse(fn, "frame_idx is NULL (instance b observes frame b): F must equal B");
+  if (n_iter < 1) return refuse(fn, "n_iter must be >= 1");
+  if (!(max_dist > 0.f && max_dist < 3.0e38f)) return refuse(fn, "max_dist must be positive and finite");
+  if (min_points < 6) return refuse(fn, "min_points must be >= 6 (six pose parameters)");
+  if (K9_host)
+    if (const char *why = pinhole_defect(K9_host)) {
+      set_error("%s: K9_host is not a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]]: %s", fn, why);
+      return 2;
+    }
+  const IcpCall c{depth_frames, F, frame_idx, K9_host, K_frames, cls_idx, pose_in, B, n_iter, znear, zfar, max_dist,
+                  min_points, poses_out, inliers, status, rms};
+  return icp_launch(ctx, c, (cudaStream_t)stream);
+}
+
+DIM_API int32_t dim_depth_from_u16(dim_ctx *ctx, const uint16_t *depth_u16, int32_t F, float depth_factor, float *depth,
+                                   void *stream) {
+  const char *fn = "dim_depth_from_u16";
+  if (!(ctx && depth_u16 && depth)) return refuse(fn, "NULL argument");
+  if (F < 1) return refuse(fn, "F must be >= 1");
+  if (!(depth_factor > 0.f && depth_factor < 3.0e38f)) return refuse(fn, "depth_factor must be positive and finite");
+  return depth_u16_launch(depth_u16, (size_t)F * ctx->H * ctx->W, depth_factor, depth, (cudaStream_t)stream);
 }
 
 // status of the LAST dim_refine / dim_refine_host_async call on this context: [min(n_iter, 8), B] int32, device -> host

@@ -150,6 +150,7 @@ struct dim_ctx {
   float *lit_intensity = nullptr;  // [8, max_batch, 3] lit dim_refine_host_async: the caller's light intensities on the device
   uint16_t *depth_u16 = nullptr;   // [max_batch,H,W] RGB-D dim_refine_host_async: the caller's depth file values
   int *bbox_obs = nullptr;         // [max_batch,4] image-only network: the observed image's colour-valid box (ZoomImage)
+  double *icp_partial = nullptr;   // [max_batch, H / ICP_ROWS, ICP_SLOT] dim_icp: one reduction slot per association CTA
   // background bank of dim_replace_background (dim_bg_upload): BGR u8 photos, each allocated at its upload
   struct BgImage { uint8_t *data = nullptr; int h = 0, w = 0; };
   std::vector<BgImage> bg;

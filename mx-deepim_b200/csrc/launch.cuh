@@ -111,6 +111,26 @@ int replace_bg_launch(dim_ctx *ctx, const BgLaunch &L, int nb, const float *obs,
                       uint8_t *comp, cudaStream_t st);
 int mask_dilate_launch(dim_ctx *ctx, const float *in, const int *draws, int B, float *out, cudaStream_t st);
 
+// icp.cu
+constexpr int ICP_ROWS = 8;   // frame rows per association CTA
+constexpr int ICP_SLOT = 30;  // doubles per CTA slot: A (21 upper entries), g (6), inliers, sum r^2, model pixels
+struct IcpCall {  // dim_icp's arguments, checked
+  const float *depth;  // [F,H,W] metres
+  int F;
+  const int32_t *frame_idx;
+  const float *K9, *K_frames;  // exactly one non-null
+  const int32_t *cls_idx;
+  const double *pose_in;
+  int B, n_iter;
+  float zn, zf, max_dist;
+  int min_points;
+  double *poses_out;
+  int32_t *inliers, *status;
+  float *rms;
+};
+int icp_launch(dim_ctx *ctx, const IcpCall &c, cudaStream_t st);
+int depth_u16_launch(const uint16_t *in, size_t n, float factor, float *out, cudaStream_t st);
+
 // net.cu
 int net_create(dim_ctx *ctx);
 void net_destroy(dim_ctx *ctx);

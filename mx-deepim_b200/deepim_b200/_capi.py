@@ -76,6 +76,8 @@ SIGNATURES = {
     "dim_debug_activation": (i32, [vp, i32, i32, vp, u64]),
     "dim_debug_layer_geometry": (i32, [vp, i32, C.POINTER(i32)]),
     "dim_refine_status": (i32, [vp, i32, i32, vp, vp]),
+    "dim_icp": (i32, [vp, vp, i32, vp, pf32, vp, vp, vp, i32, i32, f32, f32, f32, i32, vp, vp, vp, vp, vp]),
+    "dim_depth_from_u16": (i32, [vp, vp, i32, f32, vp, vp]),
     "dim_debug_set_option": (i32, [vp, C.c_char_p, i32]),
     "dim_debug_graph_count": (i32, [vp]),
     "dim_debug_layer_profile": (i32, [vp, i32, pf32]),

@@ -635,6 +635,53 @@ class Context:
         return poses_out, se3_out
 
 
+    # ------------------------------------------------------------------------------ ICP
+    def icp(self, depth_frames, cls_idx, poses, K, n_iter=10, max_dist=0.02, min_points=64, frame_idx=None, znear=0.25,
+            zfar=6.0):
+        """Projective point-to-plane ICP of poses against observed depth (dim_icp; the contract is oracle/icp.py): the model
+        surface is rendered once at float32(poses), then n_iter Gauss-Newton steps, all in float64.
+        depth_frames f32 [F,H,W] (or [F,1,H,W]) CUDA, metres, 0 = hole; cls_idx i32 [B] CUDA; poses f64 [B,3,4] CUDA.
+        frame_idx None = instance b observes frame b (F == B), else i32 [B] CUDA (an index outside [0, F) means frame 0 and
+        status bit 3).  K: [3,3] (one camera) or [F,3,3] (one per frame), as refine_frames.
+        max_dist (metres) bounds the inlier depth residual and the depth step between neighbouring model pixels;
+        min_points is the fewest inliers an update needs.  The defaults (10 iterations, 2 cm, 64 points) are starting
+        values and have not been tuned.
+        Returns CUDA tensors: poses f64 [n_iter,B,3,4] (after each iteration), inliers i32 [n_iter,B], rms f32 [n_iter,B]
+        (both before that iteration's update), status i32 [n_iter,B] (bit 0 no model pixel, bit 1 bad class, bit 3 frame
+        index out of range, bit 4 too few inliers or a singular system; with bit 0 or 4 the pose is unchanged)."""
+        F = depth_frames.shape[0]
+        B = F if frame_idx is None else cls_idx.shape[0]
+        _chk(depth_frames, torch.float32, (F, 1, self.H, self.W) if depth_frames.dim() == 4 else (F, self.H, self.W),
+             "depth_frames")
+        if frame_idx is not None:
+            _chk(frame_idx, torch.int32, (B,), "frame_idx")
+        _chk(cls_idx, torch.int32, (B,), "cls_idx")
+        _chk(poses, torch.float64, (B, 3, 4), "poses")
+        K9 = K_frames = None
+        if _per_frame_k(K, F):
+            K_frames = K
+            if not (isinstance(K, torch.Tensor) and K.device == self.device and K.dtype == torch.float32 and K.is_contiguous()):
+                K_frames = torch.as_tensor(np.ascontiguousarray(K if not isinstance(K, torch.Tensor) else K.cpu(), np.float32),
+                                           device=self.device)
+        else:
+            K9 = farr(np.asarray(K if not isinstance(K, torch.Tensor) else K.cpu(), np.float32).reshape(9), 9)
+        out = {"poses": self._new((n_iter, B, 3, 4), torch.float64), "inliers": self._new((n_iter, B), torch.int32),
+               "rms": self._new((n_iter, B)), "status": self._new((n_iter, B), torch.int32)}
+        check(lib.dim_icp(self._h, _p(depth_frames), F, _p(frame_idx), K9, _p(K_frames), _p(cls_idx), _p(poses), B, n_iter,
+                          znear, zfar, float(max_dist), int(min_points), _p(out["poses"]), _p(out["inliers"]), _p(out["rms"]),
+                          _p(out["status"]), self._stream()))
+        return out
+
+    def depth_from_u16(self, depth_u16, depth_factor=1000.0):
+        """uint16 depth file values [F,H,W] CUDA -> metres f32 [F,H,W], float32(u16) / float32(depth_factor) (the
+        reference's loader, lib/utils/image.py:203,218)."""
+        F = depth_u16.shape[0]
+        _chk(depth_u16, torch.uint16, (F, self.H, self.W), "depth_u16")
+        out = self._new((F, self.H, self.W))
+        check(lib.dim_depth_from_u16(self._h, _p(depth_u16), F, float(np.float32(depth_factor)), _p(out), self._stream()))
+        return out
+
+
 def _refine_status(self, B, n_iter, out=None, sync=True):
     """Per-iteration status of the last refine / refine_host / refine_frames(_host) call: int32 [min(n_iter,8), B]; 0 = ok,
     bit 0 = empty rendered mask in that iteration (pose meaningless; the reference crashes there), bit 1 = bad class index,

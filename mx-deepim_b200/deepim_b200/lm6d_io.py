@@ -177,7 +177,7 @@ class LM6DRefine:
 
 
 def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl", "cup"), n_iter=4, max_batch=16, device=0,
-             precision="fp16", input_depth=False, input_mask=True):
+             precision="fp16", input_depth=False, input_mask=True, icp_iters=0):
     """Batched pred_eval (deepim/core/tester.py:50-527 without its batch = 1 limit): refine every pair of the image set
     and score it the way the reference's dataset class does: ADD / ADI accuracy + AUC (evaluate_pose_add), 5 cm 5 deg
     (evaluate_pose) and Proj. 2D (evaluate_pose_arp_2d); the last two under res["rot_trans"] / res["arp_2d"].
@@ -187,6 +187,10 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
     A pair whose observed frame has a `-K.txt` (load_pair) is refined with that camera, for the render and the zoom, and the
     other pairs with K, in one set of batches (PoseRefiner.refine with a K per instance).  Proj. 2D projects with K for every
     pair, as the reference's evaluate_pose_arp_2d does with config.dataset.INTRINSIC_MATRIX (LM6D_REFINE.py:526).
+    icp_iters > 0 polishes the last refined poses against each pair's observed `-depth.png` with PoseRefiner.icp (icp_iters
+    iterations at its default max_dist / min_points, each pair with its own `-K.txt` camera where it has one) and scores
+    the result as one more row, the "+ ICP" row of the reference's evaluation (TEST.PRECOMPUTED_ICP): poses_est and every
+    table then have n_iter + 1 rows, the last one after ICP.  With icp_iters = 0 nothing changes.
     Returns (evaluate_pose_add result + the two extra tables, poses_est [n_iter,M,3,4], poses_gt)."""
     from . import pose_eval
     from .refiner import PoseRefiner
@@ -202,14 +206,18 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
             cls_idx.append(ci)
             init.append(rec["pose_rendered"])
             gt.append(rec["pose_observed"])
-            if input_depth:
+            if input_depth or icp_iters > 0:
                 depths.append(read_depth_u16(os.path.join(dataset.root, "data", "observed", pair[0] + "-depth.png")))
     imgs, cls_idx = np.stack(imgs), np.asarray(cls_idx, np.int32)
     init, gt = np.stack(init).astype(np.float64), np.stack(gt).astype(np.float64)
     K_pairs = None  # one camera for every pair unless some pair has its own
     if any(k is not None for k in Ks):
         K_pairs = np.stack([np.asarray(K if k is None else k, np.float32).reshape(3, 3) for k in Ks])
-    poses = ref.refine(imgs, cls_idx, init, depths_u16=np.stack(depths).astype(np.uint16) if input_depth else None, K=K_pairs)
+    depths = np.stack(depths).astype(np.uint16) if depths else None
+    poses = ref.refine(imgs, cls_idx, init, depths_u16=depths if input_depth else None, K=K_pairs)
+    if icp_iters > 0:
+        polished = ref.icp(depths, cls_idx, poses[-1], K_frames=K_pairs, n_iter=icp_iters)["poses"][-1]
+        poses = np.concatenate([poses, polished[None]])
     res = pose_eval.evaluate_pose_add(ref.ctx, poses, gt, cls_idx, [dataset.points(c) for c in dataset.classes],
                                       [dataset.diameters[c] for c in dataset.classes], [c in symmetric for c in dataset.classes])
     pts_all = [dataset.points(c) for c in dataset.classes]

@@ -232,6 +232,57 @@ class PoseRefiner:
             out[:, pa - lo:pb - lo] = self.result(t)
         return sharding.gather_results(out, n, axis=1, dist=dist, device=self.ctx.device if world > 1 else None)
 
+    def icp(self, depths_u16, cls_idx, poses, K_frames=None, frame_of=None, n_iter=10, max_dist=0.02, min_points=64):
+        """Point-to-plane ICP of poses against the observed depth (Context.icp, dim_icp), typically on refine()'s last poses.
+        depths_u16 uint16 [F,H,W] host (the *-depth.png values), converted on the device as float32(u16) /
+        float32(depth_factor); cls_idx [N]; poses [N,3,4] float64 host.  frame_of None = instance i observes frame i (F == N),
+        else int [N]; K_frames None = the refiner's K, else float32 [F,3,3] = each frame's camera.
+        The device batches are refine_frames()'s (plan_frame_batches), pipelined over the slots, so instance i's results
+        equal Context.icp's on its batch.  The defaults (10 iterations, 2 cm, 64 points) are starting values and have not
+        been tuned.
+        Returns host arrays: poses [n_iter,N,3,4] float64, inliers [n_iter,N] int32, rms [n_iter,N] float32 and status
+        [n_iter,N] int32 (see Context.icp)."""
+        depths_u16 = np.asarray(depths_u16, np.uint16)
+        n = len(cls_idx)
+        if frame_of is None:
+            if len(depths_u16) != n:
+                raise ValueError("frame_of is None (instance i observes frame i): %d frames for %d instances" % (len(depths_u16), n))
+            frame_of = np.arange(n)
+        elif len(frame_of) != n:
+            raise ValueError("frame_of has %d entries for %d instances" % (len(frame_of), n))
+        cls_idx, poses = np.asarray(cls_idx, np.int32), np.asarray(poses, np.float64)
+        out = {"poses": np.zeros((n_iter, n, 3, 4)), "inliers": np.zeros((n_iter, n), np.int32),
+               "rms": np.zeros((n_iter, n), np.float32), "status": np.zeros((n_iter, n), np.int32)}
+        pending = []
+
+        def collect(i, a, b, res):
+            self.slots[i]["stream"].synchronize()
+            self.slots[i]["busy"] = False
+            for k in out:
+                out[k][:, a:b] = res[k].numpy()
+
+        for a, b, frames, local, *k in plan_frame_batches(frame_of, len(depths_u16), self.max_batch, 0, n, K_frames):
+            if len(pending) == len(self.slots):
+                collect(*pending.pop(0))
+            i = self._next
+            slot = self.slots[i]
+            if slot["busy"]:
+                raise RuntimeError("PoseRefiner: slot still in flight; call result() first")
+            ctx = slot["ctx"]
+            with torch.cuda.stream(slot["stream"]):
+                dev = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(ctx.device, non_blocking=True)
+                depth = ctx.depth_from_u16(dev(depths_u16[frames]), self.depth_factor)
+                r = ctx.icp(depth, dev(cls_idx[a:b]), dev(poses[a:b]), k[0] if k else self.K, n_iter, max_dist, min_points,
+                            dev(local))
+                res = {key: torch.empty(v.shape, dtype=v.dtype).pin_memory().copy_(v, non_blocking=True)
+                       for key, v in r.items()}
+            slot["busy"] = True
+            self._next = (i + 1) % len(self.slots)
+            pending.append((i, a, b, res))
+        for p in pending:
+            collect(*p)
+        return out
+
     def close(self):
         for s in self.slots:
             s["ctx"].close()
