@@ -387,6 +387,28 @@ DIM_API int32_t dim_icp(dim_ctx *ctx, const float *depth_frames, int32_t F, cons
 DIM_API int32_t dim_depth_from_u16(dim_ctx *ctx, const uint16_t *depth_u16, int32_t F, float depth_factor,
                                    float *depth, void *stream);
 
+/* Visible Surface Discrepancy (Hodan et al., "On Evaluation of 6D Object Pose Estimation", ECCVW 2016; the render-based
+ * error of the reference's lib/utils/pose_error.py): per instance, the depth renders at float32(poses_est) and
+ * float32(poses_gt) by the refinement loop's rasteriser, the distance images of them and of the observed depth
+ * (lib/utils/misc.py depth_im_to_dist_im), the visibility masks V_gt and V_est (lib/utils/visibility.py, tolerance delta,
+ * compared in float32), and for each tau the step cost e = (c_tau + |union| - |inter|) / |union|, c_tau = the pixels of
+ * V_gt & V_est whose distances differ by >= tau; e = 1 when the union is empty.  The contract is oracle/vsd.py.  Every sum is
+ * an integer count: the results are identical run to run and for any batch composition.
+ *   depth_frames f32 [F,H,W] device, metres (0 = hole); frame_idx / F / K9_host / K_frames as dim_refine (a device index
+ *   outside [0, F) means frame 0 and status bit 3; K9_host must be a finite pinhole matrix).
+ *   cls_idx i32[B], poses_est / poses_gt f64[B,3,4] device; 1 <= B, F <= max_batch; delta > 0 (metres, finite);
+ *   taus_host f64[n_tau] host, 1 <= n_tau <= 16, each > 0 and finite.
+ *   outputs (device): err f64[B,n_tau]; status i32[B] (nullable): 0 = ok; bit 0 = empty union (e = 1), bit 1 = bad class
+ *   index, bit 3 = frame index out of range.
+ * Never reads the network: runs on every context variant.  A refused call enqueues nothing and leaves the outputs untouched.
+ * The call overwrites the context's render scratch; refinement graphs captured before it replay unchanged after it.
+ * With dim_profile_enable on, each call adds one record to dim_profile_read: ms4[0] = the two renders, ms4[1] = VSD pass. */
+DIM_API int32_t dim_pose_error_vsd(dim_ctx *ctx, const float *depth_frames, int32_t F, const int32_t *frame_idx,
+                                   const float *K9_host, const float *K_frames, const int32_t *cls_idx,
+                                   const double *poses_est, const double *poses_gt, int32_t B, float znear, float zfar,
+                                   float delta, const double *taus_host, int32_t n_tau, double *err, int32_t *status,
+                                   void *stream);
+
 /* BGR u8 HWC -> RGB-mean f32 CHW on device (lib/utils/image.py:583-594 transform). */
 DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int32_t B,
                                        const double *pixel_means_rgb_host, float *image,

@@ -2,7 +2,7 @@
 
     python mx-deepim_b200/build.py [--force] [--verbose]
 
-raster.cu / zoom.cu / geom.cu / icp.cu are compiled with -fmad=false: their float32 (icp.cu: float64)
+raster.cu / zoom.cu / geom.cu / icp.cu / vsd.cu are compiled with -fmad=false: their float32 (icp.cu, vsd.cu: float64)
 sequences are specified operation by operation (the CPU checker used by tests/ is built with -ffp-contract=off) so that integer
 outputs (bbox, masks, coverage) and the rendered images are bit-exact against the oracle.
 """
@@ -22,6 +22,7 @@ UNITS = {
     "geom.cu": ["-fmad=false"],
     "augment.cu": ["-fmad=false"],
     "icp.cu": ["-fmad=false"],
+    "vsd.cu": ["-fmad=false"],
     "net.cu": [],
     "train.cu": [],
     "capi.cu": [],

@@ -89,6 +89,8 @@ DIM_API int32_t dim_ctx_create(int32_t device, int32_t max_batch, int32_t H, int
   rc |= dev_alloc(ctx, &ctx->light_pos, Bm * 3);
   rc |= dev_alloc(ctx, &ctx->lit_intensity, 8 * Bm * 3);
   rc |= dev_alloc(ctx, &ctx->icp_partial, Bm * (size_t)cdiv(H, ICP_ROWS) * ICP_SLOT);
+  rc |= dev_alloc(ctx, &ctx->vsd_partial, Bm * (size_t)cdiv(H, VSD_ROWS) * VSD_SLOT);
+  rc |= dev_alloc(ctx, &ctx->vsd_box, Bm * 4);
   if (rc) { dim_ctx_destroy(ctx); return 12; }
   ctx->meshes_host.assign(max_classes, MeshDev{nullptr, nullptr, nullptr, nullptr, 0, 0, 0, 0, nullptr});
   DIM_CHECK(cudaMemset(ctx->meshes, 0, sizeof(MeshDev) * max_classes));
@@ -782,6 +784,33 @@ DIM_API int32_t dim_icp(dim_ctx *ctx, const float *depth_frames, int32_t F, cons
   const IcpCall c{depth_frames, F, frame_idx, K9_host, K_frames, cls_idx, pose_in, B, n_iter, znear, zfar, max_dist,
                   min_points, poses_out, inliers, status, rms};
   return icp_launch(ctx, c, (cudaStream_t)stream);
+}
+
+// Visible Surface Discrepancy (vsd.cu; the contract is oracle/vsd.py).  Refused calls enqueue nothing and leave the outputs
+// untouched.  The call writes ren4, vbox, bbox_ren, cls_flag, pose_cur_f32 and mask_rendered, which every refinement
+// iteration (and dim_train_update, for mask_rendered) rewrites before reading, so graphs captured before it replay unchanged.
+DIM_API int32_t dim_pose_error_vsd(dim_ctx *ctx, const float *depth_frames, int32_t F, const int32_t *frame_idx,
+                                   const float *K9_host, const float *K_frames, const int32_t *cls_idx, const double *poses_est,
+                                   const double *poses_gt, int32_t B, float znear, float zfar, float delta,
+                                   const double *taus_host, int32_t n_tau, double *err, int32_t *status, void *stream) {
+  const char *fn = "dim_pose_error_vsd";
+  if (!(ctx && depth_frames && cls_idx && poses_est && poses_gt && taus_host && err)) return refuse(fn, "NULL argument");
+  if (!K9_host == !K_frames) return refuse(fn, "exactly one of K9_host and K_frames must be non-NULL");
+  if (B < 1 || B > ctx->max_batch) return refuse(fn, "batch exceeds max_batch");
+  if (F < 1 || F > ctx->max_batch) return refuse(fn, "frame count F outside [1, max_batch]");
+  if (!frame_idx && F != B) return refuse(fn, "frame_idx is NULL (instance b observes frame b): F must equal B");
+  if (n_tau < 1 || n_tau > VSD_MAX_TAU) return refuse(fn, "n_tau must be in [1,16]");
+  if (!(delta > 0.f && delta < 3.0e38f)) return refuse(fn, "delta must be positive and finite");
+  for (int32_t k = 0; k < n_tau; ++k)
+    if (!(taus_host[k] > 0.0 && taus_host[k] < 1.0e308)) return refuse(fn, "every tau must be positive and finite");
+  if (K9_host)
+    if (const char *why = pinhole_defect(K9_host)) {
+      set_error("%s: K9_host is not a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]]: %s", fn, why);
+      return 2;
+    }
+  const VsdCall c{depth_frames, F, frame_idx, K9_host, K_frames, cls_idx, poses_est, poses_gt, B, znear, zfar, delta,
+                  taus_host, n_tau, err, status};
+  return vsd_launch(ctx, c, (cudaStream_t)stream);
 }
 
 DIM_API int32_t dim_depth_from_u16(dim_ctx *ctx, const uint16_t *depth_u16, int32_t F, float depth_factor, float *depth,

@@ -151,6 +151,8 @@ struct dim_ctx {
   uint16_t *depth_u16 = nullptr;   // [max_batch,H,W] RGB-D dim_refine_host_async: the caller's depth file values
   int *bbox_obs = nullptr;         // [max_batch,4] image-only network: the observed image's colour-valid box (ZoomImage)
   double *icp_partial = nullptr;   // [max_batch, H / ICP_ROWS, ICP_SLOT] dim_icp: one reduction slot per association CTA
+  int32_t *vsd_partial = nullptr;  // [max_batch, H / VSD_ROWS, VSD_SLOT] dim_pose_error_vsd: one count slot per pass CTA
+  int *vsd_box = nullptr;          // [max_batch,4] dim_pose_error_vsd: the ground-truth render's vertex box
   // background bank of dim_replace_background (dim_bg_upload): BGR u8 photos, each allocated at its upload
   struct BgImage { uint8_t *data = nullptr; int h = 0, w = 0; };
   std::vector<BgImage> bg;

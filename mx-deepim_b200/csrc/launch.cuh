@@ -131,6 +131,26 @@ struct IcpCall {  // dim_icp's arguments, checked
 int icp_launch(dim_ctx *ctx, const IcpCall &c, cudaStream_t st);
 int depth_u16_launch(const uint16_t *in, size_t n, float factor, float *out, cudaStream_t st);
 
+// vsd.cu
+constexpr int VSD_ROWS = 8;                     // frame rows per VSD pass CTA
+constexpr int VSD_MAX_TAU = 16;
+constexpr int VSD_SLOT = 2 + VSD_MAX_TAU;       // int32 per CTA slot: |union|, |inter|, c_tau
+struct VsdCall {  // dim_pose_error_vsd's arguments, checked
+  const float *depth;  // [F,H,W] metres
+  int F;
+  const int32_t *frame_idx;
+  const float *K9, *K_frames;  // exactly one non-null
+  const int32_t *cls_idx;
+  const double *pose_est, *pose_gt;
+  int B;
+  float zn, zf, delta;
+  const double *taus;  // host [n_tau]
+  int n_tau;
+  double *err;
+  int32_t *status;  // nullable
+};
+int vsd_launch(dim_ctx *ctx, const VsdCall &c, cudaStream_t st);
+
 // net.cu
 int net_create(dim_ctx *ctx);
 void net_destroy(dim_ctx *ctx);

@@ -78,6 +78,7 @@ SIGNATURES = {
     "dim_refine_status": (i32, [vp, i32, i32, vp, vp]),
     "dim_icp": (i32, [vp, vp, i32, vp, pf32, vp, vp, vp, i32, i32, f32, f32, f32, i32, vp, vp, vp, vp, vp]),
     "dim_depth_from_u16": (i32, [vp, vp, i32, f32, vp, vp]),
+    "dim_pose_error_vsd": (i32, [vp, vp, i32, vp, pf32, vp, vp, vp, vp, i32, f32, f32, f32, pf64, i32, vp, vp, vp]),
     "dim_debug_set_option": (i32, [vp, C.c_char_p, i32]),
     "dim_debug_graph_count": (i32, [vp]),
     "dim_debug_layer_profile": (i32, [vp, i32, pf32]),

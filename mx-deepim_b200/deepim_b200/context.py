@@ -649,6 +649,37 @@ class Context:
         Returns CUDA tensors: poses f64 [n_iter,B,3,4] (after each iteration), inliers i32 [n_iter,B], rms f32 [n_iter,B]
         (both before that iteration's update), status i32 [n_iter,B] (bit 0 no model pixel, bit 1 bad class, bit 3 frame
         index out of range, bit 4 too few inliers or a singular system; with bit 0 or 4 the pose is unchanged)."""
+        F, B, K9, K_frames = self._depth_args(depth_frames, cls_idx, frame_idx, K)
+        _chk(poses, torch.float64, (B, 3, 4), "poses")
+        out = {"poses": self._new((n_iter, B, 3, 4), torch.float64), "inliers": self._new((n_iter, B), torch.int32),
+               "rms": self._new((n_iter, B)), "status": self._new((n_iter, B), torch.int32)}
+        check(lib.dim_icp(self._h, _p(depth_frames), F, _p(frame_idx), K9, _p(K_frames), _p(cls_idx), _p(poses), B, n_iter,
+                          znear, zfar, float(max_dist), int(min_points), _p(out["poses"]), _p(out["inliers"]), _p(out["rms"]),
+                          _p(out["status"]), self._stream()))
+        return out
+
+    def pose_error_vsd(self, depth_frames, cls_idx, poses_est, poses_gt, K, delta=0.015, taus=(0.02,), frame_idx=None,
+                       znear=0.25, zfar=6.0):
+        """Visible Surface Discrepancy of poses_est against poses_gt (dim_pose_error_vsd; Hodan et al., ECCVW 2016; the
+        contract is oracle/vsd.py): both poses are rendered at float32, and the visible surfaces are compared against the
+        observed depth with tolerance delta (metres) and the step cost at each tau (metres, at most 16 of them).
+        depth_frames f32 [F,H,W] (or [F,1,H,W]) CUDA, metres, 0 = hole; cls_idx i32 [B] CUDA; poses_est / poses_gt f64
+        [B,3,4] CUDA; frame_idx and K as icp.
+        Returns CUDA tensors: err f64 [B,n_tau] (1 = worst; 1 when neither pose leaves a visible pixel) and status i32 [B]
+        (bit 0 empty union, bit 1 bad class, bit 3 frame index out of range)."""
+        F, B, K9, K_frames = self._depth_args(depth_frames, cls_idx, frame_idx, K)
+        _chk(poses_est, torch.float64, (B, 3, 4), "poses_est")
+        _chk(poses_gt, torch.float64, (B, 3, 4), "poses_gt")
+        taus = np.ascontiguousarray(np.asarray(taus, np.float64).reshape(-1))
+        out = {"err": self._new((B, len(taus)), torch.float64), "status": self._new((B,), torch.int32)}
+        check(lib.dim_pose_error_vsd(self._h, _p(depth_frames), F, _p(frame_idx), K9, _p(K_frames), _p(cls_idx),
+                                     _p(poses_est), _p(poses_gt), B, znear, zfar, float(delta), farr(taus, ctype=C.c_double),
+                                     len(taus), _p(out["err"]), _p(out["status"]), self._stream()))
+        return out
+
+    def _depth_args(self, depth_frames, cls_idx, frame_idx, K):
+        """icp / pose_error_vsd: checks the frames, classes and frame map -> (F, B, K9 host array or None, K_frames CUDA
+        tensor or None)"""
         F = depth_frames.shape[0]
         B = F if frame_idx is None else cls_idx.shape[0]
         _chk(depth_frames, torch.float32, (F, 1, self.H, self.W) if depth_frames.dim() == 4 else (F, self.H, self.W),
@@ -656,7 +687,6 @@ class Context:
         if frame_idx is not None:
             _chk(frame_idx, torch.int32, (B,), "frame_idx")
         _chk(cls_idx, torch.int32, (B,), "cls_idx")
-        _chk(poses, torch.float64, (B, 3, 4), "poses")
         K9 = K_frames = None
         if _per_frame_k(K, F):
             K_frames = K
@@ -665,12 +695,7 @@ class Context:
                                            device=self.device)
         else:
             K9 = farr(np.asarray(K if not isinstance(K, torch.Tensor) else K.cpu(), np.float32).reshape(9), 9)
-        out = {"poses": self._new((n_iter, B, 3, 4), torch.float64), "inliers": self._new((n_iter, B), torch.int32),
-               "rms": self._new((n_iter, B)), "status": self._new((n_iter, B), torch.int32)}
-        check(lib.dim_icp(self._h, _p(depth_frames), F, _p(frame_idx), K9, _p(K_frames), _p(cls_idx), _p(poses), B, n_iter,
-                          znear, zfar, float(max_dist), int(min_points), _p(out["poses"]), _p(out["inliers"]), _p(out["rms"]),
-                          _p(out["status"]), self._stream()))
-        return out
+        return F, B, K9, K_frames
 
     def depth_from_u16(self, depth_u16, depth_factor=1000.0):
         """uint16 depth file values [F,H,W] CUDA -> metres f32 [F,H,W], float32(u16) / float32(depth_factor) (the

@@ -177,7 +177,7 @@ class LM6DRefine:
 
 
 def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl", "cup"), n_iter=4, max_batch=16, device=0,
-             precision="fp16", input_depth=False, input_mask=True, icp_iters=0):
+             precision="fp16", input_depth=False, input_mask=True, icp_iters=0, vsd=False):
     """Batched pred_eval (deepim/core/tester.py:50-527 without its batch = 1 limit): refine every pair of the image set
     and score it the way the reference's dataset class does: ADD / ADI accuracy + AUC (evaluate_pose_add), 5 cm 5 deg
     (evaluate_pose) and Proj. 2D (evaluate_pose_arp_2d); the last two under res["rot_trans"] / res["arp_2d"].
@@ -191,6 +191,11 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
     iterations at its default max_dist / min_points, each pair with its own `-K.txt` camera where it has one) and scores
     the result as one more row, the "+ ICP" row of the reference's evaluation (TEST.PRECOMPUTED_ICP): poses_est and every
     table then have n_iter + 1 rows, the last one after ICP.  With icp_iters = 0 nothing changes.
+    vsd=True also scores every row (each iteration, and the ICP row) with the Visible Surface Discrepancy against each
+    pair's observed `-depth.png` (PoseRefiner.vsd, each pair with its own `-K.txt` camera where it has one, because the
+    depth belongs to that camera), with the values of Hodan et al. and the SIXD Challenge 2017: delta 15 mm, tau 20 mm,
+    recall at e < 0.3.  res["vsd"] holds evaluate_pose_vsd's per-class and mean recall per row and the errors [rows,M].
+    With vsd=False the result is unchanged.
     Returns (evaluate_pose_add result + the two extra tables, poses_est [n_iter,M,3,4], poses_gt)."""
     from . import pose_eval
     from .refiner import PoseRefiner
@@ -206,7 +211,7 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
             cls_idx.append(ci)
             init.append(rec["pose_rendered"])
             gt.append(rec["pose_observed"])
-            if input_depth or icp_iters > 0:
+            if input_depth or icp_iters > 0 or vsd:
                 depths.append(read_depth_u16(os.path.join(dataset.root, "data", "observed", pair[0] + "-depth.png")))
     imgs, cls_idx = np.stack(imgs), np.asarray(cls_idx, np.int32)
     init, gt = np.stack(init).astype(np.float64), np.stack(gt).astype(np.float64)
@@ -221,6 +226,10 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
     res = pose_eval.evaluate_pose_add(ref.ctx, poses, gt, cls_idx, [dataset.points(c) for c in dataset.classes],
                                       [dataset.diameters[c] for c in dataset.classes], [c in symmetric for c in dataset.classes])
     pts_all = [dataset.points(c) for c in dataset.classes]
+    if vsd:
+        errs = np.stack([ref.vsd(depths, cls_idx, p, gt, K_frames=K_pairs, delta=0.015, taus=(0.02,))["err"][:, 0]
+                         for p in poses])
+        res["vsd"] = dict(pose_eval.evaluate_pose_vsd(errs, cls_idx, len(dataset.classes), 0.3), errors=errs)
     res["rot_trans"] = pose_eval.evaluate_pose(ref.ctx, poses, gt, cls_idx, pts_all, K, class_names=list(dataset.classes))
     res["arp_2d"] = pose_eval.evaluate_pose_arp_2d(ref.ctx, poses, gt, cls_idx, pts_all, K, class_names=list(dataset.classes))
     ref.close()

@@ -152,6 +152,25 @@ def evaluate_pose_arp_2d(ctx, poses_est, poses_gt, cls_idx, points_per_class, K,
     return res
 
 
+def evaluate_pose_vsd(errors, cls_idx, n_classes, theta=0.3):
+    """Recall of the Visible Surface Discrepancy (Hodan et al., ECCVW 2016; the SIXD Challenge 2017 counts a pose as correct
+    when e < theta = 0.3): errors [n_rows,M] float64 (one tau; e.g. PoseRefiner.vsd's err[:, k] per row), cls_idx [M].
+    Returns per class and the mean over the classes that have instances: the percentage of instances with e < theta, per
+    row (lists of n_rows)."""
+    errors, cls_idx = np.asarray(errors, np.float64), np.asarray(cls_idx)
+    res = {"classes": {}, "mean": {}}
+    per = []
+    for c in range(n_classes):
+        sel = np.nonzero(cls_idx == c)[0]
+        if len(sel) == 0:
+            continue
+        rec = [100.0 * float((e < theta).sum()) / float(len(sel)) for e in errors[:, sel]]
+        res["classes"][c] = rec
+        per.append(rec)
+    res["mean"]["recall"] = np.mean(per, axis=0).tolist() if per else [0.0] * len(errors)
+    return res
+
+
 def simpson(y, dx):
     """Composite Simpson rule as scipy.integrate.simps(y, dx=dx) with the default even='avg' handling for an even
     number of samples (average of 'first N-2 intervals + trapezoid on the last' and 'trapezoid on the first + last N-2')."""

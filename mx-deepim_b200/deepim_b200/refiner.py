@@ -242,6 +242,37 @@ class PoseRefiner:
         been tuned.
         Returns host arrays: poses [n_iter,N,3,4] float64, inliers [n_iter,N] int32, rms [n_iter,N] float32 and status
         [n_iter,N] int32 (see Context.icp)."""
+        n = len(cls_idx)
+        poses = np.asarray(poses, np.float64)
+        out = {"poses": np.zeros((n_iter, n, 3, 4)), "inliers": np.zeros((n_iter, n), np.int32),
+               "rms": np.zeros((n_iter, n), np.float32), "status": np.zeros((n_iter, n), np.int32)}
+
+        def call(ctx, dev, depth, cls, a, b, K, local):
+            return ctx.icp(depth, cls, dev(poses[a:b]), K, n_iter, max_dist, min_points, local)
+
+        return self._depth_batches(depths_u16, cls_idx, K_frames, frame_of, out, 1, call)
+
+    def vsd(self, depths_u16, cls_idx, poses_est, poses_gt, K_frames=None, frame_of=None, delta=0.015, taus=(0.02,)):
+        """Visible Surface Discrepancy of poses_est against poses_gt (Context.pose_error_vsd, dim_pose_error_vsd), batched
+        and pipelined exactly as icp(): depths_u16, cls_idx, K_frames and frame_of as there, poses_est / poses_gt [N,3,4]
+        float64 host; delta and taus in metres (the defaults are the SIXD Challenge 2017's 15 mm and 20 mm).
+        Returns host arrays: err [N,n_tau] float64 and status [N] int32 (see Context.pose_error_vsd)."""
+        n = len(cls_idx)
+        poses_est, poses_gt = np.asarray(poses_est, np.float64), np.asarray(poses_gt, np.float64)
+        taus = np.asarray(taus, np.float64).reshape(-1)
+        out = {"err": np.zeros((n, len(taus))), "status": np.zeros(n, np.int32)}
+
+        def call(ctx, dev, depth, cls, a, b, K, local):
+            return ctx.pose_error_vsd(depth, cls, dev(poses_est[a:b]), dev(poses_gt[a:b]), K, delta, taus, local,
+                                      self.zn, self.zf)
+
+        return self._depth_batches(depths_u16, cls_idx, K_frames, frame_of, out, 0, call)
+
+    def _depth_batches(self, depths_u16, cls_idx, K_frames, frame_of, out, axis, call):
+        """icp / vsd over refine_frames()'s device batches (plan_frame_batches), pipelined over the slots: per batch the
+        u16 depth of its frames is converted on the device, call(ctx, dev, depth, cls, a, b, K, local) enqueues the
+        operation for instances a..b-1 on the slot's stream and returns its CUDA tensors, and out[key] receives them at
+        [a:b] along `axis`.  Returns out."""
         depths_u16 = np.asarray(depths_u16, np.uint16)
         n = len(cls_idx)
         if frame_of is None:
@@ -250,16 +281,14 @@ class PoseRefiner:
             frame_of = np.arange(n)
         elif len(frame_of) != n:
             raise ValueError("frame_of has %d entries for %d instances" % (len(frame_of), n))
-        cls_idx, poses = np.asarray(cls_idx, np.int32), np.asarray(poses, np.float64)
-        out = {"poses": np.zeros((n_iter, n, 3, 4)), "inliers": np.zeros((n_iter, n), np.int32),
-               "rms": np.zeros((n_iter, n), np.float32), "status": np.zeros((n_iter, n), np.int32)}
+        cls_idx = np.asarray(cls_idx, np.int32)
         pending = []
 
         def collect(i, a, b, res):
             self.slots[i]["stream"].synchronize()
             self.slots[i]["busy"] = False
             for k in out:
-                out[k][:, a:b] = res[k].numpy()
+                out[k][(slice(None),) * axis + (slice(a, b),)] = res[k].numpy()
 
         for a, b, frames, local, *k in plan_frame_batches(frame_of, len(depths_u16), self.max_batch, 0, n, K_frames):
             if len(pending) == len(self.slots):
@@ -272,8 +301,7 @@ class PoseRefiner:
             with torch.cuda.stream(slot["stream"]):
                 dev = lambda x: torch.from_numpy(np.ascontiguousarray(x)).to(ctx.device, non_blocking=True)
                 depth = ctx.depth_from_u16(dev(depths_u16[frames]), self.depth_factor)
-                r = ctx.icp(depth, dev(cls_idx[a:b]), dev(poses[a:b]), k[0] if k else self.K, n_iter, max_dist, min_points,
-                            dev(local))
+                r = call(ctx, dev, depth, dev(cls_idx[a:b]), a, b, k[0] if k else self.K, dev(local))
                 res = {key: torch.empty(v.shape, dtype=v.dtype).pin_memory().copy_(v, non_blocking=True)
                        for key, v in r.items()}
             slot["busy"] = True
