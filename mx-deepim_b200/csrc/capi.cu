@@ -18,6 +18,20 @@ void set_error(const char *fmt, ...) {
   va_end(ap);
 }
 
+int prof_begin(dim_ctx *ctx, cudaStream_t st, cudaEvent_t **ev) {
+  *ev = nullptr;
+  if (!ctx->prof) return 0;
+  while (ctx->prof_events.size() < ctx->prof_used + 5) {
+    cudaEvent_t e;
+    DIM_CHECK(cudaEventCreate(&e));
+    ctx->prof_events.push_back(e);
+  }
+  *ev = &ctx->prof_events[ctx->prof_used];
+  ctx->prof_used += 5;
+  DIM_CHECK(cudaEventRecord((*ev)[0], st));
+  return 0;
+}
+
 }  // namespace dim
 
 using namespace dim;
@@ -142,8 +156,10 @@ DIM_API int32_t dim_render(dim_ctx *ctx, const int32_t *cls_idx, const float *po
                            float zn, float zf, const double *means, int32_t trunc_u8, float *out_image,
                            float *out_depth, float *out_mask, float *out_bgr, int32_t *out_bbox, void *stream) {
   DIM_REQUIRE(ctx && cls_idx && pose && K9, "dim_render: NULL argument");
-  return render_launch(ctx, cls_idx, pose, B, K9, zn, zf, means, trunc_u8, out_image, out_depth, out_mask, out_bgr,
-                       out_bbox, nullptr, (cudaStream_t)stream);
+  return render_launch(ctx, cls_idx, pose, B, zn, zf, means,
+                       {.cams = frame_cams(K9), .out_image = out_image, .out_depth = out_depth, .out_mask = out_mask,
+                        .out_bgr = out_bgr, .out_bbox = out_bbox, .trunc_u8 = trunc_u8},
+                       (cudaStream_t)stream);
 }
 
 // lit renderer (lib/render_glumpy/render_py_light_modelnet_multi.py)
@@ -199,8 +215,10 @@ DIM_API int32_t dim_render_lit(dim_ctx *ctx, const int32_t *cls_idx, const float
   DIM_REQUIRE(ctx && cls_idx && pose && K9 && light_pos && light_int, "dim_render_lit: NULL argument");
   if (int rc = normals_check(ctx, "dim_render_lit")) return rc;
   const LitParams lit = lit_params(light_pos, light_int, brightness_ratio);
-  return render_launch(ctx, cls_idx, pose, B, K9, zn, zf, means, 1, out_image, out_depth, out_mask, out_bgr, out_bbox, nullptr,
-                       (cudaStream_t)stream, &lit);
+  return render_launch(ctx, cls_idx, pose, B, zn, zf, means,
+                       {.cams = frame_cams(K9), .out_image = out_image, .out_depth = out_depth, .out_mask = out_mask,
+                        .out_bgr = out_bgr, .out_bbox = out_bbox, .trunc_u8 = 1, .lit = &lit},
+                       (cudaStream_t)stream);
 }
 
 // data-preparation render (toolkit/LM6d_ds_1, ds_2, ds_4, LM6d_0): Render_Py_Light and Render_Py outputs of one pass
@@ -488,21 +506,12 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
   // image-only network (ZoomImage): both boxes come from the colours; the observed one once per call and frame
   const bool mask = net_input_mask(ctx);
   if (!mask)
-    if (int rc = obs_colour_box_launch(ctx, a.obs4, a.n_frames, ctx->bbox_obs, st)) return rc;
+    if (int rc = obs_colour_box_launch(ctx, a.obs4, a.cams.n_frames, ctx->bbox_obs, st)) return rc;
   const double *pose_src = a.pose_init;
   for (int it = 0; it < a.n_iter; ++it) {
     DimNvtxRange r_it("dim_refine iteration");
-    cudaEvent_t *ev = nullptr;
-    if (ctx->prof) {
-      while (ctx->prof_events.size() < ctx->prof_used + 5) {
-        cudaEvent_t e;
-        DIM_CHECK(cudaEventCreate(&e));
-        ctx->prof_events.push_back(e);
-      }
-      ev = &ctx->prof_events[ctx->prof_used];
-      ctx->prof_used += 5;
-      DIM_CHECK(cudaEventRecord(ev[0], st));
-    }
+    cudaEvent_t *ev;
+    if (int rc = prof_begin(ctx, st, &ev)) return rc;
     if (a.pose_override) pose_src = a.pose_override + (size_t)it * a.B * 12;
     // src_pose blob is float32 (nd.array), the host pose stays float64 (tester.py:391); the lit chain also derives the
     // light of this iteration's render from the float64 pose
@@ -517,9 +526,10 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
       DimNvtxRange r("render");
       const LitParams lp = a.lit ? lit_params(ctx->light_pos, a.intensity + (size_t)it * a.B * 3, a.brightness_ratio)
                                  : LitParams{nullptr, nullptr, 0.f, 0.f};
-      if (int rc = render_launch(ctx, a.cls_idx, ctx->pose_cur_f32, a.B, a.K9, a.zn, a.zf, a.means, 1, nullptr, nullptr,
-                                 nullptr, nullptr, nullptr, ctx->ren4, st, a.lit ? &lp : nullptr, depth, !mask, a.K_frames,
-                                 a.frame_idx, a.n_frames))
+      if (int rc = render_launch(ctx, a.cls_idx, ctx->pose_cur_f32, a.B, a.zn, a.zf, a.means,
+                                 {.cams = a.cams, .out_ren4 = ctx->ren4, .trunc_u8 = 1, .lit = a.lit ? &lp : nullptr,
+                                  .ren4_depth = depth, .colour_box = !mask},
+                                 st))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[1], st));
@@ -532,16 +542,16 @@ static int refine_core(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
       DimNvtxRange r("bbox + zoom");
       int *status_it = ctx->status_hist + (size_t)(it < 8 ? it : 7) * a.B;
       if (mask) {
-        if (int rc = zoom_factor_from_ren_launch(ctx, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it, bbox_it, status_it, st,
-                                                 a.frame_idx, a.n_frames, a.K_frames))
+        if (int rc = zoom_factor_from_ren_launch(ctx, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.cams, zf_it, bbox_it, status_it,
+                                                 st))
           return rc;
-      } else if (int rc = zoom_factor_from_boxes_launch(ctx, ctx->bbox_obs, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.K9, zf_it,
-                                                        bbox_it, status_it, st, a.frame_idx, a.n_frames, a.K_frames)) {
+      } else if (int rc = zoom_factor_from_boxes_launch(ctx, ctx->bbox_obs, ctx->bbox_ren, ctx->pose_cur_f32, a.B, a.cams,
+                                                        zf_it, bbox_it, status_it, st)) {
         return rc;
       }
       if (int rc = zoom_fused_launch(ctx, a.obs4, ctx->ren4, zf_it, means_f, a.B, rows, cols, pad, hi,
                                      a.precision == DIM_PREC_BF16X3 ? lo : nullptr, st, a.precision == DIM_PREC_FP16, a.means,
-                                     depth, mask, a.frame_idx, a.n_frames))
+                                     depth, mask, a.cams))
         return rc;
     }
     if (ev) DIM_CHECK(cudaEventRecord(ev[2], st));
@@ -606,13 +616,12 @@ static int refine_graphed(dim_ctx *ctx, const RefineArgs &a, cudaStream_t st) {
   return 0;
 }
 
-// the loop's host values; the caller sets the pointers (lit: nullptr = unlit; K9 nullptr = per-frame intrinsics, K9 all zero
-// so that the graph key holds only the K_frames pointer)
-static RefineArgs refine_args(int32_t B, int32_t n_iter, const float *K9, float zn, float zf, const double *means,
+// the loop's host values; the caller sets the pointers (lit: nullptr = unlit)
+static RefineArgs refine_args(int32_t B, int32_t n_iter, const FrameCams &cams, float zn, float zf, const double *means,
                               int32_t precision, const dim_lighting *lit) {
   RefineArgs a{};
   a.B = B; a.n_iter = n_iter; a.precision = precision; a.zn = zn; a.zf = zf;
-  if (K9) memcpy(a.K9, K9, sizeof(a.K9));
+  a.cams = cams;
   memcpy(a.means, means, sizeof(a.means));
   if (lit) {
     a.lit = 1;
@@ -628,53 +637,18 @@ static int refuse(const char *fn, const char *msg) {
   return 2;
 }
 
-// the argument checks both loop entries share; fn names the entry in every message.  host: dim_refine_host_async (its
-// depth argument's name, n_iter <= 8).  A NULL frame_idx means instance b observes frame b, so F must equal B.
-static int refine_check(dim_ctx *ctx, const char *fn, bool host, const void *frames, int32_t F, const int32_t *frame_idx,
-                        const float *K9, const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B,
-                        int32_t n_iter, const double *means, const void *poses, const void *depth,
-                        const dim_lighting *lighting) {
-  if (!(ctx && frames && cls_idx && pose_init && means && poses)) return refuse(fn, "NULL argument");
-  if (!K9 == !K_frames)
-    return refuse(fn, host ? "exactly one of K9_host and K_frames_host must be non-NULL"
-                           : "exactly one of K9_host and K_frames must be non-NULL");
-  if (int rc = depth_check(ctx, depth, depth, fn, host ? "depth_frames_u16_host" : "depth_frames")) return rc;
-  if (int rc = lit_check(ctx, lighting, fn)) return rc;
+// the frame batch of every entry that works against observed frames: exactly one of K9_host and the per-frame cameras
+// (K_frames_arg names them), B and F in [1, max_batch], and F == B without a frame map (instance b then observes frame b)
+static int frames_check(dim_ctx *ctx, const char *fn, const float *K9_host, const void *K_frames, const char *K_frames_arg,
+                        int32_t B, int32_t F, const int32_t *frame_idx) {
+  if (!K9_host == !K_frames) {
+    set_error("%s: exactly one of K9_host and %s must be non-NULL", fn, K_frames_arg);
+    return 2;
+  }
   if (B < 1 || B > ctx->max_batch) return refuse(fn, "batch exceeds max_batch");
   if (F < 1 || F > ctx->max_batch) return refuse(fn, "frame count F outside [1, max_batch]");
   if (!frame_idx && F != B) return refuse(fn, "frame_idx is NULL (instance b observes frame b): F must equal B");
-  if (host ? (n_iter < 1 || n_iter > 8) : n_iter < 1)
-    return refuse(fn, host ? "n_iter must be in [1,8]" : "n_iter must be >= 1");
   return 0;
-}
-
-// dim_refine once the arguments are checked: the F observed frames (and their depths) packed into obs4 outside the graph,
-// then the chain
-static int refine_device(dim_ctx *ctx, RefineArgs &a, const float *frames, int32_t F, const int32_t *frame_idx,
-                         const float *depth, cudaStream_t st) {
-  a.obs4 = ctx->obs4; a.frame_idx = frame_idx; a.n_frames = F;
-  // the graph never reads the depth: it is packed into obs4.w below, outside the graph, like the image, so a replay is
-  // correct whatever the key holds; keying on it only costs one capture per distinct depth buffer
-  a.depth_observed = depth;
-  if (int rc = pack_obs4_launch(ctx, frames, F, ctx->obs4, a.means, st)) return rc;
-  if (depth)
-    if (int rc = obs4_depth_launch(ctx, ctx->obs4, F, depth, nullptr, 0.f, st)) return rc;
-  return refine_graphed(ctx, a, st);
-}
-
-DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx, const float *K9,
-                           const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B, int32_t n_iter,
-                           float zn, float zf, const double *means, int32_t precision, const double *pose_override,
-                           double *poses, float *se3, float *zoom_factor, int32_t *bbox, const float *depth_frames,
-                           const dim_lighting *lighting, void *stream) {
-  if (int rc = refine_check(ctx, "dim_refine", false, image_frames, F, frame_idx, K9, K_frames, cls_idx, pose_init, B, n_iter,
-                            means, poses, depth_frames, lighting))
-    return rc;
-  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
-  a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
-  a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
-  a.K_frames = K_frames;
-  return refine_device(ctx, a, image_frames, F, frame_idx, depth_frames, (cudaStream_t)stream);
 }
 
 // why the host intrinsics K (row-major 3x3) are not a finite pinhole matrix [[fx, 0, cx], [0, fy, cy], [0, 0, 1]] with
@@ -686,6 +660,52 @@ static const char *pinhole_defect(const float *K) {
   if (K[1] != 0.f || K[3] != 0.f) return "K[0][1] (skew) and K[1][0] must be 0";
   if (K[6] != 0.f || K[7] != 0.f || K[8] != 1.f) return "the last row must be (0, 0, 1)";
   return nullptr;
+}
+
+// K9_host, when given, is a finite pinhole matrix
+static int pinhole_check(const char *fn, const float *K9_host) {
+  if (K9_host)
+    if (const char *why = pinhole_defect(K9_host)) {
+      set_error("%s: K9_host is not a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]]: %s", fn, why);
+      return 2;
+    }
+  return 0;
+}
+
+// the argument checks both loop entries share; fn names the entry in every message.  host: dim_refine_host_async (its
+// argument names, n_iter <= 8).
+static int refine_check(dim_ctx *ctx, const char *fn, bool host, const void *frames, int32_t F, const int32_t *frame_idx,
+                        const float *K9, const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B,
+                        int32_t n_iter, const double *means, const void *poses, const void *depth,
+                        const dim_lighting *lighting) {
+  if (!(ctx && frames && cls_idx && pose_init && means && poses)) return refuse(fn, "NULL argument");
+  if (int rc = frames_check(ctx, fn, K9, K_frames, host ? "K_frames_host" : "K_frames", B, F, frame_idx)) return rc;
+  if (int rc = depth_check(ctx, depth, depth, fn, host ? "depth_frames_u16_host" : "depth_frames")) return rc;
+  if (int rc = lit_check(ctx, lighting, fn)) return rc;
+  if (host ? (n_iter < 1 || n_iter > 8) : n_iter < 1)
+    return refuse(fn, host ? "n_iter must be in [1,8]" : "n_iter must be >= 1");
+  return 0;
+}
+
+DIM_API int32_t dim_refine(dim_ctx *ctx, const float *image_frames, int32_t F, const int32_t *frame_idx, const float *K9,
+                           const float *K_frames, const int32_t *cls_idx, const double *pose_init, int32_t B, int32_t n_iter,
+                           float zn, float zf, const double *means, int32_t precision, const double *pose_override,
+                           double *poses, float *se3, float *zoom_factor, int32_t *bbox, const float *depth_frames,
+                           const dim_lighting *lighting, void *stream) {
+  if (int rc = refine_check(ctx, "dim_refine", false, image_frames, F, frame_idx, K9, K_frames, cls_idx, pose_init, B, n_iter,
+                            means, poses, depth_frames, lighting))
+    return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  RefineArgs a = refine_args(B, n_iter, frame_cams(K9, K_frames, frame_idx, F), zn, zf, means, precision, lighting);
+  a.obs4 = ctx->obs4; a.cls_idx = cls_idx; a.pose_init = pose_init; a.pose_override = pose_override;
+  a.poses = poses; a.se3 = se3; a.zoom_factor = zoom_factor; a.bbox = bbox;
+  // the F observed frames (and their depths) are packed into obs4 outside the graph.  The graph never reads the depth, so
+  // a replay is correct whatever the key holds; keying on it only costs one capture per distinct depth buffer
+  a.depth_observed = depth_frames;
+  if (int rc = pack_obs4_launch(ctx, image_frames, F, ctx->obs4, a.means, st)) return rc;
+  if (depth_frames)
+    if (int rc = obs4_depth_launch(ctx, ctx->obs4, F, depth_frames, nullptr, 0.f, st)) return rc;
+  return refine_graphed(ctx, a, st);
 }
 
 // dim_refine_host_async once its scalar arguments are checked: the class and frame indices (and intrinsics) are checked
@@ -723,11 +743,11 @@ static int refine_host_enqueue(dim_ctx *ctx, const char *fn, const uint8_t *fram
   DIM_CHECK(cudaMemcpyAsync(ctx->pose_cur, pose_host, sizeof(double) * B * 12, cudaMemcpyHostToDevice, st));
   if (frame_host) DIM_CHECK(cudaMemcpyAsync(ctx->frame_dev, frame_host, sizeof(int) * B, cudaMemcpyHostToDevice, st));
   if (K_host) DIM_CHECK(cudaMemcpyAsync(ctx->K_dev, K_host, sizeof(float) * 9 * F, cudaMemcpyHostToDevice, st));
-  RefineArgs a = refine_args(B, n_iter, K9, zn, zf, means, precision, lighting);
-  a.K_frames = K_host ? ctx->K_dev : nullptr;
+  RefineArgs a = refine_args(B, n_iter,
+                             frame_cams(K9, K_host ? ctx->K_dev : nullptr, frame_host ? ctx->frame_dev : nullptr, F), zn, zf,
+                             means, precision, lighting);
   a.obs4 = ctx->obs4; a.cls_idx = ctx->cls_dev; a.pose_init = ctx->pose_cur; a.poses = ctx->poses_dev;
   a.se3 = ctx->se3_hist_dev;
-  a.frame_idx = frame_host ? ctx->frame_dev : nullptr; a.n_frames = F;
   if (lighting) {  // the intensities move to the context's buffer (a fixed address: graphs)
     a.intensity = ctx->lit_intensity;
     DIM_CHECK(cudaMemcpyAsync(ctx->lit_intensity, lighting->intensity, sizeof(float) * (size_t)n_iter * B * 3,
@@ -769,20 +789,13 @@ DIM_API int32_t dim_icp(dim_ctx *ctx, const float *depth_frames, int32_t F, cons
                         float *rms, int32_t *status, void *stream) {
   const char *fn = "dim_icp";
   if (!(ctx && depth_frames && cls_idx && pose_in && poses_out && inliers && rms && status)) return refuse(fn, "NULL argument");
-  if (!K9_host == !K_frames) return refuse(fn, "exactly one of K9_host and K_frames must be non-NULL");
-  if (B < 1 || B > ctx->max_batch) return refuse(fn, "batch exceeds max_batch");
-  if (F < 1 || F > ctx->max_batch) return refuse(fn, "frame count F outside [1, max_batch]");
-  if (!frame_idx && F != B) return refuse(fn, "frame_idx is NULL (instance b observes frame b): F must equal B");
+  if (int rc = frames_check(ctx, fn, K9_host, K_frames, "K_frames", B, F, frame_idx)) return rc;
   if (n_iter < 1) return refuse(fn, "n_iter must be >= 1");
   if (!(max_dist > 0.f && max_dist < 3.0e38f)) return refuse(fn, "max_dist must be positive and finite");
   if (min_points < 6) return refuse(fn, "min_points must be >= 6 (six pose parameters)");
-  if (K9_host)
-    if (const char *why = pinhole_defect(K9_host)) {
-      set_error("%s: K9_host is not a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]]: %s", fn, why);
-      return 2;
-    }
-  const IcpCall c{depth_frames, F, frame_idx, K9_host, K_frames, cls_idx, pose_in, B, n_iter, znear, zfar, max_dist,
-                  min_points, poses_out, inliers, status, rms};
+  if (int rc = pinhole_check(fn, K9_host)) return rc;
+  const IcpCall c{depth_frames, frame_cams(K9_host, K_frames, frame_idx, F), cls_idx, pose_in, B, n_iter, znear, zfar,
+                  max_dist, min_points, poses_out, inliers, status, rms};
   return icp_launch(ctx, c, (cudaStream_t)stream);
 }
 
@@ -795,21 +808,14 @@ DIM_API int32_t dim_pose_error_vsd(dim_ctx *ctx, const float *depth_frames, int3
                                    const double *taus_host, int32_t n_tau, double *err, int32_t *status, void *stream) {
   const char *fn = "dim_pose_error_vsd";
   if (!(ctx && depth_frames && cls_idx && poses_est && poses_gt && taus_host && err)) return refuse(fn, "NULL argument");
-  if (!K9_host == !K_frames) return refuse(fn, "exactly one of K9_host and K_frames must be non-NULL");
-  if (B < 1 || B > ctx->max_batch) return refuse(fn, "batch exceeds max_batch");
-  if (F < 1 || F > ctx->max_batch) return refuse(fn, "frame count F outside [1, max_batch]");
-  if (!frame_idx && F != B) return refuse(fn, "frame_idx is NULL (instance b observes frame b): F must equal B");
+  if (int rc = frames_check(ctx, fn, K9_host, K_frames, "K_frames", B, F, frame_idx)) return rc;
   if (n_tau < 1 || n_tau > VSD_MAX_TAU) return refuse(fn, "n_tau must be in [1,16]");
   if (!(delta > 0.f && delta < 3.0e38f)) return refuse(fn, "delta must be positive and finite");
   for (int32_t k = 0; k < n_tau; ++k)
     if (!(taus_host[k] > 0.0 && taus_host[k] < 1.0e308)) return refuse(fn, "every tau must be positive and finite");
-  if (K9_host)
-    if (const char *why = pinhole_defect(K9_host)) {
-      set_error("%s: K9_host is not a finite pinhole matrix [[fx,0,cx],[0,fy,cy],[0,0,1]]: %s", fn, why);
-      return 2;
-    }
-  const VsdCall c{depth_frames, F, frame_idx, K9_host, K_frames, cls_idx, poses_est, poses_gt, B, znear, zfar, delta,
-                  taus_host, n_tau, err, status};
+  if (int rc = pinhole_check(fn, K9_host)) return rc;
+  const VsdCall c{depth_frames, frame_cams(K9_host, K_frames, frame_idx, F), cls_idx, poses_est, poses_gt, B, znear, zfar,
+                  delta, taus_host, n_tau, err, status};
   return vsd_launch(ctx, c, (cudaStream_t)stream);
 }
 
@@ -857,8 +863,10 @@ DIM_API int32_t dim_train_update(dim_ctx *ctx, const int32_t *cls_idx, const flo
                         (float)K9[5], (float)K9[6], (float)K9[7], (float)K9[8]};
   // no uint8 truncation on the train path (batch_updater_py_multi.py:184,234); the lit colours are already 8-bit quantised
   const LitParams lp = lit ? lit_params(ctx->light_pos, lit->intensity, lit->brightness_ratio) : LitParams{nullptr, nullptr, 0.f, 0.f};
-  if (int rc = render_launch(ctx, cls_idx, src_pose_new, B, K9f, zn, zf, means, 0, image_rendered, depth_rendered,
-                             mask_rendered, nullptr, nullptr, nullptr, st, lit ? &lp : nullptr))
+  if (int rc = render_launch(ctx, cls_idx, src_pose_new, B, zn, zf, means,
+                             {.cams = frame_cams(K9f), .out_image = image_rendered, .out_depth = depth_rendered,
+                              .out_mask = mask_rendered, .trunc_u8 = 0, .lit = lit ? &lp : nullptr},
+                             st))
     return rc;
   if (flow && flow_weights) {
     DIM_REQUIRE(depth_gt_observed != nullptr, "dim_train_update: flow labels need depth_gt_observed");

@@ -76,28 +76,56 @@ struct MeshDev {
 
 struct NetState;  // net_state.cuh
 
-// The observed frame of instance b in the fused loop (dim_refine's frame map): frame_idx[b], or frame 0 when that lies outside
-// [0, n_frames) -- a bad index never reads outside the packed frames (or the per-frame intrinsics); the zoom factor flags it
-// as status bit 3.  frame_idx == nullptr: instance b observes frame b (no frame map).
-__device__ __forceinline__ int frame_of(const int32_t *frame_idx, int n_frames, int b) {
-  if (!frame_idx) return b;
-  const int f = __ldg(frame_idx + b);
-  return (f >= 0 && f < n_frames) ? f : 0;
-}
-__device__ __forceinline__ bool frame_bad(const int32_t *frame_idx, int n_frames, int b) {
-  if (!frame_idx) return false;
-  const int f = __ldg(frame_idx + b);
-  return f < 0 || f >= n_frames;
+// A frame batch: B instances, instance b observing frame frame(b) of n_frames through the camera pinhole(b).  Every kernel
+// that renders, zooms or compares against observed frames reads its frame map and cameras through this one type.
+struct FrameCams {
+  const int32_t *frame_idx;  // device [B]: the frame instance b observes; nullptr = frame b (no frame map)
+  const float *K_frames;     // device [n_frames,9]: the camera of every frame; nullptr = K9 for every instance
+  int32_t n_frames;
+  float K9[9];               // the one camera, row-major; all zero when K_frames is given (RefineArgs keys on the pointer)
+
+  // frame_idx[b], or frame 0 when that lies outside [0, n_frames): a bad index never reads outside the frames (or the
+  // per-frame intrinsics); bad(b) flags it, as status bit 3
+  __device__ __forceinline__ int frame(int b) const {
+    if (!frame_idx) return b;
+    const int f = __ldg(frame_idx + b);
+    return (f >= 0 && f < n_frames) ? f : 0;
+  }
+  __device__ __forceinline__ bool bad(int b) const {
+    if (!frame_idx) return false;
+    const int f = __ldg(frame_idx + b);
+    return f < 0 || f >= n_frames;
+  }
+  // the camera of instance b, all nine values
+  __device__ __forceinline__ void K(int b, float k[9]) const {
+    const float *r = K_frames ? K_frames + 9 * frame(b) : nullptr;
+#pragma unroll
+    for (int e = 0; e < 9; ++e) k[e] = r ? __ldg(r + e) : K9[e];
+  }
+  // (fx, fy, cx, cy) of instance b
+  __device__ __forceinline__ float4 pinhole(int b) const {
+    float k[9];
+    K(b, k);
+    return make_float4(k[0], k[4], k[2], k[5]);
+  }
+};
+static_assert(sizeof(FrameCams) == 2 * sizeof(void *) + sizeof(int32_t) + 9 * sizeof(float), "FrameCams has no padding");
+
+// host: the FrameCams of one camera K9 (K_frames nullptr), or of per-frame cameras K_frames (K9 ignored, left all zero)
+static inline FrameCams frame_cams(const float *K9, const float *K_frames = nullptr, const int32_t *frame_idx = nullptr,
+                                   int n_frames = 0) {
+  FrameCams c{frame_idx, K_frames, n_frames, {}};
+  if (!K_frames)
+    for (int e = 0; e < 9; ++e) c.K9[e] = K9[e];
+  return c;
 }
 
 // Everything the fused refinement loop reads from its caller, and the key of its CUDA graphs, compared byte for byte (so
 // no padding).  Not in the key, because drop_graphs discards every graph when they change: ctx->cfg (trans means / stds,
 // rot_coord), mesh uploads, network weights and the "graph" option.
 struct RefineArgs {
-  const float4 *obs4;        // n_frames observed frames
-  const int32_t *frame_idx;  // device [B]: the frame instance b observes (read at replay); nullptr = frame b (no frame map)
-  const float *K_frames;     // device [n_frames,9]: the camera of every frame (read at replay; K9 is then all zero);
-                             // nullptr = K9 for every instance
+  const float4 *obs4;  // cams.n_frames observed frames (dim_refine without a frame map: B)
+  FrameCams cams;      // frame_idx and K_frames are read at replay
   const int32_t *cls_idx;
   const double *pose_init, *pose_override;  // pose_override: nullable [n_iter,B,3,4] source pose of every iteration
   double *poses;
@@ -106,12 +134,12 @@ struct RefineArgs {
   const float *intensity;    // lit: device [n_iter,B,3]; unlit: nullptr
   const float *depth_observed;  // RGB-D network, dim_refine: the caller's device depth; otherwise nullptr
   double means[3], offset[3];  // offset: the light's (lit only)
-  float K9[9], zn, zf, brightness_ratio;
+  float zn, zf, brightness_ratio;
   int32_t B, n_iter, precision, lit;
-  int32_t n_frames;  // frames in obs4 (dim_refine: B)
-  int32_t zero;      // always 0: fills what would otherwise be tail padding
+  int32_t zero;  // always 0: fills what would otherwise be tail padding
 };
-static_assert(sizeof(RefineArgs) == 12 * sizeof(void *) + 6 * sizeof(double) + 12 * sizeof(float) + 6 * sizeof(int32_t),
+static_assert(sizeof(RefineArgs) ==
+                  10 * sizeof(void *) + sizeof(FrameCams) + 6 * sizeof(double) + 3 * sizeof(float) + 5 * sizeof(int32_t),
               "RefineArgs must have no padding: its bytes are the graph key");
 
 }  // namespace dim

@@ -26,15 +26,14 @@ struct IcpParams {
   const int *vbox;            // [B,4] x0, x1, y0, y1 (conservative box of the projected vertices)
   const int *cls_flag;        // [B] 2 = bad class
   const float *depth;         // [F,H,W] observed, metres
-  const int32_t *frame_idx;   // nullable: frame b
-  const float *K_frames;      // nullable: K9 for every instance
+  FrameCams cams;
   const double *pose0;        // [B,3,4] the call's input pose
   double *partial;            // [B][chunks][ICP_SLOT]
   double *poses;              // [n_iter,B,3,4]
   int32_t *inliers, *status;  // [n_iter,B]
   float *rms;                 // [n_iter,B]
-  float fx, fy, cx, cy, max_dist;
-  int B, H, W, n_frames, chunks, min_points;
+  float max_dist;
+  int B, H, W, chunks, min_points;
 };
 
 // the model pixels an instance may have: the interior of its vertex box within the frame's interior.  Pixels outside the
@@ -48,15 +47,6 @@ __device__ __forceinline__ Range model_range(const int *vbox, int b, int H, int 
   r.i0 = max(y0 + 1, 1); r.i1 = min(y1 - 1, H - 2);
   r.j0 = max(x0 + 1, 1); r.j1 = min(x1 - 1, W - 2);
   return r;
-}
-
-__device__ __forceinline__ void intrinsics(const IcpParams &p, int b, double &fx, double &fy, double &cx, double &cy) {
-  if (p.K_frames) {
-    const float *k = p.K_frames + 9 * frame_of(p.frame_idx, p.n_frames, b);
-    fx = (double)k[0]; cx = (double)k[2]; fy = (double)k[4]; cy = (double)k[5];
-  } else {
-    fx = (double)p.fx; fy = (double)p.fy; cx = (double)p.cx; cy = (double)p.cy;
-  }
 }
 
 __global__ void __launch_bounds__(ICP_THREADS) icp_assoc_kernel(IcpParams p, const double *pose_k) {
@@ -77,12 +67,12 @@ __global__ void __launch_bounds__(ICP_THREADS) icp_assoc_kernel(IcpParams p, con
   double R[12];
 #pragma unroll
   for (int k = 0; k < 12; ++k) R[k] = sRt[k];
-  double fx, fy, cx, cy;
-  intrinsics(p, b, fx, fy, cx, cy);
+  const float4 k = p.cams.pinhole(b);
+  const double fx = (double)k.x, fy = (double)k.y, cx = (double)k.z, cy = (double)k.w;
   const double md = (double)p.max_dist;
   const size_t P = (size_t)p.H * p.W;
   const float4 *ren = p.ren4 + (size_t)b * P;
-  const float *obs = p.depth + (size_t)frame_of(p.frame_idx, p.n_frames, b) * P;
+  const float *obs = p.depth + (size_t)p.cams.frame(b) * P;
 
   double acc[ICP_SLOT];
 #pragma unroll
@@ -216,7 +206,7 @@ __global__ void icp_solve_kernel(IcpParams p, const double *pose_k, int it) {
       const double *slot = p.partial + ((size_t)b * p.chunks + ch) * ICP_SLOT;
       for (int k = 0; k < ICP_SLOT; ++k) S[k] += slot[k];
     }
-  int st = (p.cls_flag[b] ? 2 : 0) | (frame_bad(p.frame_idx, p.n_frames, b) ? 8 : 0);
+  int st = (p.cls_flag[b] ? 2 : 0) | (p.cams.bad(b) ? 8 : 0);
   const double *Pk = pose_k + 12 * b;
   double *out = p.poses + ((size_t)it * p.B + b) * 12;
   double x[6];
@@ -253,34 +243,23 @@ int depth_u16_launch(const uint16_t *in, size_t n, float factor, float *out, cud
 }
 
 int icp_launch(dim_ctx *ctx, const IcpCall &c, cudaStream_t st) {
-  static const float K_zero[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-  const float *K9 = c.K9 ? c.K9 : K_zero;
-  // stage profiling (dim_profile_enable): one record of 5 events per call, stage 0 = render, stage 1 = association + solve
-  cudaEvent_t *ev = nullptr;
-  if (ctx->prof) {
-    while (ctx->prof_events.size() < ctx->prof_used + 5) {
-      cudaEvent_t e;
-      DIM_CHECK(cudaEventCreate(&e));
-      ctx->prof_events.push_back(e);
-    }
-    ev = &ctx->prof_events[ctx->prof_used];
-    ctx->prof_used += 5;
-    DIM_CHECK(cudaEventRecord(ev[0], st));
-  }
+  // stage profiling: one record per call, stage 0 = render, stage 1 = association + solve
+  cudaEvent_t *ev;
+  if (int rc = prof_begin(ctx, st, &ev)) return rc;
   if (int rc = f64_to_f32_launch(c.pose_in, ctx->pose_cur_f32, c.B * 12, st)) return rc;
   {
     DimNvtxRange r("dim_icp render");
-    if (int rc = render_launch(ctx, c.cls_idx, ctx->pose_cur_f32, c.B, K9, c.zn, c.zf, nullptr, 1, nullptr, nullptr, nullptr,
-                               nullptr, nullptr, ctx->ren4, st, nullptr, true, false, c.K_frames, c.frame_idx, c.F))
+    if (int rc = render_launch(ctx, c.cls_idx, ctx->pose_cur_f32, c.B, c.zn, c.zf, nullptr,
+                               {.cams = c.cams, .out_ren4 = ctx->ren4, .trunc_u8 = 1, .ren4_depth = true}, st))
       return rc;
   }
   if (ev) DIM_CHECK(cudaEventRecord(ev[1], st));
   IcpParams p;
   p.ren4 = ctx->ren4; p.vbox = ctx->vbox; p.cls_flag = ctx->cls_flag; p.depth = c.depth;
-  p.frame_idx = c.frame_idx; p.K_frames = c.K_frames; p.pose0 = c.pose_in; p.partial = ctx->icp_partial;
+  p.cams = c.cams; p.pose0 = c.pose_in; p.partial = ctx->icp_partial;
   p.poses = c.poses_out; p.inliers = c.inliers; p.status = c.status; p.rms = c.rms;
-  p.fx = K9[0]; p.fy = K9[4]; p.cx = K9[2]; p.cy = K9[5]; p.max_dist = c.max_dist;
-  p.B = c.B; p.H = ctx->H; p.W = ctx->W; p.n_frames = c.F; p.chunks = cdiv(ctx->H, ICP_ROWS); p.min_points = c.min_points;
+  p.max_dist = c.max_dist;
+  p.B = c.B; p.H = ctx->H; p.W = ctx->W; p.chunks = cdiv(ctx->H, ICP_ROWS); p.min_points = c.min_points;
   DimNvtxRange r("dim_icp iterations");
   for (int it = 0; it < c.n_iter; ++it) {
     const double *pk = it == 0 ? c.pose_in : c.poses_out + (size_t)(it - 1) * c.B * 12;

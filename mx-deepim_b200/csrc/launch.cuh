@@ -20,14 +20,28 @@ struct TrainIO {
   const float *zdo, *zdr;  // RGB-D network: zoomed depth_observed / depth_rendered f32 [B,1,H,W]; nullptr otherwise
 };
 
+// capi.cu
+// stage profiling (dim_profile_enable): *ev = the call's next record of 5 events, its event 0 recorded on st, or nullptr
+// when profiling is off.  dim_profile_read adds the time from ev[k] to ev[k + 1] to stage k.
+int prof_begin(dim_ctx *ctx, cudaStream_t st, cudaEvent_t **ev);
+
 // raster.cu
-// K_frames / frame_idx / n_frames (fused loop, RefineArgs): instance b projects with row frame_of(b) of the per-frame
-// intrinsics [n_frames,9]; K_frames nullptr = K9 for every instance
-int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
-                  const double *means, int trunc_u8, float *out_image, float *out_depth, float *out_mask, float *out_bgr,
-                  int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit = nullptr, bool ren4_depth = false,
-                  bool colour_box = false, const float *K_frames = nullptr, const int32_t *frame_idx = nullptr,
-                  int n_frames = 0);
+// What one render_launch call draws: instance b projects with cams.pinhole(b); every output is nullable.
+struct RenderSpec {
+  FrameCams cams;
+  float *out_image;  // [B,3,H,W] RGB - means
+  float *out_depth, *out_mask;  // [B,H,W]
+  float *out_bgr;    // [B,H,W,3] the colours, BGR
+  int *out_bbox;     // [B,4] the mask's box (-1 when empty)
+  float4 *out_ren4;  // [B,H,W] the fused loop's (R,G,B,mask) image, RGB + means; written only inside the vertex box when
+                     // it is the only output
+  int trunc_u8;      // 1: colours truncated to uint8 and means subtracted in float64 (test path); 0: train path
+  const LitParams *lit;  // nullptr: unlit
+  bool ren4_depth;   // out_ren4.w holds the depth, not the mask (RGB-D network)
+  bool colour_box;   // the box is the colour-valid one, not the mask's (image-only network); not with ren4_depth
+};
+int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, float zn, float zf, const double *means,
+                  const RenderSpec &r, cudaStream_t st);
 // the data-preparation render (dim_render_dataset): file-ready outputs of one visibility pass, each nullable; ratio and the
 // light arrays of LitParams are per instance and used only for lit_bgr
 struct DatasetOut {
@@ -46,20 +60,16 @@ int zoom_gather_launch(dim_ctx *ctx, int mode, const float *src, float *dst, con
 int zoom_factor_launch(dim_ctx *ctx, const float *mask_real, const float *mask_ren, int C, const float *src_pose, int B,
                        const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
                        const float *img_means = nullptr);
-// frame_idx / n_frames: the fused loop's map from instance to observed frame (RefineArgs); nullptr = frame b
-// K_frames: the fused loop's per-frame intrinsics [n_frames,9] (RefineArgs); nullptr = K9 for every instance
-int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *src_pose, int B, const float *K9,
-                                float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
-                                const int32_t *frame_idx = nullptr, int n_frames = 0, const float *K_frames = nullptr);
+// cams: the fused loop's frame batch (RefineArgs)
+int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *src_pose, int B, const FrameCams &cams,
+                                float *zoom_factor, int *bbox_out, int *status, cudaStream_t st);
 int obs_colour_box_launch(dim_ctx *ctx, const float4 *obs4, int F, int *bbox_obs, cudaStream_t st);
 int zoom_factor_from_boxes_launch(dim_ctx *ctx, const int *bbox_obs, const int *bbox_ren, const float *src_pose, int B,
-                                  const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
-                                  const int32_t *frame_idx = nullptr, int n_frames = 0, const float *K_frames = nullptr);
+                                  const FrameCams &cams, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st);
 int box_mask_launch(dim_ctx *ctx, const int *bbox, int B, float *mask, cudaStream_t st);
 int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, const float *zoom_factor,
                       const float *means_rgb, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
-                      cudaStream_t st, int f16, const double *means_d, bool depth = false, bool mask = true,
-                      const int32_t *frame_idx = nullptr, int n_frames = 0);
+                      cudaStream_t st, int f16, const double *means_d, bool depth, bool mask, const FrameCams &cams);
 int obs4_depth_launch(dim_ctx *ctx, float4 *obs4, int B, const float *depth, const uint16_t *depth_u16, float factor,
                       cudaStream_t st);
 int pack_nhwc10_launch(dim_ctx *ctx, const float *io, const float *ir, const float *dobs, const float *dren, const float *mo,
@@ -115,10 +125,8 @@ int mask_dilate_launch(dim_ctx *ctx, const float *in, const int *draws, int B, f
 constexpr int ICP_ROWS = 8;   // frame rows per association CTA
 constexpr int ICP_SLOT = 30;  // doubles per CTA slot: A (21 upper entries), g (6), inliers, sum r^2, model pixels
 struct IcpCall {  // dim_icp's arguments, checked
-  const float *depth;  // [F,H,W] metres
-  int F;
-  const int32_t *frame_idx;
-  const float *K9, *K_frames;  // exactly one non-null
+  const float *depth;  // [cams.n_frames,H,W] metres
+  FrameCams cams;
   const int32_t *cls_idx;
   const double *pose_in;
   int B, n_iter;
@@ -136,10 +144,8 @@ constexpr int VSD_ROWS = 8;                     // frame rows per VSD pass CTA
 constexpr int VSD_MAX_TAU = 16;
 constexpr int VSD_SLOT = 2 + VSD_MAX_TAU;       // int32 per CTA slot: |union|, |inter|, c_tau
 struct VsdCall {  // dim_pose_error_vsd's arguments, checked
-  const float *depth;  // [F,H,W] metres
-  int F;
-  const int32_t *frame_idx;
-  const float *K9, *K_frames;  // exactly one non-null
+  const float *depth;  // [cams.n_frames,H,W] metres
+  FrameCams cams;
   const int32_t *cls_idx;
   const double *pose_est, *pose_gt;
   int B;

@@ -37,10 +37,8 @@ struct RasterParams {
   int max_verts, max_faces, H, W;
   int num_classes;  // size of the mesh table: class indices are range-checked on the device (mesh_for)
   int *cls_flag;    // [B] 0 ok / 2 = class index out of range or no mesh uploaded for it (renders nothing); nullable
-  float fx, fy, cx, cy, zn, zf;
-  const float *K_frames;     // fused loop, nullable: [n_frames,9] intrinsics; instance b projects with row frame_of(b) of them
-  const int32_t *frame_idx;  // instead of fx, fy, cx, cy (RefineArgs)
-  int n_frames;
+  FrameCams cams;  // instance b projects with cams.pinhole(b)
+  float zn, zf;
   double mean[3];
   float bg[3];  // (float)(0.0 - mean)
   int trunc_u8;
@@ -87,11 +85,8 @@ __global__ void __launch_bounds__(256) raster_vertex_kernel(RasterParams p) {
   if (p.cls_flag && v == 0) p.cls_flag[b] = m.V > 0 ? 0 : 2;
   const float *pose = p.pose + 12 * b;
   int ok = 0, X = 0, Y = 0;
-  float fx = p.fx, fy = p.fy, cx = p.cx, cy = p.cy;
-  if (p.K_frames) {
-    const float *k = p.K_frames + 9 * frame_of(p.frame_idx, p.n_frames, b);
-    fx = __ldg(k + 0); cx = __ldg(k + 2); fy = __ldg(k + 4); cy = __ldg(k + 5);
-  }
+  const float4 k = p.cams.pinhole(b);
+  const float fx = k.x, fy = k.y, cx = k.z, cy = k.w;
   if (v < m.V) {
     float x = m.verts[3 * v], y = m.verts[3 * v + 1], z = m.verts[3 * v + 2];
     float xc = ((pose[0] * x + pose[1] * y) + pose[2] * z) + pose[3];
@@ -536,37 +531,41 @@ static int raster_front(dim_ctx *ctx, const RasterParams &p, int B, cudaStream_t
   return 0;
 }
 
-int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const float *K9, float zn, float zf,
-                  const double *means, int trunc_u8, float *out_image, float *out_depth, float *out_mask,
-                  float *out_bgr, int *out_bbox, float4 *out_ren4, cudaStream_t st, const LitParams *lit, bool ren4_depth,
-                  bool colour_box, const float *K_frames, const int32_t *frame_idx, int n_frames) {
-  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_render: batch exceeds max_batch");
-  DIM_REQUIRE((ctx->W & 3) == 0, "dim_render: width must be a multiple of 4");
-  RasterParams p;
+// the RasterParams of every render; the caller fills what it outputs
+static RasterParams raster_params(dim_ctx *ctx, const int *cls, const float *pose, const FrameCams &cams, float zn, float zf) {
+  RasterParams p = {};
   p.meshes = ctx->meshes; p.cls = cls; p.pose = pose; p.pverts = ctx->pverts; p.vis = ctx->vis;
   p.vbox = ctx->vbox; p.bbox_ren = ctx->bbox_ren;
   p.max_verts = ctx->max_verts; p.max_faces = ctx->max_faces; p.H = ctx->H; p.W = ctx->W;
   p.num_classes = ctx->max_classes; p.cls_flag = ctx->cls_flag;
-  p.fx = K9[0]; p.fy = K9[4]; p.cx = K9[2]; p.cy = K9[5]; p.zn = zn; p.zf = zf;
-  p.K_frames = K_frames; p.frame_idx = frame_idx; p.n_frames = n_frames;
+  p.cams = cams; p.zn = zn; p.zf = zf;
+  return p;
+}
+
+int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, float zn, float zf, const double *means,
+                  const RenderSpec &r, cudaStream_t st) {
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_render: batch exceeds max_batch");
+  DIM_REQUIRE((ctx->W & 3) == 0, "dim_render: width must be a multiple of 4");
+  RasterParams p = raster_params(ctx, cls, pose, r.cams, zn, zf);
   for (int c = 0; c < 3; ++c) {
     p.mean[c] = means ? means[c] : 0.0;
-    p.bg[c] = trunc_u8 ? (float)(0.0 - p.mean[c]) : 0.0f - (float)p.mean[c];
+    p.bg[c] = r.trunc_u8 ? (float)(0.0 - p.mean[c]) : 0.0f - (float)p.mean[c];
   }
-  p.trunc_u8 = trunc_u8;
-  p.out_image = out_image; p.out_depth = out_depth; p.out_mask = out_mask; p.out_bgr = out_bgr;
-  p.out_ren4 = out_ren4;
-  p.ren4_box_only = (out_ren4 && !out_image && !out_depth && !out_mask && !out_bgr) ? 1 : 0;
-  p.lit = lit ? 1 : 0;
-  p.light_pos = lit ? lit->light_pos : nullptr; p.light_int = lit ? lit->light_int : nullptr;
-  p.a0 = lit ? lit->a0 : 0.f; p.a1 = lit ? lit->a1 : 0.f;
+  p.trunc_u8 = r.trunc_u8;
+  p.out_image = r.out_image; p.out_depth = r.out_depth; p.out_mask = r.out_mask; p.out_bgr = r.out_bgr;
+  p.out_ren4 = r.out_ren4;
+  p.ren4_box_only = (r.out_ren4 && !r.out_image && !r.out_depth && !r.out_mask && !r.out_bgr) ? 1 : 0;
+  if (const LitParams *lit = r.lit) {
+    p.lit = 1;
+    p.light_pos = lit->light_pos; p.light_int = lit->light_int; p.a0 = lit->a0; p.a1 = lit->a1;
+  }
   if (int rc = raster_front(ctx, p, B, st)) return rc;
   const dim3 rgrid(cdiv((ctx->W / 4) * ctx->H, 256), B);
-  DIM_REQUIRE(!(ren4_depth && colour_box), "dim_render: the colour bbox has no RGB-D variant");
-  if (colour_box) {
+  DIM_REQUIRE(!(r.ren4_depth && r.colour_box), "dim_render: the colour bbox has no RGB-D variant");
+  if (r.colour_box) {
     if (p.lit) raster_resolve_kernel<true, false, true><<<rgrid, 256, 0, st>>>(p);
     else raster_resolve_kernel<false, false, true><<<rgrid, 256, 0, st>>>(p);
-  } else if (ren4_depth) {
+  } else if (r.ren4_depth) {
     if (p.lit) raster_resolve_kernel<true, true><<<rgrid, 256, 0, st>>>(p);
     else raster_resolve_kernel<false, true><<<rgrid, 256, 0, st>>>(p);
   } else if (p.lit) {
@@ -575,7 +574,7 @@ int render_launch(dim_ctx *ctx, const int *cls, const float *pose, int B, const 
     raster_resolve_kernel<false><<<rgrid, 256, 0, st>>>(p);
   }
   DIM_LAUNCH_CHECK();
-  raster_finish_kernel<<<cdiv(B, 128), 128, 0, st>>>(ctx->bbox_ren, out_bbox, B);
+  raster_finish_kernel<<<cdiv(B, 128), 128, 0, st>>>(ctx->bbox_ren, r.out_bbox, B);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -584,12 +583,7 @@ int render_dataset_launch(dim_ctx *ctx, const int *cls, const float *pose, int B
                           const float *light_pos, const float *light_int, const DatasetOut &o, cudaStream_t st) {
   DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_render_dataset: batch exceeds max_batch");
   DIM_REQUIRE((ctx->W & 3) == 0, "dim_render_dataset: width must be a multiple of 4");
-  RasterParams p = {};
-  p.meshes = ctx->meshes; p.cls = cls; p.pose = pose; p.pverts = ctx->pverts; p.vis = ctx->vis;
-  p.vbox = ctx->vbox; p.bbox_ren = ctx->bbox_ren;
-  p.max_verts = ctx->max_verts; p.max_faces = ctx->max_faces; p.H = ctx->H; p.W = ctx->W;
-  p.num_classes = ctx->max_classes; p.cls_flag = ctx->cls_flag;
-  p.fx = K9[0]; p.fy = K9[4]; p.cx = K9[2]; p.cy = K9[5]; p.zn = zn; p.zf = zf;
+  RasterParams p = raster_params(ctx, cls, pose, frame_cams(K9), zn, zf);
   p.lit = o.lit_bgr ? 1 : 0;
   p.light_pos = light_pos; p.light_int = light_int;
   if (int rc = raster_front(ctx, p, B, st)) return rc;

@@ -25,14 +25,13 @@ struct VsdParams {
   const int *vbox_est, *vbox_gt;  // [B,4] x0, x1, y0, y1
   const int *cls_flag;       // [B] 2 = bad class
   const float *depth;        // [F,H,W] observed, metres
-  const int32_t *frame_idx;  // nullable: frame b
-  const float *K_frames;     // nullable: K9 for every instance
+  FrameCams cams;
   int32_t *partial;          // [B][chunks][VSD_SLOT]
   double *err;               // [B,n_tau]
   int32_t *status;           // [B], nullable
   double taus[VSD_MAX_TAU];
-  float fx, fy, cx, cy, delta;
-  int B, H, W, n_frames, chunks, n_tau;
+  float delta;
+  int B, H, W, chunks, n_tau;
 };
 
 struct Box { int i0, i1, j0, j1; };  // inclusive; empty when i1 < i0 or j1 < j0
@@ -68,18 +67,13 @@ __global__ void __launch_bounds__(VSD_THREADS) vsd_pass_kernel(VsdParams p) {
   const int r0 = max(ch * VSD_ROWS, rg.i0), r1 = min(ch * VSD_ROWS + VSD_ROWS - 1, rg.i1);
   if (r1 < r0 || rg.j1 < rg.j0) return;  // the finish reads only the slots of chunks that meet the range
   __shared__ int red[VSD_THREADS / 32][VSD_SLOT];
-  const int f = frame_of(p.frame_idx, p.n_frames, b);
-  float fx = p.fx, fy = p.fy, cxf = p.cx, cyf = p.cy;
-  if (p.K_frames) {
-    const float *k = p.K_frames + 9 * f;
-    fx = k[0]; cxf = k[2]; fy = k[4]; cyf = k[5];
-  }
-  const double rfx = (double)(1.0f / fx), rfy = (double)(1.0f / fy), cx = (double)cxf, cy = (double)cyf;
-  const int ex0 = p.vbox_est[4 * b], ex1 = p.vbox_est[4 * b + 1], ey0 = p.vbox_est[4 * b + 2], ey1 = p.vbox_est[4 * b + 3];
   const size_t P = (size_t)p.H * p.W;
+  const float *obs = p.depth + (size_t)p.cams.frame(b) * P;
+  const float4 k = p.cams.pinhole(b);
+  const double rfx = (double)(1.0f / k.x), rfy = (double)(1.0f / k.y), cx = (double)k.z, cy = (double)k.w;
+  const int ex0 = p.vbox_est[4 * b], ex1 = p.vbox_est[4 * b + 1], ey0 = p.vbox_est[4 * b + 2], ey1 = p.vbox_est[4 * b + 3];
   const float4 *ren = p.ren4 + (size_t)b * P;
   const float *dgt = p.depth_gt + (size_t)b * P;
-  const float *obs = p.depth + (size_t)f * P;
 
   int cnt[VSD_SLOT];
 #pragma unroll
@@ -133,44 +127,33 @@ __global__ void vsd_finish_kernel(VsdParams p) {
   double *e = p.err + (size_t)b * p.n_tau;
   for (int k = 0; k < p.n_tau; ++k) e[k] = S[0] ? ((double)S[2 + k] + (double)(S[0] - S[1])) / (double)S[0] : 1.0;
   if (p.status)
-    p.status[b] = (S[0] ? 0 : 1) | (p.cls_flag[b] ? 2 : 0) | (frame_bad(p.frame_idx, p.n_frames, b) ? 8 : 0);
+    p.status[b] = (S[0] ? 0 : 1) | (p.cls_flag[b] ? 2 : 0) | (p.cams.bad(b) ? 8 : 0);
 }
 
 int vsd_launch(dim_ctx *ctx, const VsdCall &c, cudaStream_t st) {
-  static const float K_zero[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-  const float *K9 = c.K9 ? c.K9 : K_zero;
-  // stage profiling (dim_profile_enable): one record of 5 events per call, stage 0 = the two renders, stage 1 = VSD pass
-  cudaEvent_t *ev = nullptr;
-  if (ctx->prof) {
-    while (ctx->prof_events.size() < ctx->prof_used + 5) {
-      cudaEvent_t e;
-      DIM_CHECK(cudaEventCreate(&e));
-      ctx->prof_events.push_back(e);
-    }
-    ev = &ctx->prof_events[ctx->prof_used];
-    ctx->prof_used += 5;
-    DIM_CHECK(cudaEventRecord(ev[0], st));
-  }
+  // stage profiling: one record per call, stage 0 = the two renders, stage 1 = VSD pass
+  cudaEvent_t *ev;
+  if (int rc = prof_begin(ctx, st, &ev)) return rc;
   {
     DimNvtxRange r("dim_pose_error_vsd render");
     if (int rc = f64_to_f32_launch(c.pose_gt, ctx->pose_cur_f32, c.B * 12, st)) return rc;
-    if (int rc = render_launch(ctx, c.cls_idx, ctx->pose_cur_f32, c.B, K9, c.zn, c.zf, nullptr, 1, nullptr, ctx->mask_rendered,
-                               nullptr, nullptr, nullptr, nullptr, st, nullptr, true, false, c.K_frames, c.frame_idx, c.F))
+    if (int rc = render_launch(ctx, c.cls_idx, ctx->pose_cur_f32, c.B, c.zn, c.zf, nullptr,
+                               {.cams = c.cams, .out_depth = ctx->mask_rendered, .trunc_u8 = 1, .ren4_depth = true}, st))
       return rc;
     DIM_CHECK(cudaMemcpyAsync(ctx->vsd_box, ctx->vbox, sizeof(int) * 4 * c.B, cudaMemcpyDeviceToDevice, st));
     if (int rc = f64_to_f32_launch(c.pose_est, ctx->pose_cur_f32, c.B * 12, st)) return rc;
-    if (int rc = render_launch(ctx, c.cls_idx, ctx->pose_cur_f32, c.B, K9, c.zn, c.zf, nullptr, 1, nullptr, nullptr, nullptr,
-                               nullptr, nullptr, ctx->ren4, st, nullptr, true, false, c.K_frames, c.frame_idx, c.F))
+    if (int rc = render_launch(ctx, c.cls_idx, ctx->pose_cur_f32, c.B, c.zn, c.zf, nullptr,
+                               {.cams = c.cams, .out_ren4 = ctx->ren4, .trunc_u8 = 1, .ren4_depth = true}, st))
       return rc;
   }
   if (ev) DIM_CHECK(cudaEventRecord(ev[1], st));
   VsdParams p;
   p.ren4 = ctx->ren4; p.depth_gt = ctx->mask_rendered; p.vbox_est = ctx->vbox; p.vbox_gt = ctx->vsd_box;
-  p.cls_flag = ctx->cls_flag; p.depth = c.depth; p.frame_idx = c.frame_idx; p.K_frames = c.K_frames;
+  p.cls_flag = ctx->cls_flag; p.depth = c.depth; p.cams = c.cams;
   p.partial = ctx->vsd_partial; p.err = c.err; p.status = c.status;
   for (int k = 0; k < VSD_MAX_TAU; ++k) p.taus[k] = k < c.n_tau ? c.taus[k] : 0.0;
-  p.fx = K9[0]; p.fy = K9[4]; p.cx = K9[2]; p.cy = K9[5]; p.delta = c.delta;
-  p.B = c.B; p.H = ctx->H; p.W = ctx->W; p.n_frames = c.F; p.chunks = cdiv(ctx->H, VSD_ROWS); p.n_tau = c.n_tau;
+  p.delta = c.delta;
+  p.B = c.B; p.H = ctx->H; p.W = ctx->W; p.chunks = cdiv(ctx->H, VSD_ROWS); p.n_tau = c.n_tau;
   {
     DimNvtxRange r("dim_pose_error_vsd pass");
     vsd_pass_kernel<<<dim3(p.chunks, c.B), VSD_THREADS, 0, st>>>(p);

@@ -62,22 +62,15 @@ __global__ void __launch_bounds__(160) mask_bbox_kernel(const float *mask_real, 
 // zoom factor, one thread per instance (zoom_mask.py:59-103; ZoomImage's is the same code, zoom_image.py:41-86).  Mixed
 // precision as the reference's numpy 1.x: c = K.t and c_x = c0/c2 in float32, everything after in float64, stored as float32.
 // ren_empty_bit: status bit set where the rendered box is empty and the zoom centres on the observed box (0: none)
-// frame_idx / n_frames (fused loop, nullable): an instance whose frame index is out of range gets status bit 3
-// K_frames (fused loop, nullable): [n_frames,9] intrinsics; instance b uses its frame's row (frame_of) instead of k0 ... k8
-__global__ void zoom_factor_kernel(int *bbox8, const float *src_pose, int B, int H, int W, float k0, float k1,
-                                   float k2, float k3, float k4, float k5, float k6, float k7, float k8,
-                                   float *zoom_factor, int *bbox_out, int *status, const int *cls_flag, int ren_empty_bit,
-                                   const int32_t *frame_idx, int n_frames, const float *K_frames) {
+// cams: instance b uses the camera cams.K(b); an instance whose frame index is out of range gets status bit 3
+__global__ void zoom_factor_kernel(int *bbox8, const float *src_pose, int B, int H, int W, FrameCams cams,
+                                   float *zoom_factor, int *bbox_out, int *status, const int *cls_flag, int ren_empty_bit) {
   int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  if (K_frames) {
-    const float *k = K_frames + 9 * frame_of(frame_idx, n_frames, b);
-    k0 = __ldg(k + 0); k1 = __ldg(k + 1); k2 = __ldg(k + 2);
-    k3 = __ldg(k + 3); k4 = __ldg(k + 4); k5 = __ldg(k + 5);
-    k6 = __ldg(k + 6); k7 = __ldg(k + 7); k8 = __ldg(k + 8);
-  }
+  float k[9];
+  cams.K(b, k);
   // rasteriser: bad class index (bit 1); frame index out of range (bit 3)
-  const int cf = (cls_flag ? cls_flag[b] : 0) | (frame_bad(frame_idx, n_frames, b) ? 8 : 0);
+  const int cf = (cls_flag ? cls_flag[b] : 0) | (cams.bad(b) ? 8 : 0);
   int *bb = bbox8 + 8 * b;
   if (bb[1] < 0) bb[0] = bb[1] = bb[2] = bb[3] = -1;
   if (bb[5] < 0) bb[4] = bb[5] = bb[6] = bb[7] = -1;
@@ -94,9 +87,9 @@ __global__ void zoom_factor_kernel(int *bbox8, const float *src_pose, int B, int
   const double real_x0 = bb[0], real_x1 = bb[1], real_y0 = bb[2], real_y1 = bb[3];
   const float *sp = src_pose + 12 * b;
   const float t0 = sp[3], t1 = sp[7], t2 = sp[11];
-  const float c0 = (k0 * t0 + k1 * t1) + k2 * t2;
-  const float c1 = (k3 * t0 + k4 * t1) + k5 * t2;
-  const float c2 = (k6 * t0 + k7 * t1) + k8 * t2;
+  const float c0 = (k[0] * t0 + k[1] * t1) + k[2] * t2;
+  const float c1 = (k[3] * t0 + k[4] * t1) + k[5] * t2;
+  const float c2 = (k[6] * t0 + k[7] * t1) + k[8] * t2;
   const float cxf = c0 / c2, cyf = c1 / c2;
   double ren_x0, ren_x1, ren_y0, ren_y1, zcx, zcy;
   if (bb[5] < 0) {  // "NO POINT VALID IN MASK rendered" (zoom_mask.py:70-77)
@@ -252,9 +245,8 @@ int zoom_factor_launch(dim_ctx *ctx, const float *mask_real, const float *mask_r
                                                        img_means ? 1 : 0, img_means ? img_means[0] : 0.f,
                                                        img_means ? img_means[1] : 0.f, img_means ? img_means[2] : 0.f);
   DIM_LAUNCH_CHECK();
-  zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
-                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, nullptr, 0,
-                                                  nullptr, 0, nullptr);
+  zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, frame_cams(K9), zoom_factor,
+                                                  bbox_out, status, nullptr, 0);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -275,14 +267,12 @@ __global__ void zoom_factor_from_ren_kernel(const int *bbox_ren, int *bbox8, int
   }
 }
 
-int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *src_pose, int B, const float *K9,
-                                float *zoom_factor, int *bbox_out, int *status, cudaStream_t st, const int32_t *frame_idx,
-                                int n_frames, const float *K_frames) {
+int zoom_factor_from_ren_launch(dim_ctx *ctx, const int *bbox_ren, const float *src_pose, int B, const FrameCams &cams,
+                                float *zoom_factor, int *bbox_out, int *status, cudaStream_t st) {
   zoom_factor_from_ren_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_ren, ctx->bbox8, B);
   DIM_LAUNCH_CHECK();
-  zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
-                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag, 0,
-                                                  frame_idx, n_frames, K_frames);
+  zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, cams, zoom_factor, bbox_out, status,
+                                                  ctx->cls_flag, 0);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -334,12 +324,11 @@ int obs_colour_box_launch(dim_ctx *ctx, const float4 *obs4, int F, int *bbox_obs
 // colour-valid bbox (raster.cu COLOUR_BOX), then ZoomImage's arithmetic -- zoom_factor_kernel, with the observed-centre
 // fallback for an empty render flagged as status bit 2 (the reference prints "NO POINT VALID IN rendered" and goes on); an
 // empty observed image is bit 0 with the (1,1,0,0) factor (the reference raises).
-// bbox_obs holds one box per frame; the instance's observed box is gathered here from its frame (frame_of).
-__global__ void boxes_to_bbox8_kernel(const int *bbox_obs, const int *bbox_ren, int *bbox8, int B, const int32_t *frame_idx,
-                                      int n_frames) {
+// bbox_obs holds one box per frame; the instance's observed box is gathered here from its frame (cams.frame).
+__global__ void boxes_to_bbox8_kernel(const int *bbox_obs, const int *bbox_ren, int *bbox8, int B, FrameCams cams) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  const int f = frame_of(frame_idx, n_frames, b);
+  const int f = cams.frame(b);
   for (int k = 0; k < 4; ++k) {
     bbox8[8 * b + k] = bbox_obs[4 * f + k];
     bbox8[8 * b + 4 + k] = bbox_ren[4 * b + k];
@@ -347,13 +336,11 @@ __global__ void boxes_to_bbox8_kernel(const int *bbox_obs, const int *bbox_ren, 
 }
 
 int zoom_factor_from_boxes_launch(dim_ctx *ctx, const int *bbox_obs, const int *bbox_ren, const float *src_pose, int B,
-                                  const float *K9, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st,
-                                  const int32_t *frame_idx, int n_frames, const float *K_frames) {
-  boxes_to_bbox8_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_obs, bbox_ren, ctx->bbox8, B, frame_idx, n_frames);
+                                  const FrameCams &cams, float *zoom_factor, int *bbox_out, int *status, cudaStream_t st) {
+  boxes_to_bbox8_kernel<<<cdiv(B, 64), 64, 0, st>>>(bbox_obs, bbox_ren, ctx->bbox8, B, cams);
   DIM_LAUNCH_CHECK();
-  zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, K9[0], K9[1], K9[2], K9[3],
-                                                  K9[4], K9[5], K9[6], K9[7], K9[8], zoom_factor, bbox_out, status, ctx->cls_flag, 4,
-                                                  frame_idx, n_frames, K_frames);
+  zoom_factor_kernel<<<cdiv(B, 64), 64, 0, st>>>(ctx->bbox8, src_pose, B, ctx->H, ctx->W, cams, zoom_factor, bbox_out, status,
+                                                  ctx->cls_flag, 4);
   DIM_LAUNCH_CHECK();
   return 0;
 }
@@ -387,7 +374,7 @@ int box_mask_launch(dim_ctx *ctx, const int *bbox, int B, float *mask, cudaStrea
 // same float32 addition -- so a tap costs no arithmetic before its weight.
 struct FusedZoomParams {
   const float4 *obs4;   // [F,H,W,4] observed frames (RGB - mean) + mean, w unused (RGB-D network: w = depth_observed)
-  const int32_t *frame_idx;  // [B] frame of each instance (frame_of); nullptr: frame b
+  const int32_t *frame_idx;  // [B] frame of each instance (FrameCams::frame); nullptr: frame b
   int n_frames;
   const float4 *ren4;   // [B,H,W,4] rendered (RGB - mean) + mean, w = mask_rendered (0/1) (RGB-D network: w = depth)
   const int *bbox8;     // observed box = bb[0..3] (inclusive)
@@ -525,7 +512,7 @@ __device__ __forceinline__ void zoom_fused_pixel(const FusedZoomParams &p, const
 // slots are rewritten with zeros.  Sources are the pixel-interleaved float4 images, so each tap is one 16-byte load
 // per image; the column taps of the quad's two columns and the row taps of its two rows are computed once each.
 // DEPTH: the RGB-D network's input, two chunk planes per quad slot: [B*Hs rows][8 planes = (slot, half)][Ws cols][8 ch]
-// Instance b's observed taps come from frame frame_of(b) of obs4 (dim_refine's frame map), its rendered taps from ren4[b].
+// Instance b's observed taps come from frame frame(b) of obs4 (dim_refine's frame map), its rendered taps from ren4[b].
 template <bool LO, bool F16, bool DEPTH = false, bool MASK = true>
 __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParams p) {
   const int b = blockIdx.y;
@@ -546,7 +533,8 @@ __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParam
     yt[k] = axis_tap(i0 + k, z.y, z.w, p.H, p.stepy, vb.z, vb.w, bb.z, bb.w);
   }
   const size_t P = (size_t)p.H * p.W;
-  const float4 *ob = p.obs4 + (size_t)frame_of(p.frame_idx, p.n_frames, b) * P, *rn = p.ren4 + (size_t)b * P;
+  const FrameCams fc{p.frame_idx, nullptr, p.n_frames, {}};
+  const float4 *ob = p.obs4 + (size_t)fc.frame(b) * P, *rn = p.ren4 + (size_t)b * P;
   // conv1 strip layout: [B*Hs rows][4 chunks (= quad slot)][Ws cols][8 ch] (DEPTH: 2 chunks per slot)
   constexpr int NC = DEPTH ? 2 : 1;
 #pragma unroll
@@ -567,11 +555,11 @@ __global__ void __launch_bounds__(128, 8) zoom_fused_nhwc8_kernel(FusedZoomParam
 
 int zoom_fused_launch(dim_ctx *ctx, const float4 *obs4, const float4 *ren4, const float *zoom_factor,
                       const float *means_rgb, int B, int Hs, int Ws, int pad, __nv_bfloat16 *hi, __nv_bfloat16 *lo,
-                      cudaStream_t st, int f16, const double *means_d, bool depth, bool mask, const int32_t *frame_idx,
-                      int n_frames) {
+                      cudaStream_t st, int f16, const double *means_d, bool depth, bool mask, const FrameCams &cams) {
   FusedZoomParams p;
   p.obs4 = obs4; p.ren4 = ren4;
-  p.frame_idx = frame_idx; p.n_frames = n_frames;
+  // the frame map only: the kernel runs at its 64-register bound, and the whole FrameCams in its parameters makes it spill
+  p.frame_idx = cams.frame_idx; p.n_frames = cams.n_frames;
   p.bbox8 = ctx->bbox8; p.zoom_factor = zoom_factor;
   p.vbox = means_d ? ctx->vbox : nullptr;  // means_d given: ren4 comes from the fused loop's box-only render
   for (int c = 0; c < 3; ++c) p.bg[c] = (means_d ? (float)(0.0 - means_d[c]) : 0.f) + means_rgb[c];

@@ -559,12 +559,8 @@ class Context:
                 pose_override, out, lighting, depth, names):
         """refine / refine_frames: one dim_refine call.  frame_idx None = instance b observes frames[b]; K [3,3] or [F,3,3]
         (_per_frame_k); names = the caller's names of the frames and depth arguments, for the messages."""
-        F = frames.shape[0]
-        B = F if frame_idx is None else cls_idx.shape[0]
+        F, B, K9, K_frames = self._frame_batch(frames, frame_idx, cls_idx, K)
         _chk(frames, torch.float32, (F, 3, self.H, self.W), names[0])
-        if frame_idx is not None:
-            _chk(frame_idx, torch.int32, (B,), "frame_idx")
-        _chk(cls_idx, torch.int32, (B,), "cls_idx")
         _chk(pose_init, torch.float64, (B, 3, 4), "pose_init")
         if out is not None:
             poses, se3, zf, bbox = out["poses"], out["se3"], out["zoom_factor"], out["bbox"]
@@ -582,14 +578,6 @@ class Context:
         if depth is not None:
             _chk(depth, torch.float32, (F, 1, self.H, self.W), names[1])
         lit = None if lighting is None else C.byref(_lighting_arg(lighting, (n_iter, B, 3), True)[0])
-        K9 = K_frames = None
-        if _per_frame_k(K, F):
-            K_frames = K
-            if not (isinstance(K, torch.Tensor) and K.device == self.device and K.dtype == torch.float32 and K.is_contiguous()):
-                K_frames = torch.as_tensor(np.ascontiguousarray(K if not isinstance(K, torch.Tensor) else K.cpu(), np.float32),
-                                           device=self.device)
-        else:
-            K9 = farr(np.asarray(K, np.float32).reshape(9), 9)
         check(lib.dim_refine(self._h, _p(frames), F, _p(frame_idx), K9, _p(K_frames), _p(cls_idx), _p(pose_init), B, n_iter,
                              znear, zfar, farr(pixel_means_rgb, 3, C.c_double), precision, _p(pose_override), _p(poses),
                              _p(se3), _p(zf), _p(bbox), _p(depth), lit, self._stream()))
@@ -600,13 +588,10 @@ class Context:
         """refine_host / refine_frames_host / PoseRefiner: one dim_refine_host_async call, then (sync) a synchronise of the
         stream.  frame_idx None = instance b observes frames_u8[b]; K [3,3] or [F,3,3] (_per_frame_k); names = the caller's
         names of the frames and depth arguments, for the messages."""
-        F = frames_u8.shape[0]
         fidx = None if frame_idx is None else _host(frame_idx, np.int32, torch.int32, "frame_idx")
         cls = _host(cls_idx, np.int32, torch.int32, "cls_idx")
         pose = _host(pose_init, np.float64, torch.float64, "pose_init")
-        B = F if fidx is None else cls.shape[0]
-        if fidx is not None and tuple(fidx.shape) != (B,):
-            raise ValueError("frame_idx: expected shape %s, got %s" % ((B,), tuple(fidx.shape)))
+        F, B, K9, K_frames = self._frame_batch(frames_u8, fidx, cls, K, host=True)
         if tuple(frames_u8.shape) != (F, self.H, self.W, 3):
             raise ValueError("%s: expected shape %s, got %s" % (names[0], (F, self.H, self.W, 3), tuple(frames_u8.shape)))
         if poses_out is None:
@@ -620,11 +605,6 @@ class Context:
                 raise ValueError("%s: expected shape %s, got %s" % (names[1], (F, self.H, self.W), tuple(dkeep.shape)))
         frames = frames_u8 if isinstance(frames_u8, torch.Tensor) else np.ascontiguousarray(frames_u8, np.uint8)
         lit, _keep = (None, None) if lighting is None else _lighting_arg(lighting, (n_iter, B, 3), False)
-        K9 = K_frames = None
-        if _per_frame_k(K, F):
-            K_frames = _host(K, np.float32, torch.float32, "K")
-        else:
-            K9 = farr(np.asarray(K, np.float32).reshape(9), 9)
         check(lib.dim_refine_host_async(self._h, hptr(frames), F, None if fidx is None else hptr(fidx), K9,
                                         None if K_frames is None else hptr(K_frames), hptr(cls), hptr(pose), B, n_iter, znear,
                                         zfar, farr(pixel_means_rgb, 3, C.c_double), precision, hptr(poses_out),
@@ -649,7 +629,9 @@ class Context:
         Returns CUDA tensors: poses f64 [n_iter,B,3,4] (after each iteration), inliers i32 [n_iter,B], rms f32 [n_iter,B]
         (both before that iteration's update), status i32 [n_iter,B] (bit 0 no model pixel, bit 1 bad class, bit 3 frame
         index out of range, bit 4 too few inliers or a singular system; with bit 0 or 4 the pose is unchanged)."""
-        F, B, K9, K_frames = self._depth_args(depth_frames, cls_idx, frame_idx, K)
+        F, B, K9, K_frames = self._frame_batch(depth_frames, frame_idx, cls_idx, K)
+        _chk(depth_frames, torch.float32, (F, 1, self.H, self.W) if depth_frames.dim() == 4 else (F, self.H, self.W),
+             "depth_frames")
         _chk(poses, torch.float64, (B, 3, 4), "poses")
         out = {"poses": self._new((n_iter, B, 3, 4), torch.float64), "inliers": self._new((n_iter, B), torch.int32),
                "rms": self._new((n_iter, B)), "status": self._new((n_iter, B), torch.int32)}
@@ -667,7 +649,9 @@ class Context:
         [B,3,4] CUDA; frame_idx and K as icp.
         Returns CUDA tensors: err f64 [B,n_tau] (1 = worst; 1 when neither pose leaves a visible pixel) and status i32 [B]
         (bit 0 empty union, bit 1 bad class, bit 3 frame index out of range)."""
-        F, B, K9, K_frames = self._depth_args(depth_frames, cls_idx, frame_idx, K)
+        F, B, K9, K_frames = self._frame_batch(depth_frames, frame_idx, cls_idx, K)
+        _chk(depth_frames, torch.float32, (F, 1, self.H, self.W) if depth_frames.dim() == 4 else (F, self.H, self.W),
+             "depth_frames")
         _chk(poses_est, torch.float64, (B, 3, 4), "poses_est")
         _chk(poses_gt, torch.float64, (B, 3, 4), "poses_gt")
         taus = np.ascontiguousarray(np.asarray(taus, np.float64).reshape(-1))
@@ -677,25 +661,31 @@ class Context:
                                      len(taus), _p(out["err"]), _p(out["status"]), self._stream()))
         return out
 
-    def _depth_args(self, depth_frames, cls_idx, frame_idx, K):
-        """icp / pose_error_vsd: checks the frames, classes and frame map -> (F, B, K9 host array or None, K_frames CUDA
-        tensor or None)"""
-        F = depth_frames.shape[0]
+    def _frame_batch(self, frames, frame_idx, cls_idx, K, host=False):
+        """The frame batch of refine*, icp and pose_error_vsd: F = frames.shape[0] frames, instance b observing frame
+        frame_idx[b] (None: frame b, so B = F) through K, [3,3] for every instance or [F,3,3] one per frame (_per_frame_k).
+        Checks frame_idx and cls_idx, int32 CUDA tensors; host: the refine*_host entries' host arrays (_host), whose K is
+        host too.  -> (F, B, K9 host array or None, K_frames or None: a float32 CUDA tensor, K itself when it is one
+        already; host: a host array)"""
+        F = frames.shape[0]
         B = F if frame_idx is None else cls_idx.shape[0]
-        _chk(depth_frames, torch.float32, (F, 1, self.H, self.W) if depth_frames.dim() == 4 else (F, self.H, self.W),
-             "depth_frames")
-        if frame_idx is not None:
-            _chk(frame_idx, torch.int32, (B,), "frame_idx")
-        _chk(cls_idx, torch.int32, (B,), "cls_idx")
-        K9 = K_frames = None
-        if _per_frame_k(K, F):
-            K_frames = K
-            if not (isinstance(K, torch.Tensor) and K.device == self.device and K.dtype == torch.float32 and K.is_contiguous()):
-                K_frames = torch.as_tensor(np.ascontiguousarray(K if not isinstance(K, torch.Tensor) else K.cpu(), np.float32),
-                                           device=self.device)
+        if host:
+            if frame_idx is not None and tuple(frame_idx.shape) != (B,):
+                raise ValueError("frame_idx: expected shape %s, got %s" % ((B,), tuple(frame_idx.shape)))
         else:
-            K9 = farr(np.asarray(K if not isinstance(K, torch.Tensor) else K.cpu(), np.float32).reshape(9), 9)
-        return F, B, K9, K_frames
+            if frame_idx is not None:
+                _chk(frame_idx, torch.int32, (B,), "frame_idx")
+            _chk(cls_idx, torch.int32, (B,), "cls_idx")
+        if not _per_frame_k(K, F):
+            if isinstance(K, torch.Tensor) and not host:
+                K = K.cpu()
+            return F, B, farr(np.asarray(K, np.float32).reshape(9), 9), None
+        if host:
+            return F, B, None, _host(K, np.float32, torch.float32, "K")
+        if not (isinstance(K, torch.Tensor) and K.device == self.device and K.dtype == torch.float32 and K.is_contiguous()):
+            K = torch.as_tensor(np.ascontiguousarray(K.cpu() if isinstance(K, torch.Tensor) else K, np.float32),
+                                device=self.device)
+        return F, B, None, K
 
     def depth_from_u16(self, depth_u16, depth_factor=1000.0):
         """uint16 depth file values [F,H,W] CUDA -> metres f32 [F,H,W], float32(u16) / float32(depth_factor) (the

@@ -16,6 +16,9 @@ from oracle import oracle as O
 
 import py_light_oracle as PL
 
+if not torch.cuda.is_available():
+    pytest.skip("no CUDA device", allow_module_level=True)
+
 pytestmark = pytest.mark.gpu
 K = toolkit.K_LM.astype(np.float32)
 GOLD = np.load(os.path.join(os.path.dirname(__file__), "golden", "ref_syn.npz"))
