@@ -469,6 +469,11 @@ DIM_API int32_t dim_debug_set_option(dim_ctx *ctx, const char *key, int32_t valu
 DIM_API int32_t dim_debug_layer_profile(dim_ctx *ctx, int32_t enable, float *ms10);
 /* dim_debug_graph_count: how many refinement chains this context holds captured as CUDA graphs (-1: NULL ctx). */
 DIM_API int32_t dim_debug_graph_count(dim_ctx *ctx);
+/* dim_debug_train_update: what the last dim_train_update of B instances computed besides its outputs, copied to the host
+ * (synchronises the device): kt_host [B,3,4] float32 KT = K . calc_se3(refined, tgt), the matrix of its reprojection-flow
+ * labels; light_host (nullable) [B,3] the light position of its lit re-render (meaningful after a call with lighting).  Valid
+ * until the next dim_refine*, dim_icp or dim_pose_error_vsd call on this context, which reuse the same scratch. */
+DIM_API int32_t dim_debug_train_update(dim_ctx *ctx, int32_t B, float *kt_host, float *light_host);
 
 /* Stage profiling of dim_refine with CUDA events on the launching stream (used by bench.py for the
  * live roofline numbers).  enable=1 starts recording; dim_profile_read synchronises the device and

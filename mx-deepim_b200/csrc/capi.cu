@@ -948,6 +948,14 @@ DIM_API int32_t dim_debug_graph_count(dim_ctx *ctx) {
   for (const auto &g : ctx->graphs) n += g.exec != nullptr;
   return n;
 }
+DIM_API int32_t dim_debug_train_update(dim_ctx *ctx, int32_t B, float *kt_host, float *light_host) {
+  DIM_REQUIRE(ctx && kt_host, "dim_debug_train_update: NULL argument");
+  DIM_REQUIRE(B >= 1 && B <= ctx->max_batch, "dim_debug_train_update: batch exceeds max_batch");
+  DIM_CHECK(cudaDeviceSynchronize());
+  DIM_CHECK(cudaMemcpy(kt_host, ctx->pose_cur_f32, (size_t)B * 12 * sizeof(float), cudaMemcpyDeviceToHost));
+  if (light_host) DIM_CHECK(cudaMemcpy(light_host, ctx->light_pos, (size_t)B * 3 * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
 DIM_API int32_t dim_debug_layer_profile(dim_ctx *ctx, int32_t enable, float *ms10) {
   DIM_REQUIRE(ctx, "dim_debug_layer_profile: NULL ctx");
   return net_layer_profile(ctx, enable, ms10);

@@ -81,6 +81,7 @@ SIGNATURES = {
     "dim_pose_error_vsd": (i32, [vp, vp, i32, vp, pf32, vp, vp, vp, vp, i32, f32, f32, f32, pf64, i32, vp, vp, vp]),
     "dim_debug_set_option": (i32, [vp, C.c_char_p, i32]),
     "dim_debug_graph_count": (i32, [vp]),
+    "dim_debug_train_update": (i32, [vp, i32, pf32, pf32]),
     "dim_debug_layer_profile": (i32, [vp, i32, pf32]),
     "dim_profile_enable": (i32, [vp, i32]),
     "dim_profile_read": (i32, [vp, pf32, C.POINTER(i32)]),

@@ -379,6 +379,10 @@ class Context:
                      pixel_means_rgb=(103.939, 116.779, 123.68), T_means=(0, 0, 0), T_stds=(1, 1, 1),
                      rot_coord="camera", znear=0.25, zfar=6.0, want_flow=True, lighting=None):
         """batchUpdaterPyMulti.forward on the device (lib/pair_matching/batch_updater_py_multi.py:91-328).
+        T_means / T_stds / rot_coord: the pose parameterisation of rot_est / trans_est and of the labels.  The defaults are
+        the standalone operator's; inside a training loop pass the context's (get_config()), which the training step's
+        Transform3D and refine() use, as the reference composes with network.ROT_COORD and dataset.trans_means / trans_stds
+        (l.23-27, 179-180).  trainer.fit_batch does.
         lighting: None = the unlit re-render (LINEMOD); a dict {intensity float32 [B,3] CUDA, offset, brightness_ratio}
         = the ModelNet branch's lit re-render (l.187-229; see deepim_b200.lighting), every other output unchanged."""
         B = src_pose.shape[0]
@@ -470,6 +474,14 @@ class Context:
         check(lib.dim_debug_activation(self._h, idx, int(lo), buf.ctypes.data, n * 2))
         f = buf.view(np.float16).astype(np.float32) if fp16 else (buf.astype(np.uint32) << 16).view(np.float32)
         return f.reshape(B, rows, cols, ch), tuple(g)
+
+    def debug_train_update(self, B):
+        """What the last train_update of B instances computed besides its outputs (dim_debug_train_update): float32 numpy
+        KT [B,3,4] = K . calc_se3(refined, tgt), the matrix of its flow labels, and the light position [B,3] of its lit
+        re-render (meaningful after a call with lighting)"""
+        kt, light = np.empty((B, 3, 4), np.float32), np.empty((B, 3), np.float32)
+        check(lib.dim_debug_train_update(self._h, B, kt.ctypes.data_as(capi.pf32), light.ctypes.data_as(capi.pf32)))
+        return kt, light
 
     # ------------------------------------------------------------------------------ refine
     def get_config(self) -> dict:

@@ -342,6 +342,8 @@ def make_device_batch(ctx, meshes, B, seed, K, pixel_means_rgb, num_points=3000,
         if np.ndim(draws) == 0:
             draws = augment.background_draws(B, np.random.RandomState(int(draws)), len(bank))
         image_observed = ctx.replace_background(r["bgr"], r["mask"], draws, pixel_means_rgb)
+    # the identity update: (0, 0, 0) is the zero translation delta only under T_means = 0, T_stds = 1, so this call keeps
+    # train_update's defaults whatever the context's configuration
     ident = torch.tensor([[1.0, 0, 0, 0]] * B, dtype=torch.float32, device=dev)
     upd = ctx.train_update(cls, src, ident, torch.zeros(B, 3, device=dev), tgt, r["depth"], K, pixel_means_rgb=pixel_means_rgb,
                            lighting=_device_lighting(light, B, dev))
@@ -378,9 +380,12 @@ def fit_batch(trainer, batch, cls, tgt_pose, depth_gt, K, n_inner=4, dist=None, 
     batch re-rendered at the predicted pose in between (batchUpdaterPyMulti.forward -> Context.train_update).
     lighting = None or the ModelNet branch's light ({"seed", "offset", "brightness_ratio"} or a lighting.LightSource, which
     keeps drawing fresh intensities across calls): the re-renders are lit (batch_updater_py_multi.py:187-229).
+    The re-render composes the predicted delta under the context's trans_means / trans_stds / rot_coord, the
+    parameterisation the step's Transform3D trained it in (batch_updater_py_multi.py:23-27, 179-180).
     Returns the objective of every inner iteration (device tensor [n_inner])."""
     ctx = trainer.ctx
     light = _lighting.LightSource.of(lighting)
+    cfg = ctx.get_config()
     b = dict(batch)
     objs = []
     for it in range(n_inner):
@@ -389,7 +394,8 @@ def fit_batch(trainer, batch, cls, tgt_pose, depth_gt, K, n_inner=4, dist=None, 
         objs.append(res["losses"][3])
         if it != n_inner - 1:
             upd = ctx.train_update(cls, b["src_pose"], res["rot_est_norm"], res["trans_est"], tgt_pose, depth_gt, K,
-                                   pixel_means_rgb=batch["pixel_means_rgb"],
+                                   pixel_means_rgb=batch["pixel_means_rgb"], T_means=cfg["trans_means"],
+                                   T_stds=cfg["trans_stds"], rot_coord=cfg["rot_coord"],
                                    lighting=_device_lighting(light, cls.shape[0], ctx.device))
             for k in ("image_rendered", "mask_rendered", "src_pose", "flow", "flow_weights"):
                 b[k] = upd[k]

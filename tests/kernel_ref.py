@@ -198,15 +198,30 @@ def _t3d_common(t, pose_src, Tm, Ts):
     return Ts, z2, a, e2, Sa
 
 
+def _t3d_camera_new(t, pose_src, Tm, Ts):
+    """T_transform for rot_coord camera_new: (x, y) = src_z d + src_(x, y), and the scale of their fp32 evaluation"""
+    Tm, Ts = (torch.as_tensor(v, dtype=t.dtype, device=t.device) for v in (Tm, Ts))
+    src = pose_src[:, :, 3]
+    d = t[:, :2] * Ts[:2] + Tm[:2]
+    Sd = (t[:, :2] * Ts[:2]).abs() + Tm[:2].abs()
+    return src[:, 2:3] * d + src[:, :2], src[:, 2:3].abs() * Sd + src[:, :2].abs()
+
+
 def transform3d_fwd(P, q, t, pose_src, Tm, Ts, rot_coord):
-    """Transform3D forward (transform3d.py:34-97; rot_coord 'MODEL' or 'CAMERA'): points P [B, 3, N] under the rotation
-    q [B, 4] and the translation t [B, 3] relative to pose_src [B, 3, 4] -> (ref, S), S bounding the fp32 evaluation"""
+    """Transform3D forward (transform3d.py:34-97; rot_coord 'MODEL', 'CAMERA' or 'CAMERA_NEW'): points P [B, 3, N] under the
+    rotation q [B, 4] and the translation t [B, 3] relative to pose_src [B, 3, 4] -> (ref, S), S bounding the fp32
+    evaluation"""
     Rd, Rs = quat2mat_t3d(q), pose_src[:, :, :3]
     model = rot_coord.lower() == "model"
     Rt, SRt = (Rs @ Rd, Rs.abs() @ Rd.abs()) if model else (Rd @ Rs, Rd.abs() @ Rs.abs())
     _, z2, a, e2, Sa = _t3d_common(t, pose_src, Tm, Ts)
-    Tt = torch.cat([z2[:, None] * a, z2[:, None]], 1)
-    STt = z2.abs()[:, None] * torch.cat([e2[:, None] * a.abs() + Sa, e2[:, None]], 1)
+    if rot_coord.lower() == "camera_new":
+        xy, Sxy = _t3d_camera_new(t, pose_src, Tm, Ts)
+        Tt = torch.cat([xy, z2[:, None]], 1)
+        STt = torch.cat([Sxy, z2.abs()[:, None] * e2[:, None]], 1)
+    else:
+        Tt = torch.cat([z2[:, None] * a, z2[:, None]], 1)
+        STt = z2.abs()[:, None] * torch.cat([e2[:, None] * a.abs() + Sa, e2[:, None]], 1)
     return Rt @ P + Tt[:, :, None], SRt @ P.abs() + STt[:, :, None]
 
 
@@ -228,13 +243,18 @@ def transform3d_bwd(D, P, q, t, pose_src, Tm, Ts, rot_coord):
     Ts, z2, a, e2, Sa = _t3d_common(t, pose_src, Tm, Ts)
     Dt, SDt = D.sum(2), D.abs().sum(2)
     share = -Ts[2] * z2
-    tg = torch.stack([Dt[:, 0] * Ts[0] * z2, Dt[:, 1] * Ts[1] * z2, Dt[:, 0] * share * a[:, 0] + Dt[:, 1] * share * a[:, 1]
-                      + Dt[:, 2] * share], 1)
-    Stg = e2[:, None] * torch.stack([SDt[:, 0] * (Ts[0] * z2).abs(), SDt[:, 1] * (Ts[1] * z2).abs(),
-                                     share.abs() * (SDt[:, 0] * Sa[:, 0] + SDt[:, 1] * Sa[:, 1] + SDt[:, 2])], 1)
+    if rot_coord.lower() == "camera_new":  # x, y no longer depend on d_z: d_x, d_y scale by src_z
+        sz = pose_src[:, 2, 3]
+        tg = torch.stack([Dt[:, 0] * Ts[0] * sz, Dt[:, 1] * Ts[1] * sz, Dt[:, 2] * share], 1)
+        Stg = torch.stack([SDt[:, 0] * (Ts[0] * sz).abs(), SDt[:, 1] * (Ts[1] * sz).abs(), e2 * SDt[:, 2] * share.abs()], 1)
+    else:
+        tg = torch.stack([Dt[:, 0] * Ts[0] * z2, Dt[:, 1] * Ts[1] * z2,
+                          Dt[:, 0] * share * a[:, 0] + Dt[:, 1] * share * a[:, 1] + Dt[:, 2] * share], 1)
+        Stg = e2[:, None] * torch.stack([SDt[:, 0] * (Ts[0] * z2).abs(), SDt[:, 1] * (Ts[1] * z2).abs(),
+                                         share.abs() * (SDt[:, 0] * Sa[:, 0] + SDt[:, 1] * Sa[:, 1] + SDt[:, 2])], 1)
     RtD, SRtD = D @ P.transpose(1, 2), D.abs() @ P.abs().transpose(1, 2)
     Rs = pose_src[:, :, :3]
-    if rot_coord.lower() == "model":
+    if rot_coord.lower() == "model":  # camera and camera_new share R_delta R_src
         Dm, SDm = Rs.transpose(1, 2) @ RtD, Rs.abs().transpose(1, 2) @ SRtD
     else:
         Dm, SDm = RtD @ Rs.transpose(1, 2), SRtD @ Rs.abs().transpose(1, 2)

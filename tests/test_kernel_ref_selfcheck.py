@@ -70,7 +70,7 @@ def test_point_matching_gradient():
     assert not ref[:, :, 2].any()
 
 
-@pytest.mark.parametrize("rot_coord", ["MODEL", "CAMERA"])
+@pytest.mark.parametrize("rot_coord", ["MODEL", "CAMERA", "CAMERA_NEW"])
 def test_transform3d_matches_oracle(rot_coord):
     """the float64 Transform3D forward / hand-written backward against the oracle's restatement of transform3d.py"""
     rng = np.random.default_rng(5)
