@@ -409,6 +409,34 @@ DIM_API int32_t dim_pose_error_vsd(dim_ctx *ctx, const float *depth_frames, int3
                                    float delta, const double *taus_host, int32_t n_tau, double *err, int32_t *status,
                                    void *stream);
 
+/* dim_pose_error_vsd with BOP 2019's variant (Hodan et al., "BOP Challenge 2019"): dim_pose_error_vsd's arguments plus
+ *   visib_mode: 0 = the SIXD 2017 visibility above (dim_pose_error_vsd is this call with 0 and NULL); 1 = BOP 2019's:
+ *     vis(a) = dist_a > 0 & (float32(dist_a) - float32(dist_test) <= float32(delta) | dist_test == 0), so sensor holes count
+ *     as visible; V_est = vis(est) | (V_gt & dist_est > 0) as before.
+ *   diam_host: f64[B] host, nullable; each finite and > 0 (metres).  Given, the tau test is |dist_gt - dist_est| / diam[b]
+ *     >= tau (a float64 division) and the taus are fractions of the diameter.  It is copied to the context before the call
+ *     returns.
+ * Everything else, the refusals and the guarantees are dim_pose_error_vsd's.  The contract is oracle/bop.py's vsd(),
+ * oracle/vsd.py's with these two switches. */
+DIM_API int32_t dim_pose_error_vsd_ex(dim_ctx *ctx, const float *depth_frames, int32_t F, const int32_t *frame_idx,
+                                      const float *K9_host, const float *K_frames, const int32_t *cls_idx,
+                                      const double *poses_est, const double *poses_gt, int32_t B, float znear, float zfar,
+                                      float delta, const double *taus_host, int32_t n_tau, int32_t visib_mode,
+                                      const double *diam_host, double *err, int32_t *status, void *stream);
+
+/* BOP 2019's symmetry-aware point errors (Hodan et al., "BOP Challenge 2019"), float64, all pointers on the device:
+ *   poses_est / poses_gt f64[M,3,4], points f64[N,3] (one class), syms f64[S,3,4] the object's symmetry transforms (row 0
+ *   normally the identity), K_inst f64[M,9] each instance's camera.
+ *   err2 f64[M,2]: MSSD = min_s max_p |T_est p - T_gs p| (metres) and MSPD = min_s max_p |proj(K, T_est p) - proj(K, T_gs p)|
+ *   (pixels), with T_gs = T_gt . sym_s (R_gt R_s, R_gt t_s + t_gt); a point with Z <= 0 under either pose makes that
+ *   symmetry's MSPD +inf.  sym_idx2 i32[M,2] (nullable): the minimising symmetry of each error, the lowest index on ties.
+ *   1 <= M <= max_batch, N >= 1, 1 <= S <= 4096.
+ * The contract is oracle/bop.py; the results equal it bit for bit and do not depend on M, the batch or the SM count.  Never
+ * reads the network or the render scratch.  A refused call enqueues nothing and leaves the outputs untouched. */
+DIM_API int32_t dim_pose_error_sym(dim_ctx *ctx, const double *poses_est, const double *poses_gt, int32_t M,
+                                   const double *points, int32_t N, const double *syms, int32_t S, const double *K_inst,
+                                   double *err2, int32_t *sym_idx2, void *stream);
+
 /* BGR u8 HWC -> RGB-mean f32 CHW on device (lib/utils/image.py:583-594 transform). */
 DIM_API int32_t dim_transform_image_u8(dim_ctx *ctx, const uint8_t *bgr_u8, int32_t B,
                                        const double *pixel_means_rgb_host, float *image,
@@ -472,7 +500,7 @@ DIM_API int32_t dim_debug_graph_count(dim_ctx *ctx);
 /* dim_debug_train_update: what the last dim_train_update of B instances computed besides its outputs, copied to the host
  * (synchronises the device): kt_host [B,3,4] float32 KT = K . calc_se3(refined, tgt), the matrix of its reprojection-flow
  * labels; light_host (nullable) [B,3] the light position of its lit re-render (meaningful after a call with lighting).  Valid
- * until the next dim_refine*, dim_icp or dim_pose_error_vsd call on this context, which reuse the same scratch. */
+ * until the next dim_refine*, dim_icp or dim_pose_error_vsd(_ex) call on this context, which reuse the same scratch. */
 DIM_API int32_t dim_debug_train_update(dim_ctx *ctx, int32_t B, float *kt_host, float *light_host);
 
 /* Stage profiling of dim_refine with CUDA events on the launching stream (used by bench.py for the

@@ -105,6 +105,8 @@ DIM_API int32_t dim_ctx_create(int32_t device, int32_t max_batch, int32_t H, int
   rc |= dev_alloc(ctx, &ctx->icp_partial, Bm * (size_t)cdiv(H, ICP_ROWS) * ICP_SLOT);
   rc |= dev_alloc(ctx, &ctx->vsd_partial, Bm * (size_t)cdiv(H, VSD_ROWS) * VSD_SLOT);
   rc |= dev_alloc(ctx, &ctx->vsd_box, Bm * 4);
+  rc |= dev_alloc(ctx, &ctx->vsd_diam, Bm);
+  rc |= dev_alloc(ctx, &ctx->sym_partial, Bm * SYM_SLOTS * 2);
   if (rc) { dim_ctx_destroy(ctx); return 12; }
   ctx->meshes_host.assign(max_classes, MeshDev{nullptr, nullptr, nullptr, nullptr, 0, 0, 0, 0, nullptr});
   DIM_CHECK(cudaMemset(ctx->meshes, 0, sizeof(MeshDev) * max_classes));
@@ -802,11 +804,11 @@ DIM_API int32_t dim_icp(dim_ctx *ctx, const float *depth_frames, int32_t F, cons
 // Visible Surface Discrepancy (vsd.cu; the contract is oracle/vsd.py).  Refused calls enqueue nothing and leave the outputs
 // untouched.  The call writes ren4, vbox, bbox_ren, cls_flag, pose_cur_f32 and mask_rendered, which every refinement
 // iteration (and dim_train_update, for mask_rendered) rewrites before reading, so graphs captured before it replay unchanged.
-DIM_API int32_t dim_pose_error_vsd(dim_ctx *ctx, const float *depth_frames, int32_t F, const int32_t *frame_idx,
-                                   const float *K9_host, const float *K_frames, const int32_t *cls_idx, const double *poses_est,
-                                   const double *poses_gt, int32_t B, float znear, float zfar, float delta,
-                                   const double *taus_host, int32_t n_tau, double *err, int32_t *status, void *stream) {
-  const char *fn = "dim_pose_error_vsd";
+static int32_t pose_error_vsd(const char *fn, dim_ctx *ctx, const float *depth_frames, int32_t F, const int32_t *frame_idx,
+                              const float *K9_host, const float *K_frames, const int32_t *cls_idx, const double *poses_est,
+                              const double *poses_gt, int32_t B, float znear, float zfar, float delta, const double *taus_host,
+                              int32_t n_tau, int32_t visib_mode, const double *diam_host, double *err, int32_t *status,
+                              cudaStream_t st) {
   if (!(ctx && depth_frames && cls_idx && poses_est && poses_gt && taus_host && err)) return refuse(fn, "NULL argument");
   if (int rc = frames_check(ctx, fn, K9_host, K_frames, "K_frames", B, F, frame_idx)) return rc;
   if (n_tau < 1 || n_tau > VSD_MAX_TAU) return refuse(fn, "n_tau must be in [1,16]");
@@ -814,9 +816,46 @@ DIM_API int32_t dim_pose_error_vsd(dim_ctx *ctx, const float *depth_frames, int3
   for (int32_t k = 0; k < n_tau; ++k)
     if (!(taus_host[k] > 0.0 && taus_host[k] < 1.0e308)) return refuse(fn, "every tau must be positive and finite");
   if (int rc = pinhole_check(fn, K9_host)) return rc;
+  if (visib_mode != 0 && visib_mode != 1) return refuse(fn, "visib_mode must be 0 (SIXD 2017) or 1 (BOP 2019)");
+  if (diam_host) {
+    for (int32_t b = 0; b < B; ++b)
+      if (!(diam_host[b] > 0.0 && diam_host[b] < 1.0e308)) return refuse(fn, "every diameter must be positive and finite");
+    DIM_CHECK(cudaMemcpyAsync(ctx->vsd_diam, diam_host, sizeof(double) * B, cudaMemcpyHostToDevice, st));
+  }
   const VsdCall c{depth_frames, frame_cams(K9_host, K_frames, frame_idx, F), cls_idx, poses_est, poses_gt, B, znear, zfar,
-                  delta, taus_host, n_tau, err, status};
-  return vsd_launch(ctx, c, (cudaStream_t)stream);
+                  delta, taus_host, n_tau, err, status, visib_mode, diam_host ? ctx->vsd_diam : nullptr};
+  return vsd_launch(ctx, c, st);
+}
+
+DIM_API int32_t dim_pose_error_vsd(dim_ctx *ctx, const float *depth_frames, int32_t F, const int32_t *frame_idx,
+                                   const float *K9_host, const float *K_frames, const int32_t *cls_idx, const double *poses_est,
+                                   const double *poses_gt, int32_t B, float znear, float zfar, float delta,
+                                   const double *taus_host, int32_t n_tau, double *err, int32_t *status, void *stream) {
+  return pose_error_vsd("dim_pose_error_vsd", ctx, depth_frames, F, frame_idx, K9_host, K_frames, cls_idx, poses_est,
+                        poses_gt, B, znear, zfar, delta, taus_host, n_tau, 0, nullptr, err, status, (cudaStream_t)stream);
+}
+
+DIM_API int32_t dim_pose_error_vsd_ex(dim_ctx *ctx, const float *depth_frames, int32_t F, const int32_t *frame_idx,
+                                      const float *K9_host, const float *K_frames, const int32_t *cls_idx,
+                                      const double *poses_est, const double *poses_gt, int32_t B, float znear, float zfar,
+                                      float delta, const double *taus_host, int32_t n_tau, int32_t visib_mode,
+                                      const double *diam_host, double *err, int32_t *status, void *stream) {
+  return pose_error_vsd("dim_pose_error_vsd_ex", ctx, depth_frames, F, frame_idx, K9_host, K_frames, cls_idx, poses_est,
+                        poses_gt, B, znear, zfar, delta, taus_host, n_tau, visib_mode, diam_host, err, status,
+                        (cudaStream_t)stream);
+}
+
+// BOP 2019 MSSD / MSPD over a symmetry set (bop.cu; the contract is oracle/bop.py).  Refused calls enqueue nothing and leave
+// the outputs untouched.  The call writes only sym_partial, which nothing else reads.
+DIM_API int32_t dim_pose_error_sym(dim_ctx *ctx, const double *poses_est, const double *poses_gt, int32_t M,
+                                   const double *points, int32_t N, const double *syms, int32_t S, const double *K_inst,
+                                   double *err2, int32_t *sym_idx2, void *stream) {
+  const char *fn = "dim_pose_error_sym";
+  if (!(ctx && poses_est && poses_gt && points && syms && K_inst && err2)) return refuse(fn, "NULL argument");
+  if (M < 1 || M > ctx->max_batch) return refuse(fn, "M must be in [1, max_batch]");
+  if (N < 1) return refuse(fn, "N must be >= 1");
+  if (S < 1 || S > SYM_MAX) return refuse(fn, "S must be in [1,4096]");
+  return sym_launch(ctx, SymCall{poses_est, poses_gt, M, points, N, syms, S, K_inst, err2, sym_idx2}, (cudaStream_t)stream);
 }
 
 DIM_API int32_t dim_depth_from_u16(dim_ctx *ctx, const uint16_t *depth_u16, int32_t F, float depth_factor, float *depth,

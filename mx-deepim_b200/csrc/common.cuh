@@ -181,6 +181,8 @@ struct dim_ctx {
   double *icp_partial = nullptr;   // [max_batch, H / ICP_ROWS, ICP_SLOT] dim_icp: one reduction slot per association CTA
   int32_t *vsd_partial = nullptr;  // [max_batch, H / VSD_ROWS, VSD_SLOT] dim_pose_error_vsd: one count slot per pass CTA
   int *vsd_box = nullptr;          // [max_batch,4] dim_pose_error_vsd: the ground-truth render's vertex box
+  double *vsd_diam = nullptr;      // [max_batch] dim_pose_error_vsd_ex: the caller's object diameters
+  double *sym_partial = nullptr;   // [max_batch, SYM_SLOTS, 2] dim_pose_error_sym: squared maxima per (symmetry, chunk)
   // background bank of dim_replace_background (dim_bg_upload): BGR u8 photos, each allocated at its upload
   struct BgImage { uint8_t *data = nullptr; int h = 0, w = 0; };
   std::vector<BgImage> bg;

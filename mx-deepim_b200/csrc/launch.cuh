@@ -154,8 +154,27 @@ struct VsdCall {  // dim_pose_error_vsd's arguments, checked
   int n_tau;
   double *err;
   int32_t *status;  // nullable
+  int visib_mode;   // 0: SIXD 2017 visibility (oracle/vsd.py), 1: BOP 2019 (sensor holes count as visible)
+  const double *diam;  // device [B] object diameters (taus are fractions of them), or nullptr (taus in metres)
 };
 int vsd_launch(dim_ctx *ctx, const VsdCall &c, cudaStream_t st);
+
+// bop.cu
+constexpr int SYM_MAX = 4096;     // symmetries per dim_pose_error_sym call
+constexpr int SYM_SLOTS = 16384;  // scratch slots (symmetry x point chunk) per instance
+constexpr int SYM_WAVES = 8;      // pass CTAs per SM the point chunking aims for
+struct SymCall {  // dim_pose_error_sym's arguments, checked
+  const double *pose_est, *pose_gt;  // [M,3,4]
+  int M;
+  const double *pts;  // [N,3]
+  int N;
+  const double *syms;  // [S,3,4]
+  int S;
+  const double *K;  // [M,9]
+  double *err2;     // [M,2]
+  int32_t *sym_idx2;  // [M,2], nullable
+};
+int sym_launch(dim_ctx *ctx, const SymCall &c, cudaStream_t st);
 
 // net.cu
 int net_create(dim_ctx *ctx);

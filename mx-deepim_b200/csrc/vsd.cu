@@ -1,8 +1,12 @@
-// vsd.cu -- the Visible Surface Discrepancy of Hodan et al. (dim_pose_error_vsd), compiled with -fmad=false.
+// vsd.cu -- the Visible Surface Discrepancy of Hodan et al. (dim_pose_error_vsd, dim_pose_error_vsd_ex), compiled with
+// -fmad=false.
 //
 // oracle/vsd.py states the contract in float64 numpy (the reference's depth_im_to_dist_im and visibility.py, pinned by
 // tests/golden/ref_vsd.npz, and the paper's step cost); this file restates it operation by operation, so every count, and
-// with it every error, equals the oracle's fed the same renders.
+// with it every error, equals the oracle's fed the same renders.  The BOP 2019 variant (oracle/bop.py's vsd()) changes only
+// the visibility rule (sensor holes are visible) and, with diameters, divides the distance difference by the instance's
+// diameter before the tau test; both are template parameters of the pass, so the SIXD 2017 instantiation is the original
+// kernel.
 //
 // Per call: the depth render at float32(P_gt), written full-frame into mask_rendered through the render's out_depth (its
 // vertex box saved in vsd_box), then the box-only depth render at float32(P_est) into ren4.w (valid only inside vbox), then
@@ -32,6 +36,7 @@ struct VsdParams {
   double taus[VSD_MAX_TAU];
   float delta;
   int B, H, W, chunks, n_tau;
+  const double *diam;        // [B] with relative taus (vsd_pass_kernel<VIS, true>)
 };
 
 struct Box { int i0, i1, j0, j1; };  // inclusive; empty when i1 < i0 or j1 < j0
@@ -57,10 +62,15 @@ __device__ __forceinline__ double dist_of(float d, double di, double dj, double 
   return sqrt((X * X + Y * Y) + z * z);
 }
 
+// VIS = 0: the SIXD 2017 rule (visibility.py); VIS = 1: BOP 2019's, where a sensor hole (dist_test == 0) counts as visible
+template <int VIS>
 __device__ __forceinline__ bool visible(double dist_test, double dist_model, float delta) {
-  return dist_test > 0.0 && dist_model > 0.0 && (float)dist_model - (float)dist_test <= delta;
+  if (VIS == 0) return dist_test > 0.0 && dist_model > 0.0 && (float)dist_model - (float)dist_test <= delta;
+  return dist_model > 0.0 && ((float)dist_model - (float)dist_test <= delta || dist_test == 0.0);
 }
 
+// DIAM: the taus are fractions of the instance's diameter p.diam[b] (BOP 2019), else metres
+template <int VIS, bool DIAM>
 __global__ void __launch_bounds__(VSD_THREADS) vsd_pass_kernel(VsdParams p) {
   const int b = blockIdx.y, ch = blockIdx.x;
   const Box rg = pass_range(p, b);
@@ -74,6 +84,7 @@ __global__ void __launch_bounds__(VSD_THREADS) vsd_pass_kernel(VsdParams p) {
   const int ex0 = p.vbox_est[4 * b], ex1 = p.vbox_est[4 * b + 1], ey0 = p.vbox_est[4 * b + 2], ey1 = p.vbox_est[4 * b + 3];
   const float4 *ren = p.ren4 + (size_t)b * P;
   const float *dgt = p.depth_gt + (size_t)b * P;
+  const double diam = DIAM ? p.diam[b] : 0.0;
 
   int cnt[VSD_SLOT];
 #pragma unroll
@@ -87,12 +98,12 @@ __global__ void __launch_bounds__(VSD_THREADS) vsd_pass_kernel(VsdParams p) {
     const double t = dist_of(obs[o], di, dj, cx, cy, rfx, rfy);
     const double g = dist_of(dgt[o], di, dj, cx, cy, rfx, rfy);
     const double e = dist_of(de, di, dj, cx, cy, rfx, rfy);
-    const bool v_gt = visible(t, g, p.delta);
-    const bool v_est = visible(t, e, p.delta) || (v_gt && e > 0.0);
+    const bool v_gt = visible<VIS>(t, g, p.delta);
+    const bool v_est = visible<VIS>(t, e, p.delta) || (v_gt && e > 0.0);
     cnt[0] += (v_gt || v_est) ? 1 : 0;
     if (v_gt && v_est) {
       cnt[1] += 1;
-      const double a = fabs(g - e);
+      const double a = DIAM ? fabs(g - e) / diam : fabs(g - e);
 #pragma unroll
       for (int k = 0; k < VSD_MAX_TAU; ++k)
         if (k < p.n_tau && a >= p.taus[k]) cnt[2 + k] += 1;
@@ -150,13 +161,15 @@ int vsd_launch(dim_ctx *ctx, const VsdCall &c, cudaStream_t st) {
   VsdParams p;
   p.ren4 = ctx->ren4; p.depth_gt = ctx->mask_rendered; p.vbox_est = ctx->vbox; p.vbox_gt = ctx->vsd_box;
   p.cls_flag = ctx->cls_flag; p.depth = c.depth; p.cams = c.cams;
-  p.partial = ctx->vsd_partial; p.err = c.err; p.status = c.status;
+  p.partial = ctx->vsd_partial; p.err = c.err; p.status = c.status; p.diam = c.diam;
   for (int k = 0; k < VSD_MAX_TAU; ++k) p.taus[k] = k < c.n_tau ? c.taus[k] : 0.0;
   p.delta = c.delta;
   p.B = c.B; p.H = ctx->H; p.W = ctx->W; p.chunks = cdiv(ctx->H, VSD_ROWS); p.n_tau = c.n_tau;
   {
     DimNvtxRange r("dim_pose_error_vsd pass");
-    vsd_pass_kernel<<<dim3(p.chunks, c.B), VSD_THREADS, 0, st>>>(p);
+    auto pass = c.visib_mode ? (c.diam ? vsd_pass_kernel<1, true> : vsd_pass_kernel<1, false>)
+                             : (c.diam ? vsd_pass_kernel<0, true> : vsd_pass_kernel<0, false>);
+    pass<<<dim3(p.chunks, c.B), VSD_THREADS, 0, st>>>(p);
     DIM_LAUNCH_CHECK();
     vsd_finish_kernel<<<cdiv(c.B, 64), 64, 0, st>>>(p);
     DIM_LAUNCH_CHECK();

@@ -79,6 +79,9 @@ SIGNATURES = {
     "dim_icp": (i32, [vp, vp, i32, vp, pf32, vp, vp, vp, i32, i32, f32, f32, f32, i32, vp, vp, vp, vp, vp]),
     "dim_depth_from_u16": (i32, [vp, vp, i32, f32, vp, vp]),
     "dim_pose_error_vsd": (i32, [vp, vp, i32, vp, pf32, vp, vp, vp, vp, i32, f32, f32, f32, pf64, i32, vp, vp, vp]),
+    "dim_pose_error_vsd_ex": (i32, [vp, vp, i32, vp, pf32, vp, vp, vp, vp, i32, f32, f32, f32, pf64, i32, i32, pf64, vp, vp,
+                                    vp]),
+    "dim_pose_error_sym": (i32, [vp, vp, vp, i32, vp, i32, vp, i32, vp, vp, vp, vp]),
     "dim_debug_set_option": (i32, [vp, C.c_char_p, i32]),
     "dim_debug_graph_count": (i32, [vp]),
     "dim_debug_train_update": (i32, [vp, i32, pf32, pf32]),

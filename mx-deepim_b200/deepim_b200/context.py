@@ -20,6 +20,9 @@ WEIGHT_ORDER = ["flow_conv1", "conv2", "conv3", "conv3_1", "conv4", "conv4_1", "
 
 
 
+VISIB_MODES = {"sixd17": 0, "bop19": 1}  # pose_error_vsd's visib_mode -> dim_pose_error_vsd_ex's
+
+
 def _p(t):
     if t is None:
         return None
@@ -653,24 +656,66 @@ class Context:
         return out
 
     def pose_error_vsd(self, depth_frames, cls_idx, poses_est, poses_gt, K, delta=0.015, taus=(0.02,), frame_idx=None,
-                       znear=0.25, zfar=6.0):
+                       znear=0.25, zfar=6.0, visib_mode="sixd17", diameters=None):
         """Visible Surface Discrepancy of poses_est against poses_gt (dim_pose_error_vsd; Hodan et al., ECCVW 2016; the
         contract is oracle/vsd.py): both poses are rendered at float32, and the visible surfaces are compared against the
         observed depth with tolerance delta (metres) and the step cost at each tau (metres, at most 16 of them).
         depth_frames f32 [F,H,W] (or [F,1,H,W]) CUDA, metres, 0 = hole; cls_idx i32 [B] CUDA; poses_est / poses_gt f64
         [B,3,4] CUDA; frame_idx and K as icp.
+        visib_mode "sixd17" (default) is the SIXD 2017 visibility; "bop19" is BOP 2019's, where sensor holes count as
+        visible.  diameters: None (taus in metres) or [B] host values in metres, each finite and > 0, making the taus
+        fractions of each instance's diameter, as BOP 2019 does (dim_pose_error_vsd_ex; the contract is oracle/bop.py's vsd()).
         Returns CUDA tensors: err f64 [B,n_tau] (1 = worst; 1 when neither pose leaves a visible pixel) and status i32 [B]
         (bit 0 empty union, bit 1 bad class, bit 3 frame index out of range)."""
+        if visib_mode not in VISIB_MODES:
+            raise ValueError("visib_mode must be one of %s, got %r" % (tuple(VISIB_MODES), visib_mode))
         F, B, K9, K_frames = self._frame_batch(depth_frames, frame_idx, cls_idx, K)
         _chk(depth_frames, torch.float32, (F, 1, self.H, self.W) if depth_frames.dim() == 4 else (F, self.H, self.W),
              "depth_frames")
         _chk(poses_est, torch.float64, (B, 3, 4), "poses_est")
         _chk(poses_gt, torch.float64, (B, 3, 4), "poses_gt")
         taus = np.ascontiguousarray(np.asarray(taus, np.float64).reshape(-1))
+        diam = None
+        if diameters is not None:
+            diam = np.ascontiguousarray(np.asarray(diameters, np.float64).reshape(-1))
+            if diam.shape != (B,):
+                raise ValueError("diameters: expected shape %s, got %s" % ((B,), diam.shape))
         out = {"err": self._new((B, len(taus)), torch.float64), "status": self._new((B,), torch.int32)}
-        check(lib.dim_pose_error_vsd(self._h, _p(depth_frames), F, _p(frame_idx), K9, _p(K_frames), _p(cls_idx),
-                                     _p(poses_est), _p(poses_gt), B, znear, zfar, float(delta), farr(taus, ctype=C.c_double),
-                                     len(taus), _p(out["err"]), _p(out["status"]), self._stream()))
+        args = (self._h, _p(depth_frames), F, _p(frame_idx), K9, _p(K_frames), _p(cls_idx), _p(poses_est), _p(poses_gt), B,
+                znear, zfar, float(delta), farr(taus, ctype=C.c_double), len(taus))
+        tail = (_p(out["err"]), _p(out["status"]), self._stream())
+        if visib_mode == "sixd17" and diam is None:
+            check(lib.dim_pose_error_vsd(*args, *tail))
+        else:
+            check(lib.dim_pose_error_vsd_ex(*args, VISIB_MODES[visib_mode], None if diam is None else diam.ctypes.data_as(C.POINTER(C.c_double)), *tail))
+        return out
+
+    def pose_error_sym(self, poses_est, poses_gt, points, syms, K):
+        """BOP 2019's MSSD (metres) and MSPD (pixels) of poses_est against poses_gt over one class's symmetry set
+        (dim_pose_error_sym; the contract is oracle/bop.py): the max over the model points, then the min over the symmetries.
+        poses_est / poses_gt f64 [M,3,4] CUDA (any M: called in slices of max_batch); points [N,3] and syms [S,3,4] (e.g.
+        bop.symmetry_transforms, S <= 4096), float64 CUDA tensors or host arrays; K [3,3] (one camera, broadcast) or [M,3,3].
+        A point with Z <= 0 under either pose makes that symmetry's MSPD inf.
+        Returns CUDA tensors: err f64 [M,2] (MSSD, MSPD) and sym_idx i32 [M,2] (the minimising symmetry of each, the lowest
+        index on ties)."""
+        M = poses_est.shape[0]
+        _chk(poses_est, torch.float64, (M, 3, 4), "poses_est")
+        _chk(poses_gt, torch.float64, (M, 3, 4), "poses_gt")
+        dev = lambda a: torch.as_tensor(a, dtype=torch.float64).to(self.device).contiguous()
+        pts = dev(points).reshape(-1, 3).contiguous()
+        sy = dev(syms).reshape(-1, 3, 4).contiguous()
+        Kd = dev(K)
+        if Kd.numel() == 9:
+            Kd = Kd.reshape(1, 9).expand(M, 9).contiguous()
+        elif tuple(Kd.shape) != (M, 3, 3):
+            raise ValueError("K: expected shape (3, 3) or %s, got %s" % ((M, 3, 3), tuple(Kd.shape)))
+        Kd = Kd.reshape(M, 9)
+        out = {"err": self._new((M, 2), torch.float64), "sym_idx": self._new((M, 2), torch.int32)}
+        for a in range(0, M, self.max_batch):
+            b = min(M, a + self.max_batch)
+            check(lib.dim_pose_error_sym(self._h, _p(poses_est[a:b]), _p(poses_gt[a:b]), b - a, _p(pts), pts.shape[0],
+                                         _p(sy), sy.shape[0], _p(Kd[a:b]), _p(out["err"][a:b]), _p(out["sym_idx"][a:b]),
+                                         self._stream()))
         return out
 
     def _frame_batch(self, frames, frame_idx, cls_idx, K, host=False):

@@ -177,7 +177,7 @@ class LM6DRefine:
 
 
 def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl", "cup"), n_iter=4, max_batch=16, device=0,
-             precision="fp16", input_depth=False, input_mask=True, icp_iters=0, vsd=False):
+             precision="fp16", input_depth=False, input_mask=True, icp_iters=0, vsd=False, bop=False, models_info_json=None):
     """Batched pred_eval (deepim/core/tester.py:50-527 without its batch = 1 limit): refine every pair of the image set
     and score it the way the reference's dataset class does: ADD / ADI accuracy + AUC (evaluate_pose_add), 5 cm 5 deg
     (evaluate_pose) and Proj. 2D (evaluate_pose_arp_2d); the last two under res["rot_trans"] / res["arp_2d"].
@@ -196,6 +196,13 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
     depth belongs to that camera), with the values of Hodan et al. and the SIXD Challenge 2017: delta 15 mm, tau 20 mm,
     recall at e < 0.3.  res["vsd"] holds evaluate_pose_vsd's per-class and mean recall per row and the errors [rows,M].
     With vsd=False the result is unchanged.
+    bop=True also scores every row with BOP 2019's average recall (pose_eval.evaluate_bop19) into res["bop"], with the
+    per-instance errors under res["bop"]["errors"] ("vsd" [rows,M,10], "mssd" and "mspd" [rows,M]): the BOP 2019 VSD
+    against each pair's observed `-depth.png` (delta 15 mm, taus relative to the class's diameter from models_info.txt), and
+    MSSD / MSPD over each class's symmetries, each pair projected with its own `-K.txt` camera where it has one.  The
+    symmetries come from BOP's `models_info.json` (models_info_json; object ids are the dataset's LINEMOD ids, idx2class);
+    without it every class has only the identity.  The model points are each class's points.xyz, not BOP's evaluation
+    models, so these are not the official BOP numbers.  With bop=False the result is unchanged.
     Returns (evaluate_pose_add result + the two extra tables, poses_est [n_iter,M,3,4], poses_gt)."""
     from . import pose_eval
     from .refiner import PoseRefiner
@@ -211,7 +218,7 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
             cls_idx.append(ci)
             init.append(rec["pose_rendered"])
             gt.append(rec["pose_observed"])
-            if input_depth or icp_iters > 0 or vsd:
+            if input_depth or icp_iters > 0 or vsd or bop:
                 depths.append(read_depth_u16(os.path.join(dataset.root, "data", "observed", pair[0] + "-depth.png")))
     imgs, cls_idx = np.stack(imgs), np.asarray(cls_idx, np.int32)
     init, gt = np.stack(init).astype(np.float64), np.stack(gt).astype(np.float64)
@@ -230,7 +237,30 @@ def evaluate(dataset: LM6DRefine, weights, K, symmetric=("eggbox", "glue", "bowl
         errs = np.stack([ref.vsd(depths, cls_idx, p, gt, K_frames=K_pairs, delta=0.015, taus=(0.02,))["err"][:, 0]
                          for p in poses])
         res["vsd"] = dict(pose_eval.evaluate_pose_vsd(errs, cls_idx, len(dataset.classes), 0.3), errors=errs)
+    if bop:
+        res["bop"] = _evaluate_bop19(dataset, ref, poses, gt, cls_idx, depths, K, K_pairs, pts_all, models_info_json)
     res["rot_trans"] = pose_eval.evaluate_pose(ref.ctx, poses, gt, cls_idx, pts_all, K, class_names=list(dataset.classes))
     res["arp_2d"] = pose_eval.evaluate_pose_arp_2d(ref.ctx, poses, gt, cls_idx, pts_all, K, class_names=list(dataset.classes))
     ref.close()
     return res, poses, gt
+
+
+def _evaluate_bop19(dataset, ref, poses, gt, cls_idx, depths, K, K_pairs, pts_all, models_info_json):
+    """evaluate(bop=True)'s table: BOP 2019 VSD, MSSD and MSPD of every row and their average recall"""
+    from . import bop, pose_eval
+    info = {} if models_info_json is None else bop.load_models_info_json(models_info_json)
+    class2id = {c: i for i, c in dataset.idx2class.items()}
+    syms = [bop.symmetry_transforms(info.get(class2id.get(c), {})) for c in dataset.classes]
+    diam_cls = np.array([dataset.diameters[c] for c in dataset.classes])
+    K_inst = np.broadcast_to(np.asarray(K, np.float32).reshape(3, 3), (len(cls_idx), 3, 3)) if K_pairs is None else K_pairs
+    vsd_err, mssd, mspd = [], [], []
+    for p in poses:
+        vsd_err.append(ref.vsd(depths, cls_idx, p, gt, K_frames=K_pairs, delta=pose_eval.BOP19_VSD_DELTA,
+                               taus=pose_eval.BOP19_VSD_TAUS, visib_mode="bop19", diameters=diam_cls[cls_idx])["err"])
+        e = ref.pose_error_sym(cls_idx, p, gt, pts_all, syms, K_inst)["err"]
+        mssd.append(e[:, 0])
+        mspd.append(e[:, 1])
+    errors = {"vsd": np.stack(vsd_err), "mssd": np.stack(mssd), "mspd": np.stack(mspd)}
+    res = pose_eval.evaluate_bop19(errors["vsd"], errors["mssd"], errors["mspd"], cls_idx, len(dataset.classes), diam_cls,
+                                   ref.ctx.W)
+    return dict(res, errors=errors)

@@ -171,6 +171,47 @@ def evaluate_pose_vsd(errors, cls_idx, n_classes, theta=0.3):
     return res
 
 
+BOP19_VSD_DELTA = 0.015                            # metres
+BOP19_VSD_TAUS = np.arange(0.05, 0.51, 0.05)       # fractions of the diameter; also the VSD thresholds
+BOP19_MSSD_THRESHOLDS = np.arange(0.05, 0.51, 0.05)  # fractions of the diameter
+BOP19_MSPD_THRESHOLDS = np.arange(5, 51, 5)        # pixels at a width of 640
+
+
+def evaluate_bop19(vsd_errors, mssd, mspd, cls_idx, n_classes, diameters, width=640):
+    """BOP 2019's average recall: vsd_errors [n_rows,M,10] (BOP 2019 VSD at the taus BOP19_VSD_TAUS, e.g. PoseRefiner.vsd
+    with visib_mode="bop19" and the diameters), mssd / mspd [n_rows,M] (PoseRefiner.pose_error_sym), cls_idx [M],
+    diameters [n_classes] metres, width the image width in pixels.  An instance is correct when its error is below the
+    threshold:
+      AR_VSD  = the recall averaged over every (tau, threshold) pair, the thresholds being BOP19_VSD_TAUS;
+      AR_MSSD = the recall averaged over the thresholds BOP19_MSSD_THRESHOLDS * the class's diameter;
+      AR_MSPD = the recall averaged over the thresholds BOP19_MSPD_THRESHOLDS * width / 640 pixels;
+      AR      = (AR_VSD + AR_MSSD + AR_MSPD) / 3.
+    Returns per class and over all instances together ("mean", as BOP aggregates), each as a list of n_rows percentages:
+    {"classes": {c: {"AR", "AR_VSD", "AR_MSSD", "AR_MSPD"}}, "mean": {...}}."""
+    vsd_errors = np.asarray(vsd_errors, np.float64)
+    mssd, mspd, cls_idx = np.asarray(mssd, np.float64), np.asarray(mspd, np.float64), np.asarray(cls_idx)
+    if vsd_errors.shape[-1] != len(BOP19_VSD_TAUS):
+        raise ValueError("vsd_errors: expected %d taus, got %d" % (len(BOP19_VSD_TAUS), vsd_errors.shape[-1]))
+    diam = np.asarray(diameters, np.float64)[cls_idx]                       # [M]
+    vsd_ok = vsd_errors[..., :, None] < BOP19_VSD_TAUS                      # [rows,M,tau,threshold]
+    mssd_ok = mssd[..., None] < BOP19_MSSD_THRESHOLDS * diam[:, None]       # [rows,M,threshold]
+    mspd_ok = mspd[..., None] < BOP19_MSPD_THRESHOLDS * (width / 640.0)
+
+    def recall(sel):
+        r = {"AR_VSD": 100.0 * vsd_ok[:, sel].mean(axis=(1, 2, 3)), "AR_MSSD": 100.0 * mssd_ok[:, sel].mean(axis=(1, 2)),
+             "AR_MSPD": 100.0 * mspd_ok[:, sel].mean(axis=(1, 2))}
+        r["AR"] = (r["AR_VSD"] + r["AR_MSSD"] + r["AR_MSPD"]) / 3.0
+        return {k: v.tolist() for k, v in r.items()}
+
+    res = {"classes": {}, "mean": {}}
+    for c in range(n_classes):
+        sel = np.nonzero(cls_idx == c)[0]
+        if len(sel):
+            res["classes"][c] = recall(sel)
+    res["mean"] = recall(np.arange(len(cls_idx))) if len(cls_idx) else {}
+    return res
+
+
 def simpson(y, dx):
     """Composite Simpson rule as scipy.integrate.simps(y, dx=dx) with the default even='avg' handling for an even
     number of samples (average of 'first N-2 intervals + trapezoid on the last' and 'trapezoid on the first + last N-2')."""

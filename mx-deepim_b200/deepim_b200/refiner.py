@@ -252,21 +252,51 @@ class PoseRefiner:
 
         return self._depth_batches(depths_u16, cls_idx, K_frames, frame_of, out, 1, call)
 
-    def vsd(self, depths_u16, cls_idx, poses_est, poses_gt, K_frames=None, frame_of=None, delta=0.015, taus=(0.02,)):
+    def vsd(self, depths_u16, cls_idx, poses_est, poses_gt, K_frames=None, frame_of=None, delta=0.015, taus=(0.02,),
+            visib_mode="sixd17", diameters=None):
         """Visible Surface Discrepancy of poses_est against poses_gt (Context.pose_error_vsd, dim_pose_error_vsd), batched
         and pipelined exactly as icp(): depths_u16, cls_idx, K_frames and frame_of as there, poses_est / poses_gt [N,3,4]
         float64 host; delta and taus in metres (the defaults are the SIXD Challenge 2017's 15 mm and 20 mm).
+        visib_mode "bop19" and diameters [N] (metres; taus become fractions of them) give BOP 2019's VSD, as
+        Context.pose_error_vsd.
         Returns host arrays: err [N,n_tau] float64 and status [N] int32 (see Context.pose_error_vsd)."""
         n = len(cls_idx)
         poses_est, poses_gt = np.asarray(poses_est, np.float64), np.asarray(poses_gt, np.float64)
         taus = np.asarray(taus, np.float64).reshape(-1)
+        diam = None if diameters is None else np.asarray(diameters, np.float64).reshape(-1)
+        if diam is not None and len(diam) != n:
+            raise ValueError("diameters has %d entries for %d instances" % (len(diam), n))
         out = {"err": np.zeros((n, len(taus))), "status": np.zeros(n, np.int32)}
 
         def call(ctx, dev, depth, cls, a, b, K, local):
             return ctx.pose_error_vsd(depth, cls, dev(poses_est[a:b]), dev(poses_gt[a:b]), K, delta, taus, local,
-                                      self.zn, self.zf)
+                                      self.zn, self.zf, visib_mode, None if diam is None else diam[a:b])
 
         return self._depth_batches(depths_u16, cls_idx, K_frames, frame_of, out, 0, call)
+
+    def pose_error_sym(self, cls_idx, poses_est, poses_gt, points_per_class, syms_per_class, K=None):
+        """BOP 2019's MSSD and MSPD (Context.pose_error_sym, dim_pose_error_sym) of N instances: cls_idx [N], poses_est /
+        poses_gt [N,3,4] float64 host, points_per_class[c] [N_c,3] and syms_per_class[c] [S_c,3,4] (bop.symmetry_transforms)
+        of every class present; K None = the refiner's K, [3,3] = one camera, [N,3,3] = each instance's own.
+        The instances of each class go to the device in slices of max_batch, in their order, on the first slot's context.
+        Returns host arrays: err [N,2] float64 (MSSD metres, MSPD pixels) and sym_idx [N,2] int32."""
+        cls_idx = np.asarray(cls_idx)
+        n = len(cls_idx)
+        poses_est, poses_gt = np.asarray(poses_est, np.float64), np.asarray(poses_gt, np.float64)
+        Ks = np.asarray(self.K if K is None else K, np.float64)
+        Ks = np.broadcast_to(Ks.reshape(3, 3), (n, 3, 3)) if Ks.size == 9 else Ks.reshape(n, 3, 3)
+        out = {"err": np.zeros((n, 2)), "sym_idx": np.zeros((n, 2), np.int32)}
+        ctx = self.ctx
+        dev = lambda x: torch.from_numpy(np.ascontiguousarray(x, np.float64)).to(ctx.device)
+        for c in np.unique(cls_idx):
+            sel = np.nonzero(cls_idx == c)[0]
+            pts, sy = dev(points_per_class[c]), dev(syms_per_class[c])
+            for a in range(0, len(sel), self.max_batch):
+                s = sel[a:a + self.max_batch]
+                r = ctx.pose_error_sym(dev(poses_est[s]), dev(poses_gt[s]), pts, sy, Ks[s])
+                for k in out:
+                    out[k][s] = r[k].cpu().numpy()
+        return out
 
     def _depth_batches(self, depths_u16, cls_idx, K_frames, frame_of, out, axis, call):
         """icp / vsd over refine_frames()'s device batches (plan_frame_batches), pipelined over the slots: per batch the
