@@ -52,6 +52,18 @@ DIM_API int32_t dim_mesh_upload(dim_ctx *ctx, int32_t cls_idx, const float *vert
                                 const float *uvs_host, int32_t V, const int32_t *faces_host,
                                 int32_t F, const uint8_t *tex_host, int32_t Th, int32_t Tw);
 
+/* Upload a vertex-coloured mesh for class cls_idx (the models of LINEMOD's and BOP's PLY files): verts f32[V,3] in metres,
+ * colours f32[V,3] RGB in [0,1], faces i32[F,3], all host arrays.  A fragment's GL float colour is the perspective-correct
+ * interpolation of its winner triangle's vertex colours, ((w0 cA + w1 cB) + w2 cC) / iz in float32 with w_k = b_k iz_k;
+ * a textured mesh's is texel / 255.  Everything else of a render (coverage, depth, mask, boxes, status) does not depend
+ * on the colour source, and every render, refinement, update, ICP and VSD entry draws both kinds, mixed in one batch.
+ * Refused (nothing allocated or changed, the class keeps its previous mesh): a bad class index, a mesh beyond the
+ * context's limits, a face index outside [0, V), a colour that is not finite or lies outside [0,1] (the error names the
+ * vertex).  Uploading a class again, with this call or dim_mesh_upload, replaces its mesh and its colour source;
+ * dim_mesh_upload_normals works on both kinds. */
+DIM_API int32_t dim_mesh_upload_colours(dim_ctx *ctx, int32_t cls_idx, const float *verts_host,
+                                        const float *colours_host, int32_t V, const int32_t *faces_host, int32_t F);
+
 /* Rasterise B instances.  Replaces Render_Py.render (render_py_multi.py:101-129) plus the
  * post-render glue (deepim/core/tester.py:185-188,433-442; lib/utils/image.py:583-594).
  *   cls_idx i32[B] (device), pose f32[B,3,4] (device), K9 host f32[9], pixel_means_rgb host f64[3]

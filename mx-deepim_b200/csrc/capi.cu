@@ -108,7 +108,7 @@ DIM_API int32_t dim_ctx_create(int32_t device, int32_t max_batch, int32_t H, int
   rc |= dev_alloc(ctx, &ctx->vsd_diam, Bm);
   rc |= dev_alloc(ctx, &ctx->sym_partial, Bm * SYM_SLOTS * 2);
   if (rc) { dim_ctx_destroy(ctx); return 12; }
-  ctx->meshes_host.assign(max_classes, MeshDev{nullptr, nullptr, nullptr, nullptr, 0, 0, 0, 0, nullptr});
+  ctx->meshes_host.assign(max_classes, MeshDev{nullptr, nullptr, nullptr, nullptr, 0, 0, 0, 0, nullptr, nullptr});
   DIM_CHECK(cudaMemset(ctx->meshes, 0, sizeof(MeshDev) * max_classes));
   DIM_CHECK(cudaMemset(ctx->vis, 0xFF, sizeof(unsigned long long) * Bm * P));  // all pixels empty
   DIM_CHECK(cudaMemset(ctx->pverts, 0, sizeof(PVert) * Bm * max_verts));
@@ -149,6 +149,39 @@ DIM_API int32_t dim_mesh_upload(dim_ctx *ctx, int32_t cls, const float *verts, c
   DIM_CHECK(cudaMemcpy(df, faces, sizeof(int) * 3 * F, cudaMemcpyHostToDevice));
   DIM_CHECK(cudaMemcpy(dt, tex, (size_t)3 * Th * Tw, cudaMemcpyHostToDevice));
   m.verts = dv; m.uvs = du; m.faces = df; m.tex = dt; m.V = V; m.F = F; m.Th = Th; m.Tw = Tw; m.normals = nullptr;
+  m.colours = nullptr;
+  ctx->meshes_host[cls] = m;
+  DIM_CHECK(cudaMemcpy(ctx->meshes + cls, &m, sizeof(MeshDev), cudaMemcpyHostToDevice));
+  return 0;
+}
+
+// vertex-coloured mesh: the fragment colour interpolates the winner triangle's vertex colours (raster.cu, fragment_colour).
+// Every check runs before anything is allocated or changed, so a refused call leaves the class's previous mesh in place.
+DIM_API int32_t dim_mesh_upload_colours(dim_ctx *ctx, int32_t cls, const float *verts, const float *colours, int32_t V,
+                                        const int32_t *faces, int32_t F) {
+  DIM_REQUIRE(ctx && cls >= 0 && cls < ctx->max_classes, "dim_mesh_upload_colours: bad class index");
+  DIM_REQUIRE(verts && colours && faces, "dim_mesh_upload_colours: NULL argument");
+  DIM_REQUIRE(V > 0 && V <= ctx->max_verts && F > 0 && F <= ctx->max_faces, "dim_mesh_upload_colours: mesh exceeds ctx limits");
+  for (int32_t i = 0; i < 3 * F; ++i)
+    DIM_REQUIRE(faces[i] >= 0 && faces[i] < V, "dim_mesh_upload_colours: face index out of range");
+  std::vector<float4> c4((size_t)V);
+  for (int32_t v = 0; v < V; ++v) {
+    const float *c = colours + 3 * (size_t)v;
+    for (int e = 0; e < 3; ++e)
+      if (!(c[e] >= 0.f && c[e] <= 1.f)) {  // NaN fails both comparisons
+        set_error("dim_mesh_upload_colours: the colour of vertex %d is not finite or lies outside [0, 1]", v);
+        return 2;
+      }
+    c4[v] = make_float4(c[0], c[1], c[2], 0.f);
+  }
+  drop_graphs(ctx);  // the render launch grid follows the largest uploaded mesh
+  MeshDev m{};
+  float *dv; int *df; float4 *dc;
+  if (dev_alloc(ctx, &dv, (size_t)3 * V) || dev_alloc(ctx, &df, (size_t)3 * F) || dev_alloc(ctx, &dc, (size_t)V)) return 12;
+  DIM_CHECK(cudaMemcpy(dv, verts, sizeof(float) * 3 * V, cudaMemcpyHostToDevice));
+  DIM_CHECK(cudaMemcpy(df, faces, sizeof(int) * 3 * F, cudaMemcpyHostToDevice));
+  DIM_CHECK(cudaMemcpy(dc, c4.data(), sizeof(float4) * V, cudaMemcpyHostToDevice));
+  m.verts = dv; m.faces = df; m.colours = dc; m.V = V; m.F = F;
   ctx->meshes_host[cls] = m;
   DIM_CHECK(cudaMemcpy(ctx->meshes + cls, &m, sizeof(MeshDev), cudaMemcpyHostToDevice));
   return 0;

@@ -72,6 +72,8 @@ struct MeshDev {
   const uint8_t *tex;   // [Th,Tw,3]
   int V, F, Th, Tw;
   const float *normals; // [V,3] per-vertex normals (lit renderer only; nullptr otherwise)
+  const float4 *colours; // [V] per-vertex RGB in [0,1] (w unused) of a vertex-coloured mesh, whose uvs and tex are nullptr;
+                         // nullptr on a textured mesh.  The colour source is fixed at upload (raster.cu, fragment_colour).
 };
 
 struct NetState;  // net_state.cuh

@@ -13,9 +13,9 @@
 //   raster_coverage  : one thread per (instance, triangle): int64 edge functions, antisymmetric
 //                      tie rule, perspective 1/Z, 64-bit atomicMin of (Z bits << 32 | tri id) into a
 //                      visibility buffer.  Triangles with large boxes are swept by the whole warp.
-//   raster_resolve   : one thread per 4 pixels: winner triangle -> perspective-correct UV -> nearest
-//                      texel -> writes RGB-mean / depth / mask (/ BGR) with 16-byte stores, resets
-//                      the visibility buffer, reduces the mask bbox.
+//   raster_resolve   : one thread per 4 pixels: winner triangle -> fragment colour (nearest texel of the
+//                      perspective-correct UV, or interpolated vertex colours) -> writes RGB-mean / depth / mask
+//                      (/ BGR) with 16-byte stores, resets the visibility buffer, reduces the mask bbox.
 // Algorithmic HBM bytes per instance: 16 B/px written (RGB + depth, SURVEY 8(d)); this version also
 // writes the mask plane (4 B/px) and touches the visibility buffer only inside the vertex box.  In the fused
 // refinement loop the only output is the pixel-interleaved (R,G,B,mask) image and it is written only inside the
@@ -60,6 +60,7 @@ __device__ __forceinline__ MeshDev mesh_for(const RasterParams &p, int b) {
   if (c < 0 || c >= p.num_classes) {
     MeshDev e;
     e.verts = nullptr; e.uvs = nullptr; e.faces = nullptr; e.tex = nullptr; e.V = e.F = e.Th = e.Tw = 0; e.normals = nullptr;
+    e.colours = nullptr;
     return e;
   }
   return p.meshes[c];
@@ -108,8 +109,12 @@ __global__ void __launch_bounds__(256) raster_vertex_kernel(RasterParams p) {
       o.X = X;
       o.Y = Y;
       o.iz = iz;
-      o.uz = m.uvs[2 * v] * iz;
-      o.vz = m.uvs[2 * v + 1] * iz;
+      if (m.uvs) {  // a vertex-coloured mesh has no UVs: its colour is interpolated in fragment_colour
+        o.uz = m.uvs[2 * v] * iz;
+        o.vz = m.uvs[2 * v + 1] * iz;
+      } else {
+        o.uz = o.vz = 0.f;
+      }
     } else {
       o.X = o.Y = 0;
       o.iz = o.uz = o.vz = 0.f;
@@ -144,6 +149,7 @@ struct TriSetup {
   int ax, ay, bx, by, cx, cy;
   float aiz, biz, ciz;
   long long area;
+  bool swapped;  // B and C exchanged to make the area positive
 };
 
 // returns false for degenerate / culled triangles; orients to positive area (swaps b,c)
@@ -151,6 +157,7 @@ __device__ __forceinline__ bool tri_setup(const PVert &A, PVert &Bv, PVert &Cv, 
   if (!(A.ok && Bv.ok && Cv.ok)) return false;
   long long area = edge_fn(A.X, A.Y, Bv.X, Bv.Y, Cv.X, Cv.Y);
   if (area == 0) return false;
+  t.swapped = area < 0;
   if (area < 0) {
     PVert tmp = Bv;
     Bv = Cv;
@@ -255,10 +262,48 @@ __global__ void __launch_bounds__(128) raster_coverage_kernel(RasterParams p) {
   }
 }
 
-// colour chain of the reference: u8 texel -> GL float (c/255) -> "*255" (render_py_multi.py:124)
+// vertices A, B, C of face f in the order tri_setup uses them: B and C exchanged when the projected triangle is negatively
+// oriented
+__device__ __forceinline__ void tri_order(const MeshDev &m, const PVert *pv, int f, int &iA, int &iB, int &iC) {
+  iA = m.faces[3 * f];
+  iB = m.faces[3 * f + 1];
+  iC = m.faces[3 * f + 2];
+  if (edge_fn(pv[iA].X, pv[iA].Y, pv[iB].X, pv[iB].Y, pv[iC].X, pv[iC].Y) < 0) { const int tmp = iB; iB = iC; iC = tmp; }
+}
+
+// The GL float colour (RGB in [0,1]) of the fragment (b0, b1, b2, iz) of winner triangle f; A, Bv, Cv and `swapped` as tri_setup
+// left them.
+// Every resolve path takes its colour from here.  The source is the mesh's, fixed at upload; each CTA renders one instance,
+// so the branch is uniform within a CTA.
+//   textured mesh  nearest texel t of the perspective-correct UV: (float)t / 255.0f
+//   coloured mesh  perspective-correct interpolation of the vertex colours: ((w0 cA + w1 cB) + w2 cC) / iz, w_k = b_k iz_k
+__device__ __forceinline__ void fragment_colour(const MeshDev &m, int f, bool swapped, float b0, float b1, float b2,
+                                                float iz, const PVert &A, const PVert &Bv, const PVert &Cv, float c[3]) {
+  if (m.colours) {
+    const int iA = m.faces[3 * f], iB = m.faces[3 * f + (swapped ? 2 : 1)], iC = m.faces[3 * f + (swapped ? 1 : 2)];
+    const float4 cA = m.colours[iA], cB = m.colours[iB], cC = m.colours[iC];
+    const float w0 = b0 * A.iz, w1 = b1 * Bv.iz, w2 = b2 * Cv.iz;
+    c[0] = ((w0 * cA.x + w1 * cB.x) + w2 * cC.x) / iz;
+    c[1] = ((w0 * cA.y + w1 * cB.y) + w2 * cC.y) / iz;
+    c[2] = ((w0 * cA.z + w1 * cB.z) + w2 * cC.z) / iz;
+    return;
+  }
+  float un = (b0 * A.uz + b1 * Bv.uz) + b2 * Cv.uz;
+  float vn = (b0 * A.vz + b1 * Bv.vz) + b2 * Cv.vz;
+  float u = un / iz, v = vn / iz;
+  int tx = (int)floorf(u * (float)m.Tw), ty = (int)floorf(v * (float)m.Th);
+  tx = min(max(tx, 0), m.Tw - 1);
+  ty = min(max(ty, 0), m.Th - 1);
+  const unsigned char *tp = m.tex + ((size_t)ty * m.Tw + tx) * 3;
+  c[0] = (float)tp[0] / 255.0f;
+  c[1] = (float)tp[1] / 255.0f;
+  c[2] = (float)tp[2] / 255.0f;
+}
+
+// colour chain of the reference: GL float colour c (texel / 255) -> "*255" (render_py_multi.py:124)
 // -> optional uint8 truncation (deepim/core/tester.py:188)
-__device__ __forceinline__ float colour_of(unsigned char c, int trunc_u8) {
-  float f = ((float)c / 255.0f) * 255.0f;
+__device__ __forceinline__ float colour_of(float c, int trunc_u8) {
+  float f = c * 255.0f;
   if (trunc_u8) f = (float)(unsigned char)f;
   return f;
 }
@@ -266,18 +311,17 @@ __device__ __forceinline__ float colour_of(unsigned char c, int trunc_u8) {
 // The two lit renderers of the reference share the Lambert term and differ in where the light colour enters:
 //   SHADE_MODELNET  (render_py_light_modelnet_multi.py)  colour_c = texel_c * ((a0 + a1 * brightness) * I_c)
 //   SHADE_PY_LIGHT  (render_py_light.py, get_fragment)   colour_c = texel_c * (a0 + (a1 * brightness) * I_c)
-// with a0 = 1 - ratio, a1 = ratio; the fragment (b0, b1, b2, iz) is winner triangle f of instance b.  Returns the colours
-// quantised like the 8-bit framebuffer the reference reads back.
+// with a0 = 1 - ratio, a1 = ratio and texel_c the GL float colour tc of fragment_colour; the fragment (b0, b1, b2, iz) is
+// winner triangle f of instance b.  Returns the colours quantised like the 8-bit framebuffer the reference reads back.
 enum Shade { SHADE_MODELNET, SHADE_PY_LIGHT };
 
 template <Shade S>
 __device__ __forceinline__ void shade_lit(const RasterParams &p, const MeshDev &m, const PVert *pv, int b, int f, float b0,
                                           float b1, float b2, float iz, const PVert &A, const PVert &Bv, const PVert &Cv,
-                                          const unsigned char *tp, float a0, float a1, float q[3]) {
+                                          const float tc[3], float a0, float a1, float q[3]) {
   // Lambert shading, same float32 sequence as the CPU checker (see DESIGN.md "lit renderer")
-  const int iA = m.faces[3 * f];
-  int iB = m.faces[3 * f + 1], iC = m.faces[3 * f + 2];
-  if (edge_fn(pv[iA].X, pv[iA].Y, pv[iB].X, pv[iB].Y, pv[iC].X, pv[iC].Y) < 0) { const int tmp = iB; iB = iC; iC = tmp; }
+  int iA, iB, iC;
+  tri_order(m, pv, f, iA, iB, iC);
   const float w0 = b0 * A.iz, w1 = b1 * Bv.iz, w2 = b2 * Cv.iz;
   const float *ps = p.pose + 12 * b;
   float pm[3], nm[3], pc[3], nc[3];
@@ -304,7 +348,7 @@ __device__ __forceinline__ void shade_lit(const RasterParams &p, const MeshDev &
   const float scale = S == SHADE_MODELNET ? a0 + a1 * br : a1 * br;
 #pragma unroll
   for (int e = 0; e < 3; ++e) {
-    float col = S == SHADE_MODELNET ? ((float)tp[e] / 255.0f) * (scale * li[e]) : ((float)tp[e] / 255.0f) * (a0 + scale * li[e]);
+    float col = S == SHADE_MODELNET ? tc[e] * (scale * li[e]) : tc[e] * (a0 + scale * li[e]);
     col = col < 1.f ? col : 1.f;
     col = col > 0.f ? col : 0.f;
     q[e] = rintf(col * 255.0f);
@@ -344,56 +388,57 @@ __global__ void __launch_bounds__(256) raster_resolve_kernel(RasterParams p) {
     ulonglong2 k23 = *reinterpret_cast<const ulonglong2 *>(vis + 2);
     unsigned long long keys[4] = {k01.x, k01.y, k23.x, k23.y};
     bool any = false;
-    const MeshDev m = mesh_for(p, b);
+    const MeshDev mesh = mesh_for(p, b);
     const PVert *pv = p.pverts + (size_t)b * p.max_verts;
+    // the colour source is uniform within the CTA: one copy of the 4-pixel loop per source, so that the textured path
+    // keeps its own register allocation (fragment_colour folds its branch in each copy)
+    auto quad = [&](const MeshDev &m) {
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (keys[k] == VIS_EMPTY) continue;
-      any = true;
-      const int f = (int)(unsigned)(keys[k] & 0xffffffffull);
-      PVert A = pv[m.faces[3 * f]], Bv = pv[m.faces[3 * f + 1]], Cv = pv[m.faces[3 * f + 2]];
-      TriSetup t;
-      tri_setup(A, Bv, Cv, t);
-      float b0 = 0.f, b1 = 0.f, b2 = 0.f, iz = 1.f, z = 0.f;
-      tri_fragment(t, i, j4 + k, p.zn, p.zf, b0, b1, b2, iz, z);
-      float un = (b0 * A.uz + b1 * Bv.uz) + b2 * Cv.uz;
-      float vn = (b0 * A.vz + b1 * Bv.vz) + b2 * Cv.vz;
-      float u = un / iz, v = vn / iz;
-      int tx = (int)floorf(u * (float)m.Tw), ty = (int)floorf(v * (float)m.Th);
-      tx = min(max(tx, 0), m.Tw - 1);
-      ty = min(max(ty, 0), m.Th - 1);
-      const unsigned char *tp = m.tex + ((size_t)ty * m.Tw + tx) * 3;
-      float c0, c1, c2;
-      if (LIT) {
-        float q[3];
-        shade_lit<SHADE_MODELNET>(p, m, pv, b, f, b0, b1, b2, iz, A, Bv, Cv, tp, p.a0, p.a1, q);
-        c0 = q[0]; c1 = q[1]; c2 = q[2];
-      } else {
-        c0 = colour_of(tp[0], p.trunc_u8); c1 = colour_of(tp[1], p.trunc_u8); c2 = colour_of(tp[2], p.trunc_u8);
+      for (int k = 0; k < 4; ++k) {
+        if (keys[k] == VIS_EMPTY) continue;
+        any = true;
+        const int f = (int)(unsigned)(keys[k] & 0xffffffffull);
+        PVert A = pv[m.faces[3 * f]], Bv = pv[m.faces[3 * f + 1]], Cv = pv[m.faces[3 * f + 2]];
+        TriSetup t;
+        tri_setup(A, Bv, Cv, t);
+        float b0 = 0.f, b1 = 0.f, b2 = 0.f, iz = 1.f, z = 0.f;
+        tri_fragment(t, i, j4 + k, p.zn, p.zf, b0, b1, b2, iz, z);
+        float tc[3];
+        fragment_colour(m, f, t.swapped, b0, b1, b2, iz, A, Bv, Cv, tc);
+        float c0, c1, c2;
+        if (LIT) {
+          float q[3];
+          shade_lit<SHADE_MODELNET>(p, m, pv, b, f, b0, b1, b2, iz, A, Bv, Cv, tc, p.a0, p.a1, q);
+          c0 = q[0]; c1 = q[1]; c2 = q[2];
+        } else {
+          c0 = colour_of(tc[0], p.trunc_u8); c1 = colour_of(tc[1], p.trunc_u8); c2 = colour_of(tc[2], p.trunc_u8);
+        }
+        raw[k][0] = c0; raw[k][1] = c1; raw[k][2] = c2;
+        // image.transform works in float64 and nd.array casts to float32 (lib/utils/image.py:583-594)
+        if (p.trunc_u8) {
+          r[k] = (float)((double)c0 - p.mean[0]);
+          g[k] = (float)((double)c1 - p.mean[1]);
+          bl[k] = (float)((double)c2 - p.mean[2]);
+        } else {  // train path (batch_updater_py_multi.py:234-235): float32 image -= float32 pixel_means
+          r[k] = c0 - (float)p.mean[0];
+          g[k] = c1 - (float)p.mean[1];
+          bl[k] = c2 - (float)p.mean[2];
+        }
+        d[k] = z;
+        if (z > 0.2f) mk[k] = 1.f;  // mask = depth > 0.2 (deepim/core/tester.py:440)
+        bool in_bbox = z > 0.2f;
+        if (COLOUR_BOX)
+          in_bbox = ((r[k] + (float)p.mean[0]) + (g[k] + (float)p.mean[1])) + (bl[k] + (float)p.mean[2]) > 0.01f;
+        if (in_bbox) {
+          mx0 = min(mx0, j4 + k);
+          mx1 = max(mx1, j4 + k);
+          my0 = i;
+          my1 = i;
+        }
       }
-      raw[k][0] = c0; raw[k][1] = c1; raw[k][2] = c2;
-      // image.transform works in float64 and nd.array casts to float32 (lib/utils/image.py:583-594)
-      if (p.trunc_u8) {
-        r[k] = (float)((double)c0 - p.mean[0]);
-        g[k] = (float)((double)c1 - p.mean[1]);
-        bl[k] = (float)((double)c2 - p.mean[2]);
-      } else {  // train path (batch_updater_py_multi.py:234-235): float32 image -= float32 pixel_means
-        r[k] = c0 - (float)p.mean[0];
-        g[k] = c1 - (float)p.mean[1];
-        bl[k] = c2 - (float)p.mean[2];
-      }
-      d[k] = z;
-      if (z > 0.2f) mk[k] = 1.f;  // mask = depth > 0.2 (deepim/core/tester.py:440)
-      bool in_bbox = z > 0.2f;
-      if (COLOUR_BOX)
-        in_bbox = ((r[k] + (float)p.mean[0]) + (g[k] + (float)p.mean[1])) + (bl[k] + (float)p.mean[2]) > 0.01f;
-      if (in_bbox) {
-        mx0 = min(mx0, j4 + k);
-        mx1 = max(mx1, j4 + k);
-        my0 = i;
-        my1 = i;
-      }
-    }
+    };
+    if (mesh.colours) quad(mesh);
+    else quad(mesh);
     if (any) {  // hand the visibility buffer back empty for the next render
       *reinterpret_cast<ulonglong2 *>(vis) = make_ulonglong2(VIS_EMPTY, VIS_EMPTY);
       *reinterpret_cast<ulonglong2 *>(vis + 2) = make_ulonglong2(VIS_EMPTY, VIS_EMPTY);
@@ -481,21 +526,16 @@ __global__ void __launch_bounds__(256) raster_dataset_kernel(RasterParams p, Dat
       tri_setup(A, Bv, Cv, t);
       float b0 = 0.f, b1 = 0.f, b2 = 0.f, iz = 1.f, z = 0.f;
       tri_fragment(t, i, j4 + k, p.zn, p.zf, b0, b1, b2, iz, z);
-      float un_ = (b0 * A.uz + b1 * Bv.uz) + b2 * Cv.uz;
-      float vn_ = (b0 * A.vz + b1 * Bv.vz) + b2 * Cv.vz;
-      float u = un_ / iz, v = vn_ / iz;
-      int tx = (int)floorf(u * (float)m.Tw), ty = (int)floorf(v * (float)m.Th);
-      tx = min(max(tx, 0), m.Tw - 1);
-      ty = min(max(ty, 0), m.Th - 1);
-      const unsigned char *tp = m.tex + ((size_t)ty * m.Tw + tx) * 3;
+      float tc[3];
+      fragment_colour(m, f, t.swapped, b0, b1, b2, iz, A, Bv, Cv, tc);
 #pragma unroll
       for (int e = 0; e < 3; ++e) {  // BGR byte 3k + e of the 12 holds channel 2 - e
         const int byte = 3 * k + e;
-        un[byte >> 2] |= (unsigned)(unsigned char)colour_of(tp[2 - e], 0) << ((byte & 3) * 8);
+        un[byte >> 2] |= (unsigned)(unsigned char)colour_of(tc[2 - e], 0) << ((byte & 3) * 8);
       }
       if (LIT) {
         float c[3];
-        shade_lit<SHADE_PY_LIGHT>(p, m, pv, b, f, b0, b1, b2, iz, A, Bv, Cv, tp, a0, a1, c);
+        shade_lit<SHADE_PY_LIGHT>(p, m, pv, b, f, b0, b1, b2, iz, A, Bv, Cv, tc, a0, a1, c);
 #pragma unroll
         for (int e = 0; e < 3; ++e) {
           const int byte = 3 * k + e;

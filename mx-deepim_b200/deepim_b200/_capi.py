@@ -41,6 +41,7 @@ SIGNATURES = {
     "dim_ctx_create": (i32, [i32, i32, i32, i32, i32, i32, i32, C.POINTER(vp)]),
     "dim_ctx_destroy": (None, [vp]),
     "dim_mesh_upload": (i32, [vp, i32, vp, vp, i32, vp, i32, vp, i32, i32]),
+    "dim_mesh_upload_colours": (i32, [vp, i32, vp, vp, i32, vp, i32]),
     "dim_render": (i32, [vp, vp, vp, i32, pf32, f32, f32, pf64, i32, vp, vp, vp, vp, vp, vp]),
     "dim_zoom_mask_fwd": (i32, [vp, vp, vp, vp, vp, i32, pf32, vp, vp, vp, vp, vp, vp, vp]),
     "dim_zoom_image_with_factor_fwd": (i32, [vp, vp, vp, vp, i32, pf32, vp, vp, vp]),

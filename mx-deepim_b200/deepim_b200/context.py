@@ -131,12 +131,18 @@ class Context:
 
     # ------------------------------------------------------------------------------ setup
     def upload_mesh(self, cls_idx, mesh):
+        """a textured mesh (uvs + tex) or a vertex-coloured one (colours), with its normals when it has them"""
         v = np.ascontiguousarray(mesh.verts, np.float32)
-        uv = np.ascontiguousarray(mesh.uvs, np.float32)
         f = np.ascontiguousarray(mesh.faces, np.int32)
-        tex = np.ascontiguousarray(mesh.tex, np.uint8)
-        check(lib.dim_mesh_upload(self._h, cls_idx, v.ctypes.data, uv.ctypes.data, len(v), f.ctypes.data, len(f),
-                                  tex.ctypes.data, tex.shape[0], tex.shape[1]))
+        colours = getattr(mesh, "colours", None)
+        if colours is not None:
+            c = np.ascontiguousarray(colours, np.float32)
+            check(lib.dim_mesh_upload_colours(self._h, cls_idx, v.ctypes.data, c.ctypes.data, len(v), f.ctypes.data, len(f)))
+        else:
+            uv = np.ascontiguousarray(mesh.uvs, np.float32)
+            tex = np.ascontiguousarray(mesh.tex, np.uint8)
+            check(lib.dim_mesh_upload(self._h, cls_idx, v.ctypes.data, uv.ctypes.data, len(v), f.ctypes.data, len(f),
+                                      tex.ctypes.data, tex.shape[0], tex.shape[1]))
         self.num_classes = max(self.num_classes, cls_idx + 1)
         if getattr(mesh, "normals", None) is not None:
             self.upload_normals(cls_idx, mesh.normals)

@@ -83,6 +83,150 @@ def write_textured_obj(mesh: Mesh, obj_path, texture_path):
     _cv2().imwrite(texture_path, np.ascontiguousarray(mesh.tex[::-1, :, ::-1]))
 
 
+# PLY scalar types and their aliases -> little-endian numpy dtypes
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "<i2", "int16": "<i2", "ushort": "<u2",
+              "uint16": "<u2", "int": "<i4", "int32": "<i4", "uint": "<u4", "uint32": "<u4", "float": "<f4",
+              "float32": "<f4", "double": "<f8", "float64": "<f8"}
+
+
+def _ply_type(t):
+    if t not in _PLY_TYPES:
+        raise ValueError("PLY: unknown property type %r" % t)
+    return np.dtype(_PLY_TYPES[t])
+
+
+def _ply_header(data):
+    """format, comments and elements [(name, count, [(prop, dtype) or (prop, count dtype, item dtype)])], data offset"""
+    end = data.find(b"end_header")
+    if not data.startswith(b"ply") or end < 0:
+        raise ValueError("PLY: not a PLY file")
+    body = data.index(b"\n", end) + 1
+    fmt, comments, elements = None, [], []
+    for line in data[:end].decode("ascii", "replace").splitlines()[1:]:
+        t = line.split()
+        if not t:
+            continue
+        if t[0] == "format":
+            fmt = " ".join(t[1:])
+        elif t[0] == "comment":
+            comments.append(t[1:])
+        elif t[0] == "element":
+            elements.append((t[1], int(t[2]), []))
+        elif t[0] == "property" and elements:
+            if t[1] == "list":
+                elements[-1][2].append((t[4], _ply_type(t[2]), _ply_type(t[3])))
+            else:
+                elements[-1][2].append((t[2], _ply_type(t[1])))
+    if fmt not in ("ascii 1.0", "binary_little_endian 1.0"):
+        raise ValueError("PLY: format %r is not supported (ascii 1.0 and binary_little_endian 1.0 are)" % fmt)
+    return fmt == "ascii 1.0", comments, elements, body
+
+
+def _ply_binary_element(data, pos, count, props):
+    """one element of a binary file -> ({scalar prop: [count] array, list prop: [count] list of arrays}, next offset)"""
+    if all(len(p) == 2 for p in props):  # fixed-size rows
+        dt = np.dtype([(n, t) for n, t in props])
+        if pos + dt.itemsize * count > len(data):
+            raise ValueError("PLY: file ends inside an element")
+        rows = np.frombuffer(data, dt, count, pos)
+        return {n: rows[n] for n, _ in props}, pos + dt.itemsize * count
+    out = {p[0]: [] for p in props}
+    for _ in range(count):
+        for p in props:
+            if len(p) == 2:
+                out[p[0]].append(np.frombuffer(data, p[1], 1, pos)[0])
+                pos += p[1].itemsize
+            else:
+                n = int(np.frombuffer(data, p[1], 1, pos)[0])
+                pos += p[1].itemsize
+                out[p[0]].append(np.frombuffer(data, p[2], n, pos))
+                pos += p[2].itemsize * n
+    return {k: (np.array(v) if len(p) == 2 else v) for (k, v), p in zip(out.items(), props)}, pos
+
+
+def _ply_ascii_element(tokens, pos, count, props):
+    out = {p[0]: [] for p in props}
+    for _ in range(count):
+        for p in props:
+            if len(p) == 2:
+                out[p[0]].append(tokens[pos])
+                pos += 1
+            else:
+                n = int(tokens[pos])
+                out[p[0]].append(np.array(tokens[pos + 1:pos + 1 + n], np.float64).astype(p[2]))
+                pos += 1 + n
+    return {k: (np.array(v, np.float64).astype(p[1]) if len(p) == 2 else v) for (k, v), p in zip(out.items(), props)}, pos
+
+
+def load_ply(path, scale=1.0) -> Mesh:
+    """A triangle mesh from a PLY file (ascii 1.0 or binary_little_endian 1.0): LINEMOD's obj_xx.ply and BOP's
+    models/obj_NNNNNN.ply.  Vertex properties x y z (required), nx ny nz (-> mesh.normals), red green blue (alpha is
+    ignored), texture_u texture_v with a `comment TextureFile <file>`; faces from the `vertex_indices` or `vertex_index`
+    list of the face element; every other element is skipped.  Positions are float32(float64(x) * scale) (BOP's
+    millimetres load with scale=1e-3).  The colour source:
+      - a model that names a texture and has UVs: a textured Mesh, the image flipped as load_textured_obj flips it;
+      - else per-vertex colours: uchar channels c -> float32(c) / float32(255), float channels as they are (the property
+        type decides, unlike the SIXD renderer's "divide by 255 if max > 1", so a dark uchar model is not misread);
+      - a model without colours is drawn in the SIXD renderer's 0.5 grey.
+    ValueError for big-endian or unknown formats, missing x y z, faces that are not triangles, face indices out of
+    range and a texture file that does not exist."""
+    with open(path, "rb") as f:
+        data = f.read()
+    ascii_, comments, elements, pos = _ply_header(data)
+    tokens = data[pos:].split() if ascii_ else None
+    if ascii_:
+        pos = 0
+    got = {}
+    for name, count, props in elements:
+        if ascii_:
+            vals, pos = _ply_ascii_element(tokens, pos, count, props)
+        else:
+            vals, pos = _ply_binary_element(data, pos, count, props)
+        got[name] = (vals, {p[0]: p for p in props})
+    if "vertex" not in got or not {"x", "y", "z"} <= set(got["vertex"][0]):
+        raise ValueError("PLY %s: the vertex element has no x y z" % path)
+    vert, vprops = got["vertex"]
+    V = len(vert["x"])
+    pts = (np.stack([vert[k] for k in "xyz"], 1).astype(np.float64) * float(scale)).astype(np.float32)
+    fvals, fprops = got.get("face", ({}, {}))
+    key = "vertex_indices" if "vertex_indices" in fvals else "vertex_index"
+    if key not in fvals or len(fprops[key]) != 3:
+        raise ValueError("PLY %s: no face list vertex_indices / vertex_index" % path)
+    lists = fvals[key]
+    bad = [i for i, l in enumerate(lists) if len(l) != 3]
+    if bad:
+        raise ValueError("PLY %s: face %d has %d corners; only triangles are supported" % (path, bad[0], len(lists[bad[0]])))
+    faces = np.array(lists, np.int64).reshape(-1, 3)
+    if faces.size and (faces.min() < 0 or faces.max() >= V):
+        raise ValueError("PLY %s: a face index lies outside [0, %d)" % (path, V))
+    faces = faces.astype(np.int32)
+    name = os.path.splitext(os.path.basename(path))[0]
+    tex_file = [c[1] for c in comments if len(c) >= 2 and c[0] == "TextureFile"]
+    if tex_file and {"texture_u", "texture_v"} <= set(vert):
+        tex_path = os.path.join(os.path.dirname(os.path.abspath(path)), tex_file[0])
+        tex = _cv2().imread(tex_path, _cv2().IMREAD_COLOR) if os.path.exists(tex_path) else None
+        if tex is None:
+            raise ValueError("PLY %s: texture file %s cannot be read" % (path, tex_path))
+        uv = np.stack([vert["texture_u"], vert["texture_v"]], 1).astype(np.float32)
+        m = Mesh(pts, uv, faces, np.ascontiguousarray(tex[::-1, :, ::-1]), name=name)
+    elif {"red", "green", "blue"} <= set(vert):
+        cols = []
+        for k in ("red", "green", "blue"):
+            t = vprops[k][1]
+            if t == np.uint8:
+                cols.append(vert[k].astype(np.float32) / np.float32(255))
+            elif t.kind == "f":
+                cols.append(vert[k].astype(np.float32))
+            else:
+                raise ValueError("PLY %s: colour property %s of type %s (uchar or float expected)" % (path, k, t))
+        m = Mesh(pts, None, faces, None, name=name, colours=np.stack(cols, 1))
+    else:
+        m = Mesh(pts, None, faces, None, name=name, colours=np.full((V, 3), 0.5, np.float32))
+    if {"nx", "ny", "nz"} <= set(vert):
+        m.normals = np.stack([vert[k] for k in ("nx", "ny", "nz")], 1).astype(np.float32)
+    return m
+
+
 def load_points_xyz(path):
     return np.loadtxt(path).reshape(-1, 3)
 

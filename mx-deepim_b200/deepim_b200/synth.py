@@ -20,13 +20,19 @@ PIXEL_MEANS_RGB = PIXEL_MEANS[::-1].copy()
 
 
 class Mesh:
-    """verts [V,3] f32 (metres), uvs [V,2] f32, faces [F,3] i32, tex [Th,Tw,3] u8 (row 0 = v 0)."""
+    """verts [V,3] f32 (metres), faces [F,3] i32 and one colour source: a texture, uvs [V,2] f32 with tex [Th,Tw,3] u8
+    (row 0 = v 0), or per-vertex colours [V,3] f32 RGB in [0,1] (uvs = tex = None), never both."""
 
-    def __init__(self, verts, uvs, faces, tex, name="mesh"):
+    def __init__(self, verts, uvs, faces, tex, name="mesh", colours=None):
+        if colours is None and (uvs is None or tex is None):
+            raise ValueError("Mesh: give uvs and tex, or colours")
+        if colours is not None and (uvs is not None or tex is not None):
+            raise ValueError("Mesh: a mesh has uvs and tex or colours, never both")
         self.verts = np.ascontiguousarray(verts, dtype=np.float32)
-        self.uvs = np.ascontiguousarray(uvs, dtype=np.float32)
+        self.uvs = None if uvs is None else np.ascontiguousarray(uvs, dtype=np.float32)
         self.faces = np.ascontiguousarray(faces, dtype=np.int32)
-        self.tex = np.ascontiguousarray(tex, dtype=np.uint8)
+        self.tex = None if tex is None else np.ascontiguousarray(tex, dtype=np.uint8)
+        self.colours = None if colours is None else np.ascontiguousarray(colours, dtype=np.float32).reshape(-1, 3)
         self.name = name
 
     @property
